@@ -113,6 +113,13 @@ int p2m_debug_set_dedup_padding(p2m_model_t* m, int enable);
  * (sum_rows dz (x) T_k(x) = sum_rows T_k(dz) (x) x, L~ symmetric), re-using the L~dz the backward-data pass computes;
  * 0 = from the basis of the layer input, rebuilt on chip with its 2-hop halo.  Same result up to fp32 association. */
 int p2m_debug_set_dw_swap(p2m_model_t* m, int enable);
+/* Debug: which kernels the single-layer entry points (p2m_cheb_conv_fwd / _bwd) select for one layer of `level` at
+ * the handle's current precision.  out[0] = forward conv on tensor cores, out[1] its X staging depth (1 or 2; 0 off
+ * the tensor cores), out[2] / out[3] = the same for the weight gradient, out[4] / out[5] = the backward-data GEMM
+ * (dT = dz W_k), out[6] = own rows arrive by TMA (V % 128 == 0), out[7] / out[8] = the level's largest 1-hop / 2-hop
+ * staged-row count per 128-row tile (0 when the level has no tensor-core metadata), out[9] = isolated rows that
+ * padding elision would route to the dense path (0: elision not applicable).                                    */
+int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[10]);
 
 /* Bytes of device workspace p2m_meshnet_forward needs for batch B.  In training mode the workspace
  * also carries what p2m_meshnet_backward reads, so it must stay alive and untouched in between.   */

@@ -1794,10 +1794,7 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
       for (int e = rowptr[halo[i]]; e < rowptr[halo[i] + 1]; ++e) add(colidx[e]);
     }
     const int h2 = (int)halo.size();
-    if (h2 > 65535) {
-      set_error("umma meta: halo too large");
-      return P2M_ERR_INVALID;
-    }
+    if (h2 > 65535) return P2M_OK;  // beyond 16-bit staged-row slots: no tensor-core metadata, the level runs on SIMT
     // One local CSR serves both products: row i < h1 lists (staged-row slot, value) of vertex halo[i].
     // T1 rows read X slots (< h2); the T2 pass only walks the 128 tile rows, whose columns are < h1,
     // i.e. valid T1 slots (slot numbering of X and T1 coincides below h1).
@@ -1814,10 +1811,7 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
       rp[i + 1] = (unsigned short)(ent.size() / 2);
     }
     const int nnz = (int)(ent.size() / 2);
-    if (nnz > 65535) {
-      set_error("umma meta: too many entries in a tile");
-      return P2M_ERR_INVALID;
-    }
+    if (nnz > 65535) return P2M_OK;  // beyond 16-bit local-CSR offsets: likewise
     auto row_len = [&](int i) { return (int)rp[i + 1] - (int)rp[i]; };
     std::vector<unsigned short> ord1(h1), ord2(TILE_M);
     for (int i = 0; i < h1; ++i) ord1[i] = (unsigned short)i;
@@ -2106,6 +2100,16 @@ bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
   if (fout != 64 && fout != 128 && fout != 256) return false;
   return smem_bytes_for(CONV_N, ring_stages(CONV_N), 1, g) <= SMEM_LIMIT;
 }
+
+// X staging depth launch_n picks for a launch on the level's consecutive tiles: `t1_given` = mode 1 (T1 precomputed,
+// what the single-layer forward and the network run), `plain` = mode 2 (backward-data GEMM)
+int umma_conv_x_stages(const DevLevel& g, bool t1_given, bool plain) {
+  const int mode = plain ? 2 : (t1_given ? 1 : 0);
+  if (mode == 0) return x_stages(CONV_N, g);
+  return smem_bytes_for(CONV_N, ring_stages(CONV_N), 2, g, mode) <= SMEM_LIMIT ? 2 : 1;
+}
+int umma_dw_x_stages(const DevLevel& g) { return dw_smem_bytes(2, g) <= SMEM_LIMIT ? 2 : 1; }
+bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && g_umma_tma && tmap_encoder() != nullptr; }
 
 __global__ void __launch_bounds__(256) k_pack_plain(const float* __restrict__ Bmat, long long ld_n, long long ld_k, int N,
                                                     int K, unsigned char* __restrict__ out, float W_SCALE = 64.f) {

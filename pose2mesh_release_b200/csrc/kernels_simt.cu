@@ -707,13 +707,13 @@ __global__ void __launch_bounds__(256) k_absmax(const float* __restrict__ x, lon
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));  // non-negative floats order as uints
 }
-__global__ void k_scale_from_absmax(unsigned int* io) {
+__global__ void k_scale_from_absmax(unsigned int* io, int headroom_log2) {
   const float m = __uint_as_float(*io);
   float s = 1.f;
   if (m > 0.f && isfinite(m)) {
     int e;
-    frexpf(m, &e);            // m = f * 2^e, f in [0.5, 1)
-    s = ldexpf(1.f, 10 - e);  // m * s in [2^9, 2^10)
+    frexpf(m, &e);                            // m = f * 2^e, f in [0.5, 1)
+    s = ldexpf(1.f, 10 - e - headroom_log2);  // m * s in [2^(9-h), 2^(10-h))
   }
   *reinterpret_cast<float*>(io) = s;
 }
@@ -724,14 +724,47 @@ static int current_sm_count(int* sms) {
   P2M_CUDA_OK(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
   return P2M_OK;
 }
-int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s) {
+int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s, int headroom_log2) {
   P2M_CUDA_OK(cudaMemsetAsync(scale_out, 0, sizeof(float), s));
   int sms = 0;
   P2M_TRY(current_sm_count(&sms));
   const int grid = (int)std::min<long long>((n + 255) / 256, (long long)sms * 8);
   k_absmax<<<grid, 256, 0, s>>>(x, n, reinterpret_cast<unsigned int*>(scale_out));
   P2M_LAUNCH_OK();
-  k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(scale_out));
+  k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(scale_out), headroom_log2);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+__global__ void __launch_bounds__(256) k_scale_by(const float* __restrict__ x, long long n, const float* __restrict__ sp,
+                                                  int invert, float mul, float* __restrict__ y) {
+  const float f = (invert ? 1.f / *sp : *sp) * mul;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    y[i] = x[i] * f;
+}
+int launch_scale_by(const float* x, long long n, const float* scale, int invert, float mul, float* y, cudaStream_t s) {
+  if (n <= 0) return P2M_OK;
+  int sms = 0;
+  P2M_TRY(current_sm_count(&sms));
+  const int grid = (int)std::min<long long>((n + 255) / 256, (long long)sms * 8);
+  k_scale_by<<<grid, 256, 0, s>>>(x, n, scale, invert, mul, y);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+__global__ void k_rescaled_epilogue(const float* __restrict__ bias, const float* __restrict__ scale,
+                                    const float* __restrict__ shift, const float* __restrict__ w_scale, float w_packed,
+                                    int n, float* __restrict__ out_scale, float* __restrict__ out_shift) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float sc = scale ? scale[i] : 1.f;
+  out_scale[i] = sc * (w_packed / *w_scale);
+  out_shift[i] = fmaf(bias ? bias[i] : 0.f, sc, shift ? shift[i] : 0.f);
+}
+int launch_rescaled_epilogue(const Epilogue& ep, const float* w_scale, float w_packed, int n, float* out_scale,
+                             float* out_shift, cudaStream_t s) {
+  k_rescaled_epilogue<<<(n + 127) / 128, 128, 0, s>>>(ep.bias, ep.scale, ep.shift, w_scale, w_packed, n, out_scale,
+                                                      out_shift);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -1091,7 +1124,7 @@ int launch_bn_relu_bwd(const float* z, const float* g_a, int rows, int F, const 
                                                   reinterpret_cast<unsigned int*>(gz_scale_out));
     P2M_LAUNCH_OK();
     if (gz_scale_out) {
-      k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(gz_scale_out));
+      k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(gz_scale_out), 0);
       P2M_LAUNCH_OK();
     }
     return P2M_OK;

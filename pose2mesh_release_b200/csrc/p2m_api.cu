@@ -7,6 +7,7 @@
 #include <cmath>
 #include <cstring>
 #include <string>
+#include <tuple>
 #include <vector>
 
 #include "p2m_internal.h"
@@ -291,7 +292,8 @@ bool conv_on_tensor_cores(const p2m_model* m, const Layer& L, const unsigned cha
 int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpool, const float* w_ref, float* T,
                 float* wp, unsigned char* wpack, const Epilogue& ep, float* y, cudaStream_t s,
                 const float* head_wt = nullptr, float* head_z = nullptr, bool keep_wp = true, bool may_elide = false,
-                int iso_mode = 0 /* 0: every isolated row, 1: class representatives only, 2: none */) {
+                int iso_mode = 0 /* 0: every isolated row, 1: class representatives only, 2: none */,
+                const float* a_scale = nullptr /* device scalar: the basis is scaled by it before the fp16 split */) {
   const int rows = B * L.V;
   const DevLevel& g = m->levels[L.level];
   // k-major copy of the weights: what the SIMT GEMM reads, and (training, keep_wp) what backward's SIMT dT GEMM reads
@@ -326,6 +328,7 @@ int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpo
     a.wpack = wpack;
     a.ep = ep;
     a.y = y;
+    a.a_scale = a_scale;
     if (!elide) return launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s);
     a.tiles = &g.real_tiles;
     P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
@@ -498,6 +501,33 @@ int p2m_model_create(const p2m_model_desc_t* d, p2m_model_t** out) {
         }
         rel[p] = c - v;
       }
+    }
+    {
+      // exact symmetry of the fp32 values: the entries sorted by (row, col) against the transposed ones
+      std::vector<std::tuple<int, int, float>> e, et;
+      e.reserve(g.nnz);
+      et.reserve(g.nnz);
+      double r_max = 0.0;
+      for (int v = 0; v < g.V; ++v) {
+        double r = 0.0;
+        for (int p = rp[v]; p < rp[v + 1]; ++p) {
+          const float x = d->values[l][p];
+          e.emplace_back(v, d->colidx[l][p], x);
+          et.emplace_back(d->colidx[l][p], v, x);
+          r += std::fabs((double)x);
+        }
+        r_max = std::max(r_max, r);
+      }
+      std::sort(e.begin(), e.end());
+      std::sort(et.begin(), et.end());
+      g.symmetric = (e == et);
+      g.headroom_log2 = (int)std::ceil(std::log2(2.0 * r_max * r_max + 1.0));
+    }
+    if (d->n_blocks != 0 && !g.symmetric) {
+      set_error("model_create: the Laplacian of level " + std::to_string(l) +
+                " is not symmetric (the network's backward uses L~ in place of L~^T)");
+      p2m_model_destroy(m);
+      return P2M_ERR_INVALID;
     }
     int st;
     if ((st = upload(m, rowptr, &g.rowptr)) || (st = upload(m, rel, &g.reloff)) || (st = upload(m, val, &g.val)) ||
@@ -672,6 +702,30 @@ int p2m_debug_set_dw_swap(p2m_model_t* m, int enable) {
   m->dw_swap = enable ? 1 : 0;
   return P2M_OK;
 }
+int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[10]) {
+  if (!m || !out || level < 0 || level >= (int)m->levels.size() || fin <= 0 || fout <= 0) {
+    set_error("debug_conv_path: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  const DevLevel& g = m->levels[level];
+  const bool tc = (m->precision == P2M_PREC_FP16X3_TC);
+  const bool conv = tc && umma_conv_supported(g, fin, fout);
+  const bool dw = tc && umma_dw_supported(g, fin, fout);
+  const bool dt = tc && umma_conv_supported(g, fout, fin) &&
+                  umma_plain_pack_bytes(fin, fout) <= umma_wpack_bytes(((fin + 31) / 32) * 32, fout);
+  out[0] = conv;
+  out[1] = conv ? umma_conv_x_stages(g, m->split_t1 != 0, false) : 0;
+  out[2] = dw;
+  out[3] = dw ? umma_dw_x_stages(g) : 0;
+  out[4] = dt;
+  out[5] = dt ? umma_conv_x_stages(g, false, true) : 0;
+  out[6] = (g.tile_meta != nullptr && umma_tma_rows(g)) ? 1 : 0;
+  out[7] = g.tile_meta ? g.max_h1 : 0;
+  out[8] = g.tile_meta ? g.max_h2 : 0;
+  out[9] = g.n_iso;
+  return P2M_OK;
+}
+
 int p2m_debug_set_fuse_head(p2m_model_t* m, int enable) {
   if (!m) return P2M_ERR_INVALID;
   m->fuse_head = enable ? 1 : 0;
@@ -1191,8 +1245,32 @@ size_t p2m_cheb_conv_workspace_bytes(const p2m_model_t* m, int level, int batch,
   size_t rows = (size_t)batch * m->levels[level].V;
   return align_up(rows * 3 * fin * 4) + align_up((size_t)fout * 3 * fin * 4) * 2 + align_up(rows * fin * 4) +
          align_up(rows * fout * 4) + align_up(2 * (size_t)std::max(fin, fout) * 8) + align_up(2 * (size_t)fout * 4) +
-         align_up(umma_wpack_bytes(((fin + 31) / 32) * 32, fout) + 16) + ALIGN;
+         align_up(umma_wpack_bytes(((fin + 31) / 32) * 32, fout) + 16) + align_up(4 * 4) +
+         align_up(2 * (size_t)std::max(fin, fout) * 4) + ALIGN;
 }
+
+namespace {
+// The single-layer entry points take arbitrary user tensors, so on the tensor cores both fp16x3 operands are brought
+// into fp16's range first: the basis by a power of two from max|x| that leaves 2^h of headroom for T1 and T2
+// (DevLevel::headroom_log2; the kernel's a_scale, undone in its epilogue), the weights by a power of two from max|W|
+// that replaces their fixed 2^6 packing scale (undone by a rescaled epilogue).  Both are exact: the result is the one
+// an unscaled split would give wherever that split neither overflows nor loses its lo part to fp16's subnormals.
+struct RangeScales {
+  float* a_scale;  // device scalars
+  float* w_scale;
+  float* x_scale;
+  float* vec;      // [2 max(fin, fout)]: rescaled epilogue scale | shift
+};
+RangeScales take_range_scales(Bump* b, int fin, int fout) {
+  float* sc = b->take<float>(4);
+  return RangeScales{sc, sc + 1, sc + 2, b->take<float>(2 * (size_t)std::max(fin, fout))};
+}
+// w_out = W * w_scale / 2^6: what launch_umma_pack_weights / _pack_plain (x 2^6) then turn into W * w_scale
+int prescale_weights(const float* W, long long n, const RangeScales& r, float* w_out, cudaStream_t s) {
+  P2M_TRY(launch_absmax_scale(W, n, r.w_scale, s));
+  return launch_scale_by(W, n, r.w_scale, 0, 1.f / 64.f, w_out, s);
+}
+}  // namespace
 
 int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* workspace, size_t workspace_bytes,
                       p2m_stream_t stream) {
@@ -1216,17 +1294,32 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   Bump b(workspace);
   float* T = b.take<float>(rows * 3 * L.fin);
   float* wp = b.take<float>((size_t)L.fout * 3 * L.fin);
-  b.take<float>((size_t)L.fout * 3 * L.fin);
+  float* wsc = b.take<float>((size_t)L.fout * 3 * L.fin);  // range-normalised weights (tensor cores)
   b.take<float>(rows * L.fin);
   float* z = b.take<float>(rows * L.fout);
   double* sums = b.take<double>(2 * (size_t)std::max(L.fin, L.fout));
   float* sc = b.take<float>(2 * (size_t)L.fout);
   unsigned char* wpack = b.take<unsigned char>(umma_wpack_bytes(((L.fin + 31) / 32) * 32, L.fout) + 16);
+  const RangeScales rs = take_range_scales(&b, L.fin, L.fout);
+  const DevLevel& g = m->levels[a->level];
+  // on the tensor cores: range-normalised operands (take_range_scales)
+  auto conv = [&](const Epilogue& e, float* out) -> int {
+    if (!conv_on_tensor_cores(m, L, wpack)) return conv_linear(m, L, a->batch, a->x, 0, a->weight, T, wp, wpack, e, out, s);
+    P2M_TRY(prescale_weights(a->weight, (long long)L.fout * 3 * L.fin, rs, wsc, s));
+    P2M_TRY(launch_absmax_scale(a->x, (long long)rows * L.fin, rs.a_scale, s, g.headroom_log2));
+    Epilogue er;
+    er.scale = rs.vec;
+    er.shift = rs.vec + L.fout;
+    er.relu = e.relu;
+    P2M_TRY(launch_rescaled_epilogue(e, rs.w_scale, 64.f, L.fout, rs.vec, rs.vec + L.fout, s));
+    return conv_linear(m, L, a->batch, a->x, 0, wsc, T, wp, wpack, er, out, s, nullptr, nullptr, true, false, 0,
+                       rs.a_scale);
+  };
   Epilogue ep;
   if (a->bn_mode == 0) {
     ep.bias = a->bias;
     ep.relu = a->relu;
-    return conv_linear(m, L, a->batch, a->x, 0, a->weight, T, wp, wpack, ep, a->y, s);
+    return conv(ep, a->y);
   }
   if (!a->bn_weight || !a->bn_bias) {
     set_error("cheb_conv_fwd: BatchNorm parameters missing");
@@ -1242,10 +1335,10 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
     ep.scale = sc;
     ep.shift = sc + L.fout;
     ep.relu = a->relu;
-    return conv_linear(m, L, a->batch, a->x, 0, a->weight, T, wp, wpack, ep, a->y, s);
+    return conv(ep, a->y);
   }
   ep.bias = a->bias;
-  P2M_TRY(conv_linear(m, L, a->batch, a->x, 0, a->weight, T, wp, wpack, ep, z, s));
+  P2M_TRY(conv(ep, z));
   P2M_TRY(launch_col_stats(z, (int)rows, L.fout, sums, s));
   P2M_TRY(launch_bn_finalize(sums, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var,
                              a->bn_num_batches_tracked, a->save_mean, a->save_invstd, sc, sc + L.fout, s));
@@ -1279,15 +1372,26 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
   double* sums = b.take<double>(2 * (size_t)std::max(fin, fout));
   float* sc2 = b.take<float>(2 * (size_t)fout);
   unsigned char* wpack = b.take<unsigned char>(umma_wpack_bytes(((fin + 31) / 32) * 32, fout) + 16);
+  const RangeScales rs = take_range_scales(&b, fin, fout);
   float* a_scale = sc2;  // device scalar for the tensor-core paths (the forward's scale/shift slot is free here)
   const bool tc = (m->precision == P2M_PREC_FP16X3_TC);
   bool have_scale = false;
+  if (!g.symmetric) {
+    set_error("cheb_conv_bwd: the Laplacian is not symmetric; the backward kernels apply L~ where the gradient needs "
+              "L~^T");
+    return P2M_ERR_INVALID;
+  }
   P2M_TRY(launch_col_sum(a->dz, (int)rows, fout, sums, a->dbias, s));
   if (tc && umma_dw_supported(g, fin, fout)) {
     P2M_TRY(launch_absmax_scale(a->dz, (long long)rows * fout, a_scale, s));
     have_scale = true;
+    // the layer input into fp16's range as well (with the basis headroom), in U (free until the dX pass); dW then
+    // comes out multiplied by that power of two
+    P2M_TRY(launch_absmax_scale(a->x, (long long)rows * fin, rs.x_scale, s, g.headroom_log2));
+    P2M_TRY(launch_scale_by(a->x, (long long)rows * fin, rs.x_scale, 0, 1.f, U, s));
     P2M_TRY(launch_fill_zero(a->dweight, sizeof(float) * fout * 3 * fin, s));
-    P2M_TRY(launch_umma_dw(g, a->x, 0, a->batch, fin, fout, a->dz, a_scale, a->dweight, m->kernel_status, m->sm_count, s));
+    P2M_TRY(launch_umma_dw(g, U, 0, a->batch, fin, fout, a->dz, a_scale, a->dweight, m->kernel_status, m->sm_count, s));
+    P2M_TRY(launch_scale_by(a->dweight, (long long)fout * 3 * fin, rs.x_scale, 1, 1.f, a->dweight, s));
   } else {
     P2M_TRY(launch_cheb_basis(g, a->x, 0, (int)rows, fin, T, s));
     P2M_TRY(launch_fill_zero(dwp, sizeof(float) * fout * 3 * fin, s));
@@ -1298,8 +1402,14 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
     Epilogue none;
     if (tc && umma_conv_supported(g, fout, fin) && umma_plain_pack_bytes(fin, fout) <= umma_wpack_bytes(((fin + 31) / 32) * 32, fout)) {
       if (!have_scale) P2M_TRY(launch_absmax_scale(a->dz, (long long)rows * fout, a_scale, s));
+      // weights range-normalised into dwp (the SIMT weight gradient above is done with it); the plain conv's
+      // epilogue undoes the scale
+      P2M_TRY(prescale_weights(a->weight, (long long)fout * 3 * fin, rs, dwp, s));
+      none.scale = rs.vec;
+      none.shift = rs.vec + fin;
+      P2M_TRY(launch_rescaled_epilogue(Epilogue(), rs.w_scale, 64.f, fin, rs.vec, rs.vec + fin, s));
       for (int k = 0; k < 3; ++k) {
-        P2M_TRY(launch_umma_pack_plain(a->weight + k, 3, 3LL * fin, fin, fout, wpack, s));
+        P2M_TRY(launch_umma_pack_plain(dwp + k, 3, 3LL * fin, fin, fout, wpack, s));
         UmmaConvArgs u;
         u.g = &g;
         u.x = a->dz;
@@ -1310,6 +1420,7 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
         u.wpack = wpack;
         u.y = T;
         u.plain = 1;
+        u.ep = none;
         u.a_scale = a_scale;
         u.ldy = 3LL * fin;
         u.y_col0 = k * fin;

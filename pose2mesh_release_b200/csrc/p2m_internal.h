@@ -72,6 +72,10 @@ struct DevLevel {
   const int* tile_meta1_bytes = nullptr;
   int meta1_stride = 0;
   int max_h1 = 0, max_h2 = 0;
+  // L~ == L~^T exactly (the backward passes use L~ where the math needs L~^T), and h = ceil(log2(2 r^2 + 1)) for r the
+  // largest absolute row sum of L~: max|T2| <= (2 r^2 + 1) max|x|, the headroom the single-layer fp16 split leaves
+  bool symmetric = true;
+  int headroom_log2 = 0;
   // Padding-vertex elision: the fake vertices of the binary-tree reorder (lib/coarsening.py:214-258) are isolated in
   // L~ and share one diagonal value iso_diag, so on them the conv is a dense map with the combined weights
   // W0 + c W1 + (2c^2 - 1) W2.  real_tiles covers the connected rows (conv path), iso_tiles the isolated ones (plain
@@ -244,20 +248,33 @@ struct UmmaConvArgs {
   const TileSet* tiles = nullptr;
   long long* trace = nullptr;       // debug (P2M_UMMA_TRACE builds only): [8][512] event log of CTA 0
 };
-// Host: build the per-tile halo metadata of one level (uploads; device pointers appended to `owned`).
+// Host: build the per-tile halo metadata of one level (uploads; device pointers appended to `owned`).  A level whose
+// tiles exceed the metadata's 16-bit slot / entry offsets gets none (tile_meta stays null: it runs on SIMT).
 int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val, int V, DevLevel* out,
                           std::vector<void*>* owned);
 // Tiles of 128 consecutive entries of `rows` (ascending vertex ids of one level) as a TileSet (trimmed blobs).
 int build_index_tiles(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
                       TileSet* ts, std::vector<void*>* owned);
 bool umma_conv_supported(const DevLevel& g, int fin, int fout);
+// what launch_umma_conv / launch_umma_dw would select on the level's consecutive tiles (p2m_debug_conv_path)
+int umma_conv_x_stages(const DevLevel& g, bool t1_given, bool plain);
+int umma_dw_x_stages(const DevLevel& g);
+bool umma_tma_rows(const DevLevel& g);
 size_t umma_wpack_bytes(int fin, int fout);
 int launch_umma_pack_weights(const float* W /*[fout, fin*3] ref layout*/, int fin, int fout, void* wpack, cudaStream_t s);
 // B[n][k] = Bmat[n*ld_n + k*ld_k]  (n < N, k < K, K % 32 == 0) -> fp16 [hi|lo] K-blocks, one per 32 k
 size_t umma_plain_pack_bytes(int N, int K);
 int launch_umma_pack_plain(const float* Bmat, long long ld_n, long long ld_k, int N, int K, void* wpack, cudaStream_t s);
-// scale_out[0] = 2^e with max|x| * 2^e in [2^9, 2^10)  (1 if x is all zero); scratch-free, two tiny launches
-int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s);
+// scale_out[0] = 2^e with max|x| * 2^e in [2^(9-h), 2^(10-h)), h = headroom_log2  (1 if x is all zero or not
+// finite); scratch-free, two tiny launches
+int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s, int headroom_log2 = 0);
+// y[i] = x[i] * (invert ? 1 / scale[0] : scale[0]) * mul  (in place allowed; scale a device scalar)
+int launch_scale_by(const float* x, long long n, const float* scale, int invert, float mul, float* y, cudaStream_t s);
+// The epilogue of a conv whose weights were packed as W * w_scale[0] instead of W * w_packed (the fixed 2^6): per column
+// out_scale = scale * w_packed / w_scale[0] and out_shift = bias * scale + shift (absent vectors: 0 / 1 / 0), i.e. the
+// same affine map with the bias folded into the shift
+int launch_rescaled_epilogue(const Epilogue& ep, const float* w_scale, float w_packed, int n, float* out_scale,
+                             float* out_shift, cudaStream_t s);
 // dW[o, f*3+k] += sum_rows dz[row,o] * T_k(x)[row,f] on tensor cores (dw_ref zeroed by the caller)
 bool umma_dw_supported(const DevLevel& g, int fin, int fout);
 int launch_umma_dw(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, int fout, const float* dz,

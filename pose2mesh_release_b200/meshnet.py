@@ -52,9 +52,11 @@ class BakedHierarchy:
     def __init__(self, laplacians: Sequence, plan):
         self.level_size = np.array([m.shape[0] for m in laplacians], dtype=np.int32)
         self.rowptr, self.colidx, self.values = [], [], []
-        for m in laplacians:
+        for i, m in enumerate(laplacians):
             c = m.tocsr().astype(np.float32)  # noqa: keeps explicit entries
             c.sort_indices()
+            if (c != c.T).nnz:  # the backward passes apply L~ where the gradient needs L~^T
+                raise ValueError(f"Laplacian {i} is not symmetric: MeshNet's kernels need L~ == L~^T")
             self.rowptr.append(np.ascontiguousarray(c.indptr, dtype=np.int32))
             self.colidx.append(np.ascontiguousarray(c.indices, dtype=np.int32))
             self.values.append(np.ascontiguousarray(c.data, dtype=np.float32))
