@@ -245,6 +245,28 @@ int p2m_mesh_losses(const float* coord_out, const float* coord_gt, const int32_t
 int p2m_coord_loss(const float* pred, const float* target, const float* valid, int64_t n, const float* grad_scale,
                    double* sum, float* grad_out, p2m_stream_t stream);
 
+/* ---- evaluation metrics (SURVEY.md §8 row f5; lib/coord_utils.py:127-149, the datasets' compute_*_err) ----------
+ * Both take a batch of point sets pred/A, gt/B [batch, n_point, 3] (device, one device) and an optional subset of
+ * point indices (HOST int32 [n_subset], checked here: every index in [0, n_point); NULL with n_subset = 0 = all
+ * points; k = the number of points used).  Outputs are nullable, but at least one must be given.  sums (device
+ * double [batch + 1]) receives the per-sample sums of the errors and, last, their total (fp64, fixed summation order:
+ * a sample's values do not depend on its batch position).  Enqueued on `stream` of the inputs' device; the caller's
+ * current device is restored.  batch and n_point are at most 2^24.
+ *
+ * Similarity Procrustes of A[b, subset] onto B[b, subset] (rigid_transform_3D / rigid_align): fp64 centroids,
+ * centred cross-covariance and 3x3 SVD; R = Vh^T U^T with the reference's det < 0 correction, c = sum(s) / varP,
+ * t = muB - c R muA.  transform [batch, 13] = {c, R row-major, t} (double); aligned [batch, k, 3] = c R a + t;
+ * err [batch, k] = |c R a + t - b|.  A sample whose A points are all equal (varP = 0) or that holds a non-finite
+ * value gets NaN in every output; the other samples are unaffected.                                             */
+int p2m_rigid_align(const float* A, const float* B, int batch, int n_point, const int32_t* subset, int n_subset,
+                    double* transform, float* aligned, float* err, double* sums, p2m_stream_t stream);
+/* Root-aligned point errors: err [batch, k] = |(pred[b, i] - pred_root[b]) - (gt[b, i] - gt_root[b])|, roots
+ * [batch, 3] (both or neither; NULL = no root subtraction).  fp64 = 0: float32 arithmetic in numpy's order, the bits
+ * of the reference's float32 compute_*_err; fp64 = 1: fp64 arithmetic, rounded once to float32 on store.          */
+int p2m_point_errors(const float* pred, const float* gt, const float* pred_root, const float* gt_root, int batch,
+                     int n_point, const int32_t* subset, int n_subset, int fp64, float* err, double* sums,
+                     p2m_stream_t stream);
+
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),
  * entries sorted by (row, col); returns the number of clusters (or -1).  Driven by

@@ -1,0 +1,390 @@
+// Row f5 of SURVEY.md §8: the evaluation metrics of the reference's test loop on the GPU.
+//  * similarity Procrustes  coord_utils.rigid_transform_3D / rigid_align   (lib/coord_utils.py:127-149), batched
+//  * root-aligned point errors  compute_joint_err / compute_both_err  (data/Human36M/dataset.py:454-477,
+//    data/PW3D/dataset.py:263-286, data/SURREAL/dataset.py:205-226) and the per-sample errors of the datasets'
+//    evaluate methods
+// One CTA per sample (grid-stride over samples); every reduction runs in a fixed order without atomics, so a sample's
+// result is independent of its batch position, of the batch size and of the run.
+#include <cuda_runtime.h>
+
+#include <cmath>
+#include <string>
+
+#include "p2m_internal.h"
+
+namespace p2m {
+namespace {
+
+constexpr int MT = 256;          // threads per CTA
+constexpr int NW = MT / 32;      // warps per CTA
+constexpr int MAX_GRID = 4096;   // CTAs of the grid-stride loop over samples
+constexpr int MAX_BATCH = 1 << 24;
+constexpr int MAX_POINTS = 1 << 24;
+
+// v[k] <- the CTA-wide sum of v[k], the same bits in every thread: xor-shuffle tree inside each warp, then the warp
+// partials in warp order.  Ends with a barrier, so `red` can be reused by the next call.
+template <int N>
+__device__ __forceinline__ void block_sum(double (&v)[N], double (*red)[NW]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    double a = v[k];
+    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if (lane == 0) red[k][warp] = a;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < N; ++k) {
+    double a = 0.0;
+    for (int w = 0; w < NW; ++w) a += red[k][w];
+    v[k] = a;
+  }
+  __syncthreads();
+}
+
+__device__ __forceinline__ double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+// rigid_transform_3D (coord_utils.py:127-143) from the centred statistics of one sample, fp64, one thread.
+//   h[3 r + c] = sum_i (A_i - muA)_r (B_i - muB)_c / n,  varP = sum_axes var(A) (population, as np.var)
+// SVD H = U diag(s) Vh by one-sided Jacobi on the columns of H (W = H V converges to U diag(s)), singular values
+// sorted descending.  U is completed to a right-handed orthonormal basis u3 = u1 x u2, which makes the third singular
+// value signed (s3 = <w3, u3>); then  R = V diag(1, 1, det V) U^T  and  s3 *= det V  are exactly the reference's
+// R = Vh^T U^T with its `det R < 0` correction (negate s[-1] and Vh[2]), whichever sign LAPACK gave u3.
+// out = {c, R row-major, t}; a sample with varP = 0 (all points of A equal, or n = 1) or non-finite statistics gets
+// NaN throughout (the reference's 1/varP * sum(s) is 1/0 * 0 there).
+__device__ void procrustes_3x3(const double* h, double varP, const double* mu_a, const double* mu_b, double* out) {
+  bool finite = isfinite(varP);
+  for (int k = 0; k < 9; ++k) finite = finite && isfinite(h[k]);
+  for (int k = 0; k < 3; ++k) finite = finite && isfinite(mu_a[k]) && isfinite(mu_b[k]);
+  if (!finite || !(varP > 0.0)) {
+    for (int k = 0; k < 13; ++k) out[k] = nan("");
+    return;
+  }
+  double W[3][3], V[3][3];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) {
+      W[r][c] = h[3 * r + c];
+      V[r][c] = (r == c) ? 1.0 : 0.0;
+    }
+  const int P[3] = {0, 0, 1}, Q[3] = {1, 2, 2};
+  for (int sweep = 0; sweep < 40; ++sweep) {
+    bool rotated = false;
+    for (int pq = 0; pq < 3; ++pq) {
+      const int p = P[pq], q = Q[pq];
+      double alpha = 0.0, beta = 0.0, gamma = 0.0;
+      for (int r = 0; r < 3; ++r) {
+        alpha += W[r][p] * W[r][p];
+        beta += W[r][q] * W[r][q];
+        gamma += W[r][p] * W[r][q];
+      }
+      if (!(fabs(gamma) > 1e-15 * sqrt(alpha * beta))) continue;
+      const double zeta = (beta - alpha) / (2.0 * gamma);
+      const double t = copysign(1.0, zeta) / (fabs(zeta) + hypot(1.0, zeta));
+      const double cs = 1.0 / sqrt(1.0 + t * t), sn = cs * t;
+      for (int r = 0; r < 3; ++r) {
+        const double wp = W[r][p], wq = W[r][q];
+        W[r][p] = cs * wp - sn * wq;
+        W[r][q] = sn * wp + cs * wq;
+        const double vp = V[r][p], vq = V[r][q];
+        V[r][p] = cs * vp - sn * vq;
+        V[r][q] = sn * vp + cs * vq;
+      }
+      rotated = true;
+    }
+    if (!rotated) break;
+  }
+  double sv[3];
+  int ord[3] = {0, 1, 2};
+  for (int j = 0; j < 3; ++j) sv[j] = sqrt(W[0][j] * W[0][j] + W[1][j] * W[1][j] + W[2][j] * W[2][j]);
+  for (int i = 0; i < 2; ++i)  // stable sort, descending
+    for (int j = 0; j < 2 - i; ++j)
+      if (sv[ord[j]] < sv[ord[j + 1]]) {
+        const int x = ord[j];
+        ord[j] = ord[j + 1];
+        ord[j + 1] = x;
+      }
+  double w[3][3], v[3][3];  // w[j] / v[j]: column j of the sorted W / V
+  for (int j = 0; j < 3; ++j)
+    for (int r = 0; r < 3; ++r) {
+      w[j][r] = W[r][ord[j]];
+      v[j][r] = V[r][ord[j]];
+    }
+  const double s1 = sv[ord[0]], s2 = sv[ord[1]];
+  double u[3][3];
+  if (s1 > 0.0) {
+    for (int r = 0; r < 3; ++r) u[0][r] = w[0][r] / s1;
+  } else {  // H = 0: any basis
+    u[0][0] = 1.0, u[0][1] = 0.0, u[0][2] = 0.0;
+  }
+  // u2: w2 orthogonalised against u1; when w2 vanishes (rank-1 H) any unit vector orthogonal to u1
+  {
+    double x[3];
+    const double d = dot3(w[1], u[0]);
+    for (int r = 0; r < 3; ++r) x[r] = w[1][r] - d * u[0][r];
+    double nx = sqrt(dot3(x, x));
+    if (!(nx > 1e-12 * s1)) {
+      int a = 0;  // the axis least aligned with u1
+      for (int r = 1; r < 3; ++r)
+        if (fabs(u[0][r]) < fabs(u[0][a])) a = r;
+      const double e = u[0][a];
+      for (int r = 0; r < 3; ++r) x[r] = ((r == a) ? 1.0 : 0.0) - e * u[0][r];
+      nx = sqrt(dot3(x, x));
+    }
+    for (int r = 0; r < 3; ++r) u[1][r] = x[r] / nx;
+  }
+  u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];
+  u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
+  u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+  const double det_v = v[0][0] * (v[1][1] * v[2][2] - v[1][2] * v[2][1]) -
+                       v[1][0] * (v[0][1] * v[2][2] - v[0][2] * v[2][1]) +
+                       v[2][0] * (v[0][1] * v[1][2] - v[0][2] * v[1][1]);
+  const double dv = det_v < 0.0 ? -1.0 : 1.0;
+  const double s3 = dot3(w[2], u[2]) * dv;
+  const double c = (1.0 / varP) * ((s1 + s2) + s3);
+  double R[3][3];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) R[i][j] = v[0][i] * u[0][j] + v[1][i] * u[1][j] + dv * v[2][i] * u[2][j];
+  out[0] = c;
+  for (int i = 0; i < 3; ++i) {
+    for (int j = 0; j < 3; ++j) out[1 + 3 * i + j] = R[i][j];
+    out[10 + i] = -(((c * R[i][0]) * mu_a[0] + (c * R[i][1]) * mu_a[1]) + (c * R[i][2]) * mu_a[2]) + mu_b[i];
+  }
+}
+
+// Batched rigid_align on A[b, idx], B[b, idx] (idx = subset[0..k) or 0..k-1): pass 1 the centroids, pass 2 the centred
+// cross-covariance and varP, one thread the SVD and transform, pass 3 the aligned points c R a + t and their distances
+// to B.  sums[b] = sum of the sample's distances.
+__global__ void __launch_bounds__(MT) k_rigid_align(const float* __restrict__ A, const float* __restrict__ B, int batch,
+                                                    int n_point, const int* __restrict__ subset, int k,
+                                                    double* __restrict__ transform, float* __restrict__ aligned,
+                                                    float* __restrict__ err, double* __restrict__ sums) {
+  __shared__ double red[10][NW];
+  __shared__ double T[13];
+  for (int b = blockIdx.x; b < batch; b += gridDim.x) {
+    const float* a = A + (long long)b * n_point * 3;
+    const float* g = B + (long long)b * n_point * 3;
+    double m[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int i = threadIdx.x; i < k; i += MT) {
+      const long long p = subset ? subset[i] : i;
+      for (int c = 0; c < 3; ++c) {
+        m[c] += (double)a[3 * p + c];
+        m[3 + c] += (double)g[3 * p + c];
+      }
+    }
+    block_sum<6>(m, red);
+    for (int c = 0; c < 6; ++c) m[c] /= k;
+    double h[10] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int i = threadIdx.x; i < k; i += MT) {
+      const long long p = subset ? subset[i] : i;
+      double da[3], db[3];
+      for (int c = 0; c < 3; ++c) {
+        da[c] = (double)a[3 * p + c] - m[c];
+        db[c] = (double)g[3 * p + c] - m[3 + c];
+      }
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) h[3 * r + c] += da[r] * db[c];
+      h[9] += dot3(da, da);
+    }
+    block_sum<10>(h, red);
+    if (threadIdx.x == 0) {
+      for (int q = 0; q < 10; ++q) h[q] /= k;
+      procrustes_3x3(h, h[9], m, m + 3, T);
+      if (transform)
+        for (int q = 0; q < 13; ++q) transform[(long long)b * 13 + q] = T[q];
+    }
+    __syncthreads();
+    if (aligned || err || sums) {
+      double cR[9], t[3];
+      for (int q = 0; q < 9; ++q) cR[q] = T[0] * T[1 + q];
+      for (int q = 0; q < 3; ++q) t[q] = T[10 + q];
+      double es[1] = {0.0};
+      for (int i = threadIdx.x; i < k; i += MT) {
+        const long long p = subset ? subset[i] : i;
+        const double x[3] = {(double)a[3 * p], (double)a[3 * p + 1], (double)a[3 * p + 2]};
+        double d2 = 0.0;
+        for (int r = 0; r < 3; ++r) {
+          const double y = dot3(cR + 3 * r, x) + t[r];
+          if (aligned) aligned[((long long)b * k + i) * 3 + r] = (float)y;
+          const double d = y - (double)g[3 * p + r];
+          d2 += d * d;
+        }
+        const double e = sqrt(d2);
+        if (err) err[(long long)b * k + i] = (float)e;
+        es[0] += e;
+      }
+      block_sum<1>(es, red);
+      if (sums && threadIdx.x == 0) sums[b] = es[0];
+    }
+  }
+}
+
+// err[b, i] = |(P[b, idx] - pr[b]) - (G[b, idx] - gr[b])| (roots optional).  FP64 = false: float32 in numpy's order
+// (roots subtracted first, (d0^2 + d1^2) + d2^2, sqrt), each step rounded to nearest with no contraction, i.e. the
+// bits the reference's float32 numpy gives; FP64 = true: the same in fp64, rounded once on store.
+// sums[b] = the fp64 sum of the sample's errors.
+template <bool FP64>
+__global__ void __launch_bounds__(MT) k_point_errors(const float* __restrict__ P, const float* __restrict__ G,
+                                                     const float* __restrict__ pr, const float* __restrict__ gr,
+                                                     int batch, int n_point, const int* __restrict__ subset, int k,
+                                                     float* __restrict__ err, double* __restrict__ sums) {
+  __shared__ double red[1][NW];
+  for (int b = blockIdx.x; b < batch; b += gridDim.x) {
+    const float* p0 = P + (long long)b * n_point * 3;
+    const float* g0 = G + (long long)b * n_point * 3;
+    double es[1] = {0.0};
+    for (int i = threadIdx.x; i < k; i += MT) {
+      const long long p = subset ? subset[i] : i;
+      double e;
+      if (FP64) {
+        double d2 = 0.0;
+        for (int c = 0; c < 3; ++c) {
+          double x = p0[3 * p + c], y = g0[3 * p + c];
+          if (pr) {
+            x -= (double)pr[3 * b + c];
+            y -= (double)gr[3 * b + c];
+          }
+          d2 += (x - y) * (x - y);
+        }
+        e = sqrt(d2);
+      } else {
+        float d[3];
+        for (int c = 0; c < 3; ++c) {
+          float x = p0[3 * p + c], y = g0[3 * p + c];
+          if (pr) {
+            x = __fsub_rn(x, pr[3 * b + c]);
+            y = __fsub_rn(y, gr[3 * b + c]);
+          }
+          d[c] = __fsub_rn(x, y);
+        }
+        const float s = __fadd_rn(__fadd_rn(__fmul_rn(d[0], d[0]), __fmul_rn(d[1], d[1])), __fmul_rn(d[2], d[2]));
+        e = (double)__fsqrt_rn(s);
+      }
+      if (err) err[(long long)b * k + i] = (float)e;
+      es[0] += e;
+    }
+    block_sum<1>(es, red);
+    if (sums && threadIdx.x == 0) sums[b] = es[0];
+  }
+}
+
+// sums[batch] = sum of sums[0 .. batch) in a fixed order (one CTA)
+__global__ void __launch_bounds__(MT) k_batch_total(double* __restrict__ sums, int batch) {
+  __shared__ double red[1][NW];
+  double s[1] = {0.0};
+  for (int b = threadIdx.x; b < batch; b += MT) s[0] += sums[b];
+  block_sum<1>(s, red);
+  if (threadIdx.x == 0) sums[batch] = s[0];
+}
+
+// The device of the input arrays (both must be device memory of one device).
+int input_device(const char* where, const float* a, const float* b, int* dev) {
+  int devs[2];
+  const float* ptrs[2] = {a, b};
+  for (int i = 0; i < 2; ++i) {
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, ptrs[i]) != cudaSuccess ||
+        (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
+      cudaGetLastError();
+      set_error(std::string(where) + ": the point arrays must be device memory");
+      return P2M_ERR_INVALID;
+    }
+    devs[i] = attr.device;
+  }
+  if (devs[0] != devs[1]) {
+    set_error(std::string(where) + ": the point arrays are on different devices");
+    return P2M_ERR_INVALID;
+  }
+  *dev = devs[0];
+  return P2M_OK;
+}
+
+// Shared argument checks; the subset indices come from the caller and are checked here, on the host.
+int check_args(const char* where, const float* a, const float* b, int batch, int n_point, const int32_t* subset,
+               int n_subset, bool any_output) {
+  if (!a || !b || batch <= 0 || batch > MAX_BATCH || n_point <= 0 || n_point > MAX_POINTS || n_subset < 0 ||
+      (n_subset > 0) != (subset != nullptr) || !any_output) {
+    set_error(std::string(where) + ": bad argument (null input, no output, batch or n_point out of [1, 2^24], or "
+                                   "subset / n_subset inconsistent)");
+    return P2M_ERR_INVALID;
+  }
+  for (int i = 0; i < n_subset; ++i)
+    if (subset[i] < 0 || subset[i] >= n_point) {
+      set_error(std::string(where) + ": subset[" + std::to_string(i) + "] = " + std::to_string(subset[i]) +
+                " is outside [0, " + std::to_string(n_point) + ")");
+      return P2M_ERR_INVALID;
+    }
+  return P2M_OK;
+}
+
+// Stream-ordered device copy of the (host) subset, freed on the same stream after the kernels that read it.
+struct DevSubset {
+  int* ptr = nullptr;
+  cudaStream_t s;
+  explicit DevSubset(cudaStream_t st) : s(st) {}
+  int upload(const int32_t* host, int n) {
+    if (n == 0) return P2M_OK;
+    P2M_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ptr), sizeof(int) * (size_t)n, s));
+    P2M_CUDA_OK(cudaMemcpyAsync(ptr, host, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
+    return P2M_OK;
+  }
+  ~DevSubset() {
+    if (ptr) cudaFreeAsync(ptr, s);
+  }
+};
+
+inline unsigned grid_for(int batch) { return (unsigned)(batch < MAX_GRID ? batch : MAX_GRID); }
+
+}  // namespace
+}  // namespace p2m
+
+using namespace p2m;
+
+extern "C" {
+
+int p2m_rigid_align(const float* A, const float* B, int batch, int n_point, const int32_t* subset, int n_subset,
+                    double* transform, float* aligned, float* err, double* sums, p2m_stream_t stream) {
+  P2M_TRY(check_args("rigid_align", A, B, batch, n_point, subset, n_subset, transform || aligned || err || sums));
+  int dev;
+  P2M_TRY(input_device("rigid_align", A, B, &dev));
+  DeviceGuard guard(dev);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  DevSubset sub(s);
+  P2M_TRY(sub.upload(subset, n_subset));
+  const int k = n_subset > 0 ? n_subset : n_point;
+  k_rigid_align<<<grid_for(batch), MT, 0, s>>>(A, B, batch, n_point, sub.ptr, k, transform, aligned, err, sums);
+  P2M_LAUNCH_OK();
+  if (sums) {
+    k_batch_total<<<1, MT, 0, s>>>(sums, batch);
+    P2M_LAUNCH_OK();
+  }
+  return P2M_OK;
+}
+
+int p2m_point_errors(const float* pred, const float* gt, const float* pred_root, const float* gt_root, int batch,
+                     int n_point, const int32_t* subset, int n_subset, int fp64, float* err, double* sums,
+                     p2m_stream_t stream) {
+  P2M_TRY(check_args("point_errors", pred, gt, batch, n_point, subset, n_subset, err || sums));
+  if ((pred_root == nullptr) != (gt_root == nullptr)) {
+    set_error("point_errors: give both root arrays or neither");
+    return P2M_ERR_INVALID;
+  }
+  int dev;
+  P2M_TRY(input_device("point_errors", pred, gt, &dev));
+  DeviceGuard guard(dev);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  DevSubset sub(s);
+  P2M_TRY(sub.upload(subset, n_subset));
+  const int k = n_subset > 0 ? n_subset : n_point;
+  if (fp64)
+    k_point_errors<true><<<grid_for(batch), MT, 0, s>>>(pred, gt, pred_root, gt_root, batch, n_point, sub.ptr, k, err, sums);
+  else
+    k_point_errors<false><<<grid_for(batch), MT, 0, s>>>(pred, gt, pred_root, gt_root, batch, n_point, sub.ptr, k, err, sums);
+  P2M_LAUNCH_OK();
+  if (sums) {
+    k_batch_total<<<1, MT, 0, s>>>(sums, batch);
+    P2M_LAUNCH_OK();
+  }
+  return P2M_OK;
+}
+
+}  // extern "C"

@@ -70,23 +70,6 @@ struct p2m_model {
 
 namespace {
 
-// Every entry point that touches the device makes the model's device current for its own duration only: the
-// caller's current device is restored on every exit path (single-process multi-GPU callers, nn.DataParallel
-// threads, handles garbage-collected at arbitrary times).
-struct DeviceGuard {
-  int prev = -1;
-  bool switched = false;
-  explicit DeviceGuard(int dev) {
-    if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
-    if (prev != dev) switched = (cudaSetDevice(dev) == cudaSuccess);
-  }
-  ~DeviceGuard() {
-    if (switched && prev >= 0) cudaSetDevice(prev);
-  }
-  DeviceGuard(const DeviceGuard&) = delete;
-  DeviceGuard& operator=(const DeviceGuard&) = delete;
-};
-
 // A tensor-core kernel whose bounded mbarrier wait expired wrote the wait's id into the mapped host status word
 // (cheb_umma.cu: mbar_timeout).  Checked without any synchronisation at every entry point (and after the stream
 // synchronisation of the *_host entry point): the call fails instead of handing out the results of a kernel

@@ -41,6 +41,23 @@ void count_launch(int n = 1);
     if (_s != P2M_OK) return _s; \
   } while (0)
 
+// Every entry point that touches the device makes the model's device current for its own duration only: the
+// caller's current device is restored on every exit path (single-process multi-GPU callers, nn.DataParallel
+// threads, handles garbage-collected at arbitrary times).
+struct DeviceGuard {
+  int prev = -1;
+  bool switched = false;
+  explicit DeviceGuard(int dev) {
+    if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+    if (prev != dev) switched = (cudaSetDevice(dev) == cudaSuccess);
+  }
+  ~DeviceGuard() {
+    if (switched && prev >= 0) cudaSetDevice(prev);
+  }
+  DeviceGuard(const DeviceGuard&) = delete;
+  DeviceGuard& operator=(const DeviceGuard&) = delete;
+};
+
 // ---------------------------------------------------------------- device-resident hierarchy level
 // L~ of one level in CSR with RELATIVE column offsets: the neighbour of flat activation row
 // r = b*V + v is row r + reloff[p], so kernels never need (b, v) separately (block-diagonal I_B (x) L~).
