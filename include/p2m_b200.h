@@ -267,6 +267,48 @@ int p2m_point_errors(const float* pred, const float* gt, const float* pred_root,
                      int n_point, const int32_t* subset, int n_subset, int fp64, float* err, double* sums,
                      p2m_stream_t stream);
 
+/* ---- body model: batched SMPL / MANO forward (SURVEY.md §8 row f6; smplpytorch SMPL_Layer.forward,
+ * manopth ManoLayer.forward) --------------------------------------------------------------------------------------
+ * The descriptor holds HOST arrays in the reference's buffer layouts (all float32, row-major):
+ *   v_template [V, 3], shapedirs [V, 3, S], posedirs [V, 3, 9 (J - 1)], J_regressor [J, V], weights [V, J],
+ *   parents [J] (parents[0] = -1, parents[i] < i), model_betas [S] (used when the betas are absent or, under
+ *   P2M_BETAS_ZERO_MEANS_MODEL, when the whole batch's betas are zero), pose_mean [3 (J - 1)] added to the non-root
+ *   axis-angle values (MANO's hands_mean; NULL = none), joint_map [n_out_joints] (entry e >= 0: kinematic joint e;
+ *   e < 0: vertex -1 - e), scale (1 for SMPL metres, 1000 for MANO millimetres), device.
+ * Create rejects non-topological parents, out-of-range map entries and non-finite buffers with P2M_ERR_INVALID.
+ * J <= 64, S <= 512.  fp32 on the CUDA cores, three launches per forward, no host synchronisation. */
+typedef struct p2m_body_model p2m_body_model_t;
+typedef struct {
+  int32_t n_vertex, n_joint, n_betas, n_out_joints;
+  const float* v_template;
+  const float* shapedirs;
+  const float* posedirs;
+  const float* J_regressor;
+  const float* weights;
+  const int32_t* parents;
+  const float* model_betas;
+  const float* pose_mean;
+  const int32_t* joint_map;
+  float scale;
+  int32_t device;
+} p2m_body_model_desc_t;
+enum {
+  P2M_BETAS_ZERO_MEANS_MODEL = 0, /* SMPL_Layer: an all-zero (norm 0) betas batch is replaced by model_betas */
+  P2M_BETAS_AS_GIVEN = 1          /* ManoLayer: given betas are used as they are                               */
+};
+int p2m_body_model_create(const p2m_body_model_desc_t* desc, p2m_body_model_t** out);
+void p2m_body_model_destroy(p2m_body_model_t* m);
+size_t p2m_body_model_workspace_bytes(const p2m_body_model_t* m, int batch);
+/* pose [batch, 3 J] axis-angle, betas [batch, S] or NULL (= model_betas), trans [batch, 3] or NULL, all device
+ * float32 on the model's device.  trans is added when the batch's trans holds any non-zero (or NaN) value;
+ * otherwise, with center_idx >= 0, everything is re-centred on output joint center_idx.  Then * scale.
+ * verts [batch, V, 3], joints [batch, n_out_joints, 3] (device float32).  Enqueued on `stream`; decides the
+ * batch-wide betas / trans tests on the device (sync-free, CUDA-graph capturable).  A sample's result is bitwise
+ * independent of its batch position and of the batch size. */
+int p2m_body_model_forward(const p2m_body_model_t* m, const float* pose, const float* betas, int betas_rule,
+                           const float* trans, int center_idx, float* verts, float* joints, int batch,
+                           void* workspace, size_t workspace_bytes, p2m_stream_t stream);
+
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),
  * entries sorted by (row, col); returns the number of clusters (or -1).  Driven by

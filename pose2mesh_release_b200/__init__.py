@@ -7,6 +7,7 @@ Public surface (mirrors the reference's modules for this path, SURVEY.md §8b):
     graph.build_coarse_graphs (+ coarsening helpers) <- lib/graph_utils.py, lib/coarsening.py
     install.install()                                 rebinding overlay for an unmodified reference checkout
     dist.DataParallelStep                             one-process-per-GPU data parallel, single NCCL all-reduce
+    body_model.SMPLLayer / body_model.ManoLayer       <- smplpytorch SMPL_Layer, manopth ManoLayer (batched, forward)
 
 All device work is in libp2m_b200.so (csrc/, C ABI in include/p2m_b200.h); there is no CPU fallback.
 """
@@ -14,5 +15,6 @@ from . import _lib  # noqa: F401
 from .graph import build_coarse_graphs  # noqa: F401
 from .meshnet import Pose2Mesh, get_model  # noqa: F401
 from .cheby_graph_conv import graph_conv_cheby  # noqa: F401
+from .body_model import ManoLayer, SMPLLayer  # noqa: F401
 
 __version__ = "0.1.0"
