@@ -4,9 +4,11 @@
 //
 // k_cheb_t1        — T1 = L~ X for every row, written once to HBM (fp32): a 4-deep cp.async ring per 128-row tile,
 //                    gathers out of shared memory.
-// k_cheb_conv_umma — persistent CTAs; a tile is 128 consecutive vertices of one mesh (a compact patch: the reference's
-//                    binary-tree vertex order makes rows [128p,128p+128) the descendants of one coarse node), and a CTA
-//                    computes the 64 output columns [64 blockIdx.y, 64 blockIdx.y + 64) of its tiles.
+// k_cheb_conv_umma — persistent CTAs; a tile is 128 (or 64) consecutive vertices of one mesh (a compact patch: the
+//                    reference's binary-tree vertex order makes rows [128p,128p+128) the descendants of one coarse
+//                    node), and a CTA computes 64 (or 128) output columns of its tiles: 128 x 64 for the 64-wide
+//                    layers, 64 x 128 for the T1-given and plain convs of the 128- and 256-wide layers, whose A
+//                    operand is then built once per 128 output columns.
 //   * 16 producer warps build the A operand on chip, 32 features at a time: they run the second sparse product from
 //     shared memory with a tile-local CSR (the T1 rows of the tile and its 1-hop halo, staged one chunk ahead), read
 //     their own X rows straight from global memory, split every fp32 value into an fp16 (hi, lo) pair and write it
@@ -18,8 +20,8 @@
 //     through cp.async.mbarrier.arrive.noinc; thread 0 also prefetches the next tile's metadata blob.  1 thread
 //     streams the pre-packed fp16 (hi|lo) weight blocks of the CTA's column slice (cp.async.bulk, mbarrier
 //     complete_tx).
-//   * 1 warpgroup issues wgmma.mma_async (m64n64k16, f16 -> f32) on both 64-row halves of the tile into register
-//     accumulators: per 16 features three MMAs — hi*Whi + lo*Whi + hi*Wlo — an error-compensated product with ~2^-21
+//   * 1 warpgroup issues wgmma.mma_async (m64n64k16, f16 -> f32) on both 64-row halves of the tile (or both 64-column
+//     halves of the weight block) into register accumulators: per 16 features three MMAs — hi*Whi + lo*Whi + hi*Wlo — an error-compensated product with ~2^-21
 //     relative error, which is what keeps the 1e-4 fp32 parity bar (plain TF32/FP16 does not, SURVEY.md §7
 //     "hard parts" 1).  After the tile's last K-block the same warpgroup transposes the accumulator through a
 //     swizzled per-warp staging buffer so that global accesses are coalesced, and applies the fused epilogue —
@@ -332,7 +334,7 @@ struct KParams {
   int* status;
   long long* trace;  // optional [8][512] event log of CTA 0 (debug): (event << 48) | clock
   int own_table;         // 1: the tile's rows are the index list at the head of its metadata blob (TileSet), not
-                         //    the consecutive rows [128 pat, 128 pat + 128)
+                         //    the consecutive rows [TM pat, TM pat + TM) (TM = tile rows of the configuration)
   const float* head_wt;  // optional fused thin head (N == 64): epilogue writes head_z[row][12] = y_row * head_wt[64][12]
   float* head_z;
   // Dense GEMM mode (launch_umma_gemm: PoseNet's Linear layers): the A operand is PRE-PACKED like a weight image
@@ -343,7 +345,7 @@ struct KParams {
   long long wslice_bytes;  // offset of this CTA's N-slice (blockIdx.y) in the weight image
   long long wblock_stride; // bytes between consecutive K-blocks of the weight image
   int tma;           // 1: the tile's own rows of x (and t1) arrive by one 2-D TMA load each (T1-given / plain mode on
-                     //    levels whose size is a multiple of 128); with in_unpool the x box is the 64 source rows
+                     //    levels whose size is a multiple of 128); with in_unpool the x box is the TM / 2 source rows
   CUtensorMap tm_x, tm_t1;
 };
 
@@ -375,28 +377,41 @@ constexpr int REGS_LAUNCH = 80, REGS_UTIL = 40, REGS_EPI = 120;  // setmaxnreg t
 static_assert(128 * (REGS_EPI - REGS_LAUNCH) <= 128 * (REGS_LAUNCH - REGS_UTIL), "register pool balance");
 static_assert(W_XLOAD % 4 == 0 && W_EPI0 % 4 == 0 && W_EPI0 - W_XLOAD == 4, "setmaxnreg works on aligned warpgroups");
 
-// A CTA computes the N = 64 output columns [64 blockIdx.y, 64 blockIdx.y + 64) of its tiles: a 128 x 64 fp32
-// accumulator is 64 registers per thread of one warpgroup; wider layers run as several column slices.
+// Two tile shapes, both a 64-register fp32 accumulator per thread of the one MMA warpgroup:
+//   N = 64:  a CTA computes 128 tile rows x the 64 output columns [64 blockIdx.y, 64 blockIdx.y + 64); used for the
+//            64-wide layers (and the fused thin head), the dense GEMM and the split_t1 = 0 ablation.
+//   N = 128: a CTA computes 64 tile rows x the 128 output columns [128 blockIdx.y, 128 blockIdx.y + 128); used for every
+//            T1-given and plain conv with Fout % 128 == 0, so that a tile row's A operand is built once per 128 output
+//            columns instead of once per 64.  The tiles are the 64-row metadata families (DevLevel::meta64,
+//            TileSet::m64).
 // MODE 1: the production configuration — T1 given, not the plain-GEMM mode — fixed at compile time, so the on-chip first
 // sparse product, the plain path and their per-tile state drop out of the producers (registers for a deeper gather);
-// MODE 0 decides both at run time (plain GEMM, dense GEMM, the split_t1 = 0 ablation).
+// MODE 0 decides both at run time (plain GEMM, dense GEMM, the split_t1 = 0 ablation; N = 128: plain GEMM only).
+template <int N>
+__host__ __device__ constexpr int tile_rows() { return N == 128 ? 64 : TILE_M; }
 template <int N, int NS, int XS, int MODE = 0>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
+  static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
+  constexpr int TM = tile_rows<N>();  // tile rows
+  constexpr int RPT = TM / 64;        // tile rows per producer thread
+  constexpr int H = TM / 64;          // M = 64 halves of the tile (one accumulator each)
+  constexpr int ER = 16 * H;          // epilogue rows per warp of the MMA warpgroup
   constexpr bool KT1 = (MODE == 1);
   // X of the own rows straight from global memory (production mode, deep ring): the only reader of an own X row is the
   // producer thread that emits it, so staging it costs a shared-memory write plus a read back (8 % of the kernel's
   // shared-memory traffic, and more than half of the loaders' copies on index-list tiles) for nothing
   constexpr bool XDIRECT = KT1 && NS >= 3;
-  const bool plain = KT1 ? false : (p.plain != 0);
+  const bool plain = KT1 ? false : (TM == 64 || p.plain != 0);
+  constexpr int A_BYTES = TM * 128;  // one K-block of A: TM rows x (32 hi | 32 lo) fp16
   constexpr int B_BLOCK_BYTES = N * 128;
-  constexpr int SLOT_BYTES = A_BLOCK_BYTES + B_BLOCK_BYTES;
-  static_assert(N == 64, "one warpgroup holds the 128 x 64 accumulator of a CTA's column slice in registers");
+  constexpr int SLOT_BYTES = A_BYTES + B_BLOCK_BYTES;
 
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* ring = smem_raw;  // 128B-swizzled blocks need 1024-byte alignment (checked below)
   const bool t1g = KT1 ? true : (p.t1 != nullptr);
-  float* Xs = reinterpret_cast<float*>(ring + NS * SLOT_BYTES);                 // [XS][max_h2 | 128][32]
-  const size_t xs_stage_floats = (size_t)((t1g || plain) ? TILE_M : p.max_h2) * FC;
+  float* Xs = reinterpret_cast<float*>(ring + NS * SLOT_BYTES);                 // [XS][max_h2 | TM][32]
+  // (the 64-row configuration allocates no X stage where the producers read X directly: its room deepens the ring)
+  const size_t xs_stage_floats = (XDIRECT && TM == 64) ? 0 : (size_t)((t1g || plain) ? TM : p.max_h2) * FC;
   float* T1s = Xs + XS * xs_stage_floats;                                       // [1 | XS | 0][max_h1][32]
   const size_t t1_stage_floats = (size_t)p.max_h1 * FC;
   unsigned char* meta_s =
@@ -413,7 +428,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
   float* ep_mul = reinterpret_cast<float*>(flags + 4);  // [N] acc * mul + add  (weight scale, bias, folded BN)
   float* ep_add = ep_mul + N;
-  // epilogue transpose staging: [4 warps][32 rows][EC floats], 16-byte chunks XOR-swizzled by the row
+  // epilogue transpose staging: [4 warps][32 rows][EC floats], 16-byte chunks XOR-swizzled by the row (ER rows used)
   constexpr int EC = 32;
   unsigned char* epi_stage =
       reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(ep_add + N) + 127) & ~(uintptr_t)127);
@@ -446,7 +461,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     fence_barrier_init();
   }
   const float a_scale = p.a_scale ? *p.a_scale : 1.f;
-  const int ecol0 = (int)blockIdx.y * N;  // first output column of this CTA's 64-column slice
+  const int ecol0 = (int)blockIdx.y * N;  // first output column of this CTA's column slice
   for (int n = threadIdx.x; n < N; n += NUM_THREADS2) {
     const float sc = (p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f) / a_scale;
     const float sh = p.ep.scale ? p.ep.shift[ecol0 + n] : 0.f;
@@ -533,16 +548,16 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           const uint32_t x_dst = smem_u32(Xs + xs2 * xs_stage_floats) + lq * 16;
           if (p.tma) {
             if (lt == 32) {
-              const int own0 = tile2 * TILE_M;  // V is a multiple of 128: tiles never straddle meshes
-              mbar_arrive_expect_tx(xbar, (XDIRECT ? 0 : (p.in_unpool ? TILE_M / 2 : TILE_M) * 128) + (t1g ? TILE_M * 128 : 0));
+              const int own0 = tile2 * TM;  // V is a multiple of 128: tiles never straddle meshes
+              mbar_arrive_expect_tx(xbar, (XDIRECT ? 0 : (p.in_unpool ? TM / 2 : TM) * 128) + (t1g ? TM * 128 : 0));
               if (!XDIRECT)
                 tma_load_2d(smem_u32(Xs + xs2 * xs_stage_floats), &p.tm_x, c2 * FC, p.in_unpool ? own0 >> 1 : own0, xbar);
               if (t1g) tma_load_2d(smem_u32(T1s + xs2 * t1_stage_floats), &p.tm_t1, c2 * FC, own0, xbar);
             }
-            if (t1g) stage_rows(t1_dst, t1_mesh, TILE_M, h1, 0);  // only the halo rows are left
+            if (t1g) stage_rows(t1_dst, t1_mesh, TM, h1, 0);  // only the halo rows are left
           } else {
             if (t1g) stage_rows(t1_dst, t1_mesh, 0, h1, 0);
-            if (!XDIRECT) stage_rows(x_dst, x_mesh, 0, (plain || t1g) ? TILE_M : h2, sh);
+            if (!XDIRECT) stage_rows(x_dst, x_mesh, 0, (plain || t1g) ? TM : h2, sh);
             if (lt == 32) mbar_arrive(xbar);
           }
           cp_async_arrive_noinc(xbar);  // this thread's arrival once its copies have landed
@@ -567,13 +582,13 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           trace_ev(p, 1, tn, 10 + u);
           const unsigned char* wsl = p.wpack + (size_t)blockIdx.y * (size_t)p.wslice_bytes;
           if (p.apack != nullptr) {  // dense GEMM mode: the tile's pre-packed A block of chunk u rides along
-            mbar_arrive_expect_tx(smem_u32(b_ab_full + s), B_BLOCK_BYTES + A_BLOCK_BYTES);
-            bulk_g2s(smem_u32(ring + s * SLOT_BYTES), p.apack + ((size_t)tile * uses + u) * A_BLOCK_BYTES, A_BLOCK_BYTES,
+            mbar_arrive_expect_tx(smem_u32(b_ab_full + s), B_BLOCK_BYTES + A_BYTES);
+            bulk_g2s(smem_u32(ring + s * SLOT_BYTES), p.apack + ((size_t)tile * uses + u) * A_BYTES, A_BYTES,
                      smem_u32(b_ab_full + s));
           } else {
             mbar_arrive_expect_tx(smem_u32(b_ab_full + s), B_BLOCK_BYTES);
           }
-          bulk_g2s(smem_u32(ring + s * SLOT_BYTES + A_BLOCK_BYTES), wsl + (size_t)u * (size_t)p.wblock_stride, B_BLOCK_BYTES,
+          bulk_g2s(smem_u32(ring + s * SLOT_BYTES + A_BYTES), wsl + (size_t)u * (size_t)p.wblock_stride, B_BLOCK_BYTES,
                    smem_u32(b_ab_full + s));
         }
       }
@@ -582,8 +597,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   } else if (warp >= W_EPI0) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_EPI));
     // ------------------------------------------------------------ MMA + epilogue warpgroup
-    // wgmma into register accumulators: the 128-row tile is two M = 64 halves, warp wq of the warpgroup holds rows
-    // 16 wq .. 16 wq + 15 of each half (its 32 "epilogue rows": local row lr <-> tile row 64 (lr / 16) + 16 wq + lr % 16).
+    // wgmma into register accumulators, two 64 x 64 ones (m64n64): for N = 64 the two M = 64 row halves of the 128-row
+    // tile, for N = 128 the two 64-column halves of the 64-row tile (acc[h][j] then holds exactly what element j + 32 h
+    // of an m64n128 fragment would: the 128-column instruction itself needs more than the 80 registers ptxas allocates
+    // the kernel with).  Warp wq of the warpgroup holds rows 16 wq .. 16 wq + 15 of each row half (its ER "epilogue
+    // rows": local row lr <-> tile row 64 (lr / 16) + 16 wq + lr % 16).
     // A thread's fragment covers two columns of every 8-column group, so storing it directly would scatter; the rows are
     // transposed through a small per-warp staging buffer so that a warp-wide 16-byte access covers whole 128-byte row
     // pieces, and the fused epilogue (affine, ReLU, residual) runs in that layout, where the residual reads coalesce.
@@ -592,11 +610,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     constexpr int RPI = 32 / CPR;           // rows covered by one warp-wide 16-byte access
     const uint32_t stg = smem_u32(epi_stage) + (uint32_t)wq * (32 * EC * 4);
     const int prow = lane / CPR, pc = lane % CPR;
-    constexpr int NP = 32 / RPI;            // phase-2 rows (pieces) per thread and sub-slab
+    constexpr int NP = ER / RPI;            // phase-2 rows (pieces) per thread and sub-slab
     int colk[2];  // column (inside a sub-slab) of the 16-byte chunk this thread handles for rows of swizzle class k
 #pragma unroll
     for (int k = 0; k < 2; ++k) colk[k] = (int)(((uint32_t)pc ^ (uint32_t)((k * RPI + prow) & 7)) << 2);
-    const int trow = (lane >> 4) * 64 + wq * 16 + (lane & 15);  // tile row of local row `lane`
+    const int trow = (lane >> 4) * 64 + wq * 16 + (lane & 15);  // tile row of local row `lane` (lane < ER)
     const int uses = plain ? n_chunk : n_use;
     uint32_t ucnt = 0;
     int it = 0;
@@ -607,10 +625,12 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       int* own_w = own_s + wq * 32;
       {
         int v;
-        if (p.own_table) {
+        if (lane >= ER) {
+          v = -1;
+        } else if (p.own_table) {
           v = __ldg(reinterpret_cast<const int*>(p.meta + (size_t)pat * p.meta_stride + 64) + trow);
         } else {
-          v = pat * TILE_M + trow;
+          v = pat * TM + trow;
           if (v >= p.V) v = -1;
         }
         __syncwarp();  // the previous tile's readers of own_w are done
@@ -623,7 +643,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       if (p.ep.res != nullptr) {
         // pull this tile's residual rows into L2 while its main loop is still running
         const int lpr = ((p.apack != nullptr ? N : p.ep.res_F) * 4 + 127) >> 7;
-        for (int j = lane; j < 32 * lpr; j += 32) {
+        for (int j = lane; j < ER * lpr; j += 32) {
           const int rr = j / lpr, ln = j - rr * lpr;
           const int vtx = own_w[rr];
           if (vtx >= 0) {
@@ -642,13 +662,14 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         const uint32_t s = ucnt % NS;
         mbar_wait(smem_u32(b_ab_full + s), (ucnt / NS) & 1, abort_flag, p.status, 6);
         const uint32_t a0 = smem_u32(ring + s * SLOT_BYTES);
-        const uint64_t db = make_desc_sw128(a0 + A_BLOCK_BYTES);
         wg_fence();
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           // A block columns: [hi 0..31 | lo 32..63], B block columns: [Whi 0..31 | Wlo 32..63] (fp16); a 16-element
-          // K step is 32 bytes = +2 in the descriptor's start-address field; rows 64..127 start 8 KB further on
-          const uint64_t da = make_desc_sw128(a0 + (uint32_t)h * (64 * 128));
+          // K step is 32 bytes = +2 in the descriptor's start-address field; rows 64..127 of either block (A: tile
+          // rows, N = 64; B: output columns, N = 128) start 8 KB further on
+          const uint64_t da = make_desc_sw128(a0 + (TM == 128 ? (uint32_t)h * (64 * 128) : 0u));
+          const uint64_t db = make_desc_sw128(a0 + A_BYTES + (TM == 64 ? (uint32_t)h * (64 * 128) : 0u));
           wgmma_m64n64<0, 0>(acc[h], da + 0, db + 0);  // hi * Whi
           wgmma_m64n64<0, 0>(acc[h], da + 2, db + 2);
           wgmma_m64n64<0, 0>(acc[h], da + 4, db + 0);  // lo * Whi
@@ -665,16 +686,17 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       // phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by row)
       auto stage_slab = [&](int cb) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < H; ++h)
 #pragma unroll
           for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
               const int lr = 16 * h + (lane >> 2) + 8 * r;
               const int cc = 8 * jj + 2 * (lane & 3);
-              const int j = 4 * (cb / 8 + jj) + 2 * r;
+              const int ah = TM == 128 ? h : cb / 64;                 // row half / column half of the accumulator
+              const int j = 4 * ((TM == 128 ? cb : cb % 64) / 8 + jj) + 2 * r;
               sts_f2(stg + lr * (EC * 4) + ((((uint32_t)(cc >> 2)) ^ (uint32_t)(lr & 7)) << 4) + (cc & 3) * 4,
-                     acc[h][j], acc[h][j + 1]);
+                     acc[ah][j], acc[ah][j + 1]);
             }
         __syncwarp();
       };
@@ -771,13 +793,16 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
 
     constexpr int T1_ROWS = 4;  // max_h1 <= 256 rows over 64 row groups (checked on the host)
     uint32_t t1_row[T1_ROWS], t1_e[T1_ROWS];
-    uint32_t row0 = 0, row1 = 0, r0e = 0, r1e = 0, ent_a = 0;
+    // this thread's tile rows (RPT = 1 or 2: row groups rg and 64 + rg of the tile's row order) and their CSR extents
+    uint32_t row[RPT], re[RPT], ent_a = 0;
     int ptn = 0;
-    // A/B ring cursor (slot, phase parity) kept incrementally, and the four store offsets of this thread's two rows
-    // inside an A block (first / second 8-byte store of each row: odd row groups store lo first, see emit()) —
-    // per-tile constants: the hot loop carries no modulo, division or swizzle arithmetic
+    // A/B ring cursor (slot, phase parity) kept incrementally, and the store offsets of this thread's rows inside an
+    // A block (first / second 8-byte store of each row: odd row groups store lo first, see emit()) — per-tile
+    // constants: the hot loop carries no modulo, division or swizzle arithmetic
     uint32_t slot = 0, spar = 0;
-    uint32_t so_f[2] = {0, 0}, so_s[2] = {0, 0};
+    uint32_t so_f[RPT], so_s[RPT];
+#pragma unroll
+    for (int ps = 0; ps < RPT; ++ps) row[ps] = re[ps] = so_f[ps] = so_s[ps] = 0;
     const bool odd = (rg & 1) != 0;
     auto next_slot = [&]() {
       if (++slot == (uint32_t)NS) {
@@ -787,8 +812,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     };
 
     const int xsh = (p.tma && p.in_unpool) ? 1 : 0;  // TMA-staged unpooled input: staged row = tile row >> 1
-    const float* xp0 = nullptr;  // XDIRECT: this thread's two own X rows (nullptr: empty slot), at its 16-byte column
-    const float* xp1 = nullptr;
+    const float* xp[RPT];  // XDIRECT: this thread's own X rows (nullptr: empty slot), at its 16-byte column
+#pragma unroll
+    for (int ps = 0; ps < RPT; ++ps) xp[ps] = nullptr;
     int it = 0, c = -1;
     for (int g = 0; g < n_stage; ++g) {
       if (++c == n_chunk) {
@@ -797,10 +823,12 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       }
       const int m = it & 1;
       const int xs = g % XS;
-      float4 xd0 = make_float4(0.f, 0.f, 0.f, 0.f), xd1 = xd0;
-      if (XDIRECT && c != 0) {  // in flight while the stage wait and the gather run (first chunk: below, after the tile setup)
-        if (xp0) xd0 = __ldg(reinterpret_cast<const float4*>(xp0 + c * FC));
-        if (xp1) xd1 = __ldg(reinterpret_cast<const float4*>(xp1 + c * FC));
+      float4 xd[RPT];
+#pragma unroll
+      for (int ps = 0; ps < RPT; ++ps) {
+        xd[ps] = make_float4(0.f, 0.f, 0.f, 0.f);
+        // in flight while the stage wait and the gather run (first chunk: below, after the tile setup)
+        if (XDIRECT && c != 0 && xp[ps]) xd[ps] = __ldg(reinterpret_cast<const float4*>(xp[ps] + c * FC));
       }
       if (tid == 0) trace_ev(p, 0, ptn, 1);
       mbar_wait(smem_u32(b_x_full + xs), (g / XS) & 1, abort_flag, p.status, 9);
@@ -824,31 +852,27 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
             t1_e[t] = lds_u16(rp_a + 2 * i) | (lds_u16(rp_a + 2 * i + 2) << 16);
           }
         }
-        row0 = lds_u16(ord2_a + 2 * rg);
-        row1 = lds_u16(ord2_a + 2 * (64 + rg));
-        r0e = lds_u16(rp_a + 2 * row0) | (lds_u16(rp_a + 2 * row0 + 2) << 16);
-        r1e = lds_u16(rp_a + 2 * row1) | (lds_u16(rp_a + 2 * row1 + 2) << 16);
-        if (plain) {  // plain GEMM: the thread's rows are the consecutive slots rg and 64 + rg
-          row0 = rg;
-          row1 = 64 + rg;
-        }
 #pragma unroll
-        for (int ps = 0; ps < 2; ++ps) {
-          const uint32_t i = ps ? row1 : row0;
+        for (int ps = 0; ps < RPT; ++ps) {
+          // plain GEMM: the thread's rows are the consecutive slots rg (and 64 + rg)
+          row[ps] = plain ? (uint32_t)(64 * ps + rg) : lds_u16(ord2_a + 2 * (64 * ps + rg));
+          re[ps] = plain ? 0u : (lds_u16(rp_a + 2 * row[ps]) | (lds_u16(rp_a + 2 * row[ps] + 2) << 16));
+          const uint32_t i = row[ps];
           const uint32_t a_hi = sw128_off(i, q >> 1) + (q & 1) * 8, a_lo = sw128_off(i, 4 + (q >> 1)) + (q & 1) * 8;
           so_f[ps] = odd ? a_lo : a_hi;
           so_s[ps] = odd ? a_hi : a_lo;
         }
         if (XDIRECT) {
-          const int* halo = reinterpret_cast<const int*>(mb + hdr->off_halo);  // slots 0..127 = the tile's own rows
-          const int v0 = halo[row0], v1 = halo[row1];
+          const int* halo = reinterpret_cast<const int*>(mb + hdr->off_halo);  // slots 0..TM-1 = the tile's own rows
           const int sh = p.in_unpool ? 1 : 0;
           const long long mesh_row0 = (long long)((blockIdx.x + (unsigned)it * gridDim.x) / (unsigned)p.P) * p.V;
           const float* xm = p.x + (mesh_row0 >> sh) * p.fin + q * 4;
-          xp0 = (v0 >= 0) ? xm + (size_t)((uint32_t)v0 >> sh) * (uint32_t)p.fin : nullptr;
-          xp1 = (v1 >= 0) ? xm + (size_t)((uint32_t)v1 >> sh) * (uint32_t)p.fin : nullptr;
-          if (xp0) xd0 = __ldg(reinterpret_cast<const float4*>(xp0));
-          if (xp1) xd1 = __ldg(reinterpret_cast<const float4*>(xp1));
+#pragma unroll
+          for (int ps = 0; ps < RPT; ++ps) {
+            const int v = halo[row[ps]];
+            xp[ps] = (v >= 0) ? xm + (size_t)((uint32_t)v >> sh) * (uint32_t)p.fin : nullptr;
+            if (xp[ps]) xd[ps] = __ldg(reinterpret_cast<const float4*>(xp[ps]));
+          }
         }
       }
       const uint32_t xs_q = smem_u32(Xs + xs * xs_stage_floats) + q * 16;
@@ -859,7 +883,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         mbar_wait(smem_u32(b_ab_empty + s), spar ^ 1u, abort_flag, p.status, 10);
         const uint32_t ablk = ring_a + s * SLOT_BYTES;
 #pragma unroll
-        for (int ps = 0; ps < 2; ++ps) {
+        for (int ps = 0; ps < RPT; ++ps) {
           const uint32_t i = ps * 64 + rg;
           float4 v = lds_f4(xs_q + (i >> xsh) * 128);
           v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
@@ -891,21 +915,21 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         producer_barrier();
         if (tid == 0) trace_ev(p, 0, ptn, 5);
       }
-      // (2) split to fp16 (hi, lo) and write the three K-blocks of the two tile rows this thread finishes.  The X and
+      // (2) split to fp16 (hi, lo) and write the three K-blocks of the tile rows this thread finishes.  The X and
       //     T1 blocks go first: they need no gather, so the tensor core starts on them while (3) the second sparse
       //     product T2 = 2 L~ T1 - X is still being gathered (with a 2-deep ring, N = 256, the T2 block re-uses the X
       //     block's slot and would otherwise wait for its MMAs).  NS >= 3: ONE generic->async proxy fence for all
       //     three blocks (the fence drains the thread's outstanding shared stores and is expensive); NS < 3: one per
       //     block.  Odd row groups store lo first: a warp then covers both 64-byte halves of its rows per store.
       const uint32_t slot0 = slot;
-      auto emit = [&](const float4& v0, const float4& v1) {
+      auto emit = [&](const float4 (&vv)[RPT]) {
         const uint32_t s = slot;
         if (NS < 3) mbar_wait(smem_u32(b_ab_empty + s), spar ^ 1u, abort_flag, p.status, 10);
         const uint32_t ablk = ring_a + s * SLOT_BYTES;
 #pragma unroll
-        for (int ps = 0; ps < 2; ++ps) {
+        for (int ps = 0; ps < RPT; ++ps) {
           uint2 hi, lo;
-          float4 v = ps ? v1 : v0;
+          float4 v = vv[ps];
           if (p.a_scale != nullptr) {  // backward-data pass: gradients are scaled into fp16's range (power of two)
             v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
           }
@@ -923,26 +947,29 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         }
         next_slot();
       };
+      float4 x[RPT], t1v[RPT], t2[RPT];
       if (NS < 3) {
-        const float4 x0 = lds_f4(xs_q + (row0 >> xsh) * 128), x1 = lds_f4(xs_q + (row1 >> xsh) * 128);
-        emit(x0, x1);
-        {
-          const float4 t10 = lds_f4(t1s_q + row0 * 128), t11 = lds_f4(t1s_q + row1 * 128);
-          emit(t10, t11);
-        }
-        const float4 g0 = gather_row4(ent_a, r0e & 0xFFFFu, r0e >> 16, t1s_q);
-        const float4 g1 = gather_row4(ent_a, r1e & 0xFFFFu, r1e >> 16, t1s_q);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) x[ps] = lds_f4(xs_q + (row[ps] >> xsh) * 128);
+        emit(x);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) t1v[ps] = lds_f4(t1s_q + row[ps] * 128);
+        emit(t1v);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) t2[ps] = gather_row4(ent_a, re[ps] & 0xFFFFu, re[ps] >> 16, t1s_q);
         if (tid == 0) trace_ev(p, 0, ptn, 6);
-        emit(cheb_t2(g0, x0),
-             cheb_t2(g1, x1));
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) t2[ps] = cheb_t2(t2[ps], x[ps]);
+        emit(t2);
       } else {
         // deep ring: gather first, then the three blocks back to back (measured faster than the early X/T1 emit:
         // the gather then overlaps the previous chunk's tail instead of this chunk's own stores)
-        const float4 g0 = gather_row4(ent_a, r0e & 0xFFFFu, r0e >> 16, t1s_q);
-        const float4 g1 = gather_row4(ent_a, r1e & 0xFFFFu, r1e >> 16, t1s_q);
-        const float4 x0 = XDIRECT ? xd0 : lds_f4(xs_q + (row0 >> xsh) * 128);
-        const float4 x1 = XDIRECT ? xd1 : lds_f4(xs_q + (row1 >> xsh) * 128);
-        const float4 t10 = lds_f4(t1s_q + row0 * 128), t11 = lds_f4(t1s_q + row1 * 128);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) t2[ps] = gather_row4(ent_a, re[ps] & 0xFFFFu, re[ps] >> 16, t1s_q);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) x[ps] = XDIRECT ? xd[ps] : lds_f4(xs_q + (row[ps] >> xsh) * 128);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) t1v[ps] = lds_f4(t1s_q + row[ps] * 128);
         if (tid == 0) trace_ev(p, 0, ptn, 6);
         {
           // one wait for the chunk's three slots: the MMA issuer commits them in order, so the last one being free
@@ -954,10 +981,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           }
           mbar_wait(smem_u32(b_ab_empty + s2), p2 ^ 1u, abort_flag, p.status, 10);
         }
-        emit(x0, x1);
-        emit(t10, t11);
-        emit(cheb_t2(g0, x0),
-             cheb_t2(g1, x1));
+        emit(x);
+        emit(t1v);
+#pragma unroll
+        for (int ps = 0; ps < RPT; ++ps) t2[ps] = cheb_t2(t2[ps], x[ps]);
+        emit(t2);
       }
       if (NS >= 3) {
         fence_async_proxy();
@@ -1478,25 +1506,38 @@ const bool g_umma_tma = [] { const char* e = std::getenv("P2M_UMMA_TMA"); return
 
 // mode: 0 = fused (X with its 2-hop halo staged, T1 recomputed on chip), 1 = T1 given, 2 = plain GEMM
 inline int epi_stage_bytes(int) { return 4 * 32 * 32 * 4; }  // per-warp transpose staging
+// N = 128: the 64-row configuration (64-row tiles; in mode 1 with NS >= 3 no X stage: the producers read X directly)
 size_t smem_bytes_dims(int N, int NS, int XS, int max_h1, int max_h2, int meta_stride, int mode) {
-  const size_t fixed = 1024 + (size_t)NS * (A_BLOCK_BYTES + N * 128) + 8 * (2 * NS + 2 * XS + 8) + 16 +
+  const int tm = N == 128 ? 64 : TILE_M;
+  const size_t fixed = 1024 + (size_t)NS * (tm * 128 + N * 128) + 8 * (2 * NS + 2 * XS + 8) + 16 +
                        2 * (size_t)N * 4 + 16 + 128 + (size_t)epi_stage_bytes(N) + 4 * 32 * 4 +
                        (N == 64 ? 64 * 12 * 4 : 0);
-  if (mode == 1) return fixed + (size_t)XS * TILE_M * FC * 4 + (size_t)XS * max_h1 * FC * 4 + 2 * (size_t)meta_stride;
-  if (mode == 2) return fixed + (size_t)XS * TILE_M * FC * 4 + 2 * (size_t)meta_stride;
+  const size_t xs_rows = (mode == 1 && N == 128 && NS >= 3) ? 0 : (size_t)tm;
+  if (mode == 1) return fixed + (size_t)XS * xs_rows * FC * 4 + (size_t)XS * max_h1 * FC * 4 + 2 * (size_t)meta_stride;
+  if (mode == 2) return fixed + (size_t)XS * tm * FC * 4 + 2 * (size_t)meta_stride;
   return fixed + (size_t)XS * max_h2 * FC * 4 + (size_t)max_h1 * FC * 4 + 2 * (size_t)meta_stride;
 }
 size_t smem_bytes_for(int N, int NS, int XS, const DevLevel& g, int mode = 0) {
   return smem_bytes_dims(N, NS, XS, g.max_h1, g.max_h2, mode ? g.meta1_stride : g.meta_stride, mode);
 }
-// the same for an explicit launch: the level's consecutive tiles, or the tile family the caller selected
+// the tile metadata a launch with N output columns per CTA runs on: the level's consecutive tiles or the tile family the
+// caller selected, 128-row blobs for N = 64 and 64-row blobs for N = 128
+const TileBlobs& launch_tiles(int N, const UmmaConvArgs& a) {
+  if (a.tiles != nullptr) return N == 128 ? a.tiles->m64 : *a.tiles;
+  return a.g->meta64;  // N = 128 only: N = 64 launches on consecutive tiles read the DevLevel fields
+}
+// the same for an explicit launch
 size_t smem_bytes_args(int N, int NS, int XS, const UmmaConvArgs& a) {
   const int mode = a.plain ? 2 : (a.t1 != nullptr ? 1 : 0);
-  if (a.tiles != nullptr) return smem_bytes_dims(N, NS, XS, a.tiles->max_h1, a.tiles->max_h1, a.tiles->stride, mode);
+  if (a.tiles != nullptr || N == 128) {
+    const TileBlobs& t = launch_tiles(N, a);
+    return smem_bytes_dims(N, NS, XS, t.max_h1, t.max_h1, t.stride, mode);
+  }
   return smem_bytes_for(N, NS, XS, *a.g, mode);
 }
 constexpr size_t SMEM_LIMIT = 227 * 1024;
-constexpr int CONV_N = 64;  // output columns per CTA of the conv kernel (one column slice)
+constexpr int CONV_N = 64;  // output columns per CTA of the 128-row conv configuration (one column slice)
+constexpr int WIDE_N = 128; // ... and of the 64-row configuration (T1-given and plain convs with Fout % 128 == 0)
 inline int ring_stages(int) { return 3; }
 // X staging depth: 2 (prefetch the next chunk's halo during the current chunk) when it fits, else 1
 inline int x_stages(int N, const DevLevel& g) {
@@ -1552,6 +1593,7 @@ template <int N, int NS, int XS, int MODE = 0>
 int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
   if (MODE == 0 && a.t1 != nullptr && !a.plain)  // the production configuration has its own instantiation
     return launch_cfg<N, NS, XS, 1>(a, status, zero_row, sm_count, s);
+  constexpr int TM = tile_rows<N>();
   const DevLevel& g = *a.g;
   const int mode = a.plain ? 2 : (a.t1 != nullptr ? 1 : 0);
   const size_t smem = smem_bytes_args(N, NS, XS, a);
@@ -1570,14 +1612,15 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.max_h1 = g.max_h1;
   p.max_h2 = g.max_h2;
   p.own_table = 0;
-  if (a.tiles != nullptr) {  // index-list tiles (mode 1 / 2 only, checked by the caller)
-    p.P = a.tiles->n_pattern;
-    p.meta = a.tiles->meta;
-    p.meta_bytes = a.tiles->bytes;
-    p.meta_stride = a.tiles->stride;
-    p.max_h1 = a.tiles->max_h1;
-    p.max_h2 = a.tiles->max_h1;
-    p.own_table = 1;
+  if (a.tiles != nullptr || N == 128) {  // index-list tiles (mode 1 / 2 only, checked by the caller), 64-row blobs
+    const TileBlobs& t = launch_tiles(N, a);
+    p.P = t.n_pattern;
+    p.meta = t.meta;
+    p.meta_bytes = t.bytes;
+    p.meta_stride = t.stride;
+    p.max_h1 = t.max_h1;
+    p.max_h2 = t.max_h1;
+    p.own_table = a.tiles != nullptr ? 1 : 0;
   }
   p.n_tiles = a.batch * p.P;
   p.wpack = static_cast<const unsigned char*>(a.wpack);
@@ -1603,8 +1646,8 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
   if ((a.t1 != nullptr || a.plain) && a.tiles == nullptr && g.V % TILE_M == 0 && g_umma_tma) {
     const long long rows = (long long)a.batch * g.V;
-    bool ok = make_row_tmap(&p.tm_x, a.x, a.in_unpool ? rows / 2 : rows, a.fin, a.in_unpool ? TILE_M / 2 : TILE_M);
-    if (ok && a.t1 != nullptr) ok = make_row_tmap(&p.tm_t1, a.t1, rows, a.fin, TILE_M);
+    bool ok = make_row_tmap(&p.tm_x, a.x, a.in_unpool ? rows / 2 : rows, a.fin, a.in_unpool ? TM / 2 : TM);
+    if (ok && a.t1 != nullptr) ok = make_row_tmap(&p.tm_t1, a.t1, rows, a.fin, TM);
     p.tma = ok ? 1 : 0;
   }
   const int n_slices = a.fout / N;
@@ -1614,8 +1657,21 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   return P2M_OK;
 }
 
+// 64 x 128 configuration: the deepest A/B ring (6 slots = two chunks: the producers run a chunk ahead of the MMAs,
+// or 3 = one chunk) and X staging depth that fit, the ring first
+int launch_wide(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
+  constexpr int N = WIDE_N;
+  if (smem_bytes_args(N, 6, 2, a) <= SMEM_LIMIT) return launch_cfg<N, 6, 2>(a, status, zero_row, sm_count, s);
+  if (smem_bytes_args(N, 6, 1, a) <= SMEM_LIMIT) return launch_cfg<N, 6, 1>(a, status, zero_row, sm_count, s);
+  if (smem_bytes_args(N, 3, 2, a) <= SMEM_LIMIT) return launch_cfg<N, 3, 2>(a, status, zero_row, sm_count, s);
+  if (smem_bytes_args(N, 3, 1, a) <= SMEM_LIMIT) return launch_cfg<N, 3, 1>(a, status, zero_row, sm_count, s);
+  set_error("umma_conv: tile family does not fit shared memory");
+  return P2M_ERR_INVALID;
+}
+
 int launch_n(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
   constexpr int N = CONV_N, NS = 3;
+  if ((a.t1 != nullptr || a.plain) && a.fout % WIDE_N == 0) return launch_wide(a, status, zero_row, sm_count, s);
   if (a.t1 != nullptr || a.plain) {
     if (smem_bytes_args(N, NS, 2, a) <= SMEM_LIMIT) return launch_cfg<N, NS, 2>(a, status, zero_row, sm_count, s);
     if (smem_bytes_args(N, NS, 1, a) > SMEM_LIMIT) {
@@ -1655,18 +1711,18 @@ void balance_store_halves(std::vector<unsigned short>* ord) {
   }
 }
 
-// Trimmed blob of one tile whose 128 own rows are given by an index list (-1 = empty slot): own rows, their 1-hop
-// halo, the CSR of the own rows with staged-row slots as columns, the own rows in length-sorted order.
-bool make_indexed_blob(const std::vector<int>& own, const int* rowptr, const int* colidx, const float* val,
+// Trimmed blob of one tile whose tm (128 or 64) own rows are given by an index list (-1 = empty slot): own rows, their
+// 1-hop halo, the CSR of the own rows with staged-row slots as columns, the own rows in length-sorted order.
+bool make_indexed_blob(const std::vector<int>& own, int tm, const int* rowptr, const int* colidx, const float* val,
                        std::vector<int>* slot_of, std::vector<unsigned char>* blob, int* h1_out) {
   std::vector<int> halo(own);
   int n_rows = 0;
-  for (int i = 0; i < TILE_M; ++i)
+  for (int i = 0; i < tm; ++i)
     if (own[i] >= 0) {
       (*slot_of)[own[i]] = i;
       ++n_rows;
     }
-  for (int i = 0; i < TILE_M; ++i) {
+  for (int i = 0; i < tm; ++i) {
     if (own[i] < 0) continue;
     for (int e = rowptr[own[i]]; e < rowptr[own[i] + 1]; ++e) {
       const int v = colidx[e];
@@ -1677,9 +1733,9 @@ bool make_indexed_blob(const std::vector<int>& own, const int* rowptr, const int
     }
   }
   const int h1 = (int)halo.size();
-  std::vector<unsigned short> rp(TILE_M + 1, 0);
+  std::vector<unsigned short> rp(tm + 1, 0);
   std::vector<unsigned int> ent;
-  for (int i = 0; i < TILE_M; ++i) {
+  for (int i = 0; i < tm; ++i) {
     if (own[i] >= 0)
       for (int e = rowptr[own[i]]; e < rowptr[own[i] + 1]; ++e) {
         unsigned int bits;
@@ -1693,11 +1749,13 @@ bool make_indexed_blob(const std::vector<int>& own, const int* rowptr, const int
     if (v >= 0) (*slot_of)[v] = -1;
   const int nnz = (int)(ent.size() / 2);
   if (h1 > 512 || nnz > 65535) return false;
-  std::vector<unsigned short> ord2(TILE_M);
-  for (int i = 0; i < TILE_M; ++i) ord2[i] = (unsigned short)i;
+  std::vector<unsigned short> ord2(tm);
+  for (int i = 0; i < tm; ++i) ord2[i] = (unsigned short)i;
   std::stable_sort(ord2.begin(), ord2.end(), [&](unsigned short a, unsigned short b2) {
     return (int)rp[a + 1] - (int)rp[a] > (int)rp[b2 + 1] - (int)rp[b2];
   });
+  // 64-row tiles: one row per producer thread, row group rg = position rg, so the half-warp pairs are the same aligned
+  // positions (0,1), (2,3) of each group of four as for 128 rows (where a thread's second row sits 64 positions on)
   balance_store_halves(&ord2);
   TileHeader t{};
   t.n_rows = n_rows;
@@ -1706,33 +1764,33 @@ bool make_indexed_blob(const std::vector<int>& own, const int* rowptr, const int
   t.nnz = nnz;
   int o1 = 64;
   t.off_halo = o1; o1 += up16(h1 * 4);
-  t.off_rp = o1;   o1 += up16((TILE_M + 1) * 2);
+  t.off_rp = o1;   o1 += up16((tm + 1) * 2);
   t.off_ent = o1;  o1 += up16(nnz * 8);
-  t.off_ord2 = o1; o1 += up16(TILE_M * 2);
+  t.off_ord2 = o1; o1 += up16(tm * 2);
   t.off_ord1 = t.off_ord2;
   t.bytes = o1;
   blob->assign(o1, 0);
   std::memcpy(blob->data(), &t, sizeof(t));
   std::memcpy(blob->data() + t.off_halo, halo.data(), (size_t)h1 * 4);
-  std::memcpy(blob->data() + t.off_rp, rp.data(), (TILE_M + 1) * 2);
+  std::memcpy(blob->data() + t.off_rp, rp.data(), (tm + 1) * 2);
   if (nnz) std::memcpy(blob->data() + t.off_ent, ent.data(), (size_t)nnz * 8);
-  std::memcpy(blob->data() + t.off_ord2, ord2.data(), TILE_M * 2);
+  std::memcpy(blob->data() + t.off_ord2, ord2.data(), tm * 2);
   *h1_out = h1;
   return true;
 }
 
-// Tiles of 128 consecutive entries of `rows` (ascending vertex ids), uploaded as one TileSet.
-int build_tileset(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
-                  TileSet* ts, std::vector<void*>* owned) {
-  const int P = ((int)rows.size() + TILE_M - 1) / TILE_M;
+// Tiles of tm consecutive entries of `rows` (ascending vertex ids), uploaded as one set of blobs.
+int build_blobs(const std::vector<int>& rows, int tm, const int* rowptr, const int* colidx, const float* val, int V,
+                TileBlobs* ts, std::vector<void*>* owned) {
+  const int P = ((int)rows.size() + tm - 1) / tm;
   std::vector<std::vector<unsigned char>> blobs(P);
   std::vector<int> slot_of(V, -1);
   int stride = 0, max_h1 = 0;
   for (int pt = 0; pt < P; ++pt) {
-    std::vector<int> own(TILE_M, -1);
-    for (int i = 0; i < TILE_M && pt * TILE_M + i < (int)rows.size(); ++i) own[i] = rows[pt * TILE_M + i];
+    std::vector<int> own(tm, -1);
+    for (int i = 0; i < tm && pt * tm + i < (int)rows.size(); ++i) own[i] = rows[pt * tm + i];
     int h1 = 0;
-    if (!make_indexed_blob(own, rowptr, colidx, val, &slot_of, &blobs[pt], &h1)) return P2M_ERR_INVALID;
+    if (!make_indexed_blob(own, tm, rowptr, colidx, val, &slot_of, &blobs[pt], &h1)) return P2M_ERR_INVALID;
     stride = std::max(stride, (int)blobs[pt].size());
     max_h1 = std::max(max_h1, h1);
   }
@@ -1757,6 +1815,12 @@ int build_tileset(const std::vector<int>& rows, const int* rowptr, const int* co
   ts->n_pattern = P;
   ts->max_h1 = max_h1;
   return P2M_OK;
+}
+
+int build_tileset(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
+                  TileSet* ts, std::vector<void*>* owned) {
+  P2M_TRY(build_blobs(rows, TILE_M, rowptr, colidx, val, V, ts, owned));
+  return build_blobs(rows, 64, rowptr, colidx, val, V, &ts->m64, owned);
 }
 }  // namespace
 
@@ -1903,6 +1967,14 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
     out->tile_meta1 = d_meta1;
     out->tile_meta1_bytes = d_bytes1;
     out->meta1_stride = stride1;
+  }
+  {
+    // 64-row tiles of the consecutive rows (a 64-row tile's halo is within its 128-row tile's, so they fit wherever
+    // the 128-row tiles are usable; beyond the blob limits meta64 stays empty and umma_conv_supported says no)
+    std::vector<int> all_rows(V);
+    for (int v = 0; v < V; ++v) all_rows[v] = v;
+    const int st = build_blobs(all_rows, 64, rowptr, colidx, val, V, &out->meta64, owned);
+    if (st != P2M_OK && st != P2M_ERR_INVALID) return st;
   }
   {
     // padding-vertex elision: rows whose only entry is the diagonal, all with the same value
@@ -2098,6 +2170,12 @@ bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
   if (fin % FC != 0 || fin < FC || fin > 256) return false;
   if (g.max_h1 > 256) return false;  // producers keep <= 4 T1 rows per row group
   if (fout != 64 && fout != 128 && fout != 256) return false;
+  // 128- and 256-wide layers run their T1-given and plain convs on the 64-row configuration (one ring of 3, one stage)
+  if (fout % WIDE_N == 0 &&
+      (g.meta64.n_pattern <= 0 ||
+       smem_bytes_dims(WIDE_N, 3, 1, g.meta64.max_h1, g.meta64.max_h1, g.meta64.stride, 1) > SMEM_LIMIT ||
+       smem_bytes_dims(WIDE_N, 3, 1, g.meta64.max_h1, g.meta64.max_h1, g.meta64.stride, 2) > SMEM_LIMIT))
+    return false;
   return smem_bytes_for(CONV_N, ring_stages(CONV_N), 1, g) <= SMEM_LIMIT;
 }
 
@@ -2346,7 +2424,8 @@ int launch_umma_conv(const UmmaConvArgs& a, int* status, const float* zero_row, 
     set_error("umma_conv: the fused head needs fout == 64 and no residual");
     return P2M_ERR_INVALID;
   }
-  if (a.tiles != nullptr && ((a.t1 == nullptr && !a.plain) || a.tiles->max_h1 > 256 || a.tiles->n_pattern <= 0)) {
+  if (a.tiles != nullptr && ((a.t1 == nullptr && !a.plain) || a.tiles->max_h1 > 256 || a.tiles->n_pattern <= 0 ||
+                             (a.fout % WIDE_N == 0 && a.tiles->m64.n_pattern <= 0))) {
     set_error("umma_conv: index-list tiles need the T1-given or plain mode and at most 256 staged rows");
     return P2M_ERR_INVALID;
   }

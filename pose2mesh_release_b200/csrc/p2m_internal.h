@@ -61,14 +61,19 @@ struct DeviceGuard {
 // ---------------------------------------------------------------- device-resident hierarchy level
 // L~ of one level in CSR with RELATIVE column offsets: the neighbour of flat activation row
 // r = b*V + v is row r + reloff[p], so kernels never need (b, v) separately (block-diagonal I_B (x) L~).
-// A family of 128-row tile patterns of one level whose rows are given by index lists (trimmed blobs: the tile's own
-// rows, their 1-hop halo, the CSR of the own rows) instead of being the consecutive rows [128 p, 128 p + 128).
-struct TileSet {
+// Trimmed tile blobs (the tile's own rows, their 1-hop halo, the CSR of the own rows over staged-row slots, the own rows
+// in length-sorted order) of one level, for tiles of a fixed row count.
+struct TileBlobs {
   const unsigned char* meta = nullptr;  // [n_pattern][stride]
   const int* bytes = nullptr;           // [n_pattern]
   int stride = 0;
   int n_pattern = 0;                    // tiles per mesh
   int max_h1 = 0;                       // largest own + 1-hop row count
+};
+// A family of 128-row tile patterns of one level whose rows are given by index lists instead of being the consecutive
+// rows [128 p, 128 p + 128), and the same rows cut into 64-row tiles (m64: the 64-row x 128-column conv configuration).
+struct TileSet : TileBlobs {
+  TileBlobs m64;
 };
 
 struct DevLevel {
@@ -88,6 +93,8 @@ struct DevLevel {
   const unsigned char* tile_meta1 = nullptr;  // [n_pattern][meta1_stride]
   const int* tile_meta1_bytes = nullptr;
   int meta1_stride = 0;
+  // the same trimmed blobs for 64-row tiles [64 p, 64 p + 64) (the 64-row x 128-column conv configuration)
+  TileBlobs meta64;
   int max_h1 = 0, max_h2 = 0;
   // L~ == L~^T exactly (the backward passes use L~ where the math needs L~^T), and h = ceil(log2(2 r^2 + 1)) for r the
   // largest absolute row sum of L~: max|T2| <= (2 r^2 + 1) max|x|, the headroom the single-layer fp16 split leaves
@@ -269,7 +276,7 @@ struct UmmaConvArgs {
 // tiles exceed the metadata's 16-bit slot / entry offsets gets none (tile_meta stays null: it runs on SIMT).
 int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val, int V, DevLevel* out,
                           std::vector<void*>* owned);
-// Tiles of 128 consecutive entries of `rows` (ascending vertex ids of one level) as a TileSet (trimmed blobs).
+// Tiles of 128 (and, TileSet::m64, 64) consecutive entries of `rows` (ascending vertex ids of one level) as a TileSet.
 int build_index_tiles(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
                       TileSet* ts, std::vector<void*>* owned);
 bool umma_conv_supported(const DevLevel& g, int fin, int fout);
