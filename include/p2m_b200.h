@@ -94,8 +94,6 @@ int p2m_debug_kernel_status(p2m_model_t* m, int32_t* out);
 /* Debug (libraries built with -DP2M_UMMA_TRACE only; P2M_ERR_INVALID otherwise): CTA 0 of this handle's
  * tensor-core conv kernels logs (event << 48 | SM clock) into dev_buf [8][512] int64; NULL = off.        */
 int p2m_debug_set_trace(p2m_model_t* m, void* dev_buf);
-/* Debug / ablation: 1 (default) = T1 = L~x as a separate pass + conv with given T1; 0 = fully fused conv.   */
-int p2m_debug_set_split_t1(p2m_model_t* m, int enable);
 /* Debug / ablation: 1 (default) = in eval mode the 128->64 conv's epilogue produces the 64->3 head's projections
  * itself (the 64-wide activation is never written); 0 = the two layers run separately.                         */
 int p2m_debug_set_fuse_head(p2m_model_t* m, int enable);
@@ -109,17 +107,13 @@ int p2m_debug_set_elide_padding(p2m_model_t* m, int enable);
  * it at the end; p2m_meshnet_forward_vertices (which returns connected rows only) computes no isolated row at all.
  * 1 (default) = on, 0 = every isolated row is computed.  Training always computes every row (BatchNorm statistics). */
 int p2m_debug_set_dedup_padding(p2m_model_t* m, int enable);
-/* Backward, tensor-core layers: 1 (default) = the weight gradient is formed from the Chebyshev basis of the GRADIENT
- * (sum_rows dz (x) T_k(x) = sum_rows T_k(dz) (x) x, L~ symmetric), re-using the L~dz the backward-data pass computes;
- * 0 = from the basis of the layer input, rebuilt on chip with its 2-hop halo.  Same result up to fp32 association. */
-int p2m_debug_set_dw_swap(p2m_model_t* m, int enable);
 /* Debug: which kernels the single-layer entry points (p2m_cheb_conv_fwd / _bwd) select for one layer of `level` at
  * the handle's current precision.  out[0] = forward conv on tensor cores, out[1] its X staging depth (1 or 2; 0 off
  * the tensor cores), out[2] / out[3] = the same for the weight gradient, out[4] / out[5] = the backward-data GEMM
- * (dT = dz W_k), out[6] = own rows arrive by TMA (V % 128 == 0), out[7] / out[8] = the level's largest 1-hop / 2-hop
- * staged-row count per 128-row tile (0 when the level has no tensor-core metadata), out[9] = isolated rows that
+ * (dT = dz W_k), out[6] = own rows arrive by TMA (V % 128 == 0), out[7] = the level's largest staged-row count (own
+ * rows + 1-hop halo) per 128-row tile (0 when the level has no tensor-core metadata), out[8] = isolated rows that
  * padding elision would route to the dense path (0: elision not applicable).                                    */
-int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[10]);
+int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[9]);
 
 /* Bytes of device workspace p2m_meshnet_forward needs for batch B.  In training mode the workspace
  * also carries what p2m_meshnet_backward reads, so it must stay alive and untouched in between.   */

@@ -108,7 +108,7 @@ P2M_BETAS_AS_GIVEN = 1
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
-    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_split_t1", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_set_dw_swap", "p2m_debug_conv_path", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
+    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward", "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
     "p2m_rigid_align", "p2m_point_errors",
@@ -148,16 +148,12 @@ def load() -> C.CDLL:
         lib.p2m_model_set_profiling.restype = C.c_int
         lib.p2m_model_layer_times_ms.argtypes = [vp, c_float_p, C.c_int]
         lib.p2m_model_layer_times_ms.restype = C.c_int
-        lib.p2m_debug_set_split_t1.argtypes = [vp, C.c_int]
-        lib.p2m_debug_set_split_t1.restype = C.c_int
         lib.p2m_debug_set_fuse_head.argtypes = [vp, C.c_int]
         lib.p2m_debug_set_fuse_head.restype = C.c_int
         lib.p2m_debug_set_elide_padding.argtypes = [vp, C.c_int]
         lib.p2m_debug_set_elide_padding.restype = C.c_int
         lib.p2m_debug_set_dedup_padding.argtypes = [vp, C.c_int]
         lib.p2m_debug_set_dedup_padding.restype = C.c_int
-        lib.p2m_debug_set_dw_swap.argtypes = [vp, C.c_int]
-        lib.p2m_debug_set_dw_swap.restype = C.c_int
         lib.p2m_debug_set_trace.argtypes = [vp, vp]
         lib.p2m_debug_set_trace.restype = C.c_int
         lib.p2m_debug_conv_path.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]

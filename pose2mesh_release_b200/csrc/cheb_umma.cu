@@ -12,9 +12,7 @@
 //   * 16 producer warps build the A operand on chip, 32 features at a time: they run the second sparse product from
 //     shared memory with a tile-local CSR (the T1 rows of the tile and its 1-hop halo, staged one chunk ahead), read
 //     their own X rows straight from global memory, split every fp32 value into an fp16 (hi, lo) pair and write it
-//     into the 128B-swizzled K-major operand layout.  T2 is never materialised in HBM.  (Without a T1 buffer —
-//     p.t1 == nullptr, the split_t1 = 0 ablation — the same kernel stages the 2-hop halo of X and runs both sparse
-//     products on chip: the fully fused variant.)
+//     into the 128B-swizzled K-major operand layout.  T2 is never materialised in HBM.
 //   * 2 loader warps stage what the producers gather from: the tile's own T1 rows as one 2-D TMA box where the tile
 //     is a run of consecutive rows, every other row (halo, index-list tiles) by 16-byte cp.async with completion
 //     through cp.async.mbarrier.arrive.noinc; thread 0 also prefetches the next tile's metadata blob.  1 thread
@@ -54,18 +52,18 @@ constexpr float W_SCALE = 64.f;
 constexpr float W_INV_SCALE = 1.f / 64.f;
 
 // ------------------------------------------------------------------ per-tile metadata blob
+// A tile of tm (128 or 64) rows: its own rows (slots 0..tm-1) and their 1-hop halo are staged; the local CSR covers the
+// own rows only.
 struct TileHeader {  // 64 bytes
-  int n_rows;     // valid vertices in this tile (<= 128)
-  int h1;         // rows of T1 kept on chip: 128 tile slots + 1-hop halo
-  int h2;         // rows of X staged: h1 + 2-hop halo
+  int n_rows;     // valid vertices in this tile (<= tm)
+  int h1;         // staged rows: tm tile slots + 1-hop halo
   int nnz;
-  int off_halo;   // int32 [h2]    vertex id of staged row i (-1: empty slot)
-  int off_rp;     // uint16 [h1+1] local CSR: row i < h1 lists the neighbours of vertex halo[i]
+  int off_halo;   // int32 [h1]    vertex id of staged row i (-1: empty slot)
+  int off_rp;     // uint16 [tm+1] local CSR: row i < tm lists the neighbours of vertex halo[i]
   int off_ent;    // uint2 [nnz]   {byte offset of the neighbour's staged row (slot*128), value bits}
-  int off_ord1;   // uint16 [h1]   T1 rows sorted by decreasing length (warps see equal trip counts)
-  int off_ord2;   // uint16 [128]  tile rows sorted by decreasing length
+  int off_ord2;   // uint16 [tm]   tile rows sorted by decreasing length (warps see equal trip counts)
   int bytes;
-  int pad[6];
+  int pad[8];
 };
 static_assert(sizeof(TileHeader) == 64, "header size");
 
@@ -317,15 +315,13 @@ struct KParams {
   int n_tiles;
   const unsigned char* meta;
   const int* meta_bytes;
-  int meta_stride, max_h1, max_h2;
+  int meta_stride, max_h1;
   const unsigned char* wpack;
   const float* zero_row;  // 128 bytes of zeros: source of the empty halo slots of ragged tiles
   EpiDev ep;
   int res_identity;       // residual resampling is the identity (Fin_block == Fout): vector path
-  const float* t1;        // optional precomputed T1 = L~ x, [rows, fin] at LOGICAL rows (k_cheb_t1): the conv kernel
-                          // then stages the tile's own X rows and the T1 rows of its 1-hop halo, and only runs the
-                          // second sparse product on chip (no halo recomputation of T1)
-  int plain;              // 1: plain GEMM y = x * B^T (no SpMM): one K-block per chunk, rows = the tile's own
+  const float* t1;        // MODE 1: T1 = L~ x, [rows, fin] at LOGICAL rows (k_cheb_t1): the conv kernel stages the
+                          // T1 rows of the tile and its 1-hop halo and only runs the second sparse product on chip
   const float* a_scale;   // optional device scalar: x is multiplied by it before the fp16 split (power of two,
                           // chosen from max|x|: gradients are far below fp16's range) and divided out afterwards
   long long ldy;          // row stride of y in floats, and first output column
@@ -344,7 +340,7 @@ struct KParams {
   const unsigned char* apack;
   long long wslice_bytes;  // offset of this CTA's N-slice (blockIdx.y) in the weight image
   long long wblock_stride; // bytes between consecutive K-blocks of the weight image
-  int tma;           // 1: the tile's own rows of x (and t1) arrive by one 2-D TMA load each (T1-given / plain mode on
+  int tma;           // 1: the tile's own rows of x (and t1) arrive by one 2-D TMA load each (consecutive tiles on
                      //    levels whose size is a multiple of 128); with in_unpool the x box is the TM / 2 source rows
   CUtensorMap tm_x, tm_t1;
 };
@@ -364,7 +360,7 @@ __device__ __forceinline__ void trace_ev(const KParams&, int, int&, int) {}
 
 // Warp roles (24 warps = 6 warpgroups, one persistent CTA per SM):
 //   0..15  producers: SpMM out of shared memory + fp16 (hi,lo) split + swizzled A-block stores
-//   16,17  loaders: stage the T1 (and, outside the production mode, X) rows of the next chunk; thread 0 also fetches
+//   16,17  loaders: stage the T1 (and, where the producers do not read it directly, X) rows of the next chunk; thread 0 also fetches
 //          the next tile's metadata (cp.async.bulk), thread 32 issues the TMA boxes
 //   18     weight-block loader (one thread, cp.async.bulk)
 //   19     idle
@@ -379,17 +375,15 @@ static_assert(W_XLOAD % 4 == 0 && W_EPI0 % 4 == 0 && W_EPI0 - W_XLOAD == 4, "set
 
 // Two tile shapes, both a 64-register fp32 accumulator per thread of the one MMA warpgroup:
 //   N = 64:  a CTA computes 128 tile rows x the 64 output columns [64 blockIdx.y, 64 blockIdx.y + 64); used for the
-//            64-wide layers (and the fused thin head), the dense GEMM and the split_t1 = 0 ablation.
+//            64-wide layers (and the fused thin head) and the dense GEMM.
 //   N = 128: a CTA computes 64 tile rows x the 128 output columns [128 blockIdx.y, 128 blockIdx.y + 128); used for every
-//            T1-given and plain conv with Fout % 128 == 0, so that a tile row's A operand is built once per 128 output
-//            columns instead of once per 64.  The tiles are the 64-row metadata families (DevLevel::meta64,
-//            TileSet::m64).
-// MODE 1: the production configuration — T1 given, not the plain-GEMM mode — fixed at compile time, so the on-chip first
-// sparse product, the plain path and their per-tile state drop out of the producers (registers for a deeper gather);
-// MODE 0 decides both at run time (plain GEMM, dense GEMM, the split_t1 = 0 ablation; N = 128: plain GEMM only).
+//            conv with Fout % 128 == 0, so that a tile row's A operand is built once per 128 output columns instead of
+//            once per 64.  The tiles are the 64-row metadata families (DevLevel::meta64, TileSet::m64).
+// MODE 1: T1 given (k_cheb_t1): the producers run the second sparse product out of the staged T1 rows.
+// MODE 0: plain GEMM, no sparse product (the isolated rows of padding elision, the backward dT GEMMs, the dense GEMM).
 template <int N>
 __host__ __device__ constexpr int tile_rows() { return N == 128 ? 64 : TILE_M; }
-template <int N, int NS, int XS, int MODE = 0>
+template <int N, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
   constexpr int TM = tile_rows<N>();  // tile rows
@@ -397,25 +391,24 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   constexpr int H = TM / 64;          // M = 64 halves of the tile (one accumulator each)
   constexpr int ER = 16 * H;          // epilogue rows per warp of the MMA warpgroup
   constexpr bool KT1 = (MODE == 1);
-  // X of the own rows straight from global memory (production mode, deep ring): the only reader of an own X row is the
+  constexpr bool plain = !KT1;
+  // X of the own rows straight from global memory (T1 given, deep ring): the only reader of an own X row is the
   // producer thread that emits it, so staging it costs a shared-memory write plus a read back (8 % of the kernel's
   // shared-memory traffic, and more than half of the loaders' copies on index-list tiles) for nothing
   constexpr bool XDIRECT = KT1 && NS >= 3;
-  const bool plain = KT1 ? false : (TM == 64 || p.plain != 0);
   constexpr int A_BYTES = TM * 128;  // one K-block of A: TM rows x (32 hi | 32 lo) fp16
   constexpr int B_BLOCK_BYTES = N * 128;
   constexpr int SLOT_BYTES = A_BYTES + B_BLOCK_BYTES;
 
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* ring = smem_raw;  // 128B-swizzled blocks need 1024-byte alignment (checked below)
-  const bool t1g = KT1 ? true : (p.t1 != nullptr);
-  float* Xs = reinterpret_cast<float*>(ring + NS * SLOT_BYTES);                 // [XS][max_h2 | TM][32]
+  float* Xs = reinterpret_cast<float*>(ring + NS * SLOT_BYTES);                 // [XS][TM][32]
   // (the 64-row configuration allocates no X stage where the producers read X directly: its room deepens the ring)
-  const size_t xs_stage_floats = (XDIRECT && TM == 64) ? 0 : (size_t)((t1g || plain) ? TM : p.max_h2) * FC;
-  float* T1s = Xs + XS * xs_stage_floats;                                       // [1 | XS | 0][max_h1][32]
+  const size_t xs_stage_floats = (XDIRECT && TM == 64) ? 0 : (size_t)TM * FC;
+  float* T1s = Xs + XS * xs_stage_floats;                                       // [XS | 0][max_h1][32]
   const size_t t1_stage_floats = (size_t)p.max_h1 * FC;
   unsigned char* meta_s =
-      reinterpret_cast<unsigned char*>(T1s + (plain ? 0 : (t1g ? XS : 1)) * t1_stage_floats);  // [2][meta_stride]
+      reinterpret_cast<unsigned char*>(T1s + (plain ? 0 : XS) * t1_stage_floats);  // [2][meta_stride]
   uint64_t* bars = reinterpret_cast<uint64_t*>(meta_s + 2 * (size_t)p.meta_stride);
   // barrier map
   uint64_t* b_ab_full = bars;                // [NS]
@@ -485,7 +478,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     // Per stage (tile, 32-feature chunk) they bring in what the producers read: the tile's metadata blob (thread 0,
     // cp.async.bulk, one tile ahead), the own rows of X / T1 (one 2-D TMA box each where the tile is a run of
     // consecutive rows — thread 32), and every other staged row with 16-byte cp.async copies (8 lanes per 128-byte row,
-    // all 64 threads): the T1 rows of the 1-hop halo, or all rows where the tile is an index list / no T1 is given.
+    // all 64 threads): the T1 rows of the 1-hop halo, or all rows where the tile is an index list.
     // A stage needs ~60 warp-level copies; issued by the 16 producer warps (round 2 until this change) every warp paid
     // the whole preamble for its one to four rows — a fifth of the producers' instruction stream per chunk.
     if (p.apack == nullptr) {
@@ -494,7 +487,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
       if (lt == 32 && p.tma) {
         if (!XDIRECT) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tm_x)) : "memory");
-        if (t1g) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tm_t1)) : "memory");
+        if (KT1) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tm_t1)) : "memory");
       }
       auto fetch_meta = [&](int itf) {  // thread 0: blob of this CTA's tile number itf into buffer itf & 1
         const int pat = (blockIdx.x + itf * gridDim.x) % p.P;
@@ -518,7 +511,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         const unsigned char* mb2 = meta_s + (size_t)m2 * p.meta_stride;
         const TileHeader* hdr2 = reinterpret_cast<const TileHeader*>(mb2);
         const int* halo = reinterpret_cast<const int*>(mb2 + hdr2->off_halo);
-        const int h1 = hdr2->h1, h2 = hdr2->h2;
+        const int h1 = hdr2->h1;
         for (int c2 = 0; c2 < n_chunk; ++c2, ++g2) {
           const int xs2 = g2 % XS;
           mbar_wait_relaxed(smem_u32(b_x_empty + xs2), ((g2 / XS) & 1) ^ 1, abort_flag, p.status, 11);
@@ -542,22 +535,22 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
             }
           };
           const char* t1_mesh =
-              reinterpret_cast<const char*>(t1g ? p.t1 + mesh_row0 * p.fin + c2 * FC + lq * 4 : nullptr);
+              reinterpret_cast<const char*>(KT1 ? p.t1 + mesh_row0 * p.fin + c2 * FC + lq * 4 : nullptr);
           const char* x_mesh = reinterpret_cast<const char*>(p.x + (mesh_row0 >> sh) * p.fin + c2 * FC + lq * 4);
           const uint32_t t1_dst = smem_u32(T1s + xs2 * t1_stage_floats) + lq * 16;
           const uint32_t x_dst = smem_u32(Xs + xs2 * xs_stage_floats) + lq * 16;
           if (p.tma) {
             if (lt == 32) {
               const int own0 = tile2 * TM;  // V is a multiple of 128: tiles never straddle meshes
-              mbar_arrive_expect_tx(xbar, (XDIRECT ? 0 : (p.in_unpool ? TM / 2 : TM) * 128) + (t1g ? TM * 128 : 0));
+              mbar_arrive_expect_tx(xbar, (XDIRECT ? 0 : (p.in_unpool ? TM / 2 : TM) * 128) + (KT1 ? TM * 128 : 0));
               if (!XDIRECT)
                 tma_load_2d(smem_u32(Xs + xs2 * xs_stage_floats), &p.tm_x, c2 * FC, p.in_unpool ? own0 >> 1 : own0, xbar);
-              if (t1g) tma_load_2d(smem_u32(T1s + xs2 * t1_stage_floats), &p.tm_t1, c2 * FC, own0, xbar);
+              if (KT1) tma_load_2d(smem_u32(T1s + xs2 * t1_stage_floats), &p.tm_t1, c2 * FC, own0, xbar);
             }
-            if (t1g) stage_rows(t1_dst, t1_mesh, TM, h1, 0);  // only the halo rows are left
+            if (KT1) stage_rows(t1_dst, t1_mesh, TM, h1, 0);  // only the halo rows are left
           } else {
-            if (t1g) stage_rows(t1_dst, t1_mesh, 0, h1, 0);
-            if (!XDIRECT) stage_rows(x_dst, x_mesh, 0, (plain || t1g) ? TM : h2, sh);
+            if (KT1) stage_rows(t1_dst, t1_mesh, 0, h1, 0);
+            if (!XDIRECT) stage_rows(x_dst, x_mesh, 0, TM, sh);
             if (lt == 32) mbar_arrive(xbar);
           }
           cp_async_arrive_noinc(xbar);  // this thread's arrival once its copies have landed
@@ -791,8 +784,6 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int n_stage = my_tiles * n_chunk;  // flat sequence of (tile, chunk) stages of this CTA
 
-    constexpr int T1_ROWS = 4;  // max_h1 <= 256 rows over 64 row groups (checked on the host)
-    uint32_t t1_row[T1_ROWS], t1_e[T1_ROWS];
     // this thread's tile rows (RPT = 1 or 2: row groups rg and 64 + rg of the tile's row order) and their CSR extents
     uint32_t row[RPT], re[RPT], ent_a = 0;
     int ptn = 0;
@@ -839,19 +830,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         const unsigned char* mb = meta_s + (size_t)m * p.meta_stride;
         const TileHeader* hdr = reinterpret_cast<const TileHeader*>(mb);
         const uint32_t mb_a = smem_u32(mb);
-        const uint32_t rp_a = mb_a + hdr->off_rp, ord1_a = mb_a + hdr->off_ord1, ord2_a = mb_a + hdr->off_ord2;
+        const uint32_t rp_a = mb_a + hdr->off_rp, ord2_a = mb_a + hdr->off_ord2;
         ent_a = mb_a + hdr->off_ent;
-        const int h1 = (t1g || plain) ? 0 : hdr->h1;  // the trimmed metadata has no T1 row order
-#pragma unroll
-        for (int t = 0; t < T1_ROWS; ++t) {
-          const int j = rg + 64 * t;
-          t1_row[t] = 0xFFFFu;
-          if (j < h1) {
-            const uint32_t i = lds_u16(ord1_a + 2 * j);
-            t1_row[t] = i;
-            t1_e[t] = lds_u16(rp_a + 2 * i) | (lds_u16(rp_a + 2 * i + 2) << 16);
-          }
-        }
 #pragma unroll
         for (int ps = 0; ps < RPT; ++ps) {
           // plain GEMM: the thread's rows are the consecutive slots rg (and 64 + rg)
@@ -876,7 +856,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         }
       }
       const uint32_t xs_q = smem_u32(Xs + xs * xs_stage_floats) + q * 16;
-      const uint32_t t1s_q = t1s_a + (t1g ? (uint32_t)(xs * t1_stage_floats * 4) : 0u) + q * 16;
+      const uint32_t t1s_q = t1s_a + (uint32_t)(xs * t1_stage_floats * 4) + q * 16;
       if (plain) {
         // plain GEMM: the staged rows ARE the A operand (scaled into fp16 range if a_scale is given)
         const uint32_t s = slot;
@@ -903,24 +883,12 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         if (tid == 0 && c == n_chunk - 1) mbar_arrive(smem_u32(b_m_empty + m));
         continue;
       }
-      // (1) T1 = L~ X on the tile rows and their 1-hop halo (local CSR columns = staged X rows); two rows per
-      //     thread are gathered together for memory-level parallelism.
-      if (!t1g) {
-#pragma unroll
-        for (int t = 0; t < T1_ROWS; ++t) {
-          if (t1_row[t] != 0xFFFFu)
-            sts_f4(t1s_q + t1_row[t] * 128, gather_row4(ent_a, t1_e[t] & 0xFFFFu, t1_e[t] >> 16, xs_q));
-        }
-        if (tid == 0) trace_ev(p, 0, ptn, 4);
-        producer_barrier();
-        if (tid == 0) trace_ev(p, 0, ptn, 5);
-      }
-      // (2) split to fp16 (hi, lo) and write the three K-blocks of the tile rows this thread finishes.  The X and
-      //     T1 blocks go first: they need no gather, so the tensor core starts on them while (3) the second sparse
-      //     product T2 = 2 L~ T1 - X is still being gathered (with a 2-deep ring, N = 256, the T2 block re-uses the X
-      //     block's slot and would otherwise wait for its MMAs).  NS >= 3: ONE generic->async proxy fence for all
-      //     three blocks (the fence drains the thread's outstanding shared stores and is expensive); NS < 3: one per
-      //     block.  Odd row groups store lo first: a warp then covers both 64-byte halves of its rows per store.
+      // Split to fp16 (hi, lo) and write the three K-blocks of the tile rows this thread finishes.  The X and T1
+      // blocks go first: they need no gather, so the tensor core starts on them while the second sparse product
+      // T2 = 2 L~ T1 - X is still being gathered (with a 2-deep ring, N = 256, the T2 block re-uses the X block's slot
+      // and would otherwise wait for its MMAs).  NS >= 3: ONE generic->async proxy fence for all three blocks (the
+      // fence drains the thread's outstanding shared stores and is expensive); NS < 3: one per block.  Odd row groups
+      // store lo first: a warp then covers both 64-byte halves of its rows per store.
       const uint32_t slot0 = slot;
       auto emit = [&](const float4 (&vv)[RPT]) {
         const uint32_t s = slot;
@@ -1011,37 +979,41 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
 // The reduction runs over the ROWS, so both operands are "MN-major" for the tensor core (the K index of the
 // MMA is the mesh row).  The 128B-swizzled row-major blocks the forward kernel already builds — 128 rows x
 // [hi 32 | lo 32] fp16 of T_k for one 32-feature chunk — are exactly a canonical MN-major SWIZZLE_128B tile
-// (K = 128 rows of 128 bytes, MN = 64 elements), so the producers are shared with the forward and T is
-// recomputed on chip instead of being materialised (the SIMT path writes and re-reads 3x the activations).
+// (K = 128 rows of 128 bytes, MN = 64 elements), so the producers are shared with the forward and T2 is
+// formed on chip from the given T1 instead of being materialised (the SIMT path writes and re-reads 3x the activations).
 // A = the plain-side tile (dz, or the layer input in swapped mode), split (hi, lo) and stored the same way
 // ([128 rows] x 64 channels per block).  Per T block: 8 K-steps x three wgmma.m64n32k16 (g_hi T_hi + g_lo T_hi +
 // g_hi T_lo, the lo half of T addressed 64 bytes into the swizzle row) with M = 64 channels, N = 32 features,
 // accumulated in registers across ALL tiles of the CTA: one feature chunk (T0, T1, T2: 3 x 16 registers) and 64
 // channels per launch; one atomicAdd pass per CTA at the end.
 // =====================================================================================
+// Two operand roles (L~ symmetric:  sum_rows dz (x) T_k(X) = sum_rows T_k(dz) (x) X), selected by `swap`:
+//   swap = 0: `x` is the layer INPUT [rows(/2), fin] whose basis the producers build, `g` the gradient dz [rows,
+//             fout_total] (plain tile, scaled by a_scale); dw[o][f*3+k] with o from the plain side.
+//   swap = 1: `x` is the GRADIENT dz [rows, fin := layer Fout] (gathered, scaled by a_scale), `g` the layer input
+//             [rows(/2), fout_total := layer Fin] (plain tile, unscaled, read at row >> 1 under the virtual unpool);
+//             the accumulator rows are then input features and the columns output channels: dw[o][f*3+k] with o from
+//             the gathered side.
+// Either way `t1` = L~ x for every row of the level (launch_cheb_t1): the producers stage the T1 rows of the tile and its
+// 1-hop halo and form T2 on chip.
 struct DwParams {
-  const float* x;
+  const float* x;        // gathered side
   int in_unpool;
   int V, P, fin;
   int n_tiles;
   const unsigned char* meta;
   const int* meta_bytes;
-  int meta_stride, max_h1, max_h2;
-  const float* g;        // dz [rows, fout_total]
+  int meta_stride, max_h1;
+  const float* g;        // plain side [rows(/2), fout_total]
   int fout_total, m_off, m_cols;
   int chunk0;            // feature chunk of this launch (its T0, T1, T2 are the MMA warpgroup's three accumulators)
   const float* a_scale;  // device scalar (power of two) applied to the gradient tensor before the fp16 split
-  float* dw;             // [fout_total, 3*fin], column = f*3 + k  (reference layout), accumulated atomically
+  float* dw;             // reference layout [Fout, 3 Fin], column = f*3 + k, accumulated atomically
   int* status;
-  // Swapped roles (L~ symmetric:  sum_rows dz (x) T_k(X) = sum_rows T_k(dz) (x) X): `x` is the GRADIENT dz
-  // [rows, fin := layer Fout] whose basis the producers build (scaled by a_scale), `t1` = L~ dz as left behind by
-  // the backward-data pass (launch_cheb_t1), `g` the layer INPUT [rows(/2), fout_total := layer Fin] (plain tile,
-  // unscaled, read at row >> 1 under the virtual unpool).  The accumulator rows are then input features and the
-  // columns output channels: dw[o][f*3+k] with o from the gathered side.  No 2-hop halo, no on-chip T1.
   const float* t1;
   int g_unpool;
   int swap;
-  int tma;                 // T1 given, consecutive tiles, V % 128 == 0: the own rows of x and t1 arrive by one 2-D TMA box each
+  int tma;                 // consecutive tiles, V % 128 == 0, no unpool: the own rows of x and t1 arrive by one 2-D TMA box each
   CUtensorMap tm_x, tm_t1;
 };
 
@@ -1062,12 +1034,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* ring = smem_raw;                      // [DW_NS] T blocks
   unsigned char* gblk = ring + DW_NS * A_BLOCK_BYTES;  // dz tile blocks: hi g0, hi g1, lo g0, lo g1
-  float* Xs = reinterpret_cast<float*>(gblk + DW_G_BYTES);
-  const bool t1g = (p.t1 != nullptr);
-  const size_t xs_stage_floats = (size_t)(t1g ? TILE_M : p.max_h2) * FC;
-  float* T1s = Xs + XS * xs_stage_floats;                   // [XS | 1][max_h1][32]
+  float* Xs = reinterpret_cast<float*>(gblk + DW_G_BYTES);  // [XS][128][32] the tile's own rows of x
+  constexpr size_t xs_stage_floats = (size_t)TILE_M * FC;
+  float* T1s = Xs + XS * xs_stage_floats;                   // [XS][max_h1][32]
   const size_t t1_stage_floats = (size_t)p.max_h1 * FC;
-  unsigned char* meta_s = reinterpret_cast<unsigned char*>(T1s + (t1g ? XS : 1) * t1_stage_floats);
+  unsigned char* meta_s = reinterpret_cast<unsigned char*>(T1s + XS * t1_stage_floats);
   uint64_t* bars = reinterpret_cast<uint64_t*>(meta_s + 2 * (size_t)p.meta_stride);
   uint64_t* b_t_full = bars;                 // [DW_NS]
   uint64_t* b_t_empty = b_t_full + DW_NS;    // [DW_NS]
@@ -1107,7 +1078,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
   __syncthreads();
 
   if (warp >= W_XLOAD && warp < W_XLOAD + N_XLOAD) {
-    // ------------------------------------------------------------ halo loaders + tile metadata (as in the forward)
+    // ------------------------------------------------------------ row loaders + tile metadata (as in the forward)
     const int lt = tid - W_XLOAD * 32;
     const int q = lt & 7, rg = lt >> 3;
     auto fetch_meta = [&](int it2) {
@@ -1128,7 +1099,6 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
       mbar_wait_relaxed(smem_u32(b_m_full + m), (it >> 1) & 1, abort_flag, p.status, 22);
       const unsigned char* mb = meta_s + (size_t)m * p.meta_stride;
       const TileHeader* hdr = reinterpret_cast<const TileHeader*>(mb);
-      const int h2 = t1g ? TILE_M : hdr->h2;  // T1 given: only the tile's own rows of x are staged ...
       const int h1 = hdr->h1;
       const int* halo = reinterpret_cast<const int*>(mb + hdr->off_halo);
       const long long mesh_row0 = (long long)b * p.V;
@@ -1160,8 +1130,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
             mbar_arrive(xbar);
           }
         }
-        if (!p.tma)
-        for (int i = rg; i < h2; i += 8) {
+        if (!p.tma)  // the tile's own rows of x ...
+        for (int i = rg; i < TILE_M; i += 8) {
           const int v = halo[i];
           if (v >= 0) {
             long long r = mesh_row0 + v;
@@ -1171,7 +1141,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
             sts_f4(dst0 + i * 128, make_float4(0.f, 0.f, 0.f, 0.f));
           }
         }
-        if (t1g) {  // ... plus the T1 rows of the tile and its 1-hop halo
+        {  // ... plus the T1 rows of the tile and its 1-hop halo
           const uint32_t dst1 = smem_u32(T1s + xs * t1_stage_floats) + q * 16;
           const float* src1 = p.t1 + (p.chunk0 + c) * FC + q * 4;
           for (int i = (p.tma ? TILE_M : 0) + rg; i < h1; i += 8) {  // (TMA: only the halo rows are left)
@@ -1242,8 +1212,6 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
     const int q = tid & 7, rg = tid >> 3;
     const uint32_t t1s_a = smem_u32(T1s), ring_a = smem_u32(ring), g_a = smem_u32(gblk);
     uint32_t ucnt = 0, gcnt = 0;
-    constexpr int T1_ROWS = 4;
-    uint32_t t1_row[T1_ROWS], t1_e[T1_ROWS];
     uint32_t row0 = 0, row1 = 0, r0e = 0, r1e = 0, ent_a = 0;
     for (int it = 0; it < my_tiles; ++it) {
       const int tile = blockIdx.x + it * gridDim.x;
@@ -1275,20 +1243,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
         const unsigned char* mb = meta_s + (size_t)m * p.meta_stride;
         const TileHeader* hdr = reinterpret_cast<const TileHeader*>(mb);
         const uint32_t mb_a = smem_u32(mb);
-        const uint32_t rp_a = mb_a + hdr->off_rp, ord1_a = mb_a + hdr->off_ord1, ord2_a = mb_a + hdr->off_ord2;
+        const uint32_t rp_a = mb_a + hdr->off_rp, ord2_a = mb_a + hdr->off_ord2;
         ent_a = mb_a + hdr->off_ent;
-        const int h1 = t1g ? 0 : hdr->h1;  // the trimmed metadata has no T1 row order
-#pragma unroll
-        for (int t = 0; t < T1_ROWS; ++t) {
-          const int j = rg + 64 * t;
-          t1_row[t] = 0xFFFFu;
-          if (j < h1) {
-            const uint32_t i = lds_u16(ord1_a + 2 * j);
-            t1_row[t] = i;
-            t1_e[t] = lds_u16(rp_a + 2 * i) | (lds_u16(rp_a + 2 * i + 2) << 16);
-          }
-        }
-        row0 = lds_u16(ord2_a + 2 * rg);
+        row0 =lds_u16(ord2_a + 2 * rg);
         row1 = lds_u16(ord2_a + 2 * (64 + rg));
         r0e = lds_u16(rp_a + 2 * row0) | (lds_u16(rp_a + 2 * row0 + 2) << 16);
         r1e = lds_u16(rp_a + 2 * row1) | (lds_u16(rp_a + 2 * row1 + 2) << 16);
@@ -1305,7 +1262,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
             // into different 64-byte bank halves (their swizzle bits agree: consecutive rows)
             const int col = q * 4 + 32 * (jj ^ (rg & 1));  // channel inside this launch's slice (< m_cols <= 64)
             float4 v = pv[ps][jj];
-            if (!p.swap) {  // legacy roles: this side is the gradient
+            if (!p.swap) {  // input role: this side is the gradient
               v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
             }
             uint2 hi, lo;
@@ -1323,15 +1280,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
         const int xs = gcnt % XS;
         mbar_wait(smem_u32(b_x_full + xs), (gcnt / XS) & 1, abort_flag, p.status, 29);
         const uint32_t xs_q = smem_u32(Xs + xs * xs_stage_floats) + q * 16;
-        const uint32_t t1s_q = t1s_a + (t1g ? (uint32_t)(xs * t1_stage_floats * 4) : 0u) + q * 16;
-        if (!t1g) {
-#pragma unroll
-          for (int t = 0; t < T1_ROWS; ++t) {
-            if (t1_row[t] != 0xFFFFu)
-              sts_f4(t1s_q + t1_row[t] * 128, gather_row4(ent_a, t1_e[t] & 0xFFFFu, t1_e[t] >> 16, xs_q));
-          }
-          producer_barrier();
-        }
+        const uint32_t t1s_q = t1s_a + (uint32_t)(xs * t1_stage_floats * 4) + q * 16;
         float4 tv[3][2];
         {
           const float4 g0 = gather_row4(ent_a, r0e & 0xFFFFu, r0e >> 16, t1s_q);
@@ -1386,9 +1335,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
 }
 
 // =====================================================================================
-// k_cheb_t1 — T1 = L~ X for every row, written once to HBM (fp32, logical rows).  With it the conv kernel only
-// needs the tile's own X rows and the T1 rows of its 1-hop halo: the 35 % of the first sparse product that the
-// fused kernel spends re-computing T1 on halo rows disappears, and so does its 2-hop X staging.
+// k_cheb_t1 — T1 = L~ X for every row, written once to HBM (fp32, logical rows).  With it the conv and dW kernels
+// only need the tile's own X rows and the T1 rows of its 1-hop halo; no tile recomputes T1 on its halo rows.
 // Simple kernel: one CTA (512 threads, two per SM) per 128-row tile; the 1-hop halo of X is staged chunk by chunk
 // through a 4-deep cp.async ring (one barrier per chunk), the gather runs out of shared memory.
 // =====================================================================================
@@ -1504,44 +1452,42 @@ __global__ void __launch_bounds__(256) k_pack_weights(const float* __restrict__ 
 // debug: P2M_UMMA_TMA=0 stages every row with cp.async (A/B measurements of the TMA own-row loads)
 const bool g_umma_tma = [] { const char* e = std::getenv("P2M_UMMA_TMA"); return !(e && e[0] == '0'); }();
 
-// mode: 0 = fused (X with its 2-hop halo staged, T1 recomputed on chip), 1 = T1 given, 2 = plain GEMM
 inline int epi_stage_bytes(int) { return 4 * 32 * 32 * 4; }  // per-warp transpose staging
-// N = 128: the 64-row configuration (64-row tiles; in mode 1 with NS >= 3 no X stage: the producers read X directly)
-size_t smem_bytes_dims(int N, int NS, int XS, int max_h1, int max_h2, int meta_stride, int mode) {
+// Dynamic shared memory of a conv configuration: T1 given (MODE 1: the tile's own X rows and the T1 rows of the tile
+// and its 1-hop halo per stage) or plain (MODE 0: the own X rows per stage).  N = 128: the 64-row configuration (64-row
+// tiles; with a given T1 and NS >= 3 no X stage: the producers read X directly).
+size_t smem_bytes_dims(int N, int NS, int XS, int max_h1, int meta_stride, bool t1_given) {
   const int tm = N == 128 ? 64 : TILE_M;
   const size_t fixed = 1024 + (size_t)NS * (tm * 128 + N * 128) + 8 * (2 * NS + 2 * XS + 8) + 16 +
                        2 * (size_t)N * 4 + 16 + 128 + (size_t)epi_stage_bytes(N) + 4 * 32 * 4 +
                        (N == 64 ? 64 * 12 * 4 : 0);
-  const size_t xs_rows = (mode == 1 && N == 128 && NS >= 3) ? 0 : (size_t)tm;
-  if (mode == 1) return fixed + (size_t)XS * xs_rows * FC * 4 + (size_t)XS * max_h1 * FC * 4 + 2 * (size_t)meta_stride;
-  if (mode == 2) return fixed + (size_t)XS * tm * FC * 4 + 2 * (size_t)meta_stride;
-  return fixed + (size_t)XS * max_h2 * FC * 4 + (size_t)max_h1 * FC * 4 + 2 * (size_t)meta_stride;
+  const size_t xs_rows = (t1_given && N == 128 && NS >= 3) ? 0 : (size_t)tm;
+  return fixed + (size_t)XS * (xs_rows + (t1_given ? max_h1 : 0)) * FC * 4 + 2 * (size_t)meta_stride;
 }
-size_t smem_bytes_for(int N, int NS, int XS, const DevLevel& g, int mode = 0) {
-  return smem_bytes_dims(N, NS, XS, g.max_h1, g.max_h2, mode ? g.meta1_stride : g.meta_stride, mode);
-}
-// the tile metadata a launch with N output columns per CTA runs on: the level's consecutive tiles or the tile family the
-// caller selected, 128-row blobs for N = 64 and 64-row blobs for N = 128
-const TileBlobs& launch_tiles(int N, const UmmaConvArgs& a) {
-  if (a.tiles != nullptr) return N == 128 ? a.tiles->m64 : *a.tiles;
-  return a.g->meta64;  // N = 128 only: N = 64 launches on consecutive tiles read the DevLevel fields
-}
-// the same for an explicit launch
-size_t smem_bytes_args(int N, int NS, int XS, const UmmaConvArgs& a) {
-  const int mode = a.plain ? 2 : (a.t1 != nullptr ? 1 : 0);
-  if (a.tiles != nullptr || N == 128) {
-    const TileBlobs& t = launch_tiles(N, a);
-    return smem_bytes_dims(N, NS, XS, t.max_h1, t.max_h1, t.stride, mode);
-  }
-  return smem_bytes_for(N, NS, XS, *a.g, mode);
+size_t smem_bytes_for(int N, int NS, int XS, const TileBlobs& t, bool t1_given) {
+  return smem_bytes_dims(N, NS, XS, t.max_h1, t.stride, t1_given);
 }
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 constexpr int CONV_N = 64;  // output columns per CTA of the 128-row conv configuration (one column slice)
-constexpr int WIDE_N = 128; // ... and of the 64-row configuration (T1-given and plain convs with Fout % 128 == 0)
-inline int ring_stages(int) { return 3; }
-// X staging depth: 2 (prefetch the next chunk's halo during the current chunk) when it fits, else 1
-inline int x_stages(int N, const DevLevel& g) {
-  return smem_bytes_for(N, ring_stages(N), 2, g) <= SMEM_LIMIT ? 2 : 1;
+constexpr int WIDE_N = 128; // ... and of the 64-row configuration (convs with Fout % 128 == 0)
+inline int conv_n(int fout) { return fout % WIDE_N == 0 ? WIDE_N : CONV_N; }
+// the tile metadata a launch with N output columns per CTA runs on: the level's consecutive tiles or the tile family the
+// caller selected, 128-row blobs for N = 64 and 64-row blobs for N = 128
+const TileBlobs& conv_tiles(int N, const DevLevel& g, const TileSet* tiles) {
+  if (tiles != nullptr) return N == WIDE_N ? tiles->m64 : *tiles;
+  return N == WIDE_N ? g.meta64 : g.meta128;
+}
+// A/B ring depth and X staging depth of a conv launch: the deepest that fit, the ring first (N = 128: 6 slots = two
+// chunks, the producers run a chunk ahead of the MMAs, or 3 = one chunk; N = 64: 3), then 2 X stages (prefetch the next
+// chunk's rows during the current chunk) or 1.  {0, 0}: does not fit.
+struct ConvCfg {
+  int ns, xs;
+};
+ConvCfg conv_cfg(int N, const TileBlobs& t, bool t1_given) {
+  for (int ns = N == WIDE_N ? 6 : 3; ns >= 3; ns -= 3)
+    for (int xs = 2; xs >= 1; --xs)
+      if (smem_bytes_for(N, ns, xs, t, t1_given) <= SMEM_LIMIT) return {ns, xs};
+  return {0, 0};
 }
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point lookup (no link-time dependency on libcuda)
@@ -1589,39 +1535,27 @@ int check_launch_regs() {
   return P2M_OK;
 }
 
-template <int N, int NS, int XS, int MODE = 0>
+// a.plain selects the instantiation: MODE 0 (plain GEMM) or MODE 1 (T1 given)
+template <int N, int NS, int XS>
 int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
-  if (MODE == 0 && a.t1 != nullptr && !a.plain)  // the production configuration has its own instantiation
-    return launch_cfg<N, NS, XS, 1>(a, status, zero_row, sm_count, s);
   constexpr int TM = tile_rows<N>();
   const DevLevel& g = *a.g;
-  const int mode = a.plain ? 2 : (a.t1 != nullptr ? 1 : 0);
-  const size_t smem = smem_bytes_args(N, NS, XS, a);
-  auto kern = k_cheb_conv_umma<N, NS, XS, MODE>;
+  const TileBlobs& t = conv_tiles(N, g, a.tiles);
+  const size_t smem = smem_bytes_for(N, NS, XS, t, !a.plain);
+  auto kern = a.plain ? k_cheb_conv_umma<N, NS, XS, 0> : k_cheb_conv_umma<N, NS, XS, 1>;
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  P2M_TRY((check_launch_regs<N, NS, XS, MODE>()));
+  P2M_TRY((a.plain ? check_launch_regs<N, NS, XS, 0>() : check_launch_regs<N, NS, XS, 1>()));
   KParams p;
   p.x = a.x;
   p.in_unpool = a.in_unpool;
   p.V = g.V;
-  p.P = g.n_pattern;
+  p.P = t.n_pattern;
   p.fin = a.fin;
-  p.meta = mode ? g.tile_meta1 : g.tile_meta;
-  p.meta_bytes = mode ? g.tile_meta1_bytes : g.tile_meta_bytes;
-  p.meta_stride = mode ? g.meta1_stride : g.meta_stride;
-  p.max_h1 = g.max_h1;
-  p.max_h2 = g.max_h2;
-  p.own_table = 0;
-  if (a.tiles != nullptr || N == 128) {  // index-list tiles (mode 1 / 2 only, checked by the caller), 64-row blobs
-    const TileBlobs& t = launch_tiles(N, a);
-    p.P = t.n_pattern;
-    p.meta = t.meta;
-    p.meta_bytes = t.bytes;
-    p.meta_stride = t.stride;
-    p.max_h1 = t.max_h1;
-    p.max_h2 = t.max_h1;
-    p.own_table = a.tiles != nullptr ? 1 : 0;
-  }
+  p.meta = t.meta;
+  p.meta_bytes = t.bytes;
+  p.meta_stride = t.stride;
+  p.max_h1 = t.max_h1;
+  p.own_table = a.tiles != nullptr ? 1 : 0;
   p.n_tiles = a.batch * p.P;
   p.wpack = static_cast<const unsigned char*>(a.wpack);
   p.apack = nullptr;
@@ -1633,7 +1567,6 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.res_identity = (a.ep.res != nullptr && a.ep.res_F == a.fout) ? 1 : 0;
   p.y = a.y;
   p.t1 = a.t1;
-  p.plain = a.plain;
   p.a_scale = a.a_scale;
   p.ldy = a.ldy > 0 ? a.ldy : a.fout;
   p.y_col0 = a.y_col0;
@@ -1644,7 +1577,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.tma = 0;
   std::memset(&p.tm_x, 0, sizeof(p.tm_x));
   std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
-  if ((a.t1 != nullptr || a.plain) && a.tiles == nullptr && g.V % TILE_M == 0 && g_umma_tma) {
+  if (a.tiles == nullptr && g.V % TILE_M == 0 && g_umma_tma) {
     const long long rows = (long long)a.batch * g.V;
     bool ok = make_row_tmap(&p.tm_x, a.x, a.in_unpool ? rows / 2 : rows, a.fin, a.in_unpool ? TM / 2 : TM);
     if (ok && a.t1 != nullptr) ok = make_row_tmap(&p.tm_t1, a.t1, rows, a.fin, TM);
@@ -1657,31 +1590,21 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   return P2M_OK;
 }
 
-// 64 x 128 configuration: the deepest A/B ring (6 slots = two chunks: the producers run a chunk ahead of the MMAs,
-// or 3 = one chunk) and X staging depth that fit, the ring first
-int launch_wide(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
-  constexpr int N = WIDE_N;
-  if (smem_bytes_args(N, 6, 2, a) <= SMEM_LIMIT) return launch_cfg<N, 6, 2>(a, status, zero_row, sm_count, s);
-  if (smem_bytes_args(N, 6, 1, a) <= SMEM_LIMIT) return launch_cfg<N, 6, 1>(a, status, zero_row, sm_count, s);
-  if (smem_bytes_args(N, 3, 2, a) <= SMEM_LIMIT) return launch_cfg<N, 3, 2>(a, status, zero_row, sm_count, s);
-  if (smem_bytes_args(N, 3, 1, a) <= SMEM_LIMIT) return launch_cfg<N, 3, 1>(a, status, zero_row, sm_count, s);
-  set_error("umma_conv: tile family does not fit shared memory");
-  return P2M_ERR_INVALID;
-}
-
 int launch_n(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
-  constexpr int N = CONV_N, NS = 3;
-  if ((a.t1 != nullptr || a.plain) && a.fout % WIDE_N == 0) return launch_wide(a, status, zero_row, sm_count, s);
-  if (a.t1 != nullptr || a.plain) {
-    if (smem_bytes_args(N, NS, 2, a) <= SMEM_LIMIT) return launch_cfg<N, NS, 2>(a, status, zero_row, sm_count, s);
-    if (smem_bytes_args(N, NS, 1, a) > SMEM_LIMIT) {
-      set_error("umma_conv: tile family does not fit shared memory");
-      return P2M_ERR_INVALID;
-    }
-    return launch_cfg<N, NS, 1>(a, status, zero_row, sm_count, s);
+  const int N = conv_n(a.fout);
+  const ConvCfg c = conv_cfg(N, conv_tiles(N, *a.g, a.tiles), !a.plain);
+  if (c.ns == 0) {
+    set_error("umma_conv: tile family does not fit shared memory");
+    return P2M_ERR_INVALID;
   }
-  if (x_stages(N, *a.g) == 2) return launch_cfg<N, NS, 2>(a, status, zero_row, sm_count, s);
-  return launch_cfg<N, NS, 1>(a, status, zero_row, sm_count, s);
+  if (N == CONV_N)
+    return c.xs == 2 ? launch_cfg<CONV_N, 3, 2>(a, status, zero_row, sm_count, s)
+                     : launch_cfg<CONV_N, 3, 1>(a, status, zero_row, sm_count, s);
+  if (c.ns == 6)
+    return c.xs == 2 ? launch_cfg<WIDE_N, 6, 2>(a, status, zero_row, sm_count, s)
+                     : launch_cfg<WIDE_N, 6, 1>(a, status, zero_row, sm_count, s);
+  return c.xs == 2 ? launch_cfg<WIDE_N, 3, 2>(a, status, zero_row, sm_count, s)
+                   : launch_cfg<WIDE_N, 3, 1>(a, status, zero_row, sm_count, s);
 }
 
 }  // namespace
@@ -1711,7 +1634,7 @@ void balance_store_halves(std::vector<unsigned short>* ord) {
   }
 }
 
-// Trimmed blob of one tile whose tm (128 or 64) own rows are given by an index list (-1 = empty slot): own rows, their
+// Blob of one tile whose tm (128 or 64) own rows are given by an index list (-1 = empty slot): own rows, their
 // 1-hop halo, the CSR of the own rows with staged-row slots as columns, the own rows in length-sorted order.
 bool make_indexed_blob(const std::vector<int>& own, int tm, const int* rowptr, const int* colidx, const float* val,
                        std::vector<int>* slot_of, std::vector<unsigned char>* blob, int* h1_out) {
@@ -1748,6 +1671,7 @@ bool make_indexed_blob(const std::vector<int>& own, int tm, const int* rowptr, c
   for (int v : halo)
     if (v >= 0) (*slot_of)[v] = -1;
   const int nnz = (int)(ent.size() / 2);
+  // at most 512 staged rows (no kernel stages more than 256) and 16-bit local-CSR offsets
   if (h1 > 512 || nnz > 65535) return false;
   std::vector<unsigned short> ord2(tm);
   for (int i = 0; i < tm; ++i) ord2[i] = (unsigned short)i;
@@ -1760,14 +1684,12 @@ bool make_indexed_blob(const std::vector<int>& own, int tm, const int* rowptr, c
   TileHeader t{};
   t.n_rows = n_rows;
   t.h1 = h1;
-  t.h2 = h1;
   t.nnz = nnz;
   int o1 = 64;
   t.off_halo = o1; o1 += up16(h1 * 4);
   t.off_rp = o1;   o1 += up16((tm + 1) * 2);
   t.off_ent = o1;  o1 += up16(nnz * 8);
   t.off_ord2 = o1; o1 += up16(tm * 2);
-  t.off_ord1 = t.off_ord2;
   t.bytes = o1;
   blob->assign(o1, 0);
   std::memcpy(blob->data(), &t, sizeof(t));
@@ -1831,151 +1753,13 @@ int build_index_tiles(const std::vector<int>& rows, const int* rowptr, const int
 
 int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val, int V, DevLevel* out,
                           std::vector<void*>* owned) {
-  const int P = (V + TILE_M - 1) / TILE_M;
-  std::vector<std::vector<unsigned char>> blobs(P), blobs1(P);
-  int max_h1 = 0, max_h2 = 0, stride = 0, stride1 = 0;
-  std::vector<int> slot_of(V, -1);
-  for (int pt = 0; pt < P; ++pt) {
-    const int v0 = pt * TILE_M;
-    const int n_rows = std::min(TILE_M, V - v0);
-    // staged-row list: slots 0..127 = tile rows, then 1-hop halo, then 2-hop halo
-    std::vector<int> halo(TILE_M, -1);
-    for (int i = 0; i < n_rows; ++i) {
-      halo[i] = v0 + i;
-      slot_of[v0 + i] = i;
-    }
-    auto add = [&](int v) {
-      if (slot_of[v] < 0) {
-        slot_of[v] = (int)halo.size();
-        halo.push_back(v);
-      }
-    };
-    for (int i = 0; i < n_rows; ++i)
-      for (int e = rowptr[v0 + i]; e < rowptr[v0 + i + 1]; ++e) add(colidx[e]);
-    const int h1 = (int)halo.size();
-    for (int i = 0; i < h1; ++i) {
-      if (halo[i] < 0) continue;
-      for (int e = rowptr[halo[i]]; e < rowptr[halo[i] + 1]; ++e) add(colidx[e]);
-    }
-    const int h2 = (int)halo.size();
-    if (h2 > 65535) return P2M_OK;  // beyond 16-bit staged-row slots: no tensor-core metadata, the level runs on SIMT
-    // One local CSR serves both products: row i < h1 lists (staged-row slot, value) of vertex halo[i].
-    // T1 rows read X slots (< h2); the T2 pass only walks the 128 tile rows, whose columns are < h1,
-    // i.e. valid T1 slots (slot numbering of X and T1 coincides below h1).
-    std::vector<unsigned short> rp(h1 + 1, 0);
-    std::vector<unsigned int> ent;  // pairs {slot*128, float bits}
-    for (int i = 0; i < h1; ++i) {
-      if (halo[i] >= 0)
-        for (int e = rowptr[halo[i]]; e < rowptr[halo[i] + 1]; ++e) {
-          unsigned int bits;
-          std::memcpy(&bits, &val[e], 4);
-          ent.push_back((unsigned int)slot_of[colidx[e]] * 128u);
-          ent.push_back(bits);
-        }
-      rp[i + 1] = (unsigned short)(ent.size() / 2);
-    }
-    const int nnz = (int)(ent.size() / 2);
-    if (nnz > 65535) return P2M_OK;  // beyond 16-bit local-CSR offsets: likewise
-    auto row_len = [&](int i) { return (int)rp[i + 1] - (int)rp[i]; };
-    std::vector<unsigned short> ord1(h1), ord2(TILE_M);
-    for (int i = 0; i < h1; ++i) ord1[i] = (unsigned short)i;
-    for (int i = 0; i < TILE_M; ++i) ord2[i] = (unsigned short)i;
-    std::stable_sort(ord1.begin(), ord1.end(), [&](unsigned short a, unsigned short b2) { return row_len(a) > row_len(b2); });
-    std::stable_sort(ord2.begin(), ord2.end(), [&](unsigned short a, unsigned short b2) { return row_len(a) > row_len(b2); });
-    balance_store_halves(&ord2);
-    TileHeader h{};
-    h.n_rows = n_rows;
-    h.h1 = h1;
-    h.h2 = h2;
-    h.nnz = nnz;
-    int off = 64;
-    h.off_halo = off; off += up16(h2 * 4);
-    h.off_rp = off;   off += up16((h1 + 1) * 2);
-    h.off_ent = off;  off += up16(nnz * 8);
-    h.off_ord1 = off; off += up16(h1 * 2);
-    h.off_ord2 = off; off += up16(TILE_M * 2);
-    h.bytes = off;
-    std::vector<unsigned char>& blob = blobs[pt];
-    blob.assign(off, 0);
-    std::memcpy(blob.data(), &h, sizeof(h));
-    std::memcpy(blob.data() + h.off_halo, halo.data(), h2 * 4);
-    std::memcpy(blob.data() + h.off_rp, rp.data(), (h1 + 1) * 2);
-    if (nnz) std::memcpy(blob.data() + h.off_ent, ent.data(), (size_t)nnz * 8);
-    std::memcpy(blob.data() + h.off_ord1, ord1.data(), h1 * 2);
-    std::memcpy(blob.data() + h.off_ord2, ord2.data(), TILE_M * 2);
-    max_h1 = std::max(max_h1, h1);
-    max_h2 = std::max(max_h2, h2);
-    stride = std::max(stride, off);
-    {
-      // trimmed variant: staged rows = own + 1-hop (h2 := h1), CSR rows of the 128 own rows (they come first in ent)
-      const int nnz1 = rp[TILE_M <= h1 ? TILE_M : h1];
-      TileHeader t{};
-      t.n_rows = n_rows;
-      t.h1 = h1;
-      t.h2 = h1;
-      t.nnz = nnz1;
-      int o1 = 64;
-      t.off_halo = o1; o1 += up16(h1 * 4);
-      t.off_rp = o1;   o1 += up16((TILE_M + 1) * 2);
-      t.off_ent = o1;  o1 += up16(nnz1 * 8);
-      t.off_ord2 = o1; o1 += up16(TILE_M * 2);
-      t.off_ord1 = t.off_ord2;  // not used by the consumers of this variant
-      t.bytes = o1;
-      std::vector<unsigned char>& b1 = blobs1[pt];
-      b1.assign(o1, 0);
-      std::memcpy(b1.data(), &t, sizeof(t));
-      std::memcpy(b1.data() + t.off_halo, halo.data(), h1 * 4);
-      std::memcpy(b1.data() + t.off_rp, rp.data(), (TILE_M + 1) * 2);
-      if (nnz1) std::memcpy(b1.data() + t.off_ent, ent.data(), (size_t)nnz1 * 8);
-      std::memcpy(b1.data() + t.off_ord2, ord2.data(), TILE_M * 2);
-      stride1 = std::max(stride1, o1);
-    }
-    for (int v : halo)
-      if (v >= 0) slot_of[v] = -1;
-  }
-  stride = (stride + 127) & ~127;
-  std::vector<unsigned char> all((size_t)P * stride, 0);
-  std::vector<int> bytes(P);
-  for (int pt = 0; pt < P; ++pt) {
-    std::memcpy(all.data() + (size_t)pt * stride, blobs[pt].data(), blobs[pt].size());
-    bytes[pt] = (int)blobs[pt].size();
-  }
-  unsigned char* d_meta = nullptr;
-  int* d_bytes = nullptr;
-  P2M_CUDA_OK(cudaMalloc(&d_meta, all.size()));
-  owned->push_back(d_meta);
-  P2M_CUDA_OK(cudaMalloc(&d_bytes, sizeof(int) * P));
-  owned->push_back(d_bytes);
-  P2M_CUDA_OK(cudaMemcpy(d_meta, all.data(), all.size(), cudaMemcpyHostToDevice));
-  P2M_CUDA_OK(cudaMemcpy(d_bytes, bytes.data(), sizeof(int) * P, cudaMemcpyHostToDevice));
-  {
-    stride1 = (stride1 + 127) & ~127;
-    std::vector<unsigned char> all1((size_t)P * stride1, 0);
-    std::vector<int> bytes1(P);
-    for (int pt = 0; pt < P; ++pt) {
-      std::memcpy(all1.data() + (size_t)pt * stride1, blobs1[pt].data(), blobs1[pt].size());
-      bytes1[pt] = (int)blobs1[pt].size();
-    }
-    unsigned char* d_meta1 = nullptr;
-    int* d_bytes1 = nullptr;
-    P2M_CUDA_OK(cudaMalloc(&d_meta1, all1.size()));
-    owned->push_back(d_meta1);
-    P2M_CUDA_OK(cudaMalloc(&d_bytes1, sizeof(int) * P));
-    owned->push_back(d_bytes1);
-    P2M_CUDA_OK(cudaMemcpy(d_meta1, all1.data(), all1.size(), cudaMemcpyHostToDevice));
-    P2M_CUDA_OK(cudaMemcpy(d_bytes1, bytes1.data(), sizeof(int) * P, cudaMemcpyHostToDevice));
-    out->tile_meta1 = d_meta1;
-    out->tile_meta1_bytes = d_bytes1;
-    out->meta1_stride = stride1;
-  }
-  {
-    // 64-row tiles of the consecutive rows (a 64-row tile's halo is within its 128-row tile's, so they fit wherever
-    // the 128-row tiles are usable; beyond the blob limits meta64 stays empty and umma_conv_supported says no)
-    std::vector<int> all_rows(V);
-    for (int v = 0; v < V; ++v) all_rows[v] = v;
-    const int st = build_blobs(all_rows, 64, rowptr, colidx, val, V, &out->meta64, owned);
-    if (st != P2M_OK && st != P2M_ERR_INVALID) return st;
-  }
+  // 128-row and 64-row tiles of the consecutive rows (a 64-row tile's halo is within its 128-row tile's)
+  std::vector<int> all_rows(V);
+  for (int v = 0; v < V; ++v) all_rows[v] = v;
+  int st = build_blobs(all_rows, TILE_M, rowptr, colidx, val, V, &out->meta128, owned);
+  if (st == P2M_OK) st = build_blobs(all_rows, 64, rowptr, colidx, val, V, &out->meta64, owned);
+  if (st == P2M_ERR_INVALID) return P2M_OK;  // beyond the blob limits: no tensor-core metadata, the level runs on SIMT
+  if (st != P2M_OK) return st;
   {
     // padding-vertex elision: rows whose only entry is the diagonal, all with the same value
     std::vector<int> real_rows, iso_rows;
@@ -2003,47 +1787,67 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
       }
     }
   }
-  out->n_pattern = P;
-  out->tile_meta = d_meta;
-  out->tile_meta_bytes = d_bytes;
-  out->meta_stride = stride;
-  out->max_h1 = max_h1;
-  out->max_h2 = max_h2;
   return P2M_OK;
 }
 
 
-size_t dw_smem_bytes(int XS, const DevLevel& g, bool t1_given = false) {
-  const size_t stage = t1_given ? (size_t)XS * (TILE_M + g.max_h1) * FC * 4
-                                : (size_t)XS * g.max_h2 * FC * 4 + (size_t)g.max_h1 * FC * 4;
-  return 1024 + (size_t)DW_NS * A_BLOCK_BYTES + DW_G_BYTES + stage + 2 * (size_t)(t1_given ? g.meta1_stride : g.meta_stride) +
-         8 * (2 * DW_NS + 2 * XS + 8) + 32;
+size_t dw_smem_bytes(int XS, const DevLevel& g) {
+  return 1024 + (size_t)DW_NS * A_BLOCK_BYTES + DW_G_BYTES + (size_t)XS * (TILE_M + g.meta128.max_h1) * FC * 4 +
+         2 * (size_t)g.meta128.stride + 8 * (2 * DW_NS + 2 * XS + 8) + 32;
 }
 
-bool umma_dw_supported(const DevLevel& g, int fin, int fout) {
-  if (g.tile_meta == nullptr || g.n_pattern <= 0 || g.max_h1 > 256) return false;
-  if (fin % FC != 0 || fin < FC || fin > 256) return false;
-  if (fout != 64 && fout != 128 && fout != 256) return false;
+bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width) {
+  if (g.meta128.n_pattern <= 0 || g.meta128.max_h1 > 256) return false;
+  if (gathered_width % FC != 0 || gathered_width < FC || gathered_width > 256) return false;
+  if (plain_width != 64 && plain_width != 128 && plain_width != 256) return false;
   return dw_smem_bytes(1, g) <= SMEM_LIMIT;
 }
+int umma_dw_x_stages(const DevLevel& g) { return dw_smem_bytes(2, g) <= SMEM_LIMIT ? 2 : 1; }
 
-namespace {
-int launch_dw_kernels(const DevLevel& g, DwParams p, int gathered_width, int plain_width, bool t1_given, int sm_count,
-                      cudaStream_t s) {
-  const int xs = dw_smem_bytes(2, g, t1_given) <= SMEM_LIMIT ? 2 : 1;
-  const size_t smem = dw_smem_bytes(xs, g, t1_given);
-  if (smem > SMEM_LIMIT) {
-    set_error("umma_dw: does not fit shared memory");
+int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_unpool, int gathered_width,
+                   const float* t1, const float* plain, int g_unpool, int plain_width, int swap, const float* a_scale,
+                   float* dw_ref, int* status, int sm_count, cudaStream_t s) {
+  if (!umma_dw_supported(g, gathered_width, plain_width) || t1 == nullptr) {
+    set_error("umma_dw: unsupported shape");
     return P2M_ERR_INVALID;
   }
+  const TileBlobs& t = g.meta128;
+  DwParams p;
+  p.x = gathered;
+  p.in_unpool = in_unpool;
+  p.V = g.V;
+  p.P = t.n_pattern;
+  p.fin = gathered_width;
+  p.n_tiles = batch * t.n_pattern;
+  p.meta = t.meta;
+  p.meta_bytes = t.bytes;
+  p.meta_stride = t.stride;
+  p.max_h1 = t.max_h1;
+  p.g = plain;
+  p.fout_total = plain_width;
+  p.a_scale = a_scale;
+  p.dw = dw_ref;
+  p.status = status;
+  p.t1 = t1;
+  p.g_unpool = g_unpool;
+  p.swap = swap;
+  p.tma = 0;
+  std::memset(&p.tm_x, 0, sizeof(p.tm_x));
+  std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
+  if (g.V % TILE_M == 0 && !in_unpool && g_umma_tma) {
+    const long long rows = (long long)batch * g.V;
+    p.tma = (make_row_tmap(&p.tm_x, gathered, rows, gathered_width, TILE_M) &&
+             make_row_tmap(&p.tm_t1, t1, rows, gathered_width, TILE_M)) ? 1 : 0;
+  }
+  const int xs = umma_dw_x_stages(g);
+  const size_t smem = dw_smem_bytes(xs, g);
   auto kern = (xs == 2) ? k_cheb_dw_umma<2> : k_cheb_dw_umma<1>;
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = std::min(p.n_tiles, sm_count);
-  const int total_chunks = gathered_width / FC;
   for (int m_off = 0; m_off < plain_width; m_off += 64) {
     p.m_off = m_off;
     p.m_cols = std::min(64, plain_width - m_off);  // M = 64 plain-side channels per launch
-    for (int c0 = 0; c0 < total_chunks; ++c0) {  // one feature chunk per launch (the kernel's n_chunk)
+    for (int c0 = 0; c0 < gathered_width / FC; ++c0) {  // one feature chunk per launch (the kernel's n_chunk)
       p.chunk0 = c0;
       kern<<<grid, NUM_THREADS2, smem, s>>>(p);
       P2M_LAUNCH_OK();
@@ -2051,99 +1855,19 @@ int launch_dw_kernels(const DevLevel& g, DwParams p, int gathered_width, int pla
   }
   return P2M_OK;
 }
-}  // namespace
-
-int launch_umma_dw(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, int fout, const float* dz,
-                   const float* a_scale, float* dw_ref, int* status, int sm_count, cudaStream_t s) {
-  if (!umma_dw_supported(g, fin, fout)) {
-    set_error("umma_dw: unsupported shape");
-    return P2M_ERR_INVALID;
-  }
-  DwParams p;
-  p.x = x;
-  p.in_unpool = in_unpool;
-  p.V = g.V;
-  p.P = g.n_pattern;
-  p.fin = fin;
-  p.n_tiles = batch * g.n_pattern;
-  p.meta = g.tile_meta;
-  p.meta_bytes = g.tile_meta_bytes;
-  p.meta_stride = g.meta_stride;
-  p.max_h1 = g.max_h1;
-  p.max_h2 = g.max_h2;
-  p.g = dz;
-  p.fout_total = fout;
-  p.a_scale = a_scale;
-  p.dw = dw_ref;
-  p.status = status;
-  p.t1 = nullptr;
-  p.g_unpool = 0;
-  p.swap = 0;
-  p.tma = 0;
-  std::memset(&p.tm_x, 0, sizeof(p.tm_x));
-  std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
-  return launch_dw_kernels(g, p, fin, fout, false, sm_count, s);
-}
-
-// dW from the basis of the GRADIENT (see DwParams::swap): dz [rows, fout], t1_dz = L~ dz for EVERY row of the level,
-// x the layer input [rows(/2), fin]
-bool umma_dw_swapped_supported(const DevLevel& g, int fin, int fout) {
-  if (g.tile_meta1 == nullptr || g.n_pattern <= 0 || g.max_h1 > 256) return false;
-  if (fout % FC != 0 || fout < FC || fout > 256) return false;       // gathered side: dz
-  if (fin != 64 && fin != 128 && fin != 256) return false;           // plain side: x
-  return dw_smem_bytes(1, g, true) <= SMEM_LIMIT;
-}
-int launch_umma_dw_swapped(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, int fout,
-                           const float* dz, const float* t1_dz, const float* a_scale, float* dw_ref, int* status,
-                           int sm_count, cudaStream_t s) {
-  if (!umma_dw_swapped_supported(g, fin, fout) || t1_dz == nullptr) {
-    set_error("umma_dw_swapped: unsupported shape");
-    return P2M_ERR_INVALID;
-  }
-  DwParams p;
-  p.tma = 0;
-  std::memset(&p.tm_x, 0, sizeof(p.tm_x));
-  std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
-  p.x = dz;
-  p.in_unpool = 0;
-  p.V = g.V;
-  p.P = g.n_pattern;
-  p.fin = fout;                 // width of the gathered tensor
-  p.n_tiles = batch * g.n_pattern;
-  p.meta = g.tile_meta1;
-  p.meta_bytes = g.tile_meta1_bytes;
-  p.meta_stride = g.meta1_stride;
-  p.max_h1 = g.max_h1;
-  p.max_h2 = g.max_h1;
-  p.g = x;
-  p.fout_total = fin;           // width of the plain tensor
-  p.a_scale = a_scale;
-  p.dw = dw_ref;
-  p.status = status;
-  p.t1 = t1_dz;
-  p.g_unpool = in_unpool;
-  p.swap = 1;
-  if (g.V % TILE_M == 0 && g_umma_tma) {
-    const long long rows = (long long)batch * g.V;
-    p.tma = (make_row_tmap(&p.tm_x, dz, rows, fout, TILE_M) && make_row_tmap(&p.tm_t1, t1_dz, rows, fout, TILE_M)) ? 1 : 0;
-  }
-  return launch_dw_kernels(g, p, fout, fin, true, sm_count, s);
-}
 
 int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, float* t1, cudaStream_t s,
                    const TileSet* tiles) {
-  if (g.tile_meta == nullptr || fin % FC != 0) {
+  const TileBlobs& t = tiles ? *tiles : g.meta128;
+  if (t.n_pattern <= 0 || fin % FC != 0) {
     set_error("cheb_t1: unsupported shape");
     return P2M_ERR_INVALID;
   }
-  const int max_h1 = tiles ? tiles->max_h1 : g.max_h1;
-  const int stride = tiles ? tiles->stride : g.meta1_stride;
-  const int n_pattern = tiles ? tiles->n_pattern : g.n_pattern;
-  if (max_h1 > 256) {  // 4 staged slots per row group
+  if (t.max_h1 > 256) {  // 4 staged slots per row group
     set_error("cheb_t1: halo too large");
     return P2M_ERR_INVALID;
   }
-  auto smem_for = [&](int stages) { return (size_t)stride + stages * (size_t)max_h1 * FC * 4 + 16; };
+  auto smem_for = [&](int stages) { return (size_t)t.stride + stages * (size_t)t.max_h1 * FC * 4 + 16; };
   const size_t half_sm = (228 * 1024) / 2 - 1024;  // two CTAs per SM (1 KB per CTA is reserved by the system)
   const int stages = smem_for(4) <= half_sm ? 4 : (smem_for(3) <= half_sm ? 3 : 2);
   const size_t smem = smem_for(stages);
@@ -2153,40 +1877,35 @@ int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, 
   p.x = x;
   p.in_unpool = in_unpool;
   p.V = g.V;
-  p.P = n_pattern;
+  p.P = t.n_pattern;
   p.fin = fin;
-  p.meta = tiles ? tiles->meta : g.tile_meta1;
-  p.meta_bytes = tiles ? tiles->bytes : g.tile_meta1_bytes;
-  p.meta_stride = stride;
-  p.max_h1 = max_h1;
+  p.meta = t.meta;
+  p.meta_bytes = t.bytes;
+  p.meta_stride = t.stride;
+  p.max_h1 = t.max_h1;
   p.t1 = t1;
-  kern<<<batch * n_pattern, 512, smem, s>>>(p);
+  kern<<<batch * t.n_pattern, 512, smem, s>>>(p);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
 
+// What launch_n runs on the level's consecutive tiles: the T1-given conv and the plain GEMM, both with one ring of 3
+// and one X stage at least, on the 64-row tiles for Fout % 128 == 0 and on the 128-row tiles otherwise.
 bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
-  if (g.tile_meta == nullptr || g.n_pattern <= 0) return false;
+  if (g.meta128.n_pattern <= 0) return false;
   if (fin % FC != 0 || fin < FC || fin > 256) return false;
-  if (g.max_h1 > 256) return false;  // producers keep <= 4 T1 rows per row group
+  if (g.meta128.max_h1 > 256) return false;  // k_cheb_t1 keeps <= 4 staged rows per row group
   if (fout != 64 && fout != 128 && fout != 256) return false;
-  // 128- and 256-wide layers run their T1-given and plain convs on the 64-row configuration (one ring of 3, one stage)
-  if (fout % WIDE_N == 0 &&
-      (g.meta64.n_pattern <= 0 ||
-       smem_bytes_dims(WIDE_N, 3, 1, g.meta64.max_h1, g.meta64.max_h1, g.meta64.stride, 1) > SMEM_LIMIT ||
-       smem_bytes_dims(WIDE_N, 3, 1, g.meta64.max_h1, g.meta64.max_h1, g.meta64.stride, 2) > SMEM_LIMIT))
-    return false;
-  return smem_bytes_for(CONV_N, ring_stages(CONV_N), 1, g) <= SMEM_LIMIT;
+  const int N = conv_n(fout);
+  const TileBlobs& t = conv_tiles(N, g, nullptr);
+  return t.n_pattern > 0 && smem_bytes_for(N, 3, 1, t, true) <= SMEM_LIMIT && smem_bytes_for(N, 3, 1, t, false) <= SMEM_LIMIT;
 }
 
-// X staging depth launch_n picks for a launch on the level's consecutive tiles: `t1_given` = mode 1 (T1 precomputed,
-// what the single-layer forward and the network run), `plain` = mode 2 (backward-data GEMM)
-int umma_conv_x_stages(const DevLevel& g, bool t1_given, bool plain) {
-  const int mode = plain ? 2 : (t1_given ? 1 : 0);
-  if (mode == 0) return x_stages(CONV_N, g);
-  return smem_bytes_for(CONV_N, ring_stages(CONV_N), 2, g, mode) <= SMEM_LIMIT ? 2 : 1;
+// X staging depth launch_n picks for a conv of Fout columns on the level's consecutive tiles (T1 given, or plain)
+int umma_conv_x_stages(const DevLevel& g, int fout, bool plain) {
+  const int N = conv_n(fout);
+  return conv_cfg(N, conv_tiles(N, g, nullptr), !plain).xs;
 }
-int umma_dw_x_stages(const DevLevel& g) { return dw_smem_bytes(2, g) <= SMEM_LIMIT ? 2 : 1; }
 bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && g_umma_tma && tmap_encoder() != nullptr; }
 
 __global__ void __launch_bounds__(256) k_pack_plain(const float* __restrict__ Bmat, long long ld_n, long long ld_k, int N,
@@ -2346,7 +2065,7 @@ namespace {
 template <int N>
 int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
   constexpr int NS = 3;
-  const size_t smem = smem_bytes_dims(N, NS, 1, 0, 0, 0, 2);
+  const size_t smem = smem_bytes_dims(N, NS, 1, 0, 0, false);
   auto kern = k_cheb_conv_umma<N, NS, 1, 0>;
   P2M_TRY((check_launch_regs<N, NS, 1, 0>()));
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -2392,7 +2111,6 @@ int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const 
   p.apack = static_cast<const unsigned char*>(apack);
   p.ep = to_dev(ep);
   p.res_identity = (ep.res != nullptr) ? 1 : 0;
-  p.plain = 1;
   p.ldy = N;
   p.y = Y;
   p.status = status;
@@ -2424,9 +2142,13 @@ int launch_umma_conv(const UmmaConvArgs& a, int* status, const float* zero_row, 
     set_error("umma_conv: the fused head needs fout == 64 and no residual");
     return P2M_ERR_INVALID;
   }
-  if (a.tiles != nullptr && ((a.t1 == nullptr && !a.plain) || a.tiles->max_h1 > 256 || a.tiles->n_pattern <= 0 ||
+  if (a.t1 == nullptr && !a.plain) {
+    set_error("umma_conv: the conv needs T1 = L~x (launch_cheb_t1) unless it is a plain GEMM");
+    return P2M_ERR_INVALID;
+  }
+  if (a.tiles != nullptr && (a.tiles->max_h1 > 256 || a.tiles->n_pattern <= 0 ||
                              (a.fout % WIDE_N == 0 && a.tiles->m64.n_pattern <= 0))) {
-    set_error("umma_conv: index-list tiles need the T1-given or plain mode and at most 256 staged rows");
+    set_error("umma_conv: index-list tiles need at most 256 staged rows");
     return P2M_ERR_INVALID;
   }
   return launch_n(a, status, zero_row, sm_count, s);

@@ -59,10 +59,7 @@ struct p2m_model {
                                  // the tile families exist, 0 = off (p2m_debug_set_elide_padding)
   int dedup_padding = 1;         // eval: among the isolated rows only one representative per class of identical rows is
                                  // computed (DevLevel::rep_tiles); needs elide_padding == 1 (p2m_debug_set_dedup_padding)
-  int dw_swap = 1;               // backward: dW from the basis of the gradient, re-using the backward-data pass's L~dz
-                                 // (launch_umma_dw_swapped); 0 = rebuild the basis of the layer input (p2m_debug_set_dw_swap)
   int fuse_head = 1;             // eval: the 128 -> 64 conv's epilogue feeds the 64 -> 3 head directly (no 64-wide tensor)
-  int split_t1 = 1;              // tensor-core conv: T1 = L~x in a separate pass (k_cheb_t1) instead of on-chip halo recompute
   int profiling = 0;             // record a CUDA event pair around every conv layer of the eval forward
   std::vector<cudaEvent_t> ev_beg, ev_end;
   std::vector<void*> owned;  // device allocations to free
@@ -294,14 +291,12 @@ int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpo
     a.head_wt = head_wt;
     a.head_z = head_z;
     // Padding-vertex elision (DevLevel::n_iso): connected rows through the conv on index-list tiles, isolated rows
-    // through a plain GEMM with the combined weights.  Needs the T buffer of the network schedules (3 Fin wide: the
-    // packed combined weights live behind the T1 part).
-    const bool elide = may_elide && m->elide_padding && m->split_t1 && T != nullptr && g.n_iso > 0 &&
-                       rows >= 2 * L.fout && (m->elide_padding >= 2 || 5LL * g.n_iso >= 2LL * g.V);
-    if (m->split_t1 && T != nullptr) {  // first sparse product as its own pass (T doubles as the T1 buffer)
-      P2M_TRY(launch_cheb_t1(g, x, in_unpool, B, L.fin, T, s, elide ? &g.real_tiles : nullptr));
-      a.t1 = T;
-    }
+    // through a plain GEMM with the combined weights (packed into T behind the T1 part: T is 3 Fin wide).
+    const bool elide = may_elide && m->elide_padding && g.n_iso > 0 && rows >= 2 * L.fout &&
+                       (m->elide_padding >= 2 || 5LL * g.n_iso >= 2LL * g.V);
+    // first sparse product as its own pass (T doubles as the T1 buffer)
+    P2M_TRY(launch_cheb_t1(g, x, in_unpool, B, L.fin, T, s, elide ? &g.real_tiles : nullptr));
+    a.t1 = T;
     a.g = &g;
     a.x = x;
     a.in_unpool = in_unpool;
@@ -664,12 +659,6 @@ int p2m_debug_set_trace(p2m_model_t* m, void* dev_buf) {
 #endif
 }
 
-// Debug / ablation: 1 (default) = two-pass tensor-core conv (k_cheb_t1 + conv with given T1), 0 = fully fused conv.
-int p2m_debug_set_split_t1(p2m_model_t* m, int enable) {
-  if (!m) return P2M_ERR_INVALID;
-  m->split_t1 = enable ? 1 : 0;
-  return P2M_OK;
-}
 int p2m_debug_set_elide_padding(p2m_model_t* m, int enable) {
   if (!m) return P2M_ERR_INVALID;
   m->elide_padding = enable < 0 ? 0 : (enable > 2 ? 2 : enable);
@@ -680,12 +669,7 @@ int p2m_debug_set_dedup_padding(p2m_model_t* m, int enable) {
   m->dedup_padding = enable ? 1 : 0;
   return P2M_OK;
 }
-int p2m_debug_set_dw_swap(p2m_model_t* m, int enable) {
-  if (!m) return P2M_ERR_INVALID;
-  m->dw_swap = enable ? 1 : 0;
-  return P2M_OK;
-}
-int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[10]) {
+int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[9]) {
   if (!m || !out || level < 0 || level >= (int)m->levels.size() || fin <= 0 || fout <= 0) {
     set_error("debug_conv_path: bad argument");
     return P2M_ERR_INVALID;
@@ -697,15 +681,14 @@ int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int3
   const bool dt = tc && umma_conv_supported(g, fout, fin) &&
                   umma_plain_pack_bytes(fin, fout) <= umma_wpack_bytes(((fin + 31) / 32) * 32, fout);
   out[0] = conv;
-  out[1] = conv ? umma_conv_x_stages(g, m->split_t1 != 0, false) : 0;
+  out[1] = conv ? umma_conv_x_stages(g, fout, false) : 0;
   out[2] = dw;
   out[3] = dw ? umma_dw_x_stages(g) : 0;
   out[4] = dt;
-  out[5] = dt ? umma_conv_x_stages(g, false, true) : 0;
-  out[6] = (g.tile_meta != nullptr && umma_tma_rows(g)) ? 1 : 0;
-  out[7] = g.tile_meta ? g.max_h1 : 0;
-  out[8] = g.tile_meta ? g.max_h2 : 0;
-  out[9] = g.n_iso;
+  out[5] = dt ? umma_conv_x_stages(g, fin, true) : 0;
+  out[6] = (g.meta128.n_pattern > 0 && umma_tma_rows(g)) ? 1 : 0;
+  out[7] = g.meta128.max_h1;
+  out[8] = g.n_iso;
   return P2M_OK;
 }
 
@@ -1066,11 +1049,11 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
       // which path takes this layer's weight / data gradients
       const bool thin = thin_conv_bwd_supported(L.fin, L.fout) && !in_unpool && !res_here && li > 0;
       const bool tc_dw = tc && !thin && umma_dw_supported(g, L.fin, L.fout);
-      const bool tc_dx = tc && !thin && need_dx && m->split_t1 && umma_conv_supported(g, L.fout, L.fin) &&
+      const bool tc_dx = tc && !thin && need_dx && umma_conv_supported(g, L.fout, L.fin) &&
                          umma_wpack_bytes(L.fout, L.fin) <= sc.wpack_bytes && (size_t)L.fout <= 3 * (size_t)L.fin;
       const bool tc_dt = tc && !thin && need_dx && !tc_dx && umma_conv_supported(g, L.fout, L.fin) &&
                          umma_plain_pack_bytes(L.fin, L.fout) <= sc.wpack_bytes;
-      const bool dw_swapped = tc_dx && m->dw_swap && umma_dw_swapped_supported(g, L.fin, L.fout);
+      const bool dw_dz_basis = tc_dx && umma_dw_supported(g, L.fout, L.fin);
       const bool want_scale = tc_dw || tc_dx || tc_dt;
       bool have_scale = false;
       if (L.bn) {
@@ -1103,19 +1086,22 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         P2M_TRY(launch_thin_conv_bwd(g, inp, rows, L.fin, L.fout, P->cl_w[li], g_z, sc.thin, out, G->cl_w[li],
                                      m->sm_count, s));
       } else {
-        // dW.  tensor-core path: the basis is rebuilt on chip by the forward's producers and contracted with the
-        // (power-of-two scaled) dz tile by MN-major wgmma; otherwise SIMT: materialise T, dWp = g_z^T T.
-        if (dw_swapped) {
+        // dW.  tensor-core path: T2 of one side is formed on chip by the forward's producers from T1 = L~(that side)
+        // and contracted with the (power-of-two scaled) plain tiles of the other side by MN-major wgmma; otherwise
+        // SIMT: materialise T, dWp = g_z^T T.
+        if (dw_dz_basis) {
           // sum_rows dz (x) T_k(X) = sum_rows T_k(dz) (x) X  (L~ symmetric): the basis of the GRADIENT, whose first
           // sparse product the backward-data pass below needs anyway, contracted with plain tiles of the layer input
           P2M_TRY(launch_cheb_t1(g, g_z, 0, B, L.fout, w.T, s, nullptr));
           P2M_TRY(launch_fill_zero(G->cl_w[li], sizeof(float) * L.fout * 3 * L.fin, s));
-          P2M_TRY(launch_umma_dw_swapped(g, inp, in_unpool, B, L.fin, L.fout, g_z, w.T, sc.a_scale, G->cl_w[li],
-                                         m->kernel_status, m->sm_count, s));
+          P2M_TRY(launch_umma_dw(g, B, g_z, 0, L.fout, w.T, inp, in_unpool, L.fin, 1, sc.a_scale, G->cl_w[li],
+                                 m->kernel_status, m->sm_count, s));
         } else if (tc_dw) {
+          // the basis of the layer input (w.T is overwritten by the dX pass's own T1 pass below)
+          P2M_TRY(launch_cheb_t1(g, inp, in_unpool, B, L.fin, w.T, s, nullptr));
           P2M_TRY(launch_fill_zero(G->cl_w[li], sizeof(float) * L.fout * 3 * L.fin, s));
-          P2M_TRY(launch_umma_dw(g, inp, in_unpool, B, L.fin, L.fout, g_z, sc.a_scale, G->cl_w[li], m->kernel_status,
-                                 m->sm_count, s));
+          P2M_TRY(launch_umma_dw(g, B, inp, in_unpool, L.fin, w.T, g_z, 0, L.fout, 0, sc.a_scale, G->cl_w[li],
+                                 m->kernel_status, m->sm_count, s));
         } else {
           P2M_TRY(launch_cheb_basis(g, inp, in_unpool, rows, L.fin, w.T, s));
           P2M_TRY(launch_fill_zero(sc.dwp, sizeof(float) * L.fout * 3 * L.fin, s));
@@ -1134,7 +1120,7 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         float* dst = finish ? sc.U : out;
         const bool elide = m->elide_padding && g.n_iso > 0 && rows >= 2 * L.fin &&
                            (m->elide_padding >= 2 || 5LL * g.n_iso >= 2LL * g.V);
-        if (!dw_swapped)  // (the swapped dW above already left L~dz of every row in w.T)
+        if (!dw_dz_basis)  // (the dW from the basis of dz above already left L~dz of every row in w.T)
           P2M_TRY(launch_cheb_t1(g, g_z, 0, B, L.fout, w.T, s, elide ? &g.real_tiles : nullptr));
         P2M_TRY(launch_umma_pack_weights_t(P->cl_w[li], L.fin, L.fout, sc.wpack, s));
         UmmaConvArgs a;
@@ -1369,11 +1355,14 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
     P2M_TRY(launch_absmax_scale(a->dz, (long long)rows * fout, a_scale, s));
     have_scale = true;
     // the layer input into fp16's range as well (with the basis headroom), in U (free until the dX pass); dW then
-    // comes out multiplied by that power of two
+    // comes out multiplied by that power of two.  L~U goes into the first rows x fin floats of T, which nothing reads
+    // before the dX pass overwrites it.
     P2M_TRY(launch_absmax_scale(a->x, (long long)rows * fin, rs.x_scale, s, g.headroom_log2));
     P2M_TRY(launch_scale_by(a->x, (long long)rows * fin, rs.x_scale, 0, 1.f, U, s));
+    P2M_TRY(launch_cheb_t1(g, U, 0, a->batch, fin, T, s));
     P2M_TRY(launch_fill_zero(a->dweight, sizeof(float) * fout * 3 * fin, s));
-    P2M_TRY(launch_umma_dw(g, U, 0, a->batch, fin, fout, a->dz, a_scale, a->dweight, m->kernel_status, m->sm_count, s));
+    P2M_TRY(launch_umma_dw(g, a->batch, U, 0, fin, T, a->dz, 0, fout, 0, a_scale, a->dweight, m->kernel_status,
+                           m->sm_count, s));
     P2M_TRY(launch_scale_by(a->dweight, (long long)fout * 3 * fin, rs.x_scale, 1, 1.f, a->dweight, s));
   } else {
     P2M_TRY(launch_cheb_basis(g, a->x, 0, (int)rows, fin, T, s));

@@ -61,7 +61,7 @@ struct DeviceGuard {
 // ---------------------------------------------------------------- device-resident hierarchy level
 // L~ of one level in CSR with RELATIVE column offsets: the neighbour of flat activation row
 // r = b*V + v is row r + reloff[p], so kernels never need (b, v) separately (block-diagonal I_B (x) L~).
-// Trimmed tile blobs (the tile's own rows, their 1-hop halo, the CSR of the own rows over staged-row slots, the own rows
+// Tile blobs (the tile's own rows, their 1-hop halo, the CSR of the own rows over staged-row slots, the own rows
 // in length-sorted order) of one level, for tiles of a fixed row count.
 struct TileBlobs {
   const unsigned char* meta = nullptr;  // [n_pattern][stride]
@@ -83,19 +83,10 @@ struct DevLevel {
   int* rowptr = nullptr;   // [V+1]
   int* reloff = nullptr;   // [nnz] col - row
   float* val = nullptr;    // [nnz]
-  // tensor-core path: per-tile-pattern halo / local-CSR blobs (cheb_umma.cu)
-  int n_pattern = 0;                    // tiles per mesh = ceil(V / 128)
-  const unsigned char* tile_meta = nullptr;   // [n_pattern][meta_stride]
-  const int* tile_meta_bytes = nullptr;       // [n_pattern] bytes to copy (multiple of 16)
-  int meta_stride = 0;
-  // trimmed blobs for the kernels that get X / T1 rows instead of recomputing them (k_cheb_t1, conv with T1 given):
-  // halo list up to the 1-hop rows and the CSR rows of the tile's own 128 rows only
-  const unsigned char* tile_meta1 = nullptr;  // [n_pattern][meta1_stride]
-  const int* tile_meta1_bytes = nullptr;
-  int meta1_stride = 0;
-  // the same trimmed blobs for 64-row tiles [64 p, 64 p + 64) (the 64-row x 128-column conv configuration)
-  TileBlobs meta64;
-  int max_h1 = 0, max_h2 = 0;
+  // tensor-core path (cheb_umma.cu): tile blobs of the 128-row tiles [128 p, 128 p + 128) (k_cheb_t1, the dW kernel,
+  // the 128-row conv configuration; n_pattern == 0: the level has no tensor-core metadata) and of the 64-row tiles
+  // [64 p, 64 p + 64) (the 64-row x 128-column conv configuration)
+  TileBlobs meta128, meta64;
   // L~ == L~^T exactly (the backward passes use L~ where the math needs L~^T), and h = ceil(log2(2 r^2 + 1)) for r the
   // largest absolute row sum of L~: max|T2| <= (2 r^2 + 1) max|x|, the headroom the single-layer fp16 split leaves
   bool symmetric = true;
@@ -259,7 +250,7 @@ struct UmmaConvArgs {
   float* y;                 // [rows, fout]
   // plain-GEMM mode (backward dT = dz * W_k): no SpMM, x is [rows, fin] and the K-blocks come from
   // launch_umma_pack_plain; y is written at y[r*ldy + y_col0 + n]
-  const float* t1 = nullptr;        // optional precomputed T1 = L~ x [rows, fin] (launch_cheb_t1)
+  const float* t1 = nullptr;        // T1 = L~ x [rows, fin] (launch_cheb_t1): required unless plain
   int plain = 0;
   const float* a_scale = nullptr;   // device scalar from launch_absmax_scale (or null)
   long long ldy = 0;                // 0: fout
@@ -268,12 +259,12 @@ struct UmmaConvArgs {
   // (head_wt = k_thin_prep's [64][12] table); y is then not written at all
   const float* head_wt = nullptr;
   float* head_z = nullptr;
-  // optional: run on this tile family instead of the level's consecutive 128-row tiles (T1-given and plain mode)
+  // optional: run on this tile family instead of the level's consecutive tiles
   const TileSet* tiles = nullptr;
   long long* trace = nullptr;       // debug (P2M_UMMA_TRACE builds only): [8][512] event log of CTA 0
 };
 // Host: build the per-tile halo metadata of one level (uploads; device pointers appended to `owned`).  A level whose
-// tiles exceed the metadata's 16-bit slot / entry offsets gets none (tile_meta stays null: it runs on SIMT).
+// tiles stage more than 512 rows or more than 65535 local-CSR entries gets none (meta128 stays empty: it runs on SIMT).
 int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val, int V, DevLevel* out,
                           std::vector<void*>* owned);
 // Tiles of 128 (and, TileSet::m64, 64) consecutive entries of `rows` (ascending vertex ids of one level) as a TileSet.
@@ -281,7 +272,7 @@ int build_index_tiles(const std::vector<int>& rows, const int* rowptr, const int
                       TileSet* ts, std::vector<void*>* owned);
 bool umma_conv_supported(const DevLevel& g, int fin, int fout);
 // what launch_umma_conv / launch_umma_dw would select on the level's consecutive tiles (p2m_debug_conv_path)
-int umma_conv_x_stages(const DevLevel& g, bool t1_given, bool plain);
+int umma_conv_x_stages(const DevLevel& g, int fout, bool plain);
 int umma_dw_x_stages(const DevLevel& g);
 bool umma_tma_rows(const DevLevel& g);
 size_t umma_wpack_bytes(int fin, int fout);
@@ -299,16 +290,15 @@ int launch_scale_by(const float* x, long long n, const float* scale, int invert,
 // same affine map with the bias folded into the shift
 int launch_rescaled_epilogue(const Epilogue& ep, const float* w_scale, float w_packed, int n, float* out_scale,
                              float* out_shift, cudaStream_t s);
-// dW[o, f*3+k] += sum_rows dz[row,o] * T_k(x)[row,f] on tensor cores (dw_ref zeroed by the caller)
-bool umma_dw_supported(const DevLevel& g, int fin, int fout);
-int launch_umma_dw(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, int fout, const float* dz,
-                   const float* a_scale, float* dw_ref, int* status, int sm_count, cudaStream_t s);
-// The same sum through the basis of the gradient (L~ symmetric): dW[o, f*3+k] += sum_rows T_k(dz)[row,o] * x[row,f], with
-// t1_dz = L~ dz [rows, fout] given for EVERY row (the backward-data pass leaves it behind): no 2-hop halo, no T1 on chip
-bool umma_dw_swapped_supported(const DevLevel& g, int fin, int fout);
-int launch_umma_dw_swapped(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, int fout,
-                           const float* dz, const float* t1_dz, const float* a_scale, float* dw_ref, int* status,
-                           int sm_count, cudaStream_t s);
+// dW[o, f*3+k] += sum_rows dz[row,o] * T_k(x)[row,f] on tensor cores (dw_ref [fout, 3 fin] zeroed by the caller), from
+// the Chebyshev basis of one side (`gathered` [rows(/2), gathered_width], t1 = L~ gathered for EVERY row, from
+// launch_cheb_t1) and plain tiles of the other (`plain` [rows(/2), plain_width]).  swap = 0: gathered = x, plain = dz;
+// swap = 1 (L~ symmetric: sum_rows dz (x) T_k(x) = sum_rows T_k(dz) (x) x): gathered = dz, plain = x.  a_scale (device
+// scalar) scales dz into fp16's range and is divided out.
+bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width);
+int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_unpool, int gathered_width,
+                   const float* t1, const float* plain, int g_unpool, int plain_width, int swap, const float* a_scale,
+                   float* dw_ref, int* status, int sm_count, cudaStream_t s);
 // T1 = L~ x for all rows of a level (tile-staged gather), t1 [batch*V, fin] fp32
 int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, float* t1, cudaStream_t s,
                    const TileSet* tiles = nullptr);

@@ -99,21 +99,16 @@ class BakedHierarchy:
     def set_profiling(self, device_index: int, enable: bool):
         _lib.check(_lib.load().p2m_model_set_profiling(self.handle(device_index), int(enable)), "set_profiling")
 
-    def set_debug(self, device_index: int, split_t1: Optional[bool] = None, fuse_head: Optional[bool] = None,
-                  elide_padding: Optional[int] = None, dedup_padding: Optional[bool] = None,
-                  dw_swap: Optional[bool] = None):
-        """Ablation switches of the tensor-core path: separate T1 pass (default on), fused 64->3 head in eval (default
-        on), isolated padding vertices through a plain GEMM with combined weights (0 off, 1 = default: levels with
-        >= 40 % isolated rows, 2 = every level that has the tile families)."""
+    def set_debug(self, device_index: int, fuse_head: Optional[bool] = None, elide_padding: Optional[int] = None,
+                  dedup_padding: Optional[bool] = None):
+        """Ablation switches of the tensor-core path: fused 64->3 head in eval (default on), isolated padding vertices
+        through a plain GEMM with combined weights (0 off, 1 = default: levels with >= 40 % isolated rows, 2 = every
+        level that has the tile families)."""
         lib, h = _lib.load(), self.handle(device_index)
-        if split_t1 is not None:
-            _lib.check(lib.p2m_debug_set_split_t1(h, int(split_t1)), "set_split_t1")
         if fuse_head is not None:
             _lib.check(lib.p2m_debug_set_fuse_head(h, int(fuse_head)), "set_fuse_head")
         if elide_padding is not None:
             _lib.check(lib.p2m_debug_set_elide_padding(h, int(elide_padding)), "set_elide_padding")
-        if dw_swap is not None:  # backward: dW from the basis of the gradient (default on) or of the layer input
-            _lib.check(lib.p2m_debug_set_dw_swap(h, int(dw_swap)), "set_dw_swap")
         if dedup_padding is not None:  # eval: one representative per class of identical isolated rows (default on)
             _lib.check(lib.p2m_debug_set_dedup_padding(h, int(dedup_padding)), "set_dedup_padding")
 

@@ -63,8 +63,8 @@ def far_edges(V, n_far):
 
 def hub(V=1024, n_spokes=60, seed=0):
     """Path graph plus one vertex (row 5) joined to n_spokes vertices spread over the whole graph: tile 0 stages its
-    spokes as 1-hop rows, every spoke's tile stages the hub's other spokes as 2-hop rows; |L~|'s row sum at the hub
-    is far above 1 (the basis grows by (2 r^2 + 1) there)."""
+    spokes as 1-hop rows, every spoke's tile stages the hub; |L~|'s row sum at the hub is far above 1 (the basis
+    grows by (2 r^2 + 1) there)."""
     rng = np.random.default_rng(seed)
     spokes = rng.choice(np.arange(130, V), size=n_spokes, replace=False)
     e = path_chords(V, chord=2) + [(5, int(s)) for s in spokes]
@@ -97,8 +97,8 @@ def isolated(V=1024, n_real=512, two_diagonals=False):
 
 
 def dense(V=2048, degree=64, seed=0):
-    """Random graph of degree ~64: every 128-row tile's 1-hop rows carry > 65535 CSR entries, beyond what the
-    tile metadata can index (16-bit offsets)."""
+    """Random graph of degree ~64: every 128-row tile stages far more than 512 rows (own rows + 1-hop halo), beyond
+    what the tile-metadata builder accepts."""
     rng = np.random.default_rng(seed)
     a = np.repeat(np.arange(V), degree // 2)
     b = rng.integers(0, V, size=a.size)
@@ -121,19 +121,18 @@ def nonsymmetric(V=256, seed=0):
 FAMILIES = {
     **{f"V{V}": ((lambda V=V: sized(V)), "ragged last tile / V < 128 / TMA (V % 128 == 0) vs cp.async rows")
        for V in (1, 64, 127, 128, 129, 1088, 2048)},
-    # band widths around the shared-memory limits (227 KB): 8, 12: two X stages everywhere; 14: the fused conv's X
-    # staging drops to one stage, the T1-given conv keeps two; 16: the T1-given conv drops to one; 20: the
-    # conv no longer fits at all (SIMT)
-    **{f"band{bw}": ((lambda bw=bw: band(1024, bw)), "x_stages 2 -> 1 and the shared-memory cut-off to SIMT")
+    # band widths around the shared-memory limits (227 KB): 8, 12, 14: two X stages; 16: the conv drops to one;
+    # 20: the conv still fits with one, the weight-gradient kernel no longer fits (SIMT dW)
+    **{f"band{bw}": ((lambda bw=bw: band(1024, bw)), "X stages 2 -> 1 and the shared-memory cut-off to SIMT")
        for bw in (8, 12, 14, 16, 20)},
     "h1_256": (lambda: far_edges(1024, 126), "max_h1 = 256: still tensor cores"),
     "h1_257": (lambda: far_edges(1024, 127), "max_h1 = 257: the 256-staged-row cut-off to SIMT"),
     "far": (lambda: far_edges(1088, 64), "halos that cross the whole graph (tile 0 <-> last, ragged) tile"),
-    "hub": (hub, "one tile with a huge 2-hop halo, |L~| row sum >> 1"),
+    "hub": (hub, "one tile with a halo spread over the whole graph, |L~| row sum >> 1"),
     "empty_rows": (empty_rows, "rows with no entries"),
     "iso_uniform": (isolated, "isolated rows with one diagonal: elision tile families built"),
     "iso_two_diag": ((lambda: isolated(two_diagonals=True)), "isolated rows with two diagonals: no elision"),
-    "dense": (dense, "tile metadata beyond the 65535 caps: the level runs on SIMT"),
+    "dense": (dense, "tile metadata beyond the builder's caps: the level runs on SIMT"),
     "nonsymmetric": (nonsymmetric, "L~ != L~^T"),
 }
 

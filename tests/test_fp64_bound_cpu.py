@@ -140,7 +140,7 @@ def test_graph_family_structure(name):
     if name == "dense":
         c = sp.csr_matrix(L)
         rows = set(range(128)) | set(c[:128].indices.tolist())
-        assert sum(deg[r] for r in rows) > 65535                                # tile 0's 1-hop CSR alone
+        assert len(rows) > 512                                                  # tile 0's staged rows alone
 
 
 def test_torch_coo_with_duplicates_coalesces_to_the_same_matrix():

@@ -47,9 +47,9 @@ def level(name):
 def conv_path(gh, fin, fout):
     from pose2mesh_release_b200 import _lib
 
-    out = (C.c_int32 * 10)()
+    out = (C.c_int32 * 9)()
     _lib.check(_lib.load().p2m_debug_conv_path(gh.handle(0), 0, fin, fout, out), "p2m_debug_conv_path")
-    return dict(zip(("conv", "conv_xs", "dw", "dw_xs", "dt", "dt_xs", "tma", "max_h1", "max_h2", "n_iso"), list(out)))
+    return dict(zip(("conv", "conv_xs", "dw", "dw_xs", "dt", "dt_xs", "tma", "max_h1", "n_iso"), list(out)))
 
 
 def run(L, x, W, b, precision, dz=None):
@@ -153,7 +153,7 @@ FAMILY_PATH = {
     "V1": dict(conv=1, tma=0), "V64": dict(conv=1, tma=0), "V127": dict(conv=1, tma=0), "V128": dict(conv=1, tma=1),
     "V129": dict(conv=1, tma=0), "V1088": dict(conv=1, tma=0), "V2048": dict(conv=1, tma=1),
     "band8": dict(conv=1, conv_xs=2), "band12": dict(conv=1, conv_xs=2), "band14": dict(conv=1, conv_xs=2),
-    "band16": dict(conv=1, conv_xs=1), "band20": dict(conv=0, dw=0),
+    "band16": dict(conv=1, conv_xs=1), "band20": dict(conv=1, conv_xs=1, dw=0),
     "h1_256": dict(conv=1, max_h1=256), "h1_257": dict(conv=0, dw=0, max_h1=257),
     "far": dict(conv=1, tma=0), "hub": dict(conv=1), "empty_rows": dict(conv=1),
     "iso_uniform": dict(conv=1, n_iso=512), "iso_two_diag": dict(conv=1, n_iso=0),
