@@ -261,6 +261,36 @@ int p2m_point_errors(const float* pred, const float* gt, const float* pred_root,
                      int n_point, const int32_t* subset, int n_subset, int fp64, float* err, double* sums,
                      p2m_stream_t stream);
 
+/* ---- demo camera fit (SURVEY.md §8 row f7; demo/run.py:149-197 optimize_cam_param, lib/models/project_net.py) --
+ * One launch fits the weak-perspective camera (s, tx, ty) of every person, one warp per person:
+ *   bbox [batch, 4]     process_bbox(get_bbox(joints), aspect_ratio=1.0, scale=1.25), float32
+ *   target [batch, n_in_joint, 2]   j2d_processing(joints, (crop, crop), bbox, 0, 0, None)[:, :2]
+ *   cam [batch, 3]      n_iter steps of Adam (betas (0.9, 0.999), eps 1e-8) on the L1 loss between
+ *                       ((pred_joints3d[..., :2] + cam[1:]) cam[0]) crop/2 + crop/2 and target[:, :n_joint],
+ *                       starting from init_cam [batch, 3]; step i runs at lr_values[p] for the last phase p with
+ *                       lr_steps[p] <= i (lr_steps[0] == 0, increasing; at most 16 phases)
+ *   loss [batch]        the L1 loss of the final camera
+ *   orig_cam [batch, 4] convert_crop_cam_to_orig_img(cam, bbox, img_wh[b, 0], img_wh[b, 1]) (demo/run.py:24-43); only
+ *                       when img_wh [batch, 2] (float32 pixel sizes) is given
+ * joints_px is float64 [batch, n_in_joint, in_cols] (columns past the first two are ignored) holding the caller's
+ * values exactly; in_kind says which dtype they came from, because the reference's arithmetic depends on it:
+ * integer inputs truncate the transformed points towards zero, float32 inputs take their box in float32.  A person
+ * whose box the reference rejects (process_bbox returns None) or whose joints hold a NaN gets NaN outputs; the
+ * others are unaffected.  Requires 0 < n_joint <= n_in_joint <= 32, batch > 0, 0 < crop <= 2^24.  No host
+ * synchronisation and no allocation (capturable in a CUDA graph).                                              */
+enum p2m_cam_input {
+  P2M_CAM_INPUT_F64 = 0,
+  P2M_CAM_INPUT_INT = 1,
+  P2M_CAM_INPUT_F32 = 2
+};
+int p2m_fit_camera(const double* joints_px, int in_cols, int in_kind, int n_in_joint, const float* pred_joints3d,
+                   int n_joint, const float* init_cam, int batch, int crop, int n_iter, const int32_t* lr_steps,
+                   const double* lr_values, int n_lr, const float* img_wh, float* cam, float* bbox, float* target,
+                   float* loss, float* orig_cam, p2m_stream_t stream);
+/* convert_crop_cam_to_orig_img alone: orig_cam [batch, 4] from cam [batch, 3], bbox [batch, 4], img_wh [batch, 2]. */
+int p2m_crop_cam_to_orig(const float* cam, const float* bbox, const float* img_wh, int batch, float* orig_cam,
+                         p2m_stream_t stream);
+
 /* ---- body model: batched SMPL / MANO forward (SURVEY.md §8 row f6; smplpytorch SMPL_Layer.forward,
  * manopth ManoLayer.forward) --------------------------------------------------------------------------------------
  * The descriptor holds HOST arrays in the reference's buffer layouts (all float32, row-major):
