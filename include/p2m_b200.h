@@ -291,6 +291,34 @@ int p2m_fit_camera(const double* joints_px, int in_cols, int in_kind, int n_in_j
 int p2m_crop_cam_to_orig(const float* cam, const float* bbox, const float* img_wh, int batch, float* orig_cam,
                          p2m_stream_t stream);
 
+/* ---- temporal metrics (SURVEY.md §8 row f8; lib/smooth_utils.py:5-72, lib/coord_utils.py:194-222) ----------------
+ * Ragged batches of sequences concatenated along frames: offsets (HOST int64 [n_seq + 1], checked here: offsets[0] = 0,
+ * non-decreasing, offsets[n_seq] = n_frames >= 1; empty sequences allowed) are copied to the device with a
+ * stream-ordered allocation.  dtype is P2M_DTYPE_F32 or P2M_DTYPE_F64 for every data array of a call; data arrays are
+ * device memory of one device.  Enqueued on `stream`; no other host allocation or synchronisation.  A sequence's
+ * results do not depend on its batch position.
+ *
+ * One-Euro filter (smooth_pose, OneEuroFilter): y[f, c] for x [n_frames, n_channel], per sequence along its frames,
+ * in numpy's dtype and operation order (bitwise the reference's result; t = frame index, dx0 = 0).  One launch.     */
+enum p2m_dtype {
+  P2M_DTYPE_F32 = 0,
+  P2M_DTYPE_F64 = 1
+};
+int p2m_one_euro_smooth(int dtype, const void* x, void* y, int64_t n_channel, const int64_t* offsets, int n_seq,
+                        int64_t n_frames, double min_cutoff, double beta, double d_cutoff, p2m_stream_t stream);
+/* Acceleration error (compute_error_accel) of gt, pred [n_frames, n_joint, 3], n_joint <= 32: for every window
+ * (s, i), i < n_s - 2, in the order of the sequences, per_window = the joint mean of |accel_pred - accel_gt| with
+ * accel = (X[i] - 2 X[i+1]) + X[i+2] (the reference's bits), valid (uint8) = vis[i] & vis[i+1] & vis[i+2] (vis: device
+ * uint8 [n_frames] or NULL = all visible), and seq_mean (double [n_seq]) = the fp64 mean of the sequence's valid
+ * windows, NaN when it has none.  Two launches (one when no sequence has 3 frames).                                */
+int p2m_accel_error(int dtype, const void* gt, const void* pred, int n_joint, const int64_t* offsets, int n_seq,
+                    int64_t n_frames, const uint8_t* vis, void* per_window, uint8_t* valid, double* seq_mean,
+                    p2m_stream_t stream);
+/* out[s] = the fp64 mean of values [n_rows, width] over rows offsets[s] .. offsets[s + 1) whose valid (device uint8
+ * [n_rows], or NULL = all) is non-zero, in a fixed order without atomics; NaN for a segment with no such row.       */
+int p2m_segment_mean(int dtype, const void* values, int64_t width, const int64_t* offsets, int n_seg, int64_t n_rows,
+                     const uint8_t* valid, double* out, p2m_stream_t stream);
+
 /* ---- body model: batched SMPL / MANO forward (SURVEY.md §8 row f6; smplpytorch SMPL_Layer.forward,
  * manopth ManoLayer.forward) --------------------------------------------------------------------------------------
  * The descriptor holds HOST arrays in the reference's buffer layouts (all float32, row-major):

@@ -9,6 +9,7 @@ Public surface (mirrors the reference's modules for this path, SURVEY.md §8b):
     dist.DataParallelStep                             one-process-per-GPU data parallel, single NCCL all-reduce
     body_model.SMPLLayer / body_model.ManoLayer       <- smplpytorch SMPL_Layer, manopth ManoLayer (batched, forward)
     camera.fit_cameras                                <- demo/run.py optimize_cam_param (batched camera fit)
+    temporal.smooth_pose / temporal.evaluate_video    <- lib/smooth_utils.py, compute_error_accel, the 3DPW video block
 
 All device work is in libp2m_b200.so (csrc/, C ABI in include/p2m_b200.h); there is no CPU fallback.
 """
@@ -18,5 +19,6 @@ from .meshnet import Pose2Mesh, get_model  # noqa: F401
 from .cheby_graph_conv import graph_conv_cheby  # noqa: F401
 from .body_model import ManoLayer, SMPLLayer  # noqa: F401
 from .camera import convert_crop_cam_to_orig_img, fit_cameras  # noqa: F401
+from .temporal import accel_errors, compute_error_accel, evaluate_video, smooth_pose, smooth_sequences  # noqa: F401
 
 __version__ = "0.1.0"

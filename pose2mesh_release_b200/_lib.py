@@ -109,6 +109,9 @@ P2M_CAM_INPUT_F64 = 0
 P2M_CAM_INPUT_INT = 1
 P2M_CAM_INPUT_F32 = 2
 
+P2M_DTYPE_F32 = 0
+P2M_DTYPE_F64 = 1
+
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
@@ -116,6 +119,7 @@ EXPORTS = [
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward", "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
     "p2m_rigid_align", "p2m_point_errors", "p2m_fit_camera", "p2m_crop_cam_to_orig",
+    "p2m_one_euro_smooth", "p2m_accel_error", "p2m_segment_mean",
     "p2m_body_model_create", "p2m_body_model_destroy", "p2m_body_model_workspace_bytes", "p2m_body_model_forward",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
 ]
@@ -210,6 +214,13 @@ def load() -> C.CDLL:
         lib.p2m_fit_camera.restype = C.c_int
         lib.p2m_crop_cam_to_orig.argtypes = [vp, vp, vp, C.c_int, vp, vp]
         lib.p2m_crop_cam_to_orig.restype = C.c_int
+        lib.p2m_one_euro_smooth.argtypes = [C.c_int, vp, vp, i64, c_int64_p, C.c_int, i64, C.c_double, C.c_double,
+                                            C.c_double, vp]
+        lib.p2m_one_euro_smooth.restype = C.c_int
+        lib.p2m_accel_error.argtypes = [C.c_int, vp, vp, C.c_int, c_int64_p, C.c_int, i64, vp, vp, vp, vp, vp]
+        lib.p2m_accel_error.restype = C.c_int
+        lib.p2m_segment_mean.argtypes = [C.c_int, vp, i64, c_int64_p, C.c_int, i64, vp, vp, vp]
+        lib.p2m_segment_mean.restype = C.c_int
         lib.p2m_body_model_create.argtypes = [C.POINTER(BodyModelDesc), C.POINTER(vp)]
         lib.p2m_body_model_create.restype = C.c_int
         lib.p2m_body_model_destroy.argtypes = [vp]
