@@ -349,7 +349,7 @@ struct KParams {
 // production kernels carry no clock reads.
 #ifdef P2M_UMMA_TRACE
 __device__ __forceinline__ void trace_ev(const KParams& p, int role, int& n, int ev) {
-  if (p.trace != nullptr && blockIdx.x == 0 && n < 512) {
+  if (p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && n < 512) {
     p.trace[role * 512 + n] = ((long long)ev << 48) | (clock64() & 0xFFFFFFFFFFFFll);
     ++n;
   }
@@ -421,11 +421,13 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
   float* ep_mul = reinterpret_cast<float*>(flags + 4);  // [N] acc * mul + add  (weight scale, bias, folded BN)
   float* ep_add = ep_mul + N;
-  // epilogue transpose staging: [4 warps][32 rows][EC floats], 16-byte chunks XOR-swizzled by the row (ER rows used)
+  // epilogue transpose staging, 16-byte chunks XOR-swizzled by the row: N = 64: [4 warps][32 rows][EC floats], one
+  // 32-column sub-slab at a time; N = 128: [4 warps][4 sub-slabs][16 rows][EC floats], a warp's whole 16 x 128 block
   constexpr int EC = 32;
+  constexpr int STG_WARP_BYTES = N == 128 ? 4 * 16 * EC * 4 : 32 * EC * 4;
   unsigned char* epi_stage =
       reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(ep_add + N) + 127) & ~(uintptr_t)127);
-  int* own_s = reinterpret_cast<int*>(epi_stage + 4 * 32 * EC * 4);  // [4 warps][32] vertex id of each epilogue row
+  int* own_s = reinterpret_cast<int*>(epi_stage + 4 * STG_WARP_BYTES);  // [4 warps][32] vertex id of each epilogue row
   float* head_w_s = reinterpret_cast<float*>(own_s + 4 * 32);        // [64][12] (N == 64 with a fused head)
 
   const int tid = threadIdx.x;
@@ -601,7 +603,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     const int wq = warp - W_EPI0;
     constexpr int CPR = EC / 4;             // 16-byte chunks per staged row
     constexpr int RPI = 32 / CPR;           // rows covered by one warp-wide 16-byte access
-    const uint32_t stg = smem_u32(epi_stage) + (uint32_t)wq * (32 * EC * 4);
+    const uint32_t stg = smem_u32(epi_stage) + (uint32_t)wq * STG_WARP_BYTES;
     const int prow = lane / CPR, pc = lane % CPR;
     constexpr int NP = ER / RPI;            // phase-2 rows (pieces) per thread and sub-slab
     int colk[2];  // column (inside a sub-slab) of the 16-byte chunk this thread handles for rows of swizzle class k
@@ -653,7 +655,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 1);
       for (int u = 0; u < uses; ++u, ++ucnt) {
         const uint32_t s = ucnt % NS;
+        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 4);
         mbar_wait(smem_u32(b_ab_full + s), (ucnt / NS) & 1, abort_flag, p.status, 6);
+        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 5);
         const uint32_t a0 = smem_u32(ring + s * SLOT_BYTES);
         wg_fence();
 #pragma unroll
@@ -676,8 +680,10 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         if (lane == 0) mbar_arrive(smem_u32(b_ab_empty + s));  // this warp is done reading the slot
       }
       if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 2);
-      // phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by row)
+      // phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by row;
+      // N = 128: each sub-slab into its own 16-row block)
       auto stage_slab = [&](int cb) {
+        const uint32_t sb = stg + (N == 128 ? (uint32_t)(cb / 32) * (16 * EC * 4) : 0u);
 #pragma unroll
         for (int h = 0; h < H; ++h)
 #pragma unroll
@@ -688,7 +694,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
               const int cc = 8 * jj + 2 * (lane & 3);
               const int ah = TM == 128 ? h : cb / 64;                 // row half / column half of the accumulator
               const int j = 4 * ((TM == 128 ? cb : cb % 64) / 8 + jj) + 2 * r;
-              sts_f2(stg + lr * (EC * 4) + ((((uint32_t)(cc >> 2)) ^ (uint32_t)(lr & 7)) << 4) + (cc & 3) * 4,
+              sts_f2(sb + lr * (EC * 4) + ((((uint32_t)(cc >> 2)) ^ (uint32_t)(lr & 7)) << 4) + (cc & 3) * 4,
                      acc[ah][j], acc[ah][j + 1]);
             }
         __syncwarp();
@@ -727,6 +733,65 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           zr[1] = make_float4(z[4], z[5], z[6], z[7]);
           zr[2] = make_float4(z[8], z[9], z[10], z[11]);
         }
+      } else if (N == 128) {
+        // The whole 16 x 128 block of the warp is staged first: the accumulator is dead after that, and its registers
+        // hold every identity-residual load of the block, issued at once, so the tile pays one L2 round trip for its
+        // residual instead of one per 32-column sub-slab
+#pragma unroll
+        for (int cb = 0; cb < N; cb += 32) stage_slab(cb);
+        const bool res_id = p.ep.res != nullptr && p.res_identity;
+        float4 rv[N / 32][NP];
+#pragma unroll
+        for (int cb = 0; cb < N; cb += 32)
+#pragma unroll
+          for (int i = 0; i < NP; ++i) {
+            rv[cb / 32][i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (res_id && own_v[i] >= 0) {
+              const long long r = mesh0 + own_v[i];
+              rv[cb / 32][i] = __ldg(reinterpret_cast<const float4*>(
+                  p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + ecol0 + cb + colk[i & 1]));
+            }
+          }
+#pragma unroll
+        for (int cb = 0; cb < N; cb += 32) {
+          const uint32_t sb = stg + (uint32_t)(cb / 32) * (16 * EC * 4);
+          float4 mu_k[2], ad_k[2];
+#pragma unroll
+          for (int k = 0; k < 2; ++k) {
+            mu_k[k] = *reinterpret_cast<const float4*>(ep_mul + cb + colk[k]);
+            ad_k[k] = *reinterpret_cast<const float4*>(ep_add + cb + colk[k]);
+          }
+#pragma unroll
+          for (int i = 0; i < NP; ++i) {
+            const int rr = i * RPI + prow;
+            const int gn = ecol0 + cb + colk[i & 1];  // column of the layer's output
+            const float4 a = lds_f4(sb + rr * (EC * 4) + (pc << 4));
+            const int vtx = own_v[i];
+            if (vtx >= 0) {
+              const float4 mu = mu_k[i & 1], ad = ad_k[i & 1];
+              float o[4] = {fmaf(a.x, mu.x, ad.x), fmaf(a.y, mu.y, ad.y), fmaf(a.z, mu.z, ad.z), fmaf(a.w, mu.w, ad.w)};
+              if (p.ep.relu) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) o[e] = fmaxf(o[e], 0.f);
+              }
+              const long long r = mesh0 + vtx;
+              if (p.ep.res != nullptr) {
+                if (p.res_identity) {
+                  o[0] += rv[cb / 32][i].x; o[1] += rv[cb / 32][i].y; o[2] += rv[cb / 32][i].z; o[3] += rv[cb / 32][i].w;
+                } else {
+                  const float* res_row = p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F;
+#pragma unroll
+                  for (int e = 0; e < 4; ++e) {
+                    const float l = __ldg(p.ep.lam + gn + e);
+                    o[e] += (1.f - l) * __ldg(res_row + __ldg(p.ep.i0 + gn + e)) + l * __ldg(res_row + __ldg(p.ep.i1 + gn + e));
+                  }
+                }
+              }
+              *reinterpret_cast<float4*>(p.y + r * p.ldy + p.y_col0 + gn) = make_float4(o[0], o[1], o[2], o[3]);
+            }
+          }
+        }
+        __syncwarp();  // the staging block is read before the next tile overwrites it
       } else {
 #pragma unroll
         for (int cb = 0; cb < N; cb += 32) {
@@ -1452,7 +1517,8 @@ __global__ void __launch_bounds__(256) k_pack_weights(const float* __restrict__ 
 // debug: P2M_UMMA_TMA=0 stages every row with cp.async (A/B measurements of the TMA own-row loads)
 const bool g_umma_tma = [] { const char* e = std::getenv("P2M_UMMA_TMA"); return !(e && e[0] == '0'); }();
 
-inline int epi_stage_bytes(int) { return 4 * 32 * 32 * 4; }  // per-warp transpose staging
+// per-warp transpose staging: one 32 x 32 sub-slab per warp (N = 64), a warp's whole 16 x 128 block (N = 128)
+inline int epi_stage_bytes(int N) { return N == 128 ? 4 * 16 * 128 * 4 : 4 * 32 * 32 * 4; }
 // Dynamic shared memory of a conv configuration: T1 given (MODE 1: the tile's own X rows and the T1 rows of the tile
 // and its 1-hop halo per stage) or plain (MODE 0: the own X rows per stage).  N = 128: the 64-row configuration (64-row
 // tiles; with a given T1 and NS >= 3 no X stage: the producers read X directly).

@@ -51,6 +51,7 @@ struct p2m_model {
   int* kernel_status = nullptr;       // device alias of status_host (what the kernels write)
   volatile int* status_host = nullptr;  // mapped pinned host word: set by a tensor-core kernel whose mbarrier wait timed out
   long long* trace = nullptr;          // debug (P2M_UMMA_TRACE builds): CTA-0 event log of the tensor-core conv kernel
+  int trace_seen = 0;                  // matching conv launches since the trace buffer was set (P2M_TRACE_NTH)
   int* out_map = nullptr;        // optional fused output gather (vertex -> slot, -1 = dropped)
   int out_rows = 0;
   float* zero_row = nullptr;     // 128 B of zeros (halo source for the empty slots of ragged tiles)
@@ -287,6 +288,9 @@ int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpo
       const char* tu = getenv("P2M_TRACE_UNPOOL");
       const char* tf = getenv("P2M_TRACE_FOUT");
       if ((tv && atoi(tv) != L.V) || (tu && atoi(tu) != in_unpool) || (tf && atoi(tf) != L.fout)) a.trace = nullptr;
+      // P2M_TRACE_NTH = k: only the k-th (from 0) matching conv launch since p2m_debug_set_trace is logged
+      const char* tn = getenv("P2M_TRACE_NTH");
+      if (a.trace != nullptr && tn && m->trace_seen++ != atoi(tn)) a.trace = nullptr;
     }
     a.head_wt = head_wt;
     a.head_z = head_z;
@@ -316,6 +320,7 @@ int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpo
     P2M_TRY(launch_umma_pack_iso(w_ref, g.iso_diag, L.fin, L.fout, w_iso, s));
     a.t1 = nullptr;
     a.plain = 1;
+    a.trace = nullptr;  // the trace buffer holds the connected rows' launch; the isolated rows' GEMM would overwrite it
     a.tiles = reps_only ? &g.rep_tiles : &g.iso_tiles;
     a.wpack = w_iso;
     return launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s);
@@ -651,6 +656,7 @@ int p2m_debug_set_trace(p2m_model_t* m, void* dev_buf) {
   if (!m) return P2M_ERR_INVALID;
 #ifdef P2M_UMMA_TRACE
   m->trace = static_cast<long long*>(dev_buf);
+  m->trace_seen = 0;
   return P2M_OK;
 #else
   if (dev_buf == nullptr) return P2M_OK;

@@ -1,5 +1,8 @@
 """Debug aid (GPU box, P2M_TRACE=1 build): event timeline of CTA 0 of the conv kernel of ONE layer of the eval forward
-at the bench workload.  Usage: P2M_TRACE_V=12288 P2M_TRACE_UNPOOL=0 python tools/umma_trace_model.py [n_events=400]"""
+at the bench workload, and per-role busy / wait totals over the logged window.
+Usage: P2M_TRACE_V=12288 P2M_TRACE_UNPOOL=0 [P2M_TRACE_FOUT=128] [P2M_TRACE_NTH=k] python tools/umma_trace_model.py [n_events=400]
+P2M_TRACE_NTH picks the k-th (from 0) matching launch of the forward, so that exactly one launch is logged (without it
+every matching launch writes into the same buffer)."""
 import os
 import sys
 
@@ -28,24 +31,57 @@ with torch.no_grad():
     torch.cuda.synchronize()
     lib.p2m_debug_set_trace(h, None)
 t = buf.cpu().numpy().reshape(8, 512)
-names = {0: "producer", 1: "bload", 2: "mma", 3: "epilogue", 4: "loader"}
+names = {0: "producer", 1: "bload", 3: "mma + epilogue", 4: "loader"}
 ev_all = []
-for role in range(5):
+per_role = {r: [] for r in names}
+for role in names:
     for v in t[role]:
         if v:
-            ev_all.append((int(v) & 0xFFFFFFFFFFFF, role, int(v) >> 48))
+            e = (int(v) & 0xFFFFFFFFFFFF, role, int(v) >> 48)
+            ev_all.append(e)
+            per_role[role].append(e)
+if not ev_all:
+    sys.exit("no events logged: check the P2M_TRACE_* filters and the P2M_TRACE=1 build")
 ev_all.sort()
 t0 = ev_all[0][0]
-pn = {1: "wait_x", 2: "x_ready", 4: "T1 gathered", 5: "T1 barrier passed", 6: "T2 gathered", 7: "blocks emitted", 8: "end barrier"}
+pn = {1: "wait_x", 2: "x_ready", 6: "T2 gathered", 7: "blocks emitted", 8: "end barrier"}
+mn = {1: "tile start", 2: "main loop done", 4: "wait full slot", 5: "slot full -> 12 MMAs"}
 for c, role, ev in ev_all[:n_ev]:
     if role == 0:
         label = pn.get(ev, str(ev))
     elif role == 1:
         label = f"slot free -> load B block {ev - 10}"
-    elif role == 2:
-        label = "acc buffer free" if ev == 1 else f"A/B block {ev - 10} full -> 6 MMAs"
     elif role == 3:
-        label = "accumulator ready" if ev == 1 else "tile stored"
+        label = mn.get(ev, str(ev))
     else:
         label = "stage free" if ev == 1 else "copies issued"
-    print(f"{c - t0:9d}  {names[role]:9s} {label}")
+    print(f"{c - t0:9d}  {names[role]:14s} {label}")
+
+
+def spans(role, a, b):
+    """Sum of (time of event b - time of the event a before it) over the role's log, in cycles."""
+    tot, last = 0, None
+    for c, _, ev in per_role[role]:
+        if ev == a:
+            last = c
+        elif ev == b and last is not None:
+            tot += c - last
+            last = None
+    return tot
+
+
+t1 = ev_all[-1][0]
+window = max(1, t1 - t0)
+rows = [
+    ("mma", "wait on a full slot", spans(3, 4, 5)),
+    ("mma", "issue (slot full -> next wait)", spans(3, 5, 4) + spans(3, 5, 2)),
+    ("mma", "epilogue (main loop done -> next tile)", spans(3, 2, 1)),
+    ("producer", "wait on staged rows", spans(0, 1, 2)),
+    ("producer", "gather", spans(0, 2, 6)),
+    ("producer", "empty-slot wait + stores", spans(0, 6, 7)),
+    ("producer", "end barrier", spans(0, 7, 8)),
+    ("loader", "wait on a free stage", spans(4, 2, 1)),
+]
+print(f"\nlogged window: {window} cycles (CTA 0; each role's log holds at most 512 events)")
+for role, what, cyc in rows:
+    print(f"{role:9s} {what:40s} {cyc:10d} cycles  {100.0 * cyc / window:5.1f} %")
