@@ -319,6 +319,34 @@ int p2m_accel_error(int dtype, const void* gt, const void* pred, int n_joint, co
 int p2m_segment_mean(int dtype, const void* values, int64_t width, const int64_t* offsets, int n_seg, int64_t n_rows,
                      const uint8_t* valid, double* out, p2m_stream_t stream);
 
+/* ---- FreiHAND scores (SURVEY.md §8 row f9; the FreiHAND dataset's eval.py / utils/eval_util.py) ----------------
+ * All arithmetic is fp64 on the inputs' values; a distance is sqrt((dx^2 + dy^2) + dz^2), each step rounded to
+ * nearest.  Thresholds are HOST double arrays, checked here (finite, >= 0, sorted ascending) and passed to the kernels
+ * by value.  Data arrays are device memory of one device; enqueued on `stream`, no host synchronisation.  Results
+ * are bitwise deterministic and do not depend on a sample's batch position.
+ *
+ * Nearest distances between P [batch, n, 3] and Q [batch, m, 3] (dtype P2M_DTYPE_F32 or _F64 for both; n, m <= 2^20):
+ * dist_p [batch, n] = min_j |P_i - Q_j|, dist_q [batch, m] = min_i |Q_j - P_i| (f64, equal to the brute force bit for
+ * bit), from one sweep of the n x m pairs.  With 1 .. 16 thresholds t: counts [batch, 2, n_thr] (int64) = #(dist_p <
+ * t), #(dist_q < t); frac [batch, 2, n_thr] = counts / n, / m; fscore [batch, n_thr] = ((2 a) b) / (a + b), 0 when
+ * a + b = 0.  A sample holding a non-finite coordinate gets NaN distances, zero counts and NaN frac / fscore.  Every
+ * output is nullable (at least one given); a missing distance output gets stream-ordered scratch.  Three launches. */
+int p2m_nearest_distances(int dtype, const void* P, const void* Q, int batch, int n, int m, const double* thresholds,
+                          int n_thr, double* dist_p, double* dist_q, int64_t* counts, double* frac, double* fscore,
+                          p2m_stream_t stream);
+/* align_w_scale(gt, pred) per sample of [batch, n_point, 3] float32: both centred and scaled by their Frobenius norm
+ * (+ 1e-8), R = U V^T and s = sum(W) for U W V^T = svd(A^T P) (no reflection correction), aligned = (P R^T) s s1 + t1
+ * (nullable, [batch, n_point, 3] in aligned_dtype), err [batch, n_point] f64 = |aligned - gt| (nullable).  A sample
+ * holding a non-finite coordinate gets NaN.  One launch.                                                           */
+int p2m_align_w_scale(const float* gt, const float* pred, int batch, int n_point, int aligned_dtype, void* aligned,
+                      double* err, p2m_stream_t stream);
+/* PCK histogram: hist[j] (device int64 [n_thr], accumulated, not cleared) += the number of errors e whose first
+ * threshold with e <= t_j is j (NaN and e > t_last count nowhere); the count of e <= t_j is hist[0] + ... + hist[j].
+ * The errors are err [n_val] (f64), or e = |pred_i - gt_i| for n_val float32 points (then optionally stored to
+ * err_out [n_val] f64).  1 .. 128 thresholds.  One launch; integer atomics, so the histogram is order-free.         */
+int p2m_pck_accumulate(const double* err, const float* pred, const float* gt, int64_t n_val, const double* thresholds,
+                       int n_thr, double* err_out, int64_t* hist, p2m_stream_t stream);
+
 /* ---- body model: batched SMPL / MANO forward (SURVEY.md §8 row f6; smplpytorch SMPL_Layer.forward,
  * manopth ManoLayer.forward) --------------------------------------------------------------------------------------
  * The descriptor holds HOST arrays in the reference's buffer layouts (all float32, row-major):

@@ -11,6 +11,7 @@
 #include <string>
 
 #include "p2m_internal.h"
+#include "procrustes3.cuh"
 
 namespace p2m {
 namespace {
@@ -20,29 +21,6 @@ constexpr int NW = MT / 32;      // warps per CTA
 constexpr int MAX_GRID = 4096;   // CTAs of the grid-stride loop over samples
 constexpr int MAX_BATCH = 1 << 24;
 constexpr int MAX_POINTS = 1 << 24;
-
-// v[k] <- the CTA-wide sum of v[k], the same bits in every thread: xor-shuffle tree inside each warp, then the warp
-// partials in warp order.  Ends with a barrier, so `red` can be reused by the next call.
-template <int N>
-__device__ __forceinline__ void block_sum(double (&v)[N], double (*red)[NW]) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    double a = v[k];
-    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-    if (lane == 0) red[k][warp] = a;
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    double a = 0.0;
-    for (int w = 0; w < NW; ++w) a += red[k][w];
-    v[k] = a;
-  }
-  __syncthreads();
-}
-
-__device__ __forceinline__ double dot3(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
 // rigid_transform_3D (coord_utils.py:127-143) from the centred statistics of one sample, fp64, one thread.
 //   h[3 r + c] = sum_i (A_i - muA)_r (B_i - muB)_c / n,  varP = sum_axes var(A) (population, as np.var)
@@ -60,86 +38,16 @@ __device__ void procrustes_3x3(const double* h, double varP, const double* mu_a,
     for (int k = 0; k < 13; ++k) out[k] = nan("");
     return;
   }
-  double W[3][3], V[3][3];
-  for (int r = 0; r < 3; ++r)
-    for (int c = 0; c < 3; ++c) {
-      W[r][c] = h[3 * r + c];
-      V[r][c] = (r == c) ? 1.0 : 0.0;
-    }
-  const int P[3] = {0, 0, 1}, Q[3] = {1, 2, 2};
-  for (int sweep = 0; sweep < 40; ++sweep) {
-    bool rotated = false;
-    for (int pq = 0; pq < 3; ++pq) {
-      const int p = P[pq], q = Q[pq];
-      double alpha = 0.0, beta = 0.0, gamma = 0.0;
-      for (int r = 0; r < 3; ++r) {
-        alpha += W[r][p] * W[r][p];
-        beta += W[r][q] * W[r][q];
-        gamma += W[r][p] * W[r][q];
-      }
-      if (!(fabs(gamma) > 1e-15 * sqrt(alpha * beta))) continue;
-      const double zeta = (beta - alpha) / (2.0 * gamma);
-      const double t = copysign(1.0, zeta) / (fabs(zeta) + hypot(1.0, zeta));
-      const double cs = 1.0 / sqrt(1.0 + t * t), sn = cs * t;
-      for (int r = 0; r < 3; ++r) {
-        const double wp = W[r][p], wq = W[r][q];
-        W[r][p] = cs * wp - sn * wq;
-        W[r][q] = sn * wp + cs * wq;
-        const double vp = V[r][p], vq = V[r][q];
-        V[r][p] = cs * vp - sn * vq;
-        V[r][q] = sn * vp + cs * vq;
-      }
-      rotated = true;
-    }
-    if (!rotated) break;
-  }
-  double sv[3];
-  int ord[3] = {0, 1, 2};
-  for (int j = 0; j < 3; ++j) sv[j] = sqrt(W[0][j] * W[0][j] + W[1][j] * W[1][j] + W[2][j] * W[2][j]);
-  for (int i = 0; i < 2; ++i)  // stable sort, descending
-    for (int j = 0; j < 2 - i; ++j)
-      if (sv[ord[j]] < sv[ord[j + 1]]) {
-        const int x = ord[j];
-        ord[j] = ord[j + 1];
-        ord[j + 1] = x;
-      }
-  double w[3][3], v[3][3];  // w[j] / v[j]: column j of the sorted W / V
-  for (int j = 0; j < 3; ++j)
-    for (int r = 0; r < 3; ++r) {
-      w[j][r] = W[r][ord[j]];
-      v[j][r] = V[r][ord[j]];
-    }
-  const double s1 = sv[ord[0]], s2 = sv[ord[1]];
-  double u[3][3];
-  if (s1 > 0.0) {
-    for (int r = 0; r < 3; ++r) u[0][r] = w[0][r] / s1;
-  } else {  // H = 0: any basis
-    u[0][0] = 1.0, u[0][1] = 0.0, u[0][2] = 0.0;
-  }
-  // u2: w2 orthogonalised against u1; when w2 vanishes (rank-1 H) any unit vector orthogonal to u1
-  {
-    double x[3];
-    const double d = dot3(w[1], u[0]);
-    for (int r = 0; r < 3; ++r) x[r] = w[1][r] - d * u[0][r];
-    double nx = sqrt(dot3(x, x));
-    if (!(nx > 1e-12 * s1)) {
-      int a = 0;  // the axis least aligned with u1
-      for (int r = 1; r < 3; ++r)
-        if (fabs(u[0][r]) < fabs(u[0][a])) a = r;
-      const double e = u[0][a];
-      for (int r = 0; r < 3; ++r) x[r] = ((r == a) ? 1.0 : 0.0) - e * u[0][r];
-      nx = sqrt(dot3(x, x));
-    }
-    for (int r = 0; r < 3; ++r) u[1][r] = x[r] / nx;
-  }
-  u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];
-  u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
-  u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+  Svd3 sd;
+  svd3_jacobi(h, sd);
+  const double(&u)[3][3] = sd.u;
+  const double(&v)[3][3] = sd.v;
+  const double s1 = sd.s1, s2 = sd.s2;
   const double det_v = v[0][0] * (v[1][1] * v[2][2] - v[1][2] * v[2][1]) -
                        v[1][0] * (v[0][1] * v[2][2] - v[0][2] * v[2][1]) +
                        v[2][0] * (v[0][1] * v[1][2] - v[0][2] * v[1][1]);
   const double dv = det_v < 0.0 ? -1.0 : 1.0;
-  const double s3 = dot3(w[2], u[2]) * dv;
+  const double s3 = sd.w3u3 * dv;
   const double c = (1.0 / varP) * ((s1 + s2) + s3);
   double R[3][3];
   for (int i = 0; i < 3; ++i)
