@@ -21,10 +21,12 @@
 //   * 1 warpgroup issues wgmma.mma_async (m64n64k16, f16 -> f32) on both 64-row halves of the tile (or both 64-column
 //     halves of the weight block) into register accumulators: per 16 features three MMAs — hi*Whi + lo*Whi + hi*Wlo — an error-compensated product with ~2^-21
 //     relative error, which is what keeps the 1e-4 fp32 parity bar (plain TF32/FP16 does not, SURVEY.md §7
-//     "hard parts" 1).  After the tile's last K-block the same warpgroup transposes the accumulator through a
-//     swizzled per-warp staging buffer so that global accesses are coalesced, and applies the fused epilogue —
-//     bias / folded BatchNorm, ReLU, channel-resampled residual (or, for the network's last block, the 64 -> 3
-//     head's projection) — while the producers already fill the ring for the next tile.
+//     "hard parts" 1).  After the tile's last K-block the same warpgroup applies the fused epilogue — bias / folded
+//     BatchNorm, ReLU, channel-resampled residual (or, for the network's last block, the 64 -> 3 head's projection) —
+//     through a per-warp staging buffer, while the producers already fill the ring for the next tile.  N = 64: the
+//     accumulator is transposed through swizzled staging so that global accesses are coalesced.  N = 128: the
+//     epilogue runs in the fragment layout, in place in linear 512-byte staging rows that the copy engine fills with
+//     the identity residual during the main loop and drains to HBM by cp.async.bulk stores nobody waits for.
 // The unpool between levels is virtual: with in_unpool the rows are read from row r>>1 of the coarser
 // tensor.  Weights are pre-scaled by 2^6 so that their lo parts stay normal fp16 numbers (undone exactly in the
 // epilogue).  The same kernel in `plain` mode is the backward dT GEMM and, with pre-packed A blocks, the dense GEMM;
@@ -68,6 +70,11 @@ struct TileHeader {  // 64 bytes
 static_assert(sizeof(TileHeader) == 64, "header size");
 
 inline int up16(int x) { return (x + 15) & ~15; }
+
+// Epilogue staging of the 64 x 128 (N = 128) configuration: each MMA warp's 16 x 128 fp32 block as 16 linear rows of
+// 512 bytes (what one cp.async.bulk moves) at a stride of 544 bytes.  136 floats is 8 banks mod 32, so the four rows a
+// half-warp's 64-bit fragment access touches (8 consecutive words each) cover the 32 banks exactly once.
+constexpr int STG_ROW_BYTES = 544;
 
 // ------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -156,6 +163,15 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// shared -> global bulk copy, completed through the issuing thread's bulk async-groups (no mbarrier)
+__device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the thread's bulk stores have finished READING their shared-memory source (it may be overwritten)
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// ... and have completed
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
@@ -182,6 +198,11 @@ __device__ __forceinline__ void producer_barrier() { asm volatile("bar.sync 1, 5
 __device__ __forceinline__ float4 lds_f4(uint32_t a) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ float2 lds_f2(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a));
   return v;
 }
 __device__ __forceinline__ uint2 lds_u2(uint32_t a) {
@@ -421,14 +442,16 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
   float* ep_mul = reinterpret_cast<float*>(flags + 4);  // [N] acc * mul + add  (weight scale, bias, folded BN)
   float* ep_add = ep_mul + N;
-  // epilogue transpose staging, 16-byte chunks XOR-swizzled by the row: N = 64: [4 warps][32 rows][EC floats], one
-  // 32-column sub-slab at a time; N = 128: [4 warps][4 sub-slabs][16 rows][EC floats], a warp's whole 16 x 128 block
+  // epilogue staging: N = 64: [4 warps][32 rows][EC floats], 16-byte chunks XOR-swizzled by the row, one 32-column
+  // sub-slab at a time; N = 128: [4 warps][16 rows][STG_ROW_BYTES], a warp's whole 16 x 128 block in linear rows
   constexpr int EC = 32;
-  constexpr int STG_WARP_BYTES = N == 128 ? 4 * 16 * EC * 4 : 32 * EC * 4;
+  constexpr int STG_WARP_BYTES = N == 128 ? 16 * STG_ROW_BYTES : 32 * EC * 4;
   unsigned char* epi_stage =
       reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(ep_add + N) + 127) & ~(uintptr_t)127);
   int* own_s = reinterpret_cast<int*>(epi_stage + 4 * STG_WARP_BYTES);  // [4 warps][32] vertex id of each epilogue row
   float* head_w_s = reinterpret_cast<float*>(own_s + 4 * 32);        // [64][12] (N == 64 with a fused head)
+  uint64_t* b_res = reinterpret_cast<uint64_t*>(head_w_s);  // [4] (N = 128: no head) per MMA warp: its tile's identity-
+                                                            // residual rows have landed in its staging block
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
@@ -451,6 +474,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       mbar_init(smem_u32(b_m_full + s), 1);
       mbar_init(smem_u32(b_m_empty + s), 1);
     }
+    if (N == 128)
+      for (int w = 0; w < 4; ++w) mbar_init(smem_u32(b_res + w), 1);  // the warp's expect_tx arrival + its copies' bytes
     *abort_flag = (smem_u32(ring) & 1023u) ? 1 : 0;
     if (*abort_flag) mbar_timeout(abort_flag, p.status, 100);
     fence_barrier_init();
@@ -597,9 +622,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     // of an m64n128 fragment would: the 128-column instruction itself needs more than the 80 registers ptxas allocates
     // the kernel with).  Warp wq of the warpgroup holds rows 16 wq .. 16 wq + 15 of each row half (its ER "epilogue
     // rows": local row lr <-> tile row 64 (lr / 16) + 16 wq + lr % 16).
-    // A thread's fragment covers two columns of every 8-column group, so storing it directly would scatter; the rows are
-    // transposed through a small per-warp staging buffer so that a warp-wide 16-byte access covers whole 128-byte row
-    // pieces, and the fused epilogue (affine, ReLU, residual) runs in that layout, where the residual reads coalesce.
+    // A thread's fragment covers two columns of every 8-column group, so storing it directly would scatter.  N = 64: the
+    // rows are transposed through a small per-warp staging buffer so that a warp-wide 16-byte access covers whole
+    // 128-byte row pieces, and the fused epilogue (affine, ReLU, residual) runs in that layout, where the residual reads
+    // coalesce.  N = 128: the epilogue writes its results in place into the warp's linear staging rows, which then
+    // leave whole by bulk copy.
     const int wq = warp - W_EPI0;
     constexpr int CPR = EC / 4;             // 16-byte chunks per staged row
     constexpr int RPI = 32 / CPR;           // rows covered by one warp-wide 16-byte access
@@ -635,7 +662,25 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       int own_v[NP];
 #pragma unroll
       for (int i = 0; i < NP; ++i) own_v[i] = own_w[i * RPI + prow];
-      if (p.ep.res != nullptr) {
+      if (N == 128) {
+        // The staging block is this tile's again once the previous tile's output stores have read it.  An identity
+        // residual then lands in it by bulk copy (one 512-byte row per valid row, straight into the row's slot) while
+        // the main loop runs; the epilogue adds it in place.
+        if (lane < ER) bulk_wait_read0();
+        __syncwarp();
+        if (p.ep.res != nullptr && p.res_identity) {
+          const uint32_t rbar = smem_u32(b_res + wq);
+          const int n_valid = __popc(__ballot_sync(0xFFFFFFFFu, lane < ER && own_w[lane] >= 0));
+          if (lane == 0) mbar_arrive_expect_tx(rbar, (uint32_t)n_valid * (N * 4));
+          __syncwarp();
+          if (lane < ER && own_w[lane] >= 0) {
+            const long long r = mesh0 + own_w[lane];
+            bulk_g2s(stg + lane * STG_ROW_BYTES, p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + ecol0, N * 4,
+                     rbar);
+          }
+        }
+      }
+      if (p.ep.res != nullptr && (N == 64 || !p.res_identity)) {
         // pull this tile's residual rows into L2 while its main loop is still running
         const int lpr = ((p.apack != nullptr ? N : p.ep.res_F) * 4 + 127) >> 7;
         for (int j = lane; j < ER * lpr; j += 32) {
@@ -680,10 +725,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         if (lane == 0) mbar_arrive(smem_u32(b_ab_empty + s));  // this warp is done reading the slot
       }
       if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 2);
-      // phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by row;
-      // N = 128: each sub-slab into its own 16-row block)
+      // N = 64, phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by
+      // row)
       auto stage_slab = [&](int cb) {
-        const uint32_t sb = stg + (N == 128 ? (uint32_t)(cb / 32) * (16 * EC * 4) : 0u);
 #pragma unroll
         for (int h = 0; h < H; ++h)
 #pragma unroll
@@ -692,10 +736,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
             for (int r = 0; r < 2; ++r) {
               const int lr = 16 * h + (lane >> 2) + 8 * r;
               const int cc = 8 * jj + 2 * (lane & 3);
-              const int ah = TM == 128 ? h : cb / 64;                 // row half / column half of the accumulator
-              const int j = 4 * ((TM == 128 ? cb : cb % 64) / 8 + jj) + 2 * r;
-              sts_f2(sb + lr * (EC * 4) + ((((uint32_t)(cc >> 2)) ^ (uint32_t)(lr & 7)) << 4) + (cc & 3) * 4,
-                     acc[ah][j], acc[ah][j + 1]);
+              const int j = 4 * (cb / 8 + jj) + 2 * r;
+              sts_f2(stg + lr * (EC * 4) + ((((uint32_t)(cc >> 2)) ^ (uint32_t)(lr & 7)) << 4) + (cc & 3) * 4,
+                     acc[h][j], acc[h][j + 1]);
             }
         __syncwarp();
       };
@@ -734,64 +777,68 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           zr[2] = make_float4(z[8], z[9], z[10], z[11]);
         }
       } else if (N == 128) {
-        // The whole 16 x 128 block of the warp is staged first: the accumulator is dead after that, and its registers
-        // hold every identity-residual load of the block, issued at once, so the tile pays one L2 round trip for its
-        // residual instead of one per 32-column sub-slab
-#pragma unroll
-        for (int cb = 0; cb < N; cb += 32) stage_slab(cb);
+        // In the accumulator's own layout, in place: o = act(acc * mul + add), plus the identity residual the copy
+        // engine staged during the main loop, goes to the element's slot of its linear staging row
         const bool res_id = p.ep.res != nullptr && p.res_identity;
-        float4 rv[N / 32][NP];
+        if (res_id) mbar_wait(smem_u32(b_res + wq), (uint32_t)it & 1u, abort_flag, p.status, 12);
+        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 21);
 #pragma unroll
-        for (int cb = 0; cb < N; cb += 32)
+        for (int h = 0; h < 2; ++h)
 #pragma unroll
-          for (int i = 0; i < NP; ++i) {
-            rv[cb / 32][i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (res_id && own_v[i] >= 0) {
-              const long long r = mesh0 + own_v[i];
-              rv[cb / 32][i] = __ldg(reinterpret_cast<const float4*>(
-                  p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + ecol0 + cb + colk[i & 1]));
+          for (int jg = 0; jg < 8; ++jg) {
+            const int n = 64 * h + 8 * jg + 2 * (lane & 3);  // column pair of acc[h][4 jg + 2 r + {0, 1}]
+            const float2 mu = *reinterpret_cast<const float2*>(ep_mul + n);
+            const float2 ad = *reinterpret_cast<const float2*>(ep_add + n);
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+              const int j = 4 * jg + 2 * r;
+              const uint32_t a = stg + ((lane >> 2) + 8 * r) * STG_ROW_BYTES + n * 4;
+              float o0 = fmaf(acc[h][j], mu.x, ad.x), o1 = fmaf(acc[h][j + 1], mu.y, ad.y);
+              if (p.ep.relu) {
+                o0 = fmaxf(o0, 0.f);
+                o1 = fmaxf(o1, 0.f);
+              }
+              if (res_id) {
+                const float2 rv = lds_f2(a);
+                o0 += rv.x;
+                o1 += rv.y;
+              }
+              sts_f2(a, o0, o1);
             }
           }
-#pragma unroll
-        for (int cb = 0; cb < N; cb += 32) {
-          const uint32_t sb = stg + (uint32_t)(cb / 32) * (16 * EC * 4);
-          float4 mu_k[2], ad_k[2];
-#pragma unroll
-          for (int k = 0; k < 2; ++k) {
-            mu_k[k] = *reinterpret_cast<const float4*>(ep_mul + cb + colk[k]);
-            ad_k[k] = *reinterpret_cast<const float4*>(ep_add + cb + colk[k]);
-          }
-#pragma unroll
-          for (int i = 0; i < NP; ++i) {
-            const int rr = i * RPI + prow;
-            const int gn = ecol0 + cb + colk[i & 1];  // column of the layer's output
-            const float4 a = lds_f4(sb + rr * (EC * 4) + (pc << 4));
-            const int vtx = own_v[i];
+        if (p.ep.res != nullptr && !p.res_identity) {
+          // channel-resampled residual (its rows are wider than a staging row: no prefetch): one row-major pass over
+          // the staged rows, 4 columns per lane
+          __syncwarp();
+          const int gn = ecol0 + 4 * lane;  // column of the layer's output
+          for (int rr = 0; rr < ER; ++rr) {
+            const int vtx = own_w[rr];
             if (vtx >= 0) {
-              const float4 mu = mu_k[i & 1], ad = ad_k[i & 1];
-              float o[4] = {fmaf(a.x, mu.x, ad.x), fmaf(a.y, mu.y, ad.y), fmaf(a.z, mu.z, ad.z), fmaf(a.w, mu.w, ad.w)};
-              if (p.ep.relu) {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) o[e] = fmaxf(o[e], 0.f);
-              }
               const long long r = mesh0 + vtx;
-              if (p.ep.res != nullptr) {
-                if (p.res_identity) {
-                  o[0] += rv[cb / 32][i].x; o[1] += rv[cb / 32][i].y; o[2] += rv[cb / 32][i].z; o[3] += rv[cb / 32][i].w;
-                } else {
-                  const float* res_row = p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F;
+              const float* res_row = p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F;
+              const uint32_t a = stg + rr * STG_ROW_BYTES + lane * 16;
+              const float4 v = lds_f4(a);
+              float o[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float l = __ldg(p.ep.lam + gn + e);
-                    o[e] += (1.f - l) * __ldg(res_row + __ldg(p.ep.i0 + gn + e)) + l * __ldg(res_row + __ldg(p.ep.i1 + gn + e));
-                  }
-                }
+              for (int e = 0; e < 4; ++e) {
+                const float l = __ldg(p.ep.lam + gn + e);
+                o[e] += (1.f - l) * __ldg(res_row + __ldg(p.ep.i0 + gn + e)) + l * __ldg(res_row + __ldg(p.ep.i1 + gn + e));
               }
-              *reinterpret_cast<float4*>(p.y + r * p.ldy + p.y_col0 + gn) = make_float4(o[0], o[1], o[2], o[3]);
+              sts_f4(a, make_float4(o[0], o[1], o[2], o[3]));
             }
           }
         }
-        __syncwarp();  // the staging block is read before the next tile overwrites it
+        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 22);
+        // Out by bulk copy, one 512-byte row per valid row; the warpgroup does not wait for it (the next tile's
+        // residual copies and staging writes wait for the reads of these, at its start)
+        fence_async_proxy();  // this thread's staging writes -> the async proxy the copies read through
+        __syncwarp();
+        if (lane < ER) {
+          if (own_w[lane] >= 0)
+            bulk_s2g(p.y + (mesh0 + own_w[lane]) * p.ldy + p.y_col0 + ecol0, stg + lane * STG_ROW_BYTES, N * 4);
+          bulk_commit();
+        }
+        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 23);
       } else {
 #pragma unroll
         for (int cb = 0; cb < N; cb += 32) {
@@ -839,6 +886,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         }
       }
     }
+    if (N == 128 && lane < ER) bulk_wait0();  // the last tile's output stores read shared memory until they complete
   } else {
     if (p.apack == nullptr) {
     // ------------------------------------------------------------ producers (16 warps)
@@ -1517,8 +1565,9 @@ __global__ void __launch_bounds__(256) k_pack_weights(const float* __restrict__ 
 // debug: P2M_UMMA_TMA=0 stages every row with cp.async (A/B measurements of the TMA own-row loads)
 const bool g_umma_tma = [] { const char* e = std::getenv("P2M_UMMA_TMA"); return !(e && e[0] == '0'); }();
 
-// per-warp transpose staging: one 32 x 32 sub-slab per warp (N = 64), a warp's whole 16 x 128 block (N = 128)
-inline int epi_stage_bytes(int N) { return N == 128 ? 4 * 16 * 128 * 4 : 4 * 32 * 32 * 4; }
+// per-warp epilogue staging: one 32 x 32 sub-slab per warp (N = 64), a warp's whole 16 x 128 block in 16 padded linear
+// rows (N = 128)
+inline int epi_stage_bytes(int N) { return N == 128 ? 4 * 16 * STG_ROW_BYTES : 4 * 32 * 32 * 4; }
 // Dynamic shared memory of a conv configuration: T1 given (MODE 1: the tile's own X rows and the T1 rows of the tile
 // and its 1-hop halo per stage) or plain (MODE 0: the own X rows per stage).  N = 128: the 64-row configuration (64-row
 // tiles; with a given T1 and NS >= 3 no X stage: the producers read X directly).
@@ -1526,7 +1575,7 @@ size_t smem_bytes_dims(int N, int NS, int XS, int max_h1, int meta_stride, bool 
   const int tm = N == 128 ? 64 : TILE_M;
   const size_t fixed = 1024 + (size_t)NS * (tm * 128 + N * 128) + 8 * (2 * NS + 2 * XS + 8) + 16 +
                        2 * (size_t)N * 4 + 16 + 128 + (size_t)epi_stage_bytes(N) + 4 * 32 * 4 +
-                       (N == 64 ? 64 * 12 * 4 : 0);
+                       (N == 64 ? 64 * 12 * 4 : 4 * 8);  // fused-head weights (N = 64) / residual mbarriers (N = 128)
   const size_t xs_rows = (t1_given && N == 128 && NS >= 3) ? 0 : (size_t)tm;
   return fixed + (size_t)XS * (xs_rows + (t1_given ? max_h1 : 0)) * FC * 4 + 2 * (size_t)meta_stride;
 }
@@ -1640,6 +1689,16 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.trace = a.trace;
   p.head_wt = a.fout == 64 ? a.head_wt : nullptr;
   p.head_z = a.fout == 64 ? a.head_z : nullptr;
+  if (N == WIDE_N) {
+    // the epilogue moves whole 512-byte output rows (and identity-residual rows) by cp.async.bulk, which needs 16-byte
+    // aligned addresses (a CTA's first column, 128 blockIdx.y, keeps that)
+    const bool y_ok = (reinterpret_cast<uintptr_t>(p.y) & 15u) == 0 && (p.ldy * 4) % 16 == 0 && (p.y_col0 * 4) % 16 == 0;
+    const bool res_ok = !p.res_identity || ((reinterpret_cast<uintptr_t>(p.ep.res) & 15u) == 0 && (p.ep.res_F * 4) % 16 == 0);
+    if (!y_ok || !res_ok) {
+      set_error("umma_conv: the 128-column epilogue needs 16-byte aligned output and identity-residual rows");
+      return P2M_ERR_INVALID;
+    }
+  }
   p.tma = 0;
   std::memset(&p.tm_x, 0, sizeof(p.tm_x));
   std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));

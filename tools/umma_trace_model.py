@@ -45,7 +45,10 @@ if not ev_all:
 ev_all.sort()
 t0 = ev_all[0][0]
 pn = {1: "wait_x", 2: "x_ready", 6: "T2 gathered", 7: "blocks emitted", 8: "end barrier"}
-mn = {1: "tile start", 2: "main loop done", 4: "wait full slot", 5: "slot full -> 12 MMAs"}
+mn = {1: "tile start", 2: "main loop done", 4: "wait full slot", 5: "slot full -> 12 MMAs",
+      # sub-phases of the 64 x 128 (N = 128) epilogue, MMA warp 0
+      20: "epi: accumulator staged", 21: "epi: residual in hand", 22: "epi: outputs computed",
+      23: "epi: output stores issued"}
 for c, role, ev in ev_all[:n_ev]:
     if role == 0:
         label = pn.get(ev, str(ev))
@@ -85,3 +88,27 @@ rows = [
 print(f"\nlogged window: {window} cycles (CTA 0; each role's log holds at most 512 events)")
 for role, what, cyc in rows:
     print(f"{role:9s} {what:40s} {cyc:10d} cycles  {100.0 * cyc / window:5.1f} %")
+
+# Per-tile split of the MMA warpgroup's time over the tiles whose main loop and epilogue are both in the log: main loop
+# (tile start -> main loop done), then every epilogue step (named after the event that ends it), up to the next tile
+# start.
+steps, tiles, cur, last = {}, 0, None, None
+for c, _, ev in per_role[3]:
+    if ev in (4, 5):
+        continue
+    if ev == 1:
+        if cur is not None and last is not None:
+            cur["next tile start"] = c - last[0]
+            for k, v in cur.items():
+                steps[k] = steps.get(k, 0) + v
+            tiles += 1
+        cur, last = {}, (c, ev)
+    elif cur is not None:
+        cur["main loop" if ev == 2 else mn.get(ev, str(ev))] = c - last[0]
+        last = (c, ev)
+if tiles:
+    print(f"\nper tile, MMA warp 0, mean over {tiles} tiles (cycles)")
+    for k, v in steps.items():
+        print(f"  {k:32s} {v / tiles:9.0f}")
+    epi = sum(v for k, v in steps.items() if k != "main loop")
+    print(f"  {'epilogue total (to next start)':32s} {epi / tiles:9.0f}")
