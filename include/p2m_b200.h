@@ -347,6 +347,28 @@ int p2m_align_w_scale(const float* gt, const float* pred, int batch, int n_point
 int p2m_pck_accumulate(const double* err, const float* pred, const float* gt, int64_t n_val, const double* thresholds,
                        int n_thr, double* err_out, int64_t* hist, p2m_stream_t stream);
 
+/* ---- demo mesh overlay (SURVEY.md §8 row f10; demo/renderer.py:28-35,66-114 Renderer.render, demo/run.py:46-67) ---
+ * Draws person p's mesh verts [n_person, n_vertex, 3] (faces [n_face, 3] int32) over image image_index[p] (int32
+ * [n_person], NULL = all on image 0) of images_in [n_image, height, width, 3] (uint8) into images_out (same shape; may
+ * equal images_in), people in order, the later person winning where two overlap.  cams [n_person, 4] is orig_cam
+ * (sx, sy, tx, ty) of convert_crop_cam_to_orig_img; with the reference's Rx(180°) flip and weak-perspective matrix a
+ * vertex (x, y, z) lands at column u = W/2 (1 + sx (x + tx)), row v = H/2 (1 + sy (y + ty)), depth z; fragments with z
+ * outside [-1, 1] are clipped, nearer z wins and a depth tie goes to the lower face.  Coverage, depth, back-face culling,
+ * clipping and compositing order follow the reference; coverage is exact (positions snapped to 1/256 px, int64 edge
+ * functions, top-left fill rule).  The shading is this library's own, not pyrender's: flat Lambert of ambient 0.3 plus
+ * 2.4 along the camera axis, c_k = clamp(colors[p, k] (0.3 + (2.4/pi) max(0, -n_z)), 0, 1) for the face normal n in
+ * mesh coordinates, stored as floor(255 c + 0.5) into channel k.  Skipped: a triangle with a non-finite vertex or
+ * camera value, a face index outside [0, n_vertex) or a vertex beyond +-2^20 px; a person whose image_index is outside
+ * [0, n_image).  Optional outputs [n_image, height, width] (NULL = not written): face_map and person_map (int32, -1
+ * where uncovered), depth_map (float32, NaN).  Limits: n_person, n_face <= 65535; height, width <= 16384.  Device
+ * memory of one device; workspace >= p2m_render_workspace_bytes (8-byte aligned).  A memset and two launches on
+ * `stream`, no host synchronisation, bitwise deterministic.                                                        */
+size_t p2m_render_workspace_bytes(int n_image, int height, int width);
+int p2m_render_meshes(const float* verts, int n_person, int n_vertex, const int32_t* faces, int n_face,
+                      const float* cams, const float* colors, const int32_t* image_index, const uint8_t* images_in,
+                      int n_image, int height, int width, uint8_t* images_out, int32_t* face_map, int32_t* person_map,
+                      float* depth_map, void* workspace, size_t workspace_bytes, p2m_stream_t stream);
+
 /* ---- body model: batched SMPL / MANO forward (SURVEY.md §8 row f6; smplpytorch SMPL_Layer.forward,
  * manopth ManoLayer.forward) --------------------------------------------------------------------------------------
  * The descriptor holds HOST arrays in the reference's buffer layouts (all float32, row-major):

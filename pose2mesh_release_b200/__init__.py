@@ -11,6 +11,7 @@ Public surface (mirrors the reference's modules for this path, SURVEY.md §8b):
     camera.fit_cameras                                <- demo/run.py optimize_cam_param (batched camera fit)
     temporal.smooth_pose / temporal.evaluate_video    <- lib/smooth_utils.py, compute_error_accel, the 3DPW video block
     freihand.FreiHANDEvaluator / freihand.f_scores    <- the FreiHAND evaluation script (F-scores, align_w_scale, PCK)
+    render.render_meshes                              <- demo/renderer.py Renderer.render (batched mesh overlay)
 
 All device work is in libp2m_b200.so (csrc/, C ABI in include/p2m_b200.h); there is no CPU fallback.
 """
@@ -23,5 +24,7 @@ from .camera import convert_crop_cam_to_orig_img, fit_cameras  # noqa: F401
 from .temporal import accel_errors, compute_error_accel, evaluate_video, smooth_pose, smooth_sequences  # noqa: F401
 from .freihand import (FreiHANDEvaluator, align_w_scale, f_scores, mano_eval_regressor,  # noqa: F401
                        nearest_distances)
+from . import render  # noqa: F401
+from .render import render_meshes  # noqa: F401
 
 __version__ = "0.1.0"

@@ -121,6 +121,7 @@ EXPORTS = [
     "p2m_rigid_align", "p2m_point_errors", "p2m_fit_camera", "p2m_crop_cam_to_orig",
     "p2m_one_euro_smooth", "p2m_accel_error", "p2m_segment_mean",
     "p2m_nearest_distances", "p2m_align_w_scale", "p2m_pck_accumulate",
+    "p2m_render_workspace_bytes", "p2m_render_meshes",
     "p2m_body_model_create", "p2m_body_model_destroy", "p2m_body_model_workspace_bytes", "p2m_body_model_forward",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
 ]
@@ -230,6 +231,11 @@ def load() -> C.CDLL:
         lib.p2m_align_w_scale.restype = C.c_int
         lib.p2m_pck_accumulate.argtypes = [vp, vp, vp, i64, c_double_p, C.c_int, vp, vp, vp]
         lib.p2m_pck_accumulate.restype = C.c_int
+        lib.p2m_render_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        lib.p2m_render_workspace_bytes.restype = sz
+        lib.p2m_render_meshes.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int,
+                                          vp, vp, vp, vp, vp, sz, vp]
+        lib.p2m_render_meshes.restype = C.c_int
         lib.p2m_body_model_create.argtypes = [C.POINTER(BodyModelDesc), C.POINTER(vp)]
         lib.p2m_body_model_create.restype = C.c_int
         lib.p2m_body_model_destroy.argtypes = [vp]
