@@ -355,7 +355,7 @@ struct KParams {
   const float* head_wt;  // optional fused thin head (N == 64): epilogue writes head_z[row][12] = y_row * head_wt[64][12]
   float* head_z;
   // Dense GEMM mode (launch_umma_gemm: PoseNet's Linear layers): the A operand is PRE-PACKED like a weight image
-  // (k_pack_plain on the activation matrix: one 16 KB block per (128-row tile, 32-feature chunk)), so both operands of
+  // (k_pack on the activation matrix: one 16 KB block per (128-row tile, 32-feature chunk)), so both operands of
   // every K-block arrive by cp.async.bulk and no producer warp runs; blockIdx.y selects an N-wide slice of the output
   // columns (its weight image, epilogue vectors and output / residual columns).
   const unsigned char* apack;
@@ -1538,28 +1538,46 @@ __global__ void __launch_bounds__(512, 2) k_cheb_t1(const T1Params p) {
   }
 }
 
-// fp32 reference-layout weights [Fout, Fin*3] (column = f*3+k) -> K-blocks of fp16 [Whi | Wlo]
-// in the exact shared-memory image (128B-swizzled), block u = chunk*3 + k, so the kernel can
-// fetch a block with a single cp.async.bulk.
-__global__ void __launch_bounds__(256) k_pack_weights(const float* __restrict__ W, int fin, int fout,
-                                                      unsigned char* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
-  const int n_blocks = (fin / FC) * 3;
-  const int total = n_blocks * fout * 8;
+// What k_pack turns into an operand image: K-blocks of `rows` rows x 32 k as fp16 [hi 32 | lo 32] per 128-byte row, in
+// the exact shared-memory image (128B-swizzled), so a kernel fetches a block with a single cp.async.bulk.  Block
+// b = (t * n_chunk + chunk) * orders + order holds rows n = t * rows + [0, rows) and k = 32 chunk + [0, 32):
+// p[n ld_row + k ld_k + order] * scale, zero for n >= n_real; `combined`: the isolated rows' combined weights
+// (p[a] + c p[a + 1] + (2c^2 - 1) p[a + 2]) * scale at a = n ld_row + k ld_k.
+struct PackSrc {
+  const float* p;
+  long long ld_row, ld_k;
+  int rows, n_chunk, orders, n_real;
+  float scale;  // W_SCALE for weights, 1 for activations
+  int combined;
+  float c;
+};
+__global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, unsigned char* __restrict__ out) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
   if (idx >= total) return;
-  const int j = idx & 7;
-  const int n = (idx >> 3) % fout;
-  const int u = (idx >> 3) / fout;
-  const int c = u / 3, k = u % 3;
-  const int f0 = c * FC + (j & 3) * 8;
+  const int j = (int)(idx & 7);
+  const int row = (int)((idx >> 3) % s.rows);
+  const long long blk = (idx >> 3) / s.rows;
+  const int per_tile = s.n_chunk * s.orders;
+  const long long n = blk / per_tile * s.rows + row;
+  const int u = (int)(blk % per_tile);
+  const float* src = s.p + n * s.ld_row + (long long)((u / s.orders) * FC + (j & 3) * 8) * s.ld_k + u % s.orders;
+  const float c = s.c, c2 = 2.f * c * c - 1.f;
   __align__(16) __half h[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    const float w = W[(size_t)n * fin * 3 + (size_t)(f0 + e) * 3 + k] * W_SCALE;
+    const float* wr = src + e * s.ld_k;
+    float w = 0.f;
+    if (n < s.n_real) w = s.combined ? (wr[0] + c * wr[1] + c2 * wr[2]) * s.scale : wr[0] * s.scale;
     const __half hi = __float2half_rn(w);
     h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
   }
-  *reinterpret_cast<uint4*>(out + (size_t)u * fout * 128 + sw128_off(n, j)) = *reinterpret_cast<const uint4*>(h);
+  *reinterpret_cast<uint4*>(out + blk * s.rows * 128 + sw128_off(row, j)) = *reinterpret_cast<const uint4*>(h);
+}
+int launch_pack(const PackSrc& src, long long n_blocks, void* out, cudaStream_t s) {
+  const long long total = n_blocks * src.rows * 8;
+  k_pack<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(src, total, static_cast<unsigned char*>(out));
+  P2M_LAUNCH_OK();
+  return P2M_OK;
 }
 
 // debug: P2M_UMMA_TMA=0 stages every row with cp.async (A/B measurements of the TMA own-row loads)
@@ -1570,17 +1588,14 @@ const bool g_umma_tma = [] { const char* e = std::getenv("P2M_UMMA_TMA"); return
 inline int epi_stage_bytes(int N) { return N == 128 ? 4 * 16 * STG_ROW_BYTES : 4 * 32 * 32 * 4; }
 // Dynamic shared memory of a conv configuration: T1 given (MODE 1: the tile's own X rows and the T1 rows of the tile
 // and its 1-hop halo per stage) or plain (MODE 0: the own X rows per stage).  N = 128: the 64-row configuration (64-row
-// tiles; with a given T1 and NS >= 3 no X stage: the producers read X directly).
-size_t smem_bytes_dims(int N, int NS, int XS, int max_h1, int meta_stride, bool t1_given) {
+// tiles; with a given T1 and NS >= 3 no X stage: the producers read X directly).  The dense GEMM has no tile metadata.
+size_t smem_bytes_for(int N, int NS, int XS, const TileBlobs& t, bool t1_given) {
   const int tm = N == 128 ? 64 : TILE_M;
   const size_t fixed = 1024 + (size_t)NS * (tm * 128 + N * 128) + 8 * (2 * NS + 2 * XS + 8) + 16 +
                        2 * (size_t)N * 4 + 16 + 128 + (size_t)epi_stage_bytes(N) + 4 * 32 * 4 +
                        (N == 64 ? 64 * 12 * 4 : 4 * 8);  // fused-head weights (N = 64) / residual mbarriers (N = 128)
   const size_t xs_rows = (t1_given && N == 128 && NS >= 3) ? 0 : (size_t)tm;
-  return fixed + (size_t)XS * (xs_rows + (t1_given ? max_h1 : 0)) * FC * 4 + 2 * (size_t)meta_stride;
-}
-size_t smem_bytes_for(int N, int NS, int XS, const TileBlobs& t, bool t1_given) {
-  return smem_bytes_dims(N, NS, XS, t.max_h1, t.stride, t1_given);
+  return fixed + (size_t)XS * (xs_rows + (t1_given ? t.max_h1 : 0)) * FC * 4 + 2 * (size_t)t.stride;
 }
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 constexpr int CONV_N = 64;  // output columns per CTA of the 128-row conv configuration (one column slice)
@@ -1863,17 +1878,12 @@ int build_blobs(const std::vector<int>& rows, int tm, const int* rowptr, const i
   ts->max_h1 = max_h1;
   return P2M_OK;
 }
+}  // namespace
 
 int build_tileset(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
                   TileSet* ts, std::vector<void*>* owned) {
   P2M_TRY(build_blobs(rows, TILE_M, rowptr, colidx, val, V, ts, owned));
   return build_blobs(rows, 64, rowptr, colidx, val, V, &ts->m64, owned);
-}
-}  // namespace
-
-int build_index_tiles(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
-                      TileSet* ts, std::vector<void*>* owned) {
-  return build_tileset(rows, rowptr, colidx, val, V, ts, owned);
 }
 
 int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val, int V, DevLevel* out,
@@ -2033,155 +2043,9 @@ int umma_conv_x_stages(const DevLevel& g, int fout, bool plain) {
 }
 bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && g_umma_tma && tmap_encoder() != nullptr; }
 
-__global__ void __launch_bounds__(256) k_pack_plain(const float* __restrict__ Bmat, long long ld_n, long long ld_k, int N,
-                                                    int K, unsigned char* __restrict__ out, float W_SCALE = 64.f) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
-  const int total = (K / FC) * N * 8;
-  if (idx >= total) return;
-  const int j = idx & 7;
-  const int n = (idx >> 3) % N;
-  const int c = (idx >> 3) / N;
-  const int k0 = c * FC + (j & 3) * 8;
-  __align__(16) __half h[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float w = Bmat[(long long)n * ld_n + (long long)(k0 + e) * ld_k] * W_SCALE;
-    const __half hi = __float2half_rn(w);
-    h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
-  }
-  *reinterpret_cast<uint4*>(out + (size_t)c * N * 128 + sw128_off(n, j)) = *reinterpret_cast<const uint4*>(h);
-}
-
-// the same image for the combined weights of the isolated rows, straight from the reference layout
-__global__ void __launch_bounds__(256) k_pack_iso(const float* __restrict__ W, float c, int fin, int fout,
-                                                  unsigned char* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
-  const int total = (fin / FC) * fout * 8;
-  if (idx >= total) return;
-  const int j = idx & 7;
-  const int n = (idx >> 3) % fout;
-  const int cc = (idx >> 3) / fout;
-  const int f0 = cc * FC + (j & 3) * 8;
-  const float c2 = 2.f * c * c - 1.f;
-  __align__(16) __half h[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float* wr = W + (size_t)n * fin * 3 + (size_t)(f0 + e) * 3;
-    const float w = (wr[0] + c * wr[1] + c2 * wr[2]) * W_SCALE;
-    const __half hi = __float2half_rn(w);
-    h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
-  }
-  *reinterpret_cast<uint4*>(out + (size_t)cc * fout * 128 + sw128_off(n, j)) = *reinterpret_cast<const uint4*>(h);
-}
-int launch_umma_pack_iso(const float* W, float c, int fin, int fout, void* wpack, cudaStream_t s) {
-  const int total = (fin / FC) * fout * 8;
-  k_pack_iso<<<(total + 255) / 256, 256, 0, s>>>(W, c, fin, fout, static_cast<unsigned char*>(wpack));
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-
-// Backward-data as a forward conv (p2m_api.cu): dX = [dz | L~dz | (2L~^2 - I)dz] * W'^T with W'[f][o*3 + k] = W[o][f*3 + k]
-// (L~ symmetric).  Same K-block image as k_pack_weights for a layer with Fin' = fout, Fout' = fin.
-__global__ void __launch_bounds__(256) k_pack_weights_t(const float* __restrict__ W, int fin, int fout,
-                                                        unsigned char* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
-  const int n_blocks = (fout / FC) * 3;
-  const int total = n_blocks * fin * 8;
-  if (idx >= total) return;
-  const int j = idx & 7;
-  const int n = (idx >> 3) % fin;   // output channel of the backward conv = input feature f
-  const int u = (idx >> 3) / fin;
-  const int c = u / 3, k = u % 3;
-  const int o0 = c * FC + (j & 3) * 8;
-  __align__(16) __half h[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float w = W[(size_t)(o0 + e) * fin * 3 + (size_t)n * 3 + k] * W_SCALE;
-    const __half hi = __float2half_rn(w);
-    h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
-  }
-  *reinterpret_cast<uint4*>(out + (size_t)u * fin * 128 + sw128_off(n, j)) = *reinterpret_cast<const uint4*>(h);
-}
-int launch_umma_pack_weights_t(const float* W, int fin, int fout, void* wpack, cudaStream_t s) {
-  const int total = (fout / FC) * 3 * fin * 8;
-  k_pack_weights_t<<<(total + 255) / 256, 256, 0, s>>>(W, fin, fout, static_cast<unsigned char*>(wpack));
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-// ... and the combined weights of the isolated rows, transposed: B[n = f][o] = W[o][3f] + c W[o][3f+1] + (2c^2-1) W[o][3f+2]
-__global__ void __launch_bounds__(256) k_pack_iso_t(const float* __restrict__ W, float c, int fin, int fout,
-                                                    unsigned char* __restrict__ out) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  const int total = (fout / FC) * fin * 8;
-  if (idx >= total) return;
-  const int j = idx & 7;
-  const int n = (idx >> 3) % fin;
-  const int cc = (idx >> 3) / fin;
-  const int o0 = cc * FC + (j & 3) * 8;
-  const float c2 = 2.f * c * c - 1.f;
-  __align__(16) __half h[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float* wr = W + (size_t)(o0 + e) * fin * 3 + (size_t)n * 3;
-    const float w = (wr[0] + c * wr[1] + c2 * wr[2]) * W_SCALE;
-    const __half hi = __float2half_rn(w);
-    h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
-  }
-  *reinterpret_cast<uint4*>(out + (size_t)cc * fin * 128 + sw128_off(n, j)) = *reinterpret_cast<const uint4*>(h);
-}
-int launch_umma_pack_iso_t(const float* W, float c, int fin, int fout, void* wpack, cudaStream_t s) {
-  const int total = (fout / FC) * fin * 8;
-  k_pack_iso_t<<<(total + 255) / 256, 256, 0, s>>>(W, c, fin, fout, static_cast<unsigned char*>(wpack));
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-
 size_t umma_plain_pack_bytes(int N, int K) { return (size_t)(K / FC) * N * 128; }
 
 // ---------------------------------------------------------------- dense GEMM on the conv kernel's plain mode
-// A operand image of a row-major activation matrix X [M, K] (K % 32 == 0): per (128-row tile, 32-column chunk) one
-// 16 KB block [128 rows][hi 32 | lo 32] fp16, 128B-swizzled, rows >= M zero — what the producers would have built.
-__global__ void __launch_bounds__(256) k_pack_rows(const float* __restrict__ X, int M, int K, unsigned char* __restrict__ out) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
-  const int n_chunk = K / FC;
-  const long long total = (long long)((M + TILE_M - 1) / TILE_M) * n_chunk * TILE_M * 8;
-  if (idx >= total) return;
-  const int j = (int)(idx & 7);
-  const int row = (int)((idx >> 3) % TILE_M);
-  const long long blk = (idx >> 3) / TILE_M;  // tile * n_chunk + c
-  const int c = (int)(blk % n_chunk);
-  const long long r = (blk / n_chunk) * TILE_M + row;
-  __align__(16) __half h[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float v = (r < M) ? X[r * K + c * FC + (j & 3) * 8 + e] : 0.f;
-    const __half hi = __float2half_rn(v);
-    h[e] = (j < 4) ? hi : __float2half_rn(v - __half2float(hi));
-  }
-  *reinterpret_cast<uint4*>(out + (size_t)blk * A_BLOCK_BYTES + sw128_off(row, j)) = *reinterpret_cast<const uint4*>(h);
-}
-// Weight images of ALL output-column slices in one launch: slice j (rows [j ns, (j+1) ns) of W [n_real, K], rows >=
-// n_real zero) -> K/32 blocks of ns rows x 128 bytes [Whi | Wlo] (scaled by 2^6 like every weight image).
-__global__ void __launch_bounds__(256) k_pack_w_sliced(const float* __restrict__ W, int n_real, int N, int K, int ns,
-                                                       unsigned char* __restrict__ out) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
-  const int n_chunk = K / FC;
-  const long long total = (long long)N * n_chunk * 8;
-  if (idx >= total) return;
-  const int j = (int)(idx & 7);
-  const int nl = (int)((idx >> 3) % ns);
-  const long long blk = (idx >> 3) / ns;  // slice * n_chunk + c
-  const int c = (int)(blk % n_chunk);
-  const int n = (int)(blk / n_chunk) * ns + nl;
-  __align__(16) __half h[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const float w = (n < n_real) ? W[(size_t)n * K + c * FC + (j & 3) * 8 + e] * W_SCALE : 0.f;
-    const __half hi = __float2half_rn(w);
-    h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
-  }
-  *reinterpret_cast<uint4*>(out + (size_t)blk * ns * 128 + sw128_off(nl, j)) = *reinterpret_cast<const uint4*>(h);
-}
 size_t umma_gemm_apack_bytes(int M, int K) { return (size_t)((M + TILE_M - 1) / TILE_M) * (K / FC) * A_BLOCK_BYTES; }
 size_t umma_gemm_wpack_bytes(int N, int K) { return (size_t)(K / FC) * N * 128; }
 bool umma_gemm_supported(int M, int N, int K) { return M > 0 && K >= FC && K % FC == 0 && N >= 64 && N % 64 == 0; }
@@ -2190,7 +2054,7 @@ namespace {
 template <int N>
 int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
   constexpr int NS = 3;
-  const size_t smem = smem_bytes_dims(N, NS, 1, 0, 0, false);
+  const size_t smem = smem_bytes_for(N, NS, 1, TileBlobs(), false);
   auto kern = k_cheb_conv_umma<N, NS, 1, 0>;
   P2M_TRY((check_launch_regs<N, NS, 1, 0>()));
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -2214,18 +2078,12 @@ int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const 
     set_error("umma_gemm: unsupported shape");
     return P2M_ERR_INVALID;
   }
-  {
-    const long long total = (long long)((M + TILE_M - 1) / TILE_M) * (K / FC) * TILE_M * 8;
-    k_pack_rows<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(X, M, K, static_cast<unsigned char*>(apack));
-    P2M_LAUNCH_OK();
-  }
   const int tiles = (M + TILE_M - 1) / TILE_M;
   const int ns = CONV_N;  // one warpgroup's register accumulator: 64 output columns per CTA
-  {
-    const long long total = (long long)N * (K / FC) * 8;
-    k_pack_w_sliced<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(W, n_real, N, K, ns, static_cast<unsigned char*>(wpack));
-    P2M_LAUNCH_OK();
-  }
+  // A: one 16 KB block per (128-row tile, 32-column chunk), rows >= M zero (what the producers would have built);
+  // W: the images of all output-column slices, slice j = rows [j ns, (j + 1) ns) of W, rows >= n_real zero
+  P2M_TRY(launch_pack(PackSrc{X, K, 1, TILE_M, K / FC, 1, M, 1.f, 0, 0.f}, (long long)tiles * (K / FC), apack, s));
+  P2M_TRY(launch_pack(PackSrc{W, K, 1, ns, K / FC, 1, n_real, W_SCALE, 0, 0.f}, (long long)(N / ns) * (K / FC), wpack, s));
   KParams p;
   std::memset(&p, 0, sizeof(p));
   p.V = M;                // one "mesh" of M rows: the epilogue masks rows >= V of the last tile
@@ -2242,20 +2100,16 @@ int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const 
   return launch_gemm_cfg<CONV_N>(p, N / ns, sm_count, s);
 }
 
-int launch_umma_pack_plain(const float* Bmat, long long ld_n, long long ld_k, int N, int K, void* wpack, cudaStream_t s) {
-  const int total = (K / FC) * N * 8;
-  k_pack_plain<<<(total + 255) / 256, 256, 0, s>>>(Bmat, ld_n, ld_k, N, K, static_cast<unsigned char*>(wpack));
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-
 size_t umma_wpack_bytes(int fin, int fout) { return (size_t)(fin / FC) * 3 * fout * 128; }
 
-int launch_umma_pack_weights(const float* W, int fin, int fout, void* wpack, cudaStream_t s) {
-  const int total = (fin / FC) * 3 * fout * 8;
-  k_pack_weights<<<(total + 255) / 256, 256, 0, s>>>(W, fin, fout, static_cast<unsigned char*>(wpack));
-  P2M_LAUNCH_OK();
-  return P2M_OK;
+int launch_umma_pack_weights(const float* W, int fin, int fout, bool transposed, int order, float c, void* wpack,
+                             cudaStream_t s) {
+  const int rows = transposed ? fin : fout, K = transposed ? fout : fin;
+  PackSrc src{W, transposed ? 3 : 3LL * fin, transposed ? 3LL * fin : 3, rows, K / FC, 1, rows, W_SCALE, 0, c};
+  if (order == WPACK_ALL) src.orders = 3;
+  else if (order == WPACK_COMBINED) src.combined = 1;
+  else src.p = W + order;
+  return launch_pack(src, (long long)(K / FC) * src.orders, wpack, s);
 }
 
 int launch_umma_conv(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {

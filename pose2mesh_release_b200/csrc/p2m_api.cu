@@ -236,13 +236,18 @@ WsMap map_workspace(const p2m_model* m, int B, int training, void* base) {
   return w;
 }
 
+// Bytes of the weight-image scratch a backward packs into: the network's (BwdMap::wpack, >= the backward-data image of
+// any supported layer) or the single-layer workspace's (the forward image of the layer itself)
+size_t wpack_capacity(bool network, int fin, int fout) {
+  return network ? umma_wpack_bytes(256, 256) : umma_wpack_bytes(((fin + 31) / 32) * 32, fout);
+}
+
 struct BwdMap {
   float* G[4];
   float* U;
   float* dwp;
   double* sums;
   unsigned char* wpack;   // packed fp16 K-blocks of the backward-data conv (or of one W_k^T for the dT GEMM fallback)
-  size_t wpack_bytes;
   unsigned char* wpack_iso;  // combined transposed weights of the isolated rows (padding-vertex elision)
   float* thin;               // scratch of the thin head's backward
   float* a_scale;         // power-of-two gradient scale (device scalar)
@@ -256,8 +261,7 @@ BwdMap map_scratch(const p2m_model* m, int B, void* base) {
   w.U = b.take<float>(s.max_U);
   w.dwp = b.take<float>(std::max(s.max_w, (size_t)1));
   w.sums = b.take<double>(2 * (size_t)s.max_f + 2 * (size_t)m->fc_out);
-  w.wpack_bytes = umma_wpack_bytes(256, 256);   // backward-data conv image (>= the plain image of one W_k^T)
-  w.wpack = b.take<unsigned char>(w.wpack_bytes);
+  w.wpack = b.take<unsigned char>(wpack_capacity(true, 0, 0));
   w.wpack_iso = b.take<unsigned char>(umma_plain_pack_bytes(256, 256));
   w.thin = b.take<float>(s.max_thin);
   w.a_scale = b.take<float>(4);
@@ -265,65 +269,134 @@ BwdMap map_scratch(const p2m_model* m, int B, void* base) {
   return w;
 }
 
-// ---- one conv layer, linear part + epilogue -------------------------------------------------
-// y = epilogue( [T0|T1|T2](x) * Wp^T )
-bool conv_on_tensor_cores(const p2m_model* m, const Layer& L, const unsigned char* wpack) {
-  return m->precision == P2M_PREC_FP16X3_TC && wpack != nullptr && umma_conv_supported(m->levels[L.level], L.fin, L.fout);
+// ---- which kernels run a Chebyshev conv
+// Padding-vertex elision of a conv with `width` output columns over `rows` rows under p2m_debug_set_elide_padding's
+// `mode`: connected rows through the conv on index-list tiles, isolated rows (DevLevel::n_iso) through a plain GEMM with
+// the combined weights.  Mode 1 (default) takes the levels where they are >= 40 % of the rows (measured break-even),
+// mode 2 every level that has the tile families, mode 0 none.
+bool elided(int mode, const DevLevel& g, long long rows, int width) {
+  return mode > 0 && g.n_iso > 0 && rows >= 2LL * width && (mode >= 2 || 5LL * g.n_iso >= 2LL * g.V);
 }
-int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpool, const float* w_ref, float* T,
-                float* wp, unsigned char* wpack, const Epilogue& ep, float* y, cudaStream_t s,
-                const float* head_wt = nullptr, float* head_z = nullptr, bool keep_wp = true, bool may_elide = false,
-                int iso_mode = 0 /* 0: every isolated row, 1: class representatives only, 2: none */,
-                const float* a_scale = nullptr /* device scalar: the basis is scaled by it before the fp16 split */) {
+
+// The path of every pass of one conv.  Neither tc_dx nor tc_dt (nor thin): dX on SIMT (dT GEMM + basis backward).
+struct ConvRoute {
+  bool tc = false;           // forward: T1 pass + tensor-core conv (else SIMT: thin conv or basis + GEMM) ...
+  bool elide = false;        // ... with the padding-vertex elision
+  bool thin = false;         // backward: dW and dX by the thin head's weights-first backward
+  bool tc_dw = false;        // dW by k_cheb_dw_umma on the basis of x (else SIMT), unless dw_dz_basis
+  bool dw_dz_basis = false;  // dW by k_cheb_dw_umma on the basis of dz (only with tc_dx, which reuses its L~dz)
+  bool tc_dx = false;        // dX by the tensor-core conv on dz ...
+  bool dx_elide = false;     // ... with the padding-vertex elision
+  bool tc_dt = false;        // dX by three plain GEMMs dT = dz W_k (only without tc_dx)
+};
+// The one place a conv's path is chosen: fin -> fout on `level` for `batch` meshes at the handle's precision.
+// network: a layer of the network schedules, which elide padding vertices, run dX as a conv on dz and take the thin
+// head's backward where thin_ok (input neither unpooled nor a residual source, not the first layer); otherwise the
+// single-layer entry points (and p2m_debug_conv_path), which do none of these.  need_dx: the caller wants dX.
+ConvRoute conv_route(const p2m_model* m, int level, int fin, int fout, int batch, bool network, bool thin_ok = false,
+                     bool need_dx = true) {
+  const DevLevel& g = m->levels[level];
+  const long long rows = (long long)batch * g.V;
+  const bool tc = m->precision == P2M_PREC_FP16X3_TC;
+  const size_t cap = wpack_capacity(network, fin, fout);
+  ConvRoute r;
+  r.tc = tc && umma_conv_supported(g, fin, fout);
+  r.elide = network && r.tc && elided(m->elide_padding, g, rows, fout);
+  r.thin = network && thin_ok && thin_conv_bwd_supported(fin, fout);
+  r.tc_dw = tc && !r.thin && umma_dw_supported(g, fin, fout);
+  const bool dx_tc = tc && !r.thin && need_dx && umma_conv_supported(g, fout, fin);
+  // (T1 = L~dz fills fout of the 3 fin columns of the T buffer)
+  r.tc_dx = network && dx_tc && umma_wpack_bytes(fout, fin) <= cap && fout <= 3LL * fin;
+  r.dw_dz_basis = r.tc_dx && umma_dw_supported(g, fout, fin);
+  r.dx_elide = r.tc_dx && elided(m->elide_padding, g, rows, fin);
+  r.tc_dt = dx_tc && !r.tc_dx && umma_plain_pack_bytes(fin, fout) <= cap;
+  return r;
+}
+
+// UmmaConvArgs of a conv a.fin -> a.fout as the kernel runs it (the weight image is set by whoever packs it)
+UmmaConvArgs umma_args(const DevLevel& g, int batch, const float* x, int in_unpool, int fin, int fout, const Epilogue& ep,
+                       float* y, const float* a_scale) {
+  UmmaConvArgs a;
+  a.g = &g;
+  a.x = x;
+  a.in_unpool = in_unpool;
+  a.batch = batch;
+  a.fin = fin;
+  a.fout = fout;
+  a.wpack = nullptr;
+  a.ep = ep;
+  a.y = y;
+  a.a_scale = a_scale;
+  return a;
+}
+
+// A conv on the tensor cores: weight pack into wpack, T1 pass into T (unless t1_given: T already holds L~x for every
+// row), the conv; with `elide` the conv covers the connected rows and a plain GEMM with the combined weights (packed into
+// w_iso) the isolated ones: all of them (iso_mode 0), the class representatives only (1, DevLevel::rep_tiles) or none
+// (2: nothing the caller reads depends on them).  W is the layer's [fout, fin*3] weight; `transposed`: the
+// backward-data conv on dz, a.fin = the layer's fout, a.fout = its fin.
+int run_tc_conv(p2m_model* m, UmmaConvArgs a, const float* W, bool transposed, bool elide, int iso_mode, bool t1_given,
+                float* T, unsigned char* wpack, unsigned char* w_iso, cudaStream_t s) {
+  const DevLevel& g = *a.g;
+  const int fin = transposed ? a.fout : a.fin, fout = transposed ? a.fin : a.fout;
+  if (m->trace != nullptr && !transposed) {  // trace builds only: P2M_TRACE_V / P2M_TRACE_UNPOOL pick the layer logged
+    const char* tv = getenv("P2M_TRACE_V");
+    const char* tu = getenv("P2M_TRACE_UNPOOL");
+    const char* tf = getenv("P2M_TRACE_FOUT");
+    a.trace = m->trace;
+    if ((tv && atoi(tv) != g.V) || (tu && atoi(tu) != a.in_unpool) || (tf && atoi(tf) != a.fout)) a.trace = nullptr;
+    // P2M_TRACE_NTH = k: only the k-th (from 0) matching conv launch since p2m_debug_set_trace is logged
+    const char* tn = getenv("P2M_TRACE_NTH");
+    if (a.trace != nullptr && tn && m->trace_seen++ != atoi(tn)) a.trace = nullptr;
+  }
+  P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_ALL, 0.f, wpack, s));
+  if (!t1_given) P2M_TRY(launch_cheb_t1(g, a.x, a.in_unpool, a.batch, a.fin, T, s, elide ? &g.real_tiles : nullptr));
+  a.t1 = T;
+  a.wpack = wpack;
+  if (elide) a.tiles = &g.real_tiles;
+  P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
+  if (!elide || iso_mode == 2) return P2M_OK;
+  P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_COMBINED, g.iso_diag, w_iso, s));
+  a.t1 = nullptr;
+  a.plain = 1;
+  a.trace = nullptr;  // the trace buffer holds the connected rows' launch; the isolated rows' GEMM would overwrite it
+  a.tiles = (iso_mode == 1 && g.n_rep > 0) ? &g.rep_tiles : &g.iso_tiles;
+  a.wpack = w_iso;
+  return launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s);
+}
+
+// dT = dz * Wp  ([rows, Fout] x [Fout, 3 Fin]) into T on the tensor cores: three plain GEMMs (one per Chebyshev order,
+// N = Fin, K = Fout, B_k[f][o] = W[o][f*3 + k]) with dz scaled into fp16's range by a_scale
+int run_tc_dt(p2m_model* m, const DevLevel& g, int batch, const float* dz, int fin, int fout, const float* W,
+              const Epilogue& ep, const float* a_scale, unsigned char* wpack, float* T, cudaStream_t s) {
+  for (int k = 0; k < 3; ++k) {
+    P2M_TRY(launch_umma_pack_weights(W, fin, fout, true, k, 0.f, wpack, s));
+    UmmaConvArgs a = umma_args(g, batch, dz, 0, fout, fin, ep, T, a_scale);
+    a.wpack = wpack;
+    a.plain = 1;
+    a.ldy = 3LL * fin;
+    a.y_col0 = k * fin;
+    P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
+  }
+  return P2M_OK;
+}
+
+// ---- one conv layer, linear part + epilogue: y = epilogue( [T0|T1|T2](x) * Wp^T ) on the path r chose
+// keep_wp: also leave the k-major copy of the weights in wp (what the SIMT GEMM reads) for the backward's SIMT dT GEMM
+int conv_linear(p2m_model* m, const ConvRoute& r, const Layer& L, int B, const float* x, int in_unpool,
+                const float* w_ref, float* T, float* wp, unsigned char* wpack, const Epilogue& ep, float* y,
+                cudaStream_t s, bool keep_wp, int iso_mode = 0, const float* head_wt = nullptr,
+                float* head_z = nullptr) {
   const int rows = B * L.V;
   const DevLevel& g = m->levels[L.level];
-  // k-major copy of the weights: what the SIMT GEMM reads, and (training, keep_wp) what backward's SIMT dT GEMM reads
-  if (keep_wp || !conv_on_tensor_cores(m, L, wpack)) P2M_TRY(launch_permute_w(w_ref, wp, L.fout, L.fin, s));
-  if (conv_on_tensor_cores(m, L, wpack)) {
-    P2M_TRY(launch_umma_pack_weights(w_ref, L.fin, L.fout, wpack, s));
-    UmmaConvArgs a;
-    a.trace = m->trace;
-    if (a.trace != nullptr) {  // trace builds only: P2M_TRACE_V / P2M_TRACE_UNPOOL pick the layer whose launch is logged
-      const char* tv = getenv("P2M_TRACE_V");
-      const char* tu = getenv("P2M_TRACE_UNPOOL");
-      const char* tf = getenv("P2M_TRACE_FOUT");
-      if ((tv && atoi(tv) != L.V) || (tu && atoi(tu) != in_unpool) || (tf && atoi(tf) != L.fout)) a.trace = nullptr;
-      // P2M_TRACE_NTH = k: only the k-th (from 0) matching conv launch since p2m_debug_set_trace is logged
-      const char* tn = getenv("P2M_TRACE_NTH");
-      if (a.trace != nullptr && tn && m->trace_seen++ != atoi(tn)) a.trace = nullptr;
-    }
+  if (keep_wp || !r.tc) P2M_TRY(launch_permute_w(w_ref, wp, L.fout, L.fin, s));
+  if (r.tc) {
+    UmmaConvArgs a = umma_args(g, B, x, in_unpool, L.fin, L.fout, ep, y, nullptr);
     a.head_wt = head_wt;
     a.head_z = head_z;
-    // Padding-vertex elision (DevLevel::n_iso): connected rows through the conv on index-list tiles, isolated rows
-    // through a plain GEMM with the combined weights (packed into T behind the T1 part: T is 3 Fin wide).
-    const bool elide = may_elide && m->elide_padding && g.n_iso > 0 && rows >= 2 * L.fout &&
-                       (m->elide_padding >= 2 || 5LL * g.n_iso >= 2LL * g.V);
-    // first sparse product as its own pass (T doubles as the T1 buffer)
-    P2M_TRY(launch_cheb_t1(g, x, in_unpool, B, L.fin, T, s, elide ? &g.real_tiles : nullptr));
-    a.t1 = T;
-    a.g = &g;
-    a.x = x;
-    a.in_unpool = in_unpool;
-    a.batch = B;
-    a.fin = L.fin;
-    a.fout = L.fout;
-    a.wpack = wpack;
-    a.ep = ep;
-    a.y = y;
-    a.a_scale = a_scale;
-    if (!elide) return launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s);
-    a.tiles = &g.real_tiles;
-    P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
-    if (iso_mode == 2) return P2M_OK;  // nothing the caller reads depends on the isolated rows (gathered eval output)
-    const bool reps_only = (iso_mode == 1 && g.n_rep > 0);
-    unsigned char* w_iso = reinterpret_cast<unsigned char*>(T + (size_t)rows * L.fin);
-    P2M_TRY(launch_umma_pack_iso(w_ref, g.iso_diag, L.fin, L.fout, w_iso, s));
-    a.t1 = nullptr;
-    a.plain = 1;
-    a.trace = nullptr;  // the trace buffer holds the connected rows' launch; the isolated rows' GEMM would overwrite it
-    a.tiles = reps_only ? &g.rep_tiles : &g.iso_tiles;
-    a.wpack = w_iso;
-    return launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s);
+    // the isolated rows' combined weights go into T behind the T1 part (T is 3 Fin wide)
+    return run_tc_conv(m, a, w_ref, false, r.elide, iso_mode, false, T, wpack,
+                       reinterpret_cast<unsigned char*>(T + (size_t)rows * L.fin), s);
   }
   if (head_z != nullptr) {
     set_error("conv_linear: fused head requested off the tensor-core path");
@@ -338,9 +411,8 @@ int conv_linear(p2m_model* m, const Layer& L, int B, const float* x, int in_unpo
   return P2M_OK;
 }
 
-// The default elision policy (elide_padding == 1): levels that have the tile families and where at least 40 % of
-// the rows are isolated.
-inline bool policy_elided(const DevLevel& g) { return g.n_iso > 0 && 5LL * g.n_iso >= 2LL * g.V; }
+// The default elision policy (elide_padding == 1) on a level, whatever the batch and width.
+inline bool policy_elided(const DevLevel& g) { return elided(1, g, g.V, 0); }
 
 // Classes of identical isolated rows (eval mode, DevLevel::rep_tiles).  Levels are ordered fine -> coarse, the joint
 // graph last; the parent of row r of mesh level k is row r >> 1 of level k + 1 (nearest x2 unpool, meshnet.py:71-78).
@@ -396,7 +468,7 @@ int build_padding_classes(p2m_model* m, const p2m_model_desc_t* d) {
         if (iso[k][r]) ro[r] = r;
       continue;
     }
-    P2M_TRY(build_index_tiles(reps, d->rowptr[k], d->colidx[k], d->values[k], V, &g.rep_tiles, &m->owned));
+    P2M_TRY(build_tileset(reps, d->rowptr[k], d->colidx[k], d->values[k], V, &g.rep_tiles, &m->owned));
     P2M_TRY(upload(m, cdst, &g.copy_dst));
     P2M_TRY(upload(m, csrc, &g.copy_src));
     g.n_rep = (int)reps.size();
@@ -681,17 +753,13 @@ int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int3
     return P2M_ERR_INVALID;
   }
   const DevLevel& g = m->levels[level];
-  const bool tc = (m->precision == P2M_PREC_FP16X3_TC);
-  const bool conv = tc && umma_conv_supported(g, fin, fout);
-  const bool dw = tc && umma_dw_supported(g, fin, fout);
-  const bool dt = tc && umma_conv_supported(g, fout, fin) &&
-                  umma_plain_pack_bytes(fin, fout) <= umma_wpack_bytes(((fin + 31) / 32) * 32, fout);
-  out[0] = conv;
-  out[1] = conv ? umma_conv_x_stages(g, fout, false) : 0;
-  out[2] = dw;
-  out[3] = dw ? umma_dw_x_stages(g) : 0;
-  out[4] = dt;
-  out[5] = dt ? umma_conv_x_stages(g, fin, true) : 0;
+  const ConvRoute r = conv_route(m, level, fin, fout, 1, false);  // what p2m_cheb_conv_fwd / _bwd run
+  out[0] = r.tc;
+  out[1] = r.tc ? umma_conv_x_stages(g, fout, false) : 0;
+  out[2] = r.tc_dw;
+  out[3] = r.tc_dw ? umma_dw_x_stages(g) : 0;
+  out[4] = r.tc_dt;
+  out[5] = r.tc_dt ? umma_conv_x_stages(g, fin, true) : 0;
   out[6] = (g.meta128.n_pattern > 0 && umma_tma_rows(g)) ? 1 : 0;
   out[7] = g.meta128.max_h1;
   out[8] = g.n_iso;
@@ -794,6 +862,7 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
       const int rows = B * L.V;
       const bool last = (li == nl - 1);
       const bool with_res = L.block_end && blk.has_residual;
+      const ConvRoute r = conv_route(m, L.level, L.fin, L.fout, B, true);
       if (!training) {
         Epilogue ep;
         float* scale = w.scale_scratch;
@@ -842,7 +911,7 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
         // the head shrinks to its two 4-wide sparse products: the 64-wide activation never reaches HBM.
         bool fuse_head = false;
         if (m->fuse_head && !last && li + 1 == nl - 1 && j + 1 < blk.n_layers && !with_res && !blk.has_residual &&
-            L.fout == 64 && rows >= 64 && conv_on_tensor_cores(m, L, w.wpack)) {
+            L.fout == 64 && rows >= 64 && r.tc) {
           const Layer& H = m->layers[li + 1];
           fuse_head = thin_conv_supported(H.fin, H.fout) && H.fin == L.fout && H.V == L.V;
         }
@@ -853,12 +922,12 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
           float* Z = out;  // [rows][12] | U [rows][4] | W' [64][12] inside this layer's (unused) output buffer
           float* wt = Z + (size_t)rows * 16;
           P2M_TRY(launch_thin_prep(P->cl_w[li + 1], L.fout, m->layers[li + 1].fout, wt, s));
-          P2M_TRY(conv_linear(m, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, wt, Z,
-                              false, true, iso_mode));
+          P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, false,
+                              iso_mode, wt, Z));
           head_z = Z;
         } else {
-          P2M_TRY(conv_linear(m, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, nullptr,
-                              nullptr, false, true, iso_mode));
+          P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, false,
+                              iso_mode));
         }
         if (m->profiling) P2M_CUDA_OK(cudaEventRecord(m->ev_end[li], s));
         cur = out;
@@ -868,8 +937,7 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
         Epilogue ep;
         ep.bias = P->cl_b[li];
         float* z = last ? y : w.z[li];
-        P2M_TRY(conv_linear(m, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp[li], w.wpack, ep, z, s, nullptr, nullptr,
-                            true, true));
+        P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp[li], w.wpack, ep, z, s, true));
         if (L.bn) {
           P2M_TRY(launch_col_stats(z, rows, L.fout, w.sums, s));
           P2M_TRY(launch_bn_finalize(w.sums, rows, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li],
@@ -1049,18 +1117,10 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         keep_buf = g_cur_buf;
         keep_ptr = g_cur;
       }
-      const bool tc = (m->precision == P2M_PREC_FP16X3_TC);
       const bool need_dx = !(li == 0 && dx == nullptr);
       const bool res_here = (j == 0) && blk.has_residual;
-      // which path takes this layer's weight / data gradients
-      const bool thin = thin_conv_bwd_supported(L.fin, L.fout) && !in_unpool && !res_here && li > 0;
-      const bool tc_dw = tc && !thin && umma_dw_supported(g, L.fin, L.fout);
-      const bool tc_dx = tc && !thin && need_dx && umma_conv_supported(g, L.fout, L.fin) &&
-                         umma_wpack_bytes(L.fout, L.fin) <= sc.wpack_bytes && (size_t)L.fout <= 3 * (size_t)L.fin;
-      const bool tc_dt = tc && !thin && need_dx && !tc_dx && umma_conv_supported(g, L.fout, L.fin) &&
-                         umma_plain_pack_bytes(L.fin, L.fout) <= sc.wpack_bytes;
-      const bool dw_dz_basis = tc_dx && umma_dw_supported(g, L.fout, L.fin);
-      const bool want_scale = tc_dw || tc_dx || tc_dt;
+      const ConvRoute r = conv_route(m, L.level, L.fin, L.fout, B, true, !in_unpool && !res_here && li > 0, need_dx);
+      const bool want_scale = r.tc_dw || r.tc_dx || r.tc_dt;
       bool have_scale = false;
       if (L.bn) {
         int tgt = (g_cur_buf >= 0 && g_cur_buf != keep_buf) ? g_cur_buf : free_buf(g_cur_buf, keep_buf, -1);
@@ -1087,7 +1147,7 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
           out = sc.G[out_buf];
         }
       }
-      if (thin) {
+      if (r.thin) {
         // weights-first backward of the thin head: dW and dX from the 3-wide basis of dz, X read once
         P2M_TRY(launch_thin_conv_bwd(g, inp, rows, L.fin, L.fout, P->cl_w[li], g_z, sc.thin, out, G->cl_w[li],
                                      m->sm_count, s));
@@ -1095,14 +1155,14 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         // dW.  tensor-core path: T2 of one side is formed on chip by the forward's producers from T1 = L~(that side)
         // and contracted with the (power-of-two scaled) plain tiles of the other side by MN-major wgmma; otherwise
         // SIMT: materialise T, dWp = g_z^T T.
-        if (dw_dz_basis) {
+        if (r.dw_dz_basis) {
           // sum_rows dz (x) T_k(X) = sum_rows T_k(dz) (x) X  (L~ symmetric): the basis of the GRADIENT, whose first
           // sparse product the backward-data pass below needs anyway, contracted with plain tiles of the layer input
           P2M_TRY(launch_cheb_t1(g, g_z, 0, B, L.fout, w.T, s, nullptr));
           P2M_TRY(launch_fill_zero(G->cl_w[li], sizeof(float) * L.fout * 3 * L.fin, s));
           P2M_TRY(launch_umma_dw(g, B, g_z, 0, L.fout, w.T, inp, in_unpool, L.fin, 1, sc.a_scale, G->cl_w[li],
                                  m->kernel_status, m->sm_count, s));
-        } else if (tc_dw) {
+        } else if (r.tc_dw) {
           // the basis of the layer input (w.T is overwritten by the dX pass's own T1 pass below)
           P2M_TRY(launch_cheb_t1(g, inp, in_unpool, B, L.fin, w.T, s, nullptr));
           P2M_TRY(launch_fill_zero(G->cl_w[li], sizeof(float) * L.fout * 3 * L.fin, s));
@@ -1116,7 +1176,7 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         }
       }
       // dX
-      if (need_dx && tc_dx) {
+      if (need_dx && r.tc_dx) {
         // Backward-data IS a forward conv: dXl = [dz | L~dz | (2L~^2 - I)dz] W'^T with W'[f][o*3+k] = W[o][f*3+k]
         // (L~ symmetric) — the T1 pass and the tensor-core conv kernel of the forward, run on dz (scaled into fp16's
         // range by a power of two), with the padding-vertex elision of the forward.  An identity residual gradient
@@ -1124,69 +1184,27 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         const bool identity_res = res_here && blk.cin == blk.cout;
         const bool finish = in_unpool || (res_here && !identity_res);
         float* dst = finish ? sc.U : out;
-        const bool elide = m->elide_padding && g.n_iso > 0 && rows >= 2 * L.fin &&
-                           (m->elide_padding >= 2 || 5LL * g.n_iso >= 2LL * g.V);
-        if (!dw_dz_basis)  // (the dW from the basis of dz above already left L~dz of every row in w.T)
-          P2M_TRY(launch_cheb_t1(g, g_z, 0, B, L.fout, w.T, s, elide ? &g.real_tiles : nullptr));
-        P2M_TRY(launch_umma_pack_weights_t(P->cl_w[li], L.fin, L.fout, sc.wpack, s));
-        UmmaConvArgs a;
-        a.g = &g;
-        a.x = g_z;
-        a.in_unpool = 0;
-        a.batch = B;
-        a.fin = L.fout;
-        a.fout = L.fin;
-        a.wpack = sc.wpack;
-        a.t1 = w.T;
-        a.a_scale = sc.a_scale;
-        a.y = dst;
+        Epilogue ep;
         if (identity_res) {
-          a.ep.res = keep_ptr;
-          a.ep.res_F = blk.cout;
-          a.ep.res_unpool = 0;
-          a.ep.res_i0 = blk.interp.i0;
-          a.ep.res_i1 = blk.interp.i1;
-          a.ep.res_lam = blk.interp.lam;
+          ep.res = keep_ptr;
+          ep.res_F = blk.cout;
+          ep.res_i0 = blk.interp.i0;
+          ep.res_i1 = blk.interp.i1;
+          ep.res_lam = blk.interp.lam;
         }
-        if (elide) a.tiles = &g.real_tiles;
-        P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
-        if (elide) {
-          P2M_TRY(launch_umma_pack_iso_t(P->cl_w[li], g.iso_diag, L.fin, L.fout, sc.wpack_iso, s));
-          a.t1 = nullptr;
-          a.plain = 1;
-          a.tiles = &g.iso_tiles;
-          a.wpack = sc.wpack_iso;
-          P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
-        }
+        // (the dW from the basis of dz above already left L~dz of every row in w.T)
+        P2M_TRY(run_tc_conv(m, umma_args(g, B, g_z, 0, L.fout, L.fin, ep, dst, sc.a_scale), P->cl_w[li], true,
+                            r.dx_elide, 0, r.dw_dz_basis, w.T, sc.wpack, sc.wpack_iso, s));
         if (finish)
           P2M_TRY(launch_dx_finish(dst, rows, L.fin, (res_here && !identity_res) ? keep_ptr : nullptr, blk.cout,
                                    (res_here && !identity_res) ? &blk.interp : nullptr, in_unpool, out, s));
-      } else if (need_dx && !thin) {
-        Epilogue none;
-        // dT = g_z * Wp  ([rows, Fout] x [Fout, 3 Fin]).  tensor-core fallback: three plain GEMMs (one per Chebyshev
-        // order, N = Fin, K = Fout) with the gradient scaled into fp16 range by a power of two.
-        if (tc_dt) {
-          for (int k = 0; k < 3; ++k) {
-            // B_k[n = f][kk = o] = W[o, f*3 + k]   (reference layout, lib/models/backbones/cheby_graph_conv.py:32-37)
-            P2M_TRY(launch_umma_pack_plain(P->cl_w[li] + k, 3, 3LL * L.fin, L.fin, L.fout, sc.wpack, s));
-            UmmaConvArgs a;
-            a.g = &g;
-            a.x = g_z;
-            a.in_unpool = 0;
-            a.batch = B;
-            a.fin = L.fout;
-            a.fout = L.fin;
-            a.wpack = sc.wpack;
-            a.y = w.T;
-            a.plain = 1;
-            a.a_scale = sc.a_scale;
-            a.ldy = 3LL * L.fin;
-            a.y_col0 = k * L.fin;
-            P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
-          }
-        } else {
-          P2M_TRY(launch_gemm(g_z, L.fout, w.wp[li], 3 * L.fin, 1, w.T, 3 * L.fin, rows, 3 * L.fin, L.fout, none, s));
-        }
+      } else if (need_dx && !r.thin) {
+        // dT = g_z * Wp  ([rows, Fout] x [Fout, 3 Fin]) on the tensor cores or SIMT
+        if (r.tc_dt)
+          P2M_TRY(run_tc_dt(m, g, B, g_z, L.fin, L.fout, P->cl_w[li], Epilogue(), sc.a_scale, sc.wpack, w.T, s));
+        else
+          P2M_TRY(launch_gemm(g_z, L.fout, w.wp[li], 3 * L.fin, 1, w.T, 3 * L.fin, rows, 3 * L.fin, L.fout, Epilogue(),
+                              s));
         P2M_TRY(launch_cheb_basis_bwd(g, w.T, rows, L.fin, sc.U, res_here ? keep_ptr : nullptr, blk.cout,
                                       res_here ? &blk.interp : nullptr, in_unpool, out, s));
       }
@@ -1215,14 +1233,7 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
 }
 
 // -------------------------------------------------------------------------------------
-size_t p2m_cheb_conv_workspace_bytes(const p2m_model_t* m, int level, int batch, int fin, int fout) {
-  if (!m || level < 0 || level >= (int)m->levels.size()) return 0;
-  size_t rows = (size_t)batch * m->levels[level].V;
-  return align_up(rows * 3 * fin * 4) + align_up((size_t)fout * 3 * fin * 4) * 2 + align_up(rows * fin * 4) +
-         align_up(rows * fout * 4) + align_up(2 * (size_t)std::max(fin, fout) * 8) + align_up(2 * (size_t)fout * 4) +
-         align_up(umma_wpack_bytes(((fin + 31) / 32) * 32, fout) + 16) + align_up(4 * 4) +
-         align_up(2 * (size_t)std::max(fin, fout) * 4) + ALIGN;
-}
+}  // extern "C"
 
 namespace {
 // The single-layer entry points take arbitrary user tensors, so on the tensor cores both fp16x3 operands are brought
@@ -1236,16 +1247,49 @@ struct RangeScales {
   float* x_scale;
   float* vec;      // [2 max(fin, fout)]: rescaled epilogue scale | shift
 };
-RangeScales take_range_scales(Bump* b, int fin, int fout) {
-  float* sc = b->take<float>(4);
-  return RangeScales{sc, sc + 1, sc + 2, b->take<float>(2 * (size_t)std::max(fin, fout))};
-}
-// w_out = W * w_scale / 2^6: what launch_umma_pack_weights / _pack_plain (x 2^6) then turn into W * w_scale
+// w_out = W * w_scale / 2^6: what launch_umma_pack_weights (x 2^6) then turns into W * w_scale
 int prescale_weights(const float* W, long long n, const RangeScales& r, float* w_out, cudaStream_t s) {
   P2M_TRY(launch_absmax_scale(W, n, r.w_scale, s));
   return launch_scale_by(W, n, r.w_scale, 0, 1.f / 64.f, w_out, s);
 }
+
+// Workspace of the single-layer entry points (one map for forward and backward)
+struct LayerWs {
+  float* T;              // [rows, 3 fin]: basis, T1 (+ the isolated rows' image) or dT
+  float* wp;             // k-major weights of the SIMT GEMMs
+  float* w2;             // range-normalised weights (tensor cores); backward: first the SIMT dW in k-major order
+  float* U;              // backward: [rows, fin] range-normalised input, then scratch of the basis backward
+  float* z;              // forward: [rows, fout] pre-BatchNorm output
+  double* sums;          // [2 max(fin, fout)]
+  float* sc;             // [2 fout]: BatchNorm scale | shift (forward), a_scale (backward)
+  unsigned char* wpack;  // weight images of the tensor-core conv / dT GEMMs
+  RangeScales rs;
+  size_t bytes;
+};
+LayerWs map_layer_workspace(void* base, size_t rows, int fin, int fout) {
+  LayerWs w;
+  Bump b(base);
+  w.T = b.take<float>(rows * 3 * fin);
+  w.wp = b.take<float>((size_t)fout * 3 * fin);
+  w.w2 = b.take<float>((size_t)fout * 3 * fin);
+  w.U = b.take<float>(rows * fin);
+  w.z = b.take<float>(rows * fout);
+  w.sums = b.take<double>(2 * (size_t)std::max(fin, fout));
+  w.sc = b.take<float>(2 * (size_t)fout);
+  w.wpack = b.take<unsigned char>(wpack_capacity(false, fin, fout) + 16);
+  float* sc = b.take<float>(4);
+  w.rs = RangeScales{sc, sc + 1, sc + 2, b.take<float>(2 * (size_t)std::max(fin, fout))};
+  w.bytes = b.off;
+  return w;
+}
 }  // namespace
+
+extern "C" {
+
+size_t p2m_cheb_conv_workspace_bytes(const p2m_model_t* m, int level, int batch, int fin, int fout) {
+  if (!m || level < 0 || level >= (int)m->levels.size()) return 0;
+  return map_layer_workspace(nullptr, (size_t)batch * m->levels[level].V, fin, fout).bytes + ALIGN;
+}
 
 int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* workspace, size_t workspace_bytes,
                       p2m_stream_t stream) {
@@ -1260,35 +1304,27 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   P2M_TRY(check_kernel_status(m, "cheb_conv_fwd"));
   DeviceGuard guard(m->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const DevLevel& g = m->levels[a->level];
   Layer L{};
   L.level = a->level;
-  L.V = m->levels[a->level].V;
+  L.V = g.V;
   L.fin = a->fin;
   L.fout = a->fout;
   const size_t rows = (size_t)a->batch * L.V;
-  Bump b(workspace);
-  float* T = b.take<float>(rows * 3 * L.fin);
-  float* wp = b.take<float>((size_t)L.fout * 3 * L.fin);
-  float* wsc = b.take<float>((size_t)L.fout * 3 * L.fin);  // range-normalised weights (tensor cores)
-  b.take<float>(rows * L.fin);
-  float* z = b.take<float>(rows * L.fout);
-  double* sums = b.take<double>(2 * (size_t)std::max(L.fin, L.fout));
-  float* sc = b.take<float>(2 * (size_t)L.fout);
-  unsigned char* wpack = b.take<unsigned char>(umma_wpack_bytes(((L.fin + 31) / 32) * 32, L.fout) + 16);
-  const RangeScales rs = take_range_scales(&b, L.fin, L.fout);
-  const DevLevel& g = m->levels[a->level];
-  // on the tensor cores: range-normalised operands (take_range_scales)
+  const LayerWs w = map_layer_workspace(workspace, rows, L.fin, L.fout);
+  const ConvRoute r = conv_route(m, a->level, L.fin, L.fout, a->batch, false);
+  // on the tensor cores: range-normalised operands (RangeScales)
   auto conv = [&](const Epilogue& e, float* out) -> int {
-    if (!conv_on_tensor_cores(m, L, wpack)) return conv_linear(m, L, a->batch, a->x, 0, a->weight, T, wp, wpack, e, out, s);
-    P2M_TRY(prescale_weights(a->weight, (long long)L.fout * 3 * L.fin, rs, wsc, s));
-    P2M_TRY(launch_absmax_scale(a->x, (long long)rows * L.fin, rs.a_scale, s, g.headroom_log2));
+    if (!r.tc) return conv_linear(m, r, L, a->batch, a->x, 0, a->weight, w.T, w.wp, w.wpack, e, out, s, false);
+    P2M_TRY(prescale_weights(a->weight, (long long)L.fout * 3 * L.fin, w.rs, w.w2, s));
+    P2M_TRY(launch_absmax_scale(a->x, (long long)rows * L.fin, w.rs.a_scale, s, g.headroom_log2));
     Epilogue er;
-    er.scale = rs.vec;
-    er.shift = rs.vec + L.fout;
+    er.scale = w.rs.vec;
+    er.shift = w.rs.vec + L.fout;
     er.relu = e.relu;
-    P2M_TRY(launch_rescaled_epilogue(e, rs.w_scale, 64.f, L.fout, rs.vec, rs.vec + L.fout, s));
-    return conv_linear(m, L, a->batch, a->x, 0, wsc, T, wp, wpack, er, out, s, nullptr, nullptr, true, false, 0,
-                       rs.a_scale);
+    P2M_TRY(launch_rescaled_epilogue(e, w.rs.w_scale, 64.f, L.fout, w.rs.vec, w.rs.vec + L.fout, s));
+    return run_tc_conv(m, umma_args(g, a->batch, a->x, 0, L.fin, L.fout, er, out, w.rs.a_scale), w.w2, false, false, 0,
+                       false, w.T, w.wpack, nullptr, s);
   };
   Epilogue ep;
   if (a->bn_mode == 0) {
@@ -1305,19 +1341,19 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
       set_error("cheb_conv_fwd: running stats missing");
       return P2M_ERR_INVALID;
     }
-    P2M_TRY(launch_bn_fold_eval(a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var, a->bias, sc,
-                                sc + L.fout, L.fout, s));
-    ep.scale = sc;
-    ep.shift = sc + L.fout;
+    P2M_TRY(launch_bn_fold_eval(a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var, a->bias, w.sc,
+                                w.sc + L.fout, L.fout, s));
+    ep.scale = w.sc;
+    ep.shift = w.sc + L.fout;
     ep.relu = a->relu;
     return conv(ep, a->y);
   }
   ep.bias = a->bias;
-  P2M_TRY(conv(ep, z));
-  P2M_TRY(launch_col_stats(z, (int)rows, L.fout, sums, s));
-  P2M_TRY(launch_bn_finalize(sums, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var,
-                             a->bn_num_batches_tracked, a->save_mean, a->save_invstd, sc, sc + L.fout, s));
-  P2M_TRY(launch_affine_act(z, (int)rows, L.fout, sc, sc + L.fout, a->relu, nullptr, 0, 0, nullptr, a->y, s));
+  P2M_TRY(conv(ep, w.z));
+  P2M_TRY(launch_col_stats(w.z, (int)rows, L.fout, w.sums, s));
+  P2M_TRY(launch_bn_finalize(w.sums, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var,
+                             a->bn_num_batches_tracked, a->save_mean, a->save_invstd, w.sc, w.sc + L.fout, s));
+  P2M_TRY(launch_affine_act(w.z, (int)rows, L.fout, w.sc, w.sc + L.fout, a->relu, nullptr, 0, 0, nullptr, a->y, s));
   return P2M_OK;
 }
 
@@ -1338,77 +1374,50 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
   const DevLevel& g = m->levels[a->level];
   const int fin = a->fin, fout = a->fout;
   const size_t rows = (size_t)a->batch * g.V;
-  Bump b(workspace);
-  float* T = b.take<float>(rows * 3 * fin);
-  float* wp = b.take<float>((size_t)fout * 3 * fin);
-  float* dwp = b.take<float>((size_t)fout * 3 * fin);
-  float* U = b.take<float>(rows * fin);
-  b.take<float>(rows * fout);
-  double* sums = b.take<double>(2 * (size_t)std::max(fin, fout));
-  float* sc2 = b.take<float>(2 * (size_t)fout);
-  unsigned char* wpack = b.take<unsigned char>(umma_wpack_bytes(((fin + 31) / 32) * 32, fout) + 16);
-  const RangeScales rs = take_range_scales(&b, fin, fout);
-  float* a_scale = sc2;  // device scalar for the tensor-core paths (the forward's scale/shift slot is free here)
-  const bool tc = (m->precision == P2M_PREC_FP16X3_TC);
-  bool have_scale = false;
+  const LayerWs w = map_layer_workspace(workspace, rows, fin, fout);
+  const RangeScales& rs = w.rs;
+  float* a_scale = w.sc;  // device scalar for the tensor-core paths (the forward's scale/shift slot is free here)
+  const ConvRoute r = conv_route(m, a->level, fin, fout, a->batch, false, false, a->dx != nullptr);
   if (!g.symmetric) {
     set_error("cheb_conv_bwd: the Laplacian is not symmetric; the backward kernels apply L~ where the gradient needs "
               "L~^T");
     return P2M_ERR_INVALID;
   }
-  P2M_TRY(launch_col_sum(a->dz, (int)rows, fout, sums, a->dbias, s));
-  if (tc && umma_dw_supported(g, fin, fout)) {
+  P2M_TRY(launch_col_sum(a->dz, (int)rows, fout, w.sums, a->dbias, s));
+  if (r.tc_dw) {
     P2M_TRY(launch_absmax_scale(a->dz, (long long)rows * fout, a_scale, s));
-    have_scale = true;
     // the layer input into fp16's range as well (with the basis headroom), in U (free until the dX pass); dW then
     // comes out multiplied by that power of two.  L~U goes into the first rows x fin floats of T, which nothing reads
     // before the dX pass overwrites it.
     P2M_TRY(launch_absmax_scale(a->x, (long long)rows * fin, rs.x_scale, s, g.headroom_log2));
-    P2M_TRY(launch_scale_by(a->x, (long long)rows * fin, rs.x_scale, 0, 1.f, U, s));
-    P2M_TRY(launch_cheb_t1(g, U, 0, a->batch, fin, T, s));
+    P2M_TRY(launch_scale_by(a->x, (long long)rows * fin, rs.x_scale, 0, 1.f, w.U, s));
+    P2M_TRY(launch_cheb_t1(g, w.U, 0, a->batch, fin, w.T, s));
     P2M_TRY(launch_fill_zero(a->dweight, sizeof(float) * fout * 3 * fin, s));
-    P2M_TRY(launch_umma_dw(g, a->batch, U, 0, fin, T, a->dz, 0, fout, 0, a_scale, a->dweight, m->kernel_status,
+    P2M_TRY(launch_umma_dw(g, a->batch, w.U, 0, fin, w.T, a->dz, 0, fout, 0, a_scale, a->dweight, m->kernel_status,
                            m->sm_count, s));
     P2M_TRY(launch_scale_by(a->dweight, (long long)fout * 3 * fin, rs.x_scale, 1, 1.f, a->dweight, s));
   } else {
-    P2M_TRY(launch_cheb_basis(g, a->x, 0, (int)rows, fin, T, s));
-    P2M_TRY(launch_fill_zero(dwp, sizeof(float) * fout * 3 * fin, s));
-    P2M_TRY(launch_gemm_tn_atomic(a->dz, fout, T, 3 * fin, dwp, 3 * fin, (int)rows, fout, 3 * fin, s));
-    P2M_TRY(launch_unpermute_w(dwp, a->dweight, fout, fin, s));
+    P2M_TRY(launch_cheb_basis(g, a->x, 0, (int)rows, fin, w.T, s));
+    P2M_TRY(launch_fill_zero(w.w2, sizeof(float) * fout * 3 * fin, s));
+    P2M_TRY(launch_gemm_tn_atomic(a->dz, fout, w.T, 3 * fin, w.w2, 3 * fin, (int)rows, fout, 3 * fin, s));
+    P2M_TRY(launch_unpermute_w(w.w2, a->dweight, fout, fin, s));
   }
   if (a->dx) {
     Epilogue none;
-    if (tc && umma_conv_supported(g, fout, fin) && umma_plain_pack_bytes(fin, fout) <= umma_wpack_bytes(((fin + 31) / 32) * 32, fout)) {
-      if (!have_scale) P2M_TRY(launch_absmax_scale(a->dz, (long long)rows * fout, a_scale, s));
-      // weights range-normalised into dwp (the SIMT weight gradient above is done with it); the plain conv's
-      // epilogue undoes the scale
-      P2M_TRY(prescale_weights(a->weight, (long long)fout * 3 * fin, rs, dwp, s));
+    if (r.tc_dt) {
+      if (!r.tc_dw) P2M_TRY(launch_absmax_scale(a->dz, (long long)rows * fout, a_scale, s));
+      // weights range-normalised into w2 (the SIMT weight gradient above is done with it); the plain GEMMs' epilogue
+      // undoes the scale
+      P2M_TRY(prescale_weights(a->weight, (long long)fout * 3 * fin, rs, w.w2, s));
       none.scale = rs.vec;
       none.shift = rs.vec + fin;
       P2M_TRY(launch_rescaled_epilogue(Epilogue(), rs.w_scale, 64.f, fin, rs.vec, rs.vec + fin, s));
-      for (int k = 0; k < 3; ++k) {
-        P2M_TRY(launch_umma_pack_plain(dwp + k, 3, 3LL * fin, fin, fout, wpack, s));
-        UmmaConvArgs u;
-        u.g = &g;
-        u.x = a->dz;
-        u.in_unpool = 0;
-        u.batch = a->batch;
-        u.fin = fout;
-        u.fout = fin;
-        u.wpack = wpack;
-        u.y = T;
-        u.plain = 1;
-        u.ep = none;
-        u.a_scale = a_scale;
-        u.ldy = 3LL * fin;
-        u.y_col0 = k * fin;
-        P2M_TRY(launch_umma_conv(u, m->kernel_status, m->zero_row, m->sm_count, s));
-      }
+      P2M_TRY(run_tc_dt(m, g, a->batch, a->dz, fin, fout, w.w2, none, a_scale, w.wpack, w.T, s));
     } else {
-      P2M_TRY(launch_permute_w(a->weight, wp, fout, fin, s));
-      P2M_TRY(launch_gemm(a->dz, fout, wp, 3 * fin, 1, T, 3 * fin, (int)rows, 3 * fin, fout, none, s));
+      P2M_TRY(launch_permute_w(a->weight, w.wp, fout, fin, s));
+      P2M_TRY(launch_gemm(a->dz, fout, w.wp, 3 * fin, 1, w.T, 3 * fin, (int)rows, 3 * fin, fout, none, s));
     }
-    P2M_TRY(launch_cheb_basis_bwd(g, T, (int)rows, fin, U, nullptr, 0, nullptr, 0, a->dx, s));
+    P2M_TRY(launch_cheb_basis_bwd(g, w.T, (int)rows, fin, w.U, nullptr, 0, nullptr, 0, a->dx, s));
   }
   return P2M_OK;
 }

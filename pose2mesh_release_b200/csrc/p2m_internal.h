@@ -245,11 +245,11 @@ struct UmmaConvArgs {
   int in_unpool;
   int batch;                // rows = batch * g->V
   int fin, fout;
-  const void* wpack;        // packed fp16 hi/lo weights from launch_umma_pack_weights
+  const void* wpack;        // packed fp16 hi/lo weights from launch_umma_pack_weights (WPACK_ALL)
   Epilogue ep;
   float* y;                 // [rows, fout]
-  // plain-GEMM mode (backward dT = dz * W_k): no SpMM, x is [rows, fin] and the K-blocks come from
-  // launch_umma_pack_plain; y is written at y[r*ldy + y_col0 + n]
+  // plain-GEMM mode (isolated rows, backward dT = dz * W_k): no SpMM, x is [rows, fin] and the K-blocks are a plain
+  // image (launch_umma_pack_weights, WPACK_COMBINED or one order); y is written at y[r*ldy + y_col0 + n]
   const float* t1 = nullptr;        // T1 = L~ x [rows, fin] (launch_cheb_t1): required unless plain
   int plain = 0;
   const float* a_scale = nullptr;   // device scalar from launch_absmax_scale (or null)
@@ -268,18 +268,24 @@ struct UmmaConvArgs {
 int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val, int V, DevLevel* out,
                           std::vector<void*>* owned);
 // Tiles of 128 (and, TileSet::m64, 64) consecutive entries of `rows` (ascending vertex ids of one level) as a TileSet.
-int build_index_tiles(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
-                      TileSet* ts, std::vector<void*>* owned);
+int build_tileset(const std::vector<int>& rows, const int* rowptr, const int* colidx, const float* val, int V,
+                  TileSet* ts, std::vector<void*>* owned);
 bool umma_conv_supported(const DevLevel& g, int fin, int fout);
 // what launch_umma_conv / launch_umma_dw would select on the level's consecutive tiles (p2m_debug_conv_path)
 int umma_conv_x_stages(const DevLevel& g, int fout, bool plain);
 int umma_dw_x_stages(const DevLevel& g);
 bool umma_tma_rows(const DevLevel& g);
+// Weight images of a conv: fp16 [hi | lo] K-blocks of 32 k (x 2^6) from W [fout, fin*3] in the reference layout (column
+// f*3 + k), rows = output channels o and K = input features f; `transposed`: rows f and K = o, the backward-data conv's
+// W'[f][o*3 + k] = W[o][f*3 + k] (L~ symmetric: the forward conv run on dz gives dX).  `order` selects the image:
+//   WPACK_ALL       blocks u = chunk*3 + k of all three orders, umma_wpack_bytes(K, rows) bytes (the conv);
+//   WPACK_COMBINED  the isolated rows' combined weights W0 + c W1 + (2c^2 - 1) W2 (padding-vertex elision), and
+//   0, 1, 2         W_k alone (the backward's dT = dz W_k): plain images of umma_plain_pack_bytes(rows, K) bytes.
+constexpr int WPACK_ALL = -1, WPACK_COMBINED = -2;
 size_t umma_wpack_bytes(int fin, int fout);
-int launch_umma_pack_weights(const float* W /*[fout, fin*3] ref layout*/, int fin, int fout, void* wpack, cudaStream_t s);
-// B[n][k] = Bmat[n*ld_n + k*ld_k]  (n < N, k < K, K % 32 == 0) -> fp16 [hi|lo] K-blocks, one per 32 k
 size_t umma_plain_pack_bytes(int N, int K);
-int launch_umma_pack_plain(const float* Bmat, long long ld_n, long long ld_k, int N, int K, void* wpack, cudaStream_t s);
+int launch_umma_pack_weights(const float* W, int fin, int fout, bool transposed, int order, float c, void* wpack,
+                             cudaStream_t s);
 // scale_out[0] = 2^e with max|x| * 2^e in [2^(9-h), 2^(10-h)), h = headroom_log2  (1 if x is all zero or not
 // finite); scratch-free, two tiny launches
 int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s, int headroom_log2 = 0);
@@ -302,13 +308,6 @@ int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_u
 // T1 = L~ x for all rows of a level (tile-staged gather), t1 [batch*V, fin] fp32
 int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, float* t1, cudaStream_t s,
                    const TileSet* tiles = nullptr);
-// K-blocks of the combined weights of the isolated rows: B[n][f] = W[n][3f] + c W[n][3f+1] + (2c^2 - 1) W[n][3f+2]
-// (W in the reference layout [fout, fin*3]); same image as launch_umma_pack_plain(N = fout, K = fin)
-int launch_umma_pack_iso(const float* W, float c, int fin, int fout, void* wpack, cudaStream_t s);
-// Backward-data weights: the forward conv run on dz with W'[f][o*3+k] = W[o][f*3+k] gives dX (L~ is symmetric); images
-// for a layer with Fin' = fout, Fout' = fin: umma_wpack_bytes(fout, fin) / umma_plain_pack_bytes(fin, fout) bytes
-int launch_umma_pack_weights_t(const float* W /*[fout, fin*3]*/, int fin, int fout, void* wpack, cudaStream_t s);
-int launch_umma_pack_iso_t(const float* W, float c, int fin, int fout, void* wpack, cudaStream_t s);
 int launch_umma_conv(const UmmaConvArgs& a, int* status_flag, const float* zero_row, int sm_count, cudaStream_t s);
 // Dense GEMM on the tensor cores (wgmma, fp16x3): Y [M, N] = epilogue(X [M, K] W [N, K]^T), K % 32 == 0, N % 64 == 0; apack / wpack are
 // scratch of umma_gemm_apack_bytes(M, K) / umma_gemm_wpack_bytes(N, K); ep vectors and an identity residual
