@@ -410,6 +410,21 @@ size_t p2m_body_model_workspace_bytes(const p2m_body_model_t* m, int batch);
 int p2m_body_model_forward(const p2m_body_model_t* m, const float* pose, const float* betas, int betas_rule,
                            const float* trans, int center_idx, float* verts, float* joints, int batch,
                            void* workspace, size_t workspace_bytes, p2m_stream_t stream);
+/* The vector-Jacobian product of p2m_body_model_forward with respect to pose, betas and trans: the gradient the
+ * reference layer's autograd gives for the same call (same inputs, same betas_rule / center_idx).  grad_verts
+ * [batch, V, 3] and grad_joints [batch, n_out_joints, 3] are the cotangents (either NULL = zero).  Writes grad_pose
+ * [batch, 3 J] (the gradient of the axis-angle input; pose_mean is a constant), and, when not NULL, grad_betas
+ * [batch, S] (zeros when the forward does not use the given betas: NULL betas, or an all-zero batch under
+ * P2M_BETAS_ZERO_MEANS_MODEL) and grad_trans [batch, 3] (zeros when trans is not added).  With centring, the centre's
+ * gradient flows back through the centre joint (or vertex).  Recomputes what it needs; no state from the forward.
+ * fp32 on the CUDA cores, five launches, no atomics, no host synchronisation (CUDA-graph capturable); a sample's
+ * gradient is bitwise independent of its batch position and of the batch size.  Workspace >=
+ * p2m_body_model_backward_workspace_bytes (256-byte aligned). */
+size_t p2m_body_model_backward_workspace_bytes(const p2m_body_model_t* m, int batch);
+int p2m_body_model_backward(const p2m_body_model_t* m, const float* pose, const float* betas, int betas_rule,
+                            const float* trans, int center_idx, const float* grad_verts, const float* grad_joints,
+                            float* grad_pose, float* grad_betas, float* grad_trans, int batch, void* workspace,
+                            size_t workspace_bytes, p2m_stream_t stream);
 
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),

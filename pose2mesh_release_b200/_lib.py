@@ -123,6 +123,7 @@ EXPORTS = [
     "p2m_nearest_distances", "p2m_align_w_scale", "p2m_pck_accumulate",
     "p2m_render_workspace_bytes", "p2m_render_meshes",
     "p2m_body_model_create", "p2m_body_model_destroy", "p2m_body_model_workspace_bytes", "p2m_body_model_forward",
+    "p2m_body_model_backward_workspace_bytes", "p2m_body_model_backward",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
 ]
 
@@ -244,6 +245,11 @@ def load() -> C.CDLL:
         lib.p2m_body_model_workspace_bytes.restype = sz
         lib.p2m_body_model_forward.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, C.c_int, vp, sz, vp]
         lib.p2m_body_model_forward.restype = C.c_int
+        lib.p2m_body_model_backward_workspace_bytes.argtypes = [vp, C.c_int]
+        lib.p2m_body_model_backward_workspace_bytes.restype = sz
+        lib.p2m_body_model_backward.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, sz,
+                                                vp]
+        lib.p2m_body_model_backward.restype = C.c_int
         lib.p2m_graph_match_level.argtypes = [i64, c_int32_p, c_int32_p, C.POINTER(C.c_double), c_int64_p,
                                               C.POINTER(C.c_double), c_int32_p]
         lib.p2m_graph_match_level.restype = i32

@@ -14,9 +14,17 @@ kept, and decided on the device, so a forward never synchronises with the host a
     everything is re-centred on that output joint.
 
 Everything runs in libp2m_b200.so (p2m_body_model_*): fp32 on the CUDA cores, three kernel launches per forward.
-CUDA tensors only; inputs are made contiguous float32.  Deliberate differences from the reference layers:
+CUDA tensors only; inputs are made contiguous float32.
 
-  * forward only: an input that requires grad raises (Pose2Mesh never differentiates through the body model);
+Gradients are opt-in: with ``differentiable=True`` (constructor or from_reference) the outputs come from an autograd
+Function whose backward is p2m_body_model_backward (five launches), the gradient the reference layer's autograd gives
+with respect to pose, betas and trans (not the model buffers).  The forward runs the same launches, so its outputs are
+bitwise those of the default layer.  Betas the forward does not use (an all-zero SMPL batch) get a zero gradient;
+absent or single-element betas get none.  Double backward is not supported.  Deliberate differences from the reference
+layers:
+
+  * by default forward only: an input that requires grad raises, so a layer used to build targets never records a
+    graph by accident;
   * a single-element betas tensor counts as absent for SMPL as well (the reference raises for a non-zero one);
   * the zero tests compare every value with 0, where the reference's float32 norm also calls values below ~1e-19
     zero (their squares underflow).
@@ -32,6 +40,7 @@ import threading
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 from torch.nn import Module
 
 from . import _lib
@@ -54,8 +63,9 @@ class _BodyModel(Module):
     and after editing a buffer in place call refresh()."""
 
     def __init__(self, v_template, shapedirs, posedirs, J_regressor, weights, parents, betas, pose_mean, joint_map,
-                 scale, center_idx):
+                 scale, center_idx, differentiable=False):
         super().__init__()
+        self.differentiable = bool(differentiable)
         vt = _host(v_template)
         V = vt.size // 3
         J = len(parents)
@@ -126,14 +136,16 @@ class _BodyModel(Module):
             pass
 
     # ------------------------------------------------------------------------------------------- forward
-    @staticmethod
-    def _no_grad(**tensors):
+    def _no_grad(self, **tensors):
+        if self.differentiable:
+            return
         for name, t in tensors.items():
             if isinstance(t, torch.Tensor) and t.requires_grad:
-                raise RuntimeError(f"{name} requires grad: the native body model is forward only (Pose2Mesh never "
-                                   "differentiates through it); pass a detached tensor")
+                raise RuntimeError(f"{name} requires grad: this layer is forward only; build it with "
+                                   "differentiable=True to differentiate through it, or pass a detached tensor")
 
-    def _run(self, pose, betas, trans, betas_rule, pose_width):
+    def _prepare(self, pose, betas, trans, pose_width):
+        """Check and normalise the inputs (torch ops only, so autograd follows them): -> pose, betas, trans, centre."""
         if not isinstance(pose, torch.Tensor) or not pose.is_cuda:
             raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; the pose is not a CUDA tensor")
         if pose.dim() != 2 or pose.shape[1] != pose_width or pose.shape[0] == 0:
@@ -149,7 +161,9 @@ class _BodyModel(Module):
                 raise ValueError(f"betas must be [{B}, {self.n_betas}] (one row per pose); got {tuple(betas.shape)}")
             betas = betas.contiguous().float()
         if trans is not None:
-            if trans.numel() == 1 and not trans.is_cuda:  # the default torch.zeros(1), or a host scalar
+            if trans.numel() == 1 and not trans.is_cuda and trans.requires_grad:  # a host scalar to differentiate
+                trans = trans.to(dev).reshape(1, 1).expand(B, 3)
+            elif trans.numel() == 1 and not trans.is_cuda:  # the default torch.zeros(1), or a host scalar
                 value = float(trans)
                 trans = None if value == 0.0 else torch.full((B, 3), value, device=dev)
             elif trans.numel() == 1:  # a scalar is broadcast to every coordinate, as the reference does
@@ -165,42 +179,96 @@ class _BodyModel(Module):
             if not -self.n_out_joints <= int(self.center_idx) < self.n_out_joints:
                 raise ValueError(f"center_idx {self.center_idx} out of range for {self.n_out_joints} joints")
             center = int(self.center_idx) % self.n_out_joints
+        return pose, betas, trans, center
+
+    def _forward_native(self, pose, betas, trans, betas_rule, center):
+        B, dev = pose.shape[0], pose.device
         lib = _lib.load()
         h = self.handle(dev.index)
         verts = torch.empty((B, self.n_vertex, 3), device=dev, dtype=torch.float32)
         joints = torch.empty((B, self.n_out_joints, 3), device=dev, dtype=torch.float32)
         nbytes = lib.p2m_body_model_workspace_bytes(h, B)
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
         with torch.cuda.device(dev):
-            _lib.check(lib.p2m_body_model_forward(h, pose.data_ptr(), ptr(betas), betas_rule, ptr(trans), center,
+            _lib.check(lib.p2m_body_model_forward(h, pose.data_ptr(), _ptr(betas), betas_rule, _ptr(trans), center,
                                                   verts.data_ptr(), joints.data_ptr(), B, ws.data_ptr(), nbytes,
                                                   torch.cuda.current_stream(dev).cuda_stream),
                        "p2m_body_model_forward")
         return verts, joints
 
+    def _backward_native(self, pose, betas, trans, betas_rule, center, grad_verts, grad_joints, want_betas,
+                         want_trans):
+        B, dev = pose.shape[0], pose.device
+        lib = _lib.load()
+        h = self.handle(dev.index)
+        f32 = lambda g: None if g is None else g.contiguous().float()  # noqa: E731
+        grad_verts, grad_joints = f32(grad_verts), f32(grad_joints)
+        grad_pose = torch.empty_like(pose)
+        grad_betas = torch.empty_like(betas) if want_betas and betas is not None else None
+        grad_trans = torch.empty_like(trans) if want_trans and trans is not None else None
+        nbytes = lib.p2m_body_model_backward_workspace_bytes(h, B)
+        ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        with torch.cuda.device(dev):
+            _lib.check(lib.p2m_body_model_backward(h, pose.data_ptr(), _ptr(betas), betas_rule, _ptr(trans), center,
+                                                   _ptr(grad_verts), _ptr(grad_joints), grad_pose.data_ptr(),
+                                                   _ptr(grad_betas), _ptr(grad_trans), B, ws.data_ptr(), nbytes,
+                                                   torch.cuda.current_stream(dev).cuda_stream),
+                       "p2m_body_model_backward")
+        return grad_pose, grad_betas, grad_trans
+
+    def _run(self, pose, betas, trans, betas_rule, pose_width):
+        pose, betas, trans, center = self._prepare(pose, betas, trans, pose_width)
+        if self.differentiable:
+            return _BodyModelFunction.apply(self, betas_rule, center, pose, betas, trans)
+        return self._forward_native(pose, betas, trans, betas_rule, center)
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+class _BodyModelFunction(torch.autograd.Function):
+    """The native forward's outputs, with p2m_body_model_backward as their vector-Jacobian product.  The backward
+    recomputes what it needs from the saved inputs; it is not itself differentiable (no double backward)."""
+
+    @staticmethod
+    def forward(ctx, layer, betas_rule, center, pose, betas, trans):
+        ctx.layer, ctx.betas_rule, ctx.center = layer, betas_rule, center
+        ctx.set_materialize_grads(False)  # an unused output passes NULL, not a zero tensor
+        ctx.save_for_backward(pose, betas, trans)
+        return layer._forward_native(pose, betas, trans, betas_rule, center)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_verts, grad_joints):
+        pose, betas, trans = ctx.saved_tensors
+        want = ctx.needs_input_grad
+        gp, gb, gt = ctx.layer._backward_native(pose, betas, trans, ctx.betas_rule, ctx.center, grad_verts,
+                                                grad_joints, want[4], want[5])
+        return None, None, None, gp if want[3] else None, gb, gt
+
 
 class SMPLLayer(_BodyModel):
-    """Batched smplpytorch SMPL_Layer (forward only, on the GPU).
+    """Batched smplpytorch SMPL_Layer on the GPU (forward only unless differentiable=True).
 
     Arrays in the reference's layouts: v_template [V, 3], shapedirs [V, 3, S], posedirs [V, 3, 9 (J - 1)],
     J_regressor [J, V], weights [V, J], kintree_parents [J], betas [S] (the model's stored betas).  The root's entry
     of kintree_parents is ignored, as SMPL_Layer.forward ignores it (the SMPL pkl stores 2^32 - 1 there)."""
 
     def __init__(self, v_template, shapedirs, posedirs, J_regressor, weights, kintree_parents, betas,
-                 center_idx=None, gender="neutral"):
+                 center_idx=None, gender="neutral", differentiable=False):
         # the root's entry is never read by SMPL_Layer.forward; the SMPL pkl's kintree_table stores 2^32 - 1 there
         parents = [-1] + [int(p) for p in list(kintree_parents)[1:]]
         super().__init__(v_template, shapedirs, posedirs, J_regressor, weights, parents, betas, None,
-                         list(range(len(parents))), 1.0, center_idx)
+                         list(range(len(parents))), 1.0, center_idx, differentiable)
         self.gender = gender
 
     @classmethod
-    def from_reference(cls, layer) -> "SMPLLayer":
+    def from_reference(cls, layer, differentiable=False) -> "SMPLLayer":
         """Copy the buffers of an already-loaded smplpytorch SMPL_Layer."""
         return cls(layer.th_v_template, layer.th_shapedirs, layer.th_posedirs, layer.th_J_regressor, layer.th_weights,
                    list(layer.kintree_parents), layer.th_betas, center_idx=layer.center_idx,
-                   gender=getattr(layer, "gender", "neutral"))
+                   gender=getattr(layer, "gender", "neutral"), differentiable=differentiable)
 
     def forward(self, th_pose_axisang, th_betas=torch.zeros(1), th_trans=torch.zeros(1)):
         """th_pose_axisang [B, 3 J] -> verts [B, V, 3], joints [B, J, 3] (metres)."""
@@ -209,7 +277,7 @@ class SMPLLayer(_BodyModel):
 
 
 class ManoLayer(_BodyModel):
-    """Batched manopth ManoLayer (forward only, on the GPU) in the configuration Pose2Mesh uses (lib/_mano.py:37):
+    """Batched manopth ManoLayer on the GPU (forward only unless differentiable=True) in the configuration Pose2Mesh uses (lib/_mano.py:37):
     use_pca=False, axis-angle root and joints, either flat_hand_mean, either side.  The rest of ManoLayer is not
     supported, and Pose2Mesh uses none of it: use_pca=True, root_rot_mode other than 'axisang' (6-D root),
     joint_rot_mode='rotmat', and a truthy root_palm or share_betas in forward raise ValueError.
@@ -219,7 +287,7 @@ class ManoLayer(_BodyModel):
 
     def __init__(self, v_template, shapedirs, posedirs, J_regressor, weights, betas, hands_mean, center_idx=None,
                  flat_hand_mean=True, side="right", use_pca=False, root_rot_mode="axisang", joint_rot_mode="axisang",
-                 ncomps=45):
+                 ncomps=45, differentiable=False):
         if use_pca:
             raise ValueError("ManoLayer: use_pca=True is not supported (Pose2Mesh uses use_pca=False)")
         if root_rot_mode != "axisang":
@@ -231,19 +299,19 @@ class ManoLayer(_BodyModel):
         mean = np.zeros(45, np.float32) if flat_hand_mean else _host(hands_mean, (45,))
         jm = list(range(16)) + [-1 - t for t in MANO_TIPS[side]]
         super().__init__(v_template, shapedirs, posedirs, J_regressor, weights, MANO_PARENTS, betas, mean,
-                         [jm[i] for i in MANO_REORDER], 1000.0, center_idx)
+                         [jm[i] for i in MANO_REORDER], 1000.0, center_idx, differentiable)
         self.side, self.flat_hand_mean, self.use_pca, self.ncomps, self.rot = side, flat_hand_mean, False, 45, 3
         self.root_rot_mode = self.joint_rot_mode = "axisang"
 
     @classmethod
-    def from_reference(cls, layer) -> "ManoLayer":
+    def from_reference(cls, layer, differentiable=False) -> "ManoLayer":
         """Copy the buffers of an already-loaded manopth ManoLayer (its th_hands_mean already holds zeros when
         flat_hand_mean)."""
         return cls(layer.th_v_template, layer.th_shapedirs, layer.th_posedirs, layer.th_J_regressor, layer.th_weights,
                    layer.th_betas, layer.th_hands_mean, center_idx=layer.center_idx,
                    flat_hand_mean=bool(layer.flat_hand_mean), side=layer.side, use_pca=bool(layer.use_pca),
                    root_rot_mode=getattr(layer, "root_rot_mode", "axisang"),
-                   joint_rot_mode=getattr(layer, "joint_rot_mode", "axisang"))
+                   joint_rot_mode=getattr(layer, "joint_rot_mode", "axisang"), differentiable=differentiable)
 
     def forward(self, th_pose_coeffs, th_betas=torch.zeros(1), th_trans=torch.zeros(1), root_palm=torch.Tensor([0]),
                 share_betas=torch.Tensor([0])):

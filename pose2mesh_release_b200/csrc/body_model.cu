@@ -12,6 +12,8 @@
 //                    linear blend skinning over the vertex's non-zero weights
 // No atomics and fixed summation orders: a sample's result is bitwise independent of its batch position and of the
 // batch size; nothing is read back to the host, so a forward can be captured in a CUDA graph.
+// The backward (p2m_body_model_backward: the VJP with respect to pose, betas and trans) keeps the same properties in
+// five launches: k_batch_flags, k_pose, k_lbs_bwd, k_dcoef, k_pose_bwd (see the backward section below).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -323,6 +325,407 @@ constexpr size_t lbs_smem_bytes(int Kp, int J) {
 constexpr size_t LBS_SMEM_MAX = lbs_smem_bytes((MAX_K + KC - 1) / KC * KC, MAX_J);
 static_assert(LBS_SMEM_MAX <= 227 * 1024, "k_lbs shared memory exceeds the sm_90 limit");
 
+// ------------------------------------------------------------------------------------------------ backward
+// The vector-Jacobian product of the forward above, with respect to pose, betas and trans (p2m_body_model_backward).
+// It recomputes what it needs with k_batch_flags and k_pose (into the backward's own workspace), then:
+//  k_lbs_bwd   the k_lbs tiles again: v_posed x, g = scale (grad_verts + grad of the vertex's output joints),
+//              dx = T[:3,:3]^T g into the workspace, and per (sample, tile) partials of dA_j = sum_v w_vj g [x; 1]^T and
+//              of sum_v g, each summed over the tile's vertices in ascending order by one thread
+//  k_dcoef     dcoef = dx basis^T per 768-column split of the basis (a fixed split: per-(sample, split) partials)
+//  k_pose_bwd  one warp per sample: sums the partials in order, recomputes R, J, G, adds the centre term, walks the
+//              chain in reverse and applies the pose-blend, Rodrigues and J_regressor shapedirs backwards
+constexpr int DC_T = 256;               // threads per k_dcoef CTA: a 64-sample x 64-coefficient tile, 4 x 4 per thread
+constexpr int DC_BM = 64, DC_BN = 64, DC_BK = 16;
+constexpr int DC_COLS = 2 * TILE_COLS;  // basis columns per split
+constexpr int W_LD = NV + 1;            // row stride of k_lbs_bwd's dense weight tile (bank-conflict padding)
+
+struct BwdWork {
+  const float* dx;  // [B, ld]   T^T g per vertex column (zero in the padding)
+  const float* pA;  // [B, n_tiles, 12 J + 3]  per-tile partials of dA_j and of sum g
+  const float* pC;  // [B, n_split, Kp]        per-split partials of dcoef
+  int n_split;
+};
+
+// The derivative of rodrigues() as autograd takes it through batch_rodrigues: quat2mat, the renormalisation, the
+// half-angle quaternion, axis = theta / angle with angle = |theta + 1e-8|.  dR [9] -> dth [3].
+__device__ __forceinline__ void rodrigues_vjp(const float* th, const float* g, float* dth) {
+  const float a0 = th[0] + 1e-8f, a1 = th[1] + 1e-8f, a2 = th[2] + 1e-8f;
+  const float angle = sqrtf(a0 * a0 + a1 * a1 + a2 * a2);
+  const float half = angle * 0.5f;
+  const float c = cosf(half), s = sinf(half);
+  const float n0 = th[0] / angle, n1 = th[1] / angle, n2 = th[2] / angle;
+  const float q0 = c, q1 = s * n0, q2 = s * n1, q3 = s * n2;
+  const float qn = sqrtf(q0 * q0 + q1 * q1 + q2 * q2 + q3 * q3);
+  const float w = q0 / qn, x = q1 / qn, y = q2 / qn, z = q3 / qn;
+  const float dw = 2.f * (w * (g[0] + g[4] + g[8]) + x * (g[7] - g[5]) + y * (g[2] - g[6]) + z * (g[3] - g[1]));
+  const float dx = 2.f * (x * (g[0] - g[4] - g[8]) + y * (g[1] + g[3]) + z * (g[2] + g[6]) + w * (g[7] - g[5]));
+  const float dy = 2.f * (y * (g[4] - g[0] - g[8]) + x * (g[1] + g[3]) + z * (g[5] + g[7]) + w * (g[2] - g[6]));
+  const float dz = 2.f * (z * (g[8] - g[0] - g[4]) + x * (g[2] + g[6]) + y * (g[5] + g[7]) + w * (g[3] - g[1]));
+  const float dot = w * dw + x * dx + y * dy + z * dz;  // through q / |q|
+  const float e0 = (dw - w * dot) / qn, e1 = (dx - x * dot) / qn, e2 = (dy - y * dot) / qn, e3 = (dz - z * dot) / qn;
+  const float dn0 = s * e1, dn1 = s * e2, dn2 = s * e3;
+  const float ds = e1 * n0 + e2 * n1 + e3 * n2;
+  float dangle = 0.5f * (c * ds - s * e0);
+  dangle = dangle - (dn0 * th[0] + dn1 * th[1] + dn2 * th[2]) / (angle * angle);  // through theta / angle
+  const float r = dangle / angle;                                                   // through |theta + 1e-8|
+  dth[0] = dn0 / angle + r * a0, dth[1] = dn1 / angle + r * a1, dth[2] = dn2 / angle + r * a2;
+}
+
+// grid (sample groups, vertex tiles), the k_lbs tiling.  The basis loop is k_lbs's; then each thread stages (g, x) of
+// its vertex for its 8 samples, and the CTA's threads take (sample, joint) tasks: 12 entries of dA_j over the tile's
+// 128 vertices in ascending order (joint J: the 3 entries of sum g).
+__global__ void __launch_bounds__(LBS_T) k_lbs_bwd(ModelDev m, int batch, Work w, const float* __restrict__ grad_verts,
+                                                   const float* __restrict__ grad_joints, float* __restrict__ dx,
+                                                   float* __restrict__ pA) {
+  extern __shared__ float4 smem4[];
+  float* sB = reinterpret_cast<float*>(smem4);     // [2][KC][384], then [16][128][6] (g, x)
+  float* sC = sB + 2 * CHUNK_FLOATS;               // [Kp][16]
+  float* sA = sC + m.Kp * GS;                      // [16][J * 12]
+  float* sW = sA + GS * m.J * 12;                  // [J][W_LD]  dense skinning weights of the tile
+  const int tid = threadIdx.x;
+  const int g0 = blockIdx.x * GS, tile = blockIdx.y;
+  const int n_chunk = m.Kp / KC;
+  const float* btile = m.basis + (long long)tile * TILE_COLS;
+
+  auto load_chunk = [&](int ch, int stage) {
+    float* dst = sB + stage * CHUNK_FLOATS;
+    const float* src = btile + (long long)ch * KC * m.ld;
+    for (int i = tid; i < CHUNK_FLOATS / 4; i += LBS_T) {
+      const int row = i / (TILE_COLS / 4), q = i % (TILE_COLS / 4);
+      cp_async16(dst + row * TILE_COLS + 4 * q, src + (long long)row * m.ld + 4 * q);
+    }
+  };
+  load_chunk(0, 0);
+  cp_async_commit();
+
+  for (int i = tid; i < m.Kp * GS; i += LBS_T) {
+    const int s = i % GS, k = i / GS;
+    sC[i] = g0 + s < batch ? w.coef[(long long)(g0 + s) * m.Kp + k] : 0.f;
+  }
+  const int a_len = m.J * 12;
+  for (int i = tid; i < GS * a_len; i += LBS_T) {
+    const int s = i / a_len;
+    sA[i] = g0 + s < batch ? w.A[(long long)g0 * a_len + i] : 0.f;
+  }
+  const int vl = tid % NV, oct = tid / NV;
+  const int v = tile * NV + vl;
+  for (int j = oct; j < m.J; j += LBS_T / NV) {
+    float wt = 0.f;
+    if (v < m.V)
+      for (int e = m.w_ptr[v]; e < m.w_ptr[v + 1]; ++e)
+        if (m.w_idx[e] == j) wt = m.w_val[e];
+    sW[j * W_LD + vl] = wt;
+  }
+
+  float acc[8][3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float t = m.vtemp[3 * v + c];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[i][c] = t;
+  }
+  const float4* sC4 = reinterpret_cast<const float4*>(sC) + 2 * oct;
+  for (int ch = 0; ch < n_chunk; ++ch) {
+    if (ch + 1 < n_chunk) load_chunk(ch + 1, (ch + 1) & 1);
+    cp_async_commit();
+    cp_async_wait1();
+    __syncthreads();
+    const float* bs = sB + (ch & 1) * CHUNK_FLOATS + 3 * vl;
+#pragma unroll
+    for (int kk = 0; kk < KC; ++kk) {
+      const float b0 = bs[kk * TILE_COLS], b1 = bs[kk * TILE_COLS + 1], b2 = bs[kk * TILE_COLS + 2];
+      const float4 ca = sC4[(ch * KC + kk) * (GS / 4)], cb = sC4[(ch * KC + kk) * (GS / 4) + 1];
+      const float cs[8] = {ca.x, ca.y, ca.z, ca.w, cb.x, cb.y, cb.z, cb.w};
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        acc[i][0] = fmaf(b0, cs[i], acc[i][0]);
+        acc[i][1] = fmaf(b1, cs[i], acc[i][1]);
+        acc[i][2] = fmaf(b2, cs[i], acc[i][2]);
+      }
+    }
+    __syncthreads();
+  }
+  // the basis chunks are consumed: sB now holds (g, x) per (sample, vertex)
+  float* sGX = sB;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int sl = 8 * oct + i, s = g0 + sl;
+    float g[3] = {0.f, 0.f, 0.f};
+    if (v < m.V && s < batch) {
+      if (grad_verts)
+        for (int c = 0; c < 3; ++c) g[c] = grad_verts[((long long)s * m.V + v) * 3 + c];
+      if (grad_joints)
+        for (int q = 0; q < m.n_vj; ++q)
+          if (m.vj_vert[q] == v)
+            for (int c = 0; c < 3; ++c) g[c] = g[c] + grad_joints[((long long)s * m.n_out + m.vj_out[q]) * 3 + c];
+      for (int c = 0; c < 3; ++c) g[c] = g[c] * m.scale;
+    }
+    if (s < batch) {
+      // dx = T[:3,:3]^T g with T = sum_j w_vj A_j (ascending j), as the forward skins
+      float T[9];
+      for (int q = 0; q < 9; ++q) T[q] = 0.f;
+      if (v < m.V)
+        for (int e = m.w_ptr[v]; e < m.w_ptr[v + 1]; ++e) {
+          const float wt = m.w_val[e];
+          const float* a = sA + sl * a_len + 12 * m.w_idx[e];
+          for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) T[3 * r + c] = fmaf(wt, a[4 * r + c], T[3 * r + c]);
+        }
+      float* d = dx + (long long)s * m.ld + (long long)tile * TILE_COLS + 3 * vl;
+      for (int c = 0; c < 3; ++c) d[c] = fmaf(T[6 + c], g[2], fmaf(T[3 + c], g[1], T[c] * g[0]));
+    }
+    float* st = sGX + (sl * NV + vl) * 6;
+    st[0] = g[0], st[1] = g[1], st[2] = g[2], st[3] = acc[i][0], st[4] = acc[i][1], st[5] = acc[i][2];
+  }
+  __syncthreads();
+  const int PA = 12 * m.J + 3;
+  for (int t = tid; t < GS * (m.J + 1); t += LBS_T) {
+    const int sl = t / (m.J + 1), j = t % (m.J + 1), s = g0 + sl;
+    if (s >= batch) continue;
+    const float* gx = sGX + sl * NV * 6;
+    float* out = pA + ((long long)s * gridDim.y + tile) * PA;
+    if (j == m.J) {  // sum g
+      float r0 = 0.f, r1 = 0.f, r2 = 0.f;
+      for (int u = 0; u < NV; ++u) r0 = r0 + gx[6 * u], r1 = r1 + gx[6 * u + 1], r2 = r2 + gx[6 * u + 2];
+      out[12 * m.J] = r0, out[12 * m.J + 1] = r1, out[12 * m.J + 2] = r2;
+      continue;
+    }
+    float dA[12];
+#pragma unroll
+    for (int q = 0; q < 12; ++q) dA[q] = 0.f;
+    const float* wj = sW + j * W_LD;
+    for (int u = 0; u < NV; ++u) {
+      const float wt = wj[u];
+      if (wt == 0.f) continue;
+      const float* p = gx + 6 * u;
+      const float xh[4] = {p[3], p[4], p[5], 1.f};
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        const float wg = wt * p[r];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) dA[4 * r + c] = fmaf(wg, xh[c], dA[4 * r + c]);
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 12; ++q) out[12 * j + q] = dA[q];
+  }
+}
+
+// grid (sample blocks of 64, coefficient blocks of 64, column splits).  part[b, split, k] = sum over the split's columns
+// (ascending) of dx[b, col] basis[k, col]; every (b, k) is one thread's sequential sum, so it does not depend on the
+// sample's place in the batch.
+__global__ void __launch_bounds__(DC_T) k_dcoef(ModelDev m, int batch, const float* __restrict__ dx, int n_split,
+                                                float* __restrict__ part) {
+  __shared__ __align__(16) float sX[DC_BK][DC_BM];
+  __shared__ __align__(16) float sW[DC_BK][DC_BN];
+  const int tid = threadIdx.x, b0 = blockIdx.x * DC_BM, k0 = blockIdx.y * DC_BN, sp = blockIdx.z;
+  const int tx = tid % 16, ty = tid / 16;
+  const int lr = tid >> 2, lc = (tid & 3) * 4;
+  const int c_beg = sp * DC_COLS, c_end = min(c_beg + DC_COLS, m.ld);
+  float acc[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int k = 0; k < 4; ++k) acc[i][k] = 0.f;
+  for (int c0 = c_beg; c0 < c_end; c0 += DC_BK) {
+    float4 xv = make_float4(0.f, 0.f, 0.f, 0.f), bv = xv;
+    if (b0 + lr < batch) xv = *reinterpret_cast<const float4*>(dx + (long long)(b0 + lr) * m.ld + c0 + lc);
+    if (k0 + lr < m.Kp) bv = *reinterpret_cast<const float4*>(m.basis + (long long)(k0 + lr) * m.ld + c0 + lc);
+    __syncthreads();
+    sX[lc][lr] = xv.x, sX[lc + 1][lr] = xv.y, sX[lc + 2][lr] = xv.z, sX[lc + 3][lr] = xv.w;
+    sW[lc][lr] = bv.x, sW[lc + 1][lr] = bv.y, sW[lc + 2][lr] = bv.z, sW[lc + 3][lr] = bv.w;
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < DC_BK; ++kk) {
+      const float4 a = *reinterpret_cast<const float4*>(&sX[kk][4 * ty]);
+      const float4 bb = *reinterpret_cast<const float4*>(&sW[kk][4 * tx]);
+      const float av[4] = {a.x, a.y, a.z, a.w}, bw[4] = {bb.x, bb.y, bb.z, bb.w};
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) acc[i][k] = fmaf(av[i], bw[k], acc[i][k]);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int b = b0 + 4 * ty + i;
+    if (b >= batch) break;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int kc = k0 + 4 * tx + k;
+      if (kc < m.Kp) part[((long long)b * n_split + sp) * m.Kp + kc] = acc[i][k];
+    }
+  }
+}
+
+// One warp per sample: everything after the per-vertex work, in fixed orders.
+__global__ void __launch_bounds__(32) k_pose_bwd(ModelDev m, const float* __restrict__ pose,
+                                                 const float* __restrict__ betas, int betas_rule,
+                                                 const float* __restrict__ trans, int center_idx, Work w, BwdWork bw,
+                                                 const float* __restrict__ grad_joints, float* __restrict__ grad_pose,
+                                                 float* __restrict__ grad_betas, float* __restrict__ grad_trans) {
+  __shared__ float th[3 * MAX_J], R[MAX_J][9], jp[MAX_J][3], G[MAX_J][12], beta[MAX_S];
+  __shared__ float dA[MAX_J][12], dG[MAX_J][12], dR[MAX_J][9], dJ[MAX_J][3], gt[MAX_J][3], dcf[MAX_K + 16];
+  __shared__ float goff[3], dxc[3];
+  const int b = blockIdx.x, lane = threadIdx.x, J = m.J, S = m.S;
+  int flag = 0;
+  for (int i = lane; i < w.n_flag_blocks; i += 32) flag |= w.flags[i];
+  flag = __reduce_or_sync(0xffffffffu, flag);
+  const bool given = betas != nullptr && (betas_rule == P2M_BETAS_AS_GIVEN || (flag & 1));
+  const bool trans_used = trans != nullptr && (flag & 2);
+  for (int s = lane; s < S; s += 32) beta[s] = given ? betas[(long long)b * S + s] : m.mbetas[s];
+  for (int i = lane; i < 3 * J; i += 32) {
+    float x = pose[(long long)b * 3 * J + i];
+    if (m.pmean && i >= 3) x = m.pmean[i - 3] + x;
+    th[i] = x;
+  }
+  __syncwarp();
+  for (int j = lane; j < J; j += 32) rodrigues(th + 3 * j, R[j]);
+  for (int e = lane; e < 3 * J; e += 32) {
+    float acc = m.jtemp[e];
+    for (int s = 0; s < S; ++s) acc = fmaf(m.jshape[(long long)e * S + s], beta[s], acc);
+    jp[e / 3][e % 3] = acc;
+  }
+  // the partials, each summed in tile / split order
+  const int PA = 12 * J + 3, n_tiles = m.ld / TILE_COLS;
+  for (int k = lane; k < m.Kp; k += 32) {
+    float acc = 0.f;
+    for (int sp = 0; sp < bw.n_split; ++sp) acc = acc + bw.pC[((long long)b * bw.n_split + sp) * m.Kp + k];
+    dcf[k] = acc;
+  }
+  for (int e = lane; e < PA; e += 32) {
+    float acc = 0.f;
+    for (int t = 0; t < n_tiles; ++t) acc = acc + bw.pA[((long long)b * n_tiles + t) * PA + e];
+    if (e < 12 * J)
+      dA[e / 12][e % 12] = acc;
+    else
+      goff[e - 12 * J] = acc;  // sum over vertices of g, so far
+  }
+  __syncwarp();
+  const int r = lane >> 2, c = lane & 3;
+  if (lane < 12) G[0][lane] = c < 3 ? R[0][3 * r + c] : jp[0][r];
+  __syncwarp();
+  for (int j = 1; j < J; ++j) {
+    const int p = m.parents[j];
+    if (lane < 12) {
+      const float* g = G[p] + 4 * r;
+      float l0, l1, l2;
+      if (c < 3) {
+        l0 = R[j][c], l1 = R[j][3 + c], l2 = R[j][6 + c];
+      } else {
+        l0 = jp[j][0] - jp[p][0], l1 = jp[j][1] - jp[p][1], l2 = jp[j][2] - jp[p][2];
+      }
+      float v = fmaf(g[2], l2, fmaf(g[1], l1, g[0] * l0));
+      if (c == 3) v = v + g[3];
+      G[j][lane] = v;
+    }
+    __syncwarp();
+  }
+  // the gradient of the per-sample offset: every output moves with it
+  if (lane < 3) {
+    float acc = goff[lane];
+    if (grad_joints)
+      for (int o = 0; o < m.n_out; ++o)
+        if (m.jmap[o] >= 0) acc = acc + grad_joints[((long long)b * m.n_out + o) * 3 + lane] * m.scale;
+    goff[lane] = acc;
+    if (grad_trans) grad_trans[(long long)b * 3 + lane] = trans_used ? acc : 0.f;
+  }
+  __syncwarp();
+  const int ce = (!trans_used && center_idx >= 0) ? m.jmap[center_idx] : J;  // J: no centring
+  for (int e = lane; e < 3 * J; e += 32) {
+    const int j = e / 3, q = e % 3;
+    float acc = 0.f;
+    if (grad_joints)
+      for (int o = 0; o < m.n_out; ++o)
+        if (m.jmap[o] == j) acc = acc + grad_joints[((long long)b * m.n_out + o) * 3 + q] * m.scale;
+    if (ce == j) acc = acc - goff[q];
+    gt[j][q] = acc;
+  }
+  if (ce < 0) {  // centred on a vertex: - goff enters that vertex's skinning and v_posed
+    const int v = -1 - ce;
+    const float* A = w.A + (long long)b * J * 12;
+    const float* cf = w.coef + (long long)b * m.Kp;
+    if (lane == 0) {
+      float x[3], T[9];
+      for (int q = 0; q < 3; ++q) {
+        float acc = m.vtemp[3 * v + q];
+        for (int k = 0; k < m.Kp; ++k) acc = fmaf(m.basis[(long long)k * m.ld + 3 * v + q], cf[k], acc);
+        x[q] = acc;
+      }
+      for (int q = 0; q < 9; ++q) T[q] = 0.f;
+      for (int e = m.w_ptr[v]; e < m.w_ptr[v + 1]; ++e) {
+        const float wt = m.w_val[e];
+        const int j = m.w_idx[e];
+        for (int rr = 0; rr < 3; ++rr)
+          for (int cc = 0; cc < 3; ++cc) T[3 * rr + cc] = fmaf(wt, A[12 * j + 4 * rr + cc], T[3 * rr + cc]);
+        for (int rr = 0; rr < 3; ++rr) {
+          const float wg = wt * -goff[rr];
+          for (int cc = 0; cc < 3; ++cc) dA[j][4 * rr + cc] = fmaf(wg, x[cc], dA[j][4 * rr + cc]);
+          dA[j][4 * rr + 3] = dA[j][4 * rr + 3] + wg;
+        }
+      }
+      for (int q = 0; q < 3; ++q) dxc[q] = -(T[q] * goff[0] + T[3 + q] * goff[1] + T[6 + q] * goff[2]);
+    }
+    __syncwarp();
+    for (int k = lane; k < m.Kp; k += 32) {
+      const float* bk = m.basis + (long long)k * m.ld + 3 * v;
+      dcf[k] = dcf[k] + (bk[0] * dxc[0] + bk[1] * dxc[1] + bk[2] * dxc[2]);
+    }
+  }
+  __syncwarp();
+  // A_j = [G_j[:, :3] | G_j[:, 3] - G_j[:, :3] J_j]  ->  dG_j, dJ_j; the output joints add to dG_j[:, 3]
+  for (int e = lane; e < 12 * J; e += 32) {
+    const int j = e / 12, q = e % 12, rr = q >> 2, cc = q & 3;
+    dG[j][q] = cc < 3 ? dA[j][q] - dA[j][4 * rr + 3] * jp[j][cc] : dA[j][q] + gt[j][rr];
+  }
+  for (int e = lane; e < 3 * J; e += 32) {
+    const int j = e / 3, q = e % 3;
+    dJ[j][q] = -(G[j][q] * dA[j][3] + G[j][4 + q] * dA[j][7] + G[j][8 + q] * dA[j][11]);
+  }
+  __syncwarp();
+  // the chain in reverse: G_j = G_p [R_j | J_j - J_p]
+  for (int j = J - 1; j >= 1; --j) {
+    const int p = m.parents[j];
+    if (lane < 12) {
+      const float* d = dG[j] + 4 * r;
+      float v = d[3];
+      if (c < 3) v = d[0] * R[j][3 * c] + d[1] * R[j][3 * c + 1] + d[2] * R[j][3 * c + 2] + d[3] * (jp[j][c] - jp[p][c]);
+      dG[p][lane] = dG[p][lane] + v;
+    } else if (lane < 21) {
+      const int k = (lane - 12) / 3, cc = (lane - 12) % 3;
+      dR[j][3 * k + cc] = G[p][k] * dG[j][cc] + G[p][4 + k] * dG[j][4 + cc] + G[p][8 + k] * dG[j][8 + cc] +
+                          dcf[S + 9 * (j - 1) + 3 * k + cc];
+    } else if (lane < 24) {
+      const int k = lane - 21;
+      const float t = G[p][k] * dG[j][3] + G[p][4 + k] * dG[j][7] + G[p][8 + k] * dG[j][11];
+      dJ[j][k] = dJ[j][k] + t;
+      dJ[p][k] = dJ[p][k] - t;
+    }
+    __syncwarp();
+  }
+  if (lane < 9) dR[0][lane] = dG[0][4 * (lane / 3) + lane % 3];
+  if (lane < 3) dJ[0][lane] = dJ[0][lane] + dG[0][4 * lane + 3];
+  __syncwarp();
+  for (int j = lane; j < J; j += 32) {
+    float d[3];
+    rodrigues_vjp(th + 3 * j, dR[j], d);
+    for (int q = 0; q < 3; ++q) grad_pose[(long long)b * 3 * J + 3 * j + q] = d[q];
+  }
+  if (grad_betas)
+    for (int s = lane; s < S; s += 32) {
+      float acc = dcf[s];
+      for (int e = 0; e < 3 * J; ++e) acc = fmaf(m.jshape[(long long)e * S + s], dJ[e / 3][e % 3], acc);
+      grad_betas[(long long)b * S + s] = given ? acc : 0.f;
+    }
+}
+
+constexpr size_t lbs_bwd_smem_bytes(int Kp, int J) {
+  return sizeof(float) * ((size_t)2 * CHUNK_FLOATS + (size_t)Kp * GS + (size_t)GS * J * 12 + (size_t)J * W_LD);
+}
+constexpr size_t LBS_BWD_SMEM_MAX = lbs_bwd_smem_bytes((MAX_K + KC - 1) / KC * KC, MAX_J);
+static_assert(LBS_BWD_SMEM_MAX <= 227 * 1024, "k_lbs_bwd shared memory exceeds the sm_90 limit");
+static_assert(2 * CHUNK_FLOATS >= GS * NV * 6, "k_lbs_bwd stages (g, x) in the basis buffers");
+
 bool all_finite(const float* p, size_t n) {
   for (size_t i = 0; i < n; ++i)
     if (!std::isfinite(p[i])) return false;
@@ -444,6 +847,24 @@ WorkLayout work_layout(const p2m_body_model* m, int batch) {
   return l;
 }
 
+// The backward's workspace: the forward's, then k_pose's kinematic joints (unused), dx, and the two partial arrays.
+struct BwdLayout {
+  WorkLayout fwd;
+  size_t joints, dx, pA, pC, total;
+  int n_split;
+};
+BwdLayout bwd_layout(const p2m_body_model* m, int batch) {
+  BwdLayout l;
+  l.fwd = work_layout(m, batch);
+  l.n_split = (m->ld + DC_COLS - 1) / DC_COLS;
+  l.joints = l.fwd.total;
+  l.dx = l.joints + align256(sizeof(float) * (size_t)batch * m->n_out * 3);
+  l.pA = l.dx + align256(sizeof(float) * (size_t)batch * m->ld);
+  l.pC = l.pA + align256(sizeof(float) * (size_t)batch * m->n_tiles * (12 * m->J + 3));
+  l.total = l.pC + align256(sizeof(float) * (size_t)batch * l.n_split * m->Kp);
+  return l;
+}
+
 }  // namespace
 
 extern "C" {
@@ -556,6 +977,58 @@ int p2m_body_model_forward(const p2m_body_model_t* m, const float* pose, const f
   const dim3 grid((unsigned)((batch + GS - 1) / GS), (unsigned)m->n_tiles);
   P2M_CUDA_OK(cudaFuncSetAttribute(k_lbs, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LBS_SMEM_MAX));
   k_lbs<<<grid, LBS_T, m->lbs_smem, s>>>(m->dev, batch, w, verts, joints);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+size_t p2m_body_model_backward_workspace_bytes(const p2m_body_model_t* m, int batch) {
+  if (!m || batch <= 0 || batch > MAX_BATCH) return 0;
+  return bwd_layout(m, batch).total;
+}
+
+int p2m_body_model_backward(const p2m_body_model_t* m, const float* pose, const float* betas, int betas_rule,
+                            const float* trans, int center_idx, const float* grad_verts, const float* grad_joints,
+                            float* grad_pose, float* grad_betas, float* grad_trans, int batch, void* workspace,
+                            size_t workspace_bytes, p2m_stream_t stream) {
+  if (!m || !pose || !grad_pose || batch <= 0 || batch > MAX_BATCH ||
+      (betas_rule != P2M_BETAS_ZERO_MEANS_MODEL && betas_rule != P2M_BETAS_AS_GIVEN) || center_idx >= m->n_out) {
+    set_error("body_model_backward: bad argument (null model / pose / grad_pose, batch out of [1, 2^24], unknown "
+              "betas_rule or center_idx >= n_out_joints)");
+    return P2M_ERR_INVALID;
+  }
+  const BwdLayout l = bwd_layout(m, batch);
+  if (!workspace || workspace_bytes < l.total) {
+    set_error("body_model_backward: workspace needs " + std::to_string(l.total) + " bytes");
+    return P2M_ERR_WORKSPACE;
+  }
+  DeviceGuard guard(m->device);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  char* ws = static_cast<char*>(workspace);
+  const long long n_betas = (betas && betas_rule == P2M_BETAS_ZERO_MEANS_MODEL) ? (long long)batch * m->S : 0;
+  const long long n_trans = trans ? (long long)batch * 3 : 0;
+  const long long n_test = n_betas > n_trans ? n_betas : n_trans;
+  const int n_flag_blocks = (int)std::min<long long>(MAX_FLAG_BLOCKS, std::max<long long>(1, n_test / (16 * 1024)));
+  Work w{reinterpret_cast<int*>(ws + l.fwd.flags), n_flag_blocks, reinterpret_cast<float*>(ws + l.fwd.A),
+         reinterpret_cast<float*>(ws + l.fwd.coef), reinterpret_cast<float*>(ws + l.fwd.offs)};
+  float* dx = reinterpret_cast<float*>(ws + l.dx);
+  float* pA = reinterpret_cast<float*>(ws + l.pA);
+  float* pC = reinterpret_cast<float*>(ws + l.pC);
+  const int center = center_idx < 0 ? -1 : center_idx;
+  k_batch_flags<<<n_flag_blocks, FLAG_T, 0, s>>>(betas, n_betas, trans, n_trans, w.flags);
+  P2M_LAUNCH_OK();
+  k_pose<<<batch, 32, 0, s>>>(m->dev, pose, betas, betas_rule, trans, center,
+                              reinterpret_cast<float*>(ws + l.joints), w);
+  P2M_LAUNCH_OK();
+  const dim3 grid((unsigned)((batch + GS - 1) / GS), (unsigned)m->n_tiles);
+  P2M_CUDA_OK(cudaFuncSetAttribute(k_lbs_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LBS_BWD_SMEM_MAX));
+  k_lbs_bwd<<<grid, LBS_T, lbs_bwd_smem_bytes(m->Kp, m->J), s>>>(m->dev, batch, w, grad_verts, grad_joints, dx, pA);
+  P2M_LAUNCH_OK();
+  const dim3 dgrid((unsigned)((batch + DC_BM - 1) / DC_BM), (unsigned)((m->Kp + DC_BN - 1) / DC_BN),
+                   (unsigned)l.n_split);
+  k_dcoef<<<dgrid, DC_T, 0, s>>>(m->dev, batch, dx, l.n_split, pC);
+  P2M_LAUNCH_OK();
+  k_pose_bwd<<<batch, 32, 0, s>>>(m->dev, pose, betas, betas_rule, trans, center, w, BwdWork{dx, pA, pC, l.n_split},
+                                  grad_joints, grad_pose, grad_betas, grad_trans);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
