@@ -115,11 +115,13 @@ def channel_resample(x, fout):
 
 
 def forward(sd: Dict[str, torch.Tensor], laps: Sequence[torch.Tensor], x: torch.Tensor, *, mano: bool = False,
-            training: bool = False, n_in: int = 5, n_out: int = 3, collect=None) -> torch.Tensor:
+            training: bool = False, n_in: int = 5, n_out: int = 3, collect=None, plan=None) -> torch.Tensor:
     """meshnet.py:80-117.  `laps` from laplacians_to_torch (fine -> coarse, joint graph last).
     `sd` is a reference-layout state dict (tensors may require grad).  If `collect` is a list, every
-    conv layer's post-activation output is appended (layer-by-layer parity)."""
-    plan = channel_plan(n_in, n_out, mano)
+    conv layer's post-activation output is appended (layer-by-layer parity).  `plan` replaces the
+    reference's channel plan (len(laps) == len(plan) - 1); the dtype of `sd` and `x` is the one computed in."""
+    if plan is None:
+        plan = channel_plan(n_in, n_out, mano)
     n_blk = len(plan)
     n_joint = laps[-1].shape[0]
     x = x.reshape(-1, n_joint, n_in)

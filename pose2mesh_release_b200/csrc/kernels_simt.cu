@@ -836,8 +836,11 @@ int launch_bn_fold_eval(const float* gamma, const float* beta, const float* rm, 
   return P2M_OK;
 }
 
-// per-channel sum / sum of squares.  Block = 256 threads = (F-lanes x row-lanes); fp32 partials over
-// <= ROWS_PER_BLOCK/rl rows, fp64 across blocks.
+// per-channel sum / sum of squares of the SHIFTED data z - K, K = z[0][f] (k_bn_finalize reads the same K).  The
+// plain sums cancel catastrophically in var = E[z^2] - mean^2 once |mean| >> std (a constant in front of the BN);
+// around a sample of the channel they stay of the order of the variance.  Block = 256 threads = (F-lanes x
+// row-lanes); fp32 partials over <= STAT_ROWS/rl rows, fp64 across blocks.  Every thread runs the same number of
+// channel rounds (the barriers inside), also when F > 256 is not a multiple of 256.
 constexpr int STAT_ROWS = 512;
 __global__ void __launch_bounds__(256) k_col_stats(const float* __restrict__ z, long long rows, int F,
                                                    double* __restrict__ sums) {
@@ -847,11 +850,14 @@ __global__ void __launch_bounds__(256) k_col_stats(const float* __restrict__ z, 
   const int fl = threadIdx.x % lanes, rr = threadIdx.x / lanes;
   const long long rbeg = (long long)blockIdx.x * STAT_ROWS;
   const long long rend = min(rows, rbeg + STAT_ROWS);
-  for (int f = fl; f < F; f += lanes) {
+  for (int f0 = 0; f0 < F; f0 += lanes) {
+    const int f = f0 + fl;
+    const bool live = f < F;
     float s = 0.f, q = 0.f;
-    if (rr < rl) {
+    if (rr < rl && live) {
+      const float k = z[f];
       for (long long r = rbeg + rr; r < rend; r += rl) {
-        float v = z[r * F + f];
+        const float v = z[r * F + f] - k;
         s += v;
         q = fmaf(v, v, q);
       }
@@ -859,7 +865,7 @@ __global__ void __launch_bounds__(256) k_col_stats(const float* __restrict__ z, 
     sm[threadIdx.x] = s;
     sm[256 + threadIdx.x] = q;
     __syncthreads();
-    if (rr == 0) {
+    if (rr == 0 && live) {
       for (int j = 1; j < rl; ++j) {
         s += sm[j * lanes + fl];
         q += sm[256 + j * lanes + fl];
@@ -877,15 +883,17 @@ int launch_col_stats(const float* z, int rows, int F, double* sums, cudaStream_t
   return P2M_OK;
 }
 
-__global__ void k_bn_finalize(const double* __restrict__ sums, long long rows, int F, const float* gamma,
-                              const float* beta, float* rm, float* rv, long long* nbt, float* save_mean,
-                              float* save_invstd, float* scale, float* shift) {
+// sums = k_col_stats' (S, Q) of z - K around K = z[0][c]:  mean = K + S/n,  var = Q/n - (S/n)^2
+__global__ void k_bn_finalize(const double* __restrict__ sums, const float* __restrict__ z, long long rows, int F,
+                              const float* gamma, const float* beta, float* rm, float* rv, long long* nbt,
+                              float* save_mean, float* save_invstd, float* scale, float* shift) {
   int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c == 0 && nbt) *nbt += 1;
   if (c >= F) return;
   double n = (double)rows;
-  double mean = sums[c] / n;
-  double var = sums[F + c] / n - mean * mean;
+  double d = sums[c] / n;
+  double mean = (double)z[c] + d;
+  double var = sums[F + c] / n - d * d;
   if (var < 0) var = 0;
   float invstd = (float)(1.0 / sqrt(var + 1e-5));
   if (rm) rm[c] = 0.9f * rm[c] + 0.1f * (float)mean;                                  // momentum 0.1
@@ -896,9 +904,10 @@ __global__ void k_bn_finalize(const double* __restrict__ sums, long long rows, i
   scale[c] = sc;
   shift[c] = beta[c] - (float)mean * sc;
 }
-int launch_bn_finalize(const double* sums, int rows, int F, const float* gamma, const float* beta, float* rm, float* rv,
-                       int64_t* nbt, float* save_mean, float* save_invstd, float* scale, float* shift, cudaStream_t s) {
-  k_bn_finalize<<<cdiv(F, 128), 128, 0, s>>>(sums, rows, F, gamma, beta, rm, rv, (long long*)nbt, save_mean,
+int launch_bn_finalize(const double* sums, const float* z, int rows, int F, const float* gamma, const float* beta,
+                       float* rm, float* rv, int64_t* nbt, float* save_mean, float* save_invstd, float* scale,
+                       float* shift, cudaStream_t s) {
+  k_bn_finalize<<<cdiv(F, 128), 128, 0, s>>>(sums, z, rows, F, gamma, beta, rm, rv, (long long*)nbt, save_mean,
                                              save_invstd, scale, shift);
   P2M_LAUNCH_OK();
   return P2M_OK;

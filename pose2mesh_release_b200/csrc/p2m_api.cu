@@ -940,7 +940,7 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
         P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp[li], w.wpack, ep, z, s, true));
         if (L.bn) {
           P2M_TRY(launch_col_stats(z, rows, L.fout, w.sums, s));
-          P2M_TRY(launch_bn_finalize(w.sums, rows, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li],
+          P2M_TRY(launch_bn_finalize(w.sums, z, rows, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li],
                                      P->bn_nbt ? P->bn_nbt[li] : nullptr, w.mean[li], w.invstd[li], w.scale[li],
                                      w.shift[li], s));
           P2M_TRY(launch_affine_act(z, rows, L.fout, w.scale[li], w.shift[li], L.relu, with_res ? block_in : nullptr,
@@ -1313,9 +1313,14 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   const size_t rows = (size_t)a->batch * L.V;
   const LayerWs w = map_layer_workspace(workspace, rows, L.fin, L.fout);
   const ConvRoute r = conv_route(m, a->level, L.fin, L.fout, a->batch, false);
-  // on the tensor cores: range-normalised operands (RangeScales)
+  // on the tensor cores: range-normalised operands (RangeScales).  That kernel moves x and output rows in 16-byte
+  // pieces, so a caller's x or y off 16-byte alignment (e.g. a tensor view at an odd offset) takes the CUDA-core conv.
   auto conv = [&](const Epilogue& e, float* out) -> int {
-    if (!r.tc) return conv_linear(m, r, L, a->batch, a->x, 0, a->weight, w.T, w.wp, w.wpack, e, out, s, false);
+    if (!r.tc || ((reinterpret_cast<uintptr_t>(a->x) | reinterpret_cast<uintptr_t>(out)) & 15)) {
+      ConvRoute simt = r;
+      simt.tc = false;
+      return conv_linear(m, simt, L, a->batch, a->x, 0, a->weight, w.T, w.wp, w.wpack, e, out, s, false);
+    }
     P2M_TRY(prescale_weights(a->weight, (long long)L.fout * 3 * L.fin, w.rs, w.w2, s));
     P2M_TRY(launch_absmax_scale(a->x, (long long)rows * L.fin, w.rs.a_scale, s, g.headroom_log2));
     Epilogue er;
@@ -1351,8 +1356,9 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   ep.bias = a->bias;
   P2M_TRY(conv(ep, w.z));
   P2M_TRY(launch_col_stats(w.z, (int)rows, L.fout, w.sums, s));
-  P2M_TRY(launch_bn_finalize(w.sums, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var,
-                             a->bn_num_batches_tracked, a->save_mean, a->save_invstd, w.sc, w.sc + L.fout, s));
+  P2M_TRY(launch_bn_finalize(w.sums, w.z, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean,
+                             a->bn_running_var, a->bn_num_batches_tracked, a->save_mean, a->save_invstd, w.sc,
+                             w.sc + L.fout, s));
   P2M_TRY(launch_affine_act(w.z, (int)rows, L.fout, w.sc, w.sc + L.fout, a->relu, nullptr, 0, 0, nullptr, a->y, s));
   return P2M_OK;
 }

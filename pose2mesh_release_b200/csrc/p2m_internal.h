@@ -216,9 +216,11 @@ int launch_copy_rows(float* y, int batch, int V, int F, const int* dst, const in
 // BatchNorm1d over rows (cheby_graph_conv.py:38-39; meshnet.py:55): eps 1e-5, momentum 0.1
 int launch_bn_fold_eval(const float* gamma, const float* beta, const float* rm, const float* rv, const float* bias,
                         float* scale, float* shift, int F, cudaStream_t s);
+// sums of z - z[0] per channel (shifted: no cancellation for |mean| >> std); launch_bn_finalize reads the same z[0]
 int launch_col_stats(const float* z, int rows, int F, double* sums /*[2F] zeroed here*/, cudaStream_t s);
-int launch_bn_finalize(const double* sums, int rows, int F, const float* gamma, const float* beta, float* rm, float* rv,
-                       int64_t* nbt, float* save_mean, float* save_invstd, float* scale, float* shift, cudaStream_t s);
+int launch_bn_finalize(const double* sums, const float* z, int rows, int F, const float* gamma, const float* beta,
+                       float* rm, float* rv, int64_t* nbt, float* save_mean, float* save_invstd, float* scale,
+                       float* shift, cudaStream_t s);
 // a = relu?(z*scale+shift) (+ resampled residual)
 int launch_affine_act(const float* z, int rows, int F, const float* scale, const float* shift, int relu,
                       const float* res, int res_F, int res_unpool, const InterpTable* it, float* a, cudaStream_t s);

@@ -220,6 +220,103 @@ def posenet_forward(sd, x, num_stage: int, eps: float = 1e-5, precision: str = "
     return out, eout + U32 * np.abs(out)
 
 
+# --------------------------------------------------------------------------------------------- BatchNorm1d over rows
+BN_EPS, BN_MOMENTUM = 1e-5, 0.1
+STAT_ROWS = 512           # rows per statistics block of the kernels (fp32 partials inside a block, fp64 across)
+
+
+def _rows(z) -> np.ndarray:
+    z = np.asarray(z, np.float64)
+    return z.reshape(-1, z.shape[-1])
+
+
+def bn_train_fwd(z, gamma, beta, rm, rv, relu=False, eps=BN_EPS, momentum=BN_MOMENTUM):
+    """Train-mode BatchNorm1d over the rows of z [..., F] (F.batch_norm, training=True), optionally followed by ReLU.
+    Returns (y [z's shape], batch mean [F], biased batch variance [F], new running_mean, new running_var); the running
+    update uses the unbiased variance n / (n - 1) like nn.BatchNorm1d."""
+    zr = _rows(z)
+    n = zr.shape[0]
+    mean = zr.mean(axis=0)
+    var = ((zr - mean) ** 2).mean(axis=0)
+    y = (zr - mean) / np.sqrt(var + eps) * np.asarray(gamma, np.float64) + np.asarray(beta, np.float64)
+    if relu:
+        y = np.maximum(y, 0.0)
+    unbiased = var * n / (n - 1) if n > 1 else var
+    rm_new = (1 - momentum) * np.asarray(rm, np.float64) + momentum * mean
+    rv_new = (1 - momentum) * np.asarray(rv, np.float64) + momentum * unbiased
+    return y.reshape(np.shape(z)), mean, var, rm_new, rv_new
+
+
+def bn_eval_fwd(z, gamma, beta, rm, rv, relu=False, eps=BN_EPS):
+    """Eval-mode BatchNorm1d (running statistics) over the rows of z [..., F], optionally followed by ReLU."""
+    z = np.asarray(z, np.float64)
+    y = (z - rm) / np.sqrt(np.asarray(rv, np.float64) + eps) * gamma + np.asarray(beta, np.float64)
+    return np.maximum(y, 0.0) if relu else y
+
+
+def stat_allowance(n: int, F: int) -> float:
+    """Relative rounding allowance of one fp32 statistics sum (k_col_stats): a block of 256 threads splits into
+    rl = 256 / min(F, 256) row lanes, each sums <= ceil(STAT_ROWS / rl) rows in fp32, the lanes are added in fp32 and
+    the blocks in fp64 (exact at this precision); plus the rounding of z - K and of the square.  Same probabilistic
+    sqrt(m) u model as gamma()."""
+    rl = 256 // min(F, 256)
+    m = min(n, -(-STAT_ROWS // rl))
+    return LAMBDA * (math.sqrt(m) + math.sqrt(rl) + 2) * U32
+
+
+def bn_train_fwd_bound(z, E, gamma, beta, rm, rv, eps=BN_EPS, momentum=BN_MOMENTUM):
+    """Element-wise bound on the error of a train-mode BatchNorm (+ optional ReLU: 1-Lipschitz) computed from an fp32 z
+    whose every element is within E of the exact z (z: the float64 reference of the layer's pre-BN output).
+
+    First order, the error e of z moves y_i by gamma/sigma (e_i - mean(e) - zhat_i mean(zhat e)), sigma = sqrt(var +
+    eps); the local roundings are those of z's fp32 storage (u|z|, the floor of any fp32 implementation), of the
+    statistics summed around K = z[0] (stat_allowance), of scale = fp32(gamma invstd), shift = beta - mean scale and
+    of the fma(z, scale, shift).  Returns dict(y, mean, invstd, rm, rv) of bounds."""
+    zr = _rows(z)
+    n, F = zr.shape
+    Er = _rows(E) + U32 * np.abs(zr)
+    g, b = np.abs(np.asarray(gamma, np.float64)), np.abs(np.asarray(beta, np.float64))
+    mean = zr.mean(axis=0)
+    var = ((zr - mean) ** 2).mean(axis=0)
+    sig = np.sqrt(var + eps)
+    zh = np.abs(zr - mean) / sig
+    sc = g / sig
+    mE, mzE = Er.mean(axis=0), (zh * Er).mean(axis=0)
+    # local rounding of the statistics: S = sum (z - K), Q = sum (z - K)^2
+    a = stat_allowance(n, F)
+    d = zr - zr[0]
+    D, Q2 = np.abs(d).mean(axis=0), (d * d).mean(axis=0)
+    d_mean = a * D + U32 * np.abs(mean)
+    d_var_local = a * Q2 + 2 * np.abs(d.mean(axis=0)) * a * D
+    d_var = d_var_local + 2 * sig * mzE                  # + first order of e: 2 mean(|z - mean| E)
+    rel_is = d_var_local / (2 * sig ** 2) + 2 * U32
+    # scale: u gamma |zhat|; fp32 mean and mean * scale: 2 u |mean| scale; shift: u (|beta| + |mean| scale);
+    # fma: u |y| <= u (gamma |zhat| + |beta|)
+    ey = (sc * (Er + mE + zh * mzE) + sc * d_mean + g * zh * rel_is
+          + U32 * (2 * g * zh + 3 * sc * np.abs(mean) + 2 * b))
+    unb = n / (n - 1) if n > 1 else 1.0
+    e_rm = momentum * (mE + d_mean) + 4 * U32 * ((1 - momentum) * np.abs(rm) + momentum * np.abs(mean))
+    e_rv = momentum * unb * d_var + 4 * U32 * ((1 - momentum) * np.abs(rv) + momentum * unb * var)
+    e_is = (1 / sig) * (rel_is + mzE / sig)
+    return dict(y=ey.reshape(np.shape(z)), mean=mE + d_mean, invstd=e_is, rm=e_rm, rv=e_rv)
+
+
+def bn_eval_fwd_bound(z, E, gamma, beta, rm, rv, bias, eps=BN_EPS):
+    """Element-wise bound on eval-mode BatchNorm (+ optional ReLU) folded into the conv epilogue (k_bn_fold_eval;
+    on the tensor cores launch_rescaled_epilogue only multiplies scale by powers of two):
+        scale = gamma / sqrtf(rv + eps),  shift = beta + (bias - rm) scale,  y = fma(z - bias, scale, shift)
+    z: the float64 pre-BN conv output WITH bias, E: the conv's bound.  Roundings: three in scale, three in shift, the
+    epilogue's product and sum."""
+    zr = _rows(z)
+    sc = np.abs(np.asarray(gamma, np.float64)) / np.sqrt(np.asarray(rv, np.float64) + eps)
+    bias = np.asarray(bias, np.float64)
+    zb = np.abs(zr - bias)
+    bm = np.abs(bias - rm)
+    y = np.abs(bn_eval_fwd(zr, gamma, beta, rm, rv, eps=eps))
+    ey = sc * _rows(E) + U32 * (4 * zb * sc + 3 * bm * sc + 2 * np.abs(beta) + 2 * y)
+    return ey.reshape(np.shape(z))
+
+
 # --------------------------------------------------------------------------------------------- emulators (bound teeth)
 def _f16_split(v: np.ndarray):
     hi = v.astype(np.float16).astype(np.float64)
@@ -284,6 +381,59 @@ def emulate_cheb_conv(x, L, W, b=None, mode: str = "fp16x3", drop_block: int = -
     if b is not None:
         y = y + np.asarray(b, np.float64)
     return y.reshape(B, V, -1)
+
+
+BN_MUTATIONS = ("one_pass", "unbiased_in_norm", "biased_in_running", "eps_1e-3", "eps_outside_sqrt", "momentum_0.01",
+                "relu_before_affine")
+
+
+def emulate_bn_train(z, gamma, beta, rm, rv, relu=False, mutation: str = ""):
+    """What k_col_stats + k_bn_finalize + k_affine_act return for an fp32 z [..., F]: per block of STAT_ROWS rows and
+    row lane rr (rl = 256 / min(F, 256) lanes), an fp32 running sum of d = z - K and fma(d, d, q) with K = z[0] (the
+    shifted accumulation), the lanes added in fp32, the blocks in fp64; then mean = K + S/n, var = Q/n - (S/n)^2 in fp64,
+    invstd = fp32(1 / sqrt(var + eps)), scale = gamma invstd, shift = beta - fp32(mean) scale, y = fma(z, scale, shift).
+    `mutation` (one of BN_MUTATIONS) plants one defect.  Returns (y, mean, invstd, rm_new, rv_new) as float64."""
+    f32 = np.float32
+    zr = np.asarray(z, f32).reshape(-1, np.shape(z)[-1])
+    n, F = zr.shape
+    rl = 256 // min(F, 256)
+    K = np.zeros(F, f32) if mutation == "one_pass" else zr[0].copy()
+    S, Q = np.zeros(F), np.zeros(F)
+    for r0 in range(0, n, STAT_ROWS):
+        blk = zr[r0:r0 + STAT_ROWS]
+        s_l, q_l = np.zeros((rl, F), f32), np.zeros((rl, F), f32)
+        for i in range(0, blk.shape[0], rl):
+            v = (blk[i:i + rl] - K).astype(f32)
+            k = v.shape[0]
+            s_l[:k] = (s_l[:k] + v).astype(f32)
+            q_l[:k] = (v.astype(np.float64) * v + q_l[:k]).astype(f32)                # fma: one rounding
+        s, q = s_l[0].copy(), q_l[0].copy()
+        for j in range(1, rl):
+            s, q = (s + s_l[j]).astype(f32), (q + q_l[j]).astype(f32)
+        S, Q = S + s, Q + q
+    d = S / n
+    mean = K.astype(np.float64) + d
+    var = np.maximum(Q / n - d * d, 0.0)
+    unb = var * n / (n - 1) if n > 1 else var
+    eps = 1e-3 if mutation == "eps_1e-3" else BN_EPS
+    v_norm = unb if mutation == "unbiased_in_norm" else var
+    if mutation == "eps_outside_sqrt":
+        invstd = (1.0 / (np.sqrt(v_norm) + eps)).astype(f32)
+    else:
+        invstd = (1.0 / np.sqrt(v_norm + eps)).astype(f32)
+    mom = f32(0.01) if mutation == "momentum_0.01" else f32(0.1)
+    v_run = var if mutation == "biased_in_running" else unb
+    rm_new = (f32(1) - mom) * np.asarray(rm, f32) + mom * mean.astype(f32)
+    rv_new = (f32(1) - mom) * np.asarray(rv, f32) + mom * v_run.astype(f32)
+    sc = (np.asarray(gamma, f32) * invstd).astype(f32)
+    sh = (np.asarray(beta, f32) - (mean.astype(f32) * sc).astype(f32)).astype(f32)
+    if mutation == "relu_before_affine":
+        zr = np.maximum(zr, f32(0))
+    y = (zr.astype(np.float64) * sc + sh).astype(f32)
+    if relu and mutation != "relu_before_affine":
+        y = np.maximum(y, f32(0))
+    return (y.astype(np.float64).reshape(np.shape(z)), mean, invstd.astype(np.float64), rm_new.astype(np.float64),
+            rv_new.astype(np.float64))
 
 
 def bound_ratio(y, y64, bound) -> float:

@@ -101,6 +101,136 @@ def test_posenet_reference_matches_the_oracle():
     assert np.all(bound > 0)
 
 
+# ------------------------------------------------------------------------------------------------------ BatchNorm
+def _levels():
+    from helpers import graph_from_fixture
+
+    return {"joint17": graph_from_fixture("smpl_small")[0][-1], "joint21": graph_from_fixture("mano_like")[0][-1],
+            "v1088": graph_from_fixture("mano_like")[0][0]}
+
+
+def bn_layer(L, B, fin, fout, ratios, seed):
+    """A conv layer in front of a BatchNorm: channels of spread scale (sigma over ~2^5) whose conv bias carries
+    mean / sigma = ratios[f % len(ratios)] (a constant added in front of a train-mode BN cancels in exact arithmetic).
+    Returns (x, W, b, z64 [B, V, fout] float64 with the fp32 b, E = the fp32 conv's bound) and BN parameters."""
+    V = L.shape[0]
+    rng = np.random.default_rng(seed)
+    x = rng.standard_normal((B, V, fin)).astype(np.float32)
+    W = ((rng.random((fout, 3 * fin)) * 2 - 1) * np.sqrt(2 / (3 * fin + fout))
+         * 2.0 ** rng.uniform(-4, 1, (fout, 1))).astype(np.float32)
+    b = (rng.standard_normal(fout) * 0.1).astype(np.float32)
+    sig = R.cheb_conv_fwd(x, L, W, b).reshape(-1, fout).std(axis=0)
+    b = (b + np.resize(np.asarray(ratios, np.float64), fout) * sig).astype(np.float32)
+    bn = dict(gamma=((rng.random(fout) + 0.5) * rng.choice([-1, 1], fout)).astype(np.float32),
+              beta=(rng.standard_normal(fout) * 0.5).astype(np.float32),
+              rm=(rng.standard_normal(fout)).astype(np.float32), rv=(rng.random(fout) + 0.5).astype(np.float32))
+    return x, W, b, R.cheb_conv_fwd(x, L, W, b), R.cheb_conv_fwd_bound(x, L, W, b, "fp32"), bn
+
+
+def bn_ratios(got, z64, E, bn, relu):
+    """Error / bound of (y, mean, invstd, running_mean, running_var) from an emulation against float64."""
+    y64, mean, var, rm64, rv64 = R.bn_train_fwd(z64, bn["gamma"], bn["beta"], bn["rm"], bn["rv"], relu)
+    bd = R.bn_train_fwd_bound(z64, E, bn["gamma"], bn["beta"], bn["rm"], bn["rv"])
+    ref = (y64, mean, 1 / np.sqrt(var + R.BN_EPS), rm64, rv64)
+    return {k: R.bound_ratio(g, r, bd[k]) for k, g, r in zip(("y", "mean", "invstd", "rm", "rv"), got, ref)}
+
+
+BN_SHAPES = [("joint17", 1, 5, 32), ("joint17", 3, 64, 64), ("joint21", 2, 32, 64), ("joint21", 3, 64, 36),
+             ("v1088", 2, 64, 64), ("v1088", 1, 32, 300)]
+
+
+@pytest.mark.parametrize("lvl,B,fin,fout", BN_SHAPES, ids=lambda v: str(v))
+def test_bn_bound_accepts_the_shifted_statistics(lvl, B, fin, fout):
+    L = _levels()[lvl]
+    x, W, b, z64, E, bn = bn_layer(L, B, fin, fout, [0, 10, 100, 1000], seed=fin + fout + B)
+    for relu in (False, True):
+        got = R.emulate_bn_train(z64.astype(np.float32), bn["gamma"], bn["beta"], bn["rm"], bn["rv"], relu)
+        r = bn_ratios(got, z64, E, bn, relu)
+        assert max(r["mean"], r["invstd"]) <= 0.25, r
+        # y per channel group: at mean / sigma = 1000 its error is the fixed roundings of z's storage, fp32(mean),
+        # mean * scale and shift (~3 u |mean| scale against the bound's ~8 u), not a sum with statistical margin
+        y64, *_ = R.bn_train_fwd(z64, bn["gamma"], bn["beta"], bn["rm"], bn["rv"], relu)
+        by = R.bn_train_fwd_bound(z64, E, bn["gamma"], bn["beta"], bn["rm"], bn["rv"])["y"]
+        ry = (np.abs(got[0] - y64) / by).reshape(-1, fout).max(axis=0)
+        assert ry[0::4].max() <= 0.25 and ry[1::4].max() <= 0.25 and ry[2::4].max() <= 0.25, ry
+        assert ry[3::4].max() <= 0.5, ry
+        # the running updates are a few fixed fp32 roundings (0.9f, 0.1f, two products, a sum: <= ~2.5 u against the
+        # bound's 4 u), not a long sum: no statistical margin to ask for
+        assert max(r["rm"], r["rv"]) <= 0.7, r
+
+
+@pytest.mark.parametrize("ratio", [30, 100, 1000])
+def test_bn_bound_rejects_the_one_pass_variance(ratio):
+    """var = E[z^2] - mean^2 from fp32 partials cancels once |mean| >> sigma: at mean / sigma >= 30 the y it gives is
+    outside the bound on 2 x 1088 rows, while the shifted sums of the same z pass at every ratio."""
+    L = _levels()["v1088"]
+    x, W, b, z64, E, bn = bn_layer(L, 2, 64, 64, [ratio], seed=ratio)
+    z32 = z64.astype(np.float32)
+    args = (bn["gamma"], bn["beta"], bn["rm"], bn["rv"], False)
+    ok = bn_ratios(R.emulate_bn_train(z32, *args), z64, E, bn, False)
+    assert max(ok["mean"], ok["invstd"]) <= 0.25 and ok["y"] <= 0.5, ok
+    r = bn_ratios(R.emulate_bn_train(z32, *args, mutation="one_pass"), z64, E, bn, False)
+    assert r["y"] > 1.0, r
+
+
+# mutation -> the outputs of which at least one must leave the bound
+BN_TEETH = {"unbiased_in_norm": ("y", "invstd"), "biased_in_running": ("rv",), "eps_1e-3": ("y", "invstd"),
+            "eps_outside_sqrt": ("y", "invstd"), "momentum_0.01": ("rm", "rv"), "relu_before_affine": ("y",)}
+
+
+@pytest.mark.parametrize("mutation", sorted(BN_TEETH))
+@pytest.mark.parametrize("lvl,B", [("joint17", 1), ("joint21", 1), ("joint17", 3), ("joint21", 3)])
+def test_bn_bound_rejects_planted_defects(mutation, lvl, B):
+    """On the joint-graph levels (n = 17 ... 63 rows) a 1/n change (biased <-> unbiased variance) moves y by ~1/(2n),
+    far outside the bound; eps-outside-sqrt shows on the small-sigma channels the spread of scales provides."""
+    L = _levels()[lvl]
+    x, W, b, z64, E, bn = bn_layer(L, B, 64, 64, [0, 10], seed=B)
+    relu = mutation == "relu_before_affine"
+    got = R.emulate_bn_train(z64.astype(np.float32), bn["gamma"], bn["beta"], bn["rm"], bn["rv"], relu, mutation)
+    r = bn_ratios(got, z64, E, bn, relu)
+    assert max(r[k] for k in BN_TEETH[mutation]) > 1.0, r
+
+
+def test_bn_eval_bound_accepts_the_folded_affine():
+    """k_bn_fold_eval + the conv epilogue in fp32 (scale = gamma / sqrtf(rv + eps), shift = beta + (b - rm) scale,
+    y = fma(z - b, scale, shift)) within a quarter of the eval bound, with tiny and large running variances."""
+    L = _levels()["joint21"]
+    x, W, b, z64, E, bn = bn_layer(L, 3, 64, 64, [0, 10, 100, 1000], seed=4)
+    f32 = np.float32
+    rv = (np.resize([1e-8, 1e-3, 1.0, 1e4], 64) * (np.random.default_rng(5).random(64) + 0.5)).astype(f32)
+    rm = (z64.reshape(-1, 64).mean(axis=0) + np.random.default_rng(6).standard_normal(64)).astype(f32)
+    sc = (bn["gamma"] / np.sqrt((rv + f32(1e-5)).astype(f32)).astype(f32)).astype(f32)
+    sh = (bn["beta"] + ((b - rm).astype(f32) * sc).astype(f32)).astype(f32)
+    acc = (z64 - b.astype(np.float64)).astype(f32)
+    y = (acc.astype(np.float64) * sc + sh).astype(f32)
+    y64 = R.bn_eval_fwd(z64, bn["gamma"], bn["beta"], rm, rv)
+    bound = R.bn_eval_fwd_bound(z64, E, bn["gamma"], bn["beta"], rm, rv, b)
+    assert R.bound_ratio(y, y64, bound) <= 0.25
+    y_eps = (acc.astype(np.float64) * (bn["gamma"] / np.sqrt(rv + 1e-3)).astype(f32)
+             + (bn["beta"] + (b - rm) * (bn["gamma"] / np.sqrt(rv + 1e-3)))).astype(f32)
+    assert R.bound_ratio(y_eps, y64, bound) > 1.0
+
+
+def test_bn_backward_off_by_one_row_count_is_visible_at_17_rows():
+    """The network's BN backward g_z = gamma invstd (g - m1 - zhat m2), m1 = sum g / n, m2 = sum g zhat / n: with n - 1
+    in place of n, at the 17 rows of the joint level (B = 1), the gradient moves by far more than the 1e-3 of its
+    largest entry that the strict open-ReLU gradient parity allows."""
+    rng = np.random.default_rng(0)
+    z = torch.tensor(rng.standard_normal((17, 34)) * 2 + 3, requires_grad=True)
+    g = torch.tensor(rng.standard_normal((17, 34)))
+    gamma = torch.tensor(rng.random(34) + 0.5)
+    torch.nn.functional.batch_norm(z, None, None, gamma, None, True, 0.1, R.BN_EPS).backward(g)
+    zd = z.detach()
+    mean, var = zd.mean(0), zd.var(0, unbiased=False)
+    invstd = 1 / torch.sqrt(var + R.BN_EPS)
+    zh = (zd - mean) * invstd
+    ok = gamma * invstd * (g - g.mean(0) - zh * (g * zh).mean(0))
+    np.testing.assert_allclose(ok.numpy(), z.grad.numpy(), rtol=1e-10, atol=1e-12)
+    for m1, m2 in (((g.sum(0) / 16), (g * zh).mean(0)), (g.mean(0), (g * zh).sum(0) / 16)):
+        bad = gamma * invstd * (g - m1 - zh * m2)
+        assert float((bad - z.grad).abs().max() / z.grad.abs().max()) > 5e-3
+
+
 # ------------------------------------------------------------------------------------------------- graph families
 @pytest.mark.parametrize("name", sorted(G.FAMILIES))
 def test_graph_family_structure(name):
