@@ -12,7 +12,8 @@
  * Nothing here throws or aborts, and the library keeps no global mutable state (per-handle device
  * buffers and thread-local error / launch-count bookkeeping only), so one handle per device can be
  * driven from concurrent threads (nn.DataParallel, lib/core/base.py:108).  Entry points that touch
- * the device make the handle's device current for their own duration and restore the caller's.
+ * the device make the handle's device (without a handle: the data arrays' device) current for their
+ * own duration and restore the caller's.
  */
 #ifndef P2M_B200_H_
 #define P2M_B200_H_
@@ -192,6 +193,13 @@ typedef struct {
 int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* workspace, size_t workspace_bytes,
                       p2m_stream_t stream);
 
+/* ==== stateless entry points: from here to the body model, no function takes a handle ==================
+ * A call's data arrays (the device pointers of its signature: inputs, outputs, optional arrays and workspace) must be
+ * device memory of one device; NULL optional arrays are skipped.  Host-side tables (subsets, offsets, thresholds,
+ * learning-rate schedules, the PoseNet parameter struct) stay in host memory and are not data arrays.  The call runs on
+ * the data arrays' device, enqueued on `stream`, and restores the caller's current device.  A host pointer or arrays
+ * on two devices give P2M_ERR_INVALID before any device work.                                              */
+
 /* ---- the step in front of MeshNet (SURVEY.md §8 row f1) --------------------------------------------
  * FlatPose2Mesh.forward (lib/models/pose2mesh_net.py:16-22) in eval mode: PoseNet, the 2-D -> 3-D pose lifter
  * (lib/models/posenet.py:41-87: Linear(2J,H), `num_stage` residual stages of BN-ReLU-Linear(H,H)-BN-ReLU-Linear(H,H),
@@ -210,7 +218,7 @@ typedef struct {
   const p2m_posenet_stage_t* stages;           /* [num_stage] (host array of device pointers) */
 } p2m_posenet_params_t;
 size_t p2m_posenet_workspace_bytes(int batch, int hidden);
-/* pose2d [B, 2J] -> pose3d [B, 3J]; pose_combine (optional) [B, J, 5].  Enqueued on `stream` of the current device. */
+/* pose2d [B, 2J] -> pose3d [B, 3J]; pose_combine (optional) [B, J, 5]. */
 int p2m_posenet_forward(const p2m_posenet_params_t* params, const float* pose2d, float* pose3d, float* pose_combine,
                         int batch, void* workspace, size_t workspace_bytes, p2m_stream_t stream);
 
@@ -240,12 +248,11 @@ int p2m_coord_loss(const float* pred, const float* target, const float* valid, i
                    double* sum, float* grad_out, p2m_stream_t stream);
 
 /* ---- evaluation metrics (SURVEY.md §8 row f5; lib/coord_utils.py:127-149, the datasets' compute_*_err) ----------
- * Both take a batch of point sets pred/A, gt/B [batch, n_point, 3] (device, one device) and an optional subset of
- * point indices (HOST int32 [n_subset], checked here: every index in [0, n_point); NULL with n_subset = 0 = all
- * points; k = the number of points used).  Outputs are nullable, but at least one must be given.  sums (device
- * double [batch + 1]) receives the per-sample sums of the errors and, last, their total (fp64, fixed summation order:
- * a sample's values do not depend on its batch position).  Enqueued on `stream` of the inputs' device; the caller's
- * current device is restored.  batch and n_point are at most 2^24.
+ * Both take a batch of point sets pred/A, gt/B [batch, n_point, 3] and an optional subset of point indices (HOST
+ * int32 [n_subset], checked here: every index in [0, n_point); NULL with n_subset = 0 = all points; k = the number of
+ * points used).  Outputs are nullable, but at least one must be given.  sums (double [batch + 1]) receives the
+ * per-sample sums of the errors and, last, their total (fp64, fixed summation order: a sample's values do not depend
+ * on its batch position).  batch and n_point are at most 2^24.
  *
  * Similarity Procrustes of A[b, subset] onto B[b, subset] (rigid_transform_3D / rigid_align): fp64 centroids,
  * centred cross-covariance and 3x3 SVD; R = Vh^T U^T with the reference's det < 0 correction, c = sum(s) / varP,
@@ -294,9 +301,8 @@ int p2m_crop_cam_to_orig(const float* cam, const float* bbox, const float* img_w
 /* ---- temporal metrics (SURVEY.md §8 row f8; lib/smooth_utils.py:5-72, lib/coord_utils.py:194-222) ----------------
  * Ragged batches of sequences concatenated along frames: offsets (HOST int64 [n_seq + 1], checked here: offsets[0] = 0,
  * non-decreasing, offsets[n_seq] = n_frames >= 1; empty sequences allowed) are copied to the device with a
- * stream-ordered allocation.  dtype is P2M_DTYPE_F32 or P2M_DTYPE_F64 for every data array of a call; data arrays are
- * device memory of one device.  Enqueued on `stream`; no other host allocation or synchronisation.  A sequence's
- * results do not depend on its batch position.
+ * stream-ordered allocation.  dtype is P2M_DTYPE_F32 or P2M_DTYPE_F64 for every data array of a call.  No other host
+ * allocation or synchronisation.  A sequence's results do not depend on its batch position.
  *
  * One-Euro filter (smooth_pose, OneEuroFilter): y[f, c] for x [n_frames, n_channel], per sequence along its frames,
  * in numpy's dtype and operation order (bitwise the reference's result; t = frame index, dx0 = 0).  One launch.     */
@@ -322,8 +328,8 @@ int p2m_segment_mean(int dtype, const void* values, int64_t width, const int64_t
 /* ---- FreiHAND scores (SURVEY.md §8 row f9; the FreiHAND dataset's eval.py / utils/eval_util.py) ----------------
  * All arithmetic is fp64 on the inputs' values; a distance is sqrt((dx^2 + dy^2) + dz^2), each step rounded to
  * nearest.  Thresholds are HOST double arrays, checked here (finite, >= 0, sorted ascending) and passed to the kernels
- * by value.  Data arrays are device memory of one device; enqueued on `stream`, no host synchronisation.  Results
- * are bitwise deterministic and do not depend on a sample's batch position.
+ * by value.  No host synchronisation.  Results are bitwise deterministic and do not depend on a sample's batch
+ * position.
  *
  * Nearest distances between P [batch, n, 3] and Q [batch, m, 3] (dtype P2M_DTYPE_F32 or _F64 for both; n, m <= 2^20):
  * dist_p [batch, n] = min_j |P_i - Q_j|, dist_q [batch, m] = min_i |Q_j - P_i| (f64, equal to the brute force bit for
@@ -360,9 +366,9 @@ int p2m_pck_accumulate(const double* err, const float* pred, const float* gt, in
  * mesh coordinates, stored as floor(255 c + 0.5) into channel k.  Skipped: a triangle with a non-finite vertex or
  * camera value, a face index outside [0, n_vertex) or a vertex beyond +-2^20 px; a person whose image_index is outside
  * [0, n_image).  Optional outputs [n_image, height, width] (NULL = not written): face_map and person_map (int32, -1
- * where uncovered), depth_map (float32, NaN).  Limits: n_person, n_face <= 65535; height, width <= 16384.  Device
- * memory of one device; workspace >= p2m_render_workspace_bytes (8-byte aligned).  A memset and two launches on
- * `stream`, no host synchronisation, bitwise deterministic.                                                        */
+ * where uncovered), depth_map (float32, NaN).  Limits: n_person, n_face <= 65535; height, width <= 16384.
+ * workspace >= p2m_render_workspace_bytes (8-byte aligned).  A memset and two launches, no host synchronisation,
+ * bitwise deterministic.                                                                                           */
 size_t p2m_render_workspace_bytes(int n_image, int height, int width);
 int p2m_render_meshes(const float* verts, int n_person, int n_vertex, const int32_t* faces, int n_face,
                       const float* cams, const float* colors, const int32_t* image_index, const uint8_t* images_in,

@@ -9,6 +9,8 @@ import ctypes as C
 import os
 import threading
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libp2m_b200.so")
 
@@ -269,3 +271,19 @@ def check(status: int, what: str = "p2m call"):
     if status != 0:
         msg = load().p2m_last_error().decode("utf-8", "replace")
         raise RuntimeError(f"{what} failed (status {status}): {msg}")
+
+
+def call(name: str, device, *args):
+    """Run entry point `name` on `args` (a tensor is passed as its data pointer) with the current stream of `device`
+    as the last argument, which every stream-taking entry point has; raise RuntimeError if it fails.  The library
+    picks the device to run on itself (the handle's, or the data arrays'), so no device context is needed here."""
+    fn = getattr(load(), name)
+    ptrs = (a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args)
+    check(fn(*ptrs, torch.cuda.current_stream(device).cuda_stream), name)
+
+
+def cuda_tensor(x, what: str) -> torch.Tensor:
+    """x, if it is a CUDA tensor: there is no CPU path."""
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
+    return x

@@ -146,8 +146,7 @@ class _BodyModel(Module):
 
     def _prepare(self, pose, betas, trans, pose_width):
         """Check and normalise the inputs (torch ops only, so autograd follows them): -> pose, betas, trans, centre."""
-        if not isinstance(pose, torch.Tensor) or not pose.is_cuda:
-            raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; the pose is not a CUDA tensor")
+        _lib.cuda_tensor(pose, "the pose")
         if pose.dim() != 2 or pose.shape[1] != pose_width or pose.shape[0] == 0:
             raise ValueError(f"pose must be [B, {pose_width}] with B > 0; got {tuple(pose.shape)}")
         B, dev = pose.shape[0], pose.device
@@ -189,11 +188,8 @@ class _BodyModel(Module):
         joints = torch.empty((B, self.n_out_joints, 3), device=dev, dtype=torch.float32)
         nbytes = lib.p2m_body_model_workspace_bytes(h, B)
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_body_model_forward(h, pose.data_ptr(), _ptr(betas), betas_rule, _ptr(trans), center,
-                                                  verts.data_ptr(), joints.data_ptr(), B, ws.data_ptr(), nbytes,
-                                                  torch.cuda.current_stream(dev).cuda_stream),
-                       "p2m_body_model_forward")
+        _lib.call("p2m_body_model_forward", dev, h, pose, betas, betas_rule, trans, center, verts, joints, B, ws,
+                  nbytes)
         return verts, joints
 
     def _backward_native(self, pose, betas, trans, betas_rule, center, grad_verts, grad_joints, want_betas,
@@ -208,12 +204,8 @@ class _BodyModel(Module):
         grad_trans = torch.empty_like(trans) if want_trans and trans is not None else None
         nbytes = lib.p2m_body_model_backward_workspace_bytes(h, B)
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_body_model_backward(h, pose.data_ptr(), _ptr(betas), betas_rule, _ptr(trans), center,
-                                                   _ptr(grad_verts), _ptr(grad_joints), grad_pose.data_ptr(),
-                                                   _ptr(grad_betas), _ptr(grad_trans), B, ws.data_ptr(), nbytes,
-                                                   torch.cuda.current_stream(dev).cuda_stream),
-                       "p2m_body_model_backward")
+        _lib.call("p2m_body_model_backward", dev, h, pose, betas, betas_rule, trans, center, grad_verts, grad_joints,
+                  grad_pose, grad_betas, grad_trans, B, ws, nbytes)
         return grad_pose, grad_betas, grad_trans
 
     def _run(self, pose, betas, trans, betas_rule, pose_width):
@@ -221,10 +213,6 @@ class _BodyModel(Module):
         if self.differentiable:
             return _BodyModelFunction.apply(self, betas_rule, center, pose, betas, trans)
         return self._forward_native(pose, betas, trans, betas_rule, center)
-
-
-def _ptr(t):
-    return t.data_ptr() if t is not None else None
 
 
 class _BodyModelFunction(torch.autograd.Function):

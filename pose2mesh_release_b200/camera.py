@@ -23,8 +23,7 @@ N_ITER = 1500
 
 
 def _cuda(x, what: str) -> torch.Tensor:
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
+    _lib.cuda_tensor(x, what)
     if x.requires_grad:
         raise ValueError(f"{what} requires grad; the camera fit is not differentiable")
     return x
@@ -97,12 +96,8 @@ def fit_cameras(joints_px: torch.Tensor, pred_joints3d: torch.Tensor, crop_size:
     if image_size is not None:
         wh = _image_sizes(image_size, B, dev)
         orig = out["orig_cam"] = torch.empty((B, 4), device=dev, dtype=torch.float32)
-    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().p2m_fit_camera(
-            x.data_ptr(), cols, kind, n_in, p3.data_ptr(), J, init.data_ptr(), B, int(crop_size), int(n_iter), steps,
-            rates, len(phases), ptr(wh), out["cam_param"].data_ptr(), out["bbox"].data_ptr(), out["target"].data_ptr(),
-            out["loss"].data_ptr(), ptr(orig), torch.cuda.current_stream(dev).cuda_stream), "p2m_fit_camera")
+    _lib.call("p2m_fit_camera", dev, x, cols, kind, n_in, p3, J, init, B, int(crop_size), int(n_iter), steps, rates,
+              len(phases), wh, out["cam_param"], out["bbox"], out["target"], out["loss"], orig)
     if squeeze:
         out = {k: v[0] for k, v in out.items()}
     return out
@@ -122,8 +117,5 @@ def convert_crop_cam_to_orig_img(cam: torch.Tensor, bbox: torch.Tensor, img_widt
     h = torch.as_tensor(img_height, dtype=torch.float32).to(cam.device).reshape(-1).expand(B)
     wh = torch.stack([w, h], 1).contiguous()
     out = torch.empty((B, 4), device=cam.device, dtype=torch.float32)
-    with torch.cuda.device(cam.device):
-        _lib.check(_lib.load().p2m_crop_cam_to_orig(cam.data_ptr(), bbox.data_ptr(), wh.data_ptr(), B, out.data_ptr(),
-                                                    torch.cuda.current_stream(cam.device).cuda_stream),
-                   "p2m_crop_cam_to_orig")
+    _lib.call("p2m_crop_cam_to_orig", cam.device, cam, bbox, wh, B, out)
     return out[0] if squeeze else out

@@ -130,9 +130,7 @@ class ChebConvLinear(torch.autograd.Function):
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
         a = _lib.ConvFwdArgs(level=0, batch=B, fin=fin, fout=fout, x=x.data_ptr(), weight=weight.data_ptr(),
                              bias=bias.data_ptr(), bn_mode=0, relu=0, y=y.data_ptr())
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_cheb_conv_fwd(h, C.byref(a), ws.data_ptr(), nbytes,
-                                             torch.cuda.current_stream(dev).cuda_stream), "p2m_cheb_conv_fwd")
+        _lib.call("p2m_cheb_conv_fwd", dev, h, C.byref(a), ws, nbytes)
         ctx.gh = gh
         ctx.save_for_backward(x, weight)
         return y
@@ -155,9 +153,7 @@ class ChebConvLinear(torch.autograd.Function):
         a = _lib.ConvBwdArgs(level=0, batch=B, fin=fin, fout=fout, x=x.data_ptr(), weight=weight.data_ptr(),
                              dz=dz.data_ptr(), dx=None if dx is None else dx.data_ptr(), dweight=dw.data_ptr(),
                              dbias=db.data_ptr())
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_cheb_conv_bwd(h, C.byref(a), ws.data_ptr(), nbytes,
-                                             torch.cuda.current_stream(dev).cuda_stream), "p2m_cheb_conv_bwd")
+        _lib.call("p2m_cheb_conv_bwd", dev, h, C.byref(a), ws, nbytes)
         return dx, dw, db, None
 
 

@@ -314,18 +314,6 @@ __global__ void __launch_bounds__(128) k_crop_cam_to_orig(const float* __restric
     crop_cam_to_orig(cam + b * 3, bbox + b * 4, img_wh[b * 2 + 0], img_wh[b * 2 + 1], true, out + b * 4);
 }
 
-int device_of(const void* p, int* dev) {
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, p) != cudaSuccess ||
-      (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
-    cudaGetLastError();
-    set_error("fit_camera / crop_cam_to_orig: the arrays must be device memory");
-    return P2M_ERR_INVALID;
-  }
-  *dev = attr.device;
-  return P2M_OK;
-}
-
 }  // namespace
 }  // namespace p2m
 
@@ -365,10 +353,10 @@ int p2m_fit_camera(const double* joints_px, int in_cols, int in_kind, int n_in_j
     sched.lr[i] = lr_values[i];
   }
   int dev;
-  P2M_TRY(device_of(joints_px, &dev));
+  P2M_TRY(arrays_device("fit_camera", {joints_px, pred_joints3d, init_cam, img_wh, cam, bbox, target, loss, orig_cam},
+                        &dev));
   DeviceGuard guard(dev);
-  const long long ctas = ((long long)batch + WARPS - 1) / WARPS;
-  k_fit_camera<<<(unsigned)(ctas < MAX_GRID ? ctas : MAX_GRID), WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+  k_fit_camera<<<grid_for(batch, WARPS, MAX_GRID), WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(
       joints_px, in_cols, in_kind, n_in_joint, pred_joints3d, n_joint, init_cam, batch, crop, n_iter, sched, img_wh,
       cam, bbox, target, loss, orig_cam);
   P2M_LAUNCH_OK();
@@ -382,10 +370,9 @@ int p2m_crop_cam_to_orig(const float* cam, const float* bbox, const float* img_w
     return P2M_ERR_INVALID;
   }
   int dev;
-  P2M_TRY(device_of(cam, &dev));
+  P2M_TRY(arrays_device("crop_cam_to_orig", {cam, bbox, img_wh, orig_cam}, &dev));
   DeviceGuard guard(dev);
-  const long long ctas = ((long long)batch + 127) / 128;
-  k_crop_cam_to_orig<<<(unsigned)(ctas < MAX_GRID ? ctas : MAX_GRID), 128, 0, static_cast<cudaStream_t>(stream)>>>(
+  k_crop_cam_to_orig<<<grid_for(batch, 128, MAX_GRID), 128, 0, static_cast<cudaStream_t>(stream)>>>(
       cam, bbox, img_wh, batch, orig_cam);
   P2M_LAUNCH_OK();
   return P2M_OK;

@@ -310,30 +310,6 @@ __global__ void __launch_bounds__(PT) k_pck_hist(const double* __restrict__ err,
 }
 
 // ---------------------------------------------------------------- host helpers
-int device_of(const char* where, const void* p, int* dev) {
-  cudaPointerAttributes attr;
-  if (!p || cudaPointerGetAttributes(&attr, p) != cudaSuccess ||
-      (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
-    cudaGetLastError();
-    set_error(std::string(where) + ": the point arrays must be device memory");
-    return P2M_ERR_INVALID;
-  }
-  *dev = attr.device;
-  return P2M_OK;
-}
-
-int same_device(const char* where, const void* a, const void* b, int* dev) {
-  int da, db;
-  P2M_TRY(device_of(where, a, &da));
-  P2M_TRY(device_of(where, b, &db));
-  if (da != db) {
-    set_error(std::string(where) + ": the point arrays are on different devices");
-    return P2M_ERR_INVALID;
-  }
-  *dev = da;
-  return P2M_OK;
-}
-
 // Host thresholds: 1 .. max_n values, finite, >= 0, non-decreasing.
 int load_thresholds(const char* where, const double* t, int n, int max_n, Thresholds* th) {
   if (!t || n <= 0 || n > max_n) {
@@ -353,27 +329,12 @@ int load_thresholds(const char* where, const double* t, int n, int max_n, Thresh
   return P2M_OK;
 }
 
-inline unsigned grid_for(long long work) { return (unsigned)(work < MAX_GRID ? (work > 0 ? work : 1) : MAX_GRID); }
-
-struct DevScratch {
-  void* ptr = nullptr;
-  cudaStream_t s;
-  explicit DevScratch(cudaStream_t st) : s(st) {}
-  int alloc(size_t bytes) {
-    P2M_CUDA_OK(cudaMallocAsync(&ptr, bytes, s));
-    return P2M_OK;
-  }
-  ~DevScratch() {
-    if (ptr) cudaFreeAsync(ptr, s);
-  }
-};
-
 template <typename T>
 int nearest_launch(const T* P, const T* Q, int batch, int n, int m, const Thresholds& th, unsigned long long* min_p,
                    unsigned long long* min_q, double* dist_p, double* dist_q, long long* counts, double* frac,
                    double* fscore, int dev, cudaStream_t s) {
-  k_fill_inf<<<grid_for(((long long)batch * (n + m) + NT - 1) / NT), NT, 0, s>>>(min_p, (long long)batch * n, min_q,
-                                                                                 (long long)batch * m);
+  k_fill_inf<<<grid_for((long long)batch * (n + m), NT, MAX_GRID), NT, 0, s>>>(min_p, (long long)batch * n, min_q,
+                                                                               (long long)batch * m);
   P2M_LAUNCH_OK();
   // Split a sample's column tiles over CTAs until the grid holds about four CTAs per SM (B = 1 at SMPL size still
   // fills the GPU); the minima do not depend on the split.
@@ -384,12 +345,11 @@ int nearest_launch(const T* P, const T* Q, int batch, int n, int m, const Thresh
   int splits = (int)std::min<long long>(col_tiles, std::max<long long>(1, (4LL * sms + base - 1) / base));
   const int tps = (col_tiles + splits - 1) / splits;
   splits = (col_tiles + tps - 1) / tps;
-  const long long work = base * splits;
-  const unsigned grid = (unsigned)std::min<long long>(work, 1LL << 30);
-  k_nearest_sweep<T><<<grid, NT, 0, s>>>(P, Q, batch, n, m, row_tiles, splits, tps, min_p, min_q);
+  k_nearest_sweep<T><<<grid_for(base * splits, 1, 1LL << 30), NT, 0, s>>>(P, Q, batch, n, m, row_tiles, splits, tps,
+                                                                          min_p, min_q);
   P2M_LAUNCH_OK();
-  k_nearest_finish<T><<<grid_for(batch), NT, 0, s>>>(P, Q, batch, n, m, min_p, min_q, th, dist_p, dist_q, counts, frac,
-                                                    fscore);
+  k_nearest_finish<T><<<grid_for(batch, 1, MAX_GRID), NT, 0, s>>>(P, Q, batch, n, m, min_p, min_q, th, dist_p, dist_q,
+                                                                  counts, frac, fscore);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -404,10 +364,10 @@ extern "C" {
 int p2m_nearest_distances(int dtype, const void* P, const void* Q, int batch, int n, int m, const double* thresholds,
                           int n_thr, double* dist_p, double* dist_q, int64_t* counts, double* frac, double* fscore,
                           p2m_stream_t stream) {
-  if ((dtype != P2M_DTYPE_F32 && dtype != P2M_DTYPE_F64) || batch <= 0 || batch > MAX_BATCH || n <= 0 ||
+  if ((dtype != P2M_DTYPE_F32 && dtype != P2M_DTYPE_F64) || !P || !Q || batch <= 0 || batch > MAX_BATCH || n <= 0 ||
       n > MAX_POINTS || m <= 0 || m > MAX_POINTS || !(dist_p || dist_q || counts || frac || fscore)) {
-    set_error("nearest_distances: bad argument (dtype code, batch outside [1, 2^24], n or m outside [1, 2^20], or no "
-              "output)");
+    set_error("nearest_distances: bad argument (dtype code, null point array, batch outside [1, 2^24], n or m outside "
+              "[1, 2^20], or no output)");
     return P2M_ERR_INVALID;
   }
   if (n_thr < 0 || n_thr > MAX_F_THR || (n_thr == 0) != (thresholds == nullptr) ||
@@ -418,20 +378,20 @@ int p2m_nearest_distances(int dtype, const void* P, const void* Q, int batch, in
   Thresholds th{};
   if (n_thr > 0) P2M_TRY(load_thresholds("nearest_distances", thresholds, n_thr, MAX_F_THR, &th));
   int dev;
-  P2M_TRY(same_device("nearest_distances", P, Q, &dev));
+  P2M_TRY(arrays_device("nearest_distances", {P, Q, dist_p, dist_q, counts, frac, fscore}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   // the distance outputs double as the minima's bit store; a missing one gets stream-ordered scratch
-  DevScratch sp(s), sq(s);
+  StreamBuffer<unsigned long long> sp(s), sq(s);
   unsigned long long* min_p = reinterpret_cast<unsigned long long*>(dist_p);
   unsigned long long* min_q = reinterpret_cast<unsigned long long*>(dist_q);
   if (!min_p) {
-    P2M_TRY(sp.alloc(sizeof(double) * (size_t)batch * n));
-    min_p = static_cast<unsigned long long*>(sp.ptr);
+    P2M_TRY(sp.alloc((size_t)batch * n));
+    min_p = sp.ptr;
   }
   if (!min_q) {
-    P2M_TRY(sq.alloc(sizeof(double) * (size_t)batch * m));
-    min_q = static_cast<unsigned long long*>(sq.ptr);
+    P2M_TRY(sq.alloc((size_t)batch * m));
+    min_q = sq.ptr;
   }
   long long* cnt = reinterpret_cast<long long*>(counts);
   if (dtype == P2M_DTYPE_F32)
@@ -443,16 +403,17 @@ int p2m_nearest_distances(int dtype, const void* P, const void* Q, int batch, in
 
 int p2m_align_w_scale(const float* gt, const float* pred, int batch, int n_point, int aligned_dtype, void* aligned,
                       double* err, p2m_stream_t stream) {
-  if (batch <= 0 || batch > MAX_BATCH || n_point <= 0 || n_point > MAX_PCK_POINTS || !(aligned || err) ||
-      (aligned && aligned_dtype != P2M_DTYPE_F32 && aligned_dtype != P2M_DTYPE_F64)) {
-    set_error("align_w_scale: bad argument (batch or n_point outside [1, 2^24], no output, or bad aligned dtype)");
+  if (!gt || !pred || batch <= 0 || batch > MAX_BATCH || n_point <= 0 || n_point > MAX_PCK_POINTS ||
+      !(aligned || err) || (aligned && aligned_dtype != P2M_DTYPE_F32 && aligned_dtype != P2M_DTYPE_F64)) {
+    set_error("align_w_scale: bad argument (null point array, batch or n_point outside [1, 2^24], no output, or bad "
+              "aligned dtype)");
     return P2M_ERR_INVALID;
   }
   int dev;
-  P2M_TRY(same_device("align_w_scale", gt, pred, &dev));
+  P2M_TRY(arrays_device("align_w_scale", {gt, pred, aligned, err}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const unsigned grid = (unsigned)std::min(batch, 4096);
+  const unsigned grid = grid_for(batch, 1, 4096);
   if (aligned && aligned_dtype == P2M_DTYPE_F64)
     k_align_w_scale<double><<<grid, AT, 0, s>>>(gt, pred, batch, n_point, static_cast<double*>(aligned), err);
   else
@@ -472,12 +433,11 @@ int p2m_pck_accumulate(const double* err, const float* pred, const float* gt, in
   Thresholds th{};
   P2M_TRY(load_thresholds("pck_accumulate", thresholds, n_thr, MAX_THR, &th));
   int dev;
-  if (err) P2M_TRY(same_device("pck_accumulate", err, hist, &dev));
-  else P2M_TRY(same_device("pck_accumulate", pred, gt, &dev));
+  P2M_TRY(arrays_device("pck_accumulate", {err, pred, gt, err_out, hist}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const unsigned grid = (unsigned)std::min<long long>((n_val + PT - 1) / PT, 1024);
-  k_pck_hist<<<grid, PT, 0, s>>>(err, pred, gt, n_val, th, err_out, reinterpret_cast<unsigned long long*>(hist));
+  k_pck_hist<<<grid_for(n_val, PT, 1024), PT, 0, s>>>(err, pred, gt, n_val, th, err_out,
+                                                      reinterpret_cast<unsigned long long*>(hist));
   P2M_LAUNCH_OK();
   return P2M_OK;
 }

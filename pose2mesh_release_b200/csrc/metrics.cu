@@ -184,28 +184,6 @@ __global__ void __launch_bounds__(MT) k_batch_total(double* __restrict__ sums, i
   if (threadIdx.x == 0) sums[batch] = s[0];
 }
 
-// The device of the input arrays (both must be device memory of one device).
-int input_device(const char* where, const float* a, const float* b, int* dev) {
-  int devs[2];
-  const float* ptrs[2] = {a, b};
-  for (int i = 0; i < 2; ++i) {
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, ptrs[i]) != cudaSuccess ||
-        (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
-      cudaGetLastError();
-      set_error(std::string(where) + ": the point arrays must be device memory");
-      return P2M_ERR_INVALID;
-    }
-    devs[i] = attr.device;
-  }
-  if (devs[0] != devs[1]) {
-    set_error(std::string(where) + ": the point arrays are on different devices");
-    return P2M_ERR_INVALID;
-  }
-  *dev = devs[0];
-  return P2M_OK;
-}
-
 // Shared argument checks; the subset indices come from the caller and are checked here, on the host.
 int check_args(const char* where, const float* a, const float* b, int batch, int n_point, const int32_t* subset,
                int n_subset, bool any_output) {
@@ -224,24 +202,6 @@ int check_args(const char* where, const float* a, const float* b, int batch, int
   return P2M_OK;
 }
 
-// Stream-ordered device copy of the (host) subset, freed on the same stream after the kernels that read it.
-struct DevSubset {
-  int* ptr = nullptr;
-  cudaStream_t s;
-  explicit DevSubset(cudaStream_t st) : s(st) {}
-  int upload(const int32_t* host, int n) {
-    if (n == 0) return P2M_OK;
-    P2M_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ptr), sizeof(int) * (size_t)n, s));
-    P2M_CUDA_OK(cudaMemcpyAsync(ptr, host, sizeof(int) * (size_t)n, cudaMemcpyHostToDevice, s));
-    return P2M_OK;
-  }
-  ~DevSubset() {
-    if (ptr) cudaFreeAsync(ptr, s);
-  }
-};
-
-inline unsigned grid_for(int batch) { return (unsigned)(batch < MAX_GRID ? batch : MAX_GRID); }
-
 }  // namespace
 }  // namespace p2m
 
@@ -253,13 +213,14 @@ int p2m_rigid_align(const float* A, const float* B, int batch, int n_point, cons
                     double* transform, float* aligned, float* err, double* sums, p2m_stream_t stream) {
   P2M_TRY(check_args("rigid_align", A, B, batch, n_point, subset, n_subset, transform || aligned || err || sums));
   int dev;
-  P2M_TRY(input_device("rigid_align", A, B, &dev));
+  P2M_TRY(arrays_device("rigid_align", {A, B, transform, aligned, err, sums}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  DevSubset sub(s);
-  P2M_TRY(sub.upload(subset, n_subset));
+  StreamBuffer<int> sub(s);
+  P2M_TRY(sub.alloc(n_subset, subset));
   const int k = n_subset > 0 ? n_subset : n_point;
-  k_rigid_align<<<grid_for(batch), MT, 0, s>>>(A, B, batch, n_point, sub.ptr, k, transform, aligned, err, sums);
+  k_rigid_align<<<grid_for(batch, 1, MAX_GRID), MT, 0, s>>>(A, B, batch, n_point, sub.ptr, k, transform, aligned, err,
+                                                            sums);
   P2M_LAUNCH_OK();
   if (sums) {
     k_batch_total<<<1, MT, 0, s>>>(sums, batch);
@@ -277,16 +238,17 @@ int p2m_point_errors(const float* pred, const float* gt, const float* pred_root,
     return P2M_ERR_INVALID;
   }
   int dev;
-  P2M_TRY(input_device("point_errors", pred, gt, &dev));
+  P2M_TRY(arrays_device("point_errors", {pred, gt, pred_root, gt_root, err, sums}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  DevSubset sub(s);
-  P2M_TRY(sub.upload(subset, n_subset));
+  StreamBuffer<int> sub(s);
+  P2M_TRY(sub.alloc(n_subset, subset));
   const int k = n_subset > 0 ? n_subset : n_point;
+  const unsigned grid = grid_for(batch, 1, MAX_GRID);
   if (fp64)
-    k_point_errors<true><<<grid_for(batch), MT, 0, s>>>(pred, gt, pred_root, gt_root, batch, n_point, sub.ptr, k, err, sums);
+    k_point_errors<true><<<grid, MT, 0, s>>>(pred, gt, pred_root, gt_root, batch, n_point, sub.ptr, k, err, sums);
   else
-    k_point_errors<false><<<grid_for(batch), MT, 0, s>>>(pred, gt, pred_root, gt_root, batch, n_point, sub.ptr, k, err, sums);
+    k_point_errors<false><<<grid, MT, 0, s>>>(pred, gt, pred_root, gt_root, batch, n_point, sub.ptr, k, err, sums);
   P2M_LAUNCH_OK();
   if (sums) {
     k_batch_total<<<1, MT, 0, s>>>(sums, batch);

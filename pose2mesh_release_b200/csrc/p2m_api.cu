@@ -19,6 +19,31 @@ static thread_local int64_t g_launches = 0;
 void set_error(const std::string& msg) { g_error = msg; }
 void count_launch(int n) { g_launches += n; }
 
+int arrays_device(const char* where, std::initializer_list<const void*> arrays, int* dev) {
+  int found = -1;
+  for (const void* p : arrays) {
+    if (!p) continue;
+    cudaPointerAttributes attr;
+    if (cudaPointerGetAttributes(&attr, p) != cudaSuccess ||
+        (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
+      cudaGetLastError();
+      set_error(std::string(where) + ": the data arrays must be device memory");
+      return P2M_ERR_INVALID;
+    }
+    if (found >= 0 && attr.device != found) {
+      set_error(std::string(where) + ": the data arrays are on different devices");
+      return P2M_ERR_INVALID;
+    }
+    found = attr.device;
+  }
+  if (found < 0) {
+    set_error(std::string(where) + ": no data array given");
+    return P2M_ERR_INVALID;
+  }
+  *dev = found;
+  return P2M_OK;
+}
+
 struct Layer {
   int level, V, fin, fout;
   int bn, relu;
@@ -1492,6 +1517,9 @@ int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, floa
     set_error("posenet_forward: workspace too small");
     return P2M_ERR_WORKSPACE;
   }
+  int dev;
+  P2M_TRY(arrays_device("posenet_forward", {pose2d, pose3d, pose_combine, workspace}, &dev));
+  DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int H = P->hidden, J = P->num_joint;
   Bump b(workspace);
@@ -1507,8 +1535,6 @@ int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, floa
   void* wpack = tc ? b.take<unsigned char>(umma_gemm_wpack_bytes(H, H)) : nullptr;
   int sm_count = 132;
   if (tc) {
-    int dev = 0;
-    P2M_CUDA_OK(cudaGetDevice(&dev));
     P2M_CUDA_OK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
     P2M_CUDA_OK(cudaMemsetAsync(status, 0, sizeof(int), s));
   }
@@ -1672,6 +1698,9 @@ int p2m_regress_joints(const float* joint_regressor, const float* vertices, floa
     set_error("regress_joints: bad argument");
     return P2M_ERR_INVALID;
   }
+  int dev;
+  P2M_TRY(arrays_device("regress_joints", {joint_regressor, vertices, joints}, &dev));
+  DeviceGuard guard(dev);
   k_regress_joints<<<dim3(n_joint, batch), 256, 0, static_cast<cudaStream_t>(stream)>>>(joint_regressor, vertices,
                                                                                        n_vertex, chans, joints);
   P2M_LAUNCH_OK();
@@ -1684,6 +1713,9 @@ int p2m_normalize_pose2d(const float* joints_px, float* pose2d, int batch, int n
     set_error("normalize_pose2d: bad argument (at most 32 joints)");
     return P2M_ERR_INVALID;
   }
+  int dev;
+  P2M_TRY(arrays_device("normalize_pose2d", {joints_px, pose2d}, &dev));
+  DeviceGuard guard(dev);
   k_normalize_pose2d<<<(batch + 3) / 4, 128, 0, static_cast<cudaStream_t>(stream)>>>(joints_px, batch, n_joint, input_h,
                                                                                    input_w, truncate_like_int_input, pose2d);
   P2M_LAUNCH_OK();
@@ -1828,6 +1860,9 @@ int p2m_mesh_losses(const float* coord_out, const float* coord_gt, const int32_t
     set_error("mesh_losses: bad argument");
     return P2M_ERR_INVALID;
   }
+  int dev;
+  P2M_TRY(arrays_device("mesh_losses", {coord_out, coord_gt, faces, grad_scale, sums, grad_out}, &dev));
+  DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   P2M_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
   if (grad_out) P2M_CUDA_OK(cudaMemsetAsync(grad_out, 0, sizeof(float) * 3 * (size_t)batch * n_vertex, s));
@@ -1844,6 +1879,9 @@ int p2m_coord_loss(const float* pred, const float* target, const float* valid, i
     set_error("coord_loss: bad argument");
     return P2M_ERR_INVALID;
   }
+  int dev;
+  P2M_TRY(arrays_device("coord_loss", {pred, target, valid, grad_scale, sum, grad_out}, &dev));
+  DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   P2M_CUDA_OK(cudaMemsetAsync(sum, 0, sizeof(double), s));
   k_coord_loss<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(pred, target, valid, n, grad_scale, sum, grad_out);

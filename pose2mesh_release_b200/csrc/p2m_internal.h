@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -41,7 +42,8 @@ void count_launch(int n = 1);
     if (_s != P2M_OK) return _s; \
   } while (0)
 
-// Every entry point that touches the device makes the model's device current for its own duration only: the
+// Every entry point that touches the device makes its device (the handle's, or for a stateless entry point the one
+// arrays_device finds) current for its own duration only: the
 // caller's current device is restored on every exit path (single-process multi-GPU callers, nn.DataParallel
 // threads, handles garbage-collected at arbitrary times).
 struct DeviceGuard {
@@ -57,6 +59,37 @@ struct DeviceGuard {
   DeviceGuard(const DeviceGuard&) = delete;
   DeviceGuard& operator=(const DeviceGuard&) = delete;
 };
+
+// The device a stateless entry point (one without a handle) runs on.  `arrays` are the call's data arrays: inputs,
+// outputs, optional arrays and workspace, not host-side tables.  Null entries are skipped; every other entry must be
+// device or managed memory, all of one device, which is stored to *dev.  Otherwise P2M_ERR_INVALID, naming `where`.
+int arrays_device(const char* where, std::initializer_list<const void*> arrays, int* dev);
+
+// n elements of T allocated on stream s (cudaMallocAsync), optionally filled from host memory, and freed on the same
+// stream at scope exit, i.e. after the kernels enqueued in between.  n == 0 allocates nothing and leaves ptr null.
+template <typename T>
+struct StreamBuffer {
+  T* ptr = nullptr;
+  cudaStream_t s;
+  explicit StreamBuffer(cudaStream_t st) : s(st) {}
+  int alloc(size_t n, const void* host = nullptr) {
+    if (n == 0) return P2M_OK;
+    P2M_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ptr), sizeof(T) * n, s));
+    if (host) P2M_CUDA_OK(cudaMemcpyAsync(ptr, host, sizeof(T) * n, cudaMemcpyHostToDevice, s));
+    return P2M_OK;
+  }
+  ~StreamBuffer() {
+    if (ptr) cudaFreeAsync(ptr, s);
+  }
+  StreamBuffer(const StreamBuffer&) = delete;
+  StreamBuffer& operator=(const StreamBuffer&) = delete;
+};
+
+// CTAs of a grid-stride launch: ceil(work / per_cta), clamped to [1, max_ctas].
+inline unsigned grid_for(long long work, int per_cta, long long max_ctas) {
+  const long long g = (work + per_cta - 1) / per_cta;
+  return (unsigned)(g < 1 ? 1 : (g < max_ctas ? g : max_ctas));
+}
 
 // ---------------------------------------------------------------- device-resident hierarchy level
 // L~ of one level in CSR with RELATIVE column offsets: the neighbour of flat activation row

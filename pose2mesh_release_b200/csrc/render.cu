@@ -225,18 +225,6 @@ __global__ void __launch_bounds__(RESOLVE_THREADS) k_resolve(const unsigned long
   }
 }
 
-int device_of(const void* p, int* dev) {
-  cudaPointerAttributes attr;
-  if (cudaPointerGetAttributes(&attr, p) != cudaSuccess ||
-      (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
-    cudaGetLastError();
-    set_error("render_meshes: the arrays must be device memory");
-    return P2M_ERR_INVALID;
-  }
-  *dev = attr.device;
-  return P2M_OK;
-}
-
 }  // namespace
 }  // namespace p2m
 
@@ -273,20 +261,19 @@ int p2m_render_meshes(const float* verts, int n_person, int n_vertex, const int3
     return P2M_ERR_WORKSPACE;
   }
   int dev;
-  P2M_TRY(device_of(images_in, &dev));
+  P2M_TRY(arrays_device("render_meshes", {verts, faces, cams, colors, image_index, images_in, images_out, face_map,
+                                          person_map, depth_map, workspace}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   unsigned long long* keys = static_cast<unsigned long long*>(workspace);
   const long long n_pix = (long long)n_image * height * width;
   P2M_CUDA_OK(cudaMemsetAsync(keys, 0xFF, need, s));
   if (draw) {
-    const long long blocks = ((long long)n_person * n_face + RASTER_THREADS - 1) / RASTER_THREADS;
-    k_raster<<<(unsigned)(blocks < MAX_GRID ? blocks : MAX_GRID), RASTER_THREADS, 0, s>>>(
+    k_raster<<<grid_for((long long)n_person * n_face, RASTER_THREADS, MAX_GRID), RASTER_THREADS, 0, s>>>(
         verts, n_vertex, faces, n_face, cams, image_index, n_person, n_image, height, width, keys);
     P2M_LAUNCH_OK();
   }
-  const long long blocks = (n_pix + RESOLVE_THREADS - 1) / RESOLVE_THREADS;
-  k_resolve<<<(unsigned)(blocks < MAX_GRID ? blocks : MAX_GRID), RESOLVE_THREADS, 0, s>>>(
+  k_resolve<<<grid_for(n_pix, RESOLVE_THREADS, MAX_GRID), RESOLVE_THREADS, 0, s>>>(
       keys, n_pix, verts, n_vertex, faces, colors, images_in, images_out, face_map, person_map, depth_map);
   P2M_LAUNCH_OK();
   return P2M_OK;

@@ -10,7 +10,6 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -207,34 +206,6 @@ __global__ void __launch_bounds__(MEAN_THREADS) k_segment_mean(const T* __restri
   }
 }
 
-int device_of(const char* where, const void* p, int* dev) {
-  cudaPointerAttributes attr;
-  if (!p || cudaPointerGetAttributes(&attr, p) != cudaSuccess ||
-      (attr.type != cudaMemoryTypeDevice && attr.type != cudaMemoryTypeManaged)) {
-    cudaGetLastError();
-    set_error(std::string(where) + ": the data arrays must be device memory");
-    return P2M_ERR_INVALID;
-  }
-  *dev = attr.device;
-  return P2M_OK;
-}
-
-// Every array of a call on the device of the first one.
-int same_device(const char* where, std::initializer_list<const void*> ptrs, int* dev) {
-  bool first = true;
-  for (const void* p : ptrs) {
-    int d;
-    P2M_TRY(device_of(where, p, &d));
-    if (first) *dev = d;
-    else if (d != *dev) {
-      set_error(std::string(where) + ": the data arrays are on different devices");
-      return P2M_ERR_INVALID;
-    }
-    first = false;
-  }
-  return P2M_OK;
-}
-
 // Host offsets: offsets[0] == 0, non-decreasing, offsets[n_seq] == n_rows.
 int check_offsets(const char* where, const int64_t* offsets, int n_seq, int64_t n_rows) {
   if (!offsets || n_seq <= 0 || n_rows <= 0) {
@@ -254,26 +225,6 @@ int check_offsets(const char* where, const int64_t* offsets, int n_seq, int64_t 
   return P2M_OK;
 }
 
-// Stream-ordered device copy of host offsets, freed on the same stream after the kernels that read it.
-struct DevOffsets {
-  long long* ptr = nullptr;
-  cudaStream_t s;
-  explicit DevOffsets(cudaStream_t st) : s(st) {}
-  int upload(const int64_t* host, size_t n) {
-    P2M_CUDA_OK(cudaMallocAsync(reinterpret_cast<void**>(&ptr), sizeof(long long) * n, s));
-    P2M_CUDA_OK(cudaMemcpyAsync(ptr, host, sizeof(long long) * n, cudaMemcpyHostToDevice, s));
-    return P2M_OK;
-  }
-  ~DevOffsets() {
-    if (ptr) cudaFreeAsync(ptr, s);
-  }
-};
-
-inline unsigned grid_for(long long work, int per_cta) {
-  const long long g = (work + per_cta - 1) / per_cta;
-  return (unsigned)(g < MAX_GRID ? (g > 0 ? g : 1) : MAX_GRID);
-}
-
 bool known_dtype(int dtype) { return dtype == P2M_DTYPE_F32 || dtype == P2M_DTYPE_F64; }
 
 template <typename T>
@@ -285,7 +236,7 @@ EuroParams<T> euro_params(double min_cutoff, double beta, double d_cutoff) {
 template <typename T>
 int segment_mean_launch(const T* values, long long width, const long long* offsets, int n_seg,
                         const unsigned char* valid, double* out, cudaStream_t s) {
-  k_segment_mean<T><<<grid_for(n_seg, 1), MEAN_THREADS, 0, s>>>(values, width, offsets, n_seg, valid, out);
+  k_segment_mean<T><<<grid_for(n_seg, 1, MAX_GRID), MEAN_THREADS, 0, s>>>(values, width, offsets, n_seg, valid, out);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -299,18 +250,18 @@ extern "C" {
 
 int p2m_one_euro_smooth(int dtype, const void* x, void* y, int64_t n_channel, const int64_t* offsets, int n_seq,
                         int64_t n_frames, double min_cutoff, double beta, double d_cutoff, p2m_stream_t stream) {
-  if (!known_dtype(dtype) || n_channel <= 0) {
-    set_error("one_euro_smooth: bad dtype code or n_channel <= 0");
+  if (!known_dtype(dtype) || !x || !y || n_channel <= 0) {
+    set_error("one_euro_smooth: bad dtype code, null array or n_channel <= 0");
     return P2M_ERR_INVALID;
   }
   P2M_TRY(check_offsets("one_euro_smooth", offsets, n_seq, n_frames));
   int dev;
-  P2M_TRY(same_device("one_euro_smooth", {x, y}, &dev));
+  P2M_TRY(arrays_device("one_euro_smooth", {x, y}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  DevOffsets off(s);
-  P2M_TRY(off.upload(offsets, (size_t)n_seq + 1));
-  const unsigned grid = grid_for((long long)n_seq * n_channel, EULER_THREADS);
+  StreamBuffer<long long> off(s);
+  P2M_TRY(off.alloc((size_t)n_seq + 1, offsets));
+  const unsigned grid = grid_for((long long)n_seq * n_channel, EULER_THREADS, MAX_GRID);
   if (dtype == P2M_DTYPE_F32)
     k_one_euro<float><<<grid, EULER_THREADS, 0, s>>>(static_cast<const float*>(x), static_cast<float*>(y), n_channel,
                                                      off.ptr, n_seq, euro_params<float>(min_cutoff, beta, d_cutoff));
@@ -338,21 +289,22 @@ int p2m_accel_error(int dtype, const void* gt, const void* pred, int n_joint, co
     host[n_seq + 2 + i] = host[n_seq + 1 + i] + (n > 2 ? n - 2 : 0);
   }
   const long long n_win = host[2 * n_seq + 1];
-  int dev;
-  if (n_win > 0) {
-    P2M_TRY(same_device("accel_error", {gt, pred, per_window, valid, seq_mean}, &dev));
-    if (vis) P2M_TRY(same_device("accel_error", {gt, vis}, &dev));
-  } else {
-    P2M_TRY(device_of("accel_error", seq_mean, &dev));
+  if (!seq_mean || (n_win > 0 && (!gt || !pred || !per_window || !valid))) {
+    set_error("accel_error: null data array");
+    return P2M_ERR_INVALID;
   }
+  int dev;
+  if (n_win > 0) P2M_TRY(arrays_device("accel_error", {gt, pred, vis, per_window, valid, seq_mean}, &dev));
+  else P2M_TRY(arrays_device("accel_error", {seq_mean}, &dev));  // no window: only seq_mean is written
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  DevOffsets off(s);
-  P2M_TRY(off.upload(host.data(), host.size()));
+  StreamBuffer<long long> off(s);
+  P2M_TRY(off.alloc(host.size(), host.data()));
   const long long* win_off = off.ptr + n_seq + 1;
+  const unsigned grid = grid_for(n_win, ACCEL_WARPS, MAX_GRID);
   if (dtype == P2M_DTYPE_F32) {
     if (n_win > 0) {
-      k_accel_error<float><<<grid_for(n_win, ACCEL_WARPS), ACCEL_WARPS * 32, 0, s>>>(
+      k_accel_error<float><<<grid, ACCEL_WARPS * 32, 0, s>>>(
           static_cast<const float*>(gt), static_cast<const float*>(pred), n_joint, off.ptr, n_seq, n_win, vis,
           static_cast<float*>(per_window), valid);
       P2M_LAUNCH_OK();
@@ -360,7 +312,7 @@ int p2m_accel_error(int dtype, const void* gt, const void* pred, int n_joint, co
     P2M_TRY(segment_mean_launch<float>(static_cast<const float*>(per_window), 1, win_off, n_seq, valid, seq_mean, s));
   } else {
     if (n_win > 0) {
-      k_accel_error<double><<<grid_for(n_win, ACCEL_WARPS), ACCEL_WARPS * 32, 0, s>>>(
+      k_accel_error<double><<<grid, ACCEL_WARPS * 32, 0, s>>>(
           static_cast<const double*>(gt), static_cast<const double*>(pred), n_joint, off.ptr, n_seq, n_win, vis,
           static_cast<double*>(per_window), valid);
       P2M_LAUNCH_OK();
@@ -372,18 +324,17 @@ int p2m_accel_error(int dtype, const void* gt, const void* pred, int n_joint, co
 
 int p2m_segment_mean(int dtype, const void* values, int64_t width, const int64_t* offsets, int n_seg, int64_t n_rows,
                      const uint8_t* valid, double* out, p2m_stream_t stream) {
-  if (!known_dtype(dtype) || width <= 0) {
-    set_error("segment_mean: bad dtype code or width <= 0");
+  if (!known_dtype(dtype) || !values || !out || width <= 0) {
+    set_error("segment_mean: bad dtype code, null array or width <= 0");
     return P2M_ERR_INVALID;
   }
   P2M_TRY(check_offsets("segment_mean", offsets, n_seg, n_rows));
   int dev;
-  P2M_TRY(same_device("segment_mean", {values, out}, &dev));
-  if (valid) P2M_TRY(same_device("segment_mean", {values, valid}, &dev));
+  P2M_TRY(arrays_device("segment_mean", {values, valid, out}, &dev));
   DeviceGuard guard(dev);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  DevOffsets off(s);
-  P2M_TRY(off.upload(offsets, (size_t)n_seg + 1));
+  StreamBuffer<long long> off(s);
+  P2M_TRY(off.alloc((size_t)n_seg + 1, offsets));
   if (dtype == P2M_DTYPE_F32)
     return segment_mean_launch<float>(static_cast<const float*>(values), width, off.ptr, n_seg, valid, out, s);
   return segment_mean_launch<double>(static_cast<const double*>(values), width, off.ptr, n_seg, valid, out, s);

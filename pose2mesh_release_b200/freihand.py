@@ -35,8 +35,7 @@ _MAX_PCK_THRESHOLDS = 128
 
 
 def _points(x, what: str, dtypes=(torch.float32,)) -> torch.Tensor:
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
+    _lib.cuda_tensor(x, what)
     if x.dim() == 2:
         x = x.unsqueeze(0)
     if x.dim() != 3 or x.shape[-1] != 3 or x.shape[0] == 0 or x.shape[1] == 0:
@@ -62,14 +61,6 @@ def _thresholds(t, max_n: int, what: str = "thresholds"):
     return (C.c_double * a.size)(*a.tolist()), a
 
 
-def _stream(x: torch.Tensor):
-    return torch.cuda.current_stream(x.device).cuda_stream
-
-
-def _ptr(t):
-    return t.data_ptr() if t is not None else None
-
-
 def _nearest(P, Q, thr=None, n_thr=0, dist=True, counts=False, frac=False, fscore=False):
     """One p2m_nearest_distances call on contiguous [B, n, 3] / [B, m, 3] tensors of one dtype."""
     B, n, m, dev = P.shape[0], P.shape[1], Q.shape[1], P.device
@@ -79,10 +70,7 @@ def _nearest(P, Q, thr=None, n_thr=0, dist=True, counts=False, frac=False, fscor
     cnt = torch.empty((B, 2, n_thr), device=dev, dtype=torch.int64) if counts else None
     fr = torch.empty((B, 2, n_thr), **f64) if frac else None
     fs = torch.empty((B, n_thr), **f64) if fscore else None
-    with torch.cuda.device(dev):
-        _lib.check(_lib.load().p2m_nearest_distances(_DTYPES[P.dtype], P.data_ptr(), Q.data_ptr(), B, n, m, thr, n_thr,
-                                                     _ptr(dp), _ptr(dq), _ptr(cnt), _ptr(fr), _ptr(fs), _stream(P)),
-                   "p2m_nearest_distances")
+    _lib.call("p2m_nearest_distances", dev, _DTYPES[P.dtype], P, Q, B, n, m, thr, n_thr, dp, dq, cnt, fr, fs)
     return dp, dq, cnt, fr, fs
 
 
@@ -91,19 +79,15 @@ def _align(gt, pred, aligned_dtype=torch.float32, aligned=True, err=False):
     B, n = gt.shape[0], gt.shape[1]
     Y = torch.empty((B, n, 3), device=gt.device, dtype=aligned_dtype) if aligned else None
     E = torch.empty((B, n), device=gt.device, dtype=torch.float64) if err else None
-    with torch.cuda.device(gt.device):
-        _lib.check(_lib.load().p2m_align_w_scale(gt.data_ptr(), pred.data_ptr(), B, n, _DTYPES[aligned_dtype], _ptr(Y),
-                                                 _ptr(E), _stream(gt)), "p2m_align_w_scale")
+    _lib.call("p2m_align_w_scale", gt.device, gt, pred, B, n, _DTYPES[aligned_dtype], Y, E)
     return Y, E
 
 
 def _pck(hist, thr, n_thr, err=None, pred=None, gt=None, err_out=None):
     """One p2m_pck_accumulate call into hist (int64 [n_thr], accumulated)."""
     x = err if err is not None else pred
-    with torch.cuda.device(x.device):
-        _lib.check(_lib.load().p2m_pck_accumulate(_ptr(err), _ptr(pred), _ptr(gt), x.numel() // (1 if err is not None
-                                                  else 3), thr, n_thr, _ptr(err_out), hist.data_ptr(), _stream(x)),
-                   "p2m_pck_accumulate")
+    _lib.call("p2m_pck_accumulate", x.device, err, pred, gt, x.numel() // (1 if err is not None else 3), thr, n_thr,
+              err_out, hist)
 
 
 # ---------------------------------------------------------------------------------------------- public functions

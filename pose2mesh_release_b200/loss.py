@@ -32,16 +32,12 @@ class _FaceTable:
 class _MeshLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, coord_out, coord_gt, faces):
-        if not coord_out.is_cuda:
-            raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; got a CPU tensor")
+        _lib.cuda_tensor(coord_out, "coord_out")
         out, gt = coord_out.contiguous().float(), coord_gt.contiguous().float()
         B, nv, _ = out.shape
         nf = faces.shape[0]
         sums = torch.empty(2, device=out.device, dtype=torch.float64)
-        with torch.cuda.device(out.device):
-            _lib.check(_lib.load().p2m_mesh_losses(out.data_ptr(), gt.data_ptr(), faces.data_ptr(), B, nv, nf, None,
-                                                   sums.data_ptr(), None,
-                                                   torch.cuda.current_stream(out.device).cuda_stream), "p2m_mesh_losses")
+        _lib.call("p2m_mesh_losses", out.device, out, gt, faces, B, nv, nf, None, sums, None)
         ctx.save_for_backward(out, gt, faces)
         losses = (sums / (3.0 * B * nf)).float()
         return losses[0], losses[1]
@@ -54,10 +50,7 @@ class _MeshLossFn(torch.autograd.Function):
         scale = (torch.stack([g_normal, g_edge]).float() / (3.0 * B * nf)).contiguous()
         grad = torch.empty_like(out)
         sums = torch.empty(2, device=out.device, dtype=torch.float64)
-        with torch.cuda.device(out.device):
-            _lib.check(_lib.load().p2m_mesh_losses(out.data_ptr(), gt.data_ptr(), faces.data_ptr(), B, nv, nf,
-                                                   scale.data_ptr(), sums.data_ptr(), grad.data_ptr(),
-                                                   torch.cuda.current_stream(out.device).cuda_stream), "p2m_mesh_losses")
+        _lib.call("p2m_mesh_losses", out.device, out, gt, faces, B, nv, nf, scale, sums, grad)
         return grad, None, None
 
 
@@ -90,15 +83,11 @@ class EdgeLengthLoss(MeshLosses):
 class _CoordLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, target, valid):
-        if not pred.is_cuda:
-            raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; got a CPU tensor")
+        _lib.cuda_tensor(pred, "pred")
         p, t = pred.contiguous().float(), target.contiguous().float()
         v = None if valid is None else valid.expand_as(p).contiguous().float()
         s = torch.empty(1, device=p.device, dtype=torch.float64)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.load().p2m_coord_loss(p.data_ptr(), t.data_ptr(), None if v is None else v.data_ptr(), p.numel(),
-                                                  None, s.data_ptr(), None,
-                                                  torch.cuda.current_stream(p.device).cuda_stream), "p2m_coord_loss")
+        _lib.call("p2m_coord_loss", p.device, p, t, v, p.numel(), None, s, None)
         ctx.save_for_backward(p, t, v if v is not None else torch.empty(0, device=p.device))
         return (s / p.numel()).float()[0]
 
@@ -108,10 +97,7 @@ class _CoordLossFn(torch.autograd.Function):
         scale = (g.float() / p.numel()).reshape(1).contiguous()
         grad = torch.empty_like(p)
         s = torch.empty(1, device=p.device, dtype=torch.float64)
-        with torch.cuda.device(p.device):
-            _lib.check(_lib.load().p2m_coord_loss(p.data_ptr(), t.data_ptr(), v.data_ptr() if v.numel() else None,
-                                                  p.numel(), scale.data_ptr(), s.data_ptr(), grad.data_ptr(),
-                                                  torch.cuda.current_stream(p.device).cuda_stream), "p2m_coord_loss")
+        _lib.call("p2m_coord_loss", p.device, p, t, v if v.numel() else None, p.numel(), scale, s, grad)
         return grad, None, None
 
 

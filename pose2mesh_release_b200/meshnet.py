@@ -189,10 +189,7 @@ class _MeshNetFunction(torch.autograd.Function):
         ws_bytes = lib.p2m_meshnet_workspace_bytes(h, B, int(training))
         ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
         table = _param_table(fc_w, fc_b, cl_w, cl_b, bn_w, bn_b, bn_rm, bn_rv, bn_nbt)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_meshnet_forward(h, C.byref(table), x.data_ptr(), y.data_ptr(), B, int(training),
-                                               ws.data_ptr(), ws_bytes, stream), "p2m_meshnet_forward")
+        _lib.call("p2m_meshnet_forward", dev, h, C.byref(table), x, y, B, int(training), ws, ws_bytes)
         needs_grad = training and any(ctx.needs_input_grad)
         if needs_grad:
             ctx.hier, ctx.n_layers, ctx.ws, ctx.ws_bytes = hier, n_layers, ws, ws_bytes
@@ -240,12 +237,8 @@ class _MeshNetFunction(torch.autograd.Function):
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         sc_bytes = lib.p2m_meshnet_backward_scratch_bytes(h, B)
         scratch = torch.empty(sc_bytes, device=dev, dtype=torch.uint8)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_meshnet_backward(h, C.byref(ptab), C.byref(gtab), x.data_ptr(), dy.data_ptr(),
-                                                None if dx is None else dx.data_ptr(), B, ctx.ws.data_ptr(),
-                                                ctx.ws_bytes, scratch.data_ptr(), sc_bytes, stream),
-                       "p2m_meshnet_backward")
+        _lib.call("p2m_meshnet_backward", dev, h, C.byref(ptab), C.byref(gtab), x, dy, dx, B, ctx.ws, ctx.ws_bytes,
+                  scratch, sc_bytes)
         ctx.ws = None
         return (dx, None, None, None, None, *grads)
 
@@ -356,11 +349,7 @@ class Pose2Mesh(nn.Module):
         table = _param_table(params[0], params[1], params[2:2 + n], params[2 + n:2 + 2 * n],
                              list(params[2 + 2 * n:2 + 2 * n + n_bn]) + [None],
                              list(params[2 + 2 * n + n_bn:]) + [None], rm, rv, nbt)
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_meshnet_forward_vertices(h, C.byref(table), x.data_ptr(), y.data_ptr(), B,
-                                                        ws.data_ptr(), ws_bytes,
-                                                        torch.cuda.current_stream(dev).cuda_stream),
-                       "p2m_meshnet_forward_vertices")
+        _lib.call("p2m_meshnet_forward_vertices", dev, h, C.byref(table), x, y, B, ws, ws_bytes)
         return y
 
     def _set_gather(self, dev, perm_reverse, n_vertex):
@@ -404,11 +393,8 @@ class Pose2Mesh(nn.Module):
         table = _param_table(params[0], params[1], params[2:2 + n], params[2 + n:2 + 2 * n],
                              list(params[2 + 2 * n:2 + 2 * n + n_bn]) + [None],
                              list(params[2 + 2 * n + n_bn:]) + [None], rm, rv, nbt)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        fn = lib.p2m_meshnet_forward_vertices_host if gathered else lib.p2m_meshnet_forward_host
-        with torch.cuda.device(dev):
-            _lib.check(fn(h, C.byref(table), x_host.data_ptr(), out.data_ptr(), B, ws.data_ptr(), ws.numel(), stream),
-                       "p2m_meshnet_forward_host")
+        name = "p2m_meshnet_forward_vertices_host" if gathered else "p2m_meshnet_forward_host"
+        _lib.call(name, dev, h, C.byref(table), x_host, out, B, ws, ws.numel())
         return out
 
     # the reference exposes these helpers; keep them for callers that poke at them

@@ -25,8 +25,7 @@ H36M_EVAL_JOINT = (1, 2, 3, 4, 5, 6, 8, 10, 11, 12, 13, 14, 15, 16)  # data/Huma
 
 
 def _points(x: torch.Tensor, what: str) -> torch.Tensor:
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
+    _lib.cuda_tensor(x, what)
     if x.dim() == 2:
         x = x.unsqueeze(0)
     if x.dim() != 3 or x.shape[-1] != 3 or x.shape[0] == 0 or x.shape[1] == 0:
@@ -62,10 +61,6 @@ def _root_index(root: int, n: int) -> int:
     return int(root) % n
 
 
-def _stream(x: torch.Tensor):
-    return torch.cuda.current_stream(x.device).cuda_stream
-
-
 def _align(A, B, subset=None, transform=False, aligned=False, err=False, sums=None):
     """One p2m_rigid_align call on [B, n, 3] float32 CUDA tensors; returns the requested outputs."""
     batch, n = A.shape[0], A.shape[1]
@@ -73,10 +68,7 @@ def _align(A, B, subset=None, transform=False, aligned=False, err=False, sums=No
     T = torch.empty((batch, 13), device=A.device, dtype=torch.float64) if transform else None
     Y = torch.empty((batch, k, 3), device=A.device, dtype=torch.float32) if aligned else None
     E = torch.empty((batch, k), device=A.device, dtype=torch.float32) if err else None
-    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-    with torch.cuda.device(A.device):
-        _lib.check(_lib.load().p2m_rigid_align(A.data_ptr(), B.data_ptr(), batch, n, sub, k if sub is not None else 0,
-                                               ptr(T), ptr(Y), ptr(E), ptr(sums), _stream(A)), "p2m_rigid_align")
+    _lib.call("p2m_rigid_align", A.device, A, B, batch, n, sub, k if sub is not None else 0, T, Y, E, sums)
     return T, Y, E
 
 
@@ -85,20 +77,15 @@ def _errors(pred, gt, pred_root=None, gt_root=None, subset=None, fp64=False, err
     batch, n = pred.shape[0], pred.shape[1]
     sub, k = _subset(subset, n)
     E = torch.empty((batch, k), device=pred.device, dtype=torch.float32) if err else None
-    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-    with torch.cuda.device(pred.device):
-        _lib.check(_lib.load().p2m_point_errors(pred.data_ptr(), gt.data_ptr(), ptr(pred_root), ptr(gt_root), batch, n,
-                                                sub, k if sub is not None else 0, int(fp64), ptr(E), ptr(sums),
-                                                _stream(pred)), "p2m_point_errors")
+    _lib.call("p2m_point_errors", pred.device, pred, gt, pred_root, gt_root, batch, n, sub, k if sub is not None else 0,
+              int(fp64), E, sums)
     return E
 
 
 def _root_rows(x: torch.Tensor, root, what: str, batch: int, device) -> torch.Tensor:
     """A per-sample root point: an index into x ([B, n, 3]) or an explicit [B, 3] / [B, 1, 3] / [3] tensor."""
     if isinstance(root, torch.Tensor):
-        if not root.is_cuda:
-            raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
-        r = root.reshape(-1, 3)
+        r = _lib.cuda_tensor(root, what).reshape(-1, 3)
         if r.shape[0] == 1 and batch > 1:
             r = r.expand(batch, 3)
         if r.shape[0] != batch or r.device != device:

@@ -90,8 +90,7 @@ class LinearModel(nn.Module):
         with_combine additionally returns pose_combine = cat(pose2d, pose3d / 1000) [B, J, 5]
         (lib/models/pose2mesh_net.py:18-19)."""
         lib = _lib.load()
-        if not x.is_cuda:
-            raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; got a CPU tensor")
+        _lib.cuda_tensor(x, "x")
         x = x.reshape(len(x), -1).contiguous().float()
         if x.shape[1] != self.input_size:
             raise ValueError(f"PoseNet expects {self.input_size} inputs per pose, got {x.shape[1]}")
@@ -103,10 +102,7 @@ class LinearModel(nn.Module):
         nbytes = lib.p2m_posenet_workspace_bytes(B, self.linear_size)
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
         params = self._native_params()
-        with torch.cuda.device(dev):
-            _lib.check(lib.p2m_posenet_forward(C.byref(params), x.data_ptr(), out.data_ptr(),
-                                               None if comb is None else comb.data_ptr(), B, ws.data_ptr(), nbytes,
-                                               torch.cuda.current_stream(dev).cuda_stream), "p2m_posenet_forward")
+        _lib.call("p2m_posenet_forward", dev, C.byref(params), x, out, comb, B, ws, nbytes)
         return (out, comb) if with_combine else out
 
     def forward(self, x):

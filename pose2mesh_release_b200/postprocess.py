@@ -16,17 +16,13 @@ INPUT_SHAPE = (384, 288)  # cfg.MODEL.input_shape (height, width), lib/core/conf
 
 def regress_joints(vertices: torch.Tensor, joint_regressor: torch.Tensor) -> torch.Tensor:
     """vertices [B, n_vertex, C] (C <= 4), joint_regressor [n_joint, n_vertex] -> joints [B, n_joint, C]."""
-    if not vertices.is_cuda:
-        raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; got a CPU tensor")
-    v = vertices.contiguous().float()
+    v = _lib.cuda_tensor(vertices, "vertices").contiguous().float()
     jr = joint_regressor.to(v.device).contiguous().float()
     B, nv, ch = v.shape
     if jr.shape[1] != nv:
         raise ValueError(f"joint_regressor has {jr.shape[1]} columns, vertices has {nv} rows")
     out = torch.empty((B, jr.shape[0], ch), device=v.device, dtype=torch.float32)
-    with torch.cuda.device(v.device):
-        _lib.check(_lib.load().p2m_regress_joints(jr.data_ptr(), v.data_ptr(), out.data_ptr(), B, jr.shape[0], nv, ch,
-                                                  torch.cuda.current_stream(v.device).cuda_stream), "p2m_regress_joints")
+    _lib.call("p2m_regress_joints", v.device, jr, v, out, B, jr.shape[0], nv, ch)
     return out
 
 
@@ -34,14 +30,10 @@ def normalize_pose2d(joints_px: torch.Tensor, input_shape=INPUT_SHAPE) -> torch.
     """joints_px [B, J, 2] (or [J, 2]) image pixels on a CUDA device -> pose2d [B, J, 2] as demo/run.py:150-158
     computes it.  Integer tensors are treated like the reference treats integer arrays (its in-place affine transform
     truncates the transformed coordinates, aug_utils.py:57-59)."""
-    if not joints_px.is_cuda:
-        raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; got a CPU tensor")
+    _lib.cuda_tensor(joints_px, "joints_px")
     truncate = int(not joints_px.is_floating_point())
     x = joints_px.reshape(-1, joints_px.shape[-2], 2).contiguous().float()
     out = torch.empty_like(x)
-    with torch.cuda.device(x.device):
-        _lib.check(_lib.load().p2m_normalize_pose2d(x.data_ptr(), out.data_ptr(), x.shape[0], x.shape[1],
-                                                    int(input_shape[0]), int(input_shape[1]), truncate,
-                                                    torch.cuda.current_stream(x.device).cuda_stream),
-                   "p2m_normalize_pose2d")
+    _lib.call("p2m_normalize_pose2d", x.device, x, out, x.shape[0], x.shape[1], int(input_shape[0]),
+              int(input_shape[1]), truncate)
     return out

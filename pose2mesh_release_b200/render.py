@@ -27,8 +27,7 @@ MAX_SIDE = 16384
 
 
 def _cuda(x, what: str) -> torch.Tensor:
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
+    _lib.cuda_tensor(x, what)
     if x.requires_grad:
         raise ValueError(f"{what} requires grad; the renderer is not differentiable")
     return x
@@ -120,15 +119,11 @@ def render_meshes(images, verts, faces, cams, colors, image_index=None, return_m
     if return_maps:
         maps = (torch.empty((N, H, W), dtype=torch.int32, device=dev), torch.empty((N, H, W), dtype=torch.int32, device=dev),
                 torch.empty((N, H, W), dtype=torch.float32, device=dev))
-    lib = _lib.load()
-    ws_bytes = lib.p2m_render_workspace_bytes(N, H, W)
+    ws_bytes = _lib.load().p2m_render_workspace_bytes(N, H, W)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
     ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None  # noqa: E731
-    with torch.cuda.device(dev):
-        _lib.check(lib.p2m_render_meshes(
-            ptr(v), P, V, ptr(f), f.shape[0], ptr(c), ptr(col), ptr(idx), img_in.data_ptr(), N, H, W, out.data_ptr(),
-            *(ptr(m) for m in (maps or (None, None, None))), ws.data_ptr(), ws_bytes,
-            torch.cuda.current_stream(dev).cuda_stream), "p2m_render_meshes")
+    _lib.call("p2m_render_meshes", dev, ptr(v), P, V, ptr(f), f.shape[0], ptr(c), ptr(col), ptr(idx), img_in, N, H, W,
+              out, *(ptr(m) for m in (maps or (None, None, None))), ws, ws_bytes)
     if squeeze:
         out = out[0]
         maps = maps and tuple(m[0] for m in maps)

@@ -26,8 +26,7 @@ _DTYPES = {torch.float32: _lib.P2M_DTYPE_F32, torch.float64: _lib.P2M_DTYPE_F64}
 
 
 def _data(x, what: str) -> torch.Tensor:
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        raise RuntimeError(f"pose2mesh_release_b200 runs on CUDA (sm_90a) only; {what} is not a CUDA tensor")
+    _lib.cuda_tensor(x, what)
     if x.dtype not in _DTYPES:
         raise ValueError(f"{what} must be float32 or float64; got {x.dtype}")
     if x.dim() == 0 or x.shape[0] == 0:
@@ -56,15 +55,10 @@ def _offsets(lengths, n_frames: int):
     return (C.c_int64 * off.size)(*off.tolist()), int(n.size)
 
 
-def _stream(x: torch.Tensor):
-    return torch.cuda.current_stream(x.device).cuda_stream
-
-
 def _vis(vis, n_frames: int, device):
     if vis is None:
         return None
-    if not isinstance(vis, torch.Tensor) or not vis.is_cuda:
-        raise RuntimeError("pose2mesh_release_b200 runs on CUDA (sm_90a) only; vis is not a CUDA tensor")
+    _lib.cuda_tensor(vis, "vis")
     if vis.dim() != 1 or vis.shape[0] != n_frames or vis.device != device:
         raise ValueError(f"vis must be [{n_frames}] on {device}, one flag per frame; got {tuple(vis.shape)}")
     return (vis != 0).to(torch.uint8).contiguous()
@@ -74,10 +68,8 @@ def _segment_mean(values: torch.Tensor, offsets, n_seg: int, width: int = 1, val
     """fp64 mean per segment of a [rows, width] float32 / float64 tensor (one p2m_segment_mean launch)."""
     out = torch.empty((n_seg,), device=values.device, dtype=torch.float64)
     n_rows = values.numel() // width
-    with torch.cuda.device(values.device):
-        _lib.check(_lib.load().p2m_segment_mean(_DTYPES[values.dtype], values.data_ptr(), width, offsets, n_seg, n_rows,
-                                                valid.data_ptr() if valid is not None else None, out.data_ptr(),
-                                                _stream(values)), "p2m_segment_mean")
+    _lib.call("p2m_segment_mean", values.device, _DTYPES[values.dtype], values, width, offsets, n_seg, n_rows, valid,
+              out)
     return out
 
 
@@ -95,10 +87,8 @@ def smooth_sequences(x: torch.Tensor, lengths, min_cutoff: float, beta: float, d
     n_ch = x[0].numel()
     if n_ch == 0:
         raise ValueError(f"x must hold at least one channel per frame; got {tuple(x.shape)}")
-    with torch.cuda.device(x.device):
-        _lib.check(_lib.load().p2m_one_euro_smooth(_DTYPES[x.dtype], x.data_ptr(), y.data_ptr(), n_ch, off, n_seq,
-                                                   x.shape[0], float(min_cutoff), float(beta), float(d_cutoff),
-                                                   _stream(x)), "p2m_one_euro_smooth")
+    _lib.call("p2m_one_euro_smooth", x.device, _DTYPES[x.dtype], x, y, n_ch, off, n_seq, x.shape[0], float(min_cutoff),
+              float(beta), float(d_cutoff))
     return y
 
 
@@ -125,11 +115,8 @@ def accel_errors(gt: torch.Tensor, pred: torch.Tensor, lengths, vis: torch.Tenso
     per_window = torch.empty((n_win,), device=gt.device, dtype=gt.dtype)
     valid = torch.empty((n_win,), device=gt.device, dtype=torch.uint8)
     seq_mean = torch.empty((n_seq,), device=gt.device, dtype=torch.float64)
-    with torch.cuda.device(gt.device):
-        _lib.check(_lib.load().p2m_accel_error(_DTYPES[gt.dtype], gt.data_ptr(), pred.data_ptr(), gt.shape[1], off,
-                                               n_seq, gt.shape[0], v.data_ptr() if v is not None else None,
-                                               per_window.data_ptr(), valid.data_ptr(), seq_mean.data_ptr(),
-                                               _stream(gt)), "p2m_accel_error")
+    _lib.call("p2m_accel_error", gt.device, _DTYPES[gt.dtype], gt, pred, gt.shape[1], off, n_seq, gt.shape[0], v,
+              per_window, valid, seq_mean)
     return per_window, valid.view(torch.bool), seq_mean
 
 

@@ -2,6 +2,7 @@
 reference's state_dict surface and initialiser, the native graph builder reproduces the reference's
 hierarchy, the product path refuses to run without a GPU, and nothing in the product imports oracle/."""
 import ast
+import ctypes as C
 import os
 import re
 
@@ -23,8 +24,79 @@ def test_library_loads_and_exports_header_symbols():
     assert declared, "no declarations parsed"
     for name in sorted(declared):
         assert hasattr(lib, name), f"{name} declared in include/p2m_b200.h but not exported"
-    assert set(_lib.EXPORTS) <= declared
+    assert set(_lib.EXPORTS) == declared
     assert b"sm_90a" in lib.p2m_version()
+
+
+STATELESS = ["p2m_posenet_forward", "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
+             "p2m_rigid_align", "p2m_point_errors", "p2m_nearest_distances", "p2m_align_w_scale", "p2m_pck_accumulate",
+             "p2m_one_euro_smooth", "p2m_accel_error", "p2m_segment_mean", "p2m_fit_camera", "p2m_crop_cam_to_orig",
+             "p2m_render_meshes"]
+
+
+def _host_args(lib, keep):
+    """The arguments (stream excluded) of every stateless entry point: valid sizes, and a zeroed host (numpy) array in
+    every data-array slot.  Host-side tables (subsets, offsets, thresholds, schedules) are what they always are."""
+    from pose2mesh_release_b200 import _lib
+
+    def h(*shape, dtype=np.float32):
+        a = np.zeros(shape, dtype)
+        keep.append(a)
+        return a.ctypes.data
+
+    f64, i32, u8 = np.float64, np.int32, np.uint8
+    F32 = _lib.P2M_DTYPE_F32
+    B, J, V, F, H = 2, 4, 8, 3, 64        # batch, joints, vertices, faces, PoseNet width
+    off = (C.c_int64 * 2)(0, 4)          # one sequence of four frames: two acceleration windows
+    thr = (C.c_double * 2)(0.1, 0.2)
+    lr_steps, lr_values = (C.c_int32 * 1)(0), (C.c_double * 1)(0.1)
+    posenet = _lib.PoseNetParams(num_joint=J, hidden=H, num_stage=0, w1_w=h(H, 2 * J), w1_b=h(H), w2_w=h(3 * J, H),
+                                 w2_b=h(3 * J))
+    keep += [off, thr, lr_steps, lr_values, posenet]
+    ws_pose, ws_render = lib.p2m_posenet_workspace_bytes(B, H), lib.p2m_render_workspace_bytes(1, 4, 4)
+    return {
+        "p2m_posenet_forward": (C.byref(posenet), h(B, 2 * J), h(B, 3 * J), h(B, J, 5), B, h(ws_pose, dtype=u8),
+                                ws_pose),
+        "p2m_regress_joints": (h(J, V), h(B, V, 3), h(B, J, 3), B, J, V, 3),
+        "p2m_normalize_pose2d": (h(B, J, 2), h(B, J, 2), B, J, 384, 288, 0),
+        "p2m_mesh_losses": (h(B, V, 3), h(B, V, 3), h(F, 3, dtype=i32), B, V, F, h(2), h(2, dtype=f64), h(B, V, 3)),
+        "p2m_coord_loss": (h(B, J, 3), h(B, J, 3), h(B, J, 3), B * J * 3, h(1), h(1, dtype=f64), h(B, J, 3)),
+        "p2m_rigid_align": (h(B, V, 3), h(B, V, 3), B, V, None, 0, h(B, 13, dtype=f64), h(B, V, 3), h(B, V),
+                            h(B + 1, dtype=f64)),
+        "p2m_point_errors": (h(B, V, 3), h(B, V, 3), h(B, 3), h(B, 3), B, V, None, 0, 0, h(B, V), h(B + 1, dtype=f64)),
+        "p2m_nearest_distances": (F32, h(B, V, 3), h(B, V, 3), B, V, V, thr, 2, h(B, V, dtype=f64), h(B, V, dtype=f64),
+                                  h(B, 2, 2, dtype=np.int64), h(B, 2, 2, dtype=f64), h(B, 2, dtype=f64)),
+        "p2m_align_w_scale": (h(B, V, 3), h(B, V, 3), B, V, F32, h(B, V, 3), h(B, V, dtype=f64)),
+        "p2m_pck_accumulate": (None, h(B * V, 3), h(B * V, 3), B * V, thr, 2, h(B * V, dtype=f64),
+                               h(2, dtype=np.int64)),
+        "p2m_one_euro_smooth": (F32, h(4, J, 3), h(4, J, 3), J * 3, off, 1, 4, 1.0, 0.0, 1.0),
+        "p2m_accel_error": (F32, h(4, J, 3), h(4, J, 3), J, off, 1, 4, h(4, dtype=u8), h(2), h(2, dtype=u8),
+                            h(1, dtype=f64)),
+        "p2m_segment_mean": (F32, h(4, 3), 3, off, 1, 4, h(4, dtype=u8), h(1, dtype=f64)),
+        "p2m_fit_camera": (h(B, J, 2, dtype=f64), 2, _lib.P2M_CAM_INPUT_F64, J, h(B, J, 3), J, h(B, 3), B, 500, 10,
+                           lr_steps, lr_values, 1, h(B, 2), h(B, 3), h(B, 4), h(B, J, 2), h(B), h(B, 4)),
+        "p2m_crop_cam_to_orig": (h(B, 3), h(B, 4), h(B, 2), B, h(B, 4)),
+        "p2m_render_meshes": (h(B, V, 3), B, V, h(F, 3, dtype=i32), F, h(B, 4), h(B, 3), h(B, dtype=i32),
+                              h(1, 4, 4, 3, dtype=u8), 1, 4, 4, h(1, 4, 4, 3, dtype=u8), h(1, 4, 4, dtype=i32),
+                              h(1, 4, 4, dtype=i32), h(1, 4, 4), h(ws_render // 8, dtype=np.uint64), ws_render),
+    }
+
+
+@pytest.mark.parametrize("name", STATELESS)
+def test_stateless_entry_point_rejects_host_arrays(name):
+    """A stateless entry point runs on the device of its data arrays, so it checks them before any CUDA work: host
+    memory in every data-array slot is P2M_ERR_INVALID naming the call.  Skipped with a GPU, where an entry point
+    without the check would launch kernels on host pointers."""
+    if torch.cuda.is_available():
+        pytest.skip("GPU present")
+    from pose2mesh_release_b200 import _lib
+
+    lib = _lib.load()
+    keep = []
+    status = getattr(lib, name)(*_host_args(lib, keep)[name], None)
+    msg = lib.p2m_last_error().decode()
+    assert status == 1, (status, msg)
+    assert name[len("p2m_"):] in msg and "device memory" in msg, msg
 
 
 def test_conv_kernel_register_split_is_balanced_in_the_build():
