@@ -24,9 +24,10 @@
 //     "hard parts" 1).  After the tile's last K-block the same warpgroup applies the fused epilogue — bias / folded
 //     BatchNorm, ReLU, channel-resampled residual (or, for the network's last block, the 64 -> 3 head's projection) —
 //     through a per-warp staging buffer, while the producers already fill the ring for the next tile.  N = 64: the
-//     accumulator is transposed through swizzled staging so that global accesses are coalesced.  N = 128: the
-//     epilogue runs in the fragment layout, in place in linear 512-byte staging rows that the copy engine fills with
-//     the identity residual during the main loop and drains to HBM by cp.async.bulk stores nobody waits for.
+//     accumulator is transposed through swizzled staging so that global accesses are coalesced.  N = 128: two such
+//     warpgroups alternate tiles (one runs its epilogue while the other issues the next tile's MMAs; 8 producer warps
+//     then build the A operand); the epilogue runs in the fragment layout, in place in linear 512-byte staging rows
+//     that the copy engine fills with the identity residual and drains to HBM by cp.async.bulk stores.
 // The unpool between levels is virtual: with in_unpool the rows are read from row r>>1 of the coarser
 // tensor.  Weights are pre-scaled by 2^6 so that their lo parts stay normal fp16 numbers (undone exactly in the
 // epilogue).  The same kernel in `plain` mode is the backward dT GEMM and, with pre-packed A blocks, the dense GEMM;
@@ -193,7 +194,8 @@ __device__ __forceinline__ void cp_async_arrive_noinc(uint32_t bar) {
   // the mbarrier gets this thread's arrival once all of its earlier cp.async copies have landed
   asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
 }
-__device__ __forceinline__ void producer_barrier() { asm volatile("bar.sync 1, 512;" ::: "memory"); }
+template <int NT>
+__device__ __forceinline__ void producer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(NT) : "memory"); }
 // explicit shared-window accesses (32-bit addresses): keeps the hot loops on LDS/STS instead of generic LD/ST
 __device__ __forceinline__ float4 lds_f4(uint32_t a) {
   float4 v;
@@ -386,13 +388,26 @@ __device__ __forceinline__ void trace_ev(const KParams&, int, int&, int) {}
 //   18     weight-block loader (one thread, cp.async.bulk)
 //   19     idle
 //   20..23 MMA + epilogue warpgroup: wgmma into register accumulators -> fused epilogue -> HBM
+// The 64 x 128 configuration (N = 128) has two MMA + epilogue warpgroups that alternate tiles, so that one runs its
+// epilogue while the other issues the next tile's MMAs; the producers shrink to warps 0..7 (two tile rows per thread)
+// and warps 12..15 are parked:
+//   0..7   producers          8..11  MMA + epilogue warpgroup 1 (the CTA's odd tiles)
+//   12..15 parked             16..23 as above (20..23: MMA + epilogue warpgroup 0, the even tiles)
 constexpr int W_PROD = 16;
 constexpr int W_XLOAD = 16, N_XLOAD = 2, W_BLOAD = 18, W_EPI0 = 20;
+constexpr int W_EPI1 = 8, W_PARK = 12;  // N = 128 only
 constexpr int NUM_THREADS2 = 24 * 32;
 constexpr int REGS_LAUNCH = 80, REGS_UTIL = 40, REGS_EPI = 120;  // setmaxnreg targets per warpgroup (see the kernel)
+constexpr int REGS_PROD2 = 88, REGS_PARK = 24;                    // ... and those of the N = 128 layout
 // setmaxnreg.inc draws on the pool the CTA's own setmaxnreg.dec filled: requests beyond it would spin forever
 static_assert(128 * (REGS_EPI - REGS_LAUNCH) <= 128 * (REGS_LAUNCH - REGS_UTIL), "register pool balance");
+static_assert(2 * 128 * (REGS_PROD2 - REGS_LAUNCH) + 2 * 128 * (REGS_EPI - REGS_LAUNCH) <=
+                  128 * (REGS_LAUNCH - REGS_PARK) + 128 * (REGS_LAUNCH - REGS_UTIL),
+              "register pool balance of the N = 128 layout");
 static_assert(W_XLOAD % 4 == 0 && W_EPI0 % 4 == 0 && W_EPI0 - W_XLOAD == 4, "setmaxnreg works on aligned warpgroups");
+static_assert(W_EPI1 % 4 == 0 && W_PARK == W_EPI1 + 4 && W_XLOAD == W_PARK + 4, "setmaxnreg works on aligned warpgroups");
+template <int N>
+__host__ __device__ constexpr int prod_warps() { return N == 128 ? W_EPI1 : W_PROD; }
 
 // Two tile shapes, both a 64-register fp32 accumulator per thread of the one MMA warpgroup:
 //   N = 64:  a CTA computes 128 tile rows x the 64 output columns [64 blockIdx.y, 64 blockIdx.y + 64); used for the
@@ -408,7 +423,11 @@ template <int N, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
   constexpr int TM = tile_rows<N>();  // tile rows
-  constexpr int RPT = TM / 64;        // tile rows per producer thread
+  constexpr int NPW = prod_warps<N>();  // producer warps
+  constexpr int NRG = NPW * 4;        // producer row groups (8 threads each)
+  constexpr int RPT = TM / NRG;       // tile rows per producer thread (2: row groups rg and NRG + rg of the row order)
+  constexpr int NWG = N == 128 ? 2 : 1;  // MMA + epilogue warpgroups (they alternate tiles)
+  static_assert(RPT == 2, "both configurations give a producer thread two tile rows");
   constexpr int H = TM / 64;          // M = 64 halves of the tile (one accumulator each)
   constexpr int ER = 16 * H;          // epilogue rows per warp of the MMA warpgroup
   constexpr bool KT1 = (MODE == 1);
@@ -438,7 +457,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   uint64_t* b_x_empty = b_x_full + XS;       // [XS]
   uint64_t* b_m_full = b_x_empty + XS;       // [2]
   uint64_t* b_m_empty = b_m_full + 2;        // [2]
-  uint32_t* flags = reinterpret_cast<uint32_t*>(b_m_empty + 2);
+  // N = 128: the output stores of the tile before have read the staging buffer, which passes from one MMA warpgroup's
+  // epilogue to the other's (one arrival per warp); the tile before has finished its main loop (one arrival per warp)
+  uint64_t* b_stg_free = b_m_empty + 2;      // [1]
+  uint64_t* b_turn = b_stg_free + 1;         // [1]
+  uint32_t* flags = reinterpret_cast<uint32_t*>(b_turn + 1);
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
   float* ep_mul = reinterpret_cast<float*>(flags + 4);  // [N] acc * mul + add  (weight scale, bias, folded BN)
   float* ep_add = ep_mul + N;
@@ -448,10 +471,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   constexpr int STG_WARP_BYTES = N == 128 ? 16 * STG_ROW_BYTES : 32 * EC * 4;
   unsigned char* epi_stage =
       reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(ep_add + N) + 127) & ~(uintptr_t)127);
-  int* own_s = reinterpret_cast<int*>(epi_stage + 4 * STG_WARP_BYTES);  // [4 warps][32] vertex id of each epilogue row
-  float* head_w_s = reinterpret_cast<float*>(own_s + 4 * 32);        // [64][12] (N == 64 with a fused head)
-  uint64_t* b_res = reinterpret_cast<uint64_t*>(head_w_s);  // [4] (N = 128: no head) per MMA warp: its tile's identity-
-                                                            // residual rows have landed in its staging block
+  // (N = 128: the two MMA warpgroups share the staging buffer, one tile after the other)
+  int* own_s = reinterpret_cast<int*>(epi_stage + 4 * STG_WARP_BYTES);  // [NWG][4 warps][ER] vertex id of each epilogue row
+  float* head_w_s = reinterpret_cast<float*>(own_s + NWG * 4 * ER);  // [64][12] (N == 64 with a fused head)
+  uint64_t* b_res = reinterpret_cast<uint64_t*>(head_w_s);  // [4] (N = 128: no head) per staging block: its tile's
+                                                            // identity-residual rows have landed in it
 
   const int tid = threadIdx.x;
   const int warp = tid >> 5;
@@ -462,7 +486,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   if (tid == 0) {
     for (int s = 0; s < NS; ++s) {
       // one elected arrive per producer warp + the weight loader (dense GEMM mode: the loader alone)
-      mbar_init(smem_u32(b_ab_full + s), p.apack != nullptr ? 1 : W_PROD + 1);
+      mbar_init(smem_u32(b_ab_full + s), p.apack != nullptr ? 1 : NPW + 1);
       mbar_init(smem_u32(b_ab_empty + s), 4);  // one arrival per warp of the MMA warpgroup
     }
     for (int s = 0; s < XS; ++s) {
@@ -474,8 +498,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       mbar_init(smem_u32(b_m_full + s), 1);
       mbar_init(smem_u32(b_m_empty + s), 1);
     }
-    if (N == 128)
+    if (N == 128) {
       for (int w = 0; w < 4; ++w) mbar_init(smem_u32(b_res + w), 1);  // the warp's expect_tx arrival + its copies' bytes
+      mbar_init(smem_u32(b_stg_free), 4);
+      mbar_init(smem_u32(b_turn), 4);
+    }
     *abort_flag = (smem_u32(ring) & 1023u) ? 1 : 0;
     if (*abort_flag) mbar_timeout(abort_flag, p.status, 100);
     fence_barrier_init();
@@ -496,8 +523,10 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   // Register split by warpgroup (the kernel is launched with 80 per thread: 768 x 80 = 60 K of the SM's 64 K): the
   // utility warpgroup (loaders, weight loader) drops to 40 per thread and the MMA + epilogue warpgroup takes exactly
   // what that frees (120 per thread): the 64 accumulator registers plus the epilogue's addresses and residual state
-  // (at 104 ptxas spilled twice as much).  The producers stay at 80.
+  // (at 104 ptxas spilled twice as much).  The producers stay at 80.  N = 128: the parked warpgroup drops to 24 as
+  // well, which pays for the second MMA + epilogue warpgroup (120) and for the two rows per producer thread (88).
   // (each budget is set at the top of its own region: after a join ptxas has to assume the smallest one)
+  const int mma_g = warp >= W_EPI0 ? 0 : (NWG == 2 && warp >= W_EPI1 && warp < W_PARK) ? 1 : -1;
   if (warp >= W_XLOAD && warp < W_EPI0) {
   asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_UTIL));
   if (warp >= W_XLOAD && warp < W_XLOAD + N_XLOAD) {
@@ -614,9 +643,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       }
     }
   }
-  } else if (warp >= W_EPI0) {
+  } else if (mma_g >= 0) {
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_EPI));
-    // ------------------------------------------------------------ MMA + epilogue warpgroup
+    // ------------------------------------------------------------ MMA + epilogue warpgroup(s)
     // wgmma into register accumulators, two 64 x 64 ones (m64n64): for N = 64 the two M = 64 row halves of the 128-row
     // tile, for N = 128 the two 64-column halves of the 64-row tile (acc[h][j] then holds exactly what element j + 32 h
     // of an m64n128 fragment would: the 128-column instruction itself needs more than the 80 registers ptxas allocates
@@ -627,7 +656,13 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     // 128-byte row pieces, and the fused epilogue (affine, ReLU, residual) runs in that layout, where the residual reads
     // coalesce.  N = 128: the epilogue writes its results in place into the warp's linear staging rows, which then
     // leave whole by bulk copy.
-    const int wq = warp - W_EPI0;
+    // N = 128: warpgroup g takes the CTA's tiles it = g, g + 2, ...  Both walk the one A/B ring (tile it's K-blocks are
+    // uses it * uses ..), so main loops run in tile order: a warpgroup starts one when the other has finished the tile
+    // before (b_turn; the ring's parity waits then never run more than one phase ahead), and runs its epilogue while the
+    // other issues the next tile's MMAs.  The staging buffer passes from one epilogue to the next (b_stg_free).
+    const int g = mma_g;
+    const int wq = warp - (g == 0 ? W_EPI0 : W_EPI1);
+    const int tr = 3 + 2 * g;  // trace role of the warpgroup's warp 0
     constexpr int CPR = EC / 4;             // 16-byte chunks per staged row
     constexpr int RPI = 32 / CPR;           // rows covered by one warp-wide 16-byte access
     const uint32_t stg = smem_u32(epi_stage) + (uint32_t)wq * STG_WARP_BYTES;
@@ -638,13 +673,12 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     for (int k = 0; k < 2; ++k) colk[k] = (int)(((uint32_t)pc ^ (uint32_t)((k * RPI + prow) & 7)) << 2);
     const int trow = (lane >> 4) * 64 + wq * 16 + (lane & 15);  // tile row of local row `lane` (lane < ER)
     const int uses = plain ? n_chunk : n_use;
-    uint32_t ucnt = 0;
-    int it = 0;
     int etn = 0;
-    for (int tile = blockIdx.x; tile < p.n_tiles; tile += gridDim.x, ++it) {
+    for (int it = g; (int)blockIdx.x + it * (int)gridDim.x < p.n_tiles; it += NWG) {
+      const int tile = blockIdx.x + it * gridDim.x;
       const int b = tile / p.P, pat = tile - b * p.P;
       const long long mesh0 = (long long)b * p.V;
-      int* own_w = own_s + wq * 32;
+      int* own_w = own_s + (g * 4 + wq) * ER;
       {
         int v;
         if (lane >= ER) {
@@ -656,39 +690,23 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           if (v >= p.V) v = -1;
         }
         __syncwarp();  // the previous tile's readers of own_w are done
-        own_w[lane] = v;
+        if (lane < ER) own_w[lane] = v;  // (own_w is only read at rows < ER)
         __syncwarp();
       }
       int own_v[NP];
 #pragma unroll
       for (int i = 0; i < NP; ++i) own_v[i] = own_w[i * RPI + prow];
-      if (N == 128) {
-        // The staging block is this tile's again once the previous tile's output stores have read it.  An identity
-        // residual then lands in it by bulk copy (one 512-byte row per valid row, straight into the row's slot) while
-        // the main loop runs; the epilogue adds it in place.
-        if (lane < ER) bulk_wait_read0();
-        __syncwarp();
-        if (p.ep.res != nullptr && p.res_identity) {
-          const uint32_t rbar = smem_u32(b_res + wq);
-          const int n_valid = __popc(__ballot_sync(0xFFFFFFFFu, lane < ER && own_w[lane] >= 0));
-          if (lane == 0) mbar_arrive_expect_tx(rbar, (uint32_t)n_valid * (N * 4));
-          __syncwarp();
-          if (lane < ER && own_w[lane] >= 0) {
-            const long long r = mesh0 + own_w[lane];
-            bulk_g2s(stg + lane * STG_ROW_BYTES, p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + ecol0, N * 4,
-                     rbar);
-          }
-        }
-      }
-      if (p.ep.res != nullptr && (N == 64 || !p.res_identity)) {
-        // pull this tile's residual rows into L2 while its main loop is still running
-        const int lpr = ((p.apack != nullptr ? N : p.ep.res_F) * 4 + 127) >> 7;
+      if (p.ep.res != nullptr) {
+        // pull this tile's residual rows into L2 while its main loop is still running (only the CTA's own columns
+        // where they are read by column: dense GEMM, and the identity residual of N = 128)
+        const bool own_cols = p.apack != nullptr || (N == 128 && p.res_identity);
+        const int lpr = ((own_cols ? N : p.ep.res_F) * 4 + 127) >> 7;
         for (int j = lane; j < ER * lpr; j += 32) {
           const int rr = j / lpr, ln = j - rr * lpr;
           const int vtx = own_w[rr];
           if (vtx >= 0) {
             const long long r = mesh0 + vtx;
-            prefetch_l2(p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + (p.apack != nullptr ? ecol0 : 0) + ln * 32);
+            prefetch_l2(p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + (own_cols ? ecol0 : 0) + ln * 32);
           }
         }
       }
@@ -697,12 +715,17 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
-      if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 1);
+      if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 1);
+      if (NWG == 2 && it > 0) {
+        mbar_wait(smem_u32(b_turn), (uint32_t)(it - 1) & 1u, abort_flag, p.status, 13);
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 3);
+      }
+      uint32_t ucnt = (uint32_t)it * (uint32_t)uses;
       for (int u = 0; u < uses; ++u, ++ucnt) {
         const uint32_t s = ucnt % NS;
-        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 4);
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 4);
         mbar_wait(smem_u32(b_ab_full + s), (ucnt / NS) & 1, abort_flag, p.status, 6);
-        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 5);
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 5);
         const uint32_t a0 = smem_u32(ring + s * SLOT_BYTES);
         wg_fence();
 #pragma unroll
@@ -724,7 +747,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(b_ab_empty + s));  // this warp is done reading the slot
       }
-      if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 2);
+      if (NWG == 2 && lane == 0) mbar_arrive(smem_u32(b_turn));  // the next tile's main loop may start
+      if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 2);
       // N = 64, phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by
       // row)
       auto stage_slab = [&](int cb) {
@@ -777,11 +801,27 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
           zr[2] = make_float4(z[8], z[9], z[10], z[11]);
         }
       } else if (N == 128) {
-        // In the accumulator's own layout, in place: o = act(acc * mul + add), plus the identity residual the copy
-        // engine staged during the main loop, goes to the element's slot of its linear staging row
+        // The staging block is this tile's once the tile before (the other warpgroup's) has handed it over: its output
+        // stores have read it.  An identity residual then lands in it by bulk copy (one 512-byte row per valid row,
+        // straight into the row's slot, from L2: prefetched at tile start).  In the accumulator's own layout, in place:
+        // o = act(acc * mul + add), plus that residual, goes to the element's slot of its linear staging row.
+        // (b_res[wq] is armed and waited for by one tile at a time, in tile order: its phase is the tile's parity)
+        if (it > 0) mbar_wait(smem_u32(b_stg_free), (uint32_t)(it - 1) & 1u, abort_flag, p.status, 14);
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 20);
         const bool res_id = p.ep.res != nullptr && p.res_identity;
-        if (res_id) mbar_wait(smem_u32(b_res + wq), (uint32_t)it & 1u, abort_flag, p.status, 12);
-        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 21);
+        if (res_id) {
+          const uint32_t rbar = smem_u32(b_res + wq);
+          const int n_valid = __popc(__ballot_sync(0xFFFFFFFFu, lane < ER && own_w[lane] >= 0));
+          if (lane == 0) mbar_arrive_expect_tx(rbar, (uint32_t)n_valid * (N * 4));
+          __syncwarp();
+          if (lane < ER && own_w[lane] >= 0) {
+            const long long r = mesh0 + own_w[lane];
+            bulk_g2s(stg + lane * STG_ROW_BYTES, p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + ecol0, N * 4,
+                     rbar);
+          }
+          mbar_wait(rbar, (uint32_t)it & 1u, abort_flag, p.status, 12);
+        }
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 21);
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -828,9 +868,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
             }
           }
         }
-        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 22);
-        // Out by bulk copy, one 512-byte row per valid row; the warpgroup does not wait for it (the next tile's
-        // residual copies and staging writes wait for the reads of these, at its start)
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 22);
+        // Out by bulk copy, one 512-byte row per valid row; the warpgroup waits only until the copies have read the
+        // staging block, then hands it to the next tile's epilogue
         fence_async_proxy();  // this thread's staging writes -> the async proxy the copies read through
         __syncwarp();
         if (lane < ER) {
@@ -838,7 +878,11 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
             bulk_s2g(p.y + (mesh0 + own_w[lane]) * p.ldy + p.y_col0 + ecol0, stg + lane * STG_ROW_BYTES, N * 4);
           bulk_commit();
         }
-        if (wq == 0 && lane == 0) trace_ev(p, 3, etn, 23);
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 23);
+        if (lane < ER) bulk_wait_read0();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(b_stg_free));
+        if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 24);
       } else {
 #pragma unroll
         for (int cb = 0; cb < N; cb += 32) {
@@ -887,17 +931,21 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       }
     }
     if (N == 128 && lane < ER) bulk_wait0();  // the last tile's output stores read shared memory until they complete
+  } else if (warp >= NPW) {
+    // ------------------------------------------------------------ parked (N = 128): registers for the others, no work
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_PARK));
   } else {
+    if (NPW != W_PROD) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_PROD2));
     if (p.apack == nullptr) {
-    // ------------------------------------------------------------ producers (16 warps)
+    // ------------------------------------------------------------ producers (16 warps; N = 128: 8)
     const int q = tid & 7;     // float4 lane inside the 32-feature chunk
-    const int rg = tid >> 3;   // row group 0..63
+    const int rg = tid >> 3;   // row group 0..NRG-1
     const uint32_t t1s_a = smem_u32(T1s);
     const uint32_t ring_a = smem_u32(ring);
     const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
     const int n_stage = my_tiles * n_chunk;  // flat sequence of (tile, chunk) stages of this CTA
 
-    // this thread's tile rows (RPT = 1 or 2: row groups rg and 64 + rg of the tile's row order) and their CSR extents
+    // this thread's tile rows (row groups rg and NRG + rg of the tile's row order) and their CSR extents
     uint32_t row[RPT], re[RPT], ent_a = 0;
     int ptn = 0;
     // A/B ring cursor (slot, phase parity) kept incrementally, and the store offsets of this thread's rows inside an
@@ -947,8 +995,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         ent_a = mb_a + hdr->off_ent;
 #pragma unroll
         for (int ps = 0; ps < RPT; ++ps) {
-          // plain GEMM: the thread's rows are the consecutive slots rg (and 64 + rg)
-          row[ps] = plain ? (uint32_t)(64 * ps + rg) : lds_u16(ord2_a + 2 * (64 * ps + rg));
+          // plain GEMM: the thread's rows are the consecutive slots rg and NRG + rg
+          row[ps] = plain ? (uint32_t)(NRG * ps + rg) : lds_u16(ord2_a + 2 * (NRG * ps + rg));
           re[ps] = plain ? 0u : (lds_u16(rp_a + 2 * row[ps]) | (lds_u16(rp_a + 2 * row[ps] + 2) << 16));
           const uint32_t i = row[ps];
           const uint32_t a_hi = sw128_off(i, q >> 1) + (q & 1) * 8, a_lo = sw128_off(i, 4 + (q >> 1)) + (q & 1) * 8;
@@ -977,7 +1025,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         const uint32_t ablk = ring_a + s * SLOT_BYTES;
 #pragma unroll
         for (int ps = 0; ps < RPT; ++ps) {
-          const uint32_t i = ps * 64 + rg;
+          const uint32_t i = ps * NRG + rg;
           float4 v = lds_f4(xs_q + (i >> xsh) * 128);
           v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
           uint2 hi, lo;
@@ -991,7 +1039,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         __syncwarp();
         if ((tid & 31) == 0) mbar_arrive(smem_u32(b_ab_full + s));
         next_slot();
-        producer_barrier();
+        producer_barrier<NPW * 32>();
         if (tid == 0) mbar_arrive(smem_u32(b_x_empty + xs));  // stage free: the loaders may refill it
         if (tid == 0 && c == n_chunk - 1) mbar_arrive(smem_u32(b_m_empty + m));
         continue;
@@ -1077,7 +1125,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         }
       }
       if (tid == 0) trace_ev(p, 0, ptn, 7);
-      producer_barrier();  // everybody is done with Xs[xs] and T1s
+      producer_barrier<NPW * 32>();  // everybody is done with Xs[xs] and T1s
       if (tid == 0) trace_ev(p, 0, ptn, 8);
       if (tid == 0) mbar_arrive(smem_u32(b_x_empty + xs));  // stage free: the loaders may refill it
       if (tid == 0 && c == n_chunk - 1) mbar_arrive(smem_u32(b_m_empty + m));
@@ -1437,7 +1485,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
 #pragma unroll
           for (int k = 0; k < 3; ++k) mbar_arrive(smem_u32(b_t_full + (u0 + k) % DW_NS));
         }
-        producer_barrier();
+        producer_barrier<W_PROD * 32>();
         if (tid == 0) {
           mbar_arrive(smem_u32(b_x_empty + xs));
           if (c == n_chunk - 1) mbar_arrive(smem_u32(b_m_empty + m));
@@ -1818,8 +1866,8 @@ bool make_indexed_blob(const std::vector<int>& own, int tm, const int* rowptr, c
   std::stable_sort(ord2.begin(), ord2.end(), [&](unsigned short a, unsigned short b2) {
     return (int)rp[a + 1] - (int)rp[a] > (int)rp[b2 + 1] - (int)rp[b2];
   });
-  // 64-row tiles: one row per producer thread, row group rg = position rg, so the half-warp pairs are the same aligned
-  // positions (0,1), (2,3) of each group of four as for 128 rows (where a thread's second row sits 64 positions on)
+  // 64-row tiles: 32 row groups, a thread's second row sits 32 positions on (128 rows: 64), so the half-warp pairs are
+  // the same aligned positions (0,1), (2,3) of each group of four for both tile sizes
   balance_store_halves(&ord2);
   TileHeader t{};
   t.n_rows = n_rows;

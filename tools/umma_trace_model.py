@@ -31,7 +31,10 @@ with torch.no_grad():
     torch.cuda.synchronize()
     lib.p2m_debug_set_trace(h, None)
 t = buf.cpu().numpy().reshape(8, 512)
-names = {0: "producer", 1: "bload", 3: "mma + epilogue", 4: "loader"}
+# roles 3 and 5: warp 0 of MMA + epilogue warpgroup 0 (every tile, or the even tiles of the 64 x 128 configuration)
+# and 1 (its odd tiles)
+names = {0: "producer", 1: "bload", 3: "mma wg0", 4: "loader", 5: "mma wg1"}
+MMA = (3, 5)
 ev_all = []
 per_role = {r: [] for r in names}
 for role in names:
@@ -45,16 +48,17 @@ if not ev_all:
 ev_all.sort()
 t0 = ev_all[0][0]
 pn = {1: "wait_x", 2: "x_ready", 6: "T2 gathered", 7: "blocks emitted", 8: "end barrier"}
-mn = {1: "tile start", 2: "main loop done", 4: "wait full slot", 5: "slot full -> 12 MMAs",
-      # sub-phases of the 64 x 128 (N = 128) epilogue, MMA warp 0
-      20: "epi: accumulator staged", 21: "epi: residual in hand", 22: "epi: outputs computed",
-      23: "epi: output stores issued"}
+mn = {1: "tile start", 3: "turn: previous tile's main loop done", 2: "main loop done", 4: "wait full slot",
+      5: "slot full -> 12 MMAs",
+      # sub-phases of the 64 x 128 (N = 128) epilogue
+      20: "epi: staging block free", 21: "epi: residual in hand", 22: "epi: outputs computed",
+      23: "epi: output stores issued", 24: "epi: staging block handed over"}
 for c, role, ev in ev_all[:n_ev]:
     if role == 0:
         label = pn.get(ev, str(ev))
     elif role == 1:
         label = f"slot free -> load B block {ev - 10}"
-    elif role == 3:
+    elif role in MMA:
         label = mn.get(ev, str(ev))
     else:
         label = "stage free" if ev == 1 else "copies issued"
@@ -75,10 +79,15 @@ def spans(role, a, b):
 
 t1 = ev_all[-1][0]
 window = max(1, t1 - t0)
-rows = [
-    ("mma", "wait on a full slot", spans(3, 4, 5)),
-    ("mma", "issue (slot full -> next wait)", spans(3, 5, 4) + spans(3, 5, 2)),
-    ("mma", "epilogue (main loop done -> next tile)", spans(3, 2, 1)),
+rows = []
+for r in MMA:
+    if per_role[r]:
+        rows += [
+            (names[r], "wait on a full slot", spans(r, 4, 5)),
+            (names[r], "issue (slot full -> next wait)", spans(r, 5, 4) + spans(r, 5, 2)),
+            (names[r], "epilogue (main loop done -> next tile)", spans(r, 2, 1)),
+        ]
+rows += [
     ("producer", "wait on staged rows", spans(0, 1, 2)),
     ("producer", "gather", spans(0, 2, 6)),
     ("producer", "empty-slot wait + stores", spans(0, 6, 7)),
@@ -89,26 +98,52 @@ print(f"\nlogged window: {window} cycles (CTA 0; each role's log holds at most 5
 for role, what, cyc in rows:
     print(f"{role:9s} {what:40s} {cyc:10d} cycles  {100.0 * cyc / window:5.1f} %")
 
-# Per-tile split of the MMA warpgroup's time over the tiles whose main loop and epilogue are both in the log: main loop
-# (tile start -> main loop done), then every epilogue step (named after the event that ends it), up to the next tile
-# start.
-steps, tiles, cur, last = {}, 0, None, None
-for c, _, ev in per_role[3]:
-    if ev in (4, 5):
+
+def tile_intervals(role):
+    """Per tile of the warpgroup's log: {event: clock} from its tile start to the next one (complete tiles only)."""
+    out, cur = [], None
+    for c, _, ev in per_role[role]:
+        if ev in (4, 5):
+            continue
+        if ev == 1:
+            if cur is not None:
+                cur["next"] = c
+                out.append(cur)
+            cur = {1: c}
+        elif cur is not None:
+            cur[ev] = c
+    return out
+
+
+# Per-tile split of each MMA warpgroup's time over the tiles whose main loop and epilogue are both in the log: the wait
+# for the other warpgroup's main loop (64 x 128 configuration), the main loop (-> main loop done), then every epilogue
+# step (named after the event that ends it), up to the next tile start.
+main_iv, epi_iv = {}, {}
+for r in MMA:
+    tl = tile_intervals(r)
+    if not tl:
         continue
-    if ev == 1:
-        if cur is not None and last is not None:
-            cur["next tile start"] = c - last[0]
-            for k, v in cur.items():
-                steps[k] = steps.get(k, 0) + v
-            tiles += 1
-        cur, last = {}, (c, ev)
-    elif cur is not None:
-        cur["main loop" if ev == 2 else mn.get(ev, str(ev))] = c - last[0]
-        last = (c, ev)
-if tiles:
-    print(f"\nper tile, MMA warp 0, mean over {tiles} tiles (cycles)")
+    steps = {}
+    for t in tl:
+        evs = sorted((c, ev) for ev, c in t.items() if ev != "next")
+        prev = t[1]
+        for c, ev in evs[1:]:
+            k = "wait for turn" if ev == 3 else "main loop" if ev == 2 else mn.get(ev, str(ev))
+            steps[k] = steps.get(k, 0) + c - prev
+            prev = c
+        steps["next tile start"] = steps.get("next tile start", 0) + t["next"] - prev
+    print(f"\nper tile, {names[r]} warp 0, mean over {len(tl)} tiles (cycles)")
     for k, v in steps.items():
-        print(f"  {k:32s} {v / tiles:9.0f}")
-    epi = sum(v for k, v in steps.items() if k != "main loop")
-    print(f"  {'epilogue total (to next start)':32s} {epi / tiles:9.0f}")
+        print(f"  {k:32s} {v / len(tl):9.0f}")
+    epi = sum(v for k, v in steps.items() if k not in ("main loop", "wait for turn"))
+    print(f"  {'epilogue total (to next start)':32s} {epi / len(tl):9.0f}")
+    main_iv[r] = [(t.get(3, t[1]), t[2]) for t in tl if 2 in t]
+    epi_iv[r] = [(t[2], t.get(24, t["next"])) for t in tl if 2 in t]
+if len(main_iv) == 2:
+    # how much of each warpgroup's epilogue (main loop done -> staging handed over) ran while the other warpgroup's
+    # main loop did
+    for r, o in ((3, 5), (5, 3)):
+        tot = sum(b - a for a, b in epi_iv[r])
+        ov = sum(max(0, min(b, d) - max(a, c)) for a, b in epi_iv[r] for c, d in main_iv[o])
+        if tot:
+            print(f"{names[r]} epilogue under {names[o]}'s main loop: {ov} of {tot} cycles ({100.0 * ov / tot:.0f} %)")
