@@ -222,6 +222,60 @@ size_t p2m_posenet_workspace_bytes(int batch, int hidden);
 int p2m_posenet_forward(const p2m_posenet_params_t* params, const float* pose2d, float* pose3d, float* pose_combine,
                         int batch, void* workspace, size_t workspace_bytes, p2m_stream_t stream);
 
+/* ---- PoseNet in training mode: forward with batch statistics and dropout, and its backward ------------
+ * The reference's train-mode op sequence (lib/models/posenet.py:25-38,77-87), fp32 storage:
+ *   y = x W1^T + b1;  per stage  y += Wb drop(relu(bn2(Wa drop(relu(bn1(y))) + ba))) + bb;  pose3d = y W2^T + b2.
+ * BatchNorm: biased batch variance in the normalisation, unbiased in the running update, momentum 0.1, eps 1e-5;
+ * running_mean / running_var (the const pointers of p2m_posenet_stage_t) are updated in place and
+ * num_batches_tracked += 1 on the device.  The H x H layers run on the tensor cores (fp16x3, as in eval) when
+ * H % 64 == 0, in the forward, dX and dW GEMMs alike, and on the fp32 CUDA-core GEMM otherwise.  Every gradient operand
+ * of a tensor-core GEMM is scaled into fp16's range by a power of two found on the device and the scale is divided out
+ * of the result, so gradients of any magnitude keep fp32's relative accuracy; the activation operand of dW is packed
+ * times 2^6 like the weights and must stay below 2^10 in magnitude (a train-mode BatchNorm output is at most
+ * (sqrt(B - 1) |gamma| + |beta|) / (1 - p)).
+ *
+ * Dropout rule.  The mask is never stored: both calls derive it from `seed` (two int64 in DEVICE memory, read by the
+ * kernels, so the calls never synchronise and a captured graph can be replayed with fresh seeds).  Element i (flat
+ * index into [B, H]) of dropout layer d = 2 stage + {0 after bn1, 1 after bn2} is KEPT iff word (i & 3) of
+ *   Philox4x32-10(key = (low 32 bits of seed[0], high 32 bits of seed[0]),
+ *                 counter = (low 32 bits of i >> 2, high 32 bits of i >> 2, d, low 32 bits of seed[1]))
+ * is < min(floor((1 - p) 2^32), 2^32 - 1), (1 - p) evaluated in double from the float p; a kept value is multiplied by the float
+ * 1 / (1 - p).  p == 0: no dropout (no random numbers are drawn); p == 1: everything is zeroed.
+ *
+ * `saved` (p2m_posenet_train_saved_bytes; written by the forward, read by the backward) holds, each array starting
+ * at a multiple of 256 bytes: y_0 .. y_S [B, H] each (S = num_stage; y_s is the input of stage s, y_S of the output
+ * layer), then z2_0 .. z2_{S-1} [B, H] (the pre-bn2 output of each stage's first Linear), then per stage and per
+ * BatchNorm (bn1, bn2) the vectors mean | invstd | scale | shift [H] each.  The dropped activations are recomputed in
+ * the backward.  One workspace size serves both calls.  Gradients are written, not accumulated.  batch >= 2
+ * (a batch of one has no batch statistics: P2M_ERR_INVALID).                                              */
+typedef struct {
+  int64_t* bn1_nbt; int64_t* bn2_nbt;          /* num_batches_tracked of the stage's BatchNorms (device, may be NULL) */
+} p2m_posenet_train_stage_t;
+typedef struct {
+  const p2m_posenet_train_stage_t* stages;     /* [num_stage] (host array of device pointers) */
+} p2m_posenet_train_t;
+typedef struct {
+  float* w1_w; float* w1_b; float* w2_w; float* w2_b;
+  float* bn1_w; float* bn1_b; float* bn2_w; float* bn2_b;
+} p2m_posenet_stage_grads_t;
+typedef struct {
+  float* w1_w; float* w1_b; float* w2_w; float* w2_b;     /* shapes of the parameters */
+  const p2m_posenet_stage_grads_t* stages;                /* [num_stage] (host array of device pointers) */
+} p2m_posenet_grads_t;
+size_t p2m_posenet_train_workspace_bytes(int batch, int num_joint, int hidden, int num_stage);
+size_t p2m_posenet_train_saved_bytes(int batch, int num_joint, int hidden, int num_stage);
+/* pose2d [B, 2J] -> pose3d [B, 3J]; pose_combine (optional) [B, J, 5] as in p2m_posenet_forward. */
+int p2m_posenet_train_forward(const p2m_posenet_params_t* params, const p2m_posenet_train_t* extra, const float* pose2d,
+                              int batch, float p_dropout, const int64_t* seed, float* pose3d, float* pose_combine,
+                              void* saved, size_t saved_bytes, void* workspace, size_t workspace_bytes,
+                              p2m_stream_t stream);
+/* d_pose3d [B, 3J] -> grads (every pointer required) and, optionally, d_pose2d [B, 2J]; params, pose2d, p_dropout,
+ * seed and saved as in the forward that wrote `saved`. */
+int p2m_posenet_backward(const p2m_posenet_params_t* params, const float* pose2d, int batch, float p_dropout,
+                         const int64_t* seed, const void* saved, size_t saved_bytes, const float* d_pose3d,
+                         const p2m_posenet_grads_t* grads, float* d_pose2d, void* workspace, size_t workspace_bytes,
+                         p2m_stream_t stream);
+
 /* ---- the steps either side of the model in the reference's callers (SURVEY.md §8 row f2) ----------
  * Joint regression (lib/core/base.py:131,204; demo/run.py:171): joints [B, n_joint, C] = joint_regressor
  * [n_joint, n_vertex] @ vertices [B, n_vertex, C] (C <= 4), on the gathered vertices of

@@ -95,6 +95,23 @@ class PoseNetParams(C.Structure):
                 ("stages", C.POINTER(PoseNetStage))]
 
 
+class PoseNetTrainStage(C.Structure):
+    _fields_ = [("bn1_nbt", C.c_void_p), ("bn2_nbt", C.c_void_p)]
+
+
+class PoseNetTrain(C.Structure):
+    _fields_ = [("stages", C.POINTER(PoseNetTrainStage))]
+
+
+class PoseNetStageGrads(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("w1_w", "w1_b", "w2_w", "w2_b", "bn1_w", "bn1_b", "bn2_w", "bn2_b")]
+
+
+class PoseNetGrads(C.Structure):
+    _fields_ = [("w1_w", C.c_void_p), ("w1_b", C.c_void_p), ("w2_w", C.c_void_p), ("w2_b", C.c_void_p),
+                ("stages", C.POINTER(PoseNetStageGrads))]
+
+
 class BodyModelDesc(C.Structure):
     _fields_ = [
         ("n_vertex", C.c_int32), ("n_joint", C.c_int32), ("n_betas", C.c_int32), ("n_out_joints", C.c_int32),
@@ -119,7 +136,9 @@ EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
     "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
-    "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward", "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
+    "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
+    "p2m_posenet_train_workspace_bytes", "p2m_posenet_train_saved_bytes", "p2m_posenet_train_forward", "p2m_posenet_backward",
+    "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
     "p2m_rigid_align", "p2m_point_errors", "p2m_fit_camera", "p2m_crop_cam_to_orig",
     "p2m_one_euro_smooth", "p2m_accel_error", "p2m_segment_mean",
     "p2m_nearest_distances", "p2m_align_w_scale", "p2m_pck_accumulate",
@@ -202,6 +221,15 @@ def load() -> C.CDLL:
         lib.p2m_posenet_workspace_bytes.restype = sz
         lib.p2m_posenet_forward.argtypes = [C.POINTER(PoseNetParams), vp, vp, vp, C.c_int, vp, sz, vp]
         lib.p2m_posenet_forward.restype = C.c_int
+        for fn in (lib.p2m_posenet_train_workspace_bytes, lib.p2m_posenet_train_saved_bytes):
+            fn.argtypes = [C.c_int] * 4
+            fn.restype = sz
+        lib.p2m_posenet_train_forward.argtypes = [C.POINTER(PoseNetParams), C.POINTER(PoseNetTrain), vp, C.c_int,
+                                                  C.c_float, vp, vp, vp, vp, sz, vp, sz, vp]
+        lib.p2m_posenet_train_forward.restype = C.c_int
+        lib.p2m_posenet_backward.argtypes = [C.POINTER(PoseNetParams), vp, C.c_int, C.c_float, vp, vp, sz, vp,
+                                             C.POINTER(PoseNetGrads), vp, vp, sz, vp]
+        lib.p2m_posenet_backward.restype = C.c_int
         lib.p2m_regress_joints.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         lib.p2m_regress_joints.restype = C.c_int
         lib.p2m_normalize_pose2d.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]

@@ -38,6 +38,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <climits>
 #include <cstdlib>
 #include <cstring>
 #include <vector>
@@ -1589,8 +1590,8 @@ __global__ void __launch_bounds__(512, 2) k_cheb_t1(const T1Params p) {
 // What k_pack turns into an operand image: K-blocks of `rows` rows x 32 k as fp16 [hi 32 | lo 32] per 128-byte row, in
 // the exact shared-memory image (128B-swizzled), so a kernel fetches a block with a single cp.async.bulk.  Block
 // b = (t * n_chunk + chunk) * orders + order holds rows n = t * rows + [0, rows) and k = 32 chunk + [0, 32):
-// p[n ld_row + k ld_k + order] * scale, zero for n >= n_real; `combined`: the isolated rows' combined weights
-// (p[a] + c p[a + 1] + (2c^2 - 1) p[a + 2]) * scale at a = n ld_row + k ld_k.
+// p[n ld_row + k ld_k + order] * scale, zero for n >= n_real or k >= k_real (never read there); `combined`: the isolated
+// rows' combined weights (p[a] + c p[a + 1] + (2c^2 - 1) p[a + 2]) * scale at a = n ld_row + k ld_k.
 struct PackSrc {
   const float* p;
   long long ld_row, ld_k;
@@ -1598,6 +1599,7 @@ struct PackSrc {
   float scale;  // W_SCALE for weights, 1 for activations
   int combined;
   float c;
+  int k_real = INT_MAX;
 };
 __global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, unsigned char* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
@@ -1608,14 +1610,15 @@ __global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, 
   const int per_tile = s.n_chunk * s.orders;
   const long long n = blk / per_tile * s.rows + row;
   const int u = (int)(blk % per_tile);
-  const float* src = s.p + n * s.ld_row + (long long)((u / s.orders) * FC + (j & 3) * 8) * s.ld_k + u % s.orders;
+  const int k0 = (u / s.orders) * FC + (j & 3) * 8;
+  const float* src = s.p + n * s.ld_row + (long long)k0 * s.ld_k + u % s.orders;
   const float c = s.c, c2 = 2.f * c * c - 1.f;
   __align__(16) __half h[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     const float* wr = src + e * s.ld_k;
     float w = 0.f;
-    if (n < s.n_real) w = s.combined ? (wr[0] + c * wr[1] + c2 * wr[2]) * s.scale : wr[0] * s.scale;
+    if (n < s.n_real && k0 + e < s.k_real) w = s.combined ? (wr[0] + c * wr[1] + c2 * wr[2]) * s.scale : wr[0] * s.scale;
     const __half hi = __float2half_rn(w);
     h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
   }
@@ -2119,9 +2122,14 @@ int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
 // (apack / wpack: caller-provided scratch of umma_gemm_{a,w}pack_bytes), then every K-block of both operands is
 // streamed by cp.async.bulk into the conv kernel's A/B ring — no producer warps, one CTA per (128-row tile, output
 // column slice).  The epilogue vectors and an identity residual (ep.res with res_F == N) are indexed by output column.
-int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const Epilogue& ep, float* Y, void* apack,
-                     void* wpack, int* status, int sm_count, cudaStream_t s, int n_real) {
+// Either operand is read by row and k stride, so a transposed view costs nothing: the backward's dX = g W is
+// X = g, W = {W, 1, ld} and dW = g^T a is X = {g, 1, ld}, W = {a, 1, ld}.  k >= k_real is zero padding.  a_scale: X was
+// multiplied by this device scalar by the caller; the epilogue divides it out.
+int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Epilogue& ep, float* Y, void* apack,
+                     void* wpack, int* status, int sm_count, cudaStream_t s, int n_real, int k_real,
+                     const float* a_scale) {
   if (n_real <= 0 || n_real > N) n_real = N;  // W has n_real rows; output columns >= n_real are zero-weight padding
+  if (k_real <= 0 || k_real > K) k_real = K;
   if (!umma_gemm_supported(M, N, K) || (ep.res != nullptr && ep.res_F != N)) {
     set_error("umma_gemm: unsupported shape");
     return P2M_ERR_INVALID;
@@ -2130,8 +2138,10 @@ int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const 
   const int ns = CONV_N;  // one warpgroup's register accumulator: 64 output columns per CTA
   // A: one 16 KB block per (128-row tile, 32-column chunk), rows >= M zero (what the producers would have built);
   // W: the images of all output-column slices, slice j = rows [j ns, (j + 1) ns) of W, rows >= n_real zero
-  P2M_TRY(launch_pack(PackSrc{X, K, 1, TILE_M, K / FC, 1, M, 1.f, 0, 0.f}, (long long)tiles * (K / FC), apack, s));
-  P2M_TRY(launch_pack(PackSrc{W, K, 1, ns, K / FC, 1, n_real, W_SCALE, 0, 0.f}, (long long)(N / ns) * (K / FC), wpack, s));
+  P2M_TRY(launch_pack(PackSrc{X.p, X.ld_row, X.ld_k, TILE_M, K / FC, 1, M, 1.f, 0, 0.f, k_real},
+                      (long long)tiles * (K / FC), apack, s));
+  P2M_TRY(launch_pack(PackSrc{W.p, W.ld_row, W.ld_k, ns, K / FC, 1, n_real, W_SCALE, 0, 0.f, k_real},
+                      (long long)(N / ns) * (K / FC), wpack, s));
   KParams p;
   std::memset(&p, 0, sizeof(p));
   p.V = M;                // one "mesh" of M rows: the epilogue masks rows >= V of the last tile
@@ -2140,6 +2150,7 @@ int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const 
   p.n_tiles = tiles;
   p.wpack = static_cast<const unsigned char*>(wpack);
   p.apack = static_cast<const unsigned char*>(apack);
+  p.a_scale = a_scale;
   p.ep = to_dev(ep);
   p.res_identity = (ep.res != nullptr) ? 1 : 0;
   p.ldy = N;

@@ -107,21 +107,6 @@ int check_kernel_status(p2m_model* m, const char* where) {
   return P2M_ERR_CUDA;
 }
 
-constexpr size_t ALIGN = 256;
-inline size_t align_up(size_t x) { return (x + ALIGN - 1) / ALIGN * ALIGN; }
-
-struct Bump {
-  char* base;
-  size_t off = 0;
-  explicit Bump(void* p) : base(static_cast<char*>(p)) {}
-  template <class T>
-  T* take(size_t n) {
-    T* p = reinterpret_cast<T*>(base + off);
-    off += align_up(n * sizeof(T));
-    return p;
-  }
-};
-
 template <class T>
 int upload(p2m_model* m, const std::vector<T>& h, T** out) {
   T* d = nullptr;
@@ -994,7 +979,7 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
         out = w.fc_out;
       }
       if (m->precision == P2M_PREC_FP16X3_TC && w.fc_apack != nullptr)  // dense GEMM on the tensor cores (wgmma, fp16x3)
-        P2M_TRY(launch_umma_gemm(cur, P->fc_w, B, m->fc_out, m->fc_in, ep, out, w.fc_apack, w.fc_wpack, m->kernel_status,
+        P2M_TRY(launch_umma_gemm({cur, m->fc_in, 1}, {P->fc_w, m->fc_in, 1}, B, m->fc_out, m->fc_in, ep, out, w.fc_apack, w.fc_wpack, m->kernel_status,
                                  m->sm_count, s));
       else
         P2M_TRY(launch_gemm(cur, m->fc_in, P->fc_w, m->fc_in, 0, out, m->fc_out, B, m->fc_out, m->fc_in, ep, s));
@@ -1496,6 +1481,20 @@ __global__ void __launch_bounds__(256) k_pose_combine(const float* __restrict__ 
 }
 }  // namespace
 
+namespace p2m {
+int launch_take_cols(const float* src, int ld, const float* bias, int n_col, long long rows, float* dst, cudaStream_t s) {
+  const long long n = rows * n_col;
+  k_take_cols<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src, ld, bias, n_col, n, dst);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+int launch_pose_combine(const float* pose2d, const float* pose3d, long long n_joint_rows, float* out, cudaStream_t s) {
+  k_pose_combine<<<(unsigned)((n_joint_rows + 255) / 256), 256, 0, s>>>(pose2d, pose3d, n_joint_rows, out);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+}  // namespace p2m
+
 extern "C" {
 
 size_t p2m_posenet_workspace_bytes(int batch, int hidden) {
@@ -1539,7 +1538,7 @@ int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, floa
     P2M_CUDA_OK(cudaMemsetAsync(status, 0, sizeof(int), s));
   }
   auto big_gemm = [&](const float* X, const float* Wm, const Epilogue& e, float* Y) -> int {
-    if (tc) return launch_umma_gemm(X, Wm, B, H, H, e, Y, apack, wpack, status, sm_count, s);
+    if (tc) return launch_umma_gemm({X, H, 1}, {Wm, H, 1}, B, H, H, e, Y, apack, wpack, status, sm_count, s);
     return launch_gemm(X, H, Wm, H, 0, Y, H, B, H, H, e, s);
   };
   Epilogue e1;
@@ -1574,20 +1573,14 @@ int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, floa
   if (tc && 3 * J <= 64) {
     // the K = H reduction of the output layer on the tensor cores as well: N padded to 64 zero-weight columns (two CTAs of
     // the fp32 SIMT GEMM would walk the 4096-long reduction alone), then the 3J real columns are copied out + bias
-    P2M_TRY(launch_umma_gemm(y, P->w2_w, B, 64, H, Epilogue(), h, apack, wpack, status, sm_count, s, 3 * J));
-    const long long n = (long long)B * 3 * J;
-    k_take_cols<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(h, 64, P->w2_b, 3 * J, n, pose3d);
-    P2M_LAUNCH_OK();
+    P2M_TRY(launch_umma_gemm({y, H, 1}, {P->w2_w, H, 1}, B, 64, H, Epilogue(), h, apack, wpack, status, sm_count, s, 3 * J));
+    P2M_TRY(launch_take_cols(h, 64, P->w2_b, 3 * J, B, pose3d, s));
   } else {
     Epilogue e2;
     e2.bias = P->w2_b;
     P2M_TRY(launch_gemm(y, H, P->w2_w, H, 0, pose3d, 3 * J, B, 3 * J, H, e2, s));
   }
-  if (pose_combine != nullptr) {
-    const long long n = (long long)B * J;
-    k_pose_combine<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(pose2d, pose3d, n, pose_combine);
-    P2M_LAUNCH_OK();
-  }
+  if (pose_combine != nullptr) P2M_TRY(launch_pose_combine(pose2d, pose3d, (long long)B * J, pose_combine, s));
   return P2M_OK;
 }
 

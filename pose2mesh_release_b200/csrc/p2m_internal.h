@@ -85,6 +85,21 @@ struct StreamBuffer {
   StreamBuffer& operator=(const StreamBuffer&) = delete;
 };
 
+// Carving a caller-provided workspace into 256-byte aligned arrays.
+constexpr size_t ALIGN = 256;
+inline size_t align_up(size_t x) { return (x + ALIGN - 1) / ALIGN * ALIGN; }
+struct Bump {
+  char* base;
+  size_t off = 0;
+  explicit Bump(void* p) : base(static_cast<char*>(p)) {}
+  template <class T>
+  T* take(size_t n) {
+    T* p = reinterpret_cast<T*>(base + off);
+    off += align_up(n * sizeof(T));
+    return p;
+  }
+};
+
 // CTAs of a grid-stride launch: ceil(work / per_cta), clamped to [1, max_ctas].
 inline unsigned grid_for(long long work, int per_cta, long long max_ctas) {
   const long long g = (work + per_cta - 1) / per_cta;
@@ -346,12 +361,23 @@ int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, 
 int launch_umma_conv(const UmmaConvArgs& a, int* status_flag, const float* zero_row, int sm_count, cudaStream_t s);
 // Dense GEMM on the tensor cores (wgmma, fp16x3): Y [M, N] = epilogue(X [M, K] W [N, K]^T), K % 32 == 0, N % 64 == 0; apack / wpack are
 // scratch of umma_gemm_apack_bytes(M, K) / umma_gemm_wpack_bytes(N, K); ep vectors and an identity residual
-// (ep.res, res_F == N) are indexed by output column.
+// (ep.res, res_F == N) are indexed by output column.  An operand's element (row r, k) is p[r ld_row + k ld_k]: a
+// row-major matrix is {p, ld, 1}, its transpose {p, 1, ld}.
+struct GemmOperand {
+  const float* p;
+  long long ld_row, ld_k;
+};
 bool umma_gemm_supported(int M, int N, int K);
 size_t umma_gemm_apack_bytes(int M, int K);
 size_t umma_gemm_wpack_bytes(int N, int K);
-int launch_umma_gemm(const float* X, const float* W, int M, int N, int K, const Epilogue& ep, float* Y, void* apack,
-                     void* wpack, int* status, int sm_count, cudaStream_t s, int n_real = 0 /* rows of W if < N */);
+int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Epilogue& ep, float* Y, void* apack,
+                     void* wpack, int* status, int sm_count, cudaStream_t s, int n_real = 0 /* rows of W if < N */,
+                     int k_real = 0 /* k >= k_real is zero padding, if < K */,
+                     const float* a_scale = nullptr /* device scalar X was multiplied by; divided out of Y */);
+// PoseNet's output stage, shared by the eval and the train forward (p2m_api.cu): dst [rows, n_col] = src[:, :n_col] (row
+// stride ld) + bias, and pose_combine [B J, 5] = cat(pose2d [B J, 2], pose3d [B J, 3] / 1000)
+int launch_take_cols(const float* src, int ld, const float* bias, int n_col, long long rows, float* dst, cudaStream_t s);
+int launch_pose_combine(const float* pose2d, const float* pose3d, long long n_joint_rows, float* out, cudaStream_t s);
 // out[ro, :] = sum over the logical rows r of physical row ro (r = ro, or 2 ro and 2 ro + 1 under the virtual unpool)
 // of  dxl[r, :] + resample^T(g_res[r, :])   (g_res may be null)
 int launch_dx_finish(const float* dxl, int rows, int F, const float* g_res, int res_Fout, const InterpTable* it,

@@ -1,0 +1,389 @@
+// PoseNet in training mode (lib/models/posenet.py:25-38,77-87; lib/core/base.py:116,246-265): the forward with batch
+// statistics and dropout, and the backward.  include/p2m_b200.h states the math, the dropout rule and the layout of
+// `saved`.  The BatchNorm statistics, the BN + ReLU backward, the bias sums, the range scaling of the gradients and both
+// GEMMs are the library's own (kernels_simt.cu, cheb_umma.cu); new here are the counter-based dropout fused into the
+// BN-apply + ReLU pass, its backward, and the assembly.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <string>
+
+#include "p2m_internal.h"
+
+using namespace p2m;
+
+namespace {
+
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11)
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const unsigned int hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const unsigned int hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// How one dropout layer treats its elements: mode 0 keeps everything unscaled (p == 0), 1 draws, 2 zeroes (p == 1)
+struct Dropout {
+  const long long* seed;  // device [2]
+  unsigned int layer, threshold;
+  float keep_scale;
+  int mode;
+};
+// multipliers of the four elements 4 q .. 4 q + 3
+__device__ __forceinline__ void dropout_mul4(const Dropout& d, unsigned long long q, float m[4]) {
+  if (d.mode != 1) {
+    m[0] = m[1] = m[2] = m[3] = d.mode == 0 ? 1.f : 0.f;
+    return;
+  }
+  const unsigned long long s0 = (unsigned long long)d.seed[0];
+  const uint4 w = philox4x32_10(make_uint4((unsigned int)q, (unsigned int)(q >> 32), d.layer, (unsigned int)d.seed[1]),
+                                make_uint2((unsigned int)s0, (unsigned int)(s0 >> 32)));
+  m[0] = w.x < d.threshold ? d.keep_scale : 0.f;
+  m[1] = w.y < d.threshold ? d.keep_scale : 0.f;
+  m[2] = w.z < d.threshold ? d.keep_scale : 0.f;
+  m[3] = w.w < d.threshold ? d.keep_scale : 0.f;
+}
+
+// a = drop(relu(z * scale + shift)): four consecutive elements (one Philox counter) per thread
+__global__ void __launch_bounds__(256) k_pn_bn_relu_drop(const float* __restrict__ z, long long n, int F,
+                                                         const float* __restrict__ scale, const float* __restrict__ shift,
+                                                         const Dropout d, float* __restrict__ a) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (4 * q >= n) return;
+  float m[4];
+  dropout_mul4(d, (unsigned long long)q, m);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const long long i = 4 * q + e;
+    if (i < n) {
+      const int f = (int)(i % F);
+      a[i] = fmaxf(fmaf(z[i], scale[f], shift[f]), 0.f) * m[e];
+    }
+  }
+}
+// g *= the same multipliers (in place): the gradient through drop()
+__global__ void __launch_bounds__(256) k_pn_drop_bwd(float* __restrict__ g, long long n, const Dropout d) {
+  const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (4 * q >= n) return;
+  float m[4];
+  dropout_mul4(d, (unsigned long long)q, m);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const long long i = 4 * q + e;
+    if (i < n) g[i] *= m[e];
+  }
+}
+__global__ void __launch_bounds__(256) k_pn_add(float* __restrict__ y, const float* __restrict__ x, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) y[i] += x[i];
+}
+// out [C, R] = in [R, C]^T
+__global__ void __launch_bounds__(256) k_pn_transpose(const float* __restrict__ in, int R, int C, float* __restrict__ out) {
+  __shared__ float t[32][33];
+  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (int j = ty; j < 32; j += 8)
+    if (r0 + j < R && c0 + tx < C) t[j][tx] = in[(long long)(r0 + j) * C + c0 + tx];
+  __syncthreads();
+  for (int j = ty; j < 32; j += 8)
+    if (c0 + j < C && r0 + tx < R) out[(long long)(c0 + j) * R + r0 + tx] = t[tx][j];
+}
+
+inline unsigned blocks(long long n) { return (unsigned)((n + 255) / 256); }
+
+Dropout make_dropout(float p, const int64_t* seed, int layer) {
+  Dropout d;
+  d.seed = reinterpret_cast<const long long*>(seed);
+  d.layer = (unsigned int)layer;
+  d.mode = p <= 0.f ? 0 : (p >= 1.f ? 2 : 1);
+  d.threshold = d.mode == 1 ? (unsigned int)std::min((1.0 - (double)p) * 4294967296.0, 4294967295.0) : 0u;
+  d.keep_scale = d.mode == 1 ? 1.f / (1.f - p) : 1.f;
+  return d;
+}
+
+int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// Shapes, the path the H x H GEMMs take, and the two memory layouts.
+struct Plan {
+  int B, J, H, S;
+  bool tc;      // H x H GEMMs on the tensor cores in all three directions
+  int Bp;       // the dW GEMM's K = B padded with zero rows to the K-block
+  size_t bh;    // floats of one [B, H] array
+  Plan(int batch, int num_joint, int hidden, int num_stage)
+      : B(batch), J(num_joint), H(hidden), S(num_stage), tc(umma_gemm_supported(batch, hidden, hidden)),
+        Bp(round_up(batch, 32)), bh((size_t)batch * hidden) {}
+  size_t apack_bytes() const { return std::max(umma_gemm_apack_bytes(B, H), umma_gemm_apack_bytes(H, Bp)); }
+  size_t wpack_bytes() const { return std::max(umma_gemm_wpack_bytes(H, H), umma_gemm_wpack_bytes(H, Bp)); }
+  int wide() const { return std::max(H, 3 * J); }
+  size_t saved_bytes() const { return (size_t)(2 * S + 1) * align_up(bh * 4) + (size_t)S * 8 * align_up((size_t)H * 4); }
+  size_t workspace_bytes() const {
+    size_t n = 4 * align_up(bh * 4) + align_up((size_t)wide() * B * 4) + align_up((size_t)B * 64 * 4) +
+               align_up((size_t)wide() * (2 * 8 + 5 * 4)) + 2 * ALIGN;
+    if (tc) n += align_up(apack_bytes()) + align_up(wpack_bytes());
+    return n;
+  }
+};
+struct Saved {
+  char* base;
+  const Plan& p;
+  float* y(int s) const { return reinterpret_cast<float*>(base + (size_t)s * align_up(p.bh * 4)); }
+  float* z2(int s) const { return y(p.S + 1 + s); }
+  // v: 0 mean, 1 invstd, 2 scale, 3 shift of BatchNorm `bn` (0, 1) of stage s
+  float* stat(int s, int bn, int v) const {
+    return reinterpret_cast<float*>(base + (size_t)(2 * p.S + 1) * align_up(p.bh * 4) +
+                                    (size_t)((s * 2 + bn) * 4 + v) * align_up((size_t)p.H * 4));
+  }
+};
+struct Work {
+  float *g, *a, *t, *gs, *gT, *h64;
+  double* sums;  // launch_bn_relu_bwd's scratch: 2 F doubles + 5 F floats
+  float* g_scale;
+  int* status;
+  void *apack = nullptr, *wpack = nullptr;
+  Work(void* ws, const Plan& p) {
+    Bump b(ws);
+    g = b.take<float>(p.bh);
+    a = b.take<float>(p.bh);
+    t = b.take<float>(p.bh);
+    gs = b.take<float>(p.bh);
+    gT = b.take<float>((size_t)p.wide() * p.B);
+    h64 = b.take<float>((size_t)p.B * 64);
+    sums = reinterpret_cast<double*>(b.take<char>((size_t)p.wide() * (2 * 8 + 5 * 4)));
+    g_scale = b.take<float>(1);
+    status = b.take<int>(1);
+    if (p.tc) {
+      apack = b.take<unsigned char>(p.apack_bytes());
+      wpack = b.take<unsigned char>(p.wpack_bytes());
+    }
+  }
+};
+
+bool params_ok(const p2m_posenet_params_t* P) {
+  if (!P || P->num_joint <= 0 || P->hidden <= 0 || P->num_stage < 0 || !P->w1_w || !P->w1_b || !P->w2_w || !P->w2_b ||
+      (P->num_stage > 0 && !P->stages))
+    return false;
+  for (int st = 0; st < P->num_stage; ++st) {
+    const p2m_posenet_stage_t& S = P->stages[st];
+    if (!S.w1_w || !S.w1_b || !S.w2_w || !S.w2_b || !S.bn1_w || !S.bn1_b || !S.bn1_rm || !S.bn1_rv || !S.bn2_w ||
+        !S.bn2_b || !S.bn2_rm || !S.bn2_rv)
+      return false;
+  }
+  return true;
+}
+
+int check_call(const char* where, const p2m_posenet_params_t* P, int B, float p_dropout, bool pointers_ok,
+               size_t saved_bytes, size_t workspace_bytes) {
+  if (!pointers_ok || !params_ok(P) || B <= 0 || !(p_dropout >= 0.f && p_dropout <= 1.f)) {
+    set_error(std::string(where) + ": bad argument");
+    return P2M_ERR_INVALID;
+  }
+  if (B < 2) {
+    set_error(std::string(where) + ": train-mode BatchNorm needs more than one value per channel (batch of 1)");
+    return P2M_ERR_INVALID;
+  }
+  const Plan plan(B, P->num_joint, P->hidden, P->num_stage);
+  if (saved_bytes < plan.saved_bytes() || workspace_bytes < plan.workspace_bytes()) {
+    set_error(std::string(where) + ": saved or workspace buffer too small");
+    return P2M_ERR_WORKSPACE;
+  }
+  return P2M_OK;
+}
+
+// The three H x H GEMMs, on the tensor cores or on the fp32 CUDA-core GEMM by the plan.
+struct Gemms {
+  const Plan& p;
+  const Work& w;
+  int sm_count;
+  cudaStream_t s;
+  // Y [B, H] = epilogue(X [B, H] W^T)
+  int forward(const float* X, const float* W, const Epilogue& e, float* Y) const {
+    const int H = p.H;
+    if (p.tc) return launch_umma_gemm({X, H, 1}, {W, H, 1}, p.B, H, H, e, Y, w.apack, w.wpack, w.status, sm_count, s);
+    return launch_gemm(X, H, W, H, 0, Y, H, p.B, H, H, e, s);
+  }
+  // the gradient operand of the two backward GEMMs: scaled into fp16's range once (w.gs, w.g_scale) for the tensor
+  // cores, transposed once (w.gT) for the CUDA-core dW
+  int prepare(const float* g, bool have_scale) const {
+    if (!p.tc) return transpose(g, p.B, p.H);
+    if (!have_scale) P2M_TRY(launch_absmax_scale(g, (long long)p.bh, w.g_scale, s));
+    return launch_scale_by(g, (long long)p.bh, w.g_scale, 0, 1.f, w.gs, s);
+  }
+  // dX [B, H] = g [B, H] W [H, H]
+  int dx(const float* g, const float* W, float* dX) const {
+    const int H = p.H;
+    if (p.tc)
+      return launch_umma_gemm({w.gs, H, 1}, {W, 1, H}, p.B, H, H, Epilogue(), dX, w.apack, w.wpack, w.status, sm_count, s,
+                              0, 0, w.g_scale);
+    return launch_gemm(g, H, W, H, 1, dX, H, p.B, H, H, Epilogue(), s);
+  }
+  // dW [H, H] = g^T [H, B] a [B, H]
+  int dw(const float* a, float* dW) const {
+    const int H = p.H;
+    if (p.tc)
+      return launch_umma_gemm({w.gs, 1, H}, {a, 1, H}, H, H, p.Bp, Epilogue(), dW, w.apack, w.wpack, w.status, sm_count,
+                              s, 0, p.B, w.g_scale);
+    return launch_gemm(w.gT, p.B, a, H, 1, dW, H, H, H, p.B, Epilogue(), s);
+  }
+  int transpose(const float* in, int R, int C) const {
+    k_pn_transpose<<<dim3((C + 31) / 32, (R + 31) / 32), 256, 0, s>>>(in, R, C, w.gT);
+    P2M_LAUNCH_OK();
+    return P2M_OK;
+  }
+};
+
+int bn_relu_drop(const float* z, const Plan& p, const float* scale, const float* shift, const Dropout& d, float* a,
+                 cudaStream_t s) {
+  k_pn_bn_relu_drop<<<blocks(((long long)p.bh + 3) / 4), 256, 0, s>>>(z, (long long)p.bh, p.H, scale, shift, d, a);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t p2m_posenet_train_workspace_bytes(int batch, int num_joint, int hidden, int num_stage) {
+  if (batch <= 0 || num_joint <= 0 || hidden <= 0 || num_stage < 0) return 0;
+  return Plan(batch, num_joint, hidden, num_stage).workspace_bytes();
+}
+size_t p2m_posenet_train_saved_bytes(int batch, int num_joint, int hidden, int num_stage) {
+  if (batch <= 0 || num_joint <= 0 || hidden <= 0 || num_stage < 0) return 0;
+  return Plan(batch, num_joint, hidden, num_stage).saved_bytes();
+}
+
+int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra, const float* pose2d, int B,
+                              float p_dropout, const int64_t* seed, float* pose3d, float* pose_combine, void* saved,
+                              size_t saved_bytes, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  P2M_TRY(check_call("posenet_train_forward", P, B, p_dropout,
+                     pose2d && seed && pose3d && saved && workspace && (!P || P->num_stage == 0 || (extra && extra->stages)),
+                     saved_bytes, workspace_bytes));
+  int dev;
+  P2M_TRY(arrays_device("posenet_train_forward", {pose2d, seed, pose3d, pose_combine, saved, workspace}, &dev));
+  DeviceGuard guard(dev);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const Plan plan(B, P->num_joint, P->hidden, P->num_stage);
+  const Saved sv{static_cast<char*>(saved), plan};
+  const Work w(workspace, plan);
+  const int H = plan.H, J = plan.J;
+  Gemms gemm{plan, w, 132, s};
+  if (plan.tc) {
+    P2M_CUDA_OK(cudaDeviceGetAttribute(&gemm.sm_count, cudaDevAttrMultiProcessorCount, dev));
+    P2M_CUDA_OK(cudaMemsetAsync(w.status, 0, sizeof(int), s));
+  }
+  Epilogue e1;
+  e1.bias = P->w1_b;
+  P2M_TRY(launch_gemm(pose2d, 2 * J, P->w1_w, 2 * J, 0, sv.y(0), H, B, H, 2 * J, e1, s));
+  for (int st = 0; st < plan.S; ++st) {
+    const p2m_posenet_stage_t& S = P->stages[st];
+    const p2m_posenet_train_stage_t& X = extra->stages[st];
+    const float* y = sv.y(st);
+    // a = drop(relu(bn1(y)))
+    P2M_TRY(launch_col_stats(y, B, H, w.sums, s));
+    P2M_TRY(launch_bn_finalize(w.sums, y, B, H, S.bn1_w, S.bn1_b, const_cast<float*>(S.bn1_rm),
+                               const_cast<float*>(S.bn1_rv), X.bn1_nbt, sv.stat(st, 0, 0), sv.stat(st, 0, 1),
+                               sv.stat(st, 0, 2), sv.stat(st, 0, 3), s));
+    P2M_TRY(bn_relu_drop(y, plan, sv.stat(st, 0, 2), sv.stat(st, 0, 3), make_dropout(p_dropout, seed, 2 * st), w.a, s));
+    // z2 = a Wa^T + ba;  a = drop(relu(bn2(z2)))
+    Epilogue ea;
+    ea.bias = S.w1_b;
+    P2M_TRY(gemm.forward(w.a, S.w1_w, ea, sv.z2(st)));
+    P2M_TRY(launch_col_stats(sv.z2(st), B, H, w.sums, s));
+    P2M_TRY(launch_bn_finalize(w.sums, sv.z2(st), B, H, S.bn2_w, S.bn2_b, const_cast<float*>(S.bn2_rm),
+                               const_cast<float*>(S.bn2_rv), X.bn2_nbt, sv.stat(st, 1, 0), sv.stat(st, 1, 1),
+                               sv.stat(st, 1, 2), sv.stat(st, 1, 3), s));
+    P2M_TRY(bn_relu_drop(sv.z2(st), plan, sv.stat(st, 1, 2), sv.stat(st, 1, 3), make_dropout(p_dropout, seed, 2 * st + 1),
+                         w.a, s));
+    // y' = y + a Wb^T + bb
+    Epilogue eb;
+    eb.bias = S.w2_b;
+    eb.res = y;
+    eb.res_F = H;
+    P2M_TRY(gemm.forward(w.a, S.w2_w, eb, sv.y(st + 1)));
+  }
+  const float* y = sv.y(plan.S);
+  if (plan.tc && 3 * J <= 64) {  // the K = H reduction of the output layer on the tensor cores, as in p2m_posenet_forward
+    P2M_TRY(launch_umma_gemm({y, H, 1}, {P->w2_w, H, 1}, B, 64, H, Epilogue(), w.h64, w.apack, w.wpack, w.status,
+                             gemm.sm_count, s, 3 * J));
+    P2M_TRY(launch_take_cols(w.h64, 64, P->w2_b, 3 * J, B, pose3d, s));
+  } else {
+    Epilogue e2;
+    e2.bias = P->w2_b;
+    P2M_TRY(launch_gemm(y, H, P->w2_w, H, 0, pose3d, 3 * J, B, 3 * J, H, e2, s));
+  }
+  if (pose_combine != nullptr) P2M_TRY(launch_pose_combine(pose2d, pose3d, (long long)B * J, pose_combine, s));
+  return P2M_OK;
+}
+
+int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int B, float p_dropout, const int64_t* seed,
+                         const void* saved, size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
+                         float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  bool ok = pose2d && seed && saved && d_pose3d && workspace && G && G->w1_w && G->w1_b && G->w2_w && G->w2_b && P &&
+            (P->num_stage <= 0 || G->stages);
+  for (int st = 0; ok && st < P->num_stage; ++st) {
+    const p2m_posenet_stage_grads_t& g = G->stages[st];
+    ok = g.w1_w && g.w1_b && g.w2_w && g.w2_b && g.bn1_w && g.bn1_b && g.bn2_w && g.bn2_b;
+  }
+  P2M_TRY(check_call("posenet_backward", P, B, p_dropout, ok, saved_bytes, workspace_bytes));
+  int dev;
+  P2M_TRY(arrays_device("posenet_backward", {pose2d, seed, saved, d_pose3d, d_pose2d, workspace}, &dev));
+  DeviceGuard guard(dev);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const Plan plan(B, P->num_joint, P->hidden, P->num_stage);
+  const Saved sv{static_cast<char*>(const_cast<void*>(saved)), plan};
+  const Work w(workspace, plan);
+  const int H = plan.H, J = plan.J;
+  const long long n = (long long)plan.bh;
+  Gemms gemm{plan, w, 132, s};
+  if (plan.tc) {
+    P2M_CUDA_OK(cudaDeviceGetAttribute(&gemm.sm_count, cudaDevAttrMultiProcessorCount, dev));
+    P2M_CUDA_OK(cudaMemsetAsync(w.status, 0, sizeof(int), s));
+  }
+  // output layer (thin: fp32): db2, dW2 = d_pose3d^T y_S, g = d_pose3d W2
+  P2M_TRY(launch_col_sum(d_pose3d, B, 3 * J, w.sums, G->w2_b, s));
+  P2M_TRY(gemm.transpose(d_pose3d, B, 3 * J));
+  P2M_TRY(launch_gemm(w.gT, B, sv.y(plan.S), H, 1, G->w2_w, H, 3 * J, H, B, Epilogue(), s));
+  P2M_TRY(launch_gemm(d_pose3d, 3 * J, P->w2_w, H, 1, w.g, H, B, H, 3 * J, Epilogue(), s));
+  for (int st = plan.S - 1; st >= 0; --st) {
+    const p2m_posenet_stage_t& S = P->stages[st];
+    const p2m_posenet_stage_grads_t& D = G->stages[st];
+    const Dropout d1 = make_dropout(p_dropout, seed, 2 * st), d2 = make_dropout(p_dropout, seed, 2 * st + 1);
+    // second Linear: y' = y + a2 Wb^T + bb with a2 = drop(relu(bn2(z2))) recomputed; g = dL/dy'
+    P2M_TRY(launch_col_sum(w.g, B, H, w.sums, D.w2_b, s));
+    P2M_TRY(bn_relu_drop(sv.z2(st), plan, sv.stat(st, 1, 2), sv.stat(st, 1, 3), d2, w.a, s));
+    P2M_TRY(gemm.prepare(w.g, false));
+    P2M_TRY(gemm.dw(w.a, D.w2_w));
+    P2M_TRY(gemm.dx(w.g, S.w2_w, w.t));
+    // through drop, ReLU and bn2: t = dL/dz2 (its fp16-range scale found in the same pass on the tensor-core path)
+    k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.t, n, d2);
+    P2M_LAUNCH_OK();
+    P2M_TRY(launch_bn_relu_bwd(sv.z2(st), w.t, B, H, S.bn2_w, sv.stat(st, 1, 2), sv.stat(st, 1, 3), sv.stat(st, 1, 0),
+                               sv.stat(st, 1, 1), 1, w.sums, D.bn2_w, D.bn2_b, w.t, s, plan.tc ? w.g_scale : nullptr));
+    // first Linear: z2 = a1 Wa^T + ba with a1 = drop(relu(bn1(y))) recomputed
+    P2M_TRY(launch_col_sum(w.t, B, H, w.sums, D.w1_b, s));
+    P2M_TRY(bn_relu_drop(sv.y(st), plan, sv.stat(st, 0, 2), sv.stat(st, 0, 3), d1, w.a, s));
+    P2M_TRY(gemm.prepare(w.t, true));
+    P2M_TRY(gemm.dw(w.a, D.w1_w));
+    P2M_TRY(gemm.dx(w.t, S.w1_w, w.a));
+    // through drop, ReLU and bn1, plus the residual branch: g += dL/dy
+    k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.a, n, d1);
+    P2M_LAUNCH_OK();
+    P2M_TRY(launch_bn_relu_bwd(sv.y(st), w.a, B, H, S.bn1_w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), sv.stat(st, 0, 0),
+                               sv.stat(st, 0, 1), 1, w.sums, D.bn1_w, D.bn1_b, w.a, s));
+    k_pn_add<<<blocks(n), 256, 0, s>>>(w.g, w.a, n);
+    P2M_LAUNCH_OK();
+  }
+  // input layer (thin: fp32): db1, dW1 = g^T pose2d, d_pose2d = g W1
+  P2M_TRY(launch_col_sum(w.g, B, H, w.sums, G->w1_b, s));
+  P2M_TRY(gemm.transpose(w.g, B, H));
+  P2M_TRY(launch_gemm(w.gT, B, pose2d, 2 * J, 1, G->w1_w, 2 * J, H, 2 * J, B, Epilogue(), s));
+  if (d_pose2d != nullptr)
+    P2M_TRY(launch_gemm(w.g, H, P->w1_w, 2 * J, 1, d_pose2d, 2 * J, B, 2 * J, H, Epilogue(), s));
+  return P2M_OK;
+}
+
+}  // extern "C"

@@ -1,7 +1,7 @@
 """FlatPose2Mesh: drop-in for the reference's ``models.pose2mesh_net`` (lib/models/pose2mesh_net.py:8-29).
 
     pose3d       = PoseNet(pose2d)                      posenet.LinearModel      (SURVEY.md §8 row f1)
-    pose_combine = cat(pose2d, pose3d.detach() / 1000)  fused into the native PoseNet call in eval mode
+    pose_combine = cat(pose2d, pose3d.detach() / 1000)  fused into the native PoseNet call (eval and training)
     cam_mesh     = MeshNet(pose_combine)                meshnet.Pose2Mesh        (rows a1-a9)
 
 ``forward`` returns ``(cam_mesh, pose3d)`` like the reference; ``predict_vertices_and_joints`` additionally fuses the
@@ -25,8 +25,12 @@ class FlatPose2Mesh(nn.Module):
         self.pose2mesh = meshnet.Pose2Mesh(2 + 3, 3, graph_L)
 
     def _lift(self, pose2d):
-        """(pose3d [B, J, 3], pose_combine [B, J, 5]): natively in eval mode, the reference's torch ops otherwise."""
+        """(pose3d [B, J, 3], pose_combine [B, J, 5]): one native call in eval mode and, for contiguous float32 CUDA
+        tensors, in training mode; the reference's torch ops otherwise."""
         lifter, flat = self.pose_lifter, pose2d.reshape(len(pose2d), -1)
+        if lifter.training and lifter.native_train_ok(flat):
+            pose3d, combine = lifter.forward_train_native(flat, with_combine=True)
+            return pose3d.reshape(-1, self.num_joint, 3), combine
         if not lifter.training and pose2d.is_cuda and not (torch.is_grad_enabled() and pose2d.requires_grad):
             pose3d, combine = lifter.forward_native(flat, with_combine=True)
             return pose3d.reshape(-1, self.num_joint, 3), combine

@@ -5,8 +5,10 @@
 (constructed but unused by the reference's forward), ``linear_stages.<i>.{w1,batch_norm1,w2,batch_norm2}``, ``w2``)
 so PoseNet checkpoints load unchanged.  In eval mode (what FlatPose2Mesh uses for inference, demo/run.py:168) the
 forward runs in libp2m_b200.so (``p2m_posenet_forward``: fp32 GEMMs with the BatchNorm / ReLU / residual fused into
-their epilogues).  In training mode (dropout + batch statistics, lib/core/base.py PoseNet pre-training) the module
-falls through to the same torch ops the reference runs — on the GPU; there is no CPU path.
+their epilogues).  In training mode (dropout + batch statistics: lib/core/base.py:116, and the PoseNet pre-training of
+:246-265) forward and backward run there too (``p2m_posenet_train_forward`` / ``p2m_posenet_backward``) for contiguous
+float32 CUDA tensors; the dropout mask follows the rule stated in include/p2m_b200.h, not torch's generator stream.
+Anything else (CPU tensors, other dtypes, gradients through an eval-mode forward) runs the reference's torch ops.
 """
 from __future__ import annotations
 
@@ -46,6 +48,58 @@ class Linear(nn.Module):
         for bn, lin in ((self.batch_norm1, self.w1), (self.batch_norm2, self.w2)):
             y = lin(self.dropout(self.relu(bn(y))))
         return x + y
+
+
+class _PoseNetTrainFunction(torch.autograd.Function):
+    """LinearModel's train-mode forward / backward through p2m_posenet_train_forward / p2m_posenet_backward.
+    params: w1.weight, w1.bias, w2.weight, w2.bias, then per stage w1.weight, w1.bias, w2.weight, w2.bias,
+    batch_norm1.weight, batch_norm1.bias, batch_norm2.weight, batch_norm2.bias."""
+
+    @staticmethod
+    def forward(ctx, module, x, seed, with_combine, *params):
+        lib = _lib.load()
+        dev, B = x.device, x.shape[0]
+        dims = (B, module.num_joint, module.linear_size, module.num_stage)
+        out = torch.empty((B, module.output_size), device=dev, dtype=torch.float32)
+        comb = torch.empty((B, module.num_joint, 5), device=dev, dtype=torch.float32) if with_combine else None
+        n_saved, n_ws = lib.p2m_posenet_train_saved_bytes(*dims), lib.p2m_posenet_train_workspace_bytes(*dims)
+        saved = torch.empty(n_saved, device=dev, dtype=torch.uint8)
+        ws = torch.empty(n_ws, device=dev, dtype=torch.uint8)
+        native = module._native_params()
+        extra = module._native_train_extra()
+        _lib.call("p2m_posenet_train_forward", dev, C.byref(native), C.byref(extra), x, B, module.p_dropout, seed, out,
+                  comb, saved, n_saved, ws, n_ws)
+        ctx.module, ctx.saved, ctx.dims = module, saved, dims
+        ctx.save_for_backward(x, seed, *params)
+        if comb is None:
+            return out
+        ctx.mark_non_differentiable(comb)                 # the reference detaches pose3d before the concat
+        return out, comb
+
+    @staticmethod
+    def backward(ctx, d_out, *_):
+        if ctx.saved is None:
+            raise RuntimeError("pose2mesh_release_b200: the saved activations of this forward were already released "
+                               "by an earlier backward (retain_graph is not supported: run the forward again)")
+        lib = _lib.load()
+        x, seed, *params = ctx.saved_tensors
+        module, dev = ctx.module, x.device
+        grads = [torch.empty_like(p) for p in params]
+        g = _lib.PoseNetGrads()
+        g.w1_w, g.w1_b, g.w2_w, g.w2_b = (t.data_ptr() for t in grads[:4])
+        stages = (_lib.PoseNetStageGrads * module.num_stage)()
+        for i in range(module.num_stage):
+            for (name, _), t in zip(_lib.PoseNetStageGrads._fields_, grads[4 + 8 * i:12 + 8 * i]):
+                setattr(stages[i], name, t.data_ptr())
+        g.stages = stages
+        dx = torch.empty_like(x) if ctx.needs_input_grad[1] else None
+        n_ws = lib.p2m_posenet_train_workspace_bytes(*ctx.dims)
+        ws = torch.empty(n_ws, device=dev, dtype=torch.uint8)
+        native = module._native_params()
+        _lib.call("p2m_posenet_backward", dev, C.byref(native), x, ctx.dims[0], module.p_dropout, seed, ctx.saved,
+                  ctx.saved.numel(), d_out.contiguous().float(), C.byref(g), dx, ws, n_ws)
+        ctx.saved = None
+        return (None, dx, None, None, *grads)
 
 
 class LinearModel(nn.Module):
@@ -105,13 +159,68 @@ class LinearModel(nn.Module):
         _lib.call("p2m_posenet_forward", dev, C.byref(params), x, out, comb, B, ws, nbytes)
         return (out, comb) if with_combine else out
 
-    def forward(self, x):
-        if not self.training and x.is_cuda and not (torch.is_grad_enabled() and x.requires_grad):
-            return self.forward_native(x)
-        y = self.w1(x)                     # training (dropout, batch statistics): the reference's own op sequence
+    def _native_train_extra(self):
+        stages = (_lib.PoseNetTrainStage * self.num_stage)()
+        keep = []
+        for i, st in enumerate(self.linear_stages):
+            nbt = (st.batch_norm1.num_batches_tracked, st.batch_norm2.num_batches_tracked)
+            stages[i].bn1_nbt, stages[i].bn2_nbt = (None if t is None else t.data_ptr() for t in nbt)
+            keep.append(nbt)
+        e = _lib.PoseNetTrain()
+        e.stages = stages
+        e._keep = (stages, keep)
+        return e
+
+    def _trained_tensors(self):
+        """The 4 + 8 num_stage tensors the backward produces gradients for, in _PoseNetTrainFunction's order."""
+        out = [self.w1.weight, self.w1.bias, self.w2.weight, self.w2.bias]
+        for st in self.linear_stages:
+            out += [st.w1.weight, st.w1.bias, st.w2.weight, st.w2.bias, st.batch_norm1.weight, st.batch_norm1.bias,
+                    st.batch_norm2.weight, st.batch_norm2.bias]
+        return out
+
+    def native_train_ok(self, x: torch.Tensor) -> bool:
+        """Whether the train-mode forward of x runs in libp2m_b200.so: x, the trained tensors and the BatchNorm running
+        statistics are contiguous float32 CUDA tensors on one device."""
+        if not (x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()):
+            return False
+        tensors = self._trained_tensors()
+        for st in self.linear_stages:
+            for bn in (st.batch_norm1, st.batch_norm2):
+                if bn.running_mean is None or bn.running_var is None:
+                    return False
+                tensors += [bn.running_mean, bn.running_var]
+        return all(t.device == x.device and t.dtype == torch.float32 and t.is_contiguous() for t in tensors)
+
+    def forward_train_native(self, x: torch.Tensor, seed: torch.Tensor = None, with_combine: bool = False):
+        """Train-mode forward in libp2m_b200.so, differentiable (the backward runs there too).  x [B, 2J] (or
+        [B, J, 2]) -> pose3d [B, 3J]; with_combine additionally returns the detached pose_combine [B, J, 5].  seed:
+        two int64 on x's device that define the dropout masks (include/p2m_b200.h); drawn from torch's generator when
+        not given, so torch.manual_seed reproduces a run.  Updates the BatchNorm running statistics."""
+        x = x.reshape(len(x), -1)
+        if not self.native_train_ok(x):
+            raise RuntimeError("the native train-mode PoseNet needs contiguous float32 CUDA tensors on one device")
+        if x.shape[1] != self.input_size:
+            raise ValueError(f"PoseNet expects {self.input_size} inputs per pose, got {x.shape[1]}")
+        if x.shape[0] < 2:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
+        if seed is None:
+            seed = torch.empty(2, dtype=torch.int64, device=x.device).random_()
+        return _PoseNetTrainFunction.apply(self, x, seed, with_combine, *self._trained_tensors())
+
+    def _forward_torch(self, x):
+        """The reference's own op sequence (lib/models/posenet.py:77-87)."""
+        y = self.w1(x)
         for stage in self.linear_stages:
             y = stage(y)
         return self.w2(y)
+
+    def forward(self, x):
+        if self.training:
+            return self.forward_train_native(x) if self.native_train_ok(x) else self._forward_torch(x)
+        if x.is_cuda and not (torch.is_grad_enabled() and x.requires_grad):
+            return self.forward_native(x)
+        return self._forward_torch(x)
 
 
 def get_model(num_joint, hid_dim, num_layer, p_dropout, pretrained=False):
