@@ -348,6 +348,7 @@ struct KParams {
                           // T1 rows of the tile and its 1-hop halo and only runs the second sparse product on chip
   const float* a_scale;   // optional device scalar: x is multiplied by it before the fp16 split (power of two,
                           // chosen from max|x|: gradients are far below fp16's range) and divided out afterwards
+  const float* b_scale;   // dense GEMM, optional: the device scalar the B operand was packed with in place of W_SCALE
   long long ldy;          // row stride of y in floats, and first output column
   int y_col0;
   float* y;
@@ -509,12 +510,13 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     fence_barrier_init();
   }
   const float a_scale = p.a_scale ? *p.a_scale : 1.f;
+  const float b_inv = p.b_scale ? 1.f / *p.b_scale : W_INV_SCALE;
   const int ecol0 = (int)blockIdx.y * N;  // first output column of this CTA's column slice
   for (int n = threadIdx.x; n < N; n += NUM_THREADS2) {
     const float sc = (p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f) / a_scale;
     const float sh = p.ep.scale ? p.ep.shift[ecol0 + n] : 0.f;
     const float bi = p.ep.bias ? p.ep.bias[ecol0 + n] : 0.f;
-    ep_mul[n] = W_INV_SCALE * sc;
+    ep_mul[n] = b_inv * sc;
     ep_add[n] = fmaf(bi, p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f, sh);
   }
   if (N == 64 && p.head_z != nullptr)
@@ -1591,15 +1593,17 @@ __global__ void __launch_bounds__(512, 2) k_cheb_t1(const T1Params p) {
 // the exact shared-memory image (128B-swizzled), so a kernel fetches a block with a single cp.async.bulk.  Block
 // b = (t * n_chunk + chunk) * orders + order holds rows n = t * rows + [0, rows) and k = 32 chunk + [0, 32):
 // p[n ld_row + k ld_k + order] * scale, zero for n >= n_real or k >= k_real (never read there); `combined`: the isolated
-// rows' combined weights (p[a] + c p[a + 1] + (2c^2 - 1) p[a + 2]) * scale at a = n ld_row + k ld_k.
+// rows' combined weights (p[a] + c p[a + 1] + (2c^2 - 1) p[a + 2]) * scale at a = n ld_row + k ld_k.  With dscale the
+// scale is scale * *dscale.
 struct PackSrc {
   const float* p;
   long long ld_row, ld_k;
   int rows, n_chunk, orders, n_real;
-  float scale;  // W_SCALE for weights, 1 for activations
+  float scale;  // W_SCALE for weights, 1 for range-normalised activations (dscale)
   int combined;
   float c;
   int k_real = INT_MAX;
+  const float* dscale = nullptr;  // device scalar: a power of two found from the operand's largest magnitude
 };
 __global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, unsigned char* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
@@ -1613,12 +1617,13 @@ __global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, 
   const int k0 = (u / s.orders) * FC + (j & 3) * 8;
   const float* src = s.p + n * s.ld_row + (long long)k0 * s.ld_k + u % s.orders;
   const float c = s.c, c2 = 2.f * c * c - 1.f;
+  const float scale = s.dscale ? s.scale * *s.dscale : s.scale;
   __align__(16) __half h[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     const float* wr = src + e * s.ld_k;
     float w = 0.f;
-    if (n < s.n_real && k0 + e < s.k_real) w = s.combined ? (wr[0] + c * wr[1] + c2 * wr[2]) * s.scale : wr[0] * s.scale;
+    if (n < s.n_real && k0 + e < s.k_real) w = s.combined ? (wr[0] + c * wr[1] + c2 * wr[2]) * scale : wr[0] * scale;
     const __half hi = __float2half_rn(w);
     h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
   }
@@ -1749,6 +1754,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.y = a.y;
   p.t1 = a.t1;
   p.a_scale = a.a_scale;
+  p.b_scale = nullptr;
   p.ldy = a.ldy > 0 ? a.ldy : a.fout;
   p.y_col0 = a.y_col0;
   p.status = status;
@@ -2097,7 +2103,9 @@ bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && g_umma_tma &
 size_t umma_plain_pack_bytes(int N, int K) { return (size_t)(K / FC) * N * 128; }
 
 // ---------------------------------------------------------------- dense GEMM on the conv kernel's plain mode
-size_t umma_gemm_apack_bytes(int M, int K) { return (size_t)((M + TILE_M - 1) / TILE_M) * (K / FC) * A_BLOCK_BYTES; }
+// the X image, then the device scalar of X's range normalisation (128 bytes keep the image's successors aligned)
+static size_t gemm_x_image_bytes(int M, int K) { return (size_t)((M + TILE_M - 1) / TILE_M) * (K / FC) * A_BLOCK_BYTES; }
+size_t umma_gemm_apack_bytes(int M, int K) { return gemm_x_image_bytes(M, K) + 128; }
 size_t umma_gemm_wpack_bytes(int N, int K) { return (size_t)(K / FC) * N * 128; }
 bool umma_gemm_supported(int M, int N, int K) { return M > 0 && K >= FC && K % FC == 0 && N >= 64 && N % 64 == 0; }
 
@@ -2123,11 +2131,14 @@ int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
 // streamed by cp.async.bulk into the conv kernel's A/B ring — no producer warps, one CTA per (128-row tile, output
 // column slice).  The epilogue vectors and an identity residual (ep.res with res_F == N) are indexed by output column.
 // Either operand is read by row and k stride, so a transposed view costs nothing: the backward's dX = g W is
-// X = g, W = {W, 1, ld} and dW = g^T a is X = {g, 1, ld}, W = {a, 1, ld}.  k >= k_real is zero padding.  a_scale: X was
-// multiplied by this device scalar by the caller; the epilogue divides it out.
+// X = g, W = {W, 1, ld} and dW = g^T a is X = {g, 1, ld}, W = {a, 1, ld}.  k >= k_real is zero padding.
+// Operand range: X always enters the fp16 split scaled into [2^9, 2^10) by a power of two (x_scale, a device scalar
+// from launch_absmax_scale; found here over the span X's view covers when not given), so the result does not depend
+// on the scale of the activations or gradients.  W enters times the fixed W_SCALE (weights), or, when it is an
+// activation too (dW's a), times the device scalar w_scale.  The epilogue divides both out.
 int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Epilogue& ep, float* Y, void* apack,
                      void* wpack, int* status, int sm_count, cudaStream_t s, int n_real, int k_real,
-                     const float* a_scale) {
+                     const float* x_scale, const float* w_scale) {
   if (n_real <= 0 || n_real > N) n_real = N;  // W has n_real rows; output columns >= n_real are zero-weight padding
   if (k_real <= 0 || k_real > K) k_real = K;
   if (!umma_gemm_supported(M, N, K) || (ep.res != nullptr && ep.res_F != N)) {
@@ -2136,11 +2147,17 @@ int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Ep
   }
   const int tiles = (M + TILE_M - 1) / TILE_M;
   const int ns = CONV_N;  // one warpgroup's register accumulator: 64 output columns per CTA
+  if (x_scale == nullptr) {
+    float* sc = reinterpret_cast<float*>(static_cast<unsigned char*>(apack) + gemm_x_image_bytes(M, K));
+    P2M_TRY(launch_absmax_scale(X.p, (M - 1) * X.ld_row + (k_real - 1) * X.ld_k + 1, sc, s));
+    x_scale = sc;
+  }
   // A: one 16 KB block per (128-row tile, 32-column chunk), rows >= M zero (what the producers would have built);
   // W: the images of all output-column slices, slice j = rows [j ns, (j + 1) ns) of W, rows >= n_real zero
-  P2M_TRY(launch_pack(PackSrc{X.p, X.ld_row, X.ld_k, TILE_M, K / FC, 1, M, 1.f, 0, 0.f, k_real},
+  P2M_TRY(launch_pack(PackSrc{X.p, X.ld_row, X.ld_k, TILE_M, K / FC, 1, M, 1.f, 0, 0.f, k_real, x_scale},
                       (long long)tiles * (K / FC), apack, s));
-  P2M_TRY(launch_pack(PackSrc{W.p, W.ld_row, W.ld_k, ns, K / FC, 1, n_real, W_SCALE, 0, 0.f, k_real},
+  P2M_TRY(launch_pack(PackSrc{W.p, W.ld_row, W.ld_k, ns, K / FC, 1, n_real, w_scale ? 1.f : W_SCALE, 0, 0.f, k_real,
+                              w_scale},
                       (long long)(N / ns) * (K / FC), wpack, s));
   KParams p;
   std::memset(&p, 0, sizeof(p));
@@ -2150,7 +2167,8 @@ int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Ep
   p.n_tiles = tiles;
   p.wpack = static_cast<const unsigned char*>(wpack);
   p.apack = static_cast<const unsigned char*>(apack);
-  p.a_scale = a_scale;
+  p.a_scale = x_scale;
+  p.b_scale = w_scale;
   p.ep = to_dev(ep);
   p.res_identity = (ep.res != nullptr) ? 1 : 0;
   p.ldy = N;

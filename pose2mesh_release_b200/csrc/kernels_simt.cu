@@ -707,7 +707,8 @@ __global__ void __launch_bounds__(256) k_absmax(const float* __restrict__ x, lon
   for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));  // non-negative floats order as uints
 }
-__global__ void k_scale_from_absmax(unsigned int* io, int headroom_log2) {
+// the scale replaces max|x| in io, or goes to out (io zeroed for the next accumulation)
+__global__ void k_scale_from_absmax(unsigned int* io, float* out, int headroom_log2) {
   const float m = __uint_as_float(*io);
   float s = 1.f;
   if (m > 0.f && isfinite(m)) {
@@ -715,7 +716,12 @@ __global__ void k_scale_from_absmax(unsigned int* io, int headroom_log2) {
     frexpf(m, &e);                            // m = f * 2^e, f in [0.5, 1)
     s = ldexpf(1.f, 10 - e - headroom_log2);  // m * s in [2^(9-h), 2^(10-h))
   }
-  *reinterpret_cast<float*>(io) = s;
+  if (out == nullptr) {
+    *reinterpret_cast<float*>(io) = s;
+  } else {
+    *out = s;
+    *io = 0u;
+  }
 }
 // SMs of the current device: the grid-stride kernels below size their grids by it
 static int current_sm_count(int* sms) {
@@ -731,7 +737,12 @@ int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStrea
   const int grid = (int)std::min<long long>((n + 255) / 256, (long long)sms * 8);
   k_absmax<<<grid, 256, 0, s>>>(x, n, reinterpret_cast<unsigned int*>(scale_out));
   P2M_LAUNCH_OK();
-  k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(scale_out), headroom_log2);
+  k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(scale_out), nullptr, headroom_log2);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+int launch_absmax_finish(unsigned int* amax, float* scale_out, cudaStream_t s, int headroom_log2) {
+  k_scale_from_absmax<<<1, 1, 0, s>>>(amax, scale_out, headroom_log2);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -1133,7 +1144,7 @@ int launch_bn_relu_bwd(const float* z, const float* g_a, int rows, int F, const 
                                                   reinterpret_cast<unsigned int*>(gz_scale_out));
     P2M_LAUNCH_OK();
     if (gz_scale_out) {
-      k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(gz_scale_out), 0);
+      k_scale_from_absmax<<<1, 1, 0, s>>>(reinterpret_cast<unsigned int*>(gz_scale_out), nullptr, 0);
       P2M_LAUNCH_OK();
     }
     return P2M_OK;

@@ -339,6 +339,10 @@ int launch_umma_pack_weights(const float* W, int fin, int fout, bool transposed,
 // scale_out[0] = 2^e with max|x| * 2^e in [2^(9-h), 2^(10-h)), h = headroom_log2  (1 if x is all zero or not
 // finite); scratch-free, two tiny launches
 int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s, int headroom_log2 = 0);
+// its second half, for a kernel that finds max|x| as it writes x: that kernel atomicMax-es the magnitudes into a
+// zeroed amax[0] as uint bits (non-negative floats order as uints); this writes the scale to scale_out[0] and zeroes
+// amax[0] again, so one zeroing serves a sequence of them
+int launch_absmax_finish(unsigned int* amax, float* scale_out, cudaStream_t s, int headroom_log2 = 0);
 // y[i] = x[i] * (invert ? 1 / scale[0] : scale[0]) * mul  (in place allowed; scale a device scalar)
 int launch_scale_by(const float* x, long long n, const float* scale, int invert, float mul, float* y, cudaStream_t s);
 // The epilogue of a conv whose weights were packed as W * w_scale[0] instead of W * w_packed (the fixed 2^6): per column
@@ -359,7 +363,8 @@ int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_u
 int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, float* t1, cudaStream_t s,
                    const TileSet* tiles = nullptr);
 int launch_umma_conv(const UmmaConvArgs& a, int* status_flag, const float* zero_row, int sm_count, cudaStream_t s);
-// Dense GEMM on the tensor cores (wgmma, fp16x3): Y [M, N] = epilogue(X [M, K] W [N, K]^T), K % 32 == 0, N % 64 == 0; apack / wpack are
+// Dense GEMM on the tensor cores (wgmma, fp16x3): Y [M, N] = epilogue(X [M, K] W [N, K]^T), K % 32 == 0, N % 64 == 0, X
+// range-normalised before the fp16 split; apack / wpack are
 // scratch of umma_gemm_apack_bytes(M, K) / umma_gemm_wpack_bytes(N, K); ep vectors and an identity residual
 // (ep.res, res_F == N) are indexed by output column.  An operand's element (row r, k) is p[r ld_row + k ld_k]: a
 // row-major matrix is {p, ld, 1}, its transpose {p, 1, ld}.
@@ -373,7 +378,8 @@ size_t umma_gemm_wpack_bytes(int N, int K);
 int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Epilogue& ep, float* Y, void* apack,
                      void* wpack, int* status, int sm_count, cudaStream_t s, int n_real = 0 /* rows of W if < N */,
                      int k_real = 0 /* k >= k_real is zero padding, if < K */,
-                     const float* a_scale = nullptr /* device scalar X was multiplied by; divided out of Y */);
+                     const float* x_scale = nullptr /* X's range normalisation (launch_absmax_scale); found if null */,
+                     const float* w_scale = nullptr /* W is an activation: its range normalisation, not W_SCALE */);
 // PoseNet's output stage, shared by the eval and the train forward (p2m_api.cu): dst [rows, n_col] = src[:, :n_col] (row
 // stride ld) + bias, and pose_combine [B J, 5] = cat(pose2d [B J, 2], pose3d [B J, 3] / 1000)
 int launch_take_cols(const float* src, int ld, const float* bias, int n_col, long long rows, float* dst, cudaStream_t s);

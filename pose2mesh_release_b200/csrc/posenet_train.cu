@@ -49,21 +49,30 @@ __device__ __forceinline__ void dropout_mul4(const Dropout& d, unsigned long lon
   m[3] = w.w < d.threshold ? d.keep_scale : 0.f;
 }
 
-// a = drop(relu(z * scale + shift)): four consecutive elements (one Philox counter) per thread
+// a = drop(relu(z * scale + shift)): four consecutive elements (one Philox counter) per thread; amax (optional, zero on
+// entry): max(a) as uint bits, for launch_absmax_finish
 __global__ void __launch_bounds__(256) k_pn_bn_relu_drop(const float* __restrict__ z, long long n, int F,
                                                          const float* __restrict__ scale, const float* __restrict__ shift,
-                                                         const Dropout d, float* __restrict__ a) {
+                                                         const Dropout d, float* __restrict__ a,
+                                                         unsigned int* __restrict__ amax) {
   const long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (4 * q >= n) return;
-  float m[4];
-  dropout_mul4(d, (unsigned long long)q, m);
+  float mx = 0.f;
+  if (4 * q < n) {
+    float m[4];
+    dropout_mul4(d, (unsigned long long)q, m);
 #pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const long long i = 4 * q + e;
-    if (i < n) {
-      const int f = (int)(i % F);
-      a[i] = fmaxf(fmaf(z[i], scale[f], shift[f]), 0.f) * m[e];
+    for (int e = 0; e < 4; ++e) {
+      const long long i = 4 * q + e;
+      if (i < n) {
+        const int f = (int)(i % F);
+        a[i] = fmaxf(fmaf(z[i], scale[f], shift[f]), 0.f) * m[e];
+        mx = fmaxf(mx, a[i]);
+      }
     }
+  }
+  if (amax != nullptr) {
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if ((threadIdx.x & 31) == 0 && mx > 0.f) atomicMax(amax, __float_as_uint(mx));
   }
 }
 // g *= the same multipliers (in place): the gradient through drop()
@@ -122,8 +131,8 @@ struct Plan {
   int wide() const { return std::max(H, 3 * J); }
   size_t saved_bytes() const { return (size_t)(2 * S + 1) * align_up(bh * 4) + (size_t)S * 8 * align_up((size_t)H * 4); }
   size_t workspace_bytes() const {
-    size_t n = 4 * align_up(bh * 4) + align_up((size_t)wide() * B * 4) + align_up((size_t)B * 64 * 4) +
-               align_up((size_t)wide() * (2 * 8 + 5 * 4)) + 2 * ALIGN;
+    size_t n = 3 * align_up(bh * 4) + align_up((size_t)wide() * B * 4) + align_up((size_t)B * 64 * 4) +
+               align_up((size_t)wide() * (2 * 8 + 5 * 4)) + 3 * ALIGN;
     if (tc) n += align_up(apack_bytes()) + align_up(wpack_bytes());
     return n;
   }
@@ -140,22 +149,25 @@ struct Saved {
   }
 };
 struct Work {
-  float *g, *a, *t, *gs, *gT, *h64;
+  float *g, *a, *t, *gT, *h64;
   double* sums;  // launch_bn_relu_bwd's scratch: 2 F doubles + 5 F floats
-  float* g_scale;
+  float* g_scale;  // the tensor-core GEMMs' range normalisation of the gradient g and of the activation a
+  float* a_scale;
   int* status;
+  unsigned int* a_max;  // bn_relu_drop's max(a): zeroed with status at the start of a call, and by every use
   void *apack = nullptr, *wpack = nullptr;
   Work(void* ws, const Plan& p) {
     Bump b(ws);
     g = b.take<float>(p.bh);
     a = b.take<float>(p.bh);
     t = b.take<float>(p.bh);
-    gs = b.take<float>(p.bh);
     gT = b.take<float>((size_t)p.wide() * p.B);
     h64 = b.take<float>((size_t)p.B * 64);
     sums = reinterpret_cast<double*>(b.take<char>((size_t)p.wide() * (2 * 8 + 5 * 4)));
     g_scale = b.take<float>(1);
-    status = b.take<int>(1);
+    a_scale = b.take<float>(1);
+    status = b.take<int>(2);
+    a_max = reinterpret_cast<unsigned int*>(status + 1);
     if (p.tc) {
       apack = b.take<unsigned char>(p.apack_bytes());
       wpack = b.take<unsigned char>(p.wpack_bytes());
@@ -200,33 +212,35 @@ struct Gemms {
   const Work& w;
   int sm_count;
   cudaStream_t s;
-  // Y [B, H] = epilogue(X [B, H] W^T)
+  // Y [B, H] = epilogue(X [B, H] W^T), X = the activation a whose range normalisation bn_relu_drop left in w.a_scale
   int forward(const float* X, const float* W, const Epilogue& e, float* Y) const {
     const int H = p.H;
-    if (p.tc) return launch_umma_gemm({X, H, 1}, {W, H, 1}, p.B, H, H, e, Y, w.apack, w.wpack, w.status, sm_count, s);
+    if (p.tc)
+      return launch_umma_gemm({X, H, 1}, {W, H, 1}, p.B, H, H, e, Y, w.apack, w.wpack, w.status, sm_count, s, 0, 0,
+                              w.a_scale);
     return launch_gemm(X, H, W, H, 0, Y, H, p.B, H, H, e, s);
   }
-  // the gradient operand of the two backward GEMMs: scaled into fp16's range once (w.gs, w.g_scale) for the tensor
-  // cores, transposed once (w.gT) for the CUDA-core dW
+  // the gradient operand of the two backward GEMMs: its range normalisation (w.g_scale) for the tensor cores unless
+  // the BN backward found it, transposed once (w.gT) for the CUDA-core dW
   int prepare(const float* g, bool have_scale) const {
     if (!p.tc) return transpose(g, p.B, p.H);
     if (!have_scale) P2M_TRY(launch_absmax_scale(g, (long long)p.bh, w.g_scale, s));
-    return launch_scale_by(g, (long long)p.bh, w.g_scale, 0, 1.f, w.gs, s);
+    return P2M_OK;
   }
   // dX [B, H] = g [B, H] W [H, H]
   int dx(const float* g, const float* W, float* dX) const {
     const int H = p.H;
     if (p.tc)
-      return launch_umma_gemm({w.gs, H, 1}, {W, 1, H}, p.B, H, H, Epilogue(), dX, w.apack, w.wpack, w.status, sm_count, s,
+      return launch_umma_gemm({g, H, 1}, {W, 1, H}, p.B, H, H, Epilogue(), dX, w.apack, w.wpack, w.status, sm_count, s,
                               0, 0, w.g_scale);
     return launch_gemm(g, H, W, H, 1, dX, H, p.B, H, H, Epilogue(), s);
   }
-  // dW [H, H] = g^T [H, B] a [B, H]
-  int dw(const float* a, float* dW) const {
+  // dW [H, H] = g^T [H, B] a [B, H]: both operands range-normalised (a by bn_relu_drop)
+  int dw(const float* g, const float* a, float* dW) const {
     const int H = p.H;
     if (p.tc)
-      return launch_umma_gemm({w.gs, 1, H}, {a, 1, H}, H, H, p.Bp, Epilogue(), dW, w.apack, w.wpack, w.status, sm_count,
-                              s, 0, p.B, w.g_scale);
+      return launch_umma_gemm({g, 1, H}, {a, 1, H}, H, H, p.Bp, Epilogue(), dW, w.apack, w.wpack, w.status, sm_count,
+                              s, 0, p.B, w.g_scale, w.a_scale);
     return launch_gemm(w.gT, p.B, a, H, 1, dW, H, H, H, p.B, Epilogue(), s);
   }
   int transpose(const float* in, int R, int C) const {
@@ -236,11 +250,14 @@ struct Gemms {
   }
 };
 
-int bn_relu_drop(const float* z, const Plan& p, const float* scale, const float* shift, const Dropout& d, float* a,
-                 cudaStream_t s) {
-  k_pn_bn_relu_drop<<<blocks(((long long)p.bh + 3) / 4), 256, 0, s>>>(z, (long long)p.bh, p.H, scale, shift, d, a);
+// a = drop(relu(z * scale + shift)), and on the tensor-core path its range normalisation in w.a_scale
+int bn_relu_drop(const float* z, const Plan& p, const Work& w, const float* scale, const float* shift, const Dropout& d,
+                 float* a, cudaStream_t s) {
+  unsigned int* amax = p.tc ? w.a_max : nullptr;
+  k_pn_bn_relu_drop<<<blocks(((long long)p.bh + 3) / 4), 256, 0, s>>>(z, (long long)p.bh, p.H, scale, shift, d, a,
+                                                                      amax);
   P2M_LAUNCH_OK();
-  return P2M_OK;
+  return amax ? launch_absmax_finish(amax, w.a_scale, s) : P2M_OK;
 }
 
 }  // namespace
@@ -273,7 +290,7 @@ int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_t
   Gemms gemm{plan, w, 132, s};
   if (plan.tc) {
     P2M_CUDA_OK(cudaDeviceGetAttribute(&gemm.sm_count, cudaDevAttrMultiProcessorCount, dev));
-    P2M_CUDA_OK(cudaMemsetAsync(w.status, 0, sizeof(int), s));
+    P2M_CUDA_OK(cudaMemsetAsync(w.status, 0, 2 * sizeof(int), s));  // status and a_max
   }
   Epilogue e1;
   e1.bias = P->w1_b;
@@ -287,7 +304,8 @@ int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_t
     P2M_TRY(launch_bn_finalize(w.sums, y, B, H, S.bn1_w, S.bn1_b, const_cast<float*>(S.bn1_rm),
                                const_cast<float*>(S.bn1_rv), X.bn1_nbt, sv.stat(st, 0, 0), sv.stat(st, 0, 1),
                                sv.stat(st, 0, 2), sv.stat(st, 0, 3), s));
-    P2M_TRY(bn_relu_drop(y, plan, sv.stat(st, 0, 2), sv.stat(st, 0, 3), make_dropout(p_dropout, seed, 2 * st), w.a, s));
+    P2M_TRY(bn_relu_drop(y, plan, w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), make_dropout(p_dropout, seed, 2 * st), w.a,
+                         s));
     // z2 = a Wa^T + ba;  a = drop(relu(bn2(z2)))
     Epilogue ea;
     ea.bias = S.w1_b;
@@ -296,8 +314,8 @@ int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_t
     P2M_TRY(launch_bn_finalize(w.sums, sv.z2(st), B, H, S.bn2_w, S.bn2_b, const_cast<float*>(S.bn2_rm),
                                const_cast<float*>(S.bn2_rv), X.bn2_nbt, sv.stat(st, 1, 0), sv.stat(st, 1, 1),
                                sv.stat(st, 1, 2), sv.stat(st, 1, 3), s));
-    P2M_TRY(bn_relu_drop(sv.z2(st), plan, sv.stat(st, 1, 2), sv.stat(st, 1, 3), make_dropout(p_dropout, seed, 2 * st + 1),
-                         w.a, s));
+    P2M_TRY(bn_relu_drop(sv.z2(st), plan, w, sv.stat(st, 1, 2), sv.stat(st, 1, 3),
+                         make_dropout(p_dropout, seed, 2 * st + 1), w.a, s));
     // y' = y + a Wb^T + bb
     Epilogue eb;
     eb.bias = S.w2_b;
@@ -341,7 +359,7 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
   Gemms gemm{plan, w, 132, s};
   if (plan.tc) {
     P2M_CUDA_OK(cudaDeviceGetAttribute(&gemm.sm_count, cudaDevAttrMultiProcessorCount, dev));
-    P2M_CUDA_OK(cudaMemsetAsync(w.status, 0, sizeof(int), s));
+    P2M_CUDA_OK(cudaMemsetAsync(w.status, 0, 2 * sizeof(int), s));  // status and a_max
   }
   // output layer (thin: fp32): db2, dW2 = d_pose3d^T y_S, g = d_pose3d W2
   P2M_TRY(launch_col_sum(d_pose3d, B, 3 * J, w.sums, G->w2_b, s));
@@ -354,9 +372,9 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
     const Dropout d1 = make_dropout(p_dropout, seed, 2 * st), d2 = make_dropout(p_dropout, seed, 2 * st + 1);
     // second Linear: y' = y + a2 Wb^T + bb with a2 = drop(relu(bn2(z2))) recomputed; g = dL/dy'
     P2M_TRY(launch_col_sum(w.g, B, H, w.sums, D.w2_b, s));
-    P2M_TRY(bn_relu_drop(sv.z2(st), plan, sv.stat(st, 1, 2), sv.stat(st, 1, 3), d2, w.a, s));
+    P2M_TRY(bn_relu_drop(sv.z2(st), plan, w, sv.stat(st, 1, 2), sv.stat(st, 1, 3), d2, w.a, s));
     P2M_TRY(gemm.prepare(w.g, false));
-    P2M_TRY(gemm.dw(w.a, D.w2_w));
+    P2M_TRY(gemm.dw(w.g, w.a, D.w2_w));
     P2M_TRY(gemm.dx(w.g, S.w2_w, w.t));
     // through drop, ReLU and bn2: t = dL/dz2 (its fp16-range scale found in the same pass on the tensor-core path)
     k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.t, n, d2);
@@ -365,9 +383,9 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
                                sv.stat(st, 1, 1), 1, w.sums, D.bn2_w, D.bn2_b, w.t, s, plan.tc ? w.g_scale : nullptr));
     // first Linear: z2 = a1 Wa^T + ba with a1 = drop(relu(bn1(y))) recomputed
     P2M_TRY(launch_col_sum(w.t, B, H, w.sums, D.w1_b, s));
-    P2M_TRY(bn_relu_drop(sv.y(st), plan, sv.stat(st, 0, 2), sv.stat(st, 0, 3), d1, w.a, s));
+    P2M_TRY(bn_relu_drop(sv.y(st), plan, w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), d1, w.a, s));
     P2M_TRY(gemm.prepare(w.t, true));
-    P2M_TRY(gemm.dw(w.a, D.w1_w));
+    P2M_TRY(gemm.dw(w.t, w.a, D.w1_w));
     P2M_TRY(gemm.dx(w.t, S.w1_w, w.a));
     // through drop, ReLU and bn1, plus the residual branch: g += dL/dy
     k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.a, n, d1);

@@ -61,7 +61,7 @@ def dropout_masks(seed, p: float, B: int, H: int, num_stage: int):
 
 
 # --------------------------------------------------------------------------------------------- forward + backward
-def _gemm(a, ea, Wt, eW, prec, h_b=0, over_batch=False):
+def _gemm(a, ea, Wt, eW, prec, over_batch=False):
     """a [m, k] @ Wt [k, n] and its bound when a is within ea and Wt within eW of the exact operands.  over_batch: the
     sum runs over the batch, where the errors of one channel share that channel's statistics (mean, invstd) and are
     not independent: they add linearly."""
@@ -69,7 +69,7 @@ def _gemm(a, ea, Wt, eW, prec, h_b=0, over_batch=False):
     prop = ea @ np.abs(Wt) + np.abs(a) @ eW if over_batch else _rss(ea, Wt) + _rss(a, eW)
     e = R.gamma(a.shape[1], prec) * (np.abs(a) @ np.abs(Wt)) + prop
     if prec == "fp16x3":
-        e = e + R.floor_matmul(a, Wt, 0, h_b)
+        e = e + R.floor_matmul(a, Wt)
     return y, e
 
 
@@ -153,7 +153,7 @@ def forward_backward(sd, x, num_stage: int, masks, d_out, precision: str = "fp16
     out, eout = _gemm(y, e, W2.T, zero(W2.T), last_precision)
     val["out"], bnd["out"] = out + f["w2.bias"], eout + U32 * np.abs(out + f["w2.bias"])
 
-    # backward; the thin layers run in fp32, a dW's activation operand enters the fp16 split times 2^6, not normalised
+    # backward; the thin layers run in fp32, both operands of a tensor-core dW enter the fp16 split range-normalised
     def put(name, v, b):
         val["grad." + name], bnd["grad." + name] = v, b
 
@@ -164,13 +164,13 @@ def forward_backward(sd, x, num_stage: int, masks, d_out, precision: str = "fp16
         p = f"linear_stages.{s}."
         a1, ea1, c1, a2, ea2, c2 = tape[s]
         put(p + "w2.bias", *_col_sum(g, eg))
-        put(p + "w2.weight", *_gemm(g.T, eg.T, a2, ea2, precision, h_b=6, over_batch=True))
+        put(p + "w2.weight", *_gemm(g.T, eg.T, a2, ea2, precision, over_batch=True))
         ga2, ega2 = _gemm(g, eg, f[p + "w2.weight"], zero(f[p + "w2.weight"]), precision)
         gz, egz, dgam, e_dgam, dbet, e_dbet = _bn_bwd(c2, ga2, ega2)
         put(p + "batch_norm2.weight", dgam, e_dgam)
         put(p + "batch_norm2.bias", dbet, e_dbet)
         put(p + "w1.bias", *_col_sum(gz, egz))
-        put(p + "w1.weight", *_gemm(gz.T, egz.T, a1, ea1, precision, h_b=6, over_batch=True))
+        put(p + "w1.weight", *_gemm(gz.T, egz.T, a1, ea1, precision, over_batch=True))
         ga1, ega1 = _gemm(gz, egz, f[p + "w1.weight"], zero(f[p + "w1.weight"]), precision)
         gy, egy, dgam, e_dgam, dbet, e_dbet = _bn_bwd(c1, ga1, ega1)
         put(p + "batch_norm1.weight", dgam, e_dgam)

@@ -56,6 +56,29 @@ def test_bound_rejects_an_unscaled_split_of_small_inputs():
     assert R.bound_ratio(y_unscaled.reshape(y64.shape), y64, bound) > 1.0
 
 
+def test_dense_gemm_bound_needs_range_normalised_activations():
+    """PoseNet's H x H GEMM (K = 1024) on ReLU activations of scale 2^e, held to posenet_forward's per-GEMM bound: the
+    fp16 split of the activations scaled into [2^9, 2^10) by a power of two meets it at every scale; split as they
+    are, their lo parts fall into fp16's subnormals at small scales and the hi parts overflow at large ones."""
+    rng = np.random.default_rng(3)
+    K, n = 1024, 64
+    W = ((rng.random((n, K)) * 2 - 1) / np.sqrt(K)).astype(np.float32).astype(np.float64)
+    wh, wl = R._f16_split(W * 64)
+    act = np.maximum(rng.standard_normal((16, K)), 0.0)
+    ratios = {}
+    for e in range(-20, 17, 4):
+        a = (act * 2.0 ** e).astype(np.float32).astype(np.float64)
+        y64 = a @ W.T
+        bound = R.gamma(K, "fp16x3") * (np.abs(a) @ np.abs(W).T) + R.floor_matmul(a, W.T)
+        for name, s in (("normalised", R._pow2_scale(float(np.abs(a).max()))), ("as is", 1.0)):
+            with np.errstate(over="ignore", invalid="ignore"):
+                ah, al = R._f16_split(a * s)
+                y = (ah @ wh.T + al @ wh.T + ah @ wl.T) / (s * 64)
+            ratios[name, e] = R.bound_ratio(y, y64, bound)
+    assert max(r for (name, _), r in ratios.items() if name == "normalised") <= 0.1, ratios
+    assert all(ratios["as is", e] > 1.0 for e in (-20, -16, -12, 16)), ratios
+
+
 def test_fp64_backward_matches_autograd_for_a_nonsymmetric_matrix():
     L = G.get("nonsymmetric")
     rng = np.random.default_rng(1)

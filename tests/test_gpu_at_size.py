@@ -88,6 +88,12 @@ def _train_step_parity(name, n_distinct, copies, open_relus, precision="fp16x3")
     scale = max(float(v.grad.abs().max()) for v in sd_o.values() if v.requires_grad)
     worst = {}
     for k, p in model.named_parameters():
+        if k.startswith("cl.") and k.endswith(".bias") and model.bn[int(k.split(".")[1])] is not None:
+            # in front of a train-mode BatchNorm the exact gradient is zero, which the library writes; the oracle's
+            # fp32 sum over the batch leaves rounding noise there that grows with the rows (1.1e-3 of the largest
+            # gradient on cl.19 at the SMPL size), so it is no reference
+            assert torch.count_nonzero(p.grad) == 0, k
+            continue
         ok, info = grad_close(p.grad, sd_o[k].grad, scale=1e-3 * scale, strict=open_relus)
         worst[k] = info
         assert ok, (k, info)
@@ -109,9 +115,11 @@ def _train_step_parity(name, n_distinct, copies, open_relus, precision="fp16x3")
     return worst
 
 
-@pytest.mark.parametrize("open_relus", [True, False], ids=["open-relus-strict", "live-relus"])
+@pytest.mark.parametrize("open_relus", [True, False], ids=["open-relus-exact-zero-bn-bias", "live-relus"])
 def test_smpl_size_b256_train_step_against_oracle(open_relus):
-    """BASELINE configs[2]: B=256 fwd+bwd on the SMPL-size hierarchy, 32 distinct poses x 8 (see the module docstring)."""
+    """BASELINE configs[2]: B=256 fwd+bwd on the SMPL-size hierarchy, 32 distinct poses x 8 (see the module docstring).
+    With the ReLUs open every gradient is held to 1e-3 of the largest one, except the biases in front of a BatchNorm:
+    their exact gradient is zero, and the oracle's fp32 sum leaves more noise than that there at this size."""
     _train_step_parity("smpl_like", 32, 8, open_relus)
 
 

@@ -52,23 +52,22 @@ CASES = [  # H, B, J, num_stage, p, scale of the upstream gradient
 ]
 
 
-@pytest.mark.parametrize("H,B,J,S,p,gscale", CASES)
-def test_train_forward_backward_within_float64_bound(H, B, J, S, p, gscale):
-    net = _net(J, H, S, p)
+def check_train_step(net, S, p, x, d_out, seed):
+    """One native forward + backward of a freshly built `net` (_net) against posenet_train_ref with the masks `seed`
+    defines: every result finite and within its element-wise bound, and the relative check below."""
+    H, J = net.linear_size, net.num_joint
     sd = {k: v.detach().cpu().numpy().copy() for k, v in net.state_dict().items()}
-    g = torch.Generator().manual_seed(B + H)
-    x = torch.randn(B, 2 * J, generator=g).to(dev())
-    d_out = (torch.randn(B, 3 * J, generator=g) * gscale).to(dev())
-    seed = torch.tensor([0x5DEECE66D1234567, -987654321], dtype=torch.int64, device=dev())
     out, dx, grads, _ = _run(net, x, seed, d_out)
     tc = H % 64 == 0
-    masks = T.dropout_masks(seed.tolist(), p, B, H, S)
+    masks = T.dropout_masks(seed.tolist(), p, x.shape[0], H, S)
     val, bnd = T.forward_backward(sd, x.cpu().numpy(), S, masks, d_out.cpu().numpy(), "fp16x3" if tc else "fp32",
                                   "fp16x3" if tc and 3 * J <= 64 else "fp32")
     got = {"out": out, "dx": dx, **{"grad." + k: v for k, v in grads.items()}}
     after = net.state_dict()
     got.update({k: after[k] for k in val if "running_" in k})
     assert set(got) == set(val) and len(grads) == 4 + 8 * S
+    bad = [k for k, v in got.items() if not torch.isfinite(v).all()]
+    assert not bad, bad
     ratios = {k: R.bound_ratio(got[k].cpu().numpy(), val[k], bnd[k]) for k in val}
     worst = max(ratios, key=ratios.get)
     assert ratios[worst] <= 1.0, (worst, ratios[worst])
@@ -90,6 +89,17 @@ def test_train_forward_backward_within_float64_bound(H, B, J, S, p, gscale):
     for name, t in after.items():
         if name.endswith("num_batches_tracked"):
             assert int(t) == (0 if name.startswith("batch_norm1.") else 1), name
+    return max(ratios.values())
+
+
+@pytest.mark.parametrize("H,B,J,S,p,gscale", CASES)
+def test_train_forward_backward_within_float64_bound(H, B, J, S, p, gscale):
+    net = _net(J, H, S, p)
+    g = torch.Generator().manual_seed(B + H)
+    x = torch.randn(B, 2 * J, generator=g).to(dev())
+    d_out = (torch.randn(B, 3 * J, generator=g) * gscale).to(dev())
+    seed = torch.tensor([0x5DEECE66D1234567, -987654321], dtype=torch.int64, device=dev())
+    check_train_step(net, S, p, x, d_out, seed)
 
 
 def test_same_seed_is_bitwise_reproducible_and_seeds_differ():
