@@ -486,6 +486,66 @@ int p2m_body_model_backward(const p2m_body_model_t* m, const float* pose, const 
                             float* grad_pose, float* grad_betas, float* grad_trans, int batch, void* workspace,
                             size_t workspace_bytes, p2m_stream_t stream);
 
+/* ---- dataset targets: camera-frame meshes and Human3.6M sample targets (SURVEY.md §8 row f11; the datasets'
+ * get_smpl_coord / get_mano_coord and Human36M.__getitem__) -------------------------------------------------------
+ * One batched call does what each dataset's get_*_coord does for one sample, as a combination of flags:
+ *   ROTATE_ROOT       the root axis-angle becomes log(R exp(root)) (fp64, rounded to float32 as the reference stores
+ *                     it); an exactly zero root counts as the identity (the reference raises there)
+ *   CLAMP_BETAS       a sample with any |beta| > 3 gets zero betas
+ *   ZERO_BETAS_MODEL  a sample whose betas are all zero (after the clamp) uses model_betas: SMPL_Layer's rule applied to
+ *                     each sample on its own, as the datasets' one-sample calls do (set it for SMPL, not for MANO)
+ *   LAYER_TRANS_T / LAYER_TRANS   the layer's trans is t / trans
+ *   H36M_COMPENSATE   + R trans + t / 1000 - J_0 + R J_0 (J_0 the layer's root joint) after the layer
+ *   ADD_T             + t after the layer
+ *   TO_MM             then * 1000
+ * pose [batch, 3 J], betas [batch, S], trans / t [batch, 3], R [batch, 3, 3] row-major (NULL where the flags do not
+ * read them), all device float32 on the model's device.  verts [batch, V, 3]; joints [batch, n_out_joints + n_extra, 3]
+ * where the extra joints are the vertices extra_vertices (HOST int32 [n_extra], n_extra <= 8; MuCo's face keypoints),
+ * transformed like the mesh.  The model runs with P2M_BETAS_AS_GIVEN and no centring.  Five launches (prep, the body
+ * model's three, finish), no host synchronisation (CUDA-graph capturable); a sample's result is bitwise independent of
+ * its batch position and of the batch size.  Workspace >= p2m_camera_frame_workspace_bytes (256-byte aligned). */
+enum {
+  P2M_FRAME_ROTATE_ROOT = 1,
+  P2M_FRAME_CLAMP_BETAS = 2,
+  P2M_FRAME_ZERO_BETAS_MODEL = 4,
+  P2M_FRAME_LAYER_TRANS_T = 8,
+  P2M_FRAME_LAYER_TRANS = 16,
+  P2M_FRAME_H36M_COMPENSATE = 32,
+  P2M_FRAME_ADD_T = 64,
+  P2M_FRAME_TO_MM = 128
+};
+size_t p2m_camera_frame_workspace_bytes(const p2m_body_model_t* m, int batch);
+int p2m_camera_frame_coords(const p2m_body_model_t* m, int flags, const float* pose, const float* betas,
+                            const float* trans, const float* R, const float* t, const int32_t* extra_vertices,
+                            int n_extra, float* verts, float* joints, int batch, void* workspace,
+                            size_t workspace_bytes, p2m_stream_t stream);
+/* Human3.6M's two joint regressors (J_regressor_h36m_correct.npy and J_regressor_coco.npy, HOST float64 [17,
+ * n_vertex] each), kept on `device` as their non-zero entries.  Create rejects non-finite values. */
+typedef struct p2m_h36m_regressors p2m_h36m_regressors_t;
+int p2m_h36m_regressors_create(const double* reg_h36m, const double* reg_coco, int n_vertex, int device,
+                               p2m_h36m_regressors_t** out);
+void p2m_h36m_regressors_destroy(p2m_h36m_regressors_t* h);
+/* The targets and meta of Human36M.__getitem__ (pose2mesh_net; posenet's joint_valid is lift_pose3d_valid) with
+ * augmentation off, from the camera-frame mesh mesh_cam [batch, n_vertex, 3] (mm, the H36M_COMPENSATE | TO_MM
+ * output), the annotation's joint_cam [batch, 17, 3] (mm), focal f and principal point c [batch, 2].  J = 17
+ * (P2M_JOINTS_HUMAN36) or 19 (P2M_JOINTS_COCO: the COCO joints with pelvis and neck).  Outputs, device float32:
+ *   mesh [batch, n_vertex, 3]   (mesh_cam - joint_cam[0]) / 1000 (metres)
+ *   lift_pose3d [batch, J, 3]   COCO: the regressed joints rooted at the pelvis; human36: joint_cam - joint_cam[0]
+ *   reg_pose3d [batch, 17, 3]   joint_cam - joint_cam[0]
+ *   joint_img [batch, J, 2]     cam2pixel of the regressed COCO joints / of joint_cam (pixels)
+ *   fitting_error [batch]       get_fitting_error (mm)
+ *   mesh_valid [batch, n_vertex], lift_pose3d_valid [batch, J], reg_pose3d_valid [batch, 17]: 0 where
+ *   fitting_error > fitting_thr (the lift mask for COCO only), else 1.
+ * Regression, projection and the error in fp64, each output rounded once.  One launch, no host synchronisation. */
+enum {
+  P2M_JOINTS_HUMAN36 = 0,
+  P2M_JOINTS_COCO = 1
+};
+int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float fitting_thr, const float* mesh_cam,
+                     const float* joint_cam, const float* f, const float* c, int batch, float* mesh, float* lift_pose3d,
+                     float* reg_pose3d, float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid,
+                     float* joint_img, float* fitting_error, p2m_stream_t stream);
+
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),
  * entries sorted by (row, col); returns the number of clusters (or -1).  Driven by

@@ -124,6 +124,18 @@ class BodyModelDesc(C.Structure):
 P2M_BETAS_ZERO_MEANS_MODEL = 0
 P2M_BETAS_AS_GIVEN = 1
 
+P2M_FRAME_ROTATE_ROOT = 1
+P2M_FRAME_CLAMP_BETAS = 2
+P2M_FRAME_ZERO_BETAS_MODEL = 4
+P2M_FRAME_LAYER_TRANS_T = 8
+P2M_FRAME_LAYER_TRANS = 16
+P2M_FRAME_H36M_COMPENSATE = 32
+P2M_FRAME_ADD_T = 64
+P2M_FRAME_TO_MM = 128
+
+P2M_JOINTS_HUMAN36 = 0
+P2M_JOINTS_COCO = 1
+
 P2M_CAM_INPUT_F64 = 0
 P2M_CAM_INPUT_INT = 1
 P2M_CAM_INPUT_F32 = 2
@@ -145,6 +157,8 @@ EXPORTS = [
     "p2m_render_workspace_bytes", "p2m_render_meshes",
     "p2m_body_model_create", "p2m_body_model_destroy", "p2m_body_model_workspace_bytes", "p2m_body_model_forward",
     "p2m_body_model_backward_workspace_bytes", "p2m_body_model_backward",
+    "p2m_camera_frame_workspace_bytes", "p2m_camera_frame_coords", "p2m_h36m_regressors_create",
+    "p2m_h36m_regressors_destroy", "p2m_h36m_targets",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
 ]
 
@@ -280,6 +294,19 @@ def load() -> C.CDLL:
         lib.p2m_body_model_backward.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, C.c_int, vp, sz,
                                                 vp]
         lib.p2m_body_model_backward.restype = C.c_int
+        lib.p2m_camera_frame_workspace_bytes.argtypes = [vp, C.c_int]
+        lib.p2m_camera_frame_workspace_bytes.restype = sz
+        lib.p2m_camera_frame_coords.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, c_int32_p, C.c_int, vp, vp, C.c_int,
+                                                vp, sz, vp]
+        lib.p2m_camera_frame_coords.restype = C.c_int
+        lib.p2m_h36m_regressors_create.argtypes = [C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int, C.c_int,
+                                                   C.POINTER(vp)]
+        lib.p2m_h36m_regressors_create.restype = C.c_int
+        lib.p2m_h36m_regressors_destroy.argtypes = [vp]
+        lib.p2m_h36m_regressors_destroy.restype = None
+        lib.p2m_h36m_targets.argtypes = [vp, C.c_int, C.c_float, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
+                                         vp, vp]
+        lib.p2m_h36m_targets.restype = C.c_int
         lib.p2m_graph_match_level.argtypes = [i64, c_int32_p, c_int32_p, C.POINTER(C.c_double), c_int64_p,
                                               C.POINTER(C.c_double), c_int32_p]
         lib.p2m_graph_match_level.restype = i32

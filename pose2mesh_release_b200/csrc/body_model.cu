@@ -746,6 +746,12 @@ struct p2m_body_model {
   ModelDev dev{};
 };
 
+namespace p2m {
+BodyModelInfo body_model_info(const p2m_body_model_t* m) {
+  return BodyModelInfo{m->device, m->V, m->J, m->S, m->n_out, m->dev.mbetas};
+}
+}  // namespace p2m
+
 namespace {
 
 template <typename T>

@@ -106,6 +106,14 @@ inline unsigned grid_for(long long work, int per_cta, long long max_ctas) {
   return (unsigned)(g < 1 ? 1 : (g < max_ctas ? g : max_ctas));
 }
 
+// What other translation units read of a body-model handle (body_model.cu): its device, sizes and the device copy of
+// its model betas [S].
+struct BodyModelInfo {
+  int device, V, J, S, n_out;
+  const float* model_betas;
+};
+BodyModelInfo body_model_info(const p2m_body_model_t* m);
+
 // ---------------------------------------------------------------- device-resident hierarchy level
 // L~ of one level in CSR with RELATIVE column offsets: the neighbour of flat activation row
 // r = b*V + v is row r + reloff[p], so kernels never need (b, v) separately (block-diagonal I_B (x) L~).

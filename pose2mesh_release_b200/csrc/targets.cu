@@ -1,0 +1,457 @@
+// The target side of the datasets' __getitem__ for a whole batch on the GPU (SURVEY.md §8 row f11):
+//  * p2m_camera_frame_coords  every dataset's get_smpl_coord / get_mano_coord (Human36M, AMASS, FreiHAND, MuCo, COCO,
+//                             SURREAL, 3DPW): a few flags on one implementation, five launches:
+//      1. k_frame_prep    one warp per sample: the root axis-angle rotated by the camera R (fp64 Rodrigues, R M, fp64
+//                         log map, rounded to float32 where the reference stores it into its float32 pose), the betas
+//                         clamp (any |beta| > 3 -> zeros) and the per-sample "all-zero betas -> model betas" rule of a
+//                         one-sample SMPL_Layer call, and the translation the layer takes
+//      2-4. the body model's forward (k_batch_flags, k_pose, k_lbs) with P2M_BETAS_AS_GIVEN
+//      5. k_frame_finish  per (sample, 256-vertex chunk): Human36M's translation compensation or AMASS's + t, the
+//                         m -> mm scaling, MuCo's face-keypoint vertices appended to the joints
+//  * p2m_h36m_targets         Human36M.__getitem__'s targets and meta (data/Human36M/dataset.py:344-405, pose2mesh_net and
+//                             posenet, augmentation off) from the camera-frame mesh, one launch (k_h36m_targets, one
+//                             CTA per sample): both sparse joint regressors in one pass (fp64), COCO pelvis / neck,
+//                             cam2pixel, rooting, get_fitting_error and the validity masks.
+// No atomics and fixed orders: a sample's result is bitwise independent of its batch position and of the batch size;
+// nothing is read back to the host, so every call can be captured in a CUDA graph.
+#include <cuda_runtime.h>
+
+#include <cmath>
+#include <string>
+#include <vector>
+
+#include "p2m_internal.h"
+
+namespace p2m {
+namespace {
+
+constexpr int PREP_WARPS = 4;        // samples per k_frame_prep CTA
+constexpr int FIN_T = 256;           // threads (vertices) per k_frame_finish CTA
+constexpr int H36_T = 256;           // threads per k_h36m_targets CTA
+constexpr int MAX_EXTRA = 8;         // appended vertex joints (MuCo: 5 face keypoints)
+constexpr int MAX_BATCH = 1 << 24;
+constexpr int NJ = 17;               // joints of each regressor
+constexpr int NR = 2 * NJ;           // regressor rows: H36M 0..16, COCO 17..33
+constexpr int COCO_J = NJ + 2;       // + pelvis, neck (Human36M.add_pelvis_and_neck)
+constexpr int COCO_LSH = 5, COCO_RSH = 6, COCO_LHIP = 11, COCO_RHIP = 12, COCO_PELVIS = 17;
+
+constexpr int ALL_FLAGS = P2M_FRAME_ROTATE_ROOT | P2M_FRAME_CLAMP_BETAS | P2M_FRAME_ZERO_BETAS_MODEL | P2M_FRAME_LAYER_TRANS_T |
+                          P2M_FRAME_LAYER_TRANS | P2M_FRAME_H36M_COMPENSATE | P2M_FRAME_ADD_T | P2M_FRAME_TO_MM;
+
+struct Extra {
+  int n;
+  int v[MAX_EXTRA];
+};
+
+// The root's rotation in fp64: M = R axangle2mat(r / |r|, |r|) (transforms3d), then its axis-angle vector.  The log map
+// takes theta = atan2(|w|, c) with w the skew part and c = (tr M - 1) / 2: below 2 pi / 3 the axis is w / |w| (well
+// conditioned down to angle 0, where theta / |w| -> 1), above it the axis comes from the symmetric part
+// M + M^T - 2 c I = 2 (1 - c) a a^T (well conditioned up to pi), signed by w.  An exactly zero root is the identity.
+__device__ void rotate_root(const float r[3], const float* Rc, float out[3]) {
+  const double x = r[0], y = r[1], z = r[2];
+  const double ang = sqrt(x * x + y * y + z * z);
+  double A[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  if (ang > 0.0) {
+    const double ax = x / ang, ay = y / ang, az = z / ang;
+    const double c = cos(ang), s = sin(ang), C = 1.0 - c;
+    A[0] = ax * ax * C + c, A[1] = ax * ay * C - az * s, A[2] = ax * az * C + ay * s;
+    A[3] = ax * ay * C + az * s, A[4] = ay * ay * C + c, A[5] = ay * az * C - ax * s;
+    A[6] = ax * az * C - ay * s, A[7] = ay * az * C + ax * s, A[8] = az * az * C + c;
+  }
+  double M[9];
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j)
+      M[3 * i + j] = (double)Rc[3 * i] * A[j] + (double)Rc[3 * i + 1] * A[3 + j] + (double)Rc[3 * i + 2] * A[6 + j];
+  const double w0 = 0.5 * (M[7] - M[5]), w1 = 0.5 * (M[2] - M[6]), w2 = 0.5 * (M[3] - M[1]);
+  const double sn = sqrt(w0 * w0 + w1 * w1 + w2 * w2);
+  const double cs = fmin(1.0, fmax(-1.0, 0.5 * (M[0] + M[4] + M[8] - 1.0)));
+  const double th = atan2(sn, cs);
+  double o0, o1, o2;
+  if (cs > -0.5) {
+    const double k = sn > 0.0 ? th / sn : 1.0;
+    o0 = w0 * k, o1 = w1 * k, o2 = w2 * k;
+  } else {
+    // B = (M + M^T) / 2 - c I = (1 - c) a a^T; the largest diagonal entry gives the best-conditioned axis component
+    const double d0 = M[0] - cs, d1 = M[4] - cs, d2 = M[8] - cs;
+    const double b01 = 0.5 * (M[1] + M[3]), b02 = 0.5 * (M[2] + M[6]), b12 = 0.5 * (M[5] + M[7]);
+    double a0, a1, a2;
+    if (d0 >= d1 && d0 >= d2) {
+      a0 = sqrt(fmax(d0, 0.0)), a1 = b01 / a0, a2 = b02 / a0;
+    } else if (d1 >= d2) {
+      a1 = sqrt(fmax(d1, 0.0)), a0 = b01 / a1, a2 = b12 / a1;
+    } else {
+      a2 = sqrt(fmax(d2, 0.0)), a0 = b02 / a2, a1 = b12 / a2;
+    }
+    const double n = sqrt(a0 * a0 + a1 * a1 + a2 * a2);
+    const double sg = (a0 * w0 + a1 * w1 + a2 * w2) < 0.0 ? -1.0 : 1.0;
+    const double k = sg * th / n;
+    o0 = a0 * k, o1 = a1 * k, o2 = a2 * k;
+  }
+  out[0] = (float)o0, out[1] = (float)o1, out[2] = (float)o2;
+}
+
+// One warp per sample: pose' [B, 3J], betas' [B, S] (resolved per sample), layer trans [B, 3] (when the preset has one).
+__global__ void __launch_bounds__(PREP_WARPS * 32) k_frame_prep(int flags, int batch, int J, int S,
+                                                                const float* __restrict__ mbetas,
+                                                                const float* __restrict__ pose,
+                                                                const float* __restrict__ betas,
+                                                                const float* __restrict__ trans,
+                                                                const float* __restrict__ R, const float* __restrict__ t,
+                                                                float* __restrict__ pose_o, float* __restrict__ betas_o,
+                                                                float* __restrict__ trans_o) {
+  const int lane = threadIdx.x & 31;
+  const long long b = (long long)blockIdx.x * PREP_WARPS + threadIdx.x / 32;
+  if (b >= batch) return;
+  const float* p = pose + b * 3 * J;
+  float* po = pose_o + b * 3 * J;
+  for (int i = lane + ((flags & P2M_FRAME_ROTATE_ROOT) ? 3 : 0); i < 3 * J; i += 32) po[i] = p[i];
+  if ((flags & P2M_FRAME_ROTATE_ROOT) && lane == 0) {
+    const float r[3] = {p[0], p[1], p[2]};
+    float o[3];
+    rotate_root(r, R + b * 9, o);
+    po[0] = o[0], po[1] = o[1], po[2] = o[2];
+  }
+  // smpl_shape[(smpl_shape.abs() > 3).any(dim=1)] = 0, then SMPL_Layer's norm == 0 test on this one sample
+  int big = 0, nonzero = 0;
+  for (int s = lane; s < S; s += 32) {
+    const float x = betas[b * S + s];
+    big |= fabsf(x) > 3.f;
+    nonzero |= !(x == 0.f);
+  }
+  big = __any_sync(0xffffffffu, big) && (flags & P2M_FRAME_CLAMP_BETAS);
+  nonzero = __any_sync(0xffffffffu, nonzero) && !big;
+  if (!(flags & P2M_FRAME_ZERO_BETAS_MODEL)) nonzero = !big;  // ManoLayer uses explicit betas as given
+  for (int s = lane; s < S; s += 32) betas_o[b * S + s] = nonzero ? betas[b * S + s] : mbetas[s];
+  if (lane < 3 && trans_o) {
+    if (flags & P2M_FRAME_LAYER_TRANS_T) trans_o[b * 3 + lane] = t[b * 3 + lane];
+    if (flags & P2M_FRAME_LAYER_TRANS) trans_o[b * 3 + lane] = trans[b * 3 + lane];
+  }
+}
+
+// The steps after the layer, in the reference's float32 order.  grid (vertex chunks, samples); the chunk-0 CTA also
+// writes the sample's joints: the layer's, then the extra vertex joints (MuCo's face keypoints, taken from the layer's
+// mesh and scaled like it).
+__global__ void __launch_bounds__(FIN_T) k_frame_finish(int flags, int V, int n_out, Extra ex,
+                                                        const float* __restrict__ trans, const float* __restrict__ R,
+                                                        const float* __restrict__ t,
+                                                        const float* __restrict__ verts_in,
+                                                        const float* __restrict__ joints_in,
+                                                        float* __restrict__ verts, float* __restrict__ joints) {
+  const long long b = blockIdx.y;
+  const float* jin = joints_in + b * n_out * 3;
+  const float* vin = verts_in + b * V * 3;
+  float off[3] = {0.f, 0.f, 0.f};
+  if (flags & P2M_FRAME_H36M_COMPENSATE) {
+    // smpl_trans = R trans + t / 1000;  smpl_trans = smpl_trans - J_0 + R J_0  (Human36M/dataset.py:288-291)
+    const float* Rb = R + b * 9;
+    const float* tr = trans + b * 3;
+    for (int r = 0; r < 3; ++r) {
+      const float rt = __fadd_rn(__fadd_rn(__fmul_rn(Rb[3 * r], tr[0]), __fmul_rn(Rb[3 * r + 1], tr[1])),
+                                 __fmul_rn(Rb[3 * r + 2], tr[2]));
+      const float rj = __fadd_rn(__fadd_rn(__fmul_rn(Rb[3 * r], jin[0]), __fmul_rn(Rb[3 * r + 1], jin[1])),
+                                 __fmul_rn(Rb[3 * r + 2], jin[2]));
+      off[r] = __fadd_rn(__fsub_rn(__fadd_rn(rt, __fdiv_rn(t[b * 3 + r], 1000.f)), jin[r]), rj);
+    }
+  } else if (flags & P2M_FRAME_ADD_T) {
+    for (int r = 0; r < 3; ++r) off[r] = t[b * 3 + r];
+  }
+  const float scale = (flags & P2M_FRAME_TO_MM) ? 1000.f : 1.f;
+  const int v = blockIdx.x * FIN_T + threadIdx.x;
+  if (v < V)
+    for (int q = 0; q < 3; ++q) verts[(b * V + v) * 3 + q] = __fmul_rn(__fadd_rn(vin[3 * v + q], off[q]), scale);
+  if (blockIdx.x == 0) {
+    const int n_all = n_out + ex.n;
+    for (int e = threadIdx.x; e < 3 * n_all; e += FIN_T) {
+      const int o = e / 3, q = e % 3;
+      const float x = o < n_out ? jin[e] : vin[3 * ex.v[o - n_out] + q];
+      joints[b * n_all * 3 + e] = __fmul_rn(__fadd_rn(x, off[q]), scale);
+    }
+  }
+}
+
+// One CTA per sample (data/Human36M/dataset.py:301-333,344-405 with augmentation off).  Regression in fp64 over the
+// regressors' non-zero entries in ascending vertex order: rows 0..16 (H36M) on the mesh rooted at the annotation's
+// pelvis, rows 17..33 (COCO) on the camera-frame mesh; the mesh output is (mesh - root) / 1000 rounded once.
+struct H36Args {
+  int V, coco, batch;
+  double thr;
+  const int* reg_ptr;      // [NR + 1]
+  const int* reg_idx;      // vertex of each non-zero
+  const double* reg_val;
+  const float* mesh_cam;   // [B, V, 3] mm
+  const float* joint_cam;  // [B, 17, 3] mm
+  const float* f;          // [B, 2]
+  const float* c;          // [B, 2]
+  float* mesh;             // [B, V, 3] m
+  float* lift;             // [B, J, 3]
+  float* reg;              // [B, 17, 3]
+  float* mesh_valid;       // [B, V]
+  float* lift_valid;       // [B, J]
+  float* reg_valid;        // [B, 17]
+  float* joint_img;        // [B, J, 2]
+  float* fit_err;          // [B]
+};
+
+__global__ void __launch_bounds__(H36_T) k_h36m_targets(H36Args a) {
+  __shared__ double sreg[NR][3], sjc[NJ][3], sroot[3];
+  __shared__ float svalid;
+  const long long b = blockIdx.x;
+  const int tid = threadIdx.x, V = a.V;
+  const float* mc = a.mesh_cam + b * V * 3;
+  const float* jc = a.joint_cam + b * NJ * 3;
+  if (tid < 3) sroot[tid] = (double)jc[tid];
+  if (tid < 3 * NJ) sjc[tid / 3][tid % 3] = (double)jc[tid];
+  __syncthreads();
+  if (tid < 3 * NR) {
+    const int r = tid / 3, q = tid % 3;
+    const double sub = r < NJ ? sroot[q] : 0.0;
+    double acc = 0.0;
+    for (int e = a.reg_ptr[r]; e < a.reg_ptr[r + 1]; ++e)
+      acc = fma(a.reg_val[e], (double)mc[3 * a.reg_idx[e] + q] - sub, acc);
+    sreg[r][q] = acc;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    // get_fitting_error: translation-aligned mean joint distance between the annotation and the regressed H36M joints
+    double mj[3] = {0, 0, 0}, ms[3] = {0, 0, 0};
+    for (int j = 0; j < NJ; ++j)
+      for (int q = 0; q < 3; ++q) mj[q] += sjc[j][q] - sroot[q], ms[q] += sreg[j][q];
+    double err = 0.0;
+    for (int j = 0; j < NJ; ++j) {
+      double d2 = 0.0;
+      for (int q = 0; q < 3; ++q) {
+        const double d = (sjc[j][q] - sroot[q]) - (sreg[j][q] - ms[q] / NJ + mj[q] / NJ);
+        d2 += d * d;
+      }
+      err += sqrt(d2);
+    }
+    err /= NJ;
+    svalid = err > a.thr ? 0.f : 1.f;  // a NaN error keeps the sample, as `error > fitting_thr` does
+    a.fit_err[b] = (float)err;
+  }
+  __syncthreads();
+  const float valid = svalid;
+  const int J = a.coco ? COCO_J : NJ;
+  if (tid < 3 * NJ) {
+    const int j = tid / 3, q = tid % 3;
+    a.reg[b * NJ * 3 + tid] = (float)(sjc[j][q] - sroot[q]);
+    if (q == 0) a.reg_valid[b * NJ + j] = 1.f;
+  }
+  if (tid < J) {
+    const int j = tid;
+    double p[3];
+    if (a.coco) {
+      // the regressed COCO joints with pelvis and neck, rooted at the pelvis; projected from the camera frame
+      for (int q = 0; q < 3; ++q) {
+        const double pel = (sreg[NJ + COCO_LHIP][q] + sreg[NJ + COCO_RHIP][q]) * 0.5;
+        const double neck = (sreg[NJ + COCO_LSH][q] + sreg[NJ + COCO_RSH][q]) * 0.5;
+        p[q] = j < NJ ? sreg[NJ + j][q] : (j == COCO_PELVIS ? pel : neck);
+        a.lift[(b * J + j) * 3 + q] = (float)(p[q] - pel);
+      }
+    } else {
+      for (int q = 0; q < 3; ++q) {
+        p[q] = sjc[j][q];
+        a.lift[(b * J + j) * 3 + q] = (float)(sjc[j][q] - sroot[q]);
+      }
+    }
+    // cam2pixel (lib/coord_utils.py:104-109)
+    a.joint_img[(b * J + j) * 2] = (float)(p[0] / p[2] * (double)a.f[b * 2] + (double)a.c[b * 2]);
+    a.joint_img[(b * J + j) * 2 + 1] = (float)(p[1] / p[2] * (double)a.f[b * 2 + 1] + (double)a.c[b * 2 + 1]);
+    a.lift_valid[b * J + j] = a.coco ? valid : 1.f;
+  }
+  for (int e = tid; e < 3 * V; e += H36_T) {
+    a.mesh[b * V * 3 + e] = (float)(((double)mc[e] - sroot[e % 3]) / 1000.0);
+    if (e < V) a.mesh_valid[b * V + e] = valid;
+  }
+}
+
+
+struct FrameLayout {
+  size_t pose, betas, trans, verts, joints, body, total;
+};
+FrameLayout frame_layout(const BodyModelInfo& m, int batch, size_t body_bytes) {
+  FrameLayout l;
+  l.pose = 0;
+  l.betas = l.pose + align_up(sizeof(float) * (size_t)batch * 3 * m.J);
+  l.trans = l.betas + align_up(sizeof(float) * (size_t)batch * m.S);
+  l.verts = l.trans + align_up(sizeof(float) * (size_t)batch * 3);
+  l.joints = l.verts + align_up(sizeof(float) * (size_t)batch * m.V * 3);
+  l.body = l.joints + align_up(sizeof(float) * (size_t)batch * m.n_out * 3);
+  l.total = l.body + body_bytes;
+  return l;
+}
+
+}  // namespace
+}  // namespace p2m
+
+using namespace p2m;
+
+struct p2m_h36m_regressors {
+  int device = 0, V = 0;
+  int* ptr = nullptr;
+  int* idx = nullptr;
+  double* val = nullptr;
+};
+
+extern "C" {
+
+size_t p2m_camera_frame_workspace_bytes(const p2m_body_model_t* m, int batch) {
+  if (!m || batch <= 0 || batch > MAX_BATCH) return 0;
+  return frame_layout(body_model_info(m), batch, p2m_body_model_workspace_bytes(m, batch)).total;
+}
+
+int p2m_camera_frame_coords(const p2m_body_model_t* m, int flags, const float* pose, const float* betas,
+                            const float* trans, const float* R, const float* t, const int32_t* extra_vertices,
+                            int n_extra, float* verts, float* joints, int batch, void* workspace,
+                            size_t workspace_bytes, p2m_stream_t stream) {
+  if (!m || (flags & ~ALL_FLAGS) || batch <= 0 || batch > MAX_BATCH || !pose || !betas || !verts || !joints) {
+    set_error("camera_frame_coords: bad argument (null model / pose / betas / output, unknown flags or batch out of "
+              "[1, 2^24])");
+    return P2M_ERR_INVALID;
+  }
+  const bool need_R = flags & (P2M_FRAME_ROTATE_ROOT | P2M_FRAME_H36M_COMPENSATE);
+  const bool need_t = flags & (P2M_FRAME_LAYER_TRANS_T | P2M_FRAME_H36M_COMPENSATE | P2M_FRAME_ADD_T);
+  const bool need_trans = flags & (P2M_FRAME_LAYER_TRANS | P2M_FRAME_H36M_COMPENSATE);
+  const bool layer_trans = flags & (P2M_FRAME_LAYER_TRANS | P2M_FRAME_LAYER_TRANS_T);
+  if ((need_R && !R) || (need_t && !t) || (need_trans && !trans) ||
+      ((flags & P2M_FRAME_LAYER_TRANS) && (flags & P2M_FRAME_LAYER_TRANS_T)) ||
+      ((flags & P2M_FRAME_ADD_T) && (flags & P2M_FRAME_H36M_COMPENSATE))) {
+    set_error("camera_frame_coords: the flags need R / t / trans that are missing, or combine two translations");
+    return P2M_ERR_INVALID;
+  }
+  const BodyModelInfo info = body_model_info(m);
+  if (n_extra < 0 || n_extra > MAX_EXTRA || (n_extra > 0 && !extra_vertices)) {
+    set_error("camera_frame_coords: n_extra must be in [0, 8] with extra_vertices given");
+    return P2M_ERR_INVALID;
+  }
+  Extra ex{n_extra, {}};
+  for (int i = 0; i < n_extra; ++i) {
+    if (extra_vertices[i] < 0 || extra_vertices[i] >= info.V) {
+      set_error("camera_frame_coords: extra vertex " + std::to_string(extra_vertices[i]) + " is not in [0, " +
+                std::to_string(info.V) + ")");
+      return P2M_ERR_INVALID;
+    }
+    ex.v[i] = extra_vertices[i];
+  }
+  const size_t body_bytes = p2m_body_model_workspace_bytes(m, batch);
+  const FrameLayout l = frame_layout(info, batch, body_bytes);
+  if (!workspace || workspace_bytes < l.total) {
+    set_error("camera_frame_coords: workspace needs " + std::to_string(l.total) + " bytes");
+    return P2M_ERR_WORKSPACE;
+  }
+  int dev = -1;
+  P2M_TRY(arrays_device("camera_frame_coords", {pose, betas, trans, R, t, verts, joints, workspace}, &dev));
+  if (dev != info.device) {
+    set_error("camera_frame_coords: the data arrays are on device " + std::to_string(dev) + ", the body model on " +
+              std::to_string(info.device));
+    return P2M_ERR_INVALID;
+  }
+  DeviceGuard guard(dev);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  char* ws = static_cast<char*>(workspace);
+  float* pose_o = reinterpret_cast<float*>(ws + l.pose);
+  float* betas_o = reinterpret_cast<float*>(ws + l.betas);
+  float* trans_o = layer_trans ? reinterpret_cast<float*>(ws + l.trans) : nullptr;
+  float* verts_l = reinterpret_cast<float*>(ws + l.verts);
+  float* joints_l = reinterpret_cast<float*>(ws + l.joints);
+  k_frame_prep<<<(unsigned)((batch + PREP_WARPS - 1) / PREP_WARPS), PREP_WARPS * 32, 0, s>>>(
+      flags, batch, info.J, info.S, info.model_betas, pose, betas, trans, R, t, pose_o, betas_o, trans_o);
+  P2M_LAUNCH_OK();
+  P2M_TRY(p2m_body_model_forward(m, pose_o, betas_o, P2M_BETAS_AS_GIVEN, trans_o, -1, verts_l, joints_l, batch,
+                                 ws + l.body, body_bytes, stream));
+  const dim3 grid((unsigned)((info.V + FIN_T - 1) / FIN_T), (unsigned)batch);
+  k_frame_finish<<<grid, FIN_T, 0, s>>>(flags, info.V, info.n_out, ex, trans, R, t, verts_l, joints_l, verts, joints);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+int p2m_h36m_regressors_create(const double* reg_h36m, const double* reg_coco, int n_vertex, int device,
+                               p2m_h36m_regressors_t** out) {
+  if (!out) {
+    set_error("h36m_regressors_create: null output pointer");
+    return P2M_ERR_INVALID;
+  }
+  *out = nullptr;
+  if (!reg_h36m || !reg_coco || n_vertex < 1 || n_vertex > (1 << 22)) {
+    set_error("h36m_regressors_create: null regressor or n_vertex out of [1, 2^22]");
+    return P2M_ERR_INVALID;
+  }
+  std::vector<int> ptr(1, 0), idx;
+  std::vector<double> val;
+  for (int r = 0; r < NR; ++r) {
+    const double* row = (r < NJ ? reg_h36m : reg_coco) + (size_t)(r % NJ) * n_vertex;
+    for (int v = 0; v < n_vertex; ++v) {
+      if (!std::isfinite(row[v])) {
+        set_error("h36m_regressors_create: a regressor holds a non-finite value");
+        return P2M_ERR_INVALID;
+      }
+      if (row[v] != 0.0) idx.push_back(v), val.push_back(row[v]);
+    }
+    ptr.push_back((int)idx.size());
+  }
+  int n_dev = 0;
+  if (cudaGetDeviceCount(&n_dev) != cudaSuccess || device < 0 || device >= n_dev) {
+    cudaGetLastError();
+    set_error("h36m_regressors_create: device " + std::to_string(device) + " is not available");
+    return P2M_ERR_NOGPU;
+  }
+  if (idx.empty()) idx.push_back(0), val.push_back(0.0);  // keep the pointers valid for all-zero regressors
+  DeviceGuard guard(device);
+  auto* h = new p2m_h36m_regressors();
+  h->device = device, h->V = n_vertex;
+  const auto fail = [&](cudaError_t e) {
+    set_error(std::string("h36m_regressors_create: ") + cudaGetErrorString(e));
+    p2m_h36m_regressors_destroy(h);
+    return P2M_ERR_CUDA;
+  };
+  cudaError_t e;
+  if ((e = cudaMalloc(&h->ptr, sizeof(int) * ptr.size())) != cudaSuccess) return fail(e);
+  if ((e = cudaMalloc(&h->idx, sizeof(int) * idx.size())) != cudaSuccess) return fail(e);
+  if ((e = cudaMalloc(&h->val, sizeof(double) * val.size())) != cudaSuccess) return fail(e);
+  if ((e = cudaMemcpy(h->ptr, ptr.data(), sizeof(int) * ptr.size(), cudaMemcpyHostToDevice)) != cudaSuccess ||
+      (e = cudaMemcpy(h->idx, idx.data(), sizeof(int) * idx.size(), cudaMemcpyHostToDevice)) != cudaSuccess ||
+      (e = cudaMemcpy(h->val, val.data(), sizeof(double) * val.size(), cudaMemcpyHostToDevice)) != cudaSuccess)
+    return fail(e);
+  *out = h;
+  return P2M_OK;
+}
+
+void p2m_h36m_regressors_destroy(p2m_h36m_regressors_t* h) {
+  if (!h) return;
+  {
+    DeviceGuard guard(h->device);
+    cudaFree(h->ptr);
+    cudaFree(h->idx);
+    cudaFree(h->val);
+  }
+  delete h;
+}
+
+int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float fitting_thr, const float* mesh_cam,
+                     const float* joint_cam, const float* f, const float* c, int batch, float* mesh, float* lift_pose3d,
+                     float* reg_pose3d, float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid,
+                     float* joint_img, float* fitting_error, p2m_stream_t stream) {
+  if (!h || (input_joint_set != P2M_JOINTS_HUMAN36 && input_joint_set != P2M_JOINTS_COCO) || batch <= 0 ||
+      batch > MAX_BATCH || !mesh_cam || !joint_cam || !f || !c || !mesh || !lift_pose3d || !reg_pose3d ||
+      !mesh_valid || !lift_pose3d_valid || !reg_pose3d_valid || !joint_img || !fitting_error) {
+    set_error("h36m_targets: bad argument (null handle / array, unknown joint set or batch out of [1, 2^24])");
+    return P2M_ERR_INVALID;
+  }
+  int dev = -1;
+  P2M_TRY(arrays_device("h36m_targets", {mesh_cam, joint_cam, f, c, mesh, lift_pose3d, reg_pose3d, mesh_valid,
+                                         lift_pose3d_valid, reg_pose3d_valid, joint_img, fitting_error}, &dev));
+  if (dev != h->device) {
+    set_error("h36m_targets: the data arrays are on device " + std::to_string(dev) + ", the regressors on " +
+              std::to_string(h->device));
+    return P2M_ERR_INVALID;
+  }
+  DeviceGuard guard(dev);
+  H36Args a{h->V, input_joint_set == P2M_JOINTS_COCO, batch, (double)fitting_thr, h->ptr, h->idx, h->val,
+            mesh_cam, joint_cam, f, c, mesh, lift_pose3d, reg_pose3d, mesh_valid, lift_pose3d_valid, reg_pose3d_valid,
+            joint_img, fitting_error};
+  k_h36m_targets<<<(unsigned)batch, H36_T, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+}  // extern "C"

@@ -1,0 +1,201 @@
+"""The datasets' training targets for a whole batch on the GPU (SURVEY.md §8 row f11):
+
+    camera_frame_coords(layer, dataset, ...)   each dataset's get_smpl_coord / get_mano_coord:
+                                               data/{Human36M,AMASS,FreiHAND,MuCo,COCO,SURREAL,PW3D}/dataset.py
+    Human36MTargets                            the targets and meta of Human36M.__getitem__ (data/Human36M/dataset.py:
+                                               301-333,344-418) for pose2mesh_net and posenet, augmentation off
+
+Both run in libp2m_b200.so (p2m_camera_frame_coords, p2m_h36m_targets): a prep kernel, the body model's three
+launches and a finish kernel per camera-frame call, one more launch for the Human3.6M assembly.  CUDA tensors only;
+nothing is read back to the host, so a call can be captured in a CUDA graph.
+
+The datasets call the body model once per sample, so its quirks apply per sample here: the betas clamp (any
+|beta| > 3 -> zeros) and SMPL_Layer's "all-zero betas -> the model's betas" rule are decided for each sample on its
+own, and a sample's result does not depend on the rest of the batch.  The reference keeps one layer per gender; a call
+takes one layer, so callers group samples by gender.  Deliberate differences from the reference:
+
+  * the root rotation log(R exp(root)) is taken in fp64 with a log map that is accurate near angle 0 and near pi and
+    rounded to float32 where the reference stores it; below pi the axis-angle vector is unique and matches
+    transforms3d's to rounding, at pi only the rotation is defined;
+  * an exactly zero root is the identity rotation (the reference divides 0 / 0 and raises in mat2axangle);
+  * the layer must have center_idx None, as every layer the datasets build does.
+
+The 2-D joints come out in image pixels, before the crop and normalisation: feed them to
+postprocess.normalize_pose2d (the use_gt_input path) or add detector noise first.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from dataclasses import dataclass
+
+import numpy as np
+import torch
+
+from . import _lib
+from .body_model import ManoLayer, SMPLLayer
+
+FACE_KPS_VERTEX = (331, 2802, 6262, 3489, 3990)  # lib/smpl.py:22, appended to MuCo's joints
+FITTING_THR = 25.0                               # data/Human36M/dataset.py:37, millimetres
+JOINT_SETS = {"human36": _lib.P2M_JOINTS_HUMAN36, "coco": _lib.P2M_JOINTS_COCO}
+
+
+@dataclass(frozen=True)
+class _Preset:
+    flags: int
+    mano: bool = False      # FreiHAND's MANO layer; every other preset takes an SMPL layer
+    trans: bool = False     # reads trans
+    camera: bool = False    # reads R and t
+    extra: tuple = ()       # vertex joints appended to the layer's joints
+
+
+PRESETS = {
+    # Human36M/dataset.py:253-299: rotated root, clamped betas, + R trans + t / 1000 - J_0 + R J_0, mm
+    "human36m": _Preset(_lib.P2M_FRAME_ROTATE_ROOT | _lib.P2M_FRAME_CLAMP_BETAS | _lib.P2M_FRAME_H36M_COMPENSATE |
+                        _lib.P2M_FRAME_TO_MM, trans=True, camera=True),
+    # AMASS/dataset.py:182-213: rotated root, + t, mm
+    "amass": _Preset(_lib.P2M_FRAME_ROTATE_ROOT | _lib.P2M_FRAME_ADD_T | _lib.P2M_FRAME_TO_MM, camera=True),
+    # FreiHAND/dataset.py:110-134: rotated root, t into the MANO layer, the layer's mm
+    "freihand": _Preset(_lib.P2M_FRAME_ROTATE_ROOT | _lib.P2M_FRAME_LAYER_TRANS_T, mano=True, camera=True),
+    # MuCo/dataset.py:196-216: clamped betas, trans into the layer, the 5 face-keypoint vertices appended, mm
+    "muco": _Preset(_lib.P2M_FRAME_CLAMP_BETAS | _lib.P2M_FRAME_LAYER_TRANS | _lib.P2M_FRAME_TO_MM, trans=True,
+                    extra=FACE_KPS_VERTEX),
+    # COCO/dataset.py:147-166: clamped betas, mm
+    "coco": _Preset(_lib.P2M_FRAME_CLAMP_BETAS | _lib.P2M_FRAME_TO_MM),
+    # SURREAL/dataset.py:62-80, PW3D/dataset.py:84-102: trans into the layer, mm
+    "surreal": _Preset(_lib.P2M_FRAME_LAYER_TRANS | _lib.P2M_FRAME_TO_MM, trans=True),
+    "pw3d": _Preset(_lib.P2M_FRAME_LAYER_TRANS | _lib.P2M_FRAME_TO_MM, trans=True),
+}
+
+
+def _cuda(x, what: str, shape, device=None) -> torch.Tensor:
+    _lib.cuda_tensor(x, what)
+    if x.requires_grad:
+        raise ValueError(f"{what} requires grad; the targets are not differentiable")
+    if tuple(x.shape) != tuple(shape):
+        raise ValueError(f"{what} must be {list(shape)}; got {tuple(x.shape)}")
+    if device is not None and x.device != device:
+        raise ValueError(f"{what} is on {x.device}, expected {device}")
+    return x.contiguous().float()
+
+
+def camera_frame_coords(layer, dataset: str, pose, betas, trans=None, R=None, t=None):
+    """The dataset's get_smpl_coord / get_mano_coord for a batch: -> (mesh [B, V, 3], joints [B, J', 3]) float32.
+
+    layer    an SMPLLayer (every preset but 'freihand') or a ManoLayer ('freihand'), with center_idx None.
+    dataset  one of PRESETS: 'human36m', 'amass', 'freihand', 'muco', 'coco', 'surreal', 'pw3d'.
+    pose [B, 3 J], betas [B, 10]; trans [B, 3] for 'human36m', 'muco', 'surreal', 'pw3d'; the camera R [B, 3, 3] and
+    t [B, 3] for 'human36m', 'amass', 'freihand' (inputs a preset does not read are ignored).
+    Units: millimetres (MANO's own millimetres for 'freihand').  J' = the layer's joints, + 5 face keypoints for
+    'muco'."""
+    if dataset not in PRESETS:
+        raise ValueError(f"dataset must be one of {sorted(PRESETS)}; got {dataset!r}")
+    p = PRESETS[dataset]
+    want = ManoLayer if p.mano else SMPLLayer
+    if not isinstance(layer, want):
+        raise ValueError(f"the {dataset!r} preset takes a {want.__name__}; got {type(layer).__name__}")
+    if layer.center_idx is not None:
+        raise ValueError("camera_frame_coords needs a layer with center_idx None, as the datasets build them")
+    _lib.cuda_tensor(pose, "pose")
+    B, dev = pose.shape[0] if pose.dim() == 2 else -1, pose.device
+    if B < 1:
+        raise ValueError(f"pose must be [B, {3 * layer.num_joints}] with B > 0; got {tuple(pose.shape)}")
+    pose = _cuda(pose, "pose", (B, 3 * layer.num_joints), dev)
+    betas = _cuda(betas, "betas", (B, layer.n_betas), dev)
+    if p.trans and trans is None:
+        raise ValueError(f"the {dataset!r} preset needs trans [B, 3]")
+    trans = _cuda(trans, "trans", (B, 3), dev) if p.trans else None
+    if p.camera:
+        if R is None or t is None:
+            raise ValueError(f"the {dataset!r} preset needs the camera R [B, 3, 3] and t [B, 3]")
+        R, t = _cuda(R, "R", (B, 3, 3), dev), _cuda(t, "t", (B, 3), dev)
+    else:
+        R = t = None
+    flags = p.flags | (0 if p.mano else _lib.P2M_FRAME_ZERO_BETAS_MODEL)
+    lib = _lib.load()
+    h = layer.handle(dev.index)
+    mesh = torch.empty((B, layer.n_vertex, 3), device=dev, dtype=torch.float32)
+    joints = torch.empty((B, layer.n_out_joints + len(p.extra), 3), device=dev, dtype=torch.float32)
+    nbytes = lib.p2m_camera_frame_workspace_bytes(h, B)
+    ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    extra = (C.c_int32 * max(len(p.extra), 1))(*p.extra)
+    _lib.call("p2m_camera_frame_coords", dev, h, flags, pose, betas, trans, R, t, extra, len(p.extra), mesh, joints,
+              B, ws, nbytes)
+    return mesh, joints
+
+
+class Human36MTargets:
+    """The target side of Human36M.__getitem__ (pose2mesh_net and posenet, augmentation off) for a batch.
+
+    Built once from the SMPL layer, the H36M regressor (J_regressor_h36m_correct.npy) and the COCO regressor
+    (J_regressor_coco.npy), both [17, V], the input joint set ('human36' or 'coco') and fitting_thr (mm).  A call
+    takes the per-sample SMPL parameters pose [B, 72], betas [B, 10], trans [B, 3], the camera R [B, 3, 3], t [B, 3],
+    focal f [B, 2], principal point c [B, 2] and the annotation's absolute joint_cam [B, 17, 3] (mm), and returns a
+    dict of float32 device tensors shaped as the dataloader collates them (J = 17 for human36, 19 for coco):
+
+        mesh [B, V, 3]                  metres, rooted at joint_cam[:, 0]
+        lift_pose3d [B, J, 3]           coco: the regressed joints + pelvis, neck, rooted at the pelvis;
+                                        human36: joint_cam rooted at joint 0 (mm)
+        reg_pose3d [B, 17, 3]           joint_cam rooted at joint 0 (mm)
+        mesh_valid [B, V, 1], lift_pose3d_valid [B, J, 1], reg_pose3d_valid [B, 17, 1]
+                                        0 where fitting_error > fitting_thr (the lift mask for coco only)
+        joint_valid [B, J, 1]           posenet's mask: lift_pose3d_valid
+        joint_img [B, J, 2]             image pixels: cam2pixel of the regressed coco joints, or of joint_cam
+        fitting_error [B]               get_fitting_error (mm)
+
+    Six launches per call: camera_frame_coords('human36m') and one assembly kernel."""
+
+    LAUNCHES = 6
+
+    def __init__(self, layer: SMPLLayer, joint_regressor_h36m, joint_regressor_coco, input_joint_set: str = "human36",
+                 fitting_thr: float = FITTING_THR):
+        if not isinstance(layer, SMPLLayer):
+            raise ValueError(f"Human36MTargets takes an SMPLLayer; got {type(layer).__name__}")
+        if input_joint_set not in JOINT_SETS:
+            raise ValueError(f"input_joint_set must be one of {sorted(JOINT_SETS)}; got {input_joint_set!r}")
+        V = layer.n_vertex
+        host = lambda a: np.ascontiguousarray(  # noqa: E731
+            (a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)), dtype=np.float64)
+        self.reg_h36m, self.reg_coco = host(joint_regressor_h36m), host(joint_regressor_coco)
+        for name, r in (("joint_regressor_h36m", self.reg_h36m), ("joint_regressor_coco", self.reg_coco)):
+            if r.shape != (17, V):
+                raise ValueError(f"{name} must be [17, {V}]; got {tuple(r.shape)}")
+        self.layer, self.input_joint_set, self.fitting_thr = layer, input_joint_set, float(fitting_thr)
+        self.num_joints = 19 if input_joint_set == "coco" else 17
+        self._handles = {}
+
+    def handle(self, device_index: int) -> int:
+        h = self._handles.get(device_index)
+        if h is None:
+            dp = C.POINTER(C.c_double)
+            out = C.c_void_p()
+            _lib.check(_lib.load().p2m_h36m_regressors_create(self.reg_h36m.ctypes.data_as(dp),
+                                                              self.reg_coco.ctypes.data_as(dp), self.reg_h36m.shape[1],
+                                                              device_index, C.byref(out)),
+                       "p2m_h36m_regressors_create")
+            h = self._handles[device_index] = out.value
+        return h
+
+    def __del__(self):
+        try:
+            lib = _lib.load()
+            for h in self._handles.values():
+                lib.p2m_h36m_regressors_destroy(h)
+            self._handles = {}
+        except Exception:
+            pass
+
+    def __call__(self, pose, betas, trans, R, t, f, c, joint_cam) -> dict:
+        mesh_cam, _ = camera_frame_coords(self.layer, "human36m", pose, betas, trans, R, t)
+        B, dev, V, J = mesh_cam.shape[0], mesh_cam.device, self.layer.n_vertex, self.num_joints
+        f, c = _cuda(f, "f", (B, 2), dev), _cuda(c, "c", (B, 2), dev)
+        joint_cam = _cuda(joint_cam, "joint_cam", (B, 17, 3), dev)
+        e = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)  # noqa: E731
+        out = {"mesh": e(B, V, 3), "lift_pose3d": e(B, J, 3), "reg_pose3d": e(B, 17, 3), "mesh_valid": e(B, V, 1),
+               "lift_pose3d_valid": e(B, J, 1), "reg_pose3d_valid": e(B, 17, 1), "joint_img": e(B, J, 2),
+               "fitting_error": e(B)}
+        _lib.call("p2m_h36m_targets", dev, self.handle(dev.index), JOINT_SETS[self.input_joint_set],
+                  C.c_float(self.fitting_thr), mesh_cam, joint_cam, f, c, B, out["mesh"], out["lift_pose3d"],
+                  out["reg_pose3d"], out["mesh_valid"], out["lift_pose3d_valid"], out["reg_pose3d_valid"],
+                  out["joint_img"], out["fitting_error"])
+        out["joint_valid"] = out["lift_pose3d_valid"]
+        return out
