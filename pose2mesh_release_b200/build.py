@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libp2m_b200.so")
 SOURCES = ["p2m_api.cu", "kernels_simt.cu", "cheb_umma.cu", "metrics.cu", "body_model.cu", "camera.cu", "temporal.cu",
-           "fscore.cu", "render.cu", "posenet_train.cu", "targets.cu", "graph_host.cpp"]
+           "fscore.cu", "render.cu", "posenet.cu", "front_back.cu", "targets.cu", "graph_host.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 if os.environ.get("P2M_TRACE") == "1":  # debug build: per-role event timeline of the tensor-core conv kernel (tools/umma_trace.py)
@@ -28,7 +28,10 @@ def _stale() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not _stale():
         return LIB
-    srcs = [os.path.join(CSRC, f) for f in SOURCES if os.path.exists(os.path.join(CSRC, f))]
+    srcs = [os.path.join(CSRC, f) for f in SOURCES]
+    missing = [s for s in srcs if not os.path.exists(s)]
+    if missing:  # a library without them would fail only when its symbols are looked up
+        raise FileNotFoundError("listed sources missing: " + ", ".join(missing))
     objs = []
     procs = []
     for src in srcs:

@@ -1,6 +1,6 @@
-// C-ABI layer (include/p2m_b200.h): model handle, workspace planning and the forward / backward
-// schedules of Pose2Mesh.forward (lib/models/meshnet.py:80-117 of the reference), expressed as
-// sequences of the kernels in kernels_simt.cu / cheb_umma.cu on the caller's stream.
+// C-ABI layer (include/p2m_b200.h) of the model handle: the handle, workspace planning, the eval and training forward
+// and the backward schedules of Pose2Mesh.forward (lib/models/meshnet.py:80-117 of the reference) and the single-layer
+// conv entry points, expressed as sequences of the kernels in kernels_simt.cu / cheb_umma.cu on the caller's stream.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -47,7 +47,7 @@ int arrays_device(const char* where, std::initializer_list<const void*> arrays, 
 struct Layer {
   int level, V, fin, fout;
   int bn, relu;
-  int block, pos, block_end;
+  int block_end;
 };
 
 struct Block {
@@ -188,63 +188,72 @@ Sizes model_sizes(const p2m_model* m, int B) {
   return s;
 }
 
-// Workspace map shared by forward and backward (deterministic bump order).
-struct WsMap {
+// Workspace of the network schedules: this prefix, then EvalWs's or TrainWs's part; a map sizes it (null base) and carves it
+struct WsCommon {
+  Sizes s;
+  Bump b;
   float* T;
   float* wp_scratch;
   unsigned char* wpack;   // tensor-core packed weights (one layer at a time)
   float* scale_scratch;   // [2*max_f] eval folded scale/shift
   double* sums;           // [2*max_f]
-  float* rot[3];          // eval: rotating activation buffers
-  // training: saved tensors
-  std::vector<float*> z, a, mean, invstd, scale, shift, wp;
-  float* fc_out = nullptr;
   unsigned char* fc_apack = nullptr;  // operand images of the fc GEMM on the tensor cores (launch_umma_gemm)
   unsigned char* fc_wpack = nullptr;
-  size_t bytes = 0;
-};
-
-WsMap map_workspace(const p2m_model* m, int B, int training, void* base) {
-  WsMap w;
-  Sizes s = model_sizes(m, B);
-  Bump b(base);
-  w.T = b.take<float>(s.max_T);
-  w.wp_scratch = b.take<float>(s.max_w);
-  w.wpack = b.take<unsigned char>(std::max(s.max_wpack, (size_t)16));
-  w.scale_scratch = b.take<float>(2 * (size_t)s.max_f);
-  w.sums = b.take<double>(2 * (size_t)s.max_f);
-  if (umma_gemm_supported(B, m->fc_out, m->fc_in)) {
-    w.fc_apack = b.take<unsigned char>(umma_gemm_apack_bytes(B, m->fc_in));
-    w.fc_wpack = b.take<unsigned char>(umma_gemm_wpack_bytes(m->fc_out, m->fc_in));
+  WsCommon(const p2m_model* m, int B, void* base) : s(model_sizes(m, B)), b(base) {
+    T = b.take<float>(s.max_T);
+    wp_scratch = b.take<float>(s.max_w);
+    wpack = b.take<unsigned char>(std::max(s.max_wpack, (size_t)16));
+    scale_scratch = b.take<float>(2 * (size_t)s.max_f);
+    sums = b.take<double>(2 * (size_t)s.max_f);
+    if (umma_gemm_supported(B, m->fc_out, m->fc_in)) {
+      fc_apack = b.take<unsigned char>(umma_gemm_apack_bytes(B, m->fc_in));
+      fc_wpack = b.take<unsigned char>(umma_gemm_wpack_bytes(m->fc_out, m->fc_in));
+    }
   }
-  const size_t nl = m->layers.size();
-  if (!training) {
-    for (int i = 0; i < 3; ++i) w.rot[i] = b.take<float>(s.max_act);
-  } else {
-    w.rot[0] = w.rot[1] = w.rot[2] = nullptr;
-    w.z.resize(nl); w.a.resize(nl); w.mean.resize(nl); w.invstd.resize(nl);
-    w.scale.resize(nl); w.shift.resize(nl); w.wp.resize(nl);
+  size_t bytes() const { return b.off; }
+};
+// eval: three rotating activation buffers
+struct EvalWs : WsCommon {
+  float* rot[3];
+  EvalWs(const p2m_model* m, int B, void* base) : WsCommon(m, B, base) {
+    for (int i = 0; i < 3; ++i) rot[i] = b.take<float>(s.max_act);
+  }
+};
+// training: what the forward saves for the backward
+struct TrainWs : WsCommon {
+  std::vector<float*> z, a, mean, invstd, scale, shift, wp;  // per layer; z .. shift null on the last layer (no BatchNorm)
+  float* fc_out;
+  TrainWs(const p2m_model* m, int B, void* base) : WsCommon(m, B, base) {
+    const size_t nl = m->layers.size();
+    for (std::vector<float*>* v : {&z, &a, &mean, &invstd, &scale, &shift, &wp}) v->assign(nl, nullptr);
     for (size_t i = 0; i < nl; ++i) {
       const Layer& L = m->layers[i];
       size_t n = (size_t)B * L.V * L.fout;
-      w.wp[i] = b.take<float>((size_t)L.fout * 3 * L.fin);
+      wp[i] = b.take<float>((size_t)L.fout * 3 * L.fin);
       if (L.bn) {
-        w.z[i] = b.take<float>(n);
-        w.a[i] = b.take<float>(n);
-        w.mean[i] = b.take<float>(L.fout);
-        w.invstd[i] = b.take<float>(L.fout);
-        w.scale[i] = b.take<float>(L.fout);
-        w.shift[i] = b.take<float>(L.fout);
-      } else {
-        w.z[i] = w.a[i] = nullptr;  // last layer writes y directly
-        w.mean[i] = w.invstd[i] = w.scale[i] = w.shift[i] = nullptr;
+        z[i] = b.take<float>(n);
+        a[i] = b.take<float>(n);
+        mean[i] = b.take<float>(L.fout);
+        invstd[i] = b.take<float>(L.fout);
+        scale[i] = b.take<float>(L.fout);
+        shift[i] = b.take<float>(L.fout);
       }
     }
-    w.fc_out = b.take<float>((size_t)B * m->fc_out);
+    fc_out = b.take<float>((size_t)B * m->fc_out);
   }
-  w.bytes = b.off;
-  return w;
-}
+};
+
+// Device copies of the host entry points' x and y (room for every vertex), behind their forward's workspace
+struct HostIo {
+  float *x, *y;
+  size_t bytes;
+  HostIo(const p2m_model* m, int B, void* base) {
+    Bump b(base);
+    x = b.take<float>((size_t)B * m->n_joint * m->cin);
+    y = b.take<float>((size_t)B * m->levels[0].V * m->cout);
+    bytes = b.off;
+  }
+};
 
 // Bytes of the weight-image scratch a backward packs into: the network's (BwdMap::wpack, >= the backward-data image of
 // any supported layer) or the single-layer workspace's (the forward image of the layer itself)
@@ -419,6 +428,60 @@ int conv_linear(p2m_model* m, const ConvRoute& r, const Layer& L, int B, const f
   P2M_TRY(launch_cheb_basis(g, x, in_unpool, rows, L.fin, T, s));
   P2M_TRY(launch_gemm(T, 3 * L.fin, wp, 3 * L.fin, 0, y, L.fout, rows, L.fout, 3 * L.fin, ep, s));
   return P2M_OK;
+}
+
+// Train-mode BatchNorm of a conv's output z: batch statistics, finalize (running and saved statistics, scale / shift),
+// then a = relu?(z * scale + shift) (+ the resampled residual res, if not null)
+int bn_train_tail(const float* z, int rows, int F, const float* gamma, const float* beta, float* rm, float* rv,
+                  int64_t* nbt, double* sums, float* mean, float* invstd, float* scale, float* shift, int relu,
+                  const float* res, int res_F, int res_unpool, const InterpTable* it, float* a, cudaStream_t s) {
+  P2M_TRY(launch_col_stats(z, rows, F, sums, s));
+  P2M_TRY(launch_bn_finalize(sums, z, rows, F, gamma, beta, rm, rv, nbt, mean, invstd, scale, shift, s));
+  return launch_affine_act(z, rows, F, scale, shift, relu, res, res_F, res_unpool, it, a, s);
+}
+
+// dW [fout, 3 fin] of a conv on the CUDA cores: the basis of x into T, dWp = dz^T T into the k-major dwp, unpermuted
+int simt_dw(const DevLevel& g, const float* x, int in_unpool, int rows, int fin, int fout, const float* dz, float* T,
+            float* dwp, float* dw, cudaStream_t s) {
+  P2M_TRY(launch_cheb_basis(g, x, in_unpool, rows, fin, T, s));
+  P2M_TRY(launch_fill_zero(dwp, sizeof(float) * fout * 3 * fin, s));
+  P2M_TRY(launch_gemm_tn_atomic(dz, fout, T, 3 * fin, dwp, 3 * fin, rows, fout, 3 * fin, s));
+  return launch_unpermute_w(dwp, dw, fout, fin, s);
+}
+
+// dW [fout, 3 fin] of a conv on the tensor cores: T1 of one side into T, then launch_umma_dw on that basis and plain
+// tiles of the other side; basis_of_dz: T1 = L~dz (swap = 1), else T1 = L~x.  a_scale scales dz into fp16's range.
+int tc_dw(p2m_model* m, const DevLevel& g, int batch, const float* x, int in_unpool, int fin, const float* dz, int fout,
+          bool basis_of_dz, const float* a_scale, float* T, float* dw, cudaStream_t s) {
+  P2M_TRY(basis_of_dz ? launch_cheb_t1(g, dz, 0, batch, fout, T, s, nullptr)
+                      : launch_cheb_t1(g, x, in_unpool, batch, fin, T, s, nullptr));
+  P2M_TRY(launch_fill_zero(dw, sizeof(float) * fout * 3 * fin, s));
+  return basis_of_dz ? launch_umma_dw(g, batch, dz, 0, fout, T, x, in_unpool, fin, 1, a_scale, dw, m->kernel_status,
+                                      m->sm_count, s)
+                     : launch_umma_dw(g, batch, x, in_unpool, fin, T, dz, 0, fout, 0, a_scale, dw, m->kernel_status,
+                                      m->sm_count, s);
+}
+
+// fc: joints -> coarsest mesh level (meshnet.py:104-106), as a dense GEMM on the tensor cores (wgmma, fp16x3) or SIMT
+int run_fc(const p2m_model* m, const p2m_params_t* P, const WsCommon& w, int B, const float* x, float* out, cudaStream_t s) {
+  Epilogue ep;
+  ep.bias = P->fc_b;
+  if (m->precision == P2M_PREC_FP16X3_TC && w.fc_apack != nullptr)
+    return launch_umma_gemm({x, m->fc_in, 1}, {P->fc_w, m->fc_in, 1}, B, m->fc_out, m->fc_in, ep, out, w.fc_apack,
+                            w.fc_wpack, m->kernel_status, m->sm_count, s);
+  return launch_gemm(x, m->fc_in, P->fc_w, m->fc_in, 0, out, m->fc_out, B, m->fc_out, m->fc_in, ep, s);
+}
+
+// Fused head (eval): when the next layer is the network's thin head (64 -> 3, same block, no residual) and layer li runs
+// on the tensor cores, its epilogue writes Z = act(y) W' (12 floats per row) instead of y, and the head shrinks to its
+// two 4-wide sparse products: the 64-wide activation never reaches HBM.
+bool fuses_head(const p2m_model* m, const Block& blk, int li, int B, const ConvRoute& r) {
+  const Layer& L = m->layers[li];
+  if (!m->fuse_head || !r.tc || li + 2 != (int)m->layers.size() || li + 1 >= blk.first_layer + blk.n_layers ||
+      blk.has_residual || L.fout != 64 || B * L.V < 64)
+    return false;
+  const Layer& H = m->layers[li + 1];
+  return thin_conv_supported(H.fin, H.fout) && H.fin == L.fout && H.V == L.V;
 }
 
 // The default elision policy (elide_padding == 1) on a level, whatever the batch and width.
@@ -647,18 +710,8 @@ int p2m_model_create(const p2m_model_desc_t* d, p2m_model_t** out) {
     blk.cin = ch[0];
     blk.cout = ch[len - 1];
     for (int j = 0; j < len - 1; ++j) {
-      Layer L{};
-      L.level = blk.level;
-      L.V = m->levels[L.level].V;
-      L.fin = ch[j];
-      L.fout = ch[j + 1];
       const bool last = (b == nb - 1) && (j == len - 2);
-      L.bn = !last;
-      L.relu = !last;
-      L.block = b;
-      L.pos = j;
-      L.block_end = (j == len - 2);
-      m->layers.push_back(L);
+      m->layers.push_back(Layer{blk.level, m->levels[blk.level].V, ch[j], ch[j + 1], !last, !last, j == len - 2});
       ++li;
     }
     if (blk.has_residual) {
@@ -824,7 +877,7 @@ int p2m_model_set_precision(p2m_model_t* m, int precision) {
 
 size_t p2m_meshnet_workspace_bytes(const p2m_model_t* m, int batch, int training) {
   if (!m || batch <= 0 || m->layers.empty()) return 0;
-  return map_workspace(m, batch, training, nullptr).bytes;
+  return training ? TrainWs(m, batch, nullptr).bytes() : EvalWs(m, batch, nullptr).bytes();
 }
 size_t p2m_meshnet_backward_scratch_bytes(const p2m_model_t* m, int batch) {
   if (!m || batch <= 0 || m->layers.empty()) return 0;
@@ -832,36 +885,24 @@ size_t p2m_meshnet_backward_scratch_bytes(const p2m_model_t* m, int batch) {
 }
 size_t p2m_meshnet_host_io_bytes(const p2m_model_t* m, int batch) {
   if (!m || batch <= 0 || m->layers.empty()) return 0;
-  return align_up((size_t)batch * m->n_joint * m->cin * 4) + align_up((size_t)batch * m->levels[0].V * m->cout * 4);
+  return HostIo(m, batch, nullptr).bytes;
 }
 
 // -------------------------------------------------------------------------------------
-static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, int training,
-                                void* workspace, size_t workspace_bytes, p2m_stream_t stream, int gathered) {
-  if (!m || !x || !y || B <= 0 || !workspace || m->layers.empty()) {
-    set_error("meshnet_forward: bad argument");
-    return P2M_ERR_INVALID;
-  }
-  P2M_TRY(check_params(m, P, true));
-  P2M_TRY(check_kernel_status(m, "meshnet_forward"));
-  DeviceGuard guard(m->device);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  WsMap w = map_workspace(m, B, training, workspace);
-  if (w.bytes > workspace_bytes) {
-    set_error("meshnet_forward: workspace too small (" + std::to_string(workspace_bytes) + " < " +
-              std::to_string(w.bytes) + ")");
-    return P2M_ERR_WORKSPACE;
-  }
-  const int nb = (int)m->blocks.size();
+// The eval forward: folded BatchNorm, rotating buffers, fused head, padding-row dedup, fused output gather (`gathered`)
+static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, void* workspace,
+                        cudaStream_t s, int gathered) {
+  const EvalWs w(m, B, workspace);
   const int nl = (int)m->layers.size();
-  // isolated (padding) rows in eval mode: only class representatives (DevLevel::rep_tiles), or — when the caller
-  // takes the gathered real vertices — none at all: no connected row ever reads an isolated one
-  const int iso_mode = (training || !m->dedup_padding || m->elide_padding < 1) ? 0 : (gathered ? 2 : 1);
+  // isolated (padding) rows: only class representatives (DevLevel::rep_tiles), or — when the caller takes the gathered
+  // real vertices — none at all: no connected row ever reads an isolated one
+  const int iso_mode = (!m->dedup_padding || m->elide_padding < 1) ? 0 : (gathered ? 2 : 1);
   const float* cur = x;
   int cur_unpool = 0;
-  int cur_buf = -1;  // rotating buffer id holding `cur` (eval)
-  float* head_z = nullptr;  // eval: Z of the thin head, produced by the previous layer's epilogue (see below)
-  for (int b = 0; b < nb; ++b) {
+  int cur_buf = -1;  // rotating buffer id holding `cur`
+  auto free_rot = [](int a, int b) { return a != 0 && b != 0 ? 0 : (a != 1 && b != 1 ? 1 : 2); };  // not a, not b
+  float* head_z = nullptr;  // Z of the thin head, produced by the previous layer's epilogue (fuses_head)
+  for (int b = 0; b < (int)m->blocks.size(); ++b) {
     const Block& blk = m->blocks[b];
     const float* block_in = cur;
     const int block_in_unpool = cur_unpool;
@@ -873,117 +914,67 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
       const bool last = (li == nl - 1);
       const bool with_res = L.block_end && blk.has_residual;
       const ConvRoute r = conv_route(m, L.level, L.fin, L.fout, B, true);
-      if (!training) {
-        Epilogue ep;
-        float* scale = w.scale_scratch;
-        float* shift = w.scale_scratch + L.fout;
-        if (L.bn) {
-          P2M_TRY(launch_bn_fold_eval(P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li], P->cl_b[li], scale, shift,
-                                      L.fout, s));
-          ep.scale = scale;
-          ep.shift = shift;
-        } else {
-          ep.bias = P->cl_b[li];
-        }
-        ep.relu = L.relu;
-        if (with_res) {
-          ep.res = block_in;
-          ep.res_F = blk.cin;
-          ep.res_unpool = block_in_unpool;
-          ep.res_i0 = blk.interp.i0;
-          ep.res_i1 = blk.interp.i1;
-          ep.res_lam = blk.interp.lam;
-        }
-        float* out;
-        int out_buf = -1;
-        if (last) {
-          out = y;
-          if (gathered) {
-            if (!thin_conv_supported(L.fin, L.fout) || with_res) {
-              set_error("meshnet_forward_vertices: the head layer is not on the fused-gather path");
-              return P2M_ERR_INVALID;
-            }
-            ep.out_map = m->out_map;
-            ep.out_rows = m->out_rows;
-            ep.level_V = L.V;
-          }
-        } else {
-          for (int c = 0; c < 3; ++c)
-            if (c != cur_buf && c != block_in_buf) {
-              out_buf = c;
-              break;
-            }
-          out = w.rot[out_buf];
-        }
-        if (m->profiling) P2M_CUDA_OK(cudaEventRecord(m->ev_beg[li], s));
-        // Fused head: when the next layer is the network's thin head (64 -> 3, same block, no residual) and this
-        // layer runs on the tensor cores, its epilogue writes Z = act(y) W' (12 floats per row) instead of y, and
-        // the head shrinks to its two 4-wide sparse products: the 64-wide activation never reaches HBM.
-        bool fuse_head = false;
-        if (m->fuse_head && !last && li + 1 == nl - 1 && j + 1 < blk.n_layers && !with_res && !blk.has_residual &&
-            L.fout == 64 && rows >= 64 && r.tc) {
-          const Layer& H = m->layers[li + 1];
-          fuse_head = thin_conv_supported(H.fin, H.fout) && H.fin == L.fout && H.V == L.V;
-        }
-        if (head_z != nullptr) {  // this IS the head, its Z is already there
-          P2M_TRY(launch_thin_tail(m->levels[L.level], rows, L.fout, head_z, head_z + (size_t)rows * 12, ep, out, s));
-          head_z = nullptr;
-        } else if (fuse_head) {
-          float* Z = out;  // [rows][12] | U [rows][4] | W' [64][12] inside this layer's (unused) output buffer
-          float* wt = Z + (size_t)rows * 16;
-          P2M_TRY(launch_thin_prep(P->cl_w[li + 1], L.fout, m->layers[li + 1].fout, wt, s));
-          P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, false,
-                              iso_mode, wt, Z));
-          head_z = Z;
-        } else {
-          P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, false,
-                              iso_mode));
-        }
-        if (m->profiling) P2M_CUDA_OK(cudaEventRecord(m->ev_end[li], s));
-        cur = out;
-        cur_buf = out_buf;
-        cur_unpool = 0;
-      } else {
-        Epilogue ep;
-        ep.bias = P->cl_b[li];
-        float* z = last ? y : w.z[li];
-        P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp[li], w.wpack, ep, z, s, true));
-        if (L.bn) {
-          P2M_TRY(launch_col_stats(z, rows, L.fout, w.sums, s));
-          P2M_TRY(launch_bn_finalize(w.sums, z, rows, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li],
-                                     P->bn_nbt ? P->bn_nbt[li] : nullptr, w.mean[li], w.invstd[li], w.scale[li],
-                                     w.shift[li], s));
-          P2M_TRY(launch_affine_act(z, rows, L.fout, w.scale[li], w.shift[li], L.relu, with_res ? block_in : nullptr,
-                                    blk.cin, block_in_unpool, with_res ? &blk.interp : nullptr, w.a[li], s));
-          cur = w.a[li];
-        } else {
-          cur = z;
-        }
-        cur_unpool = 0;
-      }
-    }
-    if (b == 0) {  // fc: joints -> coarsest mesh level (meshnet.py:104-106)
       Epilogue ep;
-      ep.bias = P->fc_b;
-      float* out;
-      if (!training) {
-        int out_buf = -1;
-        for (int c = 0; c < 3; ++c)
-          if (c != cur_buf) {
-            out_buf = c;
-            break;
-          }
-        out = w.rot[out_buf];
-        cur_buf = out_buf;
+      float* scale = w.scale_scratch;
+      float* shift = w.scale_scratch + L.fout;
+      if (L.bn) {
+        P2M_TRY(launch_bn_fold_eval(P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li], P->cl_b[li], scale, shift,
+                                    L.fout, s));
+        ep.scale = scale;
+        ep.shift = shift;
       } else {
-        out = w.fc_out;
+        ep.bias = P->cl_b[li];
       }
-      if (m->precision == P2M_PREC_FP16X3_TC && w.fc_apack != nullptr)  // dense GEMM on the tensor cores (wgmma, fp16x3)
-        P2M_TRY(launch_umma_gemm({cur, m->fc_in, 1}, {P->fc_w, m->fc_in, 1}, B, m->fc_out, m->fc_in, ep, out, w.fc_apack, w.fc_wpack, m->kernel_status,
-                                 m->sm_count, s));
-      else
-        P2M_TRY(launch_gemm(cur, m->fc_in, P->fc_w, m->fc_in, 0, out, m->fc_out, B, m->fc_out, m->fc_in, ep, s));
+      ep.relu = L.relu;
+      if (with_res) {
+        ep.res = block_in;
+        ep.res_F = blk.cin;
+        ep.res_unpool = block_in_unpool;
+        ep.res_i0 = blk.interp.i0;
+        ep.res_i1 = blk.interp.i1;
+        ep.res_lam = blk.interp.lam;
+      }
+      float* out;
+      int out_buf = -1;
+      if (last) {
+        out = y;
+        if (gathered) {
+          if (!thin_conv_supported(L.fin, L.fout) || with_res) {
+            set_error("meshnet_forward_vertices: the head layer is not on the fused-gather path");
+            return P2M_ERR_INVALID;
+          }
+          ep.out_map = m->out_map;
+          ep.out_rows = m->out_rows;
+          ep.level_V = L.V;
+        }
+      } else {
+        out_buf = free_rot(cur_buf, block_in_buf);
+        out = w.rot[out_buf];
+      }
+      if (m->profiling) P2M_CUDA_OK(cudaEventRecord(m->ev_beg[li], s));
+      if (head_z != nullptr) {  // this IS the head, its Z is already there
+        P2M_TRY(launch_thin_tail(m->levels[L.level], rows, L.fout, head_z, head_z + (size_t)rows * 12, ep, out, s));
+        head_z = nullptr;
+      } else if (fuses_head(m, blk, li, B, r)) {
+        float* Z = out;  // [rows][12] | U [rows][4] | W' [64][12] inside this layer's (unused) output buffer
+        float* wt = Z + (size_t)rows * 16;
+        P2M_TRY(launch_thin_prep(P->cl_w[li + 1], L.fout, m->layers[li + 1].fout, wt, s));
+        P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, false,
+                            iso_mode, wt, Z));
+        head_z = Z;
+      } else {
+        P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp_scratch, w.wpack, ep, out, s, false,
+                            iso_mode));
+      }
+      if (m->profiling) P2M_CUDA_OK(cudaEventRecord(m->ev_end[li], s));
       cur = out;
+      cur_buf = out_buf;
+      cur_unpool = 0;
+    }
+    if (b == 0) {
+      cur_buf = free_rot(cur_buf, -1);
+      P2M_TRY(run_fc(m, P, w, B, cur, w.rot[cur_buf], s));
+      cur = w.rot[cur_buf];
       cur_unpool = 0;
     } else if (blk.out_unpool) {
       cur_unpool = 1;  // nearest x2 unpool is virtual: the next block reads row r>>1
@@ -997,9 +988,67 @@ static int meshnet_forward_impl(p2m_model_t* m, const p2m_params_t* P, const flo
   return P2M_OK;
 }
 
+// The training forward: batch-statistics BatchNorm; saves what p2m_meshnet_backward reads (TrainWs).
+static int forward_train(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, void* workspace,
+                         cudaStream_t s) {
+  const TrainWs w(m, B, workspace);
+  const float* cur = x;
+  int cur_unpool = 0;
+  for (int b = 0; b < (int)m->blocks.size(); ++b) {
+    const Block& blk = m->blocks[b];
+    const float* block_in = cur;
+    const int block_in_unpool = cur_unpool;
+    for (int j = 0; j < blk.n_layers; ++j) {
+      const int li = blk.first_layer + j;
+      const Layer& L = m->layers[li];
+      const bool with_res = L.block_end && blk.has_residual;
+      const ConvRoute r = conv_route(m, L.level, L.fin, L.fout, B, true);
+      Epilogue ep;
+      ep.bias = P->cl_b[li];
+      float* z = L.bn ? w.z[li] : y;  // the last layer, the only one without BatchNorm, writes y
+      P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp[li], w.wpack, ep, z, s, true));
+      if (L.bn)
+        P2M_TRY(bn_train_tail(z, B * L.V, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li],
+                              P->bn_nbt ? P->bn_nbt[li] : nullptr, w.sums, w.mean[li], w.invstd[li], w.scale[li],
+                              w.shift[li], L.relu, with_res ? block_in : nullptr, blk.cin, block_in_unpool,
+                              with_res ? &blk.interp : nullptr, w.a[li], s));
+      cur = L.bn ? w.a[li] : z;
+      cur_unpool = 0;
+    }
+    if (b == 0) {
+      P2M_TRY(run_fc(m, P, w, B, cur, w.fc_out, s));
+      cur = w.fc_out;
+      cur_unpool = 0;
+    } else if (blk.out_unpool) {
+      cur_unpool = 1;
+    }
+  }
+  return P2M_OK;
+}
+
+// Checks the arguments before anything is enqueued, then runs the eval or the training schedule
+static int meshnet_forward(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, int training,
+                           void* workspace, size_t workspace_bytes, p2m_stream_t stream, int gathered) {
+  if (!m || !x || !y || B <= 0 || !workspace || m->layers.empty()) {
+    set_error("meshnet_forward: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  P2M_TRY(check_params(m, P, true));
+  P2M_TRY(check_kernel_status(m, "meshnet_forward"));
+  DeviceGuard guard(m->device);
+  const size_t need = p2m_meshnet_workspace_bytes(m, B, training);
+  if (need > workspace_bytes) {
+    set_error("meshnet_forward: workspace too small (" + std::to_string(workspace_bytes) + " < " +
+              std::to_string(need) + ")");
+    return P2M_ERR_WORKSPACE;
+  }
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  return training ? forward_train(m, P, x, y, B, workspace, s) : forward_eval(m, P, x, y, B, workspace, s, gathered);
+}
+
 int p2m_meshnet_forward(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, int training,
                         void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
-  return meshnet_forward_impl(m, P, x, y, B, training, workspace, workspace_bytes, stream, 0);
+  return meshnet_forward(m, P, x, y, B, training, workspace, workspace_bytes, stream, 0);
 }
 
 int p2m_model_set_output_gather(p2m_model_t* m, const int32_t* vertex_of_slot, int n_slots) {
@@ -1035,7 +1084,7 @@ int p2m_meshnet_forward_vertices(p2m_model_t* m, const p2m_params_t* P, const fl
     set_error("meshnet_forward_vertices: call p2m_model_set_output_gather first");
     return P2M_ERR_INVALID;
   }
-  return meshnet_forward_impl(m, P, x, y_vertices, B, 0, workspace, workspace_bytes, stream, 1);
+  return meshnet_forward(m, P, x, y_vertices, B, 0, workspace, workspace_bytes, stream, 1);
 }
 
 static int forward_host_impl(p2m_model_t* m, const p2m_params_t* P, const float* x_host, float* y_host, int B,
@@ -1048,19 +1097,16 @@ static int forward_host_impl(p2m_model_t* m, const p2m_params_t* P, const float*
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const size_t out_rows = gathered ? (size_t)m->out_rows : (size_t)m->levels[0].V;
   const size_t xb = (size_t)B * m->n_joint * m->cin * 4, yb = (size_t)B * out_rows * m->cout * 4;
-  const size_t io = p2m_meshnet_host_io_bytes(m, B);
   const size_t need = p2m_meshnet_workspace_bytes(m, B, 0);
-  if (workspace_bytes < need + io) {
+  const HostIo io(m, B, static_cast<char*>(workspace) + need);
+  if (workspace_bytes < need + io.bytes) {
     set_error("meshnet_forward_host: workspace too small");
     return P2M_ERR_WORKSPACE;
   }
   DeviceGuard guard(m->device);
-  char* base = static_cast<char*>(workspace);
-  float* xd = reinterpret_cast<float*>(base + need);
-  float* yd = reinterpret_cast<float*>(base + need + align_up(xb));
-  P2M_CUDA_OK(cudaMemcpyAsync(xd, x_host, xb, cudaMemcpyHostToDevice, s));
-  P2M_TRY(meshnet_forward_impl(m, P, xd, yd, B, 0, workspace, need, stream, gathered));
-  P2M_CUDA_OK(cudaMemcpyAsync(y_host, yd, yb, cudaMemcpyDeviceToHost, s));
+  P2M_CUDA_OK(cudaMemcpyAsync(io.x, x_host, xb, cudaMemcpyHostToDevice, s));
+  P2M_TRY(meshnet_forward(m, P, io.x, io.y, B, 0, workspace, need, stream, gathered));
+  P2M_CUDA_OK(cudaMemcpyAsync(y_host, io.y, yb, cudaMemcpyDeviceToHost, s));
   P2M_CUDA_OK(cudaStreamSynchronize(s));
   return check_kernel_status(m, "meshnet_forward_host");
 }
@@ -1088,9 +1134,9 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
   P2M_TRY(check_kernel_status(m, "meshnet_backward"));
   DeviceGuard guard(m->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  WsMap w = map_workspace(m, B, 1, workspace);
+  const TrainWs w(m, B, workspace);
   BwdMap sc = map_scratch(m, B, scratch);
-  if (w.bytes > workspace_bytes || sc.bytes > scratch_bytes) {
+  if (w.bytes() > workspace_bytes || sc.bytes > scratch_bytes) {
     set_error("meshnet_backward: workspace/scratch too small");
     return P2M_ERR_WORKSPACE;
   }
@@ -1165,25 +1211,13 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         // dW.  tensor-core path: T2 of one side is formed on chip by the forward's producers from T1 = L~(that side)
         // and contracted with the (power-of-two scaled) plain tiles of the other side by MN-major wgmma; otherwise
         // SIMT: materialise T, dWp = g_z^T T.
-        if (r.dw_dz_basis) {
-          // sum_rows dz (x) T_k(X) = sum_rows T_k(dz) (x) X  (L~ symmetric): the basis of the GRADIENT, whose first
-          // sparse product the backward-data pass below needs anyway, contracted with plain tiles of the layer input
-          P2M_TRY(launch_cheb_t1(g, g_z, 0, B, L.fout, w.T, s, nullptr));
-          P2M_TRY(launch_fill_zero(G->cl_w[li], sizeof(float) * L.fout * 3 * L.fin, s));
-          P2M_TRY(launch_umma_dw(g, B, g_z, 0, L.fout, w.T, inp, in_unpool, L.fin, 1, sc.a_scale, G->cl_w[li],
-                                 m->kernel_status, m->sm_count, s));
-        } else if (r.tc_dw) {
-          // the basis of the layer input (w.T is overwritten by the dX pass's own T1 pass below)
-          P2M_TRY(launch_cheb_t1(g, inp, in_unpool, B, L.fin, w.T, s, nullptr));
-          P2M_TRY(launch_fill_zero(G->cl_w[li], sizeof(float) * L.fout * 3 * L.fin, s));
-          P2M_TRY(launch_umma_dw(g, B, inp, in_unpool, L.fin, w.T, g_z, 0, L.fout, 0, sc.a_scale, G->cl_w[li],
-                                 m->kernel_status, m->sm_count, s));
-        } else {
-          P2M_TRY(launch_cheb_basis(g, inp, in_unpool, rows, L.fin, w.T, s));
-          P2M_TRY(launch_fill_zero(sc.dwp, sizeof(float) * L.fout * 3 * L.fin, s));
-          P2M_TRY(launch_gemm_tn_atomic(g_z, L.fout, w.T, 3 * L.fin, sc.dwp, 3 * L.fin, rows, L.fout, 3 * L.fin, s));
-          P2M_TRY(launch_unpermute_w(sc.dwp, G->cl_w[li], L.fout, L.fin, s));
-        }
+        // With dw_dz_basis: sum_rows dz (x) T_k(X) = sum_rows T_k(dz) (x) X  (L~ symmetric), the basis of the GRADIENT,
+        // whose first sparse product the backward-data pass below needs anyway, contracted with plain tiles of the layer
+        // input.  Otherwise the basis of the layer input (w.T is overwritten by the dX pass's own T1 pass below).
+        if (r.dw_dz_basis || r.tc_dw)
+          P2M_TRY(tc_dw(m, g, B, inp, in_unpool, L.fin, g_z, L.fout, r.dw_dz_basis, sc.a_scale, w.T, G->cl_w[li], s));
+        else
+          P2M_TRY(simt_dw(g, inp, in_unpool, rows, L.fin, L.fout, g_z, w.T, sc.dwp, G->cl_w[li], s));
       }
       // dX
       if (need_dx && r.tc_dx) {
@@ -1315,11 +1349,7 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   DeviceGuard guard(m->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const DevLevel& g = m->levels[a->level];
-  Layer L{};
-  L.level = a->level;
-  L.V = g.V;
-  L.fin = a->fin;
-  L.fout = a->fout;
+  const Layer L{a->level, g.V, a->fin, a->fout};
   const size_t rows = (size_t)a->batch * L.V;
   const LayerWs w = map_layer_workspace(workspace, rows, L.fin, L.fout);
   const ConvRoute r = conv_route(m, a->level, L.fin, L.fout, a->batch, false);
@@ -1365,12 +1395,9 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   }
   ep.bias = a->bias;
   P2M_TRY(conv(ep, w.z));
-  P2M_TRY(launch_col_stats(w.z, (int)rows, L.fout, w.sums, s));
-  P2M_TRY(launch_bn_finalize(w.sums, w.z, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean,
-                             a->bn_running_var, a->bn_num_batches_tracked, a->save_mean, a->save_invstd, w.sc,
-                             w.sc + L.fout, s));
-  P2M_TRY(launch_affine_act(w.z, (int)rows, L.fout, w.sc, w.sc + L.fout, a->relu, nullptr, 0, 0, nullptr, a->y, s));
-  return P2M_OK;
+  return bn_train_tail(w.z, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var,
+                       a->bn_num_batches_tracked, w.sums, a->save_mean, a->save_invstd, w.sc, w.sc + L.fout, a->relu,
+                       nullptr, 0, 0, nullptr, a->y, s);
 }
 
 int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* workspace, size_t workspace_bytes,
@@ -1407,16 +1434,10 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
     // before the dX pass overwrites it.
     P2M_TRY(launch_absmax_scale(a->x, (long long)rows * fin, rs.x_scale, s, g.headroom_log2));
     P2M_TRY(launch_scale_by(a->x, (long long)rows * fin, rs.x_scale, 0, 1.f, w.U, s));
-    P2M_TRY(launch_cheb_t1(g, w.U, 0, a->batch, fin, w.T, s));
-    P2M_TRY(launch_fill_zero(a->dweight, sizeof(float) * fout * 3 * fin, s));
-    P2M_TRY(launch_umma_dw(g, a->batch, w.U, 0, fin, w.T, a->dz, 0, fout, 0, a_scale, a->dweight, m->kernel_status,
-                           m->sm_count, s));
+    P2M_TRY(tc_dw(m, g, a->batch, w.U, 0, fin, a->dz, fout, false, a_scale, w.T, a->dweight, s));
     P2M_TRY(launch_scale_by(a->dweight, (long long)fout * 3 * fin, rs.x_scale, 1, 1.f, a->dweight, s));
   } else {
-    P2M_TRY(launch_cheb_basis(g, a->x, 0, (int)rows, fin, w.T, s));
-    P2M_TRY(launch_fill_zero(w.w2, sizeof(float) * fout * 3 * fin, s));
-    P2M_TRY(launch_gemm_tn_atomic(a->dz, fout, w.T, 3 * fin, w.w2, 3 * fin, (int)rows, fout, 3 * fin, s));
-    P2M_TRY(launch_unpermute_w(w.w2, a->dweight, fout, fin, s));
+    P2M_TRY(simt_dw(g, a->x, 0, (int)rows, fin, fout, a->dz, w.T, w.w2, a->dweight, s));
   }
   if (a->dx) {
     Epilogue none;
@@ -1435,450 +1456,6 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
     }
     P2M_TRY(launch_cheb_basis_bwd(g, w.T, (int)rows, fin, w.U, nullptr, 0, nullptr, 0, a->dx, s));
   }
-  return P2M_OK;
-}
-
-}  // extern "C"
-
-// =====================================================================================
-// Row f1 of SURVEY.md §8: what FlatPose2Mesh runs in front of MeshNet (lib/models/pose2mesh_net.py:16-22) —
-// the PoseNet 2-D -> 3-D lifter (lib/models/posenet.py:41-87, eval mode: running-stat BatchNorm, dropout off) and
-// the concat  pose_combine = cat(pose2d, pose3d / 1000)  that becomes MeshNet's input.
-//   y  = x W1^T + b1                                                  [B, H]
-//   per stage:  y += relu(bn2(relu(bn1(y)) Wa^T + ba)) Wb^T + bb
-//   pose3d = y W2^T + b2                                              [B, 3J]
-// fp32 FFMA GEMMs (k_gemm) with the BatchNorm / ReLU / residual fused into the epilogues; B rows only, so the
-// 4 H x H weight matrices (64 MB each at H = 4096) dominate the traffic and are read once per call.
-// =====================================================================================
-namespace {
-__global__ void __launch_bounds__(256) k_bn_relu_rows(const float* __restrict__ x, long long n, int F,
-                                                      const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                      const float* __restrict__ rm, const float* __restrict__ rv,
-                                                      float* __restrict__ y) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int f = (int)(i % F);
-  const float sc = gamma[f] / sqrtf(rv[f] + 1e-5f);
-  y[i] = fmaxf(fmaf(x[i] - rm[f], sc, beta[f]), 0.f);
-}
-__global__ void __launch_bounds__(256) k_take_cols(const float* __restrict__ src, int ld, const float* __restrict__ bias,
-                                                   int n_col, long long n, float* __restrict__ dst) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const long long r = i / n_col;
-  const int c = (int)(i - r * n_col);
-  dst[i] = src[r * ld + c] + bias[c];
-}
-__global__ void __launch_bounds__(256) k_pose_combine(const float* __restrict__ pose2d, const float* __restrict__ pose3d,
-                                                      long long n_joint_rows, float* __restrict__ out) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // (b, j)
-  if (i >= n_joint_rows) return;
-  out[i * 5 + 0] = pose2d[i * 2 + 0];
-  out[i * 5 + 1] = pose2d[i * 2 + 1];
-  out[i * 5 + 2] = pose3d[i * 3 + 0] / 1000.f;
-  out[i * 5 + 3] = pose3d[i * 3 + 1] / 1000.f;
-  out[i * 5 + 4] = pose3d[i * 3 + 2] / 1000.f;
-}
-}  // namespace
-
-namespace p2m {
-int launch_take_cols(const float* src, int ld, const float* bias, int n_col, long long rows, float* dst, cudaStream_t s) {
-  const long long n = rows * n_col;
-  k_take_cols<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src, ld, bias, n_col, n, dst);
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-int launch_pose_combine(const float* pose2d, const float* pose3d, long long n_joint_rows, float* out, cudaStream_t s) {
-  k_pose_combine<<<(unsigned)((n_joint_rows + 255) / 256), 256, 0, s>>>(pose2d, pose3d, n_joint_rows, out);
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-}  // namespace p2m
-
-extern "C" {
-
-size_t p2m_posenet_workspace_bytes(int batch, int hidden) {
-  if (batch <= 0 || hidden <= 0) return 0;
-  size_t n = 3 * align_up((size_t)batch * hidden * 4) + align_up(2 * (size_t)hidden * 4) + ALIGN;
-  if (umma_gemm_supported(batch, hidden, hidden))  // operand images of the hidden x hidden GEMMs (tensor-core path)
-    n += align_up(umma_gemm_apack_bytes(batch, hidden)) + align_up(umma_gemm_wpack_bytes(hidden, hidden));
-  return n;
-}
-
-int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, float* pose3d, float* pose_combine, int B,
-                        void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
-  if (!P || !pose2d || !pose3d || B <= 0 || !workspace || P->num_joint <= 0 || P->hidden <= 0 || P->num_stage < 0 ||
-      !P->w1_w || !P->w1_b || !P->w2_w || !P->w2_b) {
-    set_error("posenet_forward: bad argument");
-    return P2M_ERR_INVALID;
-  }
-  if (workspace_bytes < p2m_posenet_workspace_bytes(B, P->hidden)) {
-    set_error("posenet_forward: workspace too small");
-    return P2M_ERR_WORKSPACE;
-  }
-  int dev;
-  P2M_TRY(arrays_device("posenet_forward", {pose2d, pose3d, pose_combine, workspace}, &dev));
-  DeviceGuard guard(dev);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int H = P->hidden, J = P->num_joint;
-  Bump b(workspace);
-  float* y = b.take<float>((size_t)B * H);
-  float* a = b.take<float>((size_t)B * H);
-  float* h = b.take<float>((size_t)B * H);
-  float* sc = b.take<float>(2 * (size_t)H);
-  int* status = b.take<int>(1);
-  // The two H x H GEMMs of every stage run on the tensor cores (wgmma, fp16x3, both operands streamed by cp.async.bulk:
-  // launch_umma_gemm) when H allows; the thin first / last layers (K = 2J, N = 3J) stay on the fp32 SIMT GEMM.
-  const bool tc = umma_gemm_supported(B, H, H);
-  void* apack = tc ? b.take<unsigned char>(umma_gemm_apack_bytes(B, H)) : nullptr;
-  void* wpack = tc ? b.take<unsigned char>(umma_gemm_wpack_bytes(H, H)) : nullptr;
-  int sm_count = 132;
-  if (tc) {
-    P2M_CUDA_OK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-    P2M_CUDA_OK(cudaMemsetAsync(status, 0, sizeof(int), s));
-  }
-  auto big_gemm = [&](const float* X, const float* Wm, const Epilogue& e, float* Y) -> int {
-    if (tc) return launch_umma_gemm({X, H, 1}, {Wm, H, 1}, B, H, H, e, Y, apack, wpack, status, sm_count, s);
-    return launch_gemm(X, H, Wm, H, 0, Y, H, B, H, H, e, s);
-  };
-  Epilogue e1;
-  e1.bias = P->w1_b;
-  P2M_TRY(launch_gemm(pose2d, 2 * J, P->w1_w, 2 * J, 0, y, H, B, H, 2 * J, e1, s));
-  for (int st = 0; st < P->num_stage; ++st) {
-    const p2m_posenet_stage_t& S = P->stages[st];
-    if (!S.w1_w || !S.w1_b || !S.w2_w || !S.w2_b || !S.bn1_w || !S.bn1_b || !S.bn1_rm || !S.bn1_rv || !S.bn2_w ||
-        !S.bn2_b || !S.bn2_rm || !S.bn2_rv) {
-      set_error("posenet_forward: null stage tensor");
-      return P2M_ERR_INVALID;
-    }
-    // a = relu(bn1(y))
-    const long long n = (long long)B * H;
-    k_bn_relu_rows<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(y, n, H, S.bn1_w, S.bn1_b, S.bn1_rm, S.bn1_rv, a);
-    P2M_LAUNCH_OK();
-    // h = relu(bn2(a Wa^T + ba)): BatchNorm folded into the GEMM epilogue
-    P2M_TRY(launch_bn_fold_eval(S.bn2_w, S.bn2_b, S.bn2_rm, S.bn2_rv, S.w1_b, sc, sc + H, H, s));
-    Epilogue ea;
-    ea.scale = sc;
-    ea.shift = sc + H;
-    ea.relu = 1;
-    P2M_TRY(big_gemm(a, S.w1_w, ea, h));
-    // y' = y + h Wb^T + bb  (written to `a`, then the buffers swap roles)
-    Epilogue eb;
-    eb.bias = S.w2_b;
-    eb.res = y;
-    eb.res_F = H;
-    P2M_TRY(big_gemm(h, S.w2_w, eb, a));
-    std::swap(y, a);
-  }
-  if (tc && 3 * J <= 64) {
-    // the K = H reduction of the output layer on the tensor cores as well: N padded to 64 zero-weight columns (two CTAs of
-    // the fp32 SIMT GEMM would walk the 4096-long reduction alone), then the 3J real columns are copied out + bias
-    P2M_TRY(launch_umma_gemm({y, H, 1}, {P->w2_w, H, 1}, B, 64, H, Epilogue(), h, apack, wpack, status, sm_count, s, 3 * J));
-    P2M_TRY(launch_take_cols(h, 64, P->w2_b, 3 * J, B, pose3d, s));
-  } else {
-    Epilogue e2;
-    e2.bias = P->w2_b;
-    P2M_TRY(launch_gemm(y, H, P->w2_w, H, 0, pose3d, 3 * J, B, 3 * J, H, e2, s));
-  }
-  if (pose_combine != nullptr) P2M_TRY(launch_pose_combine(pose2d, pose3d, (long long)B * J, pose_combine, s));
-  return P2M_OK;
-}
-
-}  // extern "C"
-
-// =====================================================================================
-// Row f2 of SURVEY.md §8: the steps either side of the model in the reference's callers.
-//  * joint regression  joints = J_regressor @ vertices   (lib/core/base.py:131,204; demo/run.py:171)
-//  * the demo's input normalisation, demo/run.py:150-158: tight box of the 2-D joints (coord_utils.py:21-39) ->
-//    aspect-preserving box of the network input (process_bbox, :42-66) -> affine map into the input_w x input_h
-//    patch (aug_utils.py:51-64,140-179 with rot = 0: a uniform scaling that maps the box centre to the patch
-//    centre) -> divide by the patch size -> per-pose zero mean / unit std per coordinate.
-// =====================================================================================
-namespace {
-__global__ void __launch_bounds__(256) k_regress_joints(const float* __restrict__ Jr, const float* __restrict__ verts,
-                                                        int n_vertex, int chans, float* __restrict__ joints) {
-  // one CTA per (joint, mesh); chans <= 4
-  const int j = blockIdx.x, n_joint = gridDim.x;
-  const long long b = blockIdx.y;
-  const float* jr = Jr + (size_t)j * n_vertex;
-  const float* vb = verts + b * (long long)n_vertex * chans;
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int v = threadIdx.x; v < n_vertex; v += 256) {
-    const float w = __ldg(jr + v);
-    for (int c = 0; c < chans; ++c) acc[c] = fmaf(w, vb[(long long)v * chans + c], acc[c]);
-  }
-  __shared__ float red[4][8];
-  for (int c = 0; c < 4; ++c) {
-    float a = acc[c];
-    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-    if ((threadIdx.x & 31) == 0) red[c][threadIdx.x >> 5] = a;
-  }
-  __syncthreads();
-  if (threadIdx.x < chans) {
-    float a = 0.f;
-    for (int w = 0; w < 8; ++w) a += red[threadIdx.x][w];
-    joints[(b * n_joint + j) * chans + threadIdx.x] = a;
-  }
-}
-
-// one warp per pose, lane = joint (n_joint <= 32)
-__global__ void __launch_bounds__(128) k_normalize_pose2d(const float* __restrict__ px, int batch, int n_joint, int in_h,
-                                                          int in_w, int truncate, float* __restrict__ out) {
-  const int pose = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (pose >= batch) return;
-  const bool on = lane < n_joint;
-  const float x = on ? px[((long long)pose * n_joint + lane) * 2 + 0] : 0.f;
-  const float y = on ? px[((long long)pose * n_joint + lane) * 2 + 1] : 0.f;
-  float xmin = on ? x : INFINITY, xmax = on ? x : -INFINITY, ymin = on ? y : INFINITY, ymax = on ? y : -INFINITY;
-  for (int o = 16; o > 0; o >>= 1) {
-    xmin = fminf(xmin, __shfl_xor_sync(0xffffffffu, xmin, o));
-    xmax = fmaxf(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
-    ymin = fminf(ymin, __shfl_xor_sync(0xffffffffu, ymin, o));
-    ymax = fmaxf(ymax, __shfl_xor_sync(0xffffffffu, ymax, o));
-  }
-  // get_bbox (float32 arithmetic like numpy on the float32 box)
-  float bx, by, bw, bh;
-  {
-    const double xc = ((double)xmin + (double)xmax) / 2.0, w = (double)xmax - (double)xmin;
-    const double yc = ((double)ymin + (double)ymax) / 2.0, h = (double)ymax - (double)ymin;
-    bx = (float)(xc - 0.5 * w); by = (float)(yc - 0.5 * h); bw = (float)w; bh = (float)h;
-  }
-  // process_bbox: sanitise (x2 = x + (w - 1)), grow to the aspect ratio width / height, scale 1.0
-  float w = (bx + (bw - 1.f)) - bx, h = (by + (bh - 1.f)) - by;
-  const float cx = bx + w / 2.f, cy = by + h / 2.f;
-  const float aspect = (float)in_w / (float)in_h;
-  if (w > aspect * h) h = w / aspect;
-  else if (w < aspect * h) w = h * aspect;
-  const float x0 = cx - w / 2.f, y0 = cy - h / 2.f;
-  // get_center_scale + get_affine_transform(rot = 0): three float32 point pairs, solved in double
-  const float ccx = x0 + w * 0.5f, ccy = y0 + h * 0.5f;
-  const float s1y = ccy + w * -0.5f;                                     // src[1] = centre + (0, -src_w / 2)
-  const double dst_w = (double)in_w, dst_h = (double)in_h;
-  const float d1y = (float)(dst_h * 0.5) + (float)(dst_w * -0.5);        // dst[1] = (dst_w / 2, dst_h / 2 - dst_w / 2)
-  const double sc = ((double)d1y - dst_h * 0.5) / ((double)s1y - (double)ccy);
-  double tx = ((double)x - (double)ccx) * sc + dst_w * 0.5;
-  double ty = ((double)y - (double)ccy) * sc + dst_h * 0.5;
-  if (truncate) {  // the reference writes the transformed point back into an INTEGER array (demo/h36m_joint_input.npy
-    tx = trunc(tx);  // is int64): truncation towards zero before astype('float32')
-    ty = trunc(ty);
-  }
-  float u = (float)tx / (float)in_w, v = (float)ty / (float)in_h;
-  // per-pose mean / std (population) per coordinate
-  float su = on ? u : 0.f, sv = on ? v : 0.f;
-  for (int o = 16; o > 0; o >>= 1) {
-    su += __shfl_xor_sync(0xffffffffu, su, o);
-    sv += __shfl_xor_sync(0xffffffffu, sv, o);
-  }
-  const float mu = su / n_joint, mv = sv / n_joint;
-  float qu = on ? (u - mu) * (u - mu) : 0.f, qv = on ? (v - mv) * (v - mv) : 0.f;
-  for (int o = 16; o > 0; o >>= 1) {
-    qu += __shfl_xor_sync(0xffffffffu, qu, o);
-    qv += __shfl_xor_sync(0xffffffffu, qv, o);
-  }
-  if (on) {
-    out[((long long)pose * n_joint + lane) * 2 + 0] = (u - mu) / sqrtf(qu / n_joint);
-    out[((long long)pose * n_joint + lane) * 2 + 1] = (v - mv) / sqrtf(qv / n_joint);
-  }
-}
-}  // namespace
-
-extern "C" {
-
-int p2m_regress_joints(const float* joint_regressor, const float* vertices, float* joints, int batch, int n_joint,
-                       int n_vertex, int chans, p2m_stream_t stream) {
-  if (!joint_regressor || !vertices || !joints || batch <= 0 || n_joint <= 0 || n_vertex <= 0 || chans <= 0 || chans > 4 ||
-      batch > 65535) {
-    set_error("regress_joints: bad argument");
-    return P2M_ERR_INVALID;
-  }
-  int dev;
-  P2M_TRY(arrays_device("regress_joints", {joint_regressor, vertices, joints}, &dev));
-  DeviceGuard guard(dev);
-  k_regress_joints<<<dim3(n_joint, batch), 256, 0, static_cast<cudaStream_t>(stream)>>>(joint_regressor, vertices,
-                                                                                       n_vertex, chans, joints);
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-
-int p2m_normalize_pose2d(const float* joints_px, float* pose2d, int batch, int n_joint, int input_h, int input_w,
-                         int truncate_like_int_input, p2m_stream_t stream) {
-  if (!joints_px || !pose2d || batch <= 0 || n_joint <= 0 || n_joint > 32 || input_h <= 0 || input_w <= 0) {
-    set_error("normalize_pose2d: bad argument (at most 32 joints)");
-    return P2M_ERR_INVALID;
-  }
-  int dev;
-  P2M_TRY(arrays_device("normalize_pose2d", {joints_px, pose2d}, &dev));
-  DeviceGuard guard(dev);
-  k_normalize_pose2d<<<(batch + 3) / 4, 128, 0, static_cast<cudaStream_t>(stream)>>>(joints_px, batch, n_joint, input_h,
-                                                                                   input_w, truncate_like_int_input, pose2d);
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-
-}  // extern "C"
-
-// =====================================================================================
-// Row f3 of SURVEY.md §8: the mesh losses of lib/core/loss.py on the GPU, forward and backward in one pass.
-//   NormalVectorLoss (:62-87)  mean over (B, 3 Nf) of |<normalize(edge_i(out)), normal(gt)>|
-//   EdgeLengthLoss   (:90-114) mean over (B, 3 Nf) of | |edge_i(out)| - |edge_i(gt)| |
-//   CoordLoss        (:10-23)  mean |pred * valid - target * valid|
-// The reference rebuilds a LongTensor of the faces on the device in EVERY call (:68, :97) and materialises ~20
-// [B, Nf, 3] temporaries; here one thread handles one (mesh, face): 18 loads, the two loss terms, and — when
-// gradients are wanted — 9 atomic adds into d(coord_out).  F.normalize semantics: v / max(|v|, 1e-12).
-// =====================================================================================
-namespace {
-struct V3 {
-  float x, y, z;
-};
-__device__ __forceinline__ V3 sub3(V3 a, V3 b) { return V3{a.x - b.x, a.y - b.y, a.z - b.z}; }
-__device__ __forceinline__ float dot3(V3 a, V3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-__device__ __forceinline__ V3 scale3(V3 a, float s) { return V3{a.x * s, a.y * s, a.z * s}; }
-__device__ __forceinline__ V3 normalize3(V3 a, float* len) {
-  const float n = sqrtf(dot3(a, a));
-  *len = n;
-  return scale3(a, 1.f / fmaxf(n, 1e-12f));
-}
-__device__ __forceinline__ V3 ld3(const float* p) { return V3{p[0], p[1], p[2]}; }
-__device__ __forceinline__ void atomic_add3(float* p, V3 g) {
-  atomicAdd(p + 0, g.x);
-  atomicAdd(p + 1, g.y);
-  atomicAdd(p + 2, g.z);
-}
-
-// sums[0] += sum of the 3 normal terms, sums[1] += sum of the 3 edge terms (fp64); grad (optional, zeroed by the
-// caller) += g_normal * d(normal sum)/d(out) + g_edge * d(edge sum)/d(out) with g_* already divided by 3 B Nf.
-__global__ void __launch_bounds__(256) k_mesh_losses(const float* __restrict__ out, const float* __restrict__ gt,
-                                                     const int* __restrict__ faces, int n_face, int n_vertex, int batch,
-                                                     const float* __restrict__ g_scale, double* __restrict__ sums,
-                                                     float* __restrict__ grad) {
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  float ln = 0.f, le = 0.f;
-  if (idx < (long long)batch * n_face) {
-    const int f = (int)(idx % n_face);
-    const long long b = idx / n_face;
-    const int i0 = faces[3 * f], i1 = faces[3 * f + 1], i2 = faces[3 * f + 2];
-    const float* ob = out + b * (long long)n_vertex * 3;
-    const float* gb = gt + b * (long long)n_vertex * 3;
-    const V3 o0 = ld3(ob + 3 * i0), o1 = ld3(ob + 3 * i1), o2 = ld3(ob + 3 * i2);
-    const V3 t0 = ld3(gb + 3 * i0), t1 = ld3(gb + 3 * i1), t2 = ld3(gb + 3 * i2);
-    // ---- normal-vector term
-    float l1, l2, l3, lg;
-    const V3 e1 = sub3(o1, o0), e2 = sub3(o2, o0), e3 = sub3(o2, o1);
-    const V3 u1 = normalize3(e1, &l1), u2 = normalize3(e2, &l2), u3 = normalize3(e3, &l3);
-    const V3 a = normalize3(sub3(t1, t0), &lg), c = normalize3(sub3(t2, t0), &lg);
-    const V3 n = normalize3(V3{a.y * c.z - a.z * c.y, a.z * c.x - a.x * c.z, a.x * c.y - a.y * c.x}, &lg);
-    const float c1 = dot3(u1, n), c2 = dot3(u2, n), c3 = dot3(u3, n);
-    ln = fabsf(c1) + fabsf(c2) + fabsf(c3);
-    // ---- edge-length term (reference edge order: (0,1), (0,2), (1,2))
-    const float d1 = l1, d2 = l2, d3 = l3;  // |o0-o1|, |o0-o2|, |o1-o2|
-    float q1, q2, q3;
-    normalize3(sub3(t0, t1), &q1);
-    normalize3(sub3(t0, t2), &q2);
-    normalize3(sub3(t1, t2), &q3);
-    const float r1 = d1 - q1, r2 = d2 - q2, r3 = d3 - q3;
-    le = fabsf(r1) + fabsf(r2) + fabsf(r3);
-    if (grad != nullptr) {
-      const float gn = g_scale[0], ge = g_scale[1];
-      float* gr = grad + b * (long long)n_vertex * 3;
-      // d|<u, n>| / de = sign(<u,n>) (n - u <u,n>) / |e|   (|e| > eps); sign(0) = 0 like torch.abs
-      auto dcos = [&](V3 u, float cs, float len) {
-        const float sg = (cs > 0.f) - (cs < 0.f);
-        const float inv = (len > 1e-12f) ? sg / len : 0.f;
-        return scale3(sub3(n, scale3(u, cs)), inv * gn);
-      };
-      // d| |e| - q | / de = sign(|e| - q) e / |e|
-      auto dlen = [&](V3 u, float r, float len) {
-        const float sg = (r > 0.f) - (r < 0.f);
-        return scale3(u, (len > 0.f) ? sg * ge : 0.f);
-      };
-      V3 g1 = dcos(u1, c1, l1), g2 = dcos(u2, c2, l2), g3 = dcos(u3, c3, l3);       // w.r.t. e1, e2, e3
-      const V3 h1 = dlen(u1, r1, l1), h2 = dlen(u2, r2, l2), h3 = dlen(u3, r3, l3);  // same edges (sign-symmetric)
-      g1 = V3{g1.x + h1.x, g1.y + h1.y, g1.z + h1.z};
-      g2 = V3{g2.x + h2.x, g2.y + h2.y, g2.z + h2.z};
-      g3 = V3{g3.x + h3.x, g3.y + h3.y, g3.z + h3.z};
-      // e1 = o1 - o0, e2 = o2 - o0, e3 = o2 - o1
-      atomic_add3(gr + 3 * i0, V3{-g1.x - g2.x, -g1.y - g2.y, -g1.z - g2.z});
-      atomic_add3(gr + 3 * i1, V3{g1.x - g3.x, g1.y - g3.y, g1.z - g3.z});
-      atomic_add3(gr + 3 * i2, V3{g2.x + g3.x, g2.y + g3.y, g2.z + g3.z});
-    }
-  }
-  __shared__ float red[2][8];
-  for (int o = 16; o > 0; o >>= 1) {
-    ln += __shfl_xor_sync(0xffffffffu, ln, o);
-    le += __shfl_xor_sync(0xffffffffu, le, o);
-  }
-  if ((threadIdx.x & 31) == 0) {
-    red[0][threadIdx.x >> 5] = ln;
-    red[1][threadIdx.x >> 5] = le;
-  }
-  __syncthreads();
-  if (threadIdx.x < 2) {
-    double s = 0.0;
-    for (int w = 0; w < 8; ++w) s += red[threadIdx.x][w];
-    atomicAdd(sums + threadIdx.x, s);
-  }
-}
-
-// CoordLoss: sums[0] += sum |p v - t v|; grad (optional) = g * sign(p v - t v) * v
-__global__ void __launch_bounds__(256) k_coord_loss(const float* __restrict__ pred, const float* __restrict__ target,
-                                                    const float* __restrict__ valid, long long n,
-                                                    const float* __restrict__ g_scale, double* __restrict__ sums,
-                                                    float* __restrict__ grad) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  float l = 0.f;
-  if (i < n) {
-    const float v = valid ? valid[i] : 1.f;
-    const float d = pred[i] * v - target[i] * v;
-    l = fabsf(d);
-    if (grad != nullptr) grad[i] = g_scale[0] * (float)((d > 0.f) - (d < 0.f)) * v;
-  }
-  __shared__ float red[8];
-  for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = l;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int w = 0; w < 8; ++w) s += red[w];
-    atomicAdd(sums, s);
-  }
-}
-}  // namespace
-
-extern "C" {
-
-int p2m_mesh_losses(const float* coord_out, const float* coord_gt, const int32_t* faces, int batch, int n_vertex,
-                    int n_face, const float* grad_scale, double* sums, float* grad_out, p2m_stream_t stream) {
-  if (!coord_out || !coord_gt || !faces || !sums || batch <= 0 || n_vertex <= 0 || n_face <= 0 ||
-      (grad_out != nullptr && grad_scale == nullptr)) {
-    set_error("mesh_losses: bad argument");
-    return P2M_ERR_INVALID;
-  }
-  int dev;
-  P2M_TRY(arrays_device("mesh_losses", {coord_out, coord_gt, faces, grad_scale, sums, grad_out}, &dev));
-  DeviceGuard guard(dev);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  P2M_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), s));
-  if (grad_out) P2M_CUDA_OK(cudaMemsetAsync(grad_out, 0, sizeof(float) * 3 * (size_t)batch * n_vertex, s));
-  const long long n = (long long)batch * n_face;
-  k_mesh_losses<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(coord_out, coord_gt, faces, n_face, n_vertex, batch, grad_scale,
-                                                            sums, grad_out);
-  P2M_LAUNCH_OK();
-  return P2M_OK;
-}
-
-int p2m_coord_loss(const float* pred, const float* target, const float* valid, int64_t n, const float* grad_scale,
-                   double* sum, float* grad_out, p2m_stream_t stream) {
-  if (!pred || !target || !sum || n <= 0 || (grad_out != nullptr && grad_scale == nullptr)) {
-    set_error("coord_loss: bad argument");
-    return P2M_ERR_INVALID;
-  }
-  int dev;
-  P2M_TRY(arrays_device("coord_loss", {pred, target, valid, grad_scale, sum, grad_out}, &dev));
-  DeviceGuard guard(dev);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  P2M_CUDA_OK(cudaMemsetAsync(sum, 0, sizeof(double), s));
-  k_coord_loss<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(pred, target, valid, n, grad_scale, sum, grad_out);
-  P2M_LAUNCH_OK();
   return P2M_OK;
 }
 

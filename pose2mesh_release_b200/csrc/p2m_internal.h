@@ -1,4 +1,4 @@
-// Internal (C++) interface between the C-ABI layer (p2m_api.cu) and the kernel translation units.
+// Internal (C++) interface between the C-ABI files (p2m_api.cu, posenet.cu, front_back.cu, ...) and the kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -388,10 +388,6 @@ int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Ep
                      int k_real = 0 /* k >= k_real is zero padding, if < K */,
                      const float* x_scale = nullptr /* X's range normalisation (launch_absmax_scale); found if null */,
                      const float* w_scale = nullptr /* W is an activation: its range normalisation, not W_SCALE */);
-// PoseNet's output stage, shared by the eval and the train forward (p2m_api.cu): dst [rows, n_col] = src[:, :n_col] (row
-// stride ld) + bias, and pose_combine [B J, 5] = cat(pose2d [B J, 2], pose3d [B J, 3] / 1000)
-int launch_take_cols(const float* src, int ld, const float* bias, int n_col, long long rows, float* dst, cudaStream_t s);
-int launch_pose_combine(const float* pose2d, const float* pose3d, long long n_joint_rows, float* out, cudaStream_t s);
 // out[ro, :] = sum over the logical rows r of physical row ro (r = ro, or 2 ro and 2 ro + 1 under the virtual unpool)
 // of  dxl[r, :] + resample^T(g_res[r, :])   (g_res may be null)
 int launch_dx_finish(const float* dxl, int rows, int F, const float* g_res, int res_Fout, const InterpTable* it,

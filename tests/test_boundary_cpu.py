@@ -123,6 +123,23 @@ def test_conv_kernel_register_split_is_balanced_in_the_build():
     assert launch == 80 and epi - launch <= launch - util and util % 8 == 0 and epi % 8 == 0
 
 
+def test_build_refuses_a_listed_source_that_does_not_exist(monkeypatch):
+    """A stale name in build.SOURCES (a renamed file) would otherwise give a library without that file's symbols, which
+    fails only when they are looked up: build() raises before any compiler runs."""
+    import subprocess
+
+    from pose2mesh_release_b200 import build
+
+    def compiler(*args, **kwargs):
+        raise AssertionError(f"a compiler ran: {args}")
+
+    monkeypatch.setattr(build, "SOURCES", build.SOURCES + ["no_such_file.cu"])
+    monkeypatch.setattr(subprocess, "Popen", compiler)
+    monkeypatch.setattr(subprocess, "run", compiler)
+    with pytest.raises(FileNotFoundError, match="no_such_file.cu"):
+        build.build(force=True)
+
+
 def test_product_never_imports_oracle():
     pkg = os.path.join(ROOT, "pose2mesh_release_b200")
     for fn in os.listdir(pkg):
