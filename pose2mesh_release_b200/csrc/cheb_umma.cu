@@ -5,10 +5,11 @@
 // k_cheb_t1        — T1 = L~ X for every row, written once to HBM (fp32): a 4-deep cp.async ring per 128-row tile,
 //                    gathers out of shared memory.
 // k_cheb_conv_umma — persistent CTAs; a tile is 128 (or 64) consecutive vertices of one mesh (a compact patch: the
-//                    reference's binary-tree vertex order makes rows [128p,128p+128) the descendants of one coarse
+// / _wide            reference's binary-tree vertex order makes rows [128p,128p+128) the descendants of one coarse
 //                    node), and a CTA computes 64 (or 128) output columns of its tiles: 128 x 64 for the 64-wide
-//                    layers, 64 x 128 for the T1-given and plain convs of the 128- and 256-wide layers, whose A
-//                    operand is then built once per 128 output columns.
+//                    layers (k_cheb_conv_umma), 64 x 128 for the T1-given and plain convs of the 128- and 256-wide
+//                    layers (k_cheb_conv_wide), whose A operand is then built once per 128 output columns.  The two
+//                    kernels share one body.
 //   * 16 producer warps build the A operand on chip, 32 features at a time: they run the second sparse product from
 //     shared memory with a tile-local CSR (the T1 rows of the tile and its 1-hop halo, staged one chunk ahead), read
 //     their own X rows straight from global memory, split every fp32 value into an fp16 (hi, lo) pair and write it
@@ -18,8 +19,9 @@
 //     through cp.async.mbarrier.arrive.noinc; thread 0 also prefetches the next tile's metadata blob.  1 thread
 //     streams the pre-packed fp16 (hi|lo) weight blocks of the CTA's column slice (cp.async.bulk, mbarrier
 //     complete_tx).
-//   * 1 warpgroup issues wgmma.mma_async (m64n64k16, f16 -> f32) on both 64-row halves of the tile (or both 64-column
-//     halves of the weight block) into register accumulators: per 16 features three MMAs — hi*Whi + lo*Whi + hi*Wlo — an error-compensated product with ~2^-21
+//   * 1 warpgroup issues wgmma.mma_async (f16 -> f32) into register accumulators: m64n64k16 on both 64-row halves of
+//     the tile, or m64n128k16 over the whole weight block in the 64 x 128 configuration (k_cheb_conv_wide, 640
+//     threads): per 16 features three MMAs — hi*Whi + lo*Whi + hi*Wlo — an error-compensated product with ~2^-21
 //     relative error, which is what keeps the 1e-4 fp32 parity bar (plain TF32/FP16 does not, SURVEY.md §7
 //     "hard parts" 1).  After the tile's last K-block the same warpgroup applies the fused epilogue — bias / folded
 //     BatchNorm, ReLU, channel-resampled residual (or, for the network's last block, the 64 -> 3 head's projection) —
@@ -289,6 +291,30 @@ __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t desc_a, ui
       : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
       : "memory");
 }
+// the same with N = 128 (64 accumulator registers): d[h][j] is element j + 32 h of the fragment, i.e. d[h] holds the
+// 64-column half h exactly as an m64n64 on that half would
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128(float (&d)[2][32], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %66, %67;\n\t}"
+      : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]),
+        "+f"(d[0][7]), "+f"(d[0][8]), "+f"(d[0][9]), "+f"(d[0][10]), "+f"(d[0][11]), "+f"(d[0][12]), "+f"(d[0][13]),
+        "+f"(d[0][14]), "+f"(d[0][15]), "+f"(d[0][16]), "+f"(d[0][17]), "+f"(d[0][18]), "+f"(d[0][19]), "+f"(d[0][20]),
+        "+f"(d[0][21]), "+f"(d[0][22]), "+f"(d[0][23]), "+f"(d[0][24]), "+f"(d[0][25]), "+f"(d[0][26]), "+f"(d[0][27]),
+        "+f"(d[0][28]), "+f"(d[0][29]), "+f"(d[0][30]), "+f"(d[0][31]), "+f"(d[1][0]), "+f"(d[1][1]), "+f"(d[1][2]),
+        "+f"(d[1][3]), "+f"(d[1][4]), "+f"(d[1][5]), "+f"(d[1][6]), "+f"(d[1][7]), "+f"(d[1][8]), "+f"(d[1][9]),
+        "+f"(d[1][10]), "+f"(d[1][11]), "+f"(d[1][12]), "+f"(d[1][13]), "+f"(d[1][14]), "+f"(d[1][15]), "+f"(d[1][16]),
+        "+f"(d[1][17]), "+f"(d[1][18]), "+f"(d[1][19]), "+f"(d[1][20]), "+f"(d[1][21]), "+f"(d[1][22]), "+f"(d[1][23]),
+        "+f"(d[1][24]), "+f"(d[1][25]), "+f"(d[1][26]), "+f"(d[1][27]), "+f"(d[1][28]), "+f"(d[1][29]), "+f"(d[1][30]),
+        "+f"(d[1][31])
+      : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
+      : "memory");
+}
 // the same with N = 32 (16 accumulator registers)
 template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t desc_a, uint64_t desc_b) {
@@ -383,33 +409,53 @@ __device__ __forceinline__ void trace_ev(const KParams& p, int role, int& n, int
 __device__ __forceinline__ void trace_ev(const KParams&, int, int&, int) {}
 #endif
 
-// Warp roles (24 warps = 6 warpgroups, one persistent CTA per SM):
+// Warp roles of the 128 x 64 configuration (N = 64, k_cheb_conv_umma: 24 warps = 6 warpgroups, one persistent CTA
+// per SM):
 //   0..15  producers: SpMM out of shared memory + fp16 (hi,lo) split + swizzled A-block stores
 //   16,17  loaders: stage the T1 (and, where the producers do not read it directly, X) rows of the next chunk; thread 0 also fetches
 //          the next tile's metadata (cp.async.bulk), thread 32 issues the TMA boxes
 //   18     weight-block loader (one thread, cp.async.bulk)
 //   19     idle
 //   20..23 MMA + epilogue warpgroup: wgmma into register accumulators -> fused epilogue -> HBM
-// The 64 x 128 configuration (N = 128) has two MMA + epilogue warpgroups that alternate tiles, so that one runs its
-// epilogue while the other issues the next tile's MMAs; the producers shrink to warps 0..7 (two tile rows per thread)
-// and warps 12..15 are parked:
-//   0..7   producers          8..11  MMA + epilogue warpgroup 1 (the CTA's odd tiles)
-//   12..15 parked             16..23 as above (20..23: MMA + epilogue warpgroup 0, the even tiles)
 constexpr int W_PROD = 16;
 constexpr int W_XLOAD = 16, N_XLOAD = 2, W_BLOAD = 18, W_EPI0 = 20;
-constexpr int W_EPI1 = 8, W_PARK = 12;  // N = 128 only
 constexpr int NUM_THREADS2 = 24 * 32;
 constexpr int REGS_LAUNCH = 80, REGS_UTIL = 40, REGS_EPI = 120;  // setmaxnreg targets per warpgroup (see the kernel)
-constexpr int REGS_PROD2 = 88, REGS_PARK = 24;                    // ... and those of the N = 128 layout
 // setmaxnreg.inc draws on the pool the CTA's own setmaxnreg.dec filled: requests beyond it would spin forever
 static_assert(128 * (REGS_EPI - REGS_LAUNCH) <= 128 * (REGS_LAUNCH - REGS_UTIL), "register pool balance");
-static_assert(2 * 128 * (REGS_PROD2 - REGS_LAUNCH) + 2 * 128 * (REGS_EPI - REGS_LAUNCH) <=
-                  128 * (REGS_LAUNCH - REGS_PARK) + 128 * (REGS_LAUNCH - REGS_UTIL),
-              "register pool balance of the N = 128 layout");
 static_assert(W_XLOAD % 4 == 0 && W_EPI0 % 4 == 0 && W_EPI0 - W_XLOAD == 4, "setmaxnreg works on aligned warpgroups");
-static_assert(W_EPI1 % 4 == 0 && W_PARK == W_EPI1 + 4 && W_XLOAD == W_PARK + 4, "setmaxnreg works on aligned warpgroups");
+// The 64 x 128 configuration (N = 128, k_cheb_conv_wide: 20 warps = 5 warpgroups) has two MMA + epilogue warpgroups
+// that alternate tiles, so that one runs its epilogue while the other issues the next tile's MMAs, and half the
+// producers (two tile rows per thread).  640 threads launch with 96 registers (65536 / 640, rounded down to a multiple
+// of 8), enough for one m64n128k16 per K step, whose 64 accumulator registers ptxas refuses below 90:
+//   0..7   producers          8..11  MMA + epilogue warpgroup 1 (the CTA's odd tiles)
+//   12..15 loaders (12, 13), weight-block loader (14), idle (15)
+//   16..19 MMA + epilogue warpgroup 0 (the even tiles)
+constexpr int W_PROD_W = 8, W_EPI1_W = 8, W_XLOAD_W = 12, W_BLOAD_W = 14, W_EPI0_W = 16;
+constexpr int NUM_THREADS_W = 20 * 32;
+constexpr int REGS_LAUNCH_W = 96, REGS_UTIL_W = 40, REGS_PROD_W = 88, REGS_EPI_W = 128;
+static_assert(2 * 128 * (REGS_EPI_W - REGS_LAUNCH_W) <=
+                  128 * (REGS_LAUNCH_W - REGS_UTIL_W) + 2 * 128 * (REGS_LAUNCH_W - REGS_PROD_W),
+              "register pool balance of the 64 x 128 layout");
+static_assert(REGS_LAUNCH_W * NUM_THREADS_W <= 65536 && (REGS_LAUNCH_W + 8) * NUM_THREADS_W > 65536,
+              "__launch_bounds__(NUM_THREADS_W, 1) gives REGS_LAUNCH_W registers per thread");
+static_assert(W_EPI1_W == W_PROD_W && W_EPI1_W % 4 == 0 && W_XLOAD_W == W_EPI1_W + 4 && W_EPI0_W == W_XLOAD_W + 4 &&
+                  (W_EPI0_W + 4) * 32 == NUM_THREADS_W,
+              "setmaxnreg works on aligned warpgroups");
+// the role map and register targets of configuration N
 template <int N>
-__host__ __device__ constexpr int prod_warps() { return N == 128 ? W_EPI1 : W_PROD; }
+struct ConvRoles {
+  static constexpr int threads = NUM_THREADS2, prod = W_PROD, xload = W_XLOAD, bload = W_BLOAD, epi0 = W_EPI0,
+                       epi1 = -1;
+  static constexpr int regs_launch = REGS_LAUNCH, regs_util = REGS_UTIL, regs_prod = REGS_LAUNCH, regs_epi = REGS_EPI;
+};
+template <>
+struct ConvRoles<128> {
+  static constexpr int threads = NUM_THREADS_W, prod = W_PROD_W, xload = W_XLOAD_W, bload = W_BLOAD_W,
+                       epi0 = W_EPI0_W, epi1 = W_EPI1_W;
+  static constexpr int regs_launch = REGS_LAUNCH_W, regs_util = REGS_UTIL_W, regs_prod = REGS_PROD_W,
+                       regs_epi = REGS_EPI_W;
+};
 
 // Two tile shapes, both a 64-register fp32 accumulator per thread of the one MMA warpgroup:
 //   N = 64:  a CTA computes 128 tile rows x the 64 output columns [64 blockIdx.y, 64 blockIdx.y + 64); used for the
@@ -421,11 +467,14 @@ __host__ __device__ constexpr int prod_warps() { return N == 128 ? W_EPI1 : W_PR
 // MODE 0: plain GEMM, no sparse product (the isolated rows of padding elision, the backward dT GEMMs, the dense GEMM).
 template <int N>
 __host__ __device__ constexpr int tile_rows() { return N == 128 ? 64 : TILE_M; }
+// The body of both conv kernels: k_cheb_conv_umma (N = 64) and k_cheb_conv_wide (N = 128) differ in their role map
+// and register targets (ConvRoles<N>) and in their launch size.
 template <int N, int NS, int XS, int MODE>
-__global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
+__device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
+  using R = ConvRoles<N>;
   constexpr int TM = tile_rows<N>();  // tile rows
-  constexpr int NPW = prod_warps<N>();  // producer warps
+  constexpr int NPW = R::prod;        // producer warps
   constexpr int NRG = NPW * 4;        // producer row groups (8 threads each)
   constexpr int RPT = TM / NRG;       // tile rows per producer thread (2: row groups rg and NRG + rg of the row order)
   constexpr int NWG = N == 128 ? 2 : 1;  // MMA + epilogue warpgroups (they alternate tiles)
@@ -512,7 +561,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
   const float a_scale = p.a_scale ? *p.a_scale : 1.f;
   const float b_inv = p.b_scale ? 1.f / *p.b_scale : W_INV_SCALE;
   const int ecol0 = (int)blockIdx.y * N;  // first output column of this CTA's column slice
-  for (int n = threadIdx.x; n < N; n += NUM_THREADS2) {
+  for (int n = threadIdx.x; n < N; n += R::threads) {
     const float sc = (p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f) / a_scale;
     const float sh = p.ep.scale ? p.ep.shift[ecol0 + n] : 0.f;
     const float bi = p.ep.bias ? p.ep.bias[ecol0 + n] : 0.f;
@@ -520,19 +569,20 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     ep_add[n] = fmaf(bi, p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f, sh);
   }
   if (N == 64 && p.head_z != nullptr)
-    for (int i = threadIdx.x; i < 64 * 12; i += NUM_THREADS2) head_w_s[i] = p.head_wt[i];
+    for (int i = threadIdx.x; i < 64 * 12; i += R::threads) head_w_s[i] = p.head_wt[i];
   __syncthreads();
 
-  // Register split by warpgroup (the kernel is launched with 80 per thread: 768 x 80 = 60 K of the SM's 64 K): the
+  // Register split by warpgroup.  N = 64 (launched with 80 per thread: 768 x 80 = 60 K of the SM's 64 K): the
   // utility warpgroup (loaders, weight loader) drops to 40 per thread and the MMA + epilogue warpgroup takes exactly
   // what that frees (120 per thread): the 64 accumulator registers plus the epilogue's addresses and residual state
-  // (at 104 ptxas spilled twice as much).  The producers stay at 80.  N = 128: the parked warpgroup drops to 24 as
-  // well, which pays for the second MMA + epilogue warpgroup (120) and for the two rows per producer thread (88).
+  // (at 104 ptxas spilled twice as much).  The producers stay at 80.  N = 128 (launched with 96: 640 x 96 = 60 K): the
+  // utility warpgroup drops to 40 and the two producer warpgroups to 88, which pays for the two MMA + epilogue
+  // warpgroups at 128.
   // (each budget is set at the top of its own region: after a join ptxas has to assume the smallest one)
-  const int mma_g = warp >= W_EPI0 ? 0 : (NWG == 2 && warp >= W_EPI1 && warp < W_PARK) ? 1 : -1;
-  if (warp >= W_XLOAD && warp < W_EPI0) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_UTIL));
-  if (warp >= W_XLOAD && warp < W_XLOAD + N_XLOAD) {
+  const int mma_g = warp >= R::epi0 ? 0 : (NWG == 2 && warp >= R::epi1 && warp < R::epi1 + 4) ? 1 : -1;
+  if (warp >= R::xload && warp < R::epi0) {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R::regs_util));
+  if (warp >= R::xload && warp < R::xload + N_XLOAD) {
     // ------------------------------------------------------------ loaders (two warps): tile metadata, own rows, halo rows
     // Per stage (tile, 32-feature chunk) they bring in what the producers read: the tile's metadata blob (thread 0,
     // cp.async.bulk, one tile ahead), the own rows of X / T1 (one 2-D TMA box each where the tile is a run of
@@ -541,7 +591,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     // A stage needs ~60 warp-level copies; issued by the 16 producer warps (round 2 until this change) every warp paid
     // the whole preamble for its one to four rows — a fifth of the producers' instruction stream per chunk.
     if (p.apack == nullptr) {
-      const int lt = tid - W_XLOAD * 32;  // 0..63
+      const int lt = tid - R::xload * 32;  // 0..63
       const int lq = lt & 7, lrg = lt >> 3;
       const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
       if (lt == 32 && p.tma) {
@@ -620,7 +670,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         }
       }
     }
-  } else if (warp == W_BLOAD) {
+  } else if (warp == R::bload) {
     // ------------------------------------------------------------ weight-block loader (one thread)
     if (lane == 0) {
       uint32_t ucnt = 0;
@@ -647,13 +697,12 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     }
   }
   } else if (mma_g >= 0) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_EPI));
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R::regs_epi));
     // ------------------------------------------------------------ MMA + epilogue warpgroup(s)
-    // wgmma into register accumulators, two 64 x 64 ones (m64n64): for N = 64 the two M = 64 row halves of the 128-row
-    // tile, for N = 128 the two 64-column halves of the 64-row tile (acc[h][j] then holds exactly what element j + 32 h
-    // of an m64n128 fragment would: the 128-column instruction itself needs more than the 80 registers ptxas allocates
-    // the kernel with).  Warp wq of the warpgroup holds rows 16 wq .. 16 wq + 15 of each row half (its ER "epilogue
-    // rows": local row lr <-> tile row 64 (lr / 16) + 16 wq + lr % 16).
+    // wgmma into register accumulators acc[2][32].  N = 64: two 64 x 64 ones (m64n64), the two M = 64 row halves of the
+    // 128-row tile.  N = 128: one m64n128 fragment over the 64-row tile, whose element j + 32 h is acc[h][j], i.e. acc[h]
+    // is the tile's 64-column half h.  Warp wq of the warpgroup holds rows 16 wq .. 16 wq + 15 of each row half (its ER
+    // "epilogue rows": local row lr <-> tile row 64 (lr / 16) + 16 wq + lr % 16).
     // A thread's fragment covers two columns of every 8-column group, so storing it directly would scatter.  N = 64: the
     // rows are transposed through a small per-warp staging buffer so that a warp-wide 16-byte access covers whole
     // 128-byte row pieces, and the fused epilogue (affine, ReLU, residual) runs in that layout, where the residual reads
@@ -664,7 +713,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     // before (b_turn; the ring's parity waits then never run more than one phase ahead), and runs its epilogue while the
     // other issues the next tile's MMAs.  The staging buffer passes from one epilogue to the next (b_stg_free).
     const int g = mma_g;
-    const int wq = warp - (g == 0 ? W_EPI0 : W_EPI1);
+    const int wq = warp - (g == 0 ? R::epi0 : R::epi1);
     const int tr = 3 + 2 * g;  // trace role of the warpgroup's warp 0
     constexpr int CPR = EC / 4;             // 16-byte chunks per staged row
     constexpr int RPI = 32 / CPR;           // rows covered by one warp-wide 16-byte access
@@ -731,19 +780,33 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
         if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 5);
         const uint32_t a0 = smem_u32(ring + s * SLOT_BYTES);
         wg_fence();
+        // A block columns: [hi 0..31 | lo 32..63], B block columns: [Whi 0..31 | Wlo 32..63] (fp16); a 16-element K
+        // step is 32 bytes = +2 in the descriptor's start-address field
+        if constexpr (N == 128) {
+          // the whole 128-row B block is one N = 128 operand (its rows 64..127 are the next eight 1024-byte atoms), so
+          // each A sub-block is read once per K step; every output element sees the same six k16 MMAs in the same
+          // order as with two m64n64 column halves
+          const uint64_t da = make_desc_sw128(a0);
+          const uint64_t db = make_desc_sw128(a0 + A_BYTES);
+          wgmma_m64n128<0, 0>(acc, da + 0, db + 0);  // hi * Whi
+          wgmma_m64n128<0, 0>(acc, da + 2, db + 2);
+          wgmma_m64n128<0, 0>(acc, da + 4, db + 0);  // lo * Whi
+          wgmma_m64n128<0, 0>(acc, da + 6, db + 2);
+          wgmma_m64n128<0, 0>(acc, da + 0, db + 4);  // hi * Wlo
+          wgmma_m64n128<0, 0>(acc, da + 2, db + 6);
+        } else {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          // A block columns: [hi 0..31 | lo 32..63], B block columns: [Whi 0..31 | Wlo 32..63] (fp16); a 16-element
-          // K step is 32 bytes = +2 in the descriptor's start-address field; rows 64..127 of either block (A: tile
-          // rows, N = 64; B: output columns, N = 128) start 8 KB further on
-          const uint64_t da = make_desc_sw128(a0 + (TM == 128 ? (uint32_t)h * (64 * 128) : 0u));
-          const uint64_t db = make_desc_sw128(a0 + A_BYTES + (TM == 64 ? (uint32_t)h * (64 * 128) : 0u));
-          wgmma_m64n64<0, 0>(acc[h], da + 0, db + 0);  // hi * Whi
-          wgmma_m64n64<0, 0>(acc[h], da + 2, db + 2);
-          wgmma_m64n64<0, 0>(acc[h], da + 4, db + 0);  // lo * Whi
-          wgmma_m64n64<0, 0>(acc[h], da + 6, db + 2);
-          wgmma_m64n64<0, 0>(acc[h], da + 0, db + 4);  // hi * Wlo
-          wgmma_m64n64<0, 0>(acc[h], da + 2, db + 6);
+          for (int h = 0; h < 2; ++h) {
+            // rows 64..127 of the A block (the tile's second M = 64 half) start 8 KB further on
+            const uint64_t da = make_desc_sw128(a0 + (uint32_t)h * (64 * 128));
+            const uint64_t db = make_desc_sw128(a0 + A_BYTES);
+            wgmma_m64n64<0, 0>(acc[h], da + 0, db + 0);  // hi * Whi
+            wgmma_m64n64<0, 0>(acc[h], da + 2, db + 2);
+            wgmma_m64n64<0, 0>(acc[h], da + 4, db + 0);  // lo * Whi
+            wgmma_m64n64<0, 0>(acc[h], da + 6, db + 2);
+            wgmma_m64n64<0, 0>(acc[h], da + 0, db + 4);  // hi * Wlo
+            wgmma_m64n64<0, 0>(acc[h], da + 2, db + 6);
+          }
         }
         wg_commit();
         wg_wait0();
@@ -934,11 +997,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
       }
     }
     if (N == 128 && lane < ER) bulk_wait0();  // the last tile's output stores read shared memory until they complete
-  } else if (warp >= NPW) {
-    // ------------------------------------------------------------ parked (N = 128): registers for the others, no work
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS_PARK));
   } else {
-    if (NPW != W_PROD) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS_PROD2));
+    if (R::regs_prod < R::regs_launch) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R::regs_prod));
     if (p.apack == nullptr) {
     // ------------------------------------------------------------ producers (16 warps; N = 128: 8)
     const int q = tid & 7;     // float4 lane inside the 32-feature chunk
@@ -1135,6 +1195,16 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid
     }
     }
   }
+}
+
+template <int N, int NS, int XS, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
+  static_assert(N == 64, "the 64 x 128 configuration is k_cheb_conv_wide");
+  cheb_conv_body<N, NS, XS, MODE>(p);
+}
+template <int NS, int XS, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS_W, 1) k_cheb_conv_wide(const __grid_constant__ KParams p) {
+  cheb_conv_body<128, NS, XS, MODE>(p);
 }
 
 // =====================================================================================
@@ -1704,18 +1774,27 @@ bool make_row_tmap(CUtensorMap* tm, const float* base, long long rows, int fin, 
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// The conv kernel's setmaxnreg split is balanced for a launch allocation of REGS_LAUNCH registers per thread: a build
-// that ends up with another count would leave the epilogue's setmaxnreg.inc spinning on an empty pool.
+// The conv kernel of configuration N: k_cheb_conv_umma (N = 64) or k_cheb_conv_wide (N = 128)
+template <int N, int NS, int XS, int MODE>
+constexpr auto conv_kernel() {
+  if constexpr (N == WIDE_N) return k_cheb_conv_wide<NS, XS, MODE>;
+  else return k_cheb_conv_umma<N, NS, XS, MODE>;
+}
+// A conv kernel's setmaxnreg split is balanced for a launch allocation of ConvRoles<N>::regs_launch registers per
+// thread (80 for k_cheb_conv_umma, 96 for k_cheb_conv_wide): a build that ends up with another count would leave the
+// epilogue's setmaxnreg.inc spinning on an empty pool.
 template <int N, int NS, int XS, int MODE>
 int check_launch_regs() {
   static int state = 0;  // per instantiation; racing first calls all compute the same value
   if (state == 0) {
     cudaFuncAttributes fa;
-    P2M_CUDA_OK(cudaFuncGetAttributes(&fa, k_cheb_conv_umma<N, NS, XS, MODE>));
-    state = (fa.numRegs == REGS_LAUNCH) ? 1 : -1;
+    P2M_CUDA_OK(cudaFuncGetAttributes(&fa, conv_kernel<N, NS, XS, MODE>()));
+    state = (fa.numRegs == ConvRoles<N>::regs_launch) ? 1 : -1;
   }
   if (state < 0) {
-    set_error("k_cheb_conv_umma was compiled with a register count other than the one its setmaxnreg split assumes");
+    set_error(N == WIDE_N
+                  ? "k_cheb_conv_wide was compiled with a register count other than the one its setmaxnreg split assumes"
+                  : "k_cheb_conv_umma was compiled with a register count other than the one its setmaxnreg split assumes");
     return P2M_ERR_CUDA;
   }
   return P2M_OK;
@@ -1728,7 +1807,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   const DevLevel& g = *a.g;
   const TileBlobs& t = conv_tiles(N, g, a.tiles);
   const size_t smem = smem_bytes_for(N, NS, XS, t, !a.plain);
-  auto kern = a.plain ? k_cheb_conv_umma<N, NS, XS, 0> : k_cheb_conv_umma<N, NS, XS, 1>;
+  auto kern = a.plain ? conv_kernel<N, NS, XS, 0>() : conv_kernel<N, NS, XS, 1>();
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   P2M_TRY((a.plain ? check_launch_regs<N, NS, XS, 0>() : check_launch_regs<N, NS, XS, 1>()));
   KParams p;
@@ -1782,7 +1861,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   }
   const int n_slices = a.fout / N;
   const dim3 grid(std::min(p.n_tiles, std::max(1, sm_count / n_slices)), n_slices);
-  kern<<<grid, NUM_THREADS2, smem, s>>>(p);
+  kern<<<grid, ConvRoles<N>::threads, smem, s>>>(p);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -2114,13 +2193,13 @@ template <int N>
 int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
   constexpr int NS = 3;
   const size_t smem = smem_bytes_for(N, NS, 1, TileBlobs(), false);
-  auto kern = k_cheb_conv_umma<N, NS, 1, 0>;
+  auto kern = conv_kernel<N, NS, 1, 0>();
   P2M_TRY((check_launch_regs<N, NS, 1, 0>()));
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   p.wslice_bytes = (long long)umma_gemm_wpack_bytes(N, p.fin);
   p.wblock_stride = (long long)N * 128;
   const dim3 grid(std::min(p.n_tiles, sm_count), n_slices);
-  kern<<<grid, NUM_THREADS2, smem, s>>>(p);
+  kern<<<grid, ConvRoles<N>::threads, smem, s>>>(p);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }

@@ -49,7 +49,7 @@ ev_all.sort()
 t0 = ev_all[0][0]
 pn = {1: "wait_x", 2: "x_ready", 6: "T2 gathered", 7: "blocks emitted", 8: "end barrier"}
 mn = {1: "tile start", 3: "turn: previous tile's main loop done", 2: "main loop done", 4: "wait full slot",
-      5: "slot full -> 12 MMAs",
+      5: "slot full -> MMAs",
       # sub-phases of the 64 x 128 (N = 128) epilogue
       20: "epi: staging block free", 21: "epi: residual in hand", 22: "epi: outputs computed",
       23: "epi: output stores issued", 24: "epi: staging block handed over"}
