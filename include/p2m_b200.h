@@ -546,6 +546,59 @@ int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float 
                      float* reg_pose3d, float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid,
                      float* joint_img, float* fitting_error, p2m_stream_t stream);
 
+/* ---- dataset inputs: synthetic detector errors and the training crop (SURVEY.md §8 row f12; lib/noise_utils.py,
+ * the datasets' generate_syn_error and replace_joint_img) --------------------------------------------------------
+ * Random-number rule.  `seed` is two int64 in DEVICE memory, read by the kernels (no host synchronisation; a captured
+ * graph replays with whatever the seed tensor holds).  Every draw is one Philox4x32-10 call with
+ *   key = (low 32 bits of seed[0], high 32 bits of seed[0]),
+ *   counter = (draw index d, stream id 16 j + purpose, sample index b, low 32 bits of seed[1])
+ * for joint j and purpose 0 jitter, 1 good, 2 inv, 3 miss around gt, 4 miss around inv, 5 miss pick, 6 choice,
+ * 7 Gaussian pair, 8 keep.  Its words (w0, w1, w2, w3) give two float64 uniforms on [0, 1),
+ * u = ((w0 >> 5) 2^26 + (w1 >> 6)) 2^-53 and the same of (w2, w3); U(a, b) = a + (b - a) u as numpy computes it;
+ * normals are Box-Muller in fp64, sqrt(-2 ln(1 - u0)) (cos, sin)(2 pi u1).  A sample's output depends only on its
+ * own inputs, its index b and the seed, not on the batch size or on other samples.  DESIGN.md §4.3 (dataset
+ * inputs) gives the draws each step takes and why the result has the reference's distribution.
+ *
+ * synthesize_pose (num_overlap = 0) on joints [batch, 17, 3] (x, y, visibility; COCO order) with area [batch] (the
+ * crop-space box area the OKS radii scale with) -> out [batch, 17, 3] float32 rows (x, y, 1), or (0, 0, 0) where
+ * every candidate is absent.  One launch, one CTA of 288 threads per sample.  Deliberate difference: where the
+ * reference's miss candidate list is empty but its inv-source part was drawn (1 to 3 inv-source survivors, none around
+ * the joint) it raises; here the miss candidate is absent. */
+typedef struct {
+  double mean[2];
+  double std[2];
+  double weight;
+} p2m_h36m_error_t;
+int p2m_synthesize_pose(const float* joints, const float* area, const int64_t* seed, int batch, float* out,
+                        p2m_stream_t stream);
+/* generate_syn_error: noise [batch, 17, 2] float32 from error_table (HOST, 17 entries in the Human3.6M joint order,
+ * copied into the kernel parameters; finite, std >= 0, 0 <= weight <= 1, else P2M_ERR_INVALID): per joint x ~ N(mean[0],
+ * std[0]), y ~ N(mean[1], std[1]) stored as float32, kept iff float32 weight > u, else (0, 0).  One launch. */
+int p2m_h36m_syn_error(const p2m_h36m_error_t* error_table, const int64_t* seed, int batch, float* noise,
+                       p2m_stream_t stream);
+/* A training sample's network input: joints_px [batch, n_joint, 2] image pixels -> pose2d [batch, n_joint, 2].  The
+ * crop box is get_bbox -> process_bbox of box_joints [batch, n_box_joint, 2] (NULL: of joints_px) and every joint goes
+ * through its rot-0 map into the (input_h, input_w) crop, as p2m_normalize_pose2d computes it; then the noise, then
+ * / input size and zero mean / unit std per pose and coordinate.  noise:
+ *   P2M_NOISE_NONE  nothing (seed may be NULL); with box_joints the test split's detections mapped through the box of
+ *                   the ground-truth joints, without it bitwise p2m_normalize_pose2d
+ *   P2M_NOISE_COCO  rows 0-16 (n_joint >= 17) through p2m_synthesize_pose's rule with every joint visible and area =
+ *                   the tight box (P2M_AREA_TIGHT) or the processed box (P2M_AREA_CROP, MuCo) mapped into the crop
+ *   P2M_NOISE_H36M  n_joint == 17: + (p2m_h36m_syn_error's noise / 256) (input_w, input_h), float32
+ * n_joint, n_box_joint <= 32.  One launch, no workspace, no host synchronisation. */
+enum {
+  P2M_NOISE_NONE = 0,
+  P2M_NOISE_COCO = 1,
+  P2M_NOISE_H36M = 2
+};
+enum {
+  P2M_AREA_TIGHT = 0,
+  P2M_AREA_CROP = 1
+};
+int p2m_training_pose2d(const float* joints_px, int batch, int n_joint, const float* box_joints, int n_box_joint,
+                        int noise, int area_box, const p2m_h36m_error_t* error_table, const int64_t* seed, int input_h,
+                        int input_w, float* pose2d, p2m_stream_t stream);
+
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),
  * entries sorted by (row, col); returns the number of clusters (or -1).  Driven by

@@ -12,6 +12,8 @@ Public surface (mirrors the reference's modules for this path, SURVEY.md §8b):
     temporal.smooth_pose / temporal.evaluate_video    <- lib/smooth_utils.py, compute_error_accel, the 3DPW video block
     freihand.FreiHANDEvaluator / freihand.f_scores    <- the FreiHAND evaluation script (F-scores, align_w_scale, PCK)
     render.render_meshes                              <- demo/renderer.py Renderer.render (batched mesh overlay)
+    targets.Human36MTargets                           <- Human36M.__getitem__'s targets (batched, on the device)
+    inputs.training_pose2d / inputs.synthesize_pose   <- the datasets' replace_joint_img, lib/noise_utils.py
 
 All device work is in libp2m_b200.so (csrc/, C ABI in include/p2m_b200.h); there is no CPU fallback.
 """
@@ -26,5 +28,6 @@ from .freihand import (FreiHANDEvaluator, align_w_scale, f_scores, mano_eval_reg
                        nearest_distances)
 from . import render  # noqa: F401
 from .render import render_meshes  # noqa: F401
+from . import inputs  # noqa: F401
 
 __version__ = "0.1.0"

@@ -143,6 +143,16 @@ P2M_CAM_INPUT_F32 = 2
 P2M_DTYPE_F32 = 0
 P2M_DTYPE_F64 = 1
 
+P2M_NOISE_NONE = 0
+P2M_NOISE_COCO = 1
+P2M_NOISE_H36M = 2
+P2M_AREA_TIGHT = 0
+P2M_AREA_CROP = 1
+
+
+class H36MError(C.Structure):
+    _fields_ = [("mean", C.c_double * 2), ("std", C.c_double * 2), ("weight", C.c_double)]
+
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
@@ -158,7 +168,8 @@ EXPORTS = [
     "p2m_body_model_create", "p2m_body_model_destroy", "p2m_body_model_workspace_bytes", "p2m_body_model_forward",
     "p2m_body_model_backward_workspace_bytes", "p2m_body_model_backward",
     "p2m_camera_frame_workspace_bytes", "p2m_camera_frame_coords", "p2m_h36m_regressors_create",
-    "p2m_h36m_regressors_destroy", "p2m_h36m_targets",
+    "p2m_h36m_regressors_destroy", "p2m_h36m_targets", "p2m_synthesize_pose", "p2m_h36m_syn_error",
+    "p2m_training_pose2d",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
 ]
 
@@ -307,6 +318,13 @@ def load() -> C.CDLL:
         lib.p2m_h36m_targets.argtypes = [vp, C.c_int, C.c_float, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp,
                                          vp, vp]
         lib.p2m_h36m_targets.restype = C.c_int
+        lib.p2m_synthesize_pose.argtypes = [vp, vp, vp, C.c_int, vp, vp]
+        lib.p2m_synthesize_pose.restype = C.c_int
+        lib.p2m_h36m_syn_error.argtypes = [C.POINTER(H36MError), vp, C.c_int, vp, vp]
+        lib.p2m_h36m_syn_error.restype = C.c_int
+        lib.p2m_training_pose2d.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.POINTER(H36MError),
+                                            vp, C.c_int, C.c_int, vp, vp]
+        lib.p2m_training_pose2d.restype = C.c_int
         lib.p2m_graph_match_level.argtypes = [i64, c_int32_p, c_int32_p, C.POINTER(C.c_double), c_int64_p,
                                               C.POINTER(C.c_double), c_int32_p]
         lib.p2m_graph_match_level.restype = i32

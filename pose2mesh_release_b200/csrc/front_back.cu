@@ -47,56 +47,9 @@ __global__ void __launch_bounds__(128) k_normalize_pose2d(const float* __restric
   const bool on = lane < n_joint;
   const float x = on ? px[((long long)pose * n_joint + lane) * 2 + 0] : 0.f;
   const float y = on ? px[((long long)pose * n_joint + lane) * 2 + 1] : 0.f;
-  float xmin = on ? x : INFINITY, xmax = on ? x : -INFINITY, ymin = on ? y : INFINITY, ymax = on ? y : -INFINITY;
-  for (int o = 16; o > 0; o >>= 1) {
-    xmin = fminf(xmin, __shfl_xor_sync(0xffffffffu, xmin, o));
-    xmax = fmaxf(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
-    ymin = fminf(ymin, __shfl_xor_sync(0xffffffffu, ymin, o));
-    ymax = fmaxf(ymax, __shfl_xor_sync(0xffffffffu, ymax, o));
-  }
-  // get_bbox (float32 arithmetic like numpy on the float32 box)
-  float bx, by, bw, bh;
-  {
-    const double xc = ((double)xmin + (double)xmax) / 2.0, w = (double)xmax - (double)xmin;
-    const double yc = ((double)ymin + (double)ymax) / 2.0, h = (double)ymax - (double)ymin;
-    bx = (float)(xc - 0.5 * w); by = (float)(yc - 0.5 * h); bw = (float)w; bh = (float)h;
-  }
-  // process_bbox: sanitise (x2 = x + (w - 1)), grow to the aspect ratio width / height, scale 1.0
-  float w = (bx + (bw - 1.f)) - bx, h = (by + (bh - 1.f)) - by;
-  const float cx = bx + w / 2.f, cy = by + h / 2.f;
-  const float aspect = (float)in_w / (float)in_h;
-  if (w > aspect * h) h = w / aspect;
-  else if (w < aspect * h) w = h * aspect;
-  const float x0 = cx - w / 2.f, y0 = cy - h / 2.f;
-  // get_center_scale + get_affine_transform(rot = 0): three float32 point pairs, solved in double
-  const float ccx = x0 + w * 0.5f, ccy = y0 + h * 0.5f;
-  const float s1y = ccy + w * -0.5f;                                     // src[1] = centre + (0, -src_w / 2)
-  const double dst_w = (double)in_w, dst_h = (double)in_h;
-  const float d1y = (float)(dst_h * 0.5) + (float)(dst_w * -0.5);        // dst[1] = (dst_w / 2, dst_h / 2 - dst_w / 2)
-  const double sc = ((double)d1y - dst_h * 0.5) / ((double)s1y - (double)ccy);
-  double tx = ((double)x - (double)ccx) * sc + dst_w * 0.5;
-  double ty = ((double)y - (double)ccy) * sc + dst_h * 0.5;
-  if (truncate) {  // the reference writes the transformed point back into an INTEGER array (demo/h36m_joint_input.npy
-    tx = trunc(tx);  // is int64): truncation towards zero before astype('float32')
-    ty = trunc(ty);
-  }
-  float u = (float)tx / (float)in_w, v = (float)ty / (float)in_h;
-  // per-pose mean / std (population) per coordinate
-  float su = on ? u : 0.f, sv = on ? v : 0.f;
-  for (int o = 16; o > 0; o >>= 1) {
-    su += __shfl_xor_sync(0xffffffffu, su, o);
-    sv += __shfl_xor_sync(0xffffffffu, sv, o);
-  }
-  const float mu = su / n_joint, mv = sv / n_joint;
-  float qu = on ? (u - mu) * (u - mu) : 0.f, qv = on ? (v - mv) * (v - mv) : 0.f;
-  for (int o = 16; o > 0; o >>= 1) {
-    qu += __shfl_xor_sync(0xffffffffu, qu, o);
-    qv += __shfl_xor_sync(0xffffffffu, qv, o);
-  }
-  if (on) {
-    out[((long long)pose * n_joint + lane) * 2 + 0] = (u - mu) / sqrtf(qu / n_joint);
-    out[((long long)pose * n_joint + lane) * 2 + 1] = (v - mv) / sqrtf(qv / n_joint);
-  }
+  const PoseCrop c = pose_crop(x, y, on, in_h, in_w);
+  const float2 t = crop_point(c, x, y, in_h, in_w, truncate);
+  normalize_crop(t.x, t.y, on, n_joint, in_h, in_w, out + (long long)pose * n_joint * 2);
 }
 }  // namespace
 

@@ -201,6 +201,98 @@ struct Epilogue {
   int level_V = 0;
 };
 #ifdef __CUDACC__
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11): PoseNet's dropout masks
+// (posenet.cu) and the training inputs' synthetic errors (inputs.cu)
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    const unsigned int hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const unsigned int hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// The crop of one pose into the (in_h, in_w) network input, one warp per pose with lane = joint (k_normalize_pose2d,
+// inputs.cu): tight box of the joints (coord_utils.py:21-39) -> aspect-preserving box (process_bbox, :42-66) -> the
+// rot-0 affine map (aug_utils.py:51-64,140-179: a uniform scaling that maps the box centre to the patch centre).
+struct PoseCrop {
+  float ccx, ccy;          // centre of the aspect-preserving box
+  double sc;               // crop pixels per image pixel
+  double tight_w, tight_h; // the tight box's xmax - xmin, ymax - ymin as replace_joint_img takes them
+  float w, h;              // the aspect-preserving box
+};
+__device__ __forceinline__ PoseCrop pose_crop(float x, float y, bool on, int in_h, int in_w) {
+  float xmin = on ? x : INFINITY, xmax = on ? x : -INFINITY, ymin = on ? y : INFINITY, ymax = on ? y : -INFINITY;
+  for (int o = 16; o > 0; o >>= 1) {
+    xmin = fminf(xmin, __shfl_xor_sync(0xffffffffu, xmin, o));
+    xmax = fmaxf(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
+    ymin = fminf(ymin, __shfl_xor_sync(0xffffffffu, ymin, o));
+    ymax = fmaxf(ymax, __shfl_xor_sync(0xffffffffu, ymax, o));
+  }
+  // get_bbox (float32 arithmetic like numpy on the float32 box)
+  float bx, by, bw, bh;
+  {
+    const double xc = ((double)xmin + (double)xmax) / 2.0, w = (double)xmax - (double)xmin;
+    const double yc = ((double)ymin + (double)ymax) / 2.0, h = (double)ymax - (double)ymin;
+    bx = (float)(xc - 0.5 * w); by = (float)(yc - 0.5 * h); bw = (float)w; bh = (float)h;
+  }
+  PoseCrop c;
+  c.tight_w = (double)(bx + bw) - (double)bx;
+  c.tight_h = (double)(by + bh) - (double)by;
+  // process_bbox: sanitise (x2 = x + (w - 1)), grow to the aspect ratio width / height, scale 1.0
+  float w = (bx + (bw - 1.f)) - bx, h = (by + (bh - 1.f)) - by;
+  const float cx = bx + w / 2.f, cy = by + h / 2.f;
+  const float aspect = (float)in_w / (float)in_h;
+  if (w > aspect * h) h = w / aspect;
+  else if (w < aspect * h) w = h * aspect;
+  const float x0 = cx - w / 2.f, y0 = cy - h / 2.f;
+  // get_center_scale + get_affine_transform(rot = 0): three float32 point pairs, solved in double
+  c.ccx = x0 + w * 0.5f;
+  c.ccy = y0 + h * 0.5f;
+  const float s1y = c.ccy + w * -0.5f;                                   // src[1] = centre + (0, -src_w / 2)
+  const double dst_w = (double)in_w, dst_h = (double)in_h;
+  const float d1y = (float)(dst_h * 0.5) + (float)(dst_w * -0.5);        // dst[1] = (dst_w / 2, dst_h / 2 - dst_w / 2)
+  c.sc = ((double)d1y - dst_h * 0.5) / ((double)s1y - (double)c.ccy);
+  c.w = w;
+  c.h = h;
+  return c;
+}
+// A point through the crop's map, in crop pixels.  truncate: the reference writes the transformed point back into an
+// INTEGER array (demo/h36m_joint_input.npy is int64): truncation towards zero before astype('float32').
+__device__ __forceinline__ float2 crop_point(const PoseCrop& c, float x, float y, int in_h, int in_w, int truncate) {
+  double tx = ((double)x - (double)c.ccx) * c.sc + (double)in_w * 0.5;
+  double ty = ((double)y - (double)c.ccy) * c.sc + (double)in_h * 0.5;
+  if (truncate) {
+    tx = trunc(tx);
+    ty = trunc(ty);
+  }
+  return make_float2((float)tx, (float)ty);
+}
+// Crop pixels -> / the input size -> per-pose mean / std (population) per coordinate, stored to out [n_joint, 2]
+__device__ __forceinline__ void normalize_crop(float cx, float cy, bool on, int n_joint, int in_h, int in_w,
+                                               float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  float u = cx / (float)in_w, v = cy / (float)in_h;
+  float su = on ? u : 0.f, sv = on ? v : 0.f;
+  for (int o = 16; o > 0; o >>= 1) {
+    su += __shfl_xor_sync(0xffffffffu, su, o);
+    sv += __shfl_xor_sync(0xffffffffu, sv, o);
+  }
+  const float mu = su / n_joint, mv = sv / n_joint;
+  float qu = on ? (u - mu) * (u - mu) : 0.f, qv = on ? (v - mv) * (v - mv) : 0.f;
+  for (int o = 16; o > 0; o >>= 1) {
+    qu += __shfl_xor_sync(0xffffffffu, qu, o);
+    qv += __shfl_xor_sync(0xffffffffu, qv, o);
+  }
+  if (on) {
+    out[lane * 2 + 0] = (u - mu) / sqrtf(qu / n_joint);
+    out[lane * 2 + 1] = (v - mv) / sqrtf(qv / n_joint);
+  }
+}
+
 // Device-side view of Epilogue + the per-element epilogue shared by the SIMT GEMM and the tensor-core conv.
 struct EpiDev {
   const float* bias;

@@ -21,7 +21,7 @@ takes one layer, so callers group samples by gender.  Deliberate differences fro
   * the layer must have center_idx None, as every layer the datasets build does.
 
 The 2-D joints come out in image pixels, before the crop and normalisation: feed them to
-postprocess.normalize_pose2d (the use_gt_input path) or add detector noise first.
+postprocess.normalize_pose2d (the use_gt_input path) or to inputs.training_pose2d (the datasets' detector noise).
 """
 from __future__ import annotations
 
