@@ -545,6 +545,38 @@ int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float 
                      const float* joint_cam, const float* f, const float* c, int batch, float* mesh, float* lift_pose3d,
                      float* reg_pose3d, float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid,
                      float* joint_img, float* fitting_error, p2m_stream_t stream);
+/* The target side of one dataset's __getitem__ for a batch (pose2mesh_net and posenet), generalising
+ * p2m_h36m_targets, which is its Human36M case without augmentation.  dataset:
+ *   P2M_DATASET_HUMAN36M  joint_cam, f, c as p2m_h36m_targets; fitting test 25 mm (the caller's fitting_thr) against
+ *                         the annotation; masks zeroed: mesh, lift (coco set only); joint_valid = lift_pose3d_valid
+ *   P2M_DATASET_COCO      joint_img = (xy / 1000) s + t with s [batch, n_s] (n_s 1 or 2) and t [batch, 2]; fitting
+ *                         test (3 px) in the 64 x 64 crop of process_bbox(get_bbox(the input set's joint_img), aspect
+ *                         1): keypoints [batch, 17, 2] and the projected regressed COCO rows 0-16, float32 distances,
+ *                         mean over keypoints_valid [batch, 17] > 0 (none: NaN, the sample stays valid); masks zeroed:
+ *                         mesh, lift, reg; joint_valid follows the test
+ *   P2M_DATASET_MUCO      joint_img = cam2pixel(joint, f, c); fitting test (45 mm) with the reference's quirk: the
+ *                         Human3.6M-ordered joints rooted at row 14 and permuted by MuCo's names against the regressor
+ *                         (DESIGN.md §4.3, sample targets); masks zeroed: mesh, lift, reg; joint_valid all ones
+ *   P2M_DATASET_AMASS     joint_img = cam2pixel(joint / 1000, f, c); no fitting test (fitting_error 0, every mask 1)
+ * For every dataset but Human36M the Human3.6M joints are the regressed ones: the mesh is rooted at their row 0 and
+ * reg_pose3d is them rooted at row 0.  mesh_cam is the camera-frame mesh (mm) of the dataset's p2m_camera_frame_coords
+ * preset.  rot [batch] degrees and flip [batch] int32 (p2m_augm_params; either NULL for none) augment lift_pose3d as
+ * j3d_processing does: x, y rotated by -rot degrees in fp64 and rounded once, then under a flip the joint set's flip
+ * pairs swapped (those of p2m_training_pose2d_augmented) and x negated; the other outputs are never augmented.
+ * joint_valid [batch, J] may be NULL.  With rot and flip NULL (or all zero), bitwise p2m_h36m_targets for Human36M.
+ * One launch, no host synchronisation. */
+enum {
+  P2M_DATASET_HUMAN36M = 0,
+  P2M_DATASET_COCO = 1,
+  P2M_DATASET_MUCO = 2,
+  P2M_DATASET_AMASS = 3
+};
+int p2m_sample_targets(const p2m_h36m_regressors_t* h, int dataset, int input_joint_set, float fitting_thr,
+                       const float* mesh_cam, const float* joint_cam, const float* f, const float* c, const float* s,
+                       int n_s, const float* t, const float* keypoints, const float* keypoints_valid, const float* rot,
+                       const int32_t* flip, int batch, float* mesh, float* lift_pose3d, float* reg_pose3d,
+                       float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid, float* joint_valid,
+                       float* joint_img, float* fitting_error, p2m_stream_t stream);
 
 /* ---- dataset inputs: synthetic detector errors and the training crop (SURVEY.md §8 row f12; lib/noise_utils.py,
  * the datasets' generate_syn_error and replace_joint_img) --------------------------------------------------------
@@ -555,9 +587,11 @@ int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float 
  * for joint j and purpose 0 jitter, 1 good, 2 inv, 3 miss around gt, 4 miss around inv, 5 miss pick, 6 choice,
  * 7 Gaussian pair, 8 keep.  Its words (w0, w1, w2, w3) give two float64 uniforms on [0, 1),
  * u = ((w0 >> 5) 2^26 + (w1 >> 6)) 2^-53 and the same of (w2, w3); U(a, b) = a + (b - a) u as numpy computes it;
- * normals are Box-Muller in fp64, sqrt(-2 ln(1 - u0)) (cos, sin)(2 pi u1).  A sample's output depends only on its
- * own inputs, its index b and the seed, not on the batch size or on other samples.  DESIGN.md §4.3 (dataset
- * inputs) gives the draws each step takes and why the result has the reference's distribution.
+ * normals are Box-Muller in fp64, sqrt(-2 ln(1 - u0)) (cos, sin)(2 pi u1).  Stream ids 2^31 + purpose are the
+ * augmentation's domain (p2m_augm_params: 0 the flip and keep uniforms, 1 the Gaussian pair), disjoint from the
+ * detector noise's 16 j + purpose, so one seed can drive both without correlating them.  A sample's output depends
+ * only on its own inputs, its index b and the seed, not on the batch size or on other samples.  DESIGN.md §4.3
+ * (dataset inputs) gives the draws each step takes and why the result has the reference's distribution.
  *
  * synthesize_pose (num_overlap = 0) on joints [batch, 17, 3] (x, y, visibility; COCO order) with area [batch] (the
  * crop-space box area the OKS radii scale with) -> out [batch, 17, 3] float32 rows (x, y, 1), or (0, 0, 0) where
@@ -598,6 +632,26 @@ enum {
 int p2m_training_pose2d(const float* joints_px, int batch, int n_joint, const float* box_joints, int n_box_joint,
                         int noise, int area_box, const p2m_h36m_error_t* error_table, const int64_t* seed, int input_h,
                         int input_w, float* pose2d, p2m_stream_t stream);
+/* A training sample's augmentation parameters (augm_params, lib/aug_utils.py:98-117) for a batch: flip_out [batch]
+ * int32 is 1 with probability 1/2 when flip is 1 (else 0); rot_out [batch] float32 degrees is
+ * clip(N(0, 1) rotate_factor, +-2 rotate_factor), then 0 with probability 1/2.  Draws from the augmentation's stream
+ * domain under the rule above; sample b's draw depends only on (seed, b).  rotate_factor finite and >= 0.  One
+ * launch, no host synchronisation. */
+int p2m_augm_params(int batch, int flip, double rotate_factor, const int64_t* seed, int32_t* flip_out, float* rot_out,
+                    p2m_stream_t stream);
+/* p2m_training_pose2d with the sample's augmentation (rot [batch] degrees, flip [batch] int32: device arrays from
+ * p2m_augm_params, either NULL for none).  rot != 0 goes into the crop's affine map as get_affine_transform builds it
+ * (get_dir in fp64, float32 point pairs, the system solved in fp64); the crop-space area of the COCO noise is
+ * unchanged (a rotation keeps the box's corner distances).  A flip is x -> input_w - x - 1 followed by swapping the
+ * flip pairs of flip_joint_set (P2M_JOINTS_COCO: n_joint >= 17, P2M_JOINTS_HUMAN36: n_joint == 17): after the noise
+ * in float32 (flip_before_noise 0: Human36M, COCO, AMASS), or in fp64 on the crop map's output before the noise
+ * (flip_before_noise 1: MuCo's j2d_processing).  With rot and flip NULL, bitwise p2m_training_pose2d, which is this
+ * call's no-augmentation case; rot = 0 and flip = 0 give the same bits.  One launch. */
+int p2m_training_pose2d_augmented(const float* joints_px, int batch, int n_joint, const float* box_joints,
+                                  int n_box_joint, int noise, int area_box, const p2m_h36m_error_t* error_table,
+                                  const int64_t* seed, int input_h, int input_w, const float* rot,
+                                  const int32_t* flip, int flip_joint_set, int flip_before_noise, float* pose2d,
+                                  p2m_stream_t stream);
 
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),

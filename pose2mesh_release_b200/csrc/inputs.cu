@@ -1,7 +1,8 @@
 // Row f12 of SURVEY.md §8: the network inputs of a training sample on the device, the train branch of the datasets'
 // replace_joint_img (data/Human36M/dataset.py:436-445) and the crop / normalisation around it (:359-392):
 //  * synthesize_pose (lib/noise_utils.py:17-285; num_overlap = 0, so no swap sources) on the COCO joints;
-//  * generate_syn_error (data/Human36M/dataset.py:143-155) on the Human3.6M joints.
+//  * generate_syn_error (data/Human36M/dataset.py:143-155) on the Human3.6M joints;
+// and row f13, the sample's augmentation: augm_params (lib/aug_utils.py:98-117) and the rotation / flip of the crop.
 // The random stream is include/p2m_b200.h's counter-based rule; DESIGN.md §4.3 (dataset inputs) argues the device's
 // shortcuts (first survivor instead of a uniform survivor, the miss pick as a two-pass mixture) are exact in
 // distribution.  Every loop is bounded by the reference's draw count.  Candidate geometry is fp64 with explicitly
@@ -268,18 +269,87 @@ __global__ void __launch_bounds__(128) k_h36m_syn_error(const ErrTable table, co
   out[t * 2 + 1] = n.y;
 }
 
+// augm_params (lib/aug_utils.py:98-117), one thread per sample: flip with probability 1/2 when enabled; rot =
+// clip(N(0, 1) rf, -2 rf, 2 rf), then 0 with probability 1/2.  Stream AUG_SID + 0 draw 0 gives the (flip, keep)
+// uniforms, AUG_SID + 1 draw 0 the Box-Muller pair.
+constexpr unsigned AUG_SID = 0x80000000u;
+__global__ void __launch_bounds__(256) k_augm_params(int batch, int do_flip, double rf,
+                                                     const long long* __restrict__ seed, int* __restrict__ flip,
+                                                     float* __restrict__ rot) {
+  const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= batch) return;
+  const Stream s = make_stream(seed, (unsigned)b);
+  const double2 u = uniforms(s, 0, AUG_SID);
+  const double2 g = uniforms(s, 0, AUG_SID + 1);
+  double sn, cs;
+  sincospi(2.0 * g.y, &sn, &cs);
+  const double z = __dmul_rn(sqrt(-2.0 * log(1.0 - g.x)), cs);
+  const double r = fmin(2.0 * rf, fmax(-2.0 * rf, __dmul_rn(z, rf)));
+  flip[b] = do_flip && u.x <= 0.5 ? 1 : 0;
+  rot[b] = u.y <= 0.5 ? 0.f : (float)r;
+}
+
+// get_affine_transform(centre, (w, h), rot, (in_w, in_h)) for rot != 0 (lib/aug_utils.py:125-185): get_dir in fp64,
+// the src / dst point pairs stored as float32 with get_3rd_point in float32, the 3-point system solved in fp64 (relative
+// to the first pair, by Cramer's rule).  A point maps to q0 + A (p - s0).
+struct RotCrop {
+  double s0x, s0y, q0x, q0y, a00, a01, a10, a11;
+};
+__device__ __forceinline__ RotCrop rot_crop(const PoseCrop& c, float rot, int in_h, int in_w) {
+  double sn, cs;
+  sincospi(__ddiv_rn((double)rot, 180.0), &sn, &cs);  // (sin, cos)(pi rot / 180), no local-memory slow path
+  const double hw = (double)(c.w * -0.5f);
+  const float s0x = c.ccx, s0y = c.ccy;
+  const float s1x = (float)__dadd_rn((double)s0x, __dsub_rn(0.0 * cs, __dmul_rn(hw, sn)));
+  const float s1y = (float)__dadd_rn((double)s0y, __dadd_rn(0.0 * sn, __dmul_rn(hw, cs)));
+  const float s2x = __fadd_rn(s1x, -__fsub_rn(s0y, s1y)), s2y = __fadd_rn(s1y, __fsub_rn(s0x, s1x));
+  const float q0x = (float)(in_w * 0.5), q0y = (float)(in_h * 0.5);
+  const float q1x = q0x, q1y = (float)(in_h * 0.5) + (float)(in_w * -0.5);
+  const float q2x = __fadd_rn(q1x, -__fsub_rn(q0y, q1y)), q2y = __fadd_rn(q1y, __fsub_rn(q0x, q1x));
+  const double e1x = (double)s1x - s0x, e1y = (double)s1y - s0y, e2x = (double)s2x - s0x, e2y = (double)s2y - s0y;
+  const double f1x = (double)q1x - q0x, f1y = (double)q1y - q0y, f2x = (double)q2x - q0x, f2y = (double)q2y - q0y;
+  const double det = __dsub_rn(__dmul_rn(e1x, e2y), __dmul_rn(e2x, e1y));
+  RotCrop m;
+  m.s0x = s0x, m.s0y = s0y, m.q0x = q0x, m.q0y = q0y;
+  m.a00 = __ddiv_rn(__dsub_rn(__dmul_rn(f1x, e2y), __dmul_rn(f2x, e1y)), det);
+  m.a01 = __ddiv_rn(__dsub_rn(__dmul_rn(f2x, e1x), __dmul_rn(f1x, e2x)), det);
+  m.a10 = __ddiv_rn(__dsub_rn(__dmul_rn(f1y, e2y), __dmul_rn(f2y, e1y)), det);
+  m.a11 = __ddiv_rn(__dsub_rn(__dmul_rn(f2y, e1x), __dmul_rn(f1y, e2x)), det);
+  return m;
+}
+__device__ __forceinline__ double2 rot_point(const RotCrop& m, float x, float y) {
+  const double dx = (double)x - m.s0x, dy = (double)y - m.s0y;
+  return make_double2(__dadd_rn(m.q0x, __dadd_rn(__dmul_rn(m.a00, dx), __dmul_rn(m.a01, dy))),
+                      __dadd_rn(m.q0y, __dadd_rn(__dmul_rn(m.a10, dx), __dmul_rn(m.a11, dy))));
+}
+// flip_2d_joint on warp 0's row (lane = joint): x -> in_w - x - 1 in float32, then the flip pairs swapped
+__device__ __forceinline__ float2 flip_row(float2 c, int joint_set, int in_w) {
+  const int p = flip_partner(joint_set, threadIdx.x & 31);
+  c.x = __fsub_rn(__fsub_rn((float)in_w, c.x), 1.f);
+  return make_float2(__shfl_sync(FULL, c.x, p), __shfl_sync(FULL, c.y, p));
+}
+
+struct Augment {
+  const float* rot;   // [B] degrees, or null
+  const int* flip;    // [B], or null
+  int joint_set;      // the flip pairs
+  int flip_before;    // MuCo: flip inside j2d_processing (fp64, before the noise); else after the noise (float32)
+};
+
 // One sample per CTA; warp 0 does the crop and the normalisation, the COCO noise takes SYNTH_THREADS threads.
 template <int NOISE>
 __global__ void __launch_bounds__(NOISE == P2M_NOISE_COCO ? SYNTH_THREADS : 32)
     k_training_pose2d(const float* __restrict__ px, int n_joint, const float* __restrict__ box, int n_box,
                       int area_box, const ErrTable table, const long long* __restrict__ seed, int in_h, int in_w,
-                      float* __restrict__ out) {
+                      const Augment aug, float* __restrict__ out) {
   __shared__ float x[32], y[32], v[N_KPS];  // crop pixels of every joint; rows 0-16 go through synthesize_sample
   __shared__ double area;
+  __shared__ int sflip;  // the COCO noise's flip after it, kept in shared memory rather than live across its calls
   const long long b = blockIdx.x;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool on = lane < n_joint;
   if (warp == 0) {
+    const int flip = aug.flip ? aug.flip[b] : 0;
     const float px_x = on ? px[(b * n_joint + lane) * 2 + 0] : 0.f, px_y = on ? px[(b * n_joint + lane) * 2 + 1] : 0.f;
     PoseCrop m;
     if (box) {
@@ -289,17 +359,24 @@ __global__ void __launch_bounds__(NOISE == P2M_NOISE_COCO ? SYNTH_THREADS : 32)
     } else {
       m = pose_crop(px_x, px_y, on, in_h, in_w);
     }
-    float2 c = crop_point(m, px_x, px_y, in_h, in_w, 0);
+    const float rot = aug.rot ? aug.rot[b] : 0.f;
+    double2 t = rot == 0.f ? crop_point_d(m, px_x, px_y, in_h, in_w) : rot_point(rot_crop(m, rot, in_h, in_w), px_x, px_y);
+    if (flip && aug.flip_before) t.x = __dsub_rn(__dsub_rn((double)in_w, t.x), 1.0);
+    float2 c = make_float2((float)t.x, (float)t.y);
+    if (flip && aug.flip_before) c = make_float2(__shfl_sync(FULL, c.x, flip_partner(aug.joint_set, lane)),
+                                                 __shfl_sync(FULL, c.y, flip_partner(aug.joint_set, lane)));
     if (NOISE == P2M_NOISE_H36M && lane < N_KPS) {  // (noise / 256) * (input_w, input_h) in float32, then added
       const float2 e = syn_error(make_stream(seed, (unsigned)b), table.e[lane], lane);
       c.x = __fadd_rn(c.x, __fmul_rn(e.x / 256.f, (float)in_w));
       c.y = __fadd_rn(c.y, __fmul_rn(e.y / 256.f, (float)in_h));
     }
+    if (NOISE != P2M_NOISE_COCO && flip && !aug.flip_before) c = flip_row(c, aug.joint_set, in_w);
     x[lane] = c.x;
     y[lane] = c.y;
     if (NOISE == P2M_NOISE_COCO) {
       if (lane < N_KPS) v[lane] = 1.f;  // the datasets' joint_img column 2 is 1 (get_coco_from_mesh)
       if (lane == 0) {
+        sflip = flip && !aug.flip_before;
         const double w = area_box == P2M_AREA_CROP ? (double)m.w : m.tight_w;
         const double h = area_box == P2M_AREA_CROP ? (double)m.h : m.tight_h;
         area = __dmul_rn(__dmul_rn(m.sc, w), __dmul_rn(m.sc, h));
@@ -312,7 +389,9 @@ __global__ void __launch_bounds__(NOISE == P2M_NOISE_COCO ? SYNTH_THREADS : 32)
   }
   if (warp == 0) {
     __syncwarp();
-    normalize_crop(x[lane], y[lane], on, n_joint, in_h, in_w, out + b * n_joint * 2);
+    float2 c = make_float2(x[lane], y[lane]);
+    if (NOISE == P2M_NOISE_COCO && sflip) c = flip_row(c, aug.joint_set, in_w);
+    normalize_crop(c.x, c.y, on, n_joint, in_h, in_w, out + b * n_joint * 2);
   }
 }
 
@@ -372,13 +451,53 @@ int p2m_h36m_syn_error(const p2m_h36m_error_t* error_table, const int64_t* seed,
   return P2M_OK;
 }
 
+int p2m_augm_params(int batch, int flip, double rotate_factor, const int64_t* seed, int32_t* flip_out, float* rot_out,
+                    p2m_stream_t stream) {
+  if (!seed || !flip_out || !rot_out || batch <= 0 || (flip != 0 && flip != 1) || !isfinite(rotate_factor) ||
+      rotate_factor < 0.0) {
+    set_error("augm_params: bad argument (seed, flip_out and rot_out required, batch > 0, flip 0 or 1, finite "
+              "rotate_factor >= 0)");
+    return P2M_ERR_INVALID;
+  }
+  int dev;
+  P2M_TRY(arrays_device("augm_params", {seed, flip_out, rot_out}, &dev));
+  DeviceGuard guard(dev);
+  k_augm_params<<<(unsigned)((batch + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      batch, flip, rotate_factor, reinterpret_cast<const long long*>(seed), flip_out, rot_out);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
 int p2m_training_pose2d(const float* joints_px, int batch, int n_joint, const float* box_joints, int n_box_joint,
                         int noise, int area_box, const p2m_h36m_error_t* error_table, const int64_t* seed, int input_h,
                         int input_w, float* pose2d, p2m_stream_t stream) {
+  return p2m_training_pose2d_augmented(joints_px, batch, n_joint, box_joints, n_box_joint, noise, area_box,
+                                       error_table, seed, input_h, input_w, nullptr, nullptr, P2M_JOINTS_COCO, 0,
+                                       pose2d, stream);
+}
+
+int p2m_training_pose2d_augmented(const float* joints_px, int batch, int n_joint, const float* box_joints,
+                                  int n_box_joint, int noise, int area_box, const p2m_h36m_error_t* error_table,
+                                  const int64_t* seed, int input_h, int input_w, const float* rot,
+                                  const int32_t* flip, int flip_joint_set, int flip_before_noise, float* pose2d,
+                                  p2m_stream_t stream) {
   if (!joints_px || !pose2d || batch <= 0 || n_joint <= 0 || n_joint > 32 || input_h <= 0 || input_w <= 0 ||
       (box_joints && (n_box_joint <= 0 || n_box_joint > 32)) ||
       (area_box != P2M_AREA_TIGHT && area_box != P2M_AREA_CROP)) {
     set_error("training_pose2d: bad argument (batch > 0, 1 .. 32 joints and box joints, positive input size)");
+    return P2M_ERR_INVALID;
+  }
+  if (flip_joint_set != P2M_JOINTS_HUMAN36 && flip_joint_set != P2M_JOINTS_COCO) {
+    set_error("training_pose2d: the flip's joint set must be P2M_JOINTS_HUMAN36 or P2M_JOINTS_COCO");
+    return P2M_ERR_INVALID;
+  }
+  if (flip && noise != P2M_NOISE_NONE && (noise == P2M_NOISE_H36M) != (flip_joint_set == P2M_JOINTS_HUMAN36)) {
+    set_error("training_pose2d: the flip's joint set must be the noise's (Human3.6M noise: P2M_JOINTS_HUMAN36, COCO "
+              "noise: P2M_JOINTS_COCO)");
+    return P2M_ERR_INVALID;
+  }
+  if (flip && (flip_joint_set == P2M_JOINTS_HUMAN36 ? n_joint != N_KPS : n_joint < N_KPS)) {
+    set_error("training_pose2d: a flip needs exactly 17 Human3.6M joints or at least the 17 COCO joints");
     return P2M_ERR_INVALID;
   }
   if (noise != P2M_NOISE_NONE && noise != P2M_NOISE_COCO && noise != P2M_NOISE_H36M) {
@@ -396,20 +515,21 @@ int p2m_training_pose2d(const float* joints_px, int batch, int n_joint, const fl
   ErrTable table = {};
   if (noise == P2M_NOISE_H36M) P2M_TRY(check_table("training_pose2d", error_table, &table));
   int dev;
-  P2M_TRY(arrays_device("training_pose2d", {joints_px, box_joints, seed, pose2d}, &dev));
+  P2M_TRY(arrays_device("training_pose2d", {joints_px, box_joints, seed, rot, flip, pose2d}, &dev));
   DeviceGuard guard(dev);
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   const long long* sd = reinterpret_cast<const long long*>(seed);
   const int nb = box_joints ? n_box_joint : 0;
+  const Augment aug{rot, flip, flip_joint_set, flip_before_noise ? 1 : 0};
   if (noise == P2M_NOISE_COCO)
     k_training_pose2d<P2M_NOISE_COCO><<<batch, SYNTH_THREADS, 0, s>>>(joints_px, n_joint, box_joints, nb, area_box,
-                                                                      table, sd, input_h, input_w, pose2d);
+                                                                      table, sd, input_h, input_w, aug, pose2d);
   else if (noise == P2M_NOISE_H36M)
     k_training_pose2d<P2M_NOISE_H36M><<<batch, 32, 0, s>>>(joints_px, n_joint, box_joints, nb, area_box, table, sd,
-                                                            input_h, input_w, pose2d);
+                                                            input_h, input_w, aug, pose2d);
   else
     k_training_pose2d<P2M_NOISE_NONE><<<batch, 32, 0, s>>>(joints_px, n_joint, box_joints, nb, area_box, table, sd,
-                                                            input_h, input_w, pose2d);
+                                                            input_h, input_w, aug, pose2d);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }

@@ -260,16 +260,29 @@ __device__ __forceinline__ PoseCrop pose_crop(float x, float y, bool on, int in_
   c.h = h;
   return c;
 }
-// A point through the crop's map, in crop pixels.  truncate: the reference writes the transformed point back into an
-// INTEGER array (demo/h36m_joint_input.npy is int64): truncation towards zero before astype('float32').
+// A point through the crop's map, in crop pixels, before rounding
+__device__ __forceinline__ double2 crop_point_d(const PoseCrop& c, float x, float y, int in_h, int in_w) {
+  return make_double2(((double)x - (double)c.ccx) * c.sc + (double)in_w * 0.5,
+                      ((double)y - (double)c.ccy) * c.sc + (double)in_h * 0.5);
+}
+// The same rounded to float32.  truncate: the reference writes the transformed point back into an INTEGER array
+// (demo/h36m_joint_input.npy is int64): truncation towards zero before astype('float32').
 __device__ __forceinline__ float2 crop_point(const PoseCrop& c, float x, float y, int in_h, int in_w, int truncate) {
-  double tx = ((double)x - (double)c.ccx) * c.sc + (double)in_w * 0.5;
-  double ty = ((double)y - (double)c.ccy) * c.sc + (double)in_h * 0.5;
+  double2 t = crop_point_d(c, x, y, in_h, in_w);
   if (truncate) {
-    tx = trunc(tx);
-    ty = trunc(ty);
+    t.x = trunc(t.x);
+    t.y = trunc(t.y);
   }
-  return make_float2((float)tx, (float)ty);
+  return make_float2((float)t.x, (float)t.y);
+}
+// The joint a horizontal flip swaps joint j with: the datasets' flip_pairs (lib/aug_utils.py flip_2d_joint /
+// flip_3d_joint), the same in Human36M, COCO, MuCo and AMASS.  COCO ((1,2),(3,4),..,(15,16)) with pelvis 17 and neck 18
+// fixed; Human3.6M ((1,4),(2,5),(3,6),(14,11),(15,12),(16,13)).
+__device__ __forceinline__ int flip_partner(int joint_set, int j) {
+  if (joint_set == P2M_JOINTS_COCO) return (j >= 1 && j <= 16) ? ((j & 1) ? j + 1 : j - 1) : j;
+  if ((j >= 1 && j <= 3) || (j >= 11 && j <= 13)) return j + 3;
+  if ((j >= 4 && j <= 6) || (j >= 14 && j <= 16)) return j - 3;
+  return j;
 }
 // Crop pixels -> / the input size -> per-pose mean / std (population) per coordinate, stored to out [n_joint, 2]
 __device__ __forceinline__ void normalize_crop(float cx, float cy, bool on, int n_joint, int in_h, int in_w,

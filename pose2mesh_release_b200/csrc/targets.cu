@@ -8,10 +8,11 @@
 //      2-4. the body model's forward (k_batch_flags, k_pose, k_lbs) with P2M_BETAS_AS_GIVEN
 //      5. k_frame_finish  per (sample, 256-vertex chunk): Human36M's translation compensation or AMASS's + t, the
 //                         m -> mm scaling, MuCo's face-keypoint vertices appended to the joints
-//  * p2m_h36m_targets         Human36M.__getitem__'s targets and meta (data/Human36M/dataset.py:344-405, pose2mesh_net and
-//                             posenet, augmentation off) from the camera-frame mesh, one launch (k_h36m_targets, one
-//                             CTA per sample): both sparse joint regressors in one pass (fp64), COCO pelvis / neck,
-//                             cam2pixel, rooting, get_fitting_error and the validity masks.
+//  * p2m_sample_targets       the targets and meta of Human36M, COCO, MuCo and AMASS __getitem__ (pose2mesh_net and
+//                             posenet) from the camera-frame mesh, one launch (k_sample_targets, one CTA per sample,
+//                             branching on the dataset): both sparse joint regressors in one pass (fp64), COCO pelvis /
+//                             neck, the dataset's projection, rooting, its fitting test and validity masks, and the lift
+//                             target's rotation and flip; p2m_h36m_targets is its unaugmented Human36M case.
 // No atomics and fixed orders: a sample's result is bitwise independent of its batch position and of the batch size;
 // nothing is read back to the host, so every call can be captured in a CUDA graph.
 #include <cuda_runtime.h>
@@ -27,12 +28,13 @@ namespace {
 
 constexpr int PREP_WARPS = 4;        // samples per k_frame_prep CTA
 constexpr int FIN_T = 256;           // threads (vertices) per k_frame_finish CTA
-constexpr int H36_T = 256;           // threads per k_h36m_targets CTA
+constexpr int H36_T = 256;           // threads per k_sample_targets CTA
 constexpr int MAX_EXTRA = 8;         // appended vertex joints (MuCo: 5 face keypoints)
 constexpr int MAX_BATCH = 1 << 24;
 constexpr int NJ = 17;               // joints of each regressor
 constexpr int NR = 2 * NJ;           // regressor rows: H36M 0..16, COCO 17..33
 constexpr int COCO_J = NJ + 2;       // + pelvis, neck (Human36M.add_pelvis_and_neck)
+constexpr int N_COCO_KPS = 17;       // COCO's annotation keypoints
 constexpr int COCO_LSH = 5, COCO_RSH = 6, COCO_LHIP = 11, COCO_RHIP = 12, COCO_PELVIS = 17;
 
 constexpr int ALL_FLAGS = P2M_FRAME_ROTATE_ROOT | P2M_FRAME_CLAMP_BETAS | P2M_FRAME_ZERO_BETAS_MODEL | P2M_FRAME_LAYER_TRANS_T |
@@ -169,49 +171,101 @@ __global__ void __launch_bounds__(FIN_T) k_frame_finish(int flags, int V, int n_
   }
 }
 
-// One CTA per sample (data/Human36M/dataset.py:301-333,344-405 with augmentation off).  Regression in fp64 over the
-// regressors' non-zero entries in ascending vertex order: rows 0..16 (H36M) on the mesh rooted at the annotation's
-// pelvis, rows 17..33 (COCO) on the camera-frame mesh; the mesh output is (mesh - root) / 1000 rounded once.
-struct H36Args {
-  int V, coco, batch;
+// One CTA per sample: the target side of the four datasets' __getitem__ (Human36M/dataset.py:301-333,344-405,
+// COCO/dataset.py:182-287, MuCo/dataset.py:232-330, AMASS/dataset.py:229-309).  Regression in fp64 over the
+// regressors' non-zero entries in ascending vertex order.  Human36M: rows 0..16 (H36M) on the mesh rooted at the
+// annotation's pelvis, the H36M joints are the annotation's; the other datasets: every row on the camera-frame mesh, the
+// H36M joints are the regressed rows 0..16 (get_joints_from_mesh).  Rows 17..33 (COCO) on the camera-frame mesh.  The
+// mesh target is (mesh - H36M joint 0) / 1000 rounded once.
+struct SampleArgs {
+  int V, coco, batch, dataset;
   double thr;
   const int* reg_ptr;      // [NR + 1]
   const int* reg_idx;      // vertex of each non-zero
   const double* reg_val;
   const float* mesh_cam;   // [B, V, 3] mm
-  const float* joint_cam;  // [B, 17, 3] mm
-  const float* f;          // [B, 2]
+  const float* joint_cam;  // [B, 17, 3] mm (Human36M)
+  const float* f;          // [B, 2] (Human36M, MuCo, AMASS)
   const float* c;          // [B, 2]
+  const float* s;          // [B, n_s] (COCO)
+  int n_s;
+  const float* t;          // [B, 2] (COCO)
+  const float* kps;        // [B, 17, 2] (COCO's annotation keypoints)
+  const float* kps_valid;  // [B, 17]
+  const float* rot;        // [B] degrees, or null (the lift target's augmentation)
+  const int* flip;         // [B], or null
   float* mesh;             // [B, V, 3] m
   float* lift;             // [B, J, 3]
   float* reg;              // [B, 17, 3]
   float* mesh_valid;       // [B, V]
   float* lift_valid;       // [B, J]
   float* reg_valid;        // [B, 17]
+  float* joint_valid;      // [B, J] posenet's mask, or null
   float* joint_img;        // [B, J, 2]
   float* fit_err;          // [B]
 };
 
-__global__ void __launch_bounds__(H36_T) k_h36m_targets(H36Args a) {
-  __shared__ double sreg[NR][3], sjc[NJ][3], sroot[3];
+// MuCo's get_fitting_error (MuCo/dataset.py:246-262) receives the Human3.6M-ordered joints where it expects MuCo's 21:
+// it roots them at row 14 (MuCo's pelvis index) and transform_joint_to_other_db moves source row MUCO_SRC[k] into
+// Human3.6M slot MUCO_DST[k] by MuCo's names; the other three slots are invalid and dropped.
+__constant__ int MUCO_DST[14] = {0, 1, 2, 3, 4, 5, 6, 10, 11, 12, 13, 14, 15, 16};
+__constant__ int MUCO_SRC[14] = {14, 8, 9, 10, 11, 12, 13, 16, 5, 6, 7, 2, 3, 4};
+constexpr int MUCO_ROOT = 14;
+constexpr int COCO_FIT_RES = 64;  // COCO.get_fitting_error's 64 x 64 crop
+
+// the input set's joint j (absolute, mm) of the sample in shared memory
+__device__ __forceinline__ double input_joint(const double (*sreg)[3], const double (*sjc)[3], int coco, int j, int q) {
+  if (!coco) return sjc[j][q];
+  if (j < NJ) return sreg[NJ + j][q];
+  const int a = j == COCO_PELVIS ? COCO_LHIP : COCO_LSH, b = j == COCO_PELVIS ? COCO_RHIP : COCO_RSH;
+  return (sreg[NJ + a][q] + sreg[NJ + b][q]) * 0.5;
+}
+// the dataset's projection of a camera-frame point p (mm) to image pixels, axis q
+__device__ __forceinline__ double project(const SampleArgs& a, long long b, const double p[3], int q) {
+  if (a.dataset == P2M_DATASET_COCO)  // (xy / 1000) s + t (COCO/dataset.py:200-210)
+    return p[q] / 1000.0 * (double)a.s[b * a.n_s + (a.n_s == 2 ? q : 0)] + (double)a.t[b * 2 + q];
+  if (a.dataset == P2M_DATASET_AMASS)  // cam2pixel(joint / 1000, f, c) (AMASS/dataset.py:229-241)
+    return (p[q] / 1000.0) / (p[2] / 1000.0) * (double)a.f[b * 2 + q] + (double)a.c[b * 2 + q];
+  return p[q] / p[2] * (double)a.f[b * 2 + q] + (double)a.c[b * 2 + q];  // cam2pixel (lib/coord_utils.py:104-109)
+}
+
+__global__ void __launch_bounds__(H36_T) k_sample_targets(SampleArgs a) {
+  __shared__ double sreg[NR][3], sjc[NJ][3], sroot[3], sfit[NJ][3];
   __shared__ float svalid;
   const long long b = blockIdx.x;
   const int tid = threadIdx.x, V = a.V;
+  const bool h36m = a.dataset == P2M_DATASET_HUMAN36M;
   const float* mc = a.mesh_cam + b * V * 3;
-  const float* jc = a.joint_cam + b * NJ * 3;
-  if (tid < 3) sroot[tid] = (double)jc[tid];
-  if (tid < 3 * NJ) sjc[tid / 3][tid % 3] = (double)jc[tid];
+  if (h36m) {
+    const float* jc = a.joint_cam + b * NJ * 3;
+    if (tid < 3) sroot[tid] = (double)jc[tid];
+    if (tid < 3 * NJ) sjc[tid / 3][tid % 3] = (double)jc[tid];
+  }
   __syncthreads();
   if (tid < 3 * NR) {
     const int r = tid / 3, q = tid % 3;
-    const double sub = r < NJ ? sroot[q] : 0.0;
+    const double sub = (h36m && r < NJ) ? sroot[q] : 0.0;
     double acc = 0.0;
     for (int e = a.reg_ptr[r]; e < a.reg_ptr[r + 1]; ++e)
       acc = fma(a.reg_val[e], (double)mc[3 * a.reg_idx[e] + q] - sub, acc);
     sreg[r][q] = acc;
   }
   __syncthreads();
-  if (tid == 0) {
+  if (!h36m) {  // the regressed H36M joints are the sample's; rooting at their row 0
+    if (tid < 3 * NJ) sjc[tid / 3][tid % 3] = sreg[tid / 3][tid % 3];
+    if (tid < 3) sroot[tid] = sreg[0][tid];
+    __syncthreads();
+  }
+  if (a.dataset == P2M_DATASET_MUCO && tid < 3 * NJ) {  // the regressor on the rooted mesh (get_fitting_error)
+    const int r = tid / 3, q = tid % 3;
+    double acc = 0.0;
+    for (int e = a.reg_ptr[r]; e < a.reg_ptr[r + 1]; ++e)
+      acc = fma(a.reg_val[e], (double)mc[3 * a.reg_idx[e] + q] - sroot[q], acc);
+    sfit[r][q] = acc;
+  }
+  __syncthreads();
+  const int J = a.coco ? COCO_J : NJ;
+  if (h36m && tid == 0) {
     // get_fitting_error: translation-aligned mean joint distance between the annotation and the regressed H36M joints
     double mj[3] = {0, 0, 0}, ms[3] = {0, 0, 0};
     for (int j = 0; j < NJ; ++j)
@@ -228,36 +282,106 @@ __global__ void __launch_bounds__(H36_T) k_h36m_targets(H36Args a) {
     err /= NJ;
     svalid = err > a.thr ? 0.f : 1.f;  // a NaN error keeps the sample, as `error > fitting_thr` does
     a.fit_err[b] = (float)err;
+  } else if (a.dataset == P2M_DATASET_MUCO && tid == 0) {
+    // the quirk above, kept: the scrambled, float32 copy of the rooted joints against the regressor on the rooted mesh
+    const auto hj = [&](int k, int q) {  // transform_joint_to_other_db's float32 array
+      return (double)(float)((sjc[MUCO_SRC[k]][q] - sroot[q]) - (sjc[MUCO_ROOT][q] - sroot[q]));
+    };
+    double mj[3] = {0, 0, 0}, ms[3] = {0, 0, 0};
+    for (int k = 0; k < 14; ++k)
+      for (int q = 0; q < 3; ++q) mj[q] += hj(k, q), ms[q] += sfit[MUCO_DST[k]][q];
+    double err = 0.0;
+    for (int k = 0; k < 14; ++k) {
+      double d2 = 0.0;
+      for (int q = 0; q < 3; ++q) {
+        const double d = hj(k, q) - (sfit[MUCO_DST[k]][q] - ms[q] / 14 + mj[q] / 14);
+        d2 += d * d;
+      }
+      err += sqrt(d2);
+    }
+    err /= 14;
+    svalid = err > a.thr ? 0.f : 1.f;
+    a.fit_err[b] = (float)err;
+  } else if (a.dataset == P2M_DATASET_COCO && tid < 32) {
+    // COCO.get_fitting_error (COCO/dataset.py:196-214): the box process_bbox(get_bbox(input-set joint_img), aspect 1),
+    // the regressed COCO rows 0-16 and the annotation keypoints through its 64 x 64 rot-0 crop, float32 distances,
+    // the mean over the annotation-visible joints (none visible: NaN, which keeps the sample)
+    const int lane = tid;
+    double p[3];
+    float ix = 0.f, iy = 0.f;
+    if (lane < J) {
+      for (int q = 0; q < 3; ++q) p[q] = input_joint(sreg, sjc, a.coco, lane, q);
+      ix = (float)project(a, b, p, 0), iy = (float)project(a, b, p, 1);
+    }
+    const PoseCrop m = pose_crop(ix, iy, lane < J, COCO_FIT_RES, COCO_FIT_RES);
+    float d = 0.f;
+    const bool vis = lane < N_COCO_KPS && a.kps_valid[b * N_COCO_KPS + lane] > 0.f;
+    if (vis) {
+      for (int q = 0; q < 3; ++q) p[q] = sreg[NJ + lane][q];
+      const float2 r = crop_point(m, (float)project(a, b, p, 0), (float)project(a, b, p, 1), COCO_FIT_RES,
+                                  COCO_FIT_RES, 0);
+      const float2 k = crop_point(m, a.kps[(b * N_COCO_KPS + lane) * 2], a.kps[(b * N_COCO_KPS + lane) * 2 + 1],
+                                  COCO_FIT_RES, COCO_FIT_RES, 0);
+      const float dx = __fsub_rn(k.x, r.x), dy = __fsub_rn(k.y, r.y);
+      d = __fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));
+    }
+    double sum = vis ? (double)d : 0.0;
+    int n = __popc(__ballot_sync(0xffffffffu, vis));
+    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if (lane == 0) {
+      const double err = sum / n;  // 0 / 0 = NaN with no visible joint
+      svalid = err > a.thr ? 0.f : 1.f;
+      a.fit_err[b] = (float)err;
+    }
+  } else if (a.dataset == P2M_DATASET_AMASS && tid == 0) {
+    svalid = 1.f;  // no fitting test
+    a.fit_err[b] = 0.f;
   }
   __syncthreads();
   const float valid = svalid;
-  const int J = a.coco ? COCO_J : NJ;
+  // masks zeroed by the test: Human36M the mesh and (coco set) the lift; COCO and MuCo the mesh, lift and reg
+  const float reg_v = (a.dataset == P2M_DATASET_COCO || a.dataset == P2M_DATASET_MUCO) ? valid : 1.f;
+  const float lift_v = (h36m && !a.coco) ? 1.f : valid;
+  // posenet's joint_valid: Human36M's coco set and COCO take the test, MuCo and AMASS are always valid
+  const float joint_v = (h36m ? a.coco : a.dataset == P2M_DATASET_COCO) ? valid : 1.f;
   if (tid < 3 * NJ) {
     const int j = tid / 3, q = tid % 3;
     a.reg[b * NJ * 3 + tid] = (float)(sjc[j][q] - sroot[q]);
-    if (q == 0) a.reg_valid[b * NJ + j] = 1.f;
+    if (q == 0) a.reg_valid[b * NJ + j] = reg_v;
   }
   if (tid < J) {
     const int j = tid;
-    double p[3];
-    if (a.coco) {
-      // the regressed COCO joints with pelvis and neck, rooted at the pelvis; projected from the camera frame
-      for (int q = 0; q < 3; ++q) {
-        const double pel = (sreg[NJ + COCO_LHIP][q] + sreg[NJ + COCO_RHIP][q]) * 0.5;
-        const double neck = (sreg[NJ + COCO_LSH][q] + sreg[NJ + COCO_RSH][q]) * 0.5;
-        p[q] = j < NJ ? sreg[NJ + j][q] : (j == COCO_PELVIS ? pel : neck);
-        a.lift[(b * J + j) * 3 + q] = (float)(p[q] - pel);
-      }
-    } else {
-      for (int q = 0; q < 3; ++q) {
-        p[q] = sjc[j][q];
-        a.lift[(b * J + j) * 3 + q] = (float)(sjc[j][q] - sroot[q]);
+    double p[3], l[3];
+    // the lift target of joint s: j, or its flip partner (j3d_processing swaps the pairs)
+    const int flip = a.flip ? a.flip[b] : 0;
+    const int s = flip ? flip_partner(a.coco ? P2M_JOINTS_COCO : P2M_JOINTS_HUMAN36, j) : j;
+    for (int q = 0; q < 3; ++q) {
+      p[q] = input_joint(sreg, sjc, a.coco, j, q);
+      if (a.coco) {
+        // the regressed COCO joints with pelvis and neck, rooted at the pelvis (fp64)
+        l[q] = input_joint(sreg, sjc, 1, s, q) - input_joint(sreg, sjc, 1, COCO_PELVIS, q);
+      } else {
+        // Human36M's joint_cam is float32 in the annotation: rooted in float32; the regressed joints in fp64
+        const double d = sjc[s][q] - sroot[q];
+        l[q] = h36m ? (double)(float)d : d;
       }
     }
-    // cam2pixel (lib/coord_utils.py:104-109)
-    a.joint_img[(b * J + j) * 2] = (float)(p[0] / p[2] * (double)a.f[b * 2] + (double)a.c[b * 2]);
-    a.joint_img[(b * J + j) * 2 + 1] = (float)(p[1] / p[2] * (double)a.f[b * 2 + 1] + (double)a.c[b * 2 + 1]);
-    a.lift_valid[b * J + j] = a.coco ? valid : 1.f;
+    // j3d_processing (lib/aug_utils.py:67-83): x, y rotated by -rot degrees in fp64, then x negated under a flip; the
+    // mesh and reg_pose3d targets are never augmented (data/Human36M/dataset.py:373, the same in every dataset)
+    const float rot = a.rot ? a.rot[b] : 0.f;
+    if (rot != 0.f) {
+      double sn, cs;
+      sincospi(__ddiv_rn(-(double)rot, 180.0), &sn, &cs);  // (sin, cos)(-pi rot / 180)
+      const double x = l[0], y = l[1];
+      l[0] = __dadd_rn(__dmul_rn(cs, x), __dmul_rn(-sn, y));
+      l[1] = __dadd_rn(__dmul_rn(sn, x), __dmul_rn(cs, y));
+    }
+    if (flip) l[0] = -l[0];
+    for (int q = 0; q < 3; ++q) a.lift[(b * J + j) * 3 + q] = (float)l[q];
+    a.joint_img[(b * J + j) * 2] = (float)project(a, b, p, 0);
+    a.joint_img[(b * J + j) * 2 + 1] = (float)project(a, b, p, 1);
+    a.lift_valid[b * J + j] = lift_v;
+    if (a.joint_valid) a.joint_valid[b * J + j] = joint_v;
   }
   for (int e = tid; e < 3 * V; e += H36_T) {
     a.mesh[b * V * 3 + e] = (float)(((double)mc[e] - sroot[e % 3]) / 1000.0);
@@ -431,25 +555,50 @@ int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float 
                      const float* joint_cam, const float* f, const float* c, int batch, float* mesh, float* lift_pose3d,
                      float* reg_pose3d, float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid,
                      float* joint_img, float* fitting_error, p2m_stream_t stream) {
+  if (!joint_cam || !f || !c) {
+    set_error("h36m_targets: joint_cam, f and c are required");
+    return P2M_ERR_INVALID;
+  }
+  return p2m_sample_targets(h, P2M_DATASET_HUMAN36M, input_joint_set, fitting_thr, mesh_cam, joint_cam, f, c, nullptr,
+                            0, nullptr, nullptr, nullptr, nullptr, nullptr, batch, mesh, lift_pose3d, reg_pose3d,
+                            mesh_valid, lift_pose3d_valid, reg_pose3d_valid, nullptr, joint_img, fitting_error,
+                            stream);
+}
+
+int p2m_sample_targets(const p2m_h36m_regressors_t* h, int dataset, int input_joint_set, float fitting_thr,
+                       const float* mesh_cam, const float* joint_cam, const float* f, const float* c, const float* s,
+                       int n_s, const float* t, const float* keypoints, const float* keypoints_valid, const float* rot,
+                       const int32_t* flip, int batch, float* mesh, float* lift_pose3d, float* reg_pose3d,
+                       float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid, float* joint_valid,
+                       float* joint_img, float* fitting_error, p2m_stream_t stream) {
   if (!h || (input_joint_set != P2M_JOINTS_HUMAN36 && input_joint_set != P2M_JOINTS_COCO) || batch <= 0 ||
-      batch > MAX_BATCH || !mesh_cam || !joint_cam || !f || !c || !mesh || !lift_pose3d || !reg_pose3d ||
-      !mesh_valid || !lift_pose3d_valid || !reg_pose3d_valid || !joint_img || !fitting_error) {
-    set_error("h36m_targets: bad argument (null handle / array, unknown joint set or batch out of [1, 2^24])");
+      batch > MAX_BATCH || !mesh_cam || !mesh || !lift_pose3d || !reg_pose3d || !mesh_valid || !lift_pose3d_valid ||
+      !reg_pose3d_valid || !joint_img || !fitting_error) {
+    set_error("sample_targets: bad argument (null handle / array, unknown joint set or batch out of [1, 2^24])");
+    return P2M_ERR_INVALID;
+  }
+  const bool need_fc = dataset == P2M_DATASET_HUMAN36M || dataset == P2M_DATASET_MUCO || dataset == P2M_DATASET_AMASS;
+  if (dataset < P2M_DATASET_HUMAN36M || dataset > P2M_DATASET_AMASS ||
+      (dataset == P2M_DATASET_HUMAN36M && !joint_cam) || (need_fc && (!f || !c)) ||
+      (dataset == P2M_DATASET_COCO && (!s || (n_s != 1 && n_s != 2) || !t || !keypoints || !keypoints_valid))) {
+    set_error("sample_targets: unknown dataset, or its inputs are missing (Human36M: joint_cam, f, c; COCO: s with "
+              "n_s 1 or 2, t, keypoints, keypoints_valid; MuCo, AMASS: f, c)");
     return P2M_ERR_INVALID;
   }
   int dev = -1;
-  P2M_TRY(arrays_device("h36m_targets", {mesh_cam, joint_cam, f, c, mesh, lift_pose3d, reg_pose3d, mesh_valid,
-                                         lift_pose3d_valid, reg_pose3d_valid, joint_img, fitting_error}, &dev));
+  P2M_TRY(arrays_device("sample_targets", {mesh_cam, joint_cam, f, c, s, t, keypoints, keypoints_valid, rot, flip,
+                                           mesh, lift_pose3d, reg_pose3d, mesh_valid, lift_pose3d_valid,
+                                           reg_pose3d_valid, joint_valid, joint_img, fitting_error}, &dev));
   if (dev != h->device) {
-    set_error("h36m_targets: the data arrays are on device " + std::to_string(dev) + ", the regressors on " +
+    set_error("sample_targets: the data arrays are on device " + std::to_string(dev) + ", the regressors on " +
               std::to_string(h->device));
     return P2M_ERR_INVALID;
   }
   DeviceGuard guard(dev);
-  H36Args a{h->V, input_joint_set == P2M_JOINTS_COCO, batch, (double)fitting_thr, h->ptr, h->idx, h->val,
-            mesh_cam, joint_cam, f, c, mesh, lift_pose3d, reg_pose3d, mesh_valid, lift_pose3d_valid, reg_pose3d_valid,
-            joint_img, fitting_error};
-  k_h36m_targets<<<(unsigned)batch, H36_T, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  SampleArgs a{h->V, input_joint_set == P2M_JOINTS_COCO, batch, dataset, (double)fitting_thr, h->ptr, h->idx, h->val,
+               mesh_cam, joint_cam, f, c, s, n_s, t, keypoints, keypoints_valid, rot, flip, mesh, lift_pose3d,
+               reg_pose3d, mesh_valid, lift_pose3d_valid, reg_pose3d_valid, joint_valid, joint_img, fitting_error};
+  k_sample_targets<<<(unsigned)batch, H36_T, 0, static_cast<cudaStream_t>(stream)>>>(a);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }

@@ -4,10 +4,13 @@
     Human36MErrorModel.generate_syn_error   data/Human36M/dataset.py:143-155, the Human3.6M joints' error model
     training_pose2d(joints_px, ...)         the train branch of the datasets' replace_joint_img with the crop and
                                             normalisation around it (data/Human36M/dataset.py:359-392,436-445); with
-                                            box_joints and noise=False, the test split's branch (:446-452)
+                                            box_joints and noise=False, the test split's branch (:446-452); with rot /
+                                            flip, the sample's rotation and flip (lib/aug_utils.py:33-64,140-195)
+    augm_params(B, flip, rotate_factor)     lib/aug_utils.py:98-117, each sample's flip and rotation
 
-All run in libp2m_b200.so (p2m_synthesize_pose, p2m_h36m_syn_error, p2m_training_pose2d), one launch per call, no
-workspace and no host synchronisation, so a call can be captured in a CUDA graph.  CUDA tensors only.
+All run in libp2m_b200.so (p2m_synthesize_pose, p2m_h36m_syn_error, p2m_training_pose2d_augmented,
+p2m_augm_params), one launch per call, no workspace and no host synchronisation, so a call can be captured in a CUDA
+graph.  CUDA tensors only.
 
 The random stream is the library's counter-based rule (include/p2m_b200.h): `seed` is an int64 [2] tensor on the
 inputs' device, read by the kernel; when it is None it is drawn from torch's generator, so torch.manual_seed
@@ -28,6 +31,7 @@ from .postprocess import INPUT_SHAPE
 
 NUM_KPS = 17
 AREA_BOXES = {"tight": _lib.P2M_AREA_TIGHT, "crop": _lib.P2M_AREA_CROP}
+JOINT_SETS = {"human36": _lib.P2M_JOINTS_HUMAN36, "coco": _lib.P2M_JOINTS_COCO}
 
 
 def _cuda(x, what: str, device=None) -> torch.Tensor:
@@ -104,19 +108,60 @@ class Human36MErrorModel:
         `device`, else the current CUDA device)."""
         if B < 1:
             raise ValueError(f"B must be positive; got {B}")
-        dev = seed.device if isinstance(seed, torch.Tensor) else torch.device(device or "cuda",
-                                                                               torch.cuda.current_device())
-        if dev.index is None:
-            dev = torch.device(dev.type, torch.cuda.current_device())
+        dev = _device(seed, device)
         s = _seed(seed, dev)
         out = torch.empty((B, NUM_KPS, 2), device=dev, dtype=torch.float32)
         _lib.call("p2m_h36m_syn_error", dev, self.table, s, B, out)
         return out
 
 
+def _device(seed, device) -> torch.device:
+    dev = seed.device if isinstance(seed, torch.Tensor) else torch.device(device or "cuda", torch.cuda.current_device())
+    if dev.index is None:
+        dev = torch.device(dev.type, torch.cuda.current_device())
+    return dev
+
+
+def augm_params(B: int, flip: bool, rotate_factor: float, seed: torch.Tensor = None, device=None):
+    """augm_params(is_train=True) for B samples under cfg.AUG.flip = flip and cfg.AUG.rotate_factor = rotate_factor:
+    -> (flip int32 [B], rot float32 [B] degrees) on seed's device (else `device`, else the current CUDA device).  flip is
+    1 with probability 1/2 when enabled; rot is clip(N(0, 1) rotate_factor, +-2 rotate_factor), then 0 with probability
+    1/2.  The draws come from the augmentation's own streams: the same seed tensor can drive training_pose2d's noise
+    without correlating the two.  Pass both results to training_pose2d and to the targets' call."""
+    if not isinstance(B, int) or B < 1:
+        raise ValueError(f"B must be a positive int; got {B!r}")
+    rf = float(rotate_factor)
+    if not math.isfinite(rf) or rf < 0:
+        raise ValueError(f"rotate_factor must be finite and >= 0; got {rotate_factor!r}")
+    dev = _device(seed, device)
+    s = _seed(seed, dev)
+    f = torch.empty(B, device=dev, dtype=torch.int32)
+    r = torch.empty(B, device=dev, dtype=torch.float32)
+    _lib.call("p2m_augm_params", dev, B, 1 if flip else 0, rf, s, f, r)
+    return f, r
+
+
+def augment_tensors(rot, flip, B: int, dev):
+    """rot [B] float and flip [B] (any integer or bool dtype) as the kernels read them; either may be None."""
+    if rot is not None:
+        _lib.cuda_tensor(rot, "rot")
+        if tuple(rot.shape) != (B,) or rot.device != dev or not rot.is_floating_point():
+            raise ValueError(f"rot must be a float [{B}] tensor on {dev}; got {rot.dtype} {tuple(rot.shape)} on "
+                             f"{rot.device}")
+        rot = rot.contiguous().float()
+    if flip is not None:
+        _lib.cuda_tensor(flip, "flip")
+        if tuple(flip.shape) != (B,) or flip.device != dev or flip.is_floating_point() or flip.is_complex():
+            raise ValueError(f"flip must be an integer [{B}] tensor on {dev}; got {flip.dtype} {tuple(flip.shape)} "
+                             f"on {flip.device}")
+        flip = (flip != 0).to(torch.int32).contiguous()
+    return rot, flip
+
+
 def training_pose2d(joints_px: torch.Tensor, input_joint_set: str, *, noise: bool = True,
                     error_model: Human36MErrorModel = None, area_box: str = "tight", box_joints: torch.Tensor = None,
-                    seed: torch.Tensor = None, input_shape=INPUT_SHAPE) -> torch.Tensor:
+                    seed: torch.Tensor = None, input_shape=INPUT_SHAPE, rot: torch.Tensor = None,
+                    flip: torch.Tensor = None, flip_before_noise: bool = False) -> torch.Tensor:
     """A training batch's pose2d: joints_px [B, J, 2] image pixels (Human36MTargets' joint_img) -> [B, J, 2].
 
     The crop box comes from box_joints [B, Jb, 2] (the ground-truth joints, for detections; default joints_px), each
@@ -125,7 +170,12 @@ def training_pose2d(joints_px: torch.Tensor, input_joint_set: str, *, noise: boo
     area_box ('tight': the joints' tight box, as Human3.6M, COCO and AMASS do; 'crop': the processed box, as MuCo
     does), and 'human36' (J = 17) adds error_model's noise scaled from 256 pixels to the crop.  Last, / input size and
     zero mean, unit std per pose.  With noise=False the result equals postprocess.normalize_pose2d(joints_px) bit for
-    bit when box_joints is None."""
+    bit when box_joints is None.
+
+    rot [B] (degrees) and flip [B] are augm_params' outputs (None: no rotation / flip, bit for bit the call without
+    them).  The rotation goes into the crop's affine map (get_affine_transform); the flip is x -> input_w - x - 1 and
+    the joint set's flip pairs swapped, after the noise as Human3.6M, COCO and AMASS do, or with
+    flip_before_noise=True before it, in float64 on the crop map's output, as MuCo's j2d_processing does."""
     if input_joint_set not in ("coco", "human36"):
         raise ValueError(f"input_joint_set must be 'coco' or 'human36'; got {input_joint_set!r}")
     if area_box not in AREA_BOXES:
@@ -154,8 +204,13 @@ def training_pose2d(joints_px: torch.Tensor, input_joint_set: str, *, noise: boo
         if bj.dim() != 3 or bj.shape[0] != B or bj.shape[2] != 2 or not 1 <= bj.shape[1] <= 32:
             raise ValueError(f"box_joints must be [{B}, Jb, 2] with Jb <= 32; got {tuple(box_joints.shape)}")
         box_joints, nb = bj, bj.shape[1]
+    rot, flip = augment_tensors(rot, flip, B, dev)
+    if flip is not None and (J != NUM_KPS if input_joint_set == "human36" else J < NUM_KPS):
+        raise ValueError(f"a flip of the {input_joint_set!r} joints needs "
+                         f"{'17' if input_joint_set == 'human36' else 'at least 17'} joints; got J = {J}")
     s = _seed(seed, dev) if mode != _lib.P2M_NOISE_NONE else None
     out = torch.empty_like(x)
-    _lib.call("p2m_training_pose2d", dev, x, B, J, box_joints, nb, mode, AREA_BOXES[area_box], table, s,
-              int(input_shape[0]), int(input_shape[1]), out)
+    _lib.call("p2m_training_pose2d_augmented", dev, x, B, J, box_joints, nb, mode, AREA_BOXES[area_box], table, s,
+              int(input_shape[0]), int(input_shape[1]), rot, flip, JOINT_SETS[input_joint_set],
+              1 if flip_before_noise else 0, out)
     return out

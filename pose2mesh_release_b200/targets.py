@@ -2,11 +2,12 @@
 
     camera_frame_coords(layer, dataset, ...)   each dataset's get_smpl_coord / get_mano_coord:
                                                data/{Human36M,AMASS,FreiHAND,MuCo,COCO,SURREAL,PW3D}/dataset.py
-    Human36MTargets                            the targets and meta of Human36M.__getitem__ (data/Human36M/dataset.py:
-                                               301-333,344-418) for pose2mesh_net and posenet, augmentation off
+    Human36MTargets, COCOTargets, MuCoTargets, AMASSTargets
+                                               the targets and meta of each dataset's __getitem__ for pose2mesh_net and
+                                               posenet, with the lift target's rotation and flip (j3d_processing)
 
-Both run in libp2m_b200.so (p2m_camera_frame_coords, p2m_h36m_targets): a prep kernel, the body model's three
-launches and a finish kernel per camera-frame call, one more launch for the Human3.6M assembly.  CUDA tensors only;
+Both run in libp2m_b200.so (p2m_camera_frame_coords, p2m_sample_targets): a prep kernel, the body model's three
+launches and a finish kernel per camera-frame call, one more launch for a dataset's assembly.  CUDA tensors only;
 nothing is read back to the host, so a call can be captured in a CUDA graph.
 
 The datasets call the body model once per sample, so its quirks apply per sample here: the betas clamp (any
@@ -33,6 +34,7 @@ import torch
 
 from . import _lib
 from .body_model import ManoLayer, SMPLLayer
+from .inputs import augment_tensors
 
 FACE_KPS_VERTEX = (331, 2802, 6262, 3489, 3990)  # lib/smpl.py:22, appended to MuCo's joints
 FITTING_THR = 25.0                               # data/Human36M/dataset.py:37, millimetres
@@ -123,43 +125,50 @@ def camera_frame_coords(layer, dataset: str, pose, betas, trans=None, R=None, t=
     return mesh, joints
 
 
-class Human36MTargets:
-    """The target side of Human36M.__getitem__ (pose2mesh_net and posenet, augmentation off) for a batch.
-
-    Built once from the SMPL layer, the H36M regressor (J_regressor_h36m_correct.npy) and the COCO regressor
-    (J_regressor_coco.npy), both [17, V], the input joint set ('human36' or 'coco') and fitting_thr (mm).  A call
-    takes the per-sample SMPL parameters pose [B, 72], betas [B, 10], trans [B, 3], the camera R [B, 3, 3], t [B, 3],
-    focal f [B, 2], principal point c [B, 2] and the annotation's absolute joint_cam [B, 17, 3] (mm), and returns a
+class _SampleTargets:
+    """The target side of one dataset's __getitem__ (pose2mesh_net and posenet) for a batch: camera_frame_coords with
+    the dataset's preset, then one assembly launch (p2m_sample_targets).  Built once from the SMPL layer, the H36M
+    regressor (J_regressor_h36m_correct.npy) and the COCO regressor (J_regressor_coco.npy), both [17, V] (the four
+    datasets use the same two files), the input joint set ('human36' or 'coco') and fitting_thr.  A call returns a
     dict of float32 device tensors shaped as the dataloader collates them (J = 17 for human36, 19 for coco):
 
-        mesh [B, V, 3]                  metres, rooted at joint_cam[:, 0]
+        mesh [B, V, 3]                  metres, rooted at the Human3.6M pelvis (the annotation's for Human36M, the
+                                        regressed one otherwise)
         lift_pose3d [B, J, 3]           coco: the regressed joints + pelvis, neck, rooted at the pelvis;
-                                        human36: joint_cam rooted at joint 0 (mm)
-        reg_pose3d [B, 17, 3]           joint_cam rooted at joint 0 (mm)
+                                        human36: the Human3.6M joints rooted at joint 0 (mm)
+        reg_pose3d [B, 17, 3]           the Human3.6M joints rooted at joint 0 (mm)
         mesh_valid [B, V, 1], lift_pose3d_valid [B, J, 1], reg_pose3d_valid [B, 17, 1]
-                                        0 where fitting_error > fitting_thr (the lift mask for coco only)
-        joint_valid [B, J, 1]           posenet's mask: lift_pose3d_valid
-        joint_img [B, J, 2]             image pixels: cam2pixel of the regressed coco joints, or of joint_cam
-        fitting_error [B]               get_fitting_error (mm)
+                                        0 where the dataset's fitting test fails, for the masks it zeroes
+        joint_valid [B, J, 1]           posenet's mask
+        joint_img [B, J, 2]             image pixels: the dataset's projection of the input set's joints
+        fitting_error [B]               the dataset's fitting error (0 where it has none)
 
-    Six launches per call: camera_frame_coords('human36m') and one assembly kernel."""
+    rot [B] (degrees) and flip [B], augm_params' outputs, augment lift_pose3d as j3d_processing does (x, y rotated by
+    -rot degrees in float64, then the flip pairs swapped and x negated); None means none, bit for bit the call without
+    them.  The other targets are never augmented (data/Human36M/dataset.py:373, the same in every dataset).
+
+    Six launches per call."""
 
     LAUNCHES = 6
+    DATASET = PRESET = None
+    FITTING_THR = None
 
     def __init__(self, layer: SMPLLayer, joint_regressor_h36m, joint_regressor_coco, input_joint_set: str = "human36",
-                 fitting_thr: float = FITTING_THR):
+                 fitting_thr: float = None):
+        name = type(self).__name__
         if not isinstance(layer, SMPLLayer):
-            raise ValueError(f"Human36MTargets takes an SMPLLayer; got {type(layer).__name__}")
+            raise ValueError(f"{name} takes an SMPLLayer; got {type(layer).__name__}")
         if input_joint_set not in JOINT_SETS:
             raise ValueError(f"input_joint_set must be one of {sorted(JOINT_SETS)}; got {input_joint_set!r}")
         V = layer.n_vertex
         host = lambda a: np.ascontiguousarray(  # noqa: E731
             (a.detach().cpu().numpy() if isinstance(a, torch.Tensor) else np.asarray(a)), dtype=np.float64)
         self.reg_h36m, self.reg_coco = host(joint_regressor_h36m), host(joint_regressor_coco)
-        for name, r in (("joint_regressor_h36m", self.reg_h36m), ("joint_regressor_coco", self.reg_coco)):
+        for rname, r in (("joint_regressor_h36m", self.reg_h36m), ("joint_regressor_coco", self.reg_coco)):
             if r.shape != (17, V):
-                raise ValueError(f"{name} must be [17, {V}]; got {tuple(r.shape)}")
-        self.layer, self.input_joint_set, self.fitting_thr = layer, input_joint_set, float(fitting_thr)
+                raise ValueError(f"{rname} must be [17, {V}]; got {tuple(r.shape)}")
+        self.layer, self.input_joint_set = layer, input_joint_set
+        self.fitting_thr = float(self.FITTING_THR if fitting_thr is None else fitting_thr)
         self.num_joints = 19 if input_joint_set == "coco" else 17
         self._handles = {}
 
@@ -184,18 +193,85 @@ class Human36MTargets:
         except Exception:
             pass
 
-    def __call__(self, pose, betas, trans, R, t, f, c, joint_cam) -> dict:
-        mesh_cam, _ = camera_frame_coords(self.layer, "human36m", pose, betas, trans, R, t)
+    def _assemble(self, mesh_cam, rot, flip, joint_cam=None, f=None, c=None, s=None, t=None, keypoints=None,
+                  keypoints_valid=None) -> dict:
         B, dev, V, J = mesh_cam.shape[0], mesh_cam.device, self.layer.n_vertex, self.num_joints
-        f, c = _cuda(f, "f", (B, 2), dev), _cuda(c, "c", (B, 2), dev)
-        joint_cam = _cuda(joint_cam, "joint_cam", (B, 17, 3), dev)
-        e = lambda *s: torch.empty(s, device=dev, dtype=torch.float32)  # noqa: E731
+        n_s = 0
+        if f is not None:
+            f, c = _cuda(f, "f", (B, 2), dev), _cuda(c, "c", (B, 2), dev)
+        if joint_cam is not None:
+            joint_cam = _cuda(joint_cam, "joint_cam", (B, 17, 3), dev)
+        if s is not None:
+            _lib.cuda_tensor(s, "s")
+            s = s.reshape(-1, 1) if s.dim() == 1 else s          # the reference's np.array(s) broadcasts [1] or [2]
+            if s.dim() != 2 or s.shape[1] not in (1, 2):
+                raise ValueError(f"s must be [{B}] or [{B}, 2]; got {tuple(s.shape)}")
+            s = _cuda(s, "s", (B, s.shape[1]), dev)
+            n_s = s.shape[1]
+            t = _cuda(t, "t", (B, 2), dev)
+            keypoints = _cuda(keypoints, "keypoints", (B, 17, 2), dev)
+            keypoints_valid = _cuda(keypoints_valid, "keypoints_valid", (B, 17), dev)
+        rot, flip = augment_tensors(rot, flip, B, dev)
+        e = lambda *sh: torch.empty(sh, device=dev, dtype=torch.float32)  # noqa: E731
         out = {"mesh": e(B, V, 3), "lift_pose3d": e(B, J, 3), "reg_pose3d": e(B, 17, 3), "mesh_valid": e(B, V, 1),
-               "lift_pose3d_valid": e(B, J, 1), "reg_pose3d_valid": e(B, 17, 1), "joint_img": e(B, J, 2),
-               "fitting_error": e(B)}
-        _lib.call("p2m_h36m_targets", dev, self.handle(dev.index), JOINT_SETS[self.input_joint_set],
-                  C.c_float(self.fitting_thr), mesh_cam, joint_cam, f, c, B, out["mesh"], out["lift_pose3d"],
-                  out["reg_pose3d"], out["mesh_valid"], out["lift_pose3d_valid"], out["reg_pose3d_valid"],
-                  out["joint_img"], out["fitting_error"])
-        out["joint_valid"] = out["lift_pose3d_valid"]
+               "lift_pose3d_valid": e(B, J, 1), "reg_pose3d_valid": e(B, 17, 1), "joint_valid": e(B, J, 1),
+               "joint_img": e(B, J, 2), "fitting_error": e(B)}
+        _lib.call("p2m_sample_targets", dev, self.handle(dev.index), self.DATASET, JOINT_SETS[self.input_joint_set],
+                  C.c_float(self.fitting_thr), mesh_cam, joint_cam, f, c, s, n_s, t, keypoints, keypoints_valid, rot,
+                  flip, B, out["mesh"], out["lift_pose3d"], out["reg_pose3d"], out["mesh_valid"],
+                  out["lift_pose3d_valid"], out["reg_pose3d_valid"], out["joint_valid"], out["joint_img"],
+                  out["fitting_error"])
         return out
+
+
+class Human36MTargets(_SampleTargets):
+    """Human36M.__getitem__'s targets (data/Human36M/dataset.py:301-333,344-418).  A call takes the SMPL parameters
+    pose [B, 72], betas [B, 10], trans [B, 3], the camera R [B, 3, 3], t [B, 3], focal f [B, 2], principal point
+    c [B, 2] and the annotation's absolute joint_cam [B, 17, 3] (mm).  Fitting test: 25 mm against the annotation;
+    zeroes the mesh mask and, for the coco set, the lift mask; joint_valid is lift_pose3d_valid."""
+
+    DATASET, FITTING_THR = _lib.P2M_DATASET_HUMAN36M, FITTING_THR
+
+    def __call__(self, pose, betas, trans, R, t, f, c, joint_cam, rot=None, flip=None) -> dict:
+        mesh_cam, _ = camera_frame_coords(self.layer, "human36m", pose, betas, trans, R, t)
+        return self._assemble(mesh_cam, rot, flip, joint_cam=joint_cam, f=f, c=c)
+
+
+class COCOTargets(_SampleTargets):
+    """COCO.__getitem__'s targets (data/COCO/dataset.py:182-287).  A call takes the SMPLify fit's pose [B, 72] and
+    betas [B, 10], its weak-perspective camera s [B] or [B, 2] and t [B, 2], and the annotation's keypoints [B, 17, 2]
+    (image pixels) with keypoints_valid [B, 17].  joint_img = (xy / 1000) s + t.  Fitting test: 3 px in a 64 x 64 crop
+    of the input set's box (aspect 1) between the keypoints and the regressed COCO joints, over the visible keypoints
+    (none visible: NaN, the sample stays valid); zeroes the mesh, lift and reg masks and posenet's joint_valid."""
+
+    DATASET, FITTING_THR = _lib.P2M_DATASET_COCO, 3.0
+
+    def __call__(self, pose, betas, s, t, keypoints, keypoints_valid, rot=None, flip=None) -> dict:
+        mesh_cam, _ = camera_frame_coords(self.layer, "coco", pose, betas)
+        return self._assemble(mesh_cam, rot, flip, s=s, t=t, keypoints=keypoints, keypoints_valid=keypoints_valid)
+
+
+class MuCoTargets(_SampleTargets):
+    """MuCo.__getitem__'s targets (data/MuCo/dataset.py:232-330).  A call takes pose [B, 72], betas [B, 10], trans
+    [B, 3], focal f [B, 2] and principal point c [B, 2].  joint_img = cam2pixel(joint, f, c).  Fitting test: 45 mm with
+    the reference's quirk kept (the Human3.6M-ordered joints handed to a function expecting MuCo's 21, so rooted at row 14
+    and permuted by MuCo's names: about 755 mm on a standing pose, INTEGRATION.md); zeroes the mesh, lift and reg masks;
+    posenet's joint_valid is all ones."""
+
+    DATASET, FITTING_THR = _lib.P2M_DATASET_MUCO, 45.0
+
+    def __call__(self, pose, betas, trans, f, c, rot=None, flip=None) -> dict:
+        mesh_cam, _ = camera_frame_coords(self.layer, "muco", pose, betas, trans)
+        return self._assemble(mesh_cam, rot, flip, f=f, c=c)
+
+
+class AMASSTargets(_SampleTargets):
+    """AMASS.__getitem__'s targets (data/AMASS/dataset.py:229-309).  A call takes pose [B, 72], betas [B, 10], the
+    camera R [B, 3, 3], t [B, 3], focal f [B, 2] and principal point c [B, 2].  joint_img = cam2pixel(joint / 1000, f,
+    c).  No fitting test: every mask is 1, fitting_error 0."""
+
+    DATASET, FITTING_THR = _lib.P2M_DATASET_AMASS, 0.0
+
+    def __call__(self, pose, betas, R, t, f, c, rot=None, flip=None) -> dict:
+        mesh_cam, _ = camera_frame_coords(self.layer, "amass", pose, betas, None, R, t)
+        return self._assemble(mesh_cam, rot, flip, f=f, c=c)
