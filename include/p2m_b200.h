@@ -539,7 +539,9 @@ void p2m_h36m_regressors_destroy(p2m_h36m_regressors_t* h);
  * Regression, projection and the error in fp64, each output rounded once.  One launch, no host synchronisation. */
 enum {
   P2M_JOINTS_HUMAN36 = 0,
-  P2M_JOINTS_COCO = 1
+  P2M_JOINTS_COCO = 1,
+  P2M_JOINTS_SMPL = 2,  /* SMPL's 24 joints (SURREAL): p2m_training_pose2d_augmented's crop and flip only */
+  P2M_JOINTS_MANO = 3   /* MANO's 21 joints (FreiHAND): p2m_training_pose2d_augmented's crop only, no flip */
 };
 int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float fitting_thr, const float* mesh_cam,
                      const float* joint_cam, const float* f, const float* c, int batch, float* mesh, float* lift_pose3d,
@@ -558,6 +560,8 @@ int p2m_h36m_targets(const p2m_h36m_regressors_t* h, int input_joint_set, float 
  *                         Human3.6M-ordered joints rooted at row 14 and permuted by MuCo's names against the regressor
  *                         (DESIGN.md §4.3, sample targets); masks zeroed: mesh, lift, reg; joint_valid all ones
  *   P2M_DATASET_AMASS     joint_img = cam2pixel(joint / 1000, f, c); no fitting test (fitting_error 0, every mask 1)
+ *   P2M_DATASET_PW3D      P2M_JOINTS_COCO only; joint_img = cam2pixel(joint, f, c); no fitting test (fitting_error 0,
+ *                         every mask 1) and no augmentation (rot and flip must be NULL)
  * For every dataset but Human36M the Human3.6M joints are the regressed ones: the mesh is rooted at their row 0 and
  * reg_pose3d is them rooted at row 0.  mesh_cam is the camera-frame mesh (mm) of the dataset's p2m_camera_frame_coords
  * preset.  rot [batch] degrees and flip [batch] int32 (p2m_augm_params; either NULL for none) augment lift_pose3d as
@@ -569,7 +573,10 @@ enum {
   P2M_DATASET_HUMAN36M = 0,
   P2M_DATASET_COCO = 1,
   P2M_DATASET_MUCO = 2,
-  P2M_DATASET_AMASS = 3
+  P2M_DATASET_AMASS = 3,
+  P2M_DATASET_PW3D = 4,
+  P2M_DATASET_SURREAL = 5,  /* p2m_layer_joint_targets only */
+  P2M_DATASET_FREIHAND = 6  /* p2m_layer_joint_targets only */
 };
 int p2m_sample_targets(const p2m_h36m_regressors_t* h, int dataset, int input_joint_set, float fitting_thr,
                        const float* mesh_cam, const float* joint_cam, const float* f, const float* c, const float* s,
@@ -577,6 +584,24 @@ int p2m_sample_targets(const p2m_h36m_regressors_t* h, int dataset, int input_jo
                        const int32_t* flip, int batch, float* mesh, float* lift_pose3d, float* reg_pose3d,
                        float* mesh_valid, float* lift_pose3d_valid, float* reg_pose3d_valid, float* joint_valid,
                        float* joint_img, float* fitting_error, p2m_stream_t stream);
+/* The targets and meta of the datasets that take the body model's own joints as both the lift and the regression
+ * target, with no joint regressor: mesh_cam [batch, n_vertex, 3] and joint_cam [batch, n_joint, 3] (the layer's
+ * joints) are p2m_camera_frame_coords' outputs for the dataset's preset (mm).  Root: joint 0.  dataset:
+ *   P2M_DATASET_SURREAL   n_joint 24 (SMPL).  joint_img [batch, 24, 2] = cam2pixel(joint_cam, f, c) of the absolute
+ *                         joints in fp64, rounded once (f, c [batch, 2]).  lift_pose3d = j3d_processing(joint_cam -
+ *                         root): the float32 rooting, x, y rotated by -rot degrees in fp64 and rounded once, then under
+ *                         a flip SMPL's flip pairs swapped and x negated (rot [batch] degrees, flip [batch] int32, either
+ *                         NULL for none).  reg_pose3d is the same augmented array, as in the reference.
+ *   P2M_DATASET_FREIHAND  n_joint 21 (MANO).  lift_pose3d = reg_pose3d = joint_cam - root in float32.  f, c, rot,
+ *                         flip and joint_img must be NULL: no projection, no augmentation.
+ * Both: mesh [batch, n_vertex, 3] = (mesh_cam - root) / 1000 in float32 (metres); every mask (mesh_valid [batch,
+ * n_vertex], lift_pose3d_valid, reg_pose3d_valid, joint_valid [batch, n_joint], the last nullable) is 1 and
+ * fitting_error [batch] is 0.  One launch, no host synchronisation. */
+int p2m_layer_joint_targets(int dataset, const float* mesh_cam, const float* joint_cam, int n_vertex, int n_joint,
+                            const float* f, const float* c, const float* rot, const int32_t* flip, int batch,
+                            float* mesh, float* lift_pose3d, float* reg_pose3d, float* mesh_valid,
+                            float* lift_pose3d_valid, float* reg_pose3d_valid, float* joint_valid, float* joint_img,
+                            float* fitting_error, p2m_stream_t stream);
 
 /* ---- dataset inputs: synthetic detector errors and the training crop (SURVEY.md §8 row f12; lib/noise_utils.py,
  * the datasets' generate_syn_error and replace_joint_img) --------------------------------------------------------
@@ -646,7 +671,11 @@ int p2m_augm_params(int batch, int flip, double rotate_factor, const int64_t* se
  * flip pairs of flip_joint_set (P2M_JOINTS_COCO: n_joint >= 17, P2M_JOINTS_HUMAN36: n_joint == 17): after the noise
  * in float32 (flip_before_noise 0: Human36M, COCO, AMASS), or in fp64 on the crop map's output before the noise
  * (flip_before_noise 1: MuCo's j2d_processing).  With rot and flip NULL, bitwise p2m_training_pose2d, which is this
- * call's no-augmentation case; rot = 0 and flip = 0 give the same bits.  One launch. */
+ * call's no-augmentation case; rot = 0 and flip = 0 give the same bits.  flip_joint_set P2M_JOINTS_SMPL (n_joint ==
+ * 24, SURREAL) and P2M_JOINTS_MANO (n_joint == 21, FreiHAND) take no noise; MANO has no flip pairs, so flip must be
+ * NULL.  SURREAL's j2d_processing flips in the joints' own dtype: float32 detections flip after the float32 crop
+ * (flip_before_noise 0), float64 ground-truth joints flip in fp64 before it is rounded (flip_before_noise 1).  One
+ * launch. */
 int p2m_training_pose2d_augmented(const float* joints_px, int batch, int n_joint, const float* box_joints,
                                   int n_box_joint, int noise, int area_box, const p2m_h36m_error_t* error_table,
                                   const int64_t* seed, int input_h, int input_w, const float* rot,

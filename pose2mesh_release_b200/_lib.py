@@ -135,10 +135,15 @@ P2M_FRAME_TO_MM = 128
 
 P2M_JOINTS_HUMAN36 = 0
 P2M_JOINTS_COCO = 1
+P2M_JOINTS_SMPL = 2
+P2M_JOINTS_MANO = 3
 P2M_DATASET_HUMAN36M = 0
 P2M_DATASET_COCO = 1
 P2M_DATASET_MUCO = 2
 P2M_DATASET_AMASS = 3
+P2M_DATASET_PW3D = 4
+P2M_DATASET_SURREAL = 5
+P2M_DATASET_FREIHAND = 6
 
 P2M_CAM_INPUT_F64 = 0
 P2M_CAM_INPUT_INT = 1
@@ -174,6 +179,7 @@ EXPORTS = [
     "p2m_camera_frame_workspace_bytes", "p2m_camera_frame_coords", "p2m_h36m_regressors_create",
     "p2m_h36m_regressors_destroy", "p2m_h36m_targets", "p2m_synthesize_pose", "p2m_h36m_syn_error",
     "p2m_training_pose2d", "p2m_augm_params", "p2m_training_pose2d_augmented", "p2m_sample_targets",
+    "p2m_layer_joint_targets",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
 ]
 
@@ -338,6 +344,9 @@ def load() -> C.CDLL:
         lib.p2m_sample_targets.argtypes = [vp, C.c_int, C.c_int, C.c_float, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp,
                                            vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
         lib.p2m_sample_targets.restype = C.c_int
+        lib.p2m_layer_joint_targets.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp,
+                                                vp, vp, vp, vp, vp, vp, vp, vp]
+        lib.p2m_layer_joint_targets.restype = C.c_int
         lib.p2m_graph_match_level.argtypes = [i64, c_int32_p, c_int32_p, C.POINTER(C.c_double), c_int64_p,
                                               C.POINTER(C.c_double), c_int32_p]
         lib.p2m_graph_match_level.restype = i32

@@ -487,16 +487,28 @@ int p2m_training_pose2d_augmented(const float* joints_px, int batch, int n_joint
     set_error("training_pose2d: bad argument (batch > 0, 1 .. 32 joints and box joints, positive input size)");
     return P2M_ERR_INVALID;
   }
-  if (flip_joint_set != P2M_JOINTS_HUMAN36 && flip_joint_set != P2M_JOINTS_COCO) {
-    set_error("training_pose2d: the flip's joint set must be P2M_JOINTS_HUMAN36 or P2M_JOINTS_COCO");
+  if (flip_joint_set != P2M_JOINTS_HUMAN36 && flip_joint_set != P2M_JOINTS_COCO && flip_joint_set != P2M_JOINTS_SMPL &&
+      flip_joint_set != P2M_JOINTS_MANO) {
+    set_error("training_pose2d: the flip's joint set must be P2M_JOINTS_HUMAN36, P2M_JOINTS_COCO, P2M_JOINTS_SMPL or "
+              "P2M_JOINTS_MANO");
     return P2M_ERR_INVALID;
+  }
+  // SURREAL's and FreiHAND's inputs are the joints themselves: no detector noise exists for these sets
+  if (flip_joint_set == P2M_JOINTS_SMPL || flip_joint_set == P2M_JOINTS_MANO) {
+    const bool smpl = flip_joint_set == P2M_JOINTS_SMPL;
+    if (noise != P2M_NOISE_NONE || n_joint != (smpl ? 24 : 21) || (!smpl && flip)) {
+      set_error("training_pose2d: P2M_JOINTS_SMPL takes 24 joints, P2M_JOINTS_MANO 21 joints and no flip, both without "
+                "noise");
+      return P2M_ERR_INVALID;
+    }
   }
   if (flip && noise != P2M_NOISE_NONE && (noise == P2M_NOISE_H36M) != (flip_joint_set == P2M_JOINTS_HUMAN36)) {
     set_error("training_pose2d: the flip's joint set must be the noise's (Human3.6M noise: P2M_JOINTS_HUMAN36, COCO "
               "noise: P2M_JOINTS_COCO)");
     return P2M_ERR_INVALID;
   }
-  if (flip && (flip_joint_set == P2M_JOINTS_HUMAN36 ? n_joint != N_KPS : n_joint < N_KPS)) {
+  if (flip && (flip_joint_set == P2M_JOINTS_HUMAN36 ? n_joint != N_KPS
+                                                    : flip_joint_set == P2M_JOINTS_COCO && n_joint < N_KPS)) {
     set_error("training_pose2d: a flip needs exactly 17 Human3.6M joints or at least the 17 COCO joints");
     return P2M_ERR_INVALID;
   }

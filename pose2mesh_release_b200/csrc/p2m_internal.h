@@ -277,9 +277,15 @@ __device__ __forceinline__ float2 crop_point(const PoseCrop& c, float x, float y
 }
 // The joint a horizontal flip swaps joint j with: the datasets' flip_pairs (lib/aug_utils.py flip_2d_joint /
 // flip_3d_joint), the same in Human36M, COCO, MuCo and AMASS.  COCO ((1,2),(3,4),..,(15,16)) with pelvis 17 and neck 18
-// fixed; Human3.6M ((1,4),(2,5),(3,6),(14,11),(15,12),(16,13)).
+// fixed; Human3.6M ((1,4),(2,5),(3,6),(14,11),(15,12),(16,13)); SURREAL's SMPL ((1,2),(4,5),(7,8),(10,11),(13,14),
+// (16,17),(18,19),(20,21),(22,23)); MANO has none.
 __device__ __forceinline__ int flip_partner(int joint_set, int j) {
   if (joint_set == P2M_JOINTS_COCO) return (j >= 1 && j <= 16) ? ((j & 1) ? j + 1 : j - 1) : j;
+  if (joint_set == P2M_JOINTS_MANO || j <= 0 || j >= 24) return j;
+  if (joint_set == P2M_JOINTS_SMPL) {
+    if (j >= 18) return (j & 1) ? j - 1 : j + 1;
+    return j % 3 == 1 ? j + 1 : (j % 3 == 2 ? j - 1 : j);
+  }
   if ((j >= 1 && j <= 3) || (j >= 11 && j <= 13)) return j + 3;
   if ((j >= 4 && j <= 6) || (j >= 14 && j <= 16)) return j - 3;
   return j;

@@ -12,7 +12,11 @@
 //                             posenet) from the camera-frame mesh, one launch (k_sample_targets, one CTA per sample,
 //                             branching on the dataset): both sparse joint regressors in one pass (fp64), COCO pelvis /
 //                             neck, the dataset's projection, rooting, its fitting test and validity masks, and the lift
-//                             target's rotation and flip; p2m_h36m_targets is its unaugmented Human36M case.
+//                             target's rotation and flip; p2m_h36m_targets is its unaugmented Human36M case.  3DPW
+//                             is its fifth case.
+//  * p2m_layer_joint_targets  SURREAL's and FreiHAND's targets, which take the layer's own joints instead of a
+//                             regressor's: one launch (k_layer_joint_targets, one CTA per sample), float32 rooting at
+//                             joint 0, SURREAL's projection and its lift target's rotation and flip.
 // No atomics and fixed orders: a sample's result is bitwise independent of its batch position and of the batch size;
 // nothing is read back to the host, so every call can be captured in a CUDA graph.
 #include <cuda_runtime.h>
@@ -29,6 +33,8 @@ namespace {
 constexpr int PREP_WARPS = 4;        // samples per k_frame_prep CTA
 constexpr int FIN_T = 256;           // threads (vertices) per k_frame_finish CTA
 constexpr int H36_T = 256;           // threads per k_sample_targets CTA
+constexpr int LJ_T = 256;            // threads per k_layer_joint_targets CTA
+constexpr int SMPL_J = 24, MANO_J = 21;
 constexpr int MAX_EXTRA = 8;         // appended vertex joints (MuCo: 5 face keypoints)
 constexpr int MAX_BATCH = 1 << 24;
 constexpr int NJ = 17;               // joints of each regressor
@@ -229,6 +235,16 @@ __device__ __forceinline__ double project(const SampleArgs& a, long long b, cons
   return p[q] / p[2] * (double)a.f[b * 2 + q] + (double)a.c[b * 2 + q];  // cam2pixel (lib/coord_utils.py:104-109)
 }
 
+// j3d_processing's rotation (lib/aug_utils.py:67-83): x, y rotated by -rot degrees in fp64 (rot 0: untouched)
+__device__ __forceinline__ void j3d_rotate(float rot, double l[3]) {
+  if (rot == 0.f) return;
+  double sn, cs;
+  sincospi(__ddiv_rn(-(double)rot, 180.0), &sn, &cs);  // (sin, cos)(-pi rot / 180)
+  const double x = l[0], y = l[1];
+  l[0] = __dadd_rn(__dmul_rn(cs, x), __dmul_rn(-sn, y));
+  l[1] = __dadd_rn(__dmul_rn(sn, x), __dmul_rn(cs, y));
+}
+
 __global__ void __launch_bounds__(H36_T) k_sample_targets(SampleArgs a) {
   __shared__ double sreg[NR][3], sjc[NJ][3], sroot[3], sfit[NJ][3];
   __shared__ float svalid;
@@ -333,7 +349,7 @@ __global__ void __launch_bounds__(H36_T) k_sample_targets(SampleArgs a) {
       svalid = err > a.thr ? 0.f : 1.f;
       a.fit_err[b] = (float)err;
     }
-  } else if (a.dataset == P2M_DATASET_AMASS && tid == 0) {
+  } else if ((a.dataset == P2M_DATASET_AMASS || a.dataset == P2M_DATASET_PW3D) && tid == 0) {
     svalid = 1.f;  // no fitting test
     a.fit_err[b] = 0.f;
   }
@@ -366,16 +382,9 @@ __global__ void __launch_bounds__(H36_T) k_sample_targets(SampleArgs a) {
         l[q] = h36m ? (double)(float)d : d;
       }
     }
-    // j3d_processing (lib/aug_utils.py:67-83): x, y rotated by -rot degrees in fp64, then x negated under a flip; the
-    // mesh and reg_pose3d targets are never augmented (data/Human36M/dataset.py:373, the same in every dataset)
-    const float rot = a.rot ? a.rot[b] : 0.f;
-    if (rot != 0.f) {
-      double sn, cs;
-      sincospi(__ddiv_rn(-(double)rot, 180.0), &sn, &cs);  // (sin, cos)(-pi rot / 180)
-      const double x = l[0], y = l[1];
-      l[0] = __dadd_rn(__dmul_rn(cs, x), __dmul_rn(-sn, y));
-      l[1] = __dadd_rn(__dmul_rn(sn, x), __dmul_rn(cs, y));
-    }
+    // j3d_processing: the rotation, then x negated under a flip; the mesh and reg_pose3d targets are never augmented
+    // (data/Human36M/dataset.py:373, the same in every dataset)
+    j3d_rotate(a.rot ? a.rot[b] : 0.f, l);
     if (flip) l[0] = -l[0];
     for (int q = 0; q < 3; ++q) a.lift[(b * J + j) * 3 + q] = (float)l[q];
     a.joint_img[(b * J + j) * 2] = (float)project(a, b, p, 0);
@@ -389,6 +398,65 @@ __global__ void __launch_bounds__(H36_T) k_sample_targets(SampleArgs a) {
   }
 }
 
+// One CTA per sample: SURREAL's and FreiHAND's targets (SURREAL/dataset.py:143-203, FreiHAND/dataset.py:139-192).
+// The reference roots its float32 arrays at the layer's joint 0 in float32 and divides the mesh by 1000 in float32;
+// SURREAL's lift target goes through j3d_processing, and its reg_pose3d is that same reassigned array (:178,195).
+struct LayerArgs {
+  int dataset, V, J;
+  const float* mesh_cam;   // [B, V, 3] mm
+  const float* joint_cam;  // [B, J, 3] mm, the layer's joints
+  const float* f;          // [B, 2] (SURREAL)
+  const float* c;
+  const float* rot;        // [B] degrees, or null (SURREAL)
+  const int* flip;         // [B], or null (SURREAL)
+  float* mesh;             // [B, V, 3] m
+  float* lift;             // [B, J, 3]
+  float* reg;              // [B, J, 3]
+  float* mesh_valid;       // [B, V]
+  float* lift_valid;       // [B, J]
+  float* reg_valid;        // [B, J]
+  float* joint_valid;      // [B, J], or null
+  float* joint_img;        // [B, J, 2] (SURREAL)
+  float* fit_err;          // [B]
+};
+
+__global__ void __launch_bounds__(LJ_T) k_layer_joint_targets(LayerArgs a) {
+  const long long b = blockIdx.x;
+  const int tid = threadIdx.x, V = a.V, J = a.J;
+  const float* jc = a.joint_cam + b * J * 3;
+  const float root[3] = {jc[0], jc[1], jc[2]};
+  if (tid < J) {
+    const int j = tid;
+    const bool surreal = a.dataset == P2M_DATASET_SURREAL;
+    const int flip = (surreal && a.flip) ? a.flip[b] : 0;
+    const int s = flip ? flip_partner(P2M_JOINTS_SMPL, j) : j;
+    double l[3];
+    for (int q = 0; q < 3; ++q) l[q] = (double)__fsub_rn(jc[3 * s + q], root[q]);
+    if (surreal) {
+      j3d_rotate(a.rot ? a.rot[b] : 0.f, l);
+      if (flip) l[0] = -l[0];
+      // cam2pixel of the absolute joints, taken before the rooting (SURREAL/dataset.py:151-153)
+      const double z = jc[3 * j + 2];
+      for (int q = 0; q < 2; ++q)
+        a.joint_img[(b * J + j) * 2 + q] = (float)((double)jc[3 * j + q] / z * (double)a.f[b * 2 + q] +
+                                                   (double)a.c[b * 2 + q]);
+    }
+    for (int q = 0; q < 3; ++q) {
+      a.lift[(b * J + j) * 3 + q] = (float)l[q];
+      a.reg[(b * J + j) * 3 + q] = (float)l[q];
+    }
+    a.lift_valid[b * J + j] = 1.f;
+    a.reg_valid[b * J + j] = 1.f;
+    if (a.joint_valid) a.joint_valid[b * J + j] = 1.f;
+  }
+  if (tid == 0) a.fit_err[b] = 0.f;
+  // bandwidth work: the mesh streamed once with strided threads
+  const float* mc = a.mesh_cam + b * V * 3;
+  for (int e = tid; e < 3 * V; e += LJ_T) {
+    a.mesh[b * V * 3 + e] = __fdiv_rn(__fsub_rn(mc[e], root[e % 3]), 1000.f);
+    if (e < V) a.mesh_valid[b * V + e] = 1.f;
+  }
+}
 
 struct FrameLayout {
   size_t pose, betas, trans, verts, joints, body, total;
@@ -577,12 +645,17 @@ int p2m_sample_targets(const p2m_h36m_regressors_t* h, int dataset, int input_jo
     set_error("sample_targets: bad argument (null handle / array, unknown joint set or batch out of [1, 2^24])");
     return P2M_ERR_INVALID;
   }
-  const bool need_fc = dataset == P2M_DATASET_HUMAN36M || dataset == P2M_DATASET_MUCO || dataset == P2M_DATASET_AMASS;
-  if (dataset < P2M_DATASET_HUMAN36M || dataset > P2M_DATASET_AMASS ||
+  const bool need_fc = dataset == P2M_DATASET_HUMAN36M || dataset == P2M_DATASET_MUCO || dataset == P2M_DATASET_AMASS ||
+                       dataset == P2M_DATASET_PW3D;
+  if (dataset < P2M_DATASET_HUMAN36M || dataset > P2M_DATASET_PW3D ||
       (dataset == P2M_DATASET_HUMAN36M && !joint_cam) || (need_fc && (!f || !c)) ||
       (dataset == P2M_DATASET_COCO && (!s || (n_s != 1 && n_s != 2) || !t || !keypoints || !keypoints_valid))) {
     set_error("sample_targets: unknown dataset, or its inputs are missing (Human36M: joint_cam, f, c; COCO: s with "
-              "n_s 1 or 2, t, keypoints, keypoints_valid; MuCo, AMASS: f, c)");
+              "n_s 1 or 2, t, keypoints, keypoints_valid; MuCo, AMASS, 3DPW: f, c)");
+    return P2M_ERR_INVALID;
+  }
+  if (dataset == P2M_DATASET_PW3D && (input_joint_set != P2M_JOINTS_COCO || rot || flip)) {
+    set_error("sample_targets: 3DPW takes the P2M_JOINTS_COCO set and no augmentation (rot and flip NULL)");
     return P2M_ERR_INVALID;
   }
   int dev = -1;
@@ -599,6 +672,42 @@ int p2m_sample_targets(const p2m_h36m_regressors_t* h, int dataset, int input_jo
                mesh_cam, joint_cam, f, c, s, n_s, t, keypoints, keypoints_valid, rot, flip, mesh, lift_pose3d,
                reg_pose3d, mesh_valid, lift_pose3d_valid, reg_pose3d_valid, joint_valid, joint_img, fitting_error};
   k_sample_targets<<<(unsigned)batch, H36_T, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  P2M_LAUNCH_OK();
+  return P2M_OK;
+}
+
+int p2m_layer_joint_targets(int dataset, const float* mesh_cam, const float* joint_cam, int n_vertex, int n_joint,
+                            const float* f, const float* c, const float* rot, const int32_t* flip, int batch,
+                            float* mesh, float* lift_pose3d, float* reg_pose3d, float* mesh_valid,
+                            float* lift_pose3d_valid, float* reg_pose3d_valid, float* joint_valid, float* joint_img,
+                            float* fitting_error, p2m_stream_t stream) {
+  if (batch <= 0 || batch > MAX_BATCH || n_vertex < 1 || n_vertex > (1 << 22) || !mesh_cam || !joint_cam || !mesh ||
+      !lift_pose3d || !reg_pose3d || !mesh_valid || !lift_pose3d_valid || !reg_pose3d_valid || !fitting_error) {
+    set_error("layer_joint_targets: bad argument (null array, batch out of [1, 2^24] or n_vertex out of [1, 2^22])");
+    return P2M_ERR_INVALID;
+  }
+  if (dataset == P2M_DATASET_SURREAL) {
+    if (n_joint != SMPL_J || !f || !c || !joint_img) {
+      set_error("layer_joint_targets: SURREAL takes SMPL's 24 joints, f, c and joint_img");
+      return P2M_ERR_INVALID;
+    }
+  } else if (dataset == P2M_DATASET_FREIHAND) {
+    if (n_joint != MANO_J || f || c || rot || flip || joint_img) {
+      set_error("layer_joint_targets: FreiHAND takes MANO's 21 joints and no f, c, rot, flip or joint_img");
+      return P2M_ERR_INVALID;
+    }
+  } else {
+    set_error("layer_joint_targets: dataset must be P2M_DATASET_SURREAL or P2M_DATASET_FREIHAND");
+    return P2M_ERR_INVALID;
+  }
+  int dev = -1;
+  P2M_TRY(arrays_device("layer_joint_targets", {mesh_cam, joint_cam, f, c, rot, flip, mesh, lift_pose3d, reg_pose3d,
+                                                mesh_valid, lift_pose3d_valid, reg_pose3d_valid, joint_valid,
+                                                joint_img, fitting_error}, &dev));
+  DeviceGuard guard(dev);
+  LayerArgs a{dataset, n_vertex, n_joint, mesh_cam, joint_cam, f, c, rot, flip, mesh, lift_pose3d, reg_pose3d,
+              mesh_valid, lift_pose3d_valid, reg_pose3d_valid, joint_valid, joint_img, fitting_error};
+  k_layer_joint_targets<<<(unsigned)batch, LJ_T, 0, static_cast<cudaStream_t>(stream)>>>(a);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }

@@ -5,7 +5,9 @@
     training_pose2d(joints_px, ...)         the train branch of the datasets' replace_joint_img with the crop and
                                             normalisation around it (data/Human36M/dataset.py:359-392,436-445); with
                                             box_joints and noise=False, the test split's branch (:446-452); with rot /
-                                            flip, the sample's rotation and flip (lib/aug_utils.py:33-64,140-195)
+                                            flip, the sample's rotation and flip (lib/aug_utils.py:33-64,140-195);
+                                            the 'smpl' / 'mano' sets are SURREAL's, FreiHAND's and 3DPW's noise-free
+                                            crop (data/SURREAL/dataset.py:143-186, data/FreiHAND/dataset.py:157-176)
     augm_params(B, flip, rotate_factor)     lib/aug_utils.py:98-117, each sample's flip and rotation
 
 All run in libp2m_b200.so (p2m_synthesize_pose, p2m_h36m_syn_error, p2m_training_pose2d_augmented,
@@ -31,7 +33,9 @@ from .postprocess import INPUT_SHAPE
 
 NUM_KPS = 17
 AREA_BOXES = {"tight": _lib.P2M_AREA_TIGHT, "crop": _lib.P2M_AREA_CROP}
-JOINT_SETS = {"human36": _lib.P2M_JOINTS_HUMAN36, "coco": _lib.P2M_JOINTS_COCO}
+JOINT_SETS = {"human36": _lib.P2M_JOINTS_HUMAN36, "coco": _lib.P2M_JOINTS_COCO, "smpl": _lib.P2M_JOINTS_SMPL,
+              "mano": _lib.P2M_JOINTS_MANO}
+LAYER_JOINTS = {"smpl": 24, "mano": 21}   # the sets that take no detector noise
 
 
 def _cuda(x, what: str, device=None) -> torch.Tensor:
@@ -175,9 +179,14 @@ def training_pose2d(joints_px: torch.Tensor, input_joint_set: str, *, noise: boo
     rot [B] (degrees) and flip [B] are augm_params' outputs (None: no rotation / flip, bit for bit the call without
     them).  The rotation goes into the crop's affine map (get_affine_transform); the flip is x -> input_w - x - 1 and
     the joint set's flip pairs swapped, after the noise as Human3.6M, COCO and AMASS do, or with
-    flip_before_noise=True before it, in float64 on the crop map's output, as MuCo's j2d_processing does."""
-    if input_joint_set not in ("coco", "human36"):
-        raise ValueError(f"input_joint_set must be 'coco' or 'human36'; got {input_joint_set!r}")
+    flip_before_noise=True before it, in float64 on the crop map's output, as MuCo's j2d_processing does.
+
+    input_joint_set 'smpl' (J = 24, SURREAL) and 'mano' (J = 21, FreiHAND) take noise=False: their inputs are the 2-D
+    joints themselves.  'mano' has no flip pairs, so it takes no flip.  SURREAL's j2d_processing flips in the joints'
+    own dtype: its float32 detections flip after the crop is rounded (flip_before_noise=False), the float64
+    cam2pixel joints of use_gt_input before (flip_before_noise=True)."""
+    if input_joint_set not in JOINT_SETS:
+        raise ValueError(f"input_joint_set must be one of {sorted(JOINT_SETS)}; got {input_joint_set!r}")
     if area_box not in AREA_BOXES:
         raise ValueError(f"area_box must be one of {sorted(AREA_BOXES)}; got {area_box!r}")
     _lib.cuda_tensor(joints_px, "joints_px")
@@ -186,6 +195,14 @@ def training_pose2d(joints_px: torch.Tensor, input_joint_set: str, *, noise: boo
     if x.dim() != 3 or x.shape[2] != 2 or x.shape[0] < 1 or not 1 <= x.shape[1] <= 32:
         raise ValueError(f"joints_px must be [B, J, 2] with B > 0 and J <= 32; got {tuple(joints_px.shape)}")
     B, J = x.shape[:2]
+    if input_joint_set in LAYER_JOINTS:
+        if noise:
+            raise ValueError(f"the {input_joint_set!r} joint set has no detector noise: pass noise=False")
+        if J != LAYER_JOINTS[input_joint_set]:
+            raise ValueError(f"the {input_joint_set!r} joint set takes {LAYER_JOINTS[input_joint_set]} joints; got "
+                             f"J = {J}")
+        if input_joint_set == "mano" and flip is not None:
+            raise ValueError("the 'mano' joint set has no flip pairs: flip must be None")
     mode = _lib.P2M_NOISE_NONE
     table = None
     if noise and input_joint_set == "coco":
@@ -205,7 +222,8 @@ def training_pose2d(joints_px: torch.Tensor, input_joint_set: str, *, noise: boo
             raise ValueError(f"box_joints must be [{B}, Jb, 2] with Jb <= 32; got {tuple(box_joints.shape)}")
         box_joints, nb = bj, bj.shape[1]
     rot, flip = augment_tensors(rot, flip, B, dev)
-    if flip is not None and (J != NUM_KPS if input_joint_set == "human36" else J < NUM_KPS):
+    if flip is not None and input_joint_set in ("coco", "human36") and \
+            (J != NUM_KPS if input_joint_set == "human36" else J < NUM_KPS):
         raise ValueError(f"a flip of the {input_joint_set!r} joints needs "
                          f"{'17' if input_joint_set == 'human36' else 'at least 17'} joints; got J = {J}")
     s = _seed(seed, dev) if mode != _lib.P2M_NOISE_NONE else None

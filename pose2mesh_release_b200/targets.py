@@ -2,13 +2,15 @@
 
     camera_frame_coords(layer, dataset, ...)   each dataset's get_smpl_coord / get_mano_coord:
                                                data/{Human36M,AMASS,FreiHAND,MuCo,COCO,SURREAL,PW3D}/dataset.py
-    Human36MTargets, COCOTargets, MuCoTargets, AMASSTargets
+    Human36MTargets, COCOTargets, MuCoTargets, AMASSTargets, PW3DTargets
                                                the targets and meta of each dataset's __getitem__ for pose2mesh_net and
                                                posenet, with the lift target's rotation and flip (j3d_processing)
+    SURREALTargets, FreiHANDTargets            the same for the datasets that take the body model's own joints as
+                                               targets (SMPL's 24, MANO's 21) instead of a regressor's
 
-Both run in libp2m_b200.so (p2m_camera_frame_coords, p2m_sample_targets): a prep kernel, the body model's three
-launches and a finish kernel per camera-frame call, one more launch for a dataset's assembly.  CUDA tensors only;
-nothing is read back to the host, so a call can be captured in a CUDA graph.
+All run in libp2m_b200.so (p2m_camera_frame_coords, p2m_sample_targets, p2m_layer_joint_targets): a prep kernel, the
+body model's three launches and a finish kernel per camera-frame call, one more launch for a dataset's assembly.  CUDA
+tensors only; nothing is read back to the host, so a call can be captured in a CUDA graph.
 
 The datasets call the body model once per sample, so its quirks apply per sample here: the betas clamp (any
 |beta| > 3 -> zeros) and SMPL_Layer's "all-zero betas -> the model's betas" rule are decided for each sample on its
@@ -275,3 +277,102 @@ class AMASSTargets(_SampleTargets):
     def __call__(self, pose, betas, R, t, f, c, rot=None, flip=None) -> dict:
         mesh_cam, _ = camera_frame_coords(self.layer, "amass", pose, betas, None, R, t)
         return self._assemble(mesh_cam, rot, flip, f=f, c=c)
+
+
+class PW3DTargets(_SampleTargets):
+    """PW3D.__getitem__'s targets (data/PW3D/dataset.py:208-261), the test split of the *_cocoJ_test_3dpw configs.  The
+    reference hard-codes the coco input set, so input_joint_set must be 'coco'.  A call takes pose [B, 72], betas
+    [B, 10], trans [B, 3], focal f [B, 2] and principal point c [B, 2].  joint_img = cam2pixel(joint, f, c) of the
+    regressed COCO joints with pelvis and neck (mm, as MuCo's).  No fitting test and no augmentation (the reference
+    hard-codes rot = flip = 0): every mask is 1, fitting_error 0."""
+
+    DATASET, FITTING_THR = _lib.P2M_DATASET_PW3D, 0.0
+
+    def __init__(self, layer: SMPLLayer, joint_regressor_h36m, joint_regressor_coco, input_joint_set: str = "coco"):
+        if input_joint_set != "coco":
+            raise ValueError(f"PW3DTargets takes the 'coco' input joint set only; got {input_joint_set!r}")
+        super().__init__(layer, joint_regressor_h36m, joint_regressor_coco, "coco")
+
+    def __call__(self, pose, betas, trans, f, c) -> dict:
+        mesh_cam, _ = camera_frame_coords(self.layer, "pw3d", pose, betas, trans)
+        return self._assemble(mesh_cam, None, None, f=f, c=c)
+
+
+class _LayerJointTargets:
+    """The target side of SURREAL's and FreiHAND's __getitem__ for a batch: camera_frame_coords with the dataset's
+    preset, then one assembly launch (p2m_layer_joint_targets).  These datasets take the layer's own joints (J = 24
+    SMPL joints, 21 MANO joints) as both the lift and the regression target, so no regressor is needed.  A call returns
+    the keys of _SampleTargets, float32 device tensors:
+
+        mesh [B, V, 3]                  metres, (mesh - joint 0) / 1000 in float32
+        lift_pose3d, reg_pose3d [B, J, 3]
+                                        the joints rooted at joint 0 in float32 (mm)
+        mesh_valid [B, V, 1], lift_pose3d_valid, reg_pose3d_valid, joint_valid [B, J, 1]
+                                        all ones: neither dataset has a fitting test
+        joint_img [B, J, 2]             SURREAL only: cam2pixel of the absolute joints (image pixels)
+        fitting_error [B]               0
+
+    Six launches per call."""
+
+    LAUNCHES = 6
+    DATASET = LAYER = None
+
+    def __init__(self, layer):
+        name = type(self).__name__
+        if not isinstance(layer, self.LAYER):
+            raise ValueError(f"{name} takes a {self.LAYER.__name__}; got {type(layer).__name__}")
+        if layer.center_idx is not None:
+            raise ValueError(f"{name} needs a layer with center_idx None, as the datasets build them")
+        self.layer, self.num_joints = layer, layer.n_out_joints
+
+    def _assemble(self, mesh_cam, joint_cam, f=None, c=None, rot=None, flip=None) -> dict:
+        """The assembly alone, on camera-frame mesh_cam [B, V, 3] and joint_cam [B, J, 3] (mm)."""
+        _lib.cuda_tensor(mesh_cam, "mesh_cam")
+        if mesh_cam.dim() != 3 or mesh_cam.shape[2] != 3 or mesh_cam.shape[0] < 1 or mesh_cam.shape[1] < 1:
+            raise ValueError(f"mesh_cam must be [B, V, 3] with B, V > 0; got {tuple(mesh_cam.shape)}")
+        B, V, J, dev = mesh_cam.shape[0], mesh_cam.shape[1], self.num_joints, mesh_cam.device
+        mesh_cam = _cuda(mesh_cam, "mesh_cam", (B, V, 3), dev)
+        joint_cam = _cuda(joint_cam, "joint_cam", (B, J, 3), dev)
+        surreal = self.DATASET == _lib.P2M_DATASET_SURREAL
+        if surreal:
+            f, c = _cuda(f, "f", (B, 2), dev), _cuda(c, "c", (B, 2), dev)
+        rot, flip = augment_tensors(rot, flip, B, dev)
+        e = lambda *sh: torch.empty(sh, device=dev, dtype=torch.float32)  # noqa: E731
+        out = {"mesh": e(B, V, 3), "lift_pose3d": e(B, J, 3), "reg_pose3d": e(B, J, 3), "mesh_valid": e(B, V, 1),
+               "lift_pose3d_valid": e(B, J, 1), "reg_pose3d_valid": e(B, J, 1), "joint_valid": e(B, J, 1)}
+        if surreal:
+            out["joint_img"] = e(B, J, 2)
+        out["fitting_error"] = e(B)
+        _lib.call("p2m_layer_joint_targets", dev, self.DATASET, mesh_cam, joint_cam, V, J, f, c, rot, flip, B,
+                  out["mesh"], out["lift_pose3d"], out["reg_pose3d"], out["mesh_valid"], out["lift_pose3d_valid"],
+                  out["reg_pose3d_valid"], out["joint_valid"], out.get("joint_img"), out["fitting_error"])
+        return out
+
+
+class SURREALTargets(_LayerJointTargets):
+    """SURREAL.__getitem__'s targets (data/SURREAL/dataset.py:143-203), 24 SMPL joints rooted at joint 0.  A call
+    takes pose [B, 72], betas [B, 10], trans [B, 3], focal f [B, 2] and principal point c [B, 2]; joint_img =
+    cam2pixel(joint, f, c) of the absolute joints, in fp64 and rounded once.  rot [B] (degrees) and flip [B],
+    augm_params' outputs, augment lift_pose3d as j3d_processing does with SMPL's flip pairs.  The reference's quirk is
+    kept: reg_pose3d is the same augmented array (both targets are its reassigned joint_coord_cam), while the mesh is
+    never augmented.  posenet_smplJ_train_surreal flips (AUG.flip True) but PoseNet reads only lift_pose3d; the
+    pose2mesh SURREAL configs, which read reg_pose3d, never augment."""
+
+    DATASET, LAYER = _lib.P2M_DATASET_SURREAL, SMPLLayer
+
+    def __call__(self, pose, betas, trans, f, c, rot=None, flip=None) -> dict:
+        mesh_cam, joint_cam = camera_frame_coords(self.layer, "surreal", pose, betas, trans)
+        return self._assemble(mesh_cam, joint_cam, f, c, rot, flip)
+
+
+class FreiHANDTargets(_LayerJointTargets):
+    """FreiHAND.__getitem__'s targets (data/FreiHAND/dataset.py:139-192), 21 MANO joints (the tips appended) rooted at
+    joint 0, the wrist.  A call takes pose [B, 48], betas [B, 10] and the camera R [B, 3, 3], t [B, 3].  No joint_img
+    (the reference's projection is commented out and its input is always the detection) and no augmentation (the
+    reference hard-codes rot = flip = 0)."""
+
+    DATASET, LAYER = _lib.P2M_DATASET_FREIHAND, ManoLayer
+
+    def __call__(self, pose, betas, R, t) -> dict:
+        mesh_cam, joint_cam = camera_frame_coords(self.layer, "freihand", pose, betas, None, R, t)
+        return self._assemble(mesh_cam, joint_cam)
