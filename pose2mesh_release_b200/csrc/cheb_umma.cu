@@ -41,7 +41,6 @@
 
 #include <algorithm>
 #include <climits>
-#include <cstdlib>
 #include <cstring>
 #include <vector>
 
@@ -79,6 +78,8 @@ inline int up16(int x) { return (x + 15) & ~15; }
 // 512 bytes (what one cp.async.bulk moves) at a stride of 544 bytes.  136 floats is 8 banks mod 32, so the four rows a
 // half-warp's 64-bit fragment access touches (8 consecutive words each) cover the 32 banks exactly once.
 constexpr int STG_ROW_BYTES = 544;
+// per-warp epilogue staging: a 32 x 32 fp32 sub-slab (N = 64), or 16 rows of STG_ROW_BYTES (N = 128)
+__host__ __device__ constexpr int stg_warp_bytes(int N) { return N == 128 ? 16 * STG_ROW_BYTES : 32 * 32 * 4; }
 
 // ------------------------------------------------------------------ PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -276,24 +277,22 @@ __device__ __forceinline__ float4 gather_row4(uint32_t ent, uint32_t e, uint32_t
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// TA / TB = 1: the operand is MN-major (transposed) in shared memory
-template <int TA, int TB>
+// both operands K-major in shared memory (the immediates after p: scale-a, scale-b, transpose-a, transpose-b)
 __device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %34, %35;\n\t}"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
         "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
         "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
         "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
+      : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
 // the same with N = 128 (64 accumulator registers): d[h][j] is element j + 32 h of the fragment, i.e. d[h] holds the
 // 64-column half h exactly as an m64n64 on that half would
-template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n128(float (&d)[2][32], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
@@ -301,7 +300,7 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[2][32], uint64_t desc_a
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
       "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
       "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %66, %67;\n\t}"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
       : "+f"(d[0][0]), "+f"(d[0][1]), "+f"(d[0][2]), "+f"(d[0][3]), "+f"(d[0][4]), "+f"(d[0][5]), "+f"(d[0][6]),
         "+f"(d[0][7]), "+f"(d[0][8]), "+f"(d[0][9]), "+f"(d[0][10]), "+f"(d[0][11]), "+f"(d[0][12]), "+f"(d[0][13]),
         "+f"(d[0][14]), "+f"(d[0][15]), "+f"(d[0][16]), "+f"(d[0][17]), "+f"(d[0][18]), "+f"(d[0][19]), "+f"(d[0][20]),
@@ -312,19 +311,18 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[2][32], uint64_t desc_a
         "+f"(d[1][17]), "+f"(d[1][18]), "+f"(d[1][19]), "+f"(d[1][20]), "+f"(d[1][21]), "+f"(d[1][22]), "+f"(d[1][23]),
         "+f"(d[1][24]), "+f"(d[1][25]), "+f"(d[1][26]), "+f"(d[1][27]), "+f"(d[1][28]), "+f"(d[1][29]), "+f"(d[1][30]),
         "+f"(d[1][31])
-      : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
+      : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
-// the same with N = 32 (16 accumulator registers)
-template <int TA, int TB>
+// M = 64, N = 32 (16 accumulator registers), both operands MN-major (transposed: 1, 1) in shared memory
 __device__ __forceinline__ void wgmma_m64n32(float (&d)[16], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
       "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %18, %19;\n\t}"
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
         "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-      : "l"(desc_a), "l"(desc_b), "n"(TA), "n"(TB)
+      : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
 
@@ -467,11 +465,45 @@ struct ConvRoles<128> {
 // MODE 0: plain GEMM, no sparse product (the isolated rows of padding elision, the backward dT GEMMs, the dense GEMM).
 template <int N>
 __host__ __device__ constexpr int tile_rows() { return N == 128 ? 64 : TILE_M; }
+
+// ------------------------------------------------------------------ dynamic shared-memory layouts
+// conv_smem, dw_smem and t1_smem describe each kernel's dynamic shared memory once: the kernel carves its buffers at
+// these byte offsets from its 1024-byte aligned base, the host takes the launch size and every fit test from `bytes`
+// (the conv and dW sizes include 1024 + 32 bytes of slack that the kernels do not use).  Stage sizes are in floats.
+
+// cheb_conv_body<N, NS, XS, MODE> on tiles of at most max_h1 staged rows, metadata blobs meta_stride bytes apart
+struct ConvSmem {
+  size_t xs, xs_stage, t1s, t1_stage, meta, bars, flags, ep, stage, own, tail, bytes;
+};
+__host__ __device__ __forceinline__ ConvSmem conv_smem(int N, int NS, int XS, int MODE, int max_h1, int meta_stride) {
+  const int tm = N == 128 ? 64 : TILE_M;
+  size_t at = 0, sum = 0;  // next offset; total size of the buffers
+  auto take = [&](size_t bytes) { sum += bytes; at += bytes; return at - bytes; };
+  ConvSmem L;
+  take((size_t)NS * (tm + N) * 128);  // the ring at offset 0, [NS] slots: A block (tm x 128 B) + B block (N x 128 B)
+  // [XS][tm][32] fp32 own X rows: read in MODE 0 only (MODE 1 reads X from global memory); none at MODE 1, tm = 64
+  L.xs_stage = (MODE == 1 && tm == 64) ? 0 : (size_t)tm * FC;
+  L.xs = take(XS * L.xs_stage * 4);
+  L.t1_stage = MODE == 1 ? (size_t)max_h1 * FC : 0;  // [XS][max_h1][32] fp32: T1 rows of the tile and its 1-hop halo
+  L.t1s = take(XS * L.t1_stage * 4);
+  L.meta = take(2 * (size_t)meta_stride);    // [2] tile metadata blobs (the dense GEMM: none)
+  L.bars = take(8 * (2 * NS + 2 * XS + 6));  // the kernel's barrier map
+  L.flags = take(16);                        // word 1: the CTA's abort flag
+  L.ep = take(2 * 4 * N);                    // epilogue vectors ep_mul, ep_add [N]
+  at = (at + 127) & ~(size_t)127;
+  L.stage = take(4 * stg_warp_bytes(N));  // [4 warps] epilogue staging, 128-byte aligned
+  L.own = take(4 * 32 * 4);               // [NWG][4 warps][ER] epilogue rows' vertex ids (NWG * ER = 32)
+  L.tail = take(N == 64 ? 64 * 12 * 4 : 4 * 8);  // N = 64: fused-head weights [64][12]; N = 128: 4 residual mbarriers
+  L.bytes = sum + 128 + 1024 + 32;               // (128: the staging buffer's alignment)
+  return L;
+}
+
 // The body of both conv kernels: k_cheb_conv_umma (N = 64) and k_cheb_conv_wide (N = 128) differ in their role map
 // and register targets (ConvRoles<N>) and in their launch size.
 template <int N, int NS, int XS, int MODE>
 __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
+  static_assert(NS == 3 || NS == 6, "the producers fill a chunk's three slots back to back");
   using R = ConvRoles<N>;
   constexpr int TM = tile_rows<N>();  // tile rows
   constexpr int NPW = R::prod;        // producer warps
@@ -483,24 +515,18 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   constexpr int ER = 16 * H;          // epilogue rows per warp of the MMA warpgroup
   constexpr bool KT1 = (MODE == 1);
   constexpr bool plain = !KT1;
-  // X of the own rows straight from global memory (T1 given, deep ring): the only reader of an own X row is the
-  // producer thread that emits it, so staging it costs a shared-memory write plus a read back (8 % of the kernel's
-  // shared-memory traffic, and more than half of the loaders' copies on index-list tiles) for nothing
-  constexpr bool XDIRECT = KT1 && NS >= 3;
   constexpr int A_BYTES = TM * 128;  // one K-block of A: TM rows x (32 hi | 32 lo) fp16
   constexpr int B_BLOCK_BYTES = N * 128;
   constexpr int SLOT_BYTES = A_BYTES + B_BLOCK_BYTES;
+  static_assert(NWG * ER == 32 && SLOT_BYTES == (TM + N) * 128, "conv_smem describes this configuration");
 
   extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const ConvSmem L = conv_smem(N, NS, XS, MODE, p.max_h1, p.meta_stride);
   unsigned char* ring = smem_raw;  // 128B-swizzled blocks need 1024-byte alignment (checked below)
-  float* Xs = reinterpret_cast<float*>(ring + NS * SLOT_BYTES);                 // [XS][TM][32]
-  // (the 64-row configuration allocates no X stage where the producers read X directly: its room deepens the ring)
-  const size_t xs_stage_floats = (XDIRECT && TM == 64) ? 0 : (size_t)TM * FC;
-  float* T1s = Xs + XS * xs_stage_floats;                                       // [XS | 0][max_h1][32]
-  const size_t t1_stage_floats = (size_t)p.max_h1 * FC;
-  unsigned char* meta_s =
-      reinterpret_cast<unsigned char*>(T1s + (plain ? 0 : XS) * t1_stage_floats);  // [2][meta_stride]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(meta_s + 2 * (size_t)p.meta_stride);
+  float* Xs = reinterpret_cast<float*>(smem_raw + L.xs);
+  float* T1s = reinterpret_cast<float*>(smem_raw + L.t1s);
+  unsigned char* meta_s = smem_raw + L.meta;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + L.bars);
   // barrier map
   uint64_t* b_ab_full = bars;                // [NS]
   uint64_t* b_ab_empty = b_ab_full + NS;     // [NS]
@@ -512,19 +538,18 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   // epilogue to the other's (one arrival per warp); the tile before has finished its main loop (one arrival per warp)
   uint64_t* b_stg_free = b_m_empty + 2;      // [1]
   uint64_t* b_turn = b_stg_free + 1;         // [1]
-  uint32_t* flags = reinterpret_cast<uint32_t*>(b_turn + 1);
+  uint32_t* flags = reinterpret_cast<uint32_t*>(smem_raw + L.flags);
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
-  float* ep_mul = reinterpret_cast<float*>(flags + 4);  // [N] acc * mul + add  (weight scale, bias, folded BN)
+  float* ep_mul = reinterpret_cast<float*>(smem_raw + L.ep);  // [N] acc * mul + add  (weight scale, bias, folded BN)
   float* ep_add = ep_mul + N;
   // epilogue staging: N = 64: [4 warps][32 rows][EC floats], 16-byte chunks XOR-swizzled by the row, one 32-column
   // sub-slab at a time; N = 128: [4 warps][16 rows][STG_ROW_BYTES], a warp's whole 16 x 128 block in linear rows
   constexpr int EC = 32;
-  constexpr int STG_WARP_BYTES = N == 128 ? 16 * STG_ROW_BYTES : 32 * EC * 4;
-  unsigned char* epi_stage =
-      reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(ep_add + N) + 127) & ~(uintptr_t)127);
+  constexpr int STG_WARP_BYTES = stg_warp_bytes(N);
+  unsigned char* epi_stage = smem_raw + L.stage;
   // (N = 128: the two MMA warpgroups share the staging buffer, one tile after the other)
-  int* own_s = reinterpret_cast<int*>(epi_stage + 4 * STG_WARP_BYTES);  // [NWG][4 warps][ER] vertex id of each epilogue row
-  float* head_w_s = reinterpret_cast<float*>(own_s + NWG * 4 * ER);  // [64][12] (N == 64 with a fused head)
+  int* own_s = reinterpret_cast<int*>(smem_raw + L.own);  // [NWG][4 warps][ER] vertex id of each epilogue row
+  float* head_w_s = reinterpret_cast<float*>(smem_raw + L.tail);  // [64][12] (N == 64 with a fused head)
   uint64_t* b_res = reinterpret_cast<uint64_t*>(head_w_s);  // [4] (N = 128: no head) per staging block: its tile's
                                                             // identity-residual rows have landed in it
 
@@ -595,7 +620,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
       const int lq = lt & 7, lrg = lt >> 3;
       const int my_tiles = (p.n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
       if (lt == 32 && p.tma) {
-        if (!XDIRECT) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tm_x)) : "memory");
+        if (plain) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tm_x)) : "memory");
         if (KT1) asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&p.tm_t1)) : "memory");
       }
       auto fetch_meta = [&](int itf) {  // thread 0: blob of this CTA's tile number itf into buffer itf & 1
@@ -646,20 +671,20 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           const char* t1_mesh =
               reinterpret_cast<const char*>(KT1 ? p.t1 + mesh_row0 * p.fin + c2 * FC + lq * 4 : nullptr);
           const char* x_mesh = reinterpret_cast<const char*>(p.x + (mesh_row0 >> sh) * p.fin + c2 * FC + lq * 4);
-          const uint32_t t1_dst = smem_u32(T1s + xs2 * t1_stage_floats) + lq * 16;
-          const uint32_t x_dst = smem_u32(Xs + xs2 * xs_stage_floats) + lq * 16;
+          const uint32_t t1_dst = smem_u32(T1s + xs2 * L.t1_stage) + lq * 16;
+          const uint32_t x_dst = smem_u32(Xs + xs2 * L.xs_stage) + lq * 16;
           if (p.tma) {
             if (lt == 32) {
               const int own0 = tile2 * TM;  // V is a multiple of 128: tiles never straddle meshes
-              mbar_arrive_expect_tx(xbar, (XDIRECT ? 0 : (p.in_unpool ? TM / 2 : TM) * 128) + (KT1 ? TM * 128 : 0));
-              if (!XDIRECT)
-                tma_load_2d(smem_u32(Xs + xs2 * xs_stage_floats), &p.tm_x, c2 * FC, p.in_unpool ? own0 >> 1 : own0, xbar);
-              if (KT1) tma_load_2d(smem_u32(T1s + xs2 * t1_stage_floats), &p.tm_t1, c2 * FC, own0, xbar);
+              mbar_arrive_expect_tx(xbar, KT1 ? TM * 128 : (p.in_unpool ? TM / 2 : TM) * 128);
+              if (plain)
+                tma_load_2d(smem_u32(Xs + xs2 * L.xs_stage), &p.tm_x, c2 * FC, p.in_unpool ? own0 >> 1 : own0, xbar);
+              if (KT1) tma_load_2d(smem_u32(T1s + xs2 * L.t1_stage), &p.tm_t1, c2 * FC, own0, xbar);
             }
             if (KT1) stage_rows(t1_dst, t1_mesh, TM, h1, 0);  // only the halo rows are left
           } else {
             if (KT1) stage_rows(t1_dst, t1_mesh, 0, h1, 0);
-            if (!XDIRECT) stage_rows(x_dst, x_mesh, 0, TM, sh);
+            if (plain) stage_rows(x_dst, x_mesh, 0, TM, sh);
             if (lt == 32) mbar_arrive(xbar);
           }
           cp_async_arrive_noinc(xbar);  // this thread's arrival once its copies have landed
@@ -788,24 +813,24 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           // order as with two m64n64 column halves
           const uint64_t da = make_desc_sw128(a0);
           const uint64_t db = make_desc_sw128(a0 + A_BYTES);
-          wgmma_m64n128<0, 0>(acc, da + 0, db + 0);  // hi * Whi
-          wgmma_m64n128<0, 0>(acc, da + 2, db + 2);
-          wgmma_m64n128<0, 0>(acc, da + 4, db + 0);  // lo * Whi
-          wgmma_m64n128<0, 0>(acc, da + 6, db + 2);
-          wgmma_m64n128<0, 0>(acc, da + 0, db + 4);  // hi * Wlo
-          wgmma_m64n128<0, 0>(acc, da + 2, db + 6);
+          wgmma_m64n128(acc, da + 0, db + 0);  // hi * Whi
+          wgmma_m64n128(acc, da + 2, db + 2);
+          wgmma_m64n128(acc, da + 4, db + 0);  // lo * Whi
+          wgmma_m64n128(acc, da + 6, db + 2);
+          wgmma_m64n128(acc, da + 0, db + 4);  // hi * Wlo
+          wgmma_m64n128(acc, da + 2, db + 6);
         } else {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             // rows 64..127 of the A block (the tile's second M = 64 half) start 8 KB further on
             const uint64_t da = make_desc_sw128(a0 + (uint32_t)h * (64 * 128));
             const uint64_t db = make_desc_sw128(a0 + A_BYTES);
-            wgmma_m64n64<0, 0>(acc[h], da + 0, db + 0);  // hi * Whi
-            wgmma_m64n64<0, 0>(acc[h], da + 2, db + 2);
-            wgmma_m64n64<0, 0>(acc[h], da + 4, db + 0);  // lo * Whi
-            wgmma_m64n64<0, 0>(acc[h], da + 6, db + 2);
-            wgmma_m64n64<0, 0>(acc[h], da + 0, db + 4);  // hi * Wlo
-            wgmma_m64n64<0, 0>(acc[h], da + 2, db + 6);
+            wgmma_m64n64(acc[h], da + 0, db + 0);  // hi * Whi
+            wgmma_m64n64(acc[h], da + 2, db + 2);
+            wgmma_m64n64(acc[h], da + 4, db + 0);  // lo * Whi
+            wgmma_m64n64(acc[h], da + 6, db + 2);
+            wgmma_m64n64(acc[h], da + 0, db + 4);  // hi * Wlo
+            wgmma_m64n64(acc[h], da + 2, db + 6);
           }
         }
         wg_commit();
@@ -1027,7 +1052,10 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
     };
 
     const int xsh = (p.tma && p.in_unpool) ? 1 : 0;  // TMA-staged unpooled input: staged row = tile row >> 1
-    const float* xp[RPT];  // XDIRECT: this thread's own X rows (nullptr: empty slot), at its 16-byte column
+    // T1 given: the thread's own X rows come straight from global memory.  Their only reader is the producer thread
+    // that emits them, so staging them would cost a shared-memory write plus a read back (8 % of the kernel's
+    // shared-memory traffic, and more than half of the loaders' copies on index-list tiles) for nothing.
+    const float* xp[RPT];  // this thread's own X rows (nullptr: empty slot), at its 16-byte column
 #pragma unroll
     for (int ps = 0; ps < RPT; ++ps) xp[ps] = nullptr;
     int it = 0, c = -1;
@@ -1043,7 +1071,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
       for (int ps = 0; ps < RPT; ++ps) {
         xd[ps] = make_float4(0.f, 0.f, 0.f, 0.f);
         // in flight while the stage wait and the gather run (first chunk: below, after the tile setup)
-        if (XDIRECT && c != 0 && xp[ps]) xd[ps] = __ldg(reinterpret_cast<const float4*>(xp[ps] + c * FC));
+        if (KT1 && c != 0 && xp[ps]) xd[ps] = __ldg(reinterpret_cast<const float4*>(xp[ps] + c * FC));
       }
       if (tid == 0) trace_ev(p, 0, ptn, 1);
       mbar_wait(smem_u32(b_x_full + xs), (g / XS) & 1, abort_flag, p.status, 9);
@@ -1066,7 +1094,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           so_f[ps] = odd ? a_lo : a_hi;
           so_s[ps] = odd ? a_hi : a_lo;
         }
-        if (XDIRECT) {
+        if (KT1) {
           const int* halo = reinterpret_cast<const int*>(mb + hdr->off_halo);  // slots 0..TM-1 = the tile's own rows
           const int sh = p.in_unpool ? 1 : 0;
           const long long mesh_row0 = (long long)((blockIdx.x + (unsigned)it * gridDim.x) / (unsigned)p.P) * p.V;
@@ -1079,8 +1107,8 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           }
         }
       }
-      const uint32_t xs_q = smem_u32(Xs + xs * xs_stage_floats) + q * 16;
-      const uint32_t t1s_q = t1s_a + (uint32_t)(xs * t1_stage_floats * 4) + q * 16;
+      const uint32_t xs_q = smem_u32(Xs + xs * L.xs_stage) + q * 16;
+      const uint32_t t1s_q = t1s_a + (uint32_t)(xs * L.t1_stage * 4) + q * 16;
       if (plain) {
         // plain GEMM: the staged rows ARE the A operand (scaled into fp16 range if a_scale is given)
         const uint32_t s = slot;
@@ -1107,17 +1135,14 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
         if (tid == 0 && c == n_chunk - 1) mbar_arrive(smem_u32(b_m_empty + m));
         continue;
       }
-      // Split to fp16 (hi, lo) and write the three K-blocks of the tile rows this thread finishes.  The X and T1
-      // blocks go first: they need no gather, so the tensor core starts on them while the second sparse product
-      // T2 = 2 L~ T1 - X is still being gathered (with a 2-deep ring, N = 256, the T2 block re-uses the X block's slot
-      // and would otherwise wait for its MMAs).  NS >= 3: ONE generic->async proxy fence for all three blocks (the
-      // fence drains the thread's outstanding shared stores and is expensive); NS < 3: one per block.  Odd row groups
+      // Split to fp16 (hi, lo) and write the three K-blocks (X, T1, T2 = 2 L~ T1 - X) of the tile rows this thread
+      // finishes: the gather first (measured faster than emitting X and T1 before it: the gather then overlaps the
+      // previous chunk's tail instead of this chunk's own stores), then the three blocks back to back under ONE
+      // generic->async proxy fence (it drains the thread's outstanding shared stores and is expensive).  Odd row groups
       // store lo first: a warp then covers both 64-byte halves of its rows per store.
       const uint32_t slot0 = slot;
       auto emit = [&](const float4 (&vv)[RPT]) {
-        const uint32_t s = slot;
-        if (NS < 3) mbar_wait(smem_u32(b_ab_empty + s), spar ^ 1u, abort_flag, p.status, 10);
-        const uint32_t ablk = ring_a + s * SLOT_BYTES;
+        const uint32_t ablk = ring_a + slot * SLOT_BYTES;
 #pragma unroll
         for (int ps = 0; ps < RPT; ++ps) {
           uint2 hi, lo;
@@ -1132,60 +1157,34 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           sts_u2(ablk + so_f[ps], odd ? lo : hi);
           sts_u2(ablk + so_s[ps], odd ? hi : lo);
         }
-        if (NS < 3) {
-          fence_async_proxy();
-          __syncwarp();
-          if ((tid & 31) == 0) mbar_arrive(smem_u32(b_ab_full + s));
-        }
         next_slot();
       };
-      float4 x[RPT], t1v[RPT], t2[RPT];
-      if (NS < 3) {
+      float4 t1v[RPT], t2[RPT];
 #pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) x[ps] = lds_f4(xs_q + (row[ps] >> xsh) * 128);
-        emit(x);
+      for (int ps = 0; ps < RPT; ++ps) t2[ps] = gather_row4(ent_a, re[ps] & 0xFFFFu, re[ps] >> 16, t1s_q);
 #pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) t1v[ps] = lds_f4(t1s_q + row[ps] * 128);
-        emit(t1v);
-#pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) t2[ps] = gather_row4(ent_a, re[ps] & 0xFFFFu, re[ps] >> 16, t1s_q);
-        if (tid == 0) trace_ev(p, 0, ptn, 6);
-#pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) t2[ps] = cheb_t2(t2[ps], x[ps]);
-        emit(t2);
-      } else {
-        // deep ring: gather first, then the three blocks back to back (measured faster than the early X/T1 emit:
-        // the gather then overlaps the previous chunk's tail instead of this chunk's own stores)
-#pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) t2[ps] = gather_row4(ent_a, re[ps] & 0xFFFFu, re[ps] >> 16, t1s_q);
-#pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) x[ps] = XDIRECT ? xd[ps] : lds_f4(xs_q + (row[ps] >> xsh) * 128);
-#pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) t1v[ps] = lds_f4(t1s_q + row[ps] * 128);
-        if (tid == 0) trace_ev(p, 0, ptn, 6);
-        {
-          // one wait for the chunk's three slots: the MMA issuer commits them in order, so the last one being free
-          // implies the other two (each mbarrier wait is a ~200-cycle round trip on the critical path of the chunk)
-          uint32_t s2 = slot + 2, p2 = spar;
-          if (s2 >= (uint32_t)NS) {
-            s2 -= (uint32_t)NS;
-            p2 ^= 1u;
-          }
-          mbar_wait(smem_u32(b_ab_empty + s2), p2 ^ 1u, abort_flag, p.status, 10);
+      for (int ps = 0; ps < RPT; ++ps) t1v[ps] = lds_f4(t1s_q + row[ps] * 128);
+      if (tid == 0) trace_ev(p, 0, ptn, 6);
+      {
+        // one wait for the chunk's three slots: the MMA issuer commits them in order, so the last one being free
+        // implies the other two (each mbarrier wait is a ~200-cycle round trip on the critical path of the chunk)
+        uint32_t s2 = slot + 2, p2 = spar;
+        if (s2 >= (uint32_t)NS) {
+          s2 -= (uint32_t)NS;
+          p2 ^= 1u;
         }
-        emit(x);
-        emit(t1v);
-#pragma unroll
-        for (int ps = 0; ps < RPT; ++ps) t2[ps] = cheb_t2(t2[ps], x[ps]);
-        emit(t2);
+        mbar_wait(smem_u32(b_ab_empty + s2), p2 ^ 1u, abort_flag, p.status, 10);
       }
-      if (NS >= 3) {
-        fence_async_proxy();
-        __syncwarp();
-        if ((tid & 31) == 0) {
+      emit(xd);
+      emit(t1v);
 #pragma unroll
-          for (int k = 0; k < 3; ++k) mbar_arrive(smem_u32(b_ab_full + (slot0 + k) % NS));  // one arrival per warp
-        }
+      for (int ps = 0; ps < RPT; ++ps) t2[ps] = cheb_t2(t2[ps], xd[ps]);
+      emit(t2);
+      fence_async_proxy();
+      __syncwarp();
+      if ((tid & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) mbar_arrive(smem_u32(b_ab_full + (slot0 + k) % NS));  // one arrival per warp
       }
       if (tid == 0) trace_ev(p, 0, ptn, 7);
       producer_barrier<NPW * 32>();  // everybody is done with Xs[xs] and T1s
@@ -1263,17 +1262,38 @@ __device__ __forceinline__ uint64_t make_desc_sw128_mn(uint32_t saddr, uint32_t 
 constexpr int DW_NS = 3;
 constexpr int DW_G_BYTES = 4 * A_BLOCK_BYTES;  // dz tile: (hi, lo) x two 64-channel groups
 
+// k_cheb_dw_umma<XS> on the level's 128-row tiles (at most max_h1 staged rows, blobs meta_stride bytes apart)
+struct DwSmem {
+  size_t gblk, xs, t1s, t1_stage, meta, bars, flags, bytes;
+};
+__host__ __device__ __forceinline__ DwSmem dw_smem(int XS, int max_h1, int meta_stride) {
+  size_t at = 0;
+  auto take = [&](size_t bytes) { at += bytes; return at - bytes; };
+  DwSmem L;
+  take(DW_NS * A_BLOCK_BYTES);                // the ring at offset 0: [DW_NS] T blocks
+  L.gblk = take(DW_G_BYTES);                  // dz tile blocks: hi g0, hi g1, lo g0, lo g1
+  L.xs = take(XS * (size_t)TILE_M * FC * 4);  // [XS][128][32] fp32: the tile's own rows of x
+  L.t1_stage = (size_t)max_h1 * FC;           // [XS][max_h1][32] fp32: T1 rows of the tile and its 1-hop halo
+  L.t1s = take(XS * L.t1_stage * 4);
+  L.meta = take(2 * (size_t)meta_stride);        // [2] tile metadata blobs
+  L.bars = take(8 * (2 * DW_NS + 2 * XS + 6));  // the kernel's barrier map
+  L.flags = take(16);                            // word 1: the CTA's abort flag
+  L.bytes = at + 1024 + 32;
+  return L;
+}
+
 template <int XS>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
+  const DwSmem L = dw_smem(XS, p.max_h1, p.meta_stride);
   unsigned char* ring = smem_raw;                      // [DW_NS] T blocks
-  unsigned char* gblk = ring + DW_NS * A_BLOCK_BYTES;  // dz tile blocks: hi g0, hi g1, lo g0, lo g1
-  float* Xs = reinterpret_cast<float*>(gblk + DW_G_BYTES);  // [XS][128][32] the tile's own rows of x
+  unsigned char* gblk = smem_raw + L.gblk;
+  float* Xs = reinterpret_cast<float*>(smem_raw + L.xs);
   constexpr size_t xs_stage_floats = (size_t)TILE_M * FC;
-  float* T1s = Xs + XS * xs_stage_floats;                   // [XS][max_h1][32]
-  const size_t t1_stage_floats = (size_t)p.max_h1 * FC;
-  unsigned char* meta_s = reinterpret_cast<unsigned char*>(T1s + XS * t1_stage_floats);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(meta_s + 2 * (size_t)p.meta_stride);
+  float* T1s = reinterpret_cast<float*>(smem_raw + L.t1s);
+  const size_t t1_stage_floats = L.t1_stage;
+  unsigned char* meta_s = smem_raw + L.meta;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + L.bars);
   uint64_t* b_t_full = bars;                 // [DW_NS]
   uint64_t* b_t_empty = b_t_full + DW_NS;    // [DW_NS]
   uint64_t* b_x_full = b_t_empty + DW_NS;    // [XS]
@@ -1282,7 +1302,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
   uint64_t* b_m_empty = b_m_full + 2;        // [2]
   uint64_t* b_g_full = b_m_empty + 2;        // [1]
   uint64_t* b_g_empty = b_g_full + 1;        // [1]
-  uint32_t* flags = reinterpret_cast<uint32_t*>(b_g_empty + 1);
+  uint32_t* flags = reinterpret_cast<uint32_t*>(smem_raw + L.flags);
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -1414,9 +1434,9 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
         wg_fence();
 #pragma unroll
         for (int ks = 0; ks < 8; ++ks) {  // 16 mesh rows per K step = 2048 bytes = +128 in the address field
-          wgmma_m64n32<1, 1>(acc[k], dh + ks * 128, dt + ks * 128);      // g_hi T_hi
-          wgmma_m64n32<1, 1>(acc[k], dl + ks * 128, dt + ks * 128);      // g_lo T_hi
-          wgmma_m64n32<1, 1>(acc[k], dh + ks * 128, dt + ks * 128 + 4);  // g_hi T_lo (+64 B)
+          wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 128);      // g_hi T_hi
+          wgmma_m64n32(acc[k], dl + ks * 128, dt + ks * 128);      // g_lo T_hi
+          wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 128 + 4);  // g_hi T_lo (+64 B)
         }
         wg_commit();
         wg_wait0();
@@ -1584,13 +1604,24 @@ struct T1Params {
   float* t1;
 };
 
+// k_cheb_t1<T1_STAGES>: the tile's metadata blob at offset 0, then [T1_STAGES][max_h1][32] fp32 X rows of the tile and
+// its 1-hop halo, and 16 bytes of slack
+struct T1Smem {
+  size_t xs, stage, bytes;
+};
+__host__ __device__ __forceinline__ T1Smem t1_smem(int T1_STAGES, int max_h1, int meta_stride) {
+  const size_t stage = (size_t)max_h1 * FC;
+  return {(size_t)meta_stride, stage, meta_stride + T1_STAGES * stage * 4 + 16};
+}
+
 // T1_STAGES = cp.async ring depth (chunks in flight per CTA): 4 when two CTAs of that size fit an SM, else 3 or 2
 template <int T1_STAGES>
 __global__ void __launch_bounds__(512, 2) k_cheb_t1(const T1Params p) {
   extern __shared__ __align__(16) unsigned char smem_t1[];
+  const T1Smem L = t1_smem(T1_STAGES, p.max_h1, p.meta_stride);
   unsigned char* meta_s = smem_t1;
-  float* Xs = reinterpret_cast<float*>(smem_t1 + p.meta_stride);  // [T1_STAGES][max_h1][32]
-  const size_t stage_floats = (size_t)p.max_h1 * FC;
+  float* Xs = reinterpret_cast<float*>(smem_t1 + L.xs);
+  const size_t stage_floats = L.stage;
   const int tid = threadIdx.x, q = tid & 7, rg = tid >> 3;
   const int tile = blockIdx.x;
   const int b = tile / p.P, pat = tile - b * p.P;
@@ -1706,23 +1737,6 @@ int launch_pack(const PackSrc& src, long long n_blocks, void* out, cudaStream_t 
   return P2M_OK;
 }
 
-// debug: P2M_UMMA_TMA=0 stages every row with cp.async (A/B measurements of the TMA own-row loads)
-const bool g_umma_tma = [] { const char* e = std::getenv("P2M_UMMA_TMA"); return !(e && e[0] == '0'); }();
-
-// per-warp epilogue staging: one 32 x 32 sub-slab per warp (N = 64), a warp's whole 16 x 128 block in 16 padded linear
-// rows (N = 128)
-inline int epi_stage_bytes(int N) { return N == 128 ? 4 * 16 * STG_ROW_BYTES : 4 * 32 * 32 * 4; }
-// Dynamic shared memory of a conv configuration: T1 given (MODE 1: the tile's own X rows and the T1 rows of the tile
-// and its 1-hop halo per stage) or plain (MODE 0: the own X rows per stage).  N = 128: the 64-row configuration (64-row
-// tiles; with a given T1 and NS >= 3 no X stage: the producers read X directly).  The dense GEMM has no tile metadata.
-size_t smem_bytes_for(int N, int NS, int XS, const TileBlobs& t, bool t1_given) {
-  const int tm = N == 128 ? 64 : TILE_M;
-  const size_t fixed = 1024 + (size_t)NS * (tm * 128 + N * 128) + 8 * (2 * NS + 2 * XS + 8) + 16 +
-                       2 * (size_t)N * 4 + 16 + 128 + (size_t)epi_stage_bytes(N) + 4 * 32 * 4 +
-                       (N == 64 ? 64 * 12 * 4 : 4 * 8);  // fused-head weights (N = 64) / residual mbarriers (N = 128)
-  const size_t xs_rows = (t1_given && N == 128 && NS >= 3) ? 0 : (size_t)tm;
-  return fixed + (size_t)XS * (xs_rows + (t1_given ? t.max_h1 : 0)) * FC * 4 + 2 * (size_t)t.stride;
-}
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 constexpr int CONV_N = 64;  // output columns per CTA of the 128-row conv configuration (one column slice)
 constexpr int WIDE_N = 128; // ... and of the 64-row configuration (convs with Fout % 128 == 0)
@@ -1742,7 +1756,7 @@ struct ConvCfg {
 ConvCfg conv_cfg(int N, const TileBlobs& t, bool t1_given) {
   for (int ns = N == WIDE_N ? 6 : 3; ns >= 3; ns -= 3)
     for (int xs = 2; xs >= 1; --xs)
-      if (smem_bytes_for(N, ns, xs, t, t1_given) <= SMEM_LIMIT) return {ns, xs};
+      if (conv_smem(N, ns, xs, t1_given, t.max_h1, t.stride).bytes <= SMEM_LIMIT) return {ns, xs};
   return {0, 0};
 }
 
@@ -1806,7 +1820,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   constexpr int TM = tile_rows<N>();
   const DevLevel& g = *a.g;
   const TileBlobs& t = conv_tiles(N, g, a.tiles);
-  const size_t smem = smem_bytes_for(N, NS, XS, t, !a.plain);
+  const size_t smem = conv_smem(N, NS, XS, !a.plain, t.max_h1, t.stride).bytes;
   auto kern = a.plain ? conv_kernel<N, NS, XS, 0>() : conv_kernel<N, NS, XS, 1>();
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   P2M_TRY((a.plain ? check_launch_regs<N, NS, XS, 0>() : check_launch_regs<N, NS, XS, 1>()));
@@ -1853,7 +1867,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.tma = 0;
   std::memset(&p.tm_x, 0, sizeof(p.tm_x));
   std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
-  if (a.tiles == nullptr && g.V % TILE_M == 0 && g_umma_tma) {
+  if (a.tiles == nullptr && g.V % TILE_M == 0) {
     const long long rows = (long long)a.batch * g.V;
     bool ok = make_row_tmap(&p.tm_x, a.x, a.in_unpool ? rows / 2 : rows, a.fin, a.in_unpool ? TM / 2 : TM);
     if (ok && a.t1 != nullptr) ok = make_row_tmap(&p.tm_t1, a.t1, rows, a.fin, TM);
@@ -2062,18 +2076,13 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
 }
 
 
-size_t dw_smem_bytes(int XS, const DevLevel& g) {
-  return 1024 + (size_t)DW_NS * A_BLOCK_BYTES + DW_G_BYTES + (size_t)XS * (TILE_M + g.meta128.max_h1) * FC * 4 +
-         2 * (size_t)g.meta128.stride + 8 * (2 * DW_NS + 2 * XS + 8) + 32;
-}
-
 bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width) {
   if (g.meta128.n_pattern <= 0 || g.meta128.max_h1 > 256) return false;
   if (gathered_width % FC != 0 || gathered_width < FC || gathered_width > 256) return false;
   if (plain_width != 64 && plain_width != 128 && plain_width != 256) return false;
-  return dw_smem_bytes(1, g) <= SMEM_LIMIT;
+  return dw_smem(1, g.meta128.max_h1, g.meta128.stride).bytes <= SMEM_LIMIT;
 }
-int umma_dw_x_stages(const DevLevel& g) { return dw_smem_bytes(2, g) <= SMEM_LIMIT ? 2 : 1; }
+int umma_dw_x_stages(const DevLevel& g) { return dw_smem(2, g.meta128.max_h1, g.meta128.stride).bytes <= SMEM_LIMIT ? 2 : 1; }
 
 int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_unpool, int gathered_width,
                    const float* t1, const float* plain, int g_unpool, int plain_width, int swap, const float* a_scale,
@@ -2105,13 +2114,13 @@ int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_u
   p.tma = 0;
   std::memset(&p.tm_x, 0, sizeof(p.tm_x));
   std::memset(&p.tm_t1, 0, sizeof(p.tm_t1));
-  if (g.V % TILE_M == 0 && !in_unpool && g_umma_tma) {
+  if (g.V % TILE_M == 0 && !in_unpool) {
     const long long rows = (long long)batch * g.V;
     p.tma = (make_row_tmap(&p.tm_x, gathered, rows, gathered_width, TILE_M) &&
              make_row_tmap(&p.tm_t1, t1, rows, gathered_width, TILE_M)) ? 1 : 0;
   }
   const int xs = umma_dw_x_stages(g);
-  const size_t smem = dw_smem_bytes(xs, g);
+  const size_t smem = dw_smem(xs, t.max_h1, t.stride).bytes;
   auto kern = (xs == 2) ? k_cheb_dw_umma<2> : k_cheb_dw_umma<1>;
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = std::min(p.n_tiles, sm_count);
@@ -2138,10 +2147,10 @@ int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, 
     set_error("cheb_t1: halo too large");
     return P2M_ERR_INVALID;
   }
-  auto smem_for = [&](int stages) { return (size_t)t.stride + stages * (size_t)t.max_h1 * FC * 4 + 16; };
   const size_t half_sm = (228 * 1024) / 2 - 1024;  // two CTAs per SM (1 KB per CTA is reserved by the system)
-  const int stages = smem_for(4) <= half_sm ? 4 : (smem_for(3) <= half_sm ? 3 : 2);
-  const size_t smem = smem_for(stages);
+  int stages = 4;
+  while (stages > 2 && t1_smem(stages, t.max_h1, t.stride).bytes > half_sm) --stages;
+  const size_t smem = t1_smem(stages, t.max_h1, t.stride).bytes;
   auto kern = stages == 4 ? k_cheb_t1<4> : (stages == 3 ? k_cheb_t1<3> : k_cheb_t1<2>);
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   T1Params p;
@@ -2169,7 +2178,8 @@ bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
   if (fout != 64 && fout != 128 && fout != 256) return false;
   const int N = conv_n(fout);
   const TileBlobs& t = conv_tiles(N, g, nullptr);
-  return t.n_pattern > 0 && smem_bytes_for(N, 3, 1, t, true) <= SMEM_LIMIT && smem_bytes_for(N, 3, 1, t, false) <= SMEM_LIMIT;
+  return t.n_pattern > 0 && conv_smem(N, 3, 1, 1, t.max_h1, t.stride).bytes <= SMEM_LIMIT &&
+         conv_smem(N, 3, 1, 0, t.max_h1, t.stride).bytes <= SMEM_LIMIT;
 }
 
 // X staging depth launch_n picks for a conv of Fout columns on the level's consecutive tiles (T1 given, or plain)
@@ -2177,7 +2187,7 @@ int umma_conv_x_stages(const DevLevel& g, int fout, bool plain) {
   const int N = conv_n(fout);
   return conv_cfg(N, conv_tiles(N, g, nullptr), !plain).xs;
 }
-bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && g_umma_tma && tmap_encoder() != nullptr; }
+bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && tmap_encoder() != nullptr; }
 
 size_t umma_plain_pack_bytes(int N, int K) { return (size_t)(K / FC) * N * 128; }
 
@@ -2192,7 +2202,7 @@ namespace {
 template <int N>
 int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
   constexpr int NS = 3;
-  const size_t smem = smem_bytes_for(N, NS, 1, TileBlobs(), false);
+  const size_t smem = conv_smem(N, NS, 1, 0, 0, 0).bytes;  // no tile metadata
   auto kern = conv_kernel<N, NS, 1, 0>();
   P2M_TRY((check_launch_regs<N, NS, 1, 0>()));
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
