@@ -115,6 +115,38 @@ int p2m_debug_set_dedup_padding(p2m_model_t* m, int enable);
  * rows + 1-hop halo) per 128-row tile (0 when the level has no tensor-core metadata), out[8] = isolated rows that
  * padding elision would route to the dense path (0: elision not applicable).                                    */
 int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[9]);
+/* Debug: the paths the network schedules (p2m_meshnet_forward / _backward) take for layer `layer` at batch `batch`,
+ * from the same route decision the schedules make.  need_dx only matters for layer 0 (the network input's gradient).
+ * out[0] = forward conv on tensor cores, out[1] = its padding-vertex elision, out[2] = backward by the thin head's
+ * weights-first kernel, out[3] = dW on tensor cores from the basis of x, out[4] = ... from the basis of dz,
+ * out[5] = dX as a tensor-core conv on dz, out[6] = its padding-vertex elision, out[7] = dX by the three tensor-core
+ * dT GEMMs, out[8] = in eval mode this layer's epilogue computes the next (64 -> 3 head) layer's projections.      */
+int p2m_debug_layer_route(const p2m_model_t* m, int layer, int batch, int need_dx, int32_t out[9]);
+
+/* Debug capture of the network schedules' intermediate tensors.  Every pointer is device memory and nullable (a null
+ * array, or a null entry of one, is not written); the arrays hold one entry per layer (p2m_model_num_layers).  While
+ * a capture is set, the schedules copy into it on their stream (cudaMemcpyAsync), so the values are those of the
+ * latest call once the stream reaches that point.  Row-major [B * V_layer, F] like every activation.
+ *   training forward:  z[l] = conv output in front of the BatchNorm, a[l] = the layer's output (BatchNorm, ReLU,
+ *                      residual; layers without BatchNorm: nothing), fc_out = the fc's output [B, fc_out];
+ *   eval forward:      y[l] = the layer's output as written (not written for a layer whose output the fused head
+ *                      replaced by its projections), fc_out;
+ *   backward:          g_a[l] = gradient entering the layer's output, g_z[l] = gradient of the conv output (after
+ *                      the BatchNorm backward), dx[l] = gradient of the layer's input (after the unpool pair-sum and the
+ *                      residual; layer 0: only when the caller asks for dx), fc_dx = gradient of the fc's input.
+ * p2m_debug_set_capture copies the struct and the arrays; NULL clears the capture.  Without one the schedules issue
+ * exactly the launches they issue without this facility.                                                         */
+typedef struct {
+  float* const* z;
+  float* const* a;
+  float* const* y;
+  float* fc_out;
+  float* const* g_a;
+  float* const* g_z;
+  float* const* dx;
+  float* fc_dx;
+} p2m_capture_t;
+int p2m_debug_set_capture(p2m_model_t* m, const p2m_capture_t* capture);
 
 /* Bytes of device workspace p2m_meshnet_forward needs for batch B.  In training mode the workspace
  * also carries what p2m_meshnet_backward reads, so it must stay alive and untouched in between.   */

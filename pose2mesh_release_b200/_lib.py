@@ -84,6 +84,16 @@ class ConvBwdArgs(C.Structure):
     ]
 
 
+class Capture(C.Structure):
+    """p2m_capture_t: per-layer device buffers the network schedules copy their tensors into (p2m_debug_set_capture)."""
+    _fields_ = [
+        ("z", C.POINTER(C.c_void_p)), ("a", C.POINTER(C.c_void_p)), ("y", C.POINTER(C.c_void_p)),
+        ("fc_out", C.c_void_p),
+        ("g_a", C.POINTER(C.c_void_p)), ("g_z", C.POINTER(C.c_void_p)), ("dx", C.POINTER(C.c_void_p)),
+        ("fc_dx", C.c_void_p),
+    ]
+
+
 class PoseNetStage(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("w1_w", "w1_b", "w2_w", "w2_b", "bn1_w", "bn1_b", "bn1_rm", "bn1_rv",
                                           "bn2_w", "bn2_b", "bn2_rm", "bn2_rv")]
@@ -165,7 +175,7 @@ class H36MError(C.Structure):
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
-    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
+    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
     "p2m_posenet_train_workspace_bytes", "p2m_posenet_train_saved_bytes", "p2m_posenet_train_forward", "p2m_posenet_backward",
@@ -225,6 +235,10 @@ def load() -> C.CDLL:
         lib.p2m_debug_set_trace.restype = C.c_int
         lib.p2m_debug_conv_path.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
         lib.p2m_debug_conv_path.restype = C.c_int
+        lib.p2m_debug_layer_route.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
+        lib.p2m_debug_layer_route.restype = C.c_int
+        lib.p2m_debug_set_capture.argtypes = [vp, C.POINTER(Capture)]
+        lib.p2m_debug_set_capture.restype = C.c_int
         lib.p2m_debug_kernel_status.argtypes = [vp, c_int32_p]
         lib.p2m_debug_kernel_status.restype = C.c_int
         lib.p2m_meshnet_workspace_bytes.argtypes = [vp, C.c_int, C.c_int]

@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <tuple>
 #include <vector>
@@ -60,6 +61,13 @@ struct Block {
   InterpTable interp;  // valid when has_residual
 };
 
+// p2m_debug_set_capture: the caller's device buffers (one per layer, or none) the schedules copy their tensors into
+struct Capture {
+  std::vector<float*> z, a, y, g_a, g_z, dx;
+  float* fc_out = nullptr;
+  float* fc_dx = nullptr;
+};
+
 }  // namespace p2m
 
 using namespace p2m;
@@ -87,6 +95,7 @@ struct p2m_model {
                                  // computed (DevLevel::rep_tiles); needs elide_padding == 1 (p2m_debug_set_dedup_padding)
   int fuse_head = 1;             // eval: the 128 -> 64 conv's epilogue feeds the 64 -> 3 head directly (no 64-wide tensor)
   int profiling = 0;             // record a CUDA event pair around every conv layer of the eval forward
+  std::unique_ptr<Capture> capture;  // debug: copies of the schedules' tensors (p2m_debug_set_capture); null = none
   std::vector<cudaEvent_t> ev_beg, ev_end;
   std::vector<void*> owned;  // device allocations to free
 };
@@ -484,6 +493,29 @@ bool fuses_head(const p2m_model* m, const Block& blk, int li, int B, const ConvR
   return thin_conv_supported(H.fin, H.fout) && H.fin == L.fout && H.V == L.V;
 }
 
+// The route of layer li's backward in p2m_meshnet_backward: the thin head's weights-first backward needs an input that
+// is neither unpooled nor a residual source, and not the network input.
+ConvRoute backward_route(const p2m_model* m, int li, int B, bool need_dx) {
+  const Layer& L = m->layers[li];
+  int b = 0;
+  while (m->blocks[b].first_layer + m->blocks[b].n_layers <= li) ++b;
+  const Block& blk = m->blocks[b];
+  const bool first = (li == blk.first_layer);
+  const bool in_unpool = first && blk.in_unpool;
+  const bool res_here = first && blk.has_residual;
+  return conv_route(m, L.level, L.fin, L.fout, B, true, !in_unpool && !res_here && li > 0, need_dx);
+}
+
+// p2m_debug_set_capture: n floats of src into the capture slot v[li] / dst, if the caller set one
+int capture_copy(float* dst, const float* src, size_t n, cudaStream_t s) {
+  if (dst == nullptr) return P2M_OK;
+  P2M_CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return P2M_OK;
+}
+int capture_copy(const std::vector<float*>& v, int li, const float* src, size_t n, cudaStream_t s) {
+  return capture_copy(v.empty() ? nullptr : v[li], src, n, s);
+}
+
 // The default elision policy (elide_padding == 1) on a level, whatever the batch and width.
 inline bool policy_elided(const DevLevel& g) { return elided(1, g, g.V, 0); }
 
@@ -829,6 +861,52 @@ int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int3
   return P2M_OK;
 }
 
+int p2m_debug_layer_route(const p2m_model_t* m, int layer, int batch, int need_dx, int32_t out[9]) {
+  if (!m || !out || layer < 0 || layer >= (int)m->layers.size() || batch <= 0) {
+    set_error("debug_layer_route: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  const Layer& L = m->layers[layer];
+  int b = 0;
+  while (m->blocks[b].first_layer + m->blocks[b].n_layers <= layer) ++b;
+  const ConvRoute f = conv_route(m, L.level, L.fin, L.fout, batch, true);  // what forward_eval / forward_train run
+  const ConvRoute r = backward_route(m, layer, batch, layer > 0 || need_dx);
+  out[0] = f.tc;
+  out[1] = f.elide;
+  out[2] = r.thin;
+  out[3] = r.tc_dw;
+  out[4] = r.dw_dz_basis;
+  out[5] = r.tc_dx;
+  out[6] = r.dx_elide;
+  out[7] = r.tc_dt;
+  out[8] = fuses_head(m, m->blocks[b], layer, batch, f);
+  return P2M_OK;
+}
+
+int p2m_debug_set_capture(p2m_model_t* m, const p2m_capture_t* c) {
+  if (!m) {
+    set_error("debug_set_capture: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  if (!c) {
+    m->capture.reset();
+    return P2M_OK;
+  }
+  const size_t nl = m->layers.size();
+  auto take = [nl](float* const* p) { return p ? std::vector<float*>(p, p + nl) : std::vector<float*>(); };
+  std::unique_ptr<Capture> cap(new Capture());
+  cap->z = take(c->z);
+  cap->a = take(c->a);
+  cap->y = take(c->y);
+  cap->g_a = take(c->g_a);
+  cap->g_z = take(c->g_z);
+  cap->dx = take(c->dx);
+  cap->fc_out = c->fc_out;
+  cap->fc_dx = c->fc_dx;
+  m->capture = std::move(cap);
+  return P2M_OK;
+}
+
 int p2m_debug_set_fuse_head(p2m_model_t* m, int enable) {
   if (!m) return P2M_ERR_INVALID;
   m->fuse_head = enable ? 1 : 0;
@@ -967,6 +1045,8 @@ static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const float* x, f
                             iso_mode));
       }
       if (m->profiling) P2M_CUDA_OK(cudaEventRecord(m->ev_end[li], s));
+      if (m->capture && head_z == nullptr && !gathered)
+        P2M_TRY(capture_copy(m->capture->y, li, out, (size_t)rows * L.fout, s));
       cur = out;
       cur_buf = out_buf;
       cur_unpool = 0;
@@ -974,6 +1054,7 @@ static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const float* x, f
     if (b == 0) {
       cur_buf = free_rot(cur_buf, -1);
       P2M_TRY(run_fc(m, P, w, B, cur, w.rot[cur_buf], s));
+      if (m->capture) P2M_TRY(capture_copy(m->capture->fc_out, w.rot[cur_buf], (size_t)B * m->fc_out, s));
       cur = w.rot[cur_buf];
       cur_unpool = 0;
     } else if (blk.out_unpool) {
@@ -1012,11 +1093,16 @@ static int forward_train(p2m_model_t* m, const p2m_params_t* P, const float* x, 
                               P->bn_nbt ? P->bn_nbt[li] : nullptr, w.sums, w.mean[li], w.invstd[li], w.scale[li],
                               w.shift[li], L.relu, with_res ? block_in : nullptr, blk.cin, block_in_unpool,
                               with_res ? &blk.interp : nullptr, w.a[li], s));
+      if (m->capture && L.bn) {
+        P2M_TRY(capture_copy(m->capture->z, li, z, (size_t)B * L.V * L.fout, s));
+        P2M_TRY(capture_copy(m->capture->a, li, w.a[li], (size_t)B * L.V * L.fout, s));
+      }
       cur = L.bn ? w.a[li] : z;
       cur_unpool = 0;
     }
     if (b == 0) {
       P2M_TRY(run_fc(m, P, w, B, cur, w.fc_out, s));
+      if (m->capture) P2M_TRY(capture_copy(m->capture->fc_out, w.fc_out, (size_t)B * m->fc_out, s));
       cur = w.fc_out;
       cur_unpool = 0;
     } else if (blk.out_unpool) {
@@ -1175,7 +1261,8 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
       }
       const bool need_dx = !(li == 0 && dx == nullptr);
       const bool res_here = (j == 0) && blk.has_residual;
-      const ConvRoute r = conv_route(m, L.level, L.fin, L.fout, B, true, !in_unpool && !res_here && li > 0, need_dx);
+      const ConvRoute r = backward_route(m, li, B, need_dx);
+      if (m->capture) P2M_TRY(capture_copy(m->capture->g_a, li, g_cur, (size_t)rows * L.fout, s));
       const bool want_scale = r.tc_dw || r.tc_dx || r.tc_dt;
       bool have_scale = false;
       if (L.bn) {
@@ -1193,6 +1280,7 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
         P2M_TRY(launch_col_sum(g_z, rows, L.fout, sc.sums, G->cl_b[li], s));
       }
       if (want_scale && !have_scale) P2M_TRY(launch_absmax_scale(g_z, (long long)rows * L.fout, sc.a_scale, s));
+      if (m->capture) P2M_TRY(capture_copy(m->capture->g_z, li, g_z, (size_t)rows * L.fout, s));
       float* out = nullptr;
       int out_buf = -1;
       if (need_dx) {
@@ -1253,6 +1341,8 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
                                       res_here ? &blk.interp : nullptr, in_unpool, out, s));
       }
       if (need_dx) {
+        if (m->capture)  // (an unpooled input has half the layer's rows)
+          P2M_TRY(capture_copy(m->capture->dx, li, out, (size_t)(in_unpool ? rows / 2 : rows) * L.fin, s));
         g_cur = out;
         g_cur_buf = out_buf;
       }
@@ -1271,6 +1361,7 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
       P2M_TRY(launch_gemm(g_cur, m->fc_out, P->fc_w, m->fc_in, 1, sc.G[out_buf], m->fc_in, B, m->fc_in, m->fc_out, none, s));
       g_cur = sc.G[out_buf];
       g_cur_buf = out_buf;
+      if (m->capture) P2M_TRY(capture_copy(m->capture->fc_dx, g_cur, (size_t)B * m->fc_in, s));
     }
   }
   return P2M_OK;

@@ -112,6 +112,35 @@ class BakedHierarchy:
         if dedup_padding is not None:  # eval: one representative per class of identical isolated rows (default on)
             _lib.check(lib.p2m_debug_set_dedup_padding(h, int(dedup_padding)), "set_dedup_padding")
 
+    def set_capture(self, device_index: int, capture: Optional[dict] = None):
+        """Debug: copy the network schedules' intermediate tensors into device tensors (p2m_debug_set_capture).
+        ``capture`` maps the p2m_capture_t field names to a list with one tensor (or None) per layer for z, a, y, g_a,
+        g_z and dx, or to one tensor for fc_out and fc_dx; missing names are not captured.  None clears the capture.
+        The tensors must stay alive until the capture is cleared."""
+        lib, h = _lib.load(), self.handle(device_index)
+        if capture is None:
+            _lib.check(lib.p2m_debug_set_capture(h, None), "set_capture")
+            return
+        c = _lib.Capture()
+        keep = []
+        for name in ("z", "a", "y", "g_a", "g_z", "dx"):
+            if capture.get(name) is not None:
+                arr = _ptr_array(capture[name])
+                keep.append(arr)
+                setattr(c, name, arr)
+        for name in ("fc_out", "fc_dx"):
+            if capture.get(name) is not None:
+                setattr(c, name, capture[name].data_ptr())
+        _lib.check(lib.p2m_debug_set_capture(h, C.byref(c)), "set_capture")  # copies the arrays
+
+    def layer_route(self, device_index: int, layer: int, batch: int, need_dx: bool = True) -> dict:
+        """Debug: the paths the network schedules take for one layer (p2m_debug_layer_route)."""
+        out = (C.c_int32 * 9)()
+        _lib.check(_lib.load().p2m_debug_layer_route(self.handle(device_index), layer, batch, int(need_dx), out),
+                   "layer_route")
+        return dict(zip(("tc", "elide", "thin", "tc_dw", "dw_dz_basis", "tc_dx", "dx_elide", "tc_dt", "fuse_head"),
+                        (bool(v) for v in out)))
+
     def layer_info(self, device_index: int):
         lib = _lib.load()
         h = self.handle(device_index)

@@ -22,6 +22,13 @@ spacing 2^-24 bounds the absolute error of a lo part.  The operands enter the sp
 by a power of two (h = 0 for the weights, h = ceil(log2(2 r^2 + 1)) for the basis, r = max absolute row sum of L~),
 so the absolute error per operand entry is <= 2^(h-34) max|operand| and the floor is that times the other operand's
 absolute row sum.  It scales with the inputs: it is never an absolute constant.
+
+The network schedules (p2m_meshnet_forward / _backward) do not range-normalise every operand: the forward conv's
+activations and the x side of dW enter the split as they are, the weights at the fixed scale 2^6.  There a lo part's
+absolute error is <= 2^-25 (half of fp16's subnormal spacing) divided by that fixed scale (split="network" of the conv
+bounds).  Next to the normalised floor 2^-34 max|x| this dominates once max|x| < 2^9, but next to the relative term
+SPLIT |x| = 3 2^-22 |x| only where |x| falls below 2^-25 / SPLIT = 1/24 (about 2^-4.6): activations after a
+BatchNorm are O(1).
 """
 from __future__ import annotations
 
@@ -87,7 +94,13 @@ def cheb_conv_fwd(x, L, W, b=None) -> np.ndarray:
     return y.reshape(B, V, -1)
 
 
-def cheb_conv_fwd_bound(x, L, W, b, precision: str) -> np.ndarray:
+NET_LO = 2.0 ** -25       # network split: absolute error of one lo part of an operand entered as it is
+NET_W_SCALE = 64.0        # ... and the fixed scale the weights are packed at
+
+
+def cheb_conv_fwd_bound(x, L, W, b, precision: str, split: str = "normalised") -> np.ndarray:
+    """split: 'normalised' (the single-layer entry points: both operands scaled into fp16's range by powers of two) or
+    'network' (the network forward: activations unscaled, weights at the fixed 2^6)."""
     Labs = abs(sp.csr_matrix(L, dtype=np.float64))
     W = np.asarray(W, dtype=np.float64)
     x = np.asarray(x, dtype=np.float64)
@@ -102,9 +115,18 @@ def cheb_conv_fwd_bound(x, L, W, b, precision: str) -> np.ndarray:
     if b is not None:
         bound = bound + U32 * np.abs(np.asarray(b, dtype=np.float64))
     h = headroom_log2(L)
-    fl = (2.0 ** (h - 34) * float(ax.max(initial=0.0)) * np.abs(W).sum(axis=1)[None, :]
-          + 2.0 ** -34 * float(np.abs(W).max(initial=0.0)) * Ta.sum(axis=1, keepdims=True))
+    if split == "network":
+        fl = NET_LO * np.abs(W).sum(axis=1)[None, :] + NET_LO / NET_W_SCALE * Ta.sum(axis=1, keepdims=True)
+    else:
+        fl = (2.0 ** (h - 34) * float(ax.max(initial=0.0)) * np.abs(W).sum(axis=1)[None, :]
+              + 2.0 ** -34 * float(np.abs(W).max(initial=0.0)) * Ta.sum(axis=1, keepdims=True))
     return (bound + fl).reshape(B, V, -1)
+
+
+def _contract_rows(dz, T):
+    """sum_rows dz[:, o] T[:, k, f] -> [o, f*3 + k] (as one GEMM)."""
+    R, K, F = T.shape
+    return (dz.T @ T.reshape(R, K * F)).reshape(-1, K, F).transpose(0, 2, 1).reshape(-1, F * K)
 
 
 def cheb_conv_bwd(x, L, W, dz):
@@ -125,12 +147,16 @@ def cheb_conv_bwd(x, L, W, dz):
 
     dx = dT[0] - dT[2] + lt(dT[1] + 2 * lt(dT[2]))
     T = basis(x, L)                                       # [B, V, 3, F]
-    dW = np.einsum("ro,rkf->ofk", dzf, T.reshape(B * V, 3, F)).reshape(fout, 3 * F)
+    dW = _contract_rows(dzf, T.reshape(B * V, 3, F))
     db = dzf.sum(axis=0)
     return dx, dW, db
 
 
-def cheb_conv_bwd_bound(x, L, W, dz, precision: str):
+def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised"):
+    """Bounds (dx, dW, db) of cheb_conv_bwd.  split: see cheb_conv_fwd_bound; in the network backward dz is scaled into
+    fp16's range by a power of two (floor 2^-34 max|dz| per entry), the weights are at the fixed 2^6 and the x side of
+    dW is unscaled.  dX there is either the dT GEMMs + the basis backward or a conv on dz ([dz | L dz | T2 dz] against
+    the transposed weights), dW either on the basis of x or on the basis of dz: the floor is the larger of the two."""
     Labs = abs(sp.csr_matrix(L, dtype=np.float64))
     W = np.abs(np.asarray(W, dtype=np.float64))
     adz = np.abs(np.asarray(dz, dtype=np.float64))
@@ -150,19 +176,36 @@ def cheb_conv_bwd_bound(x, L, W, dz, precision: str):
     dzf = adz.reshape(B * V, fout)
     A = [(dzf @ Wk[:, :, k]).reshape(B, V, F) for k in range(3)]
     mdz, mw = float(adz.max(initial=0.0)), float(W.max(initial=0.0))
-    Fl = [(2.0 ** -34 * (mdz * Wk[:, :, k].sum(axis=0)[None, :] + mw * dzf.sum(axis=1, keepdims=True))).reshape(B, V, F)
+    e_dz = 2.0 ** -34 * mdz
+    e_w = NET_LO / NET_W_SCALE if split == "network" else 2.0 ** -34 * mw
+    Fl = [(e_dz * Wk[:, :, k].sum(axis=0)[None, :] + e_w * dzf.sum(axis=1, keepdims=True)).reshape(B, V, F)
           for k in range(3)]
+    fl_dx = prop(*Fl)
+    if split == "network":   # the conv on dz: e_dz per entry of its basis, e_w per weight
+        Tdz = basis(adz, Labs)
+        Tdz[:, :, 2] += 2 * adz
+        conv_fl = (e_dz * Wk.sum(axis=(0, 2))[None, :] + e_w * Tdz.reshape(B * V, -1).sum(axis=1, keepdims=True))
+        fl_dx = np.maximum(fl_dx, conv_fl.reshape(B, V, F))
     g_dx = gamma(fout, precision, deg)
-    b_dx = g_dx * prop(*A) + prop(*Fl)
+    b_dx = g_dx * prop(*A) + fl_dx
     # dW: contraction over all B*V rows of |dz| and the absolute basis
     Tabs = basis(ax, Labs)
     Tabs[:, :, 2] += 2 * ax
     Tf = Tabs.reshape(B * V, 3, F)
     R = B * V
     g_dw = gamma(R, precision, deg) + (R.bit_length() * U32)   # + the cross-CTA fp32 atomic adds (log-depth tree)
-    b_dw = g_dw * np.einsum("ro,rkf->ofk", dzf, Tf).reshape(fout, 3 * F)
-    fl_dw = (2.0 ** -34 * mdz * np.einsum("rkf->fk", Tf).reshape(1, 3 * F)
-             + 2.0 ** (h - 34) * float(ax.max(initial=0.0)) * dzf.sum(axis=0)[:, None])
+    b_dw = g_dw * _contract_rows(dzf, Tf)
+    if split == "network":
+        Tdz = basis(adz, Labs)
+        Tdz[:, :, 2] += 2 * adz
+        Tdz = Tdz.reshape(B * V, 3, fout)
+        on_x = e_dz * np.einsum("rkf->fk", Tf).reshape(1, 3 * F) + NET_LO * dzf.sum(axis=0)[:, None]
+        on_dz = (e_dz * np.repeat(ax.reshape(B * V, F).sum(axis=0), 3)[None, :]
+                 + NET_LO * np.einsum("rko->ok", Tdz)[:, None, :].repeat(F, axis=1).reshape(fout, 3 * F))
+        fl_dw = np.maximum(on_x, on_dz)
+    else:
+        fl_dw = (2.0 ** -34 * mdz * np.einsum("rkf->fk", Tf).reshape(1, 3 * F)
+                 + 2.0 ** (h - 34) * float(ax.max(initial=0.0)) * dzf.sum(axis=0)[:, None])
     b_db = 2 * U32 * dzf.sum(axis=0)
     return b_dx, b_dw + fl_dw, b_db
 
@@ -254,6 +297,17 @@ def bn_eval_fwd(z, gamma, beta, rm, rv, relu=False, eps=BN_EPS):
     return np.maximum(y, 0.0) if relu else y
 
 
+def col_sum_bound(g) -> np.ndarray:
+    """Bound on k_col_sum (the bias gradient of a layer without BatchNorm) over the rows of g [..., F]: the layout of
+    the statistics sums (stat_allowance), bounded worst-case, (m + rl) u sum |g|, not probabilistically: the L1 loss's
+    gradient has entries of one magnitude and sign pattern, whose rounding errors do not average out."""
+    gr = _rows(g)
+    n, F = gr.shape
+    rl = 256 // min(F, 256)
+    m = min(n, -(-STAT_ROWS // rl))
+    return (m + rl) * U32 * np.abs(gr).sum(axis=0) + U32 * np.abs(gr.sum(axis=0))
+
+
 def stat_allowance(n: int, F: int) -> float:
     """Relative rounding allowance of one fp32 statistics sum (k_col_stats): a block of 256 threads splits into
     rl = 256 / min(F, 256) row lanes, each sums <= ceil(STAT_ROWS / rl) rows in fp32, the lanes are added in fp32 and
@@ -317,6 +371,137 @@ def bn_eval_fwd_bound(z, E, gamma, beta, rm, rv, bias, eps=BN_EPS):
     return ey.reshape(np.shape(z))
 
 
+def bn_train_bwd(z, g_a, gamma, beta, relu=False, eps=BN_EPS):
+    """Backward of train-mode BatchNorm1d (+ ReLU) over the rows of z [..., F] from the gradient g_a of its output, with
+    the exact batch statistics of z.  Returns (g_z, dgamma, dbeta, mask): g' = g_a [bn(z) > 0],
+    g_z = gamma invstd (g' - mean(g') - zhat mean(g' zhat)), dgamma = sum g' zhat, dbeta = sum g'."""
+    zr, gr = _rows(z), _rows(g_a)
+    mean = zr.mean(axis=0)
+    invstd = 1.0 / np.sqrt(((zr - mean) ** 2).mean(axis=0) + eps)
+    zh = (zr - mean) * invstd
+    pre = zh * np.asarray(gamma, np.float64) + np.asarray(beta, np.float64)
+    mask = pre > 0 if relu else np.ones_like(pre, bool)
+    g = np.where(mask, gr, 0.0)
+    m1, m2 = g.mean(axis=0), (g * zh).mean(axis=0)
+    g_z = np.asarray(gamma, np.float64) * invstd * (g - m1 - zh * m2)
+    return g_z.reshape(np.shape(z)), (g * zh).sum(axis=0), g.sum(axis=0), pre.reshape(np.shape(z))
+
+
+def bn_train_bwd_bound(z, g_a, gamma, beta, relu=False, eps=BN_EPS):
+    """Element-wise bounds (g_z, dgamma, dbeta) on launch_bn_relu_bwd given the exact z and g_a it read (the captured
+    fp32 tensors) and the fp32 mean / invstd the forward saved (bn_train_fwd_bound's bounds with E = 0: the error of
+    the statistics sums plus the backward error of z's fp32 storage, u |z|).
+
+    First order, with zhat = (z - mean) invstd, a = gamma invstd, m1 = mean(g'), m2 = mean(g' zhat):
+      zhat:  |z - mean| e_is + invstd e_mean + 2 u |zhat|                  (the saved statistics; z - mean, the product)
+      m1, m2: the sums in the blocks of k_bn_bwd_reduce (stat_allowance), the fp64 division's final rounding
+      g_z:   e_a |g' - m1 - zhat m2| + |a| (e_m1 + |m2| e_zhat + |zhat| e_m2) + the evaluation's own roundings.
+    Those roundings cover both forms of the kernel: the scalar k_bn_bwd_apply (a (g' - m1 - zhat m2): 5 roundings) and
+    the affine k_bn_bwd_coef + k_bn_bwd_apply4, g_z = fma(a, g', fma(b, z, c)) with b = -a invstd m2 and
+    c = -a m1 + a invstd m2 mean, whose b z + c cancels to a invstd m2 (mean - z): its coefficients' roundings
+    (3 u in b, 4 u in c) are relative to |a invstd m2| |z| and |a invstd m2 mean|, i.e. a backward error of ~3 u (|z| +
+    |mean|) in z, which is large next to |zhat| where the channel's mean / sigma is large."""
+    zr, gr = _rows(z), _rows(g_a)
+    n, F = zr.shape
+    gam = np.asarray(gamma, np.float64)
+    g_z, dgam, dbet, pre = bn_train_bwd(z, g_a, gamma, beta, relu, eps)
+    pre = _rows(pre)
+    st = bn_train_fwd_bound(zr, np.zeros_like(zr), gamma, beta, np.zeros(F), np.zeros(F), eps=eps)
+    mean = zr.mean(axis=0)
+    invstd = 1.0 / np.sqrt(((zr - mean) ** 2).mean(axis=0) + eps)
+    zh = (zr - mean) * invstd
+    g = np.where(pre > 0, gr, 0.0) if relu else gr
+    ag = np.abs(g)
+    a = np.abs(gam) * invstd
+    e_a = np.abs(gam) * st["invstd"] + U32 * a
+    e_zh = np.abs(zr - mean) * st["invstd"] + invstd * st["mean"] + 2 * U32 * np.abs(zh)
+    al = stat_allowance(n, F)
+    m1, m2 = g.mean(axis=0), (g * zh).mean(axis=0)
+    e_m1 = al * ag.mean(axis=0) + U32 * np.abs(m1)
+    e_m2 = al * (ag * np.abs(zh)).mean(axis=0) + (ag * e_zh).mean(axis=0) + U32 * np.abs(m2)
+    inner = np.abs(g - m1 - zh * m2)
+    e_gz = (e_a * inner + a * (e_m1 + np.abs(m2) * e_zh + np.abs(zh) * e_m2)
+            + U32 * (5 * a * (ag + np.abs(m1) + np.abs(zh * m2)) + 4 * a * invstd * np.abs(m2) * (np.abs(zr) + np.abs(mean))
+                     + 2 * np.abs(g_z.reshape(n, F))))
+    e_dbeta = al * ag.sum(axis=0) + U32 * np.abs(dbet)
+    e_dgamma = al * (ag * np.abs(zh)).sum(axis=0) + (ag * e_zh).sum(axis=0) + U32 * np.abs(dgam)
+    return e_gz.reshape(np.shape(z)), e_dgamma, e_dbeta
+
+
+# --------------------------------------------------------------------------------------------- network glue
+def unpool(x):
+    """Nearest x2 unpool along the vertex axis of [B, V, F] (row r reads row r >> 1; meshnet.py:71-78)."""
+    return np.repeat(np.asarray(x, np.float64), 2, axis=1)
+
+
+def unpool_t(g):
+    """Transpose of unpool: the pair-sum of rows 2r and 2r + 1."""
+    g = np.asarray(g, np.float64)
+    B, V, F = g.shape
+    return g.reshape(B, V // 2, 2, F).sum(axis=2)
+
+
+def resample_matrix(fin: int, fout: int, dtype=np.float64) -> np.ndarray:
+    """M [fout, fin] of F.interpolate(size=fout, mode='linear', align_corners=False) along the channel axis
+    (oracle.meshnet_oracle.channel_resample): src = (j + 0.5) fin / fout - 0.5 clamped at 0, taps floor(src) and the
+    next one (clamped at fin - 1), weights 1 - lam, lam.  dtype=np.float32 gives the table the library builds."""
+    M = np.zeros((fout, fin), np.float64)
+    scale = dtype(fin) / dtype(fout)
+    for j in range(fout):
+        src = max(dtype(scale * (dtype(j) + dtype(0.5)) - dtype(0.5)), dtype(0))
+        a = min(int(src), fin - 1)
+        b = a + (1 if a < fin - 1 else 0)
+        lam = float(dtype(src - dtype(a)))
+        M[j, a] += 1 - lam
+        M[j, b] += lam
+    return M
+
+
+def channel_resample(x, fout: int):
+    x = np.asarray(x, np.float64)
+    return x if x.shape[-1] == fout else x @ resample_matrix(x.shape[-1], fout).T
+
+
+def channel_resample_t(g, fin: int):
+    g = np.asarray(g, np.float64)
+    return g if g.shape[-1] == fin else g @ resample_matrix(fin, g.shape[-1])
+
+
+def channel_resample_bound(x, fout: int):
+    """fp32 evaluation of the resample, fma((1 - lam), x_a, lam x_b), against the float64 one: the table's fp32 lam (exact
+    when fin / fout is a power of two) and two roundings of the weighted sum."""
+    x = np.asarray(x, np.float64)
+    fin = x.shape[-1]
+    if fin == fout:
+        return np.zeros_like(x)
+    M, M32 = resample_matrix(fin, fout), resample_matrix(fin, fout, np.float32)
+    return np.abs(x) @ (np.abs(M - M32) + 3 * U32 * np.abs(M)).T
+
+
+def channel_resample_t_bound(g, fin: int):
+    """The transposed resample (k_dx_finish, k_basis_bwd_dx: fma over the taps of each input channel, at most
+    max_taps of them) against float64."""
+    g = np.asarray(g, np.float64)
+    fout = g.shape[-1]
+    if fin == fout:
+        return np.zeros_like(g)
+    M, M32 = resample_matrix(fin, fout), resample_matrix(fin, fout, np.float32)
+    taps = int((M32 != 0).sum(axis=0).max())
+    return np.abs(g) @ (np.abs(M - M32) + (taps + 1) * U32 * np.abs(M))
+
+
+def thin_head_fused_bound(y_in, E_in, L, W):
+    """First-order propagation of an error E_in of the head's input y_in through the 64 -> 3 head (the fused eval head:
+    the previous layer's epilogue forms Z = act(y) W' from its fp32 y): |T|(E_in) |W|^T, the head's own fp32 bound
+    added by the caller."""
+    Labs = abs(sp.csr_matrix(L, dtype=np.float64))
+    E_in = np.asarray(E_in, np.float64)
+    T = basis(E_in, Labs)
+    T[:, :, 2] += 2 * E_in
+    B, V, _ = E_in.shape
+    return (_flat(T) @ np.abs(np.asarray(W, np.float64)).T).reshape(B, V, -1)
+
+
 # --------------------------------------------------------------------------------------------- emulators (bound teeth)
 def _f16_split(v: np.ndarray):
     hi = v.astype(np.float16).astype(np.float64)
@@ -339,7 +524,8 @@ def _tf32(v: np.ndarray) -> np.ndarray:
     return b.view(np.float32).astype(np.float64)
 
 
-def emulate_cheb_conv(x, L, W, b=None, mode: str = "fp16x3", drop_block: int = -1) -> np.ndarray:
+def emulate_cheb_conv(x, L, W, b=None, mode: str = "fp16x3", drop_block: int = -1,
+                      split: str = "normalised") -> np.ndarray:
     """What a tensor-core kernel of the given arithmetic returns for the conv: the basis in fp32, the operands scaled
     by powers of two into fp16's range (h of headroom for the basis), then
       'fp16x3'    hi*hi + lo*hi + hi*lo
@@ -347,7 +533,8 @@ def emulate_cheb_conv(x, L, W, b=None, mode: str = "fp16x3", drop_block: int = -
       'tf32'      both operands rounded to TF32
     accumulated in fp32 over K (sequentially, products of one k summed in float64 first: a slightly better accumulator
     than the tensor core's).  drop_block >= 0 removes the lo*hi products of the 32 consecutive K-columns (of the
-    kernel's [k][fin] operand order) that make up K-block `drop_block`."""
+    kernel's [k][fin] operand order) that make up K-block `drop_block`.  split='network': the network forward's
+    operands, the basis as it is and the weights at the fixed 2^6."""
     L = sp.csr_matrix(L, dtype=np.float32)
     x32 = np.asarray(x, np.float32)
     B, V, F = x32.shape
@@ -358,8 +545,11 @@ def emulate_cheb_conv(x, L, W, b=None, mode: str = "fp16x3", drop_block: int = -
     T = np.concatenate([a.reshape(V, B, F).transpose(1, 0, 2) for a in (xf, t1, t2)], axis=2).reshape(B * V, 3 * F)
     T = T.astype(np.float64)
     Wp = np.asarray(W, np.float64).reshape(-1, F, 3).transpose(0, 2, 1).reshape(-1, 3 * F)   # [o, k*F + f]
-    sa = _pow2_scale(float(np.abs(x32).max(initial=0.0)), headroom_log2(L))
-    sw = _pow2_scale(float(np.abs(Wp).max(initial=0.0)))
+    if split == "network":
+        sa, sw = 1.0, NET_W_SCALE
+    else:
+        sa = _pow2_scale(float(np.abs(x32).max(initial=0.0)), headroom_log2(L))
+        sw = _pow2_scale(float(np.abs(Wp).max(initial=0.0)))
     A, Bm = T * sa, Wp * sw
     if mode == "tf32":
         terms = [(_tf32(A), _tf32(Bm))]
@@ -434,6 +624,53 @@ def emulate_bn_train(z, gamma, beta, rm, rv, relu=False, mutation: str = ""):
         y = np.maximum(y, f32(0))
     return (y.astype(np.float64).reshape(np.shape(z)), mean, invstd.astype(np.float64), rm_new.astype(np.float64),
             rv_new.astype(np.float64))
+
+
+BN_BWD_MUTATIONS = ("m2_dropped", "mean_not_subtracted", "rows_minus_one")
+
+
+def emulate_bn_bwd(z, g_a, gamma, beta, mean, invstd, relu=False, mutation: str = ""):
+    """What k_bn_bwd_reduce + k_bn_bwd_coef + k_bn_bwd_apply4 return for fp32 z, g_a [..., F] and the saved fp32
+    mean / invstd: per block of STAT_ROWS rows and row lane (as emulate_bn_train) fp32 sums s1 = sum g' and
+    s2 = fma(g', zhat, s2) with zhat = fp32((z - mean) invstd), blocks in fp64; then in fp32 m1 = s1 / n, m2 = s2 / n,
+    a = gamma invstd, b = -a invstd m2, c = -a m1 + a invstd m2 mean and g_z = fma(a, g', fma(b, z, c)).  The mask
+    g' = g_a [fma(z, scale, shift) > 0] uses scale = gamma invstd, shift = beta - mean scale like the forward.
+    `mutation` (one of BN_BWD_MUTATIONS) plants one defect.  Returns (g_z, dgamma, dbeta) as float64."""
+    f32 = np.float32
+    zr = np.asarray(z, f32).reshape(-1, np.shape(z)[-1])
+    gr = np.asarray(g_a, f32).reshape(zr.shape)
+    n, F = zr.shape
+    mu, ist = np.asarray(mean, f32), np.asarray(invstd, f32)
+    gam = np.asarray(gamma, f32)
+    sc = (gam * ist).astype(f32)
+    sh = (np.asarray(beta, f32) - (mu * sc).astype(f32)).astype(f32)
+    if relu:
+        gr = np.where((zr.astype(np.float64) * sc + sh).astype(f32) > 0, gr, f32(0))
+    zh = (((zr - mu).astype(f32)) * ist).astype(f32)
+    rl = 256 // min(F, 256)
+    S, Q = np.zeros(F), np.zeros(F)
+    for r0 in range(0, n, STAT_ROWS):
+        gb, hb = gr[r0:r0 + STAT_ROWS], zh[r0:r0 + STAT_ROWS]
+        s_l, q_l = np.zeros((rl, F), f32), np.zeros((rl, F), f32)
+        for i in range(0, gb.shape[0], rl):
+            k = gb[i:i + rl].shape[0]
+            s_l[:k] = (s_l[:k] + gb[i:i + rl]).astype(f32)
+            q_l[:k] = (gb[i:i + rl].astype(np.float64) * hb[i:i + rl] + q_l[:k]).astype(f32)
+        s, q = s_l[0].copy(), q_l[0].copy()
+        for j in range(1, rl):
+            s, q = (s + s_l[j]).astype(f32), (q + q_l[j]).astype(f32)
+        S, Q = S + s, Q + q
+    rows = n - 1 if mutation == "rows_minus_one" else n
+    m1, m2 = (S / rows).astype(f32), (Q / rows).astype(f32)
+    if mutation == "m2_dropped":
+        m2 = np.zeros(F, f32)
+    a = (gam * ist).astype(f32)
+    b = (-(a * ist).astype(f32) * m2).astype(f32)
+    t = (((a * ist).astype(f32) * m2).astype(f32) * mu).astype(f32)
+    c = (-(a * m1).astype(f32) + (f32(0) if mutation == "mean_not_subtracted" else t)).astype(f32)
+    inner = (b.astype(np.float64) * zr + c).astype(f32)
+    g_z = (a.astype(np.float64) * gr + inner).astype(f32)
+    return g_z.astype(np.float64).reshape(np.shape(z)), Q.astype(f32).astype(np.float64), S.astype(f32).astype(np.float64)
 
 
 def bound_ratio(y, y64, bound) -> float:

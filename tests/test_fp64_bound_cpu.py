@@ -317,3 +317,99 @@ def test_pose2mesh_on_a_nonsymmetric_hierarchy_raises():
     with pytest.raises(ValueError, match="symmetric"):
         Pose2Mesh(5, 3, mats, joint_set="mano")
     Pose2Mesh(5, 3, graph_from_fixture("mano_like")[0], joint_set="mano")
+
+
+# ------------------------------------------------------------------------------------------ the network's precision model
+NET_SHAPES = [(32, 64), (64, 128), (128, 64)]
+
+
+@pytest.mark.parametrize("fin,fout", NET_SHAPES)
+def test_network_split_bound_accepts_fp16x3_and_rejects_a_dropped_block(fin, fout):
+    """The network forward splits its activations as they are and its weights at the fixed 2^6 (split='network'):
+    that arithmetic meets the network bound on post-BatchNorm activations, and losing the lo(T) * hi(W) products of one
+    K-block does not."""
+    L, x, W, b = _layer(fin, fout)
+    x = np.maximum(x + np.float32(0.5), 0).astype(np.float32)     # ReLU activations of O(1)
+    y64 = R.cheb_conv_fwd(x, L, W, b)
+    bound = R.cheb_conv_fwd_bound(x, L, W, b, "fp16x3", split="network")
+    ok = R.bound_ratio(R.emulate_cheb_conv(x, L, W, b, "fp16x3", split="network"), y64, bound)
+    assert ok <= 0.25, ok
+    r = R.bound_ratio(R.emulate_cheb_conv(x, L, W, b, "fp16x3", drop_block=0, split="network"), y64, bound)
+    assert r > 1.0, ("drop lo*Whi of block 0", r)
+
+
+def test_network_split_floor_is_needed_for_small_activations():
+    """Activations of 2^-16 split as they are lose their lo parts to fp16's subnormals: the normalised floor (which
+    assumes a power-of-two range normalisation) rejects that arithmetic, the network floor (2^-25 per lo part) covers
+    it."""
+    L, x, W, b = _layer(32, 64)
+    x = x * np.float32(2.0 ** -16)
+    y64 = R.cheb_conv_fwd(x, L, W, None)
+    y = R.emulate_cheb_conv(x, L, W, None, "fp16x3", split="network")
+    assert R.bound_ratio(y, y64, R.cheb_conv_fwd_bound(x, L, W, None, "fp16x3", split="network")) <= 1.0
+    assert R.bound_ratio(y, y64, R.cheb_conv_fwd_bound(x, L, W, None, "fp16x3")) > 1.0
+
+
+def _bn_bwd_case(n, F, ratio, seed):
+    """z [n, F] with channels at mean / sigma = ratio, gradients correlated with zhat (m2 != 0), the forward's fp32
+    statistics."""
+    rng = np.random.default_rng(seed)
+    z = rng.standard_normal((n, F)) * (rng.random(F) + 0.5)
+    z = (z + ratio * z.std(axis=0)).astype(np.float32)
+    g = (rng.standard_normal((n, F)) + 0.5 * z / np.abs(z).max(axis=0)).astype(np.float32)
+    gam = ((rng.random(F) + 0.5) * rng.choice([-1, 1], F)).astype(np.float32)
+    bet = np.where(rng.random(F) < 0.5, 10.0, -10.0).astype(np.float32)    # ReLU open or closed, never near zero
+    _, mean, invstd, _, _ = R.emulate_bn_train(z, gam, bet, np.zeros(F), np.ones(F))
+    return z, g, gam, bet, mean, invstd
+
+
+BN_BWD_CASES = [(17, 36, 0), (17, 64, 1000), (1088, 64, 10), (1088, 64, 1000), (600, 256, 100)]
+
+
+@pytest.mark.parametrize("n,F,ratio", BN_BWD_CASES)
+def test_bn_backward_bound_accepts_the_affine_kernel(n, F, ratio):
+    """k_bn_bwd_coef + k_bn_bwd_apply4 in fp32 (including its ~3 u |mean| / sigma |gamma invstd m2| coefficient
+    error on channels far from zero) meets bn_train_bwd_bound, with and without the ReLU mask."""
+    z, g, gam, bet, mean, invstd = _bn_bwd_case(n, F, ratio, seed=n + F + ratio)
+    for relu in (False, True):
+        gz64, dgam64, dbet64, _ = R.bn_train_bwd(z, g, gam, bet, relu)
+        bz, bgam, bbet = R.bn_train_bwd_bound(z, g, gam, bet, relu)
+        gz, dgam, dbet = R.emulate_bn_bwd(z, g, gam, bet, mean.astype(np.float32), invstd.astype(np.float32), relu)
+        if relu:   # elements within reach of the activation test may take either branch: none in these cases
+            pre = R.bn_train_bwd(z, g, gam, bet, relu)[3]
+            assert np.abs(pre).min() > 1e-3, "a pre-activation near zero: pick another seed"
+        for what, got, ref, bd in (("g_z", gz, gz64, bz), ("dgamma", dgam, dgam64, bgam), ("dbeta", dbet, dbet64, bbet)):
+            r = R.bound_ratio(got, ref, bd)
+            assert r <= 0.5, (what, relu, r)
+
+
+@pytest.mark.parametrize("mutation", R.BN_BWD_MUTATIONS)
+def test_bn_backward_bound_rejects_a_mutated_kernel(mutation):
+    """m2 dropped, the mean not subtracted (c without its a invstd m2 mean term) or 1 / (rows - 1) in place of 1 / rows:
+    each makes g_z leave its bound."""
+    for n, F, ratio in BN_BWD_CASES:
+        z, g, gam, bet, mean, invstd = _bn_bwd_case(n, F, ratio, seed=n + F + ratio)
+        gz64 = R.bn_train_bwd(z, g, gam, bet)[0]
+        bz = R.bn_train_bwd_bound(z, g, gam, bet)[0]
+        gz = R.emulate_bn_bwd(z, g, gam, bet, mean.astype(np.float32), invstd.astype(np.float32), mutation=mutation)[0]
+        r = R.bound_ratio(gz, gz64, bz)
+        assert r > 1.0, (mutation, n, F, ratio, r)
+
+
+def test_resample_and_unpool_transposes():
+    """<resample(x), g> == <x, resample_t(g)> and <unpool(x), g> == <x, unpool_t(g)>; the resample equals the oracle's
+    F.interpolate; the library's fp32 tables are exact at the plans' power-of-two channel ratios."""
+    from oracle import meshnet_oracle as mo
+
+    rng = np.random.default_rng(5)
+    for fin, fout in ((64, 256), (256, 128), (32, 128), (128, 32), (48, 80)):
+        x = rng.standard_normal((2, 6, fin))
+        g = rng.standard_normal((2, 6, fout))
+        y = R.channel_resample(x, fout)
+        np.testing.assert_allclose(y, mo.channel_resample(torch.tensor(x), fout).numpy(), rtol=1e-12, atol=1e-12)
+        assert abs((y * g).sum() - (x * R.channel_resample_t(g, fin)).sum()) < 1e-9
+        pow2 = max(fin, fout) % min(fin, fout) == 0 and ((max(fin, fout) // min(fin, fout)) & (max(fin, fout) // min(fin, fout) - 1)) == 0
+        assert pow2 == np.array_equal(R.resample_matrix(fin, fout), R.resample_matrix(fin, fout, np.float32)) or not pow2
+    x = rng.standard_normal((2, 5, 3))
+    g = rng.standard_normal((2, 10, 3))
+    assert abs((R.unpool(x) * g).sum() - (x * R.unpool_t(g)).sum()) < 1e-12
