@@ -148,6 +148,31 @@ typedef struct {
 } p2m_capture_t;
 int p2m_debug_set_capture(p2m_model_t* m, const p2m_capture_t* capture);
 
+/* ---- per-BatchNorm options -------------------------------------------------------------------------
+ * One record per BatchNorm, the state torch's _BatchNorm.forward reads (torch/nn/modules/batchnorm.py):
+ *   stats  P2M_BN_BATCH_UPDATE: batch statistics, running statistics updated and num_batches_tracked += 1 (bn.training
+ *            with track_running_stats);
+ *          P2M_BN_BATCH: batch statistics, nothing updated (bn.training without track_running_stats, or an eval-mode
+ *            BatchNorm whose running buffers are None); the running-statistic pointers may be NULL;
+ *          P2M_BN_RUNNING: running statistics (eval-mode BatchNorm, also inside a train-mode model: frozen statistics).
+ *   cumulative  momentum None: the update factor is 1 / num_batches_tracked after its increment, read on the device
+ *            (the call never synchronises); needs num_batches_tracked.
+ *   momentum  the update factor otherwise (used as a float);  eps  added to the variance (the biased one of the batch,
+ *            or the running one).
+ * Batch statistics normalise with the biased variance and update the running variance with the unbiased one (n = the
+ * rows the BatchNorm sees: B * V for MeshNet, B for PoseNet).  A NULL option array means today's defaults: momentum 0.1,
+ * eps 1e-5, and P2M_BN_BATCH_UPDATE in training / P2M_BN_RUNNING in eval; those give bitwise the results of the entry
+ * points without options, which are calls with NULL.                                                      */
+#define P2M_BN_BATCH_UPDATE 0
+#define P2M_BN_BATCH 1
+#define P2M_BN_RUNNING 2
+typedef struct {
+  int32_t stats;       /* P2M_BN_BATCH_UPDATE | P2M_BN_BATCH | P2M_BN_RUNNING */
+  int32_t cumulative;  /* 1: momentum None (cumulative moving average) */
+  double momentum;
+  double eps;
+} p2m_bn_opts_t;
+
 /* Bytes of device workspace p2m_meshnet_forward needs for batch B.  In training mode the workspace
  * also carries what p2m_meshnet_backward reads, so it must stay alive and untouched in between.   */
 size_t p2m_meshnet_workspace_bytes(const p2m_model_t* m, int batch, int training);
@@ -172,6 +197,23 @@ int p2m_meshnet_forward_vertices(p2m_model_t* m, const p2m_params_t* params, con
 int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* params, const p2m_params_t* grads, const float* x,
                          const float* dy, float* dx, int batch, void* workspace, size_t workspace_bytes,
                          void* scratch, size_t scratch_bytes, p2m_stream_t stream);
+
+/* The same three with one p2m_bn_opts_t per layer (`bn` [n_layers], host memory; the last layer's entry, which has no
+ * BatchNorm, is ignored; NULL: the defaults above).  The eval schedule (BatchNorm folded into the conv epilogues,
+ * padding elision and dedup, fused head) runs when training == 0 and every BatchNorm uses P2M_BN_RUNNING, with each
+ * layer's eps.  Otherwise the training schedule runs with per-layer statistics (with training == 0, e.g. an eval-mode
+ * BatchNorm without running buffers, it is not followed by a backward).  A layer with P2M_BN_RUNNING in the training schedule is a frozen BatchNorm: its
+ * backward has no batch-mean terms and the conv bias in front of it gets sum_rows g_z, where a batch-statistics layer
+ * writes exactly 0.  The workspace size depends on the options; the backward takes the options of the forward that
+ * wrote the workspace.                                                                                    */
+size_t p2m_meshnet_workspace_bytes_opts(const p2m_model_t* m, int batch, int training, const p2m_bn_opts_t* bn);
+int p2m_meshnet_forward_opts(p2m_model_t* m, const p2m_params_t* params, const p2m_bn_opts_t* bn, const float* x,
+                             float* y, int batch, int training, void* workspace, size_t workspace_bytes,
+                             p2m_stream_t stream);
+int p2m_meshnet_backward_opts(p2m_model_t* m, const p2m_params_t* params, const p2m_params_t* grads,
+                              const p2m_bn_opts_t* bn, const float* x, const float* dy, float* dx, int batch,
+                              void* workspace, size_t workspace_bytes, void* scratch, size_t scratch_bytes,
+                              p2m_stream_t stream);
 
 /* End-to-end inference with HOST buffers (pageable or pinned): H2D of x, forward (eval), D2H of y,
  * stream-synchronised on return.  `workspace` must additionally hold x and y
@@ -307,6 +349,27 @@ int p2m_posenet_backward(const p2m_posenet_params_t* params, const float* pose2d
                          const int64_t* seed, const void* saved, size_t saved_bytes, const float* d_pose3d,
                          const p2m_posenet_grads_t* grads, float* d_pose2d, void* workspace, size_t workspace_bytes,
                          p2m_stream_t stream);
+
+/* The PoseNet entry points with options: `bn` [2 num_stage] (host; stage s's bn1 at 2 s, bn2 at 2 s + 1; NULL: the
+ * defaults, P2M_BN_RUNNING for the eval forward, P2M_BN_BATCH_UPDATE for the training calls), `p_dropout` [num_stage]
+ * (host; the p of stage s's Dropout, 0 when it is in eval mode; NULL: no dropout).  The dropout rule above holds with
+ * each stage's own p, so p_dropout[s] == the scalar p of the calls without options gives their masks bitwise.  The eval
+ * forward needs P2M_BN_RUNNING everywhere and reads each eps.  In the training calls a P2M_BN_RUNNING BatchNorm is
+ * frozen: scale / shift from its running statistics, backward without the batch-mean terms; batch >= 2 is required
+ * only when some BatchNorm uses batch statistics.  The running-statistic pointers of a P2M_BN_BATCH BatchNorm may be
+ * NULL.  The workspace and saved sizes do not depend on the options.  The backward takes the options and p_dropout of
+ * the forward that wrote `saved`. */
+int p2m_posenet_forward_opts(const p2m_posenet_params_t* params, const p2m_bn_opts_t* bn, const float* pose2d,
+                             float* pose3d, float* pose_combine, int batch, void* workspace, size_t workspace_bytes,
+                             p2m_stream_t stream);
+int p2m_posenet_train_forward_opts(const p2m_posenet_params_t* params, const p2m_posenet_train_t* extra,
+                                   const p2m_bn_opts_t* bn, const float* p_dropout, const float* pose2d, int batch,
+                                   const int64_t* seed, float* pose3d, float* pose_combine, void* saved,
+                                   size_t saved_bytes, void* workspace, size_t workspace_bytes, p2m_stream_t stream);
+int p2m_posenet_backward_opts(const p2m_posenet_params_t* params, const p2m_bn_opts_t* bn, const float* p_dropout,
+                              const float* pose2d, int batch, const int64_t* seed, const void* saved,
+                              size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* grads,
+                              float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream);
 
 /* ---- the steps either side of the model in the reference's callers (SURVEY.md §8 row f2) ----------
  * Joint regression (lib/core/base.py:131,204; demo/run.py:171): joints [B, n_joint, C] = joint_regressor

@@ -62,6 +62,16 @@ class Params(C.Structure):
     ]
 
 
+P2M_BN_BATCH_UPDATE = 0
+P2M_BN_BATCH = 1
+P2M_BN_RUNNING = 2
+
+
+class BnOpts(C.Structure):
+    """p2m_bn_opts_t: what one BatchNorm's forward reads (statistics mode, momentum None, momentum, eps)."""
+    _fields_ = [("stats", C.c_int32), ("cumulative", C.c_int32), ("momentum", C.c_double), ("eps", C.c_double)]
+
+
 class ConvFwdArgs(C.Structure):
     _fields_ = [
         ("level", C.c_int32), ("batch", C.c_int32), ("fin", C.c_int32), ("fout", C.c_int32),
@@ -176,9 +186,11 @@ class H36MError(C.Structure):
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
     "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
-    "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
+    "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_meshnet_workspace_bytes_opts", "p2m_meshnet_forward_opts",
+    "p2m_meshnet_backward_opts", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
     "p2m_posenet_train_workspace_bytes", "p2m_posenet_train_saved_bytes", "p2m_posenet_train_forward", "p2m_posenet_backward",
+    "p2m_posenet_forward_opts", "p2m_posenet_train_forward_opts", "p2m_posenet_backward_opts",
     "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
     "p2m_rigid_align", "p2m_point_errors", "p2m_fit_camera", "p2m_crop_cam_to_orig",
     "p2m_one_euro_smooth", "p2m_accel_error", "p2m_segment_mean",
@@ -260,6 +272,14 @@ def load() -> C.CDLL:
         lib.p2m_meshnet_backward.argtypes = [vp, C.POINTER(Params), C.POINTER(Params), vp, vp, vp, C.c_int, vp, sz,
                                              vp, sz, vp]
         lib.p2m_meshnet_backward.restype = C.c_int
+        bn_p = C.POINTER(BnOpts)
+        lib.p2m_meshnet_workspace_bytes_opts.argtypes = [vp, C.c_int, C.c_int, bn_p]
+        lib.p2m_meshnet_workspace_bytes_opts.restype = sz
+        lib.p2m_meshnet_forward_opts.argtypes = [vp, C.POINTER(Params), bn_p, vp, vp, C.c_int, C.c_int, vp, sz, vp]
+        lib.p2m_meshnet_forward_opts.restype = C.c_int
+        lib.p2m_meshnet_backward_opts.argtypes = [vp, C.POINTER(Params), C.POINTER(Params), bn_p, vp, vp, vp, C.c_int,
+                                                  vp, sz, vp, sz, vp]
+        lib.p2m_meshnet_backward_opts.restype = C.c_int
         lib.p2m_cheb_conv_workspace_bytes.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int]
         lib.p2m_cheb_conv_workspace_bytes.restype = sz
         lib.p2m_cheb_conv_fwd.argtypes = [vp, C.POINTER(ConvFwdArgs), vp, sz, vp]
@@ -279,6 +299,14 @@ def load() -> C.CDLL:
         lib.p2m_posenet_backward.argtypes = [C.POINTER(PoseNetParams), vp, C.c_int, C.c_float, vp, vp, sz, vp,
                                              C.POINTER(PoseNetGrads), vp, vp, sz, vp]
         lib.p2m_posenet_backward.restype = C.c_int
+        lib.p2m_posenet_forward_opts.argtypes = [C.POINTER(PoseNetParams), bn_p, vp, vp, vp, C.c_int, vp, sz, vp]
+        lib.p2m_posenet_forward_opts.restype = C.c_int
+        lib.p2m_posenet_train_forward_opts.argtypes = [C.POINTER(PoseNetParams), C.POINTER(PoseNetTrain), bn_p,
+                                                       c_float_p, vp, C.c_int, vp, vp, vp, vp, sz, vp, sz, vp]
+        lib.p2m_posenet_train_forward_opts.restype = C.c_int
+        lib.p2m_posenet_backward_opts.argtypes = [C.POINTER(PoseNetParams), bn_p, c_float_p, vp, C.c_int, vp, vp, sz,
+                                                  vp, C.POINTER(PoseNetGrads), vp, vp, sz, vp]
+        lib.p2m_posenet_backward_opts.restype = C.c_int
         lib.p2m_regress_joints.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         lib.p2m_regress_joints.restype = C.c_int
         lib.p2m_normalize_pose2d.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
@@ -389,6 +417,32 @@ def call(name: str, device, *args):
     fn = getattr(load(), name)
     ptrs = (a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args)
     check(fn(*ptrs, torch.cuda.current_stream(device).cuda_stream), name)
+
+
+def bn_opts(bn) -> BnOpts:
+    """The p2m_bn_opts_t of an nn.BatchNorm1d in its current state, by torch's _BatchNorm.forward: batch statistics when
+    it is in training mode or has no running buffers, an update of the buffers only in training mode with
+    track_running_stats, momentum None as the cumulative average.  ValueError for what the native kernels do not
+    implement: another module type in a BatchNorm's place, or affine=False."""
+    if not isinstance(bn, torch.nn.BatchNorm1d):
+        raise ValueError(f"pose2mesh_release_b200: expected an nn.BatchNorm1d, got {type(bn).__name__}")
+    if not bn.affine:
+        raise ValueError("pose2mesh_release_b200: BatchNorm1d(affine=False) is not supported by the native kernels")
+    batch = bn.training or (bn.running_mean is None and bn.running_var is None)
+    update = bn.training and bn.track_running_stats
+    o = BnOpts()
+    o.stats = P2M_BN_RUNNING if not batch else (P2M_BN_BATCH_UPDATE if update else P2M_BN_BATCH)
+    o.cumulative = int(bn.momentum is None)
+    o.momentum = 0.0 if bn.momentum is None else float(bn.momentum)
+    o.eps = float(bn.eps)
+    return o
+
+
+def dropout_p(drop) -> float:
+    """The p an nn.Dropout applies in its current state (0 in eval mode); ValueError for another module type."""
+    if not isinstance(drop, torch.nn.Dropout):
+        raise ValueError(f"pose2mesh_release_b200: expected an nn.Dropout, got {type(drop).__name__}")
+    return float(drop.p) if drop.training else 0.0
 
 
 def cuda_tensor(x, what: str) -> torch.Tensor:

@@ -831,18 +831,26 @@ int launch_fill_zero(void* p, size_t bytes, cudaStream_t s) {
 // =====================================================================================
 // BatchNorm1d over rows
 // =====================================================================================
+// scale / shift of a BatchNorm with running statistics: ((z + bias) - rm) * scale + beta.  bias == nullptr (a z that
+// already carries its bias: the frozen-statistics training path) folds none; save_mean / save_invstd (optional) take
+// rm and 1 / sqrt(rv + eps), what the BatchNorm backward reads
 __global__ void k_bn_fold_eval(const float* gamma, const float* beta, const float* rm, const float* rv,
-                               const float* bias, float* scale, float* shift, int F) {
+                               const float* bias, float eps, float* scale, float* shift, float* save_mean,
+                               float* save_invstd, int F) {
   int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= F) return;
-  float sc = gamma[c] / sqrtf(rv[c] + 1e-5f);
+  float sc = gamma[c] / sqrtf(rv[c] + eps);
   scale[c] = sc;
   float b = bias ? bias[c] : 0.f;
   shift[c] = beta[c] + (b - rm[c]) * sc;   // ((z + b) - rm) * sc + beta
+  if (save_mean) save_mean[c] = rm[c];
+  if (save_invstd) save_invstd[c] = 1.f / sqrtf(rv[c] + eps);
 }
 int launch_bn_fold_eval(const float* gamma, const float* beta, const float* rm, const float* rv, const float* bias,
-                        float* scale, float* shift, int F, cudaStream_t s) {
-  k_bn_fold_eval<<<cdiv(F, 128), 128, 0, s>>>(gamma, beta, rm, rv, bias, scale, shift, F);
+                        double eps, float* scale, float* shift, int F, cudaStream_t s, float* save_mean,
+                        float* save_invstd) {
+  k_bn_fold_eval<<<cdiv(F, 128), 128, 0, s>>>(gamma, beta, rm, rv, bias, (float)eps, scale, shift, save_mean,
+                                              save_invstd, F);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -894,34 +902,74 @@ int launch_col_stats(const float* z, int rows, int F, double* sums, cudaStream_t
   return P2M_OK;
 }
 
-// sums = k_col_stats' (S, Q) of z - K around K = z[0][c]:  mean = K + S/n,  var = Q/n - (S/n)^2
+// sums = k_col_stats' (S, Q) of z - K around K = z[0][c]:  mean = K + S/n,  var = Q/n - (S/n)^2.
+// update: running statistics (and num_batches_tracked) take the batch's, with factor `momentum`, or with cumulative
+// 1 / num_batches_tracked read here after k_nbt_add1 incremented it.  Otherwise rm / rv / nbt are not touched.
 __global__ void k_bn_finalize(const double* __restrict__ sums, const float* __restrict__ z, long long rows, int F,
                               const float* gamma, const float* beta, float* rm, float* rv, long long* nbt,
-                              float* save_mean, float* save_invstd, float* scale, float* shift) {
+                              double eps, float momentum, int cumulative, int update, float* save_mean,
+                              float* save_invstd, float* scale, float* shift) {
   int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c == 0 && nbt) *nbt += 1;
+  if (update && !cumulative && c == 0 && nbt) *nbt += 1;
   if (c >= F) return;
   double n = (double)rows;
   double d = sums[c] / n;
   double mean = (double)z[c] + d;
   double var = sums[F + c] / n - d * d;
   if (var < 0) var = 0;
-  float invstd = (float)(1.0 / sqrt(var + 1e-5));
-  if (rm) rm[c] = 0.9f * rm[c] + 0.1f * (float)mean;                                  // momentum 0.1
-  if (rv) rv[c] = 0.9f * rv[c] + 0.1f * (float)(rows > 1 ? var * n / (n - 1.0) : var);  // unbiased
+  float invstd = (float)(1.0 / sqrt(var + eps));
+  if (update) {
+    const float mom = cumulative ? (float)(1.0 / (double)*nbt) : momentum, keep = 1.f - mom;
+    const float var_u = (float)(rows > 1 ? var * n / (n - 1.0) : var);  // unbiased
+    if (rm) rm[c] = fmaf(mom, (float)mean, __fmul_rn(keep, rm[c]));
+    if (rv) rv[c] = fmaf(keep, rv[c], __fmul_rn(mom, var_u));
+  }
   if (save_mean) save_mean[c] = (float)mean;
   if (save_invstd) save_invstd[c] = invstd;
   float sc = gamma[c] * invstd;
   scale[c] = sc;
   shift[c] = beta[c] - (float)mean * sc;
 }
+__global__ void k_nbt_add1(long long* nbt) { *nbt += 1; }
 int launch_bn_finalize(const double* sums, const float* z, int rows, int F, const float* gamma, const float* beta,
-                       float* rm, float* rv, int64_t* nbt, float* save_mean, float* save_invstd, float* scale,
-                       float* shift, cudaStream_t s) {
-  k_bn_finalize<<<cdiv(F, 128), 128, 0, s>>>(sums, z, rows, F, gamma, beta, rm, rv, (long long*)nbt, save_mean,
-                                             save_invstd, scale, shift);
+                       float* rm, float* rv, int64_t* nbt, const p2m_bn_opts_t& o, float* save_mean,
+                       float* save_invstd, float* scale, float* shift, cudaStream_t s) {
+  const int update = o.stats == P2M_BN_BATCH_UPDATE;
+  if (update && o.cumulative) {  // a separate launch: every block of the finalize reads the incremented count
+    k_nbt_add1<<<1, 1, 0, s>>>((long long*)nbt);
+    P2M_LAUNCH_OK();
+  }
+  k_bn_finalize<<<cdiv(F, 128), 128, 0, s>>>(sums, z, rows, F, gamma, beta, rm, rv, (long long*)nbt, o.eps,
+                                             (float)o.momentum, o.cumulative, update, save_mean, save_invstd, scale,
+                                             shift);
   P2M_LAUNCH_OK();
   return P2M_OK;
+}
+
+int check_bn_opts(const p2m_bn_opts_t& o, const void* rm, const void* rv, const void* nbt, const char* where) {
+  const bool stats_ok = o.stats == P2M_BN_BATCH_UPDATE || o.stats == P2M_BN_BATCH || o.stats == P2M_BN_RUNNING;
+  if (!stats_ok || !(o.eps >= 0.0) || !(o.cumulative || (o.momentum >= 0.0 && o.momentum <= 1.0))) {
+    set_error(std::string(where) + ": bad BatchNorm options (stats, eps or momentum)");
+    return P2M_ERR_INVALID;
+  }
+  if (o.stats != P2M_BN_BATCH && (!rm || !rv)) {
+    set_error(std::string(where) + ": BatchNorm without running statistics needs stats = P2M_BN_BATCH");
+    return P2M_ERR_INVALID;
+  }
+  if (o.stats == P2M_BN_BATCH_UPDATE && o.cumulative && !nbt) {
+    set_error(std::string(where) + ": a cumulative running average needs num_batches_tracked");
+    return P2M_ERR_INVALID;
+  }
+  return P2M_OK;
+}
+
+int launch_bn_stats(const float* z, int rows, int F, const float* gamma, const float* beta, float* rm, float* rv,
+                    int64_t* nbt, const p2m_bn_opts_t& o, double* sums, float* mean, float* invstd, float* scale,
+                    float* shift, cudaStream_t s) {
+  if (o.stats == P2M_BN_RUNNING)
+    return launch_bn_fold_eval(gamma, beta, rm, rv, nullptr, o.eps, scale, shift, F, s, mean, invstd);
+  P2M_TRY(launch_col_stats(z, rows, F, sums, s));
+  return launch_bn_finalize(sums, z, rows, F, gamma, beta, rm, rv, nbt, o, mean, invstd, scale, shift, s);
 }
 
 __global__ void __launch_bounds__(256) k_affine_act(const float* __restrict__ z, long long rows, int F,
@@ -1042,13 +1090,15 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply(const float* __restrict__ 
                                                       long long rows, int F, const float* __restrict__ gamma,
                                                       const float* __restrict__ scale, const float* __restrict__ shift,
                                                       const float* __restrict__ mean,
-                                                      const float* __restrict__ invstd, int relu,
+                                                      const float* __restrict__ invstd, int relu, int frozen,
                                                       const double* __restrict__ sums, float* __restrict__ dgamma,
-                                                      float* __restrict__ dbeta, float* __restrict__ g_z) {
+                                                      float* __restrict__ dbeta, float* __restrict__ dbias,
+                                                      float* __restrict__ g_z) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx < F) {
     dbeta[idx] = (float)sums[idx];
     dgamma[idx] = (float)sums[F + idx];
+    if (dbias) dbias[idx] = (float)(sums[idx] * (double)(gamma[idx] * invstd[idx]));
   }
   if (idx >= rows * F) return;
   int f = (int)(idx % F);
@@ -1056,6 +1106,10 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply(const float* __restrict__ 
   float zh = (zv - mean[f]) * invstd[f];
   float g = g_a[idx];
   if (relu && !(fmaf(zv, scale[f], shift[f]) > 0.f)) g = 0.f;
+  if (frozen) {
+    g_z[idx] = gamma[f] * invstd[f] * g;
+    return;
+  }
   float m1 = (float)(sums[f] / (double)rows);
   float m2 = (float)(sums[F + f] / (double)rows);
   g_z[idx] = gamma[f] * invstd[f] * (g - m1 - zh * m2);
@@ -1065,10 +1119,13 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply(const float* __restrict__ 
 // (g_z = gamma invstd (g' - m1 - zhat m2), zhat = (z - mean) invstd), g' = g_a masked by the forward's own
 // activation test fma(z, scale, shift) > 0.  k_bn_bwd_coef builds coef[5][F] = a | b | c | scale | shift once per
 // layer; the streaming kernel then needs five 16-byte coefficient loads per four channels and no fp64.
+// frozen (running statistics, constants of the forward): g_z = a g', b = c = 0, and the bias in front of the BatchNorm
+// gets sum_rows g_z = a s1 (dbias, optional).
 __global__ void k_bn_bwd_coef(const double* __restrict__ sums, long long rows, int F, const float* __restrict__ gamma,
                               const float* __restrict__ scale, const float* __restrict__ shift,
-                              const float* __restrict__ mean, const float* __restrict__ invstd,
-                              float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ coef) {
+                              const float* __restrict__ mean, const float* __restrict__ invstd, int frozen,
+                              float* __restrict__ dgamma, float* __restrict__ dbeta, float* __restrict__ dbias,
+                              float* __restrict__ coef) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
   dbeta[f] = (float)sums[f];
@@ -1076,6 +1133,14 @@ __global__ void k_bn_bwd_coef(const double* __restrict__ sums, long long rows, i
   const float m1 = (float)(sums[f] / (double)rows), m2 = (float)(sums[F + f] / (double)rows);
   const float a = gamma[f] * invstd[f];
   coef[f] = a;
+  if (frozen) {
+    coef[F + f] = 0.f;
+    coef[2 * F + f] = 0.f;
+    coef[3 * F + f] = scale[f];
+    coef[4 * F + f] = shift[f];
+    if (dbias) dbias[f] = (float)(sums[f] * (double)a);
+    return;
+  }
   coef[F + f] = -a * invstd[f] * m2;
   coef[2 * F + f] = -a * m1 + a * invstd[f] * m2 * mean[f];
   coef[3 * F + f] = scale[f];
@@ -1123,7 +1188,8 @@ __global__ void __launch_bounds__(256) k_bn_bwd_apply4(const float4* __restrict_
 }
 int launch_bn_relu_bwd(const float* z, const float* g_a, int rows, int F, const float* gamma, const float* scale,
                        const float* shift, const float* mean, const float* invstd, int relu, double* sums,
-                       float* dgamma, float* dbeta, float* g_z, cudaStream_t s, float* gz_scale_out) {
+                       float* dgamma, float* dbeta, float* g_z, cudaStream_t s, float* gz_scale_out, int frozen,
+                       float* dbias) {
   P2M_CUDA_OK(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * F, s));
   k_bn_bwd_reduce<<<cdiv(rows, STAT_ROWS), 256, 2 * 256 * sizeof(float), s>>>(z, g_a, rows, F, scale, shift, mean,
                                                                                invstd, relu, sums);
@@ -1133,7 +1199,8 @@ int launch_bn_relu_bwd(const float* z, const float* g_a, int rows, int F, const 
     if (gz_scale_out) P2M_CUDA_OK(cudaMemsetAsync(gz_scale_out, 0, sizeof(float), s));
     const long long n4 = (long long)rows * (F / 4);
     float* coef = reinterpret_cast<float*>(sums + 2 * F);  // [5][F] floats behind the two fp64 sums
-    k_bn_bwd_coef<<<cdiv(F, 128), 128, 0, s>>>(sums, rows, F, gamma, scale, shift, mean, invstd, dgamma, dbeta, coef);
+    k_bn_bwd_coef<<<cdiv(F, 128), 128, 0, s>>>(sums, rows, F, gamma, scale, shift, mean, invstd, frozen, dgamma, dbeta,
+                                                dbias, coef);
     P2M_LAUNCH_OK();
     int sms = 0;
     P2M_TRY(current_sm_count(&sms));
@@ -1150,7 +1217,7 @@ int launch_bn_relu_bwd(const float* z, const float* g_a, int rows, int F, const 
     return P2M_OK;
   }
   k_bn_bwd_apply<<<cdiv((long long)rows * F, 256), 256, 0, s>>>(z, g_a, rows, F, gamma, scale, shift, mean, invstd, relu,
-                                                               sums, dgamma, dbeta, g_z);
+                                                               frozen, sums, dgamma, dbeta, dbias, g_z);
   P2M_LAUNCH_OK();
   if (gz_scale_out) return launch_absmax_scale(g_z, (long long)rows * F, gz_scale_out, s);
   return P2M_OK;

@@ -439,13 +439,13 @@ int conv_linear(p2m_model* m, const ConvRoute& r, const Layer& L, int B, const f
   return P2M_OK;
 }
 
-// Train-mode BatchNorm of a conv's output z: batch statistics, finalize (running and saved statistics, scale / shift),
-// then a = relu?(z * scale + shift) (+ the resampled residual res, if not null)
+// BatchNorm of a conv's output z in the training schedule: statistics by the layer's options (launch_bn_stats: batch
+// or running; saved statistics, scale / shift), then a = relu?(z * scale + shift) (+ the resampled residual res)
 int bn_train_tail(const float* z, int rows, int F, const float* gamma, const float* beta, float* rm, float* rv,
-                  int64_t* nbt, double* sums, float* mean, float* invstd, float* scale, float* shift, int relu,
-                  const float* res, int res_F, int res_unpool, const InterpTable* it, float* a, cudaStream_t s) {
-  P2M_TRY(launch_col_stats(z, rows, F, sums, s));
-  P2M_TRY(launch_bn_finalize(sums, z, rows, F, gamma, beta, rm, rv, nbt, mean, invstd, scale, shift, s));
+                  int64_t* nbt, const p2m_bn_opts_t& o, double* sums, float* mean, float* invstd, float* scale,
+                  float* shift, int relu, const float* res, int res_F, int res_unpool, const InterpTable* it, float* a,
+                  cudaStream_t s) {
+  P2M_TRY(launch_bn_stats(z, rows, F, gamma, beta, rm, rv, nbt, o, sums, mean, invstd, scale, shift, s));
   return launch_affine_act(z, rows, F, scale, shift, relu, res, res_F, res_unpool, it, a, s);
 }
 
@@ -585,7 +585,8 @@ int build_padding_classes(p2m_model* m, const p2m_model_desc_t* d) {
   return P2M_OK;
 }
 
-int check_params(const p2m_model* m, const p2m_params_t* p, bool need_running) {
+// bn: the forward's resolved per-layer options, whose buffers are checked too (null: the backward, which reads none)
+int check_params(const p2m_model* m, const p2m_params_t* p, const std::vector<p2m_bn_opts_t>* bn) {
   if (!p || !p->fc_w || !p->fc_b || !p->cl_w || !p->cl_b || !p->bn_w || !p->bn_b) {
     set_error("params: null table");
     return P2M_ERR_INVALID;
@@ -596,13 +597,35 @@ int check_params(const p2m_model* m, const p2m_params_t* p, bool need_running) {
       return P2M_ERR_INVALID;
     }
     if (m->layers[i].bn) {
-      if (!p->bn_w[i] || !p->bn_b[i] || (need_running && (!p->bn_rm || !p->bn_rv || !p->bn_rm[i] || !p->bn_rv[i]))) {
+      if (!p->bn_w[i] || !p->bn_b[i]) {
         set_error("params: null BatchNorm tensor for layer " + std::to_string(i));
         return P2M_ERR_INVALID;
+      }
+      if (bn) {
+        const std::string where = "params: BatchNorm of layer " + std::to_string(i);
+        P2M_TRY(check_bn_opts((*bn)[i], p->bn_rm ? p->bn_rm[i] : nullptr, p->bn_rv ? p->bn_rv[i] : nullptr,
+                              p->bn_nbt ? p->bn_nbt[i] : nullptr, where.c_str()));
       }
     }
   }
   return P2M_OK;
+}
+
+// One option record per layer: the caller's, or the defaults (batch statistics with update in training, running
+// statistics in eval).  The last layer has no BatchNorm; its entry is ignored.
+std::vector<p2m_bn_opts_t> resolve_bn_opts(const p2m_model* m, int training, const p2m_bn_opts_t* bn) {
+  std::vector<p2m_bn_opts_t> out(m->layers.size(), bn_opts_default(training ? P2M_BN_BATCH_UPDATE : P2M_BN_RUNNING));
+  for (size_t i = 0; bn && i < out.size(); ++i)
+    if (m->layers[i].bn) out[i] = bn[i];
+  return out;
+}
+// The eval schedule (folded BatchNorm, no saved activations) serves a forward without backward whose BatchNorms all
+// use running statistics
+bool eval_schedule(const p2m_model* m, int training, const std::vector<p2m_bn_opts_t>& bn) {
+  if (training) return false;
+  for (size_t i = 0; i < m->layers.size(); ++i)
+    if (m->layers[i].bn && bn[i].stats != P2M_BN_RUNNING) return false;
+  return true;
 }
 
 }  // namespace
@@ -953,9 +976,13 @@ int p2m_model_set_precision(p2m_model_t* m, int precision) {
   return P2M_OK;
 }
 
-size_t p2m_meshnet_workspace_bytes(const p2m_model_t* m, int batch, int training) {
+size_t p2m_meshnet_workspace_bytes_opts(const p2m_model_t* m, int batch, int training, const p2m_bn_opts_t* bn) {
   if (!m || batch <= 0 || m->layers.empty()) return 0;
-  return training ? TrainWs(m, batch, nullptr).bytes() : EvalWs(m, batch, nullptr).bytes();
+  return eval_schedule(m, training, resolve_bn_opts(m, training, bn)) ? EvalWs(m, batch, nullptr).bytes()
+                                                                      : TrainWs(m, batch, nullptr).bytes();
+}
+size_t p2m_meshnet_workspace_bytes(const p2m_model_t* m, int batch, int training) {
+  return p2m_meshnet_workspace_bytes_opts(m, batch, training, nullptr);
 }
 size_t p2m_meshnet_backward_scratch_bytes(const p2m_model_t* m, int batch) {
   if (!m || batch <= 0 || m->layers.empty()) return 0;
@@ -968,8 +995,8 @@ size_t p2m_meshnet_host_io_bytes(const p2m_model_t* m, int batch) {
 
 // -------------------------------------------------------------------------------------
 // The eval forward: folded BatchNorm, rotating buffers, fused head, padding-row dedup, fused output gather (`gathered`)
-static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, void* workspace,
-                        cudaStream_t s, int gathered) {
+static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const std::vector<p2m_bn_opts_t>& bn, const float* x,
+                        float* y, int B, void* workspace, cudaStream_t s, int gathered) {
   const EvalWs w(m, B, workspace);
   const int nl = (int)m->layers.size();
   // isolated (padding) rows: only class representatives (DevLevel::rep_tiles), or — when the caller takes the gathered
@@ -996,8 +1023,8 @@ static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const float* x, f
       float* scale = w.scale_scratch;
       float* shift = w.scale_scratch + L.fout;
       if (L.bn) {
-        P2M_TRY(launch_bn_fold_eval(P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li], P->cl_b[li], scale, shift,
-                                    L.fout, s));
+        P2M_TRY(launch_bn_fold_eval(P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li], P->cl_b[li], bn[li].eps,
+                                    scale, shift, L.fout, s));
         ep.scale = scale;
         ep.shift = shift;
       } else {
@@ -1069,9 +1096,10 @@ static int forward_eval(p2m_model_t* m, const p2m_params_t* P, const float* x, f
   return P2M_OK;
 }
 
-// The training forward: batch-statistics BatchNorm; saves what p2m_meshnet_backward reads (TrainWs).
-static int forward_train(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, void* workspace,
-                         cudaStream_t s) {
+// The training forward: each BatchNorm with batch or running statistics by its options; saves what
+// p2m_meshnet_backward reads (TrainWs).
+static int forward_train(p2m_model_t* m, const p2m_params_t* P, const std::vector<p2m_bn_opts_t>& bn, const float* x,
+                         float* y, int B, void* workspace, cudaStream_t s) {
   const TrainWs w(m, B, workspace);
   const float* cur = x;
   int cur_unpool = 0;
@@ -1089,8 +1117,8 @@ static int forward_train(p2m_model_t* m, const p2m_params_t* P, const float* x, 
       float* z = L.bn ? w.z[li] : y;  // the last layer, the only one without BatchNorm, writes y
       P2M_TRY(conv_linear(m, r, L, B, cur, cur_unpool, P->cl_w[li], w.T, w.wp[li], w.wpack, ep, z, s, true));
       if (L.bn)
-        P2M_TRY(bn_train_tail(z, B * L.V, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm[li], P->bn_rv[li],
-                              P->bn_nbt ? P->bn_nbt[li] : nullptr, w.sums, w.mean[li], w.invstd[li], w.scale[li],
+        P2M_TRY(bn_train_tail(z, B * L.V, L.fout, P->bn_w[li], P->bn_b[li], P->bn_rm ? P->bn_rm[li] : nullptr,
+                              P->bn_rv ? P->bn_rv[li] : nullptr, P->bn_nbt ? P->bn_nbt[li] : nullptr, bn[li], w.sums, w.mean[li], w.invstd[li], w.scale[li],
                               w.shift[li], L.relu, with_res ? block_in : nullptr, blk.cin, block_in_unpool,
                               with_res ? &blk.interp : nullptr, w.a[li], s));
       if (m->capture && L.bn) {
@@ -1113,28 +1141,39 @@ static int forward_train(p2m_model_t* m, const p2m_params_t* P, const float* x, 
 }
 
 // Checks the arguments before anything is enqueued, then runs the eval or the training schedule
-static int meshnet_forward(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, int training,
-                           void* workspace, size_t workspace_bytes, p2m_stream_t stream, int gathered) {
+static int meshnet_forward(p2m_model_t* m, const p2m_params_t* P, const p2m_bn_opts_t* bn_opts, const float* x,
+                           float* y, int B, int training, void* workspace, size_t workspace_bytes, p2m_stream_t stream,
+                           int gathered) {
   if (!m || !x || !y || B <= 0 || !workspace || m->layers.empty()) {
     set_error("meshnet_forward: bad argument");
     return P2M_ERR_INVALID;
   }
-  P2M_TRY(check_params(m, P, true));
+  const std::vector<p2m_bn_opts_t> bn = resolve_bn_opts(m, training, bn_opts);
+  const bool eval = eval_schedule(m, training, bn);
+  if (gathered && !eval) {
+    set_error("meshnet_forward_vertices: every BatchNorm must use running statistics");
+    return P2M_ERR_INVALID;
+  }
+  P2M_TRY(check_params(m, P, &bn));
   P2M_TRY(check_kernel_status(m, "meshnet_forward"));
   DeviceGuard guard(m->device);
-  const size_t need = p2m_meshnet_workspace_bytes(m, B, training);
+  const size_t need = p2m_meshnet_workspace_bytes_opts(m, B, training, bn_opts);
   if (need > workspace_bytes) {
     set_error("meshnet_forward: workspace too small (" + std::to_string(workspace_bytes) + " < " +
               std::to_string(need) + ")");
     return P2M_ERR_WORKSPACE;
   }
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  return training ? forward_train(m, P, x, y, B, workspace, s) : forward_eval(m, P, x, y, B, workspace, s, gathered);
+  return eval ? forward_eval(m, P, bn, x, y, B, workspace, s, gathered) : forward_train(m, P, bn, x, y, B, workspace, s);
 }
 
+int p2m_meshnet_forward_opts(p2m_model_t* m, const p2m_params_t* P, const p2m_bn_opts_t* bn, const float* x, float* y,
+                             int B, int training, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  return meshnet_forward(m, P, bn, x, y, B, training, workspace, workspace_bytes, stream, 0);
+}
 int p2m_meshnet_forward(p2m_model_t* m, const p2m_params_t* P, const float* x, float* y, int B, int training,
                         void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
-  return meshnet_forward(m, P, x, y, B, training, workspace, workspace_bytes, stream, 0);
+  return meshnet_forward(m, P, nullptr, x, y, B, training, workspace, workspace_bytes, stream, 0);
 }
 
 int p2m_model_set_output_gather(p2m_model_t* m, const int32_t* vertex_of_slot, int n_slots) {
@@ -1170,7 +1209,7 @@ int p2m_meshnet_forward_vertices(p2m_model_t* m, const p2m_params_t* P, const fl
     set_error("meshnet_forward_vertices: call p2m_model_set_output_gather first");
     return P2M_ERR_INVALID;
   }
-  return meshnet_forward(m, P, x, y_vertices, B, 0, workspace, workspace_bytes, stream, 1);
+  return meshnet_forward(m, P, nullptr, x, y_vertices, B, 0, workspace, workspace_bytes, stream, 1);
 }
 
 static int forward_host_impl(p2m_model_t* m, const p2m_params_t* P, const float* x_host, float* y_host, int B,
@@ -1191,7 +1230,7 @@ static int forward_host_impl(p2m_model_t* m, const p2m_params_t* P, const float*
   }
   DeviceGuard guard(m->device);
   P2M_CUDA_OK(cudaMemcpyAsync(io.x, x_host, xb, cudaMemcpyHostToDevice, s));
-  P2M_TRY(meshnet_forward(m, P, io.x, io.y, B, 0, workspace, need, stream, gathered));
+  P2M_TRY(meshnet_forward(m, P, nullptr, io.x, io.y, B, 0, workspace, need, stream, gathered));
   P2M_CUDA_OK(cudaMemcpyAsync(y_host, io.y, yb, cudaMemcpyDeviceToHost, s));
   P2M_CUDA_OK(cudaStreamSynchronize(s));
   return check_kernel_status(m, "meshnet_forward_host");
@@ -1211,12 +1250,19 @@ int p2m_meshnet_forward_vertices_host(p2m_model_t* m, const p2m_params_t* P, con
 int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params_t* G, const float* x, const float* dy,
                          float* dx, int B, void* workspace, size_t workspace_bytes, void* scratch, size_t scratch_bytes,
                          p2m_stream_t stream) {
+  return p2m_meshnet_backward_opts(m, P, G, nullptr, x, dy, dx, B, workspace, workspace_bytes, scratch, scratch_bytes,
+                                   stream);
+}
+int p2m_meshnet_backward_opts(p2m_model_t* m, const p2m_params_t* P, const p2m_params_t* G, const p2m_bn_opts_t* bn_opts,
+                              const float* x, const float* dy, float* dx, int B, void* workspace,
+                              size_t workspace_bytes, void* scratch, size_t scratch_bytes, p2m_stream_t stream) {
   if (!m || !x || !dy || B <= 0 || !workspace || !scratch || m->layers.empty()) {
     set_error("meshnet_backward: bad argument");
     return P2M_ERR_INVALID;
   }
-  P2M_TRY(check_params(m, P, false));
-  P2M_TRY(check_params(m, G, false));
+  P2M_TRY(check_params(m, P, nullptr));
+  P2M_TRY(check_params(m, G, nullptr));
+  const std::vector<p2m_bn_opts_t> bn = resolve_bn_opts(m, 1, bn_opts);
   P2M_TRY(check_kernel_status(m, "meshnet_backward"));
   DeviceGuard guard(m->device);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1267,15 +1313,17 @@ int p2m_meshnet_backward(p2m_model_t* m, const p2m_params_t* P, const p2m_params
       bool have_scale = false;
       if (L.bn) {
         int tgt = (g_cur_buf >= 0 && g_cur_buf != keep_buf) ? g_cur_buf : free_buf(g_cur_buf, keep_buf, -1);
+        // frozen (running statistics): no batch-mean terms, and the conv bias gets sum_rows g_z
+        const bool frozen = bn[li].stats == P2M_BN_RUNNING;
         P2M_TRY(launch_bn_relu_bwd(w.z[li], g_cur, rows, L.fout, P->bn_w[li], w.scale[li], w.shift[li], w.mean[li],
                                    w.invstd[li], L.relu, sc.sums, G->bn_w[li], G->bn_b[li], sc.G[tgt], s,
-                                   want_scale ? sc.a_scale : nullptr));
+                                   want_scale ? sc.a_scale : nullptr, frozen, frozen ? G->cl_b[li] : nullptr));
         have_scale = want_scale;
         g_z = sc.G[tgt];
         gz_buf = tgt;
-        // the bias of a conv in front of a BatchNorm has a mathematically zero gradient (the batch mean removes
-        // it): db = sum_rows dz = 0 exactly, where the reference accumulates fp32 rounding noise
-        P2M_TRY(launch_fill_zero(G->cl_b[li], sizeof(float) * L.fout, s));
+        // with batch statistics the bias of a conv in front of a BatchNorm has a mathematically zero gradient (the
+        // batch mean removes it): db = sum_rows dz = 0 exactly, where the reference accumulates fp32 rounding noise
+        if (!frozen) P2M_TRY(launch_fill_zero(G->cl_b[li], sizeof(float) * L.fout, s));
       } else {
         P2M_TRY(launch_col_sum(g_z, rows, L.fout, sc.sums, G->cl_b[li], s));
       }
@@ -1477,7 +1525,7 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
       set_error("cheb_conv_fwd: running stats missing");
       return P2M_ERR_INVALID;
     }
-    P2M_TRY(launch_bn_fold_eval(a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var, a->bias, w.sc,
+    P2M_TRY(launch_bn_fold_eval(a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var, a->bias, 1e-5, w.sc,
                                 w.sc + L.fout, L.fout, s));
     ep.scale = w.sc;
     ep.shift = w.sc + L.fout;
@@ -1487,7 +1535,7 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
   ep.bias = a->bias;
   P2M_TRY(conv(ep, w.z));
   return bn_train_tail(w.z, (int)rows, L.fout, a->bn_weight, a->bn_bias, a->bn_running_mean, a->bn_running_var,
-                       a->bn_num_batches_tracked, w.sums, a->save_mean, a->save_invstd, w.sc, w.sc + L.fout, a->relu,
+                       a->bn_num_batches_tracked, bn_opts_default(P2M_BN_BATCH_UPDATE), w.sums, a->save_mean, a->save_invstd, w.sc, w.sc + L.fout, a->relu,
                        nullptr, 0, 0, nullptr, a->y, s);
 }
 

@@ -380,14 +380,36 @@ int launch_fill_zero(void* p, size_t bytes, cudaStream_t s);
 // y[b, dst[i], :] = y[b, src[i], :]  for i < n, b < batch  (y [batch, V, F])
 int launch_copy_rows(float* y, int batch, int V, int F, const int* dst, const int* src, int n, cudaStream_t s);
 
-// BatchNorm1d over rows (cheby_graph_conv.py:38-39; meshnet.py:55): eps 1e-5, momentum 0.1
+// BatchNorm1d over rows (cheby_graph_conv.py:38-39; meshnet.py:55).  Each BatchNorm's p2m_bn_opts_t decides its
+// statistics here, in the launchers, and nowhere else; bn_opts_default is torch's nn.BatchNorm1d in train mode.
+inline p2m_bn_opts_t bn_opts_default(int stats) {
+  p2m_bn_opts_t o;
+  o.stats = stats;
+  o.cumulative = 0;
+  o.momentum = 0.1;
+  o.eps = 1e-5;
+  return o;
+}
+// P2M_ERR_INVALID (with the error set) unless `o` is a valid record for a BatchNorm with these buffers
+int check_bn_opts(const p2m_bn_opts_t& o, const void* rm, const void* rv, const void* nbt, const char* where);
+// scale / shift from running statistics: ((z + bias) - rm) * scale + beta (bias may be null); save_mean / save_invstd
+// (optional) take rm and 1 / sqrt(rv + eps)
 int launch_bn_fold_eval(const float* gamma, const float* beta, const float* rm, const float* rv, const float* bias,
-                        float* scale, float* shift, int F, cudaStream_t s);
+                        double eps, float* scale, float* shift, int F, cudaStream_t s, float* save_mean = nullptr,
+                        float* save_invstd = nullptr);
 // sums of z - z[0] per channel (shifted: no cancellation for |mean| >> std); launch_bn_finalize reads the same z[0]
 int launch_col_stats(const float* z, int rows, int F, double* sums /*[2F] zeroed here*/, cudaStream_t s);
+// batch statistics -> save_mean / save_invstd / scale / shift; with o.stats == P2M_BN_BATCH_UPDATE also the running
+// statistics and num_batches_tracked (o.momentum, or 1 / num_batches_tracked with o.cumulative), never synchronising
 int launch_bn_finalize(const double* sums, const float* z, int rows, int F, const float* gamma, const float* beta,
-                       float* rm, float* rv, int64_t* nbt, float* save_mean, float* save_invstd, float* scale,
-                       float* shift, cudaStream_t s);
+                       float* rm, float* rv, int64_t* nbt, const p2m_bn_opts_t& o, float* save_mean,
+                       float* save_invstd, float* scale, float* shift, cudaStream_t s);
+// The forward statistics of one BatchNorm of z [rows, F] by its options: mean / invstd (what the backward reads) and
+// the scale / shift of a = z * scale + shift, from the running statistics (P2M_BN_RUNNING) or from the batch
+// (launch_col_stats + launch_bn_finalize)
+int launch_bn_stats(const float* z, int rows, int F, const float* gamma, const float* beta, float* rm, float* rv,
+                    int64_t* nbt, const p2m_bn_opts_t& o, double* sums /*[2F]*/, float* mean, float* invstd,
+                    float* scale, float* shift, cudaStream_t s);
 // a = relu?(z*scale+shift) (+ resampled residual)
 int launch_affine_act(const float* z, int rows, int F, const float* scale, const float* shift, int relu,
                       const float* res, int res_F, int res_unpool, const InterpTable* it, float* a, cudaStream_t s);
@@ -397,7 +419,9 @@ int launch_bn_relu_bwd(const float* z, const float* g_a, int rows, int F, const 
                        const float* shift, const float* mean, const float* invstd, int relu,
                        double* sums /*scratch: 2F doubles + 5F floats, 16-byte aligned*/, float* dgamma, float* dbeta,
                        float* g_z, cudaStream_t s,
-                       float* gz_scale_out = nullptr /* optional device scalar: launch_absmax_scale(g_z) fused in */);
+                       float* gz_scale_out = nullptr /* optional device scalar: launch_absmax_scale(g_z) fused in */,
+                       int frozen = 0 /* running statistics: g_z = gamma invstd g', no batch-mean terms */,
+                       float* dbias = nullptr /* frozen: sum_rows g_z, the gradient of the bias in front */);
 int launch_col_sum(const float* g, int rows, int F, double* scratch /*[F]*/, float* out, cudaStream_t s);
 
 // dX of the Chebyshev basis: given dT [rows,3F] (blocks dT0|dT1|dT2):

@@ -96,11 +96,11 @@ __global__ void __launch_bounds__(256) k_pn_transpose(const float* __restrict__ 
 __global__ void __launch_bounds__(256) k_bn_relu_rows(const float* __restrict__ x, long long n, int F,
                                                       const float* __restrict__ gamma, const float* __restrict__ beta,
                                                       const float* __restrict__ rm, const float* __restrict__ rv,
-                                                      float* __restrict__ y) {
+                                                      float eps, float* __restrict__ y) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int f = (int)(i % F);
-  const float sc = gamma[f] / sqrtf(rv[f] + 1e-5f);
+  const float sc = gamma[f] / sqrtf(rv[f] + eps);
   y[i] = fmaxf(fmaf(x[i] - rm[f], sc, beta[f]), 0.f);
 }
 // dst [rows, n_col] = src[:, :n_col] (row stride ld) + bias
@@ -215,26 +215,56 @@ struct Work {
   }
 };
 
+// every pointer but the running statistics, which check_bn checks against each BatchNorm's options
 bool params_ok(const p2m_posenet_params_t* P) {
   if (!P || P->num_joint <= 0 || P->hidden <= 0 || P->num_stage < 0 || !P->w1_w || !P->w1_b || !P->w2_w || !P->w2_b ||
       (P->num_stage > 0 && !P->stages))
     return false;
   for (int st = 0; st < P->num_stage; ++st) {
     const p2m_posenet_stage_t& S = P->stages[st];
-    if (!S.w1_w || !S.w1_b || !S.w2_w || !S.w2_b || !S.bn1_w || !S.bn1_b || !S.bn1_rm || !S.bn1_rv || !S.bn2_w ||
-        !S.bn2_b || !S.bn2_rm || !S.bn2_rv)
-      return false;
+    if (!S.w1_w || !S.w1_b || !S.w2_w || !S.w2_b || !S.bn1_w || !S.bn1_b || !S.bn2_w || !S.bn2_b) return false;
   }
   return true;
 }
 
-int check_call(const char* where, const p2m_posenet_params_t* P, int B, float p_dropout, bool pointers_ok,
-               size_t saved_bytes, size_t workspace_bytes) {
-  if (!pointers_ok || !params_ok(P) || B <= 0 || !(p_dropout >= 0.f && p_dropout <= 1.f)) {
+// The options of a call, resolved: one record per BatchNorm (stage s: bn1 at 2 s, bn2 at 2 s + 1) and one dropout p per
+// stage, the caller's or the defaults
+struct Modes {
+  std::vector<p2m_bn_opts_t> bn;
+  std::vector<float> p;
+  bool batch_stats;  // some BatchNorm uses batch statistics (the defaults of a training call: always, also at 0 stages)
+  Modes(int num_stage, const p2m_bn_opts_t* opts, int default_stats, const float* p_stage, float p_all)
+      : bn(2 * (size_t)std::max(num_stage, 0), bn_opts_default(default_stats)),
+        p((size_t)std::max(num_stage, 0), p_all), batch_stats(!opts && default_stats != P2M_BN_RUNNING) {
+    for (size_t i = 0; opts && i < bn.size(); ++i) bn[i] = opts[i];
+    for (size_t i = 0; p_stage && i < p.size(); ++i) p[i] = p_stage[i];
+    for (const p2m_bn_opts_t& o : bn) batch_stats = batch_stats || o.stats != P2M_BN_RUNNING;
+  }
+  const p2m_bn_opts_t& of(int st, int which) const { return bn[2 * st + which]; }
+};
+
+// each BatchNorm's options against its buffers (extra: the num_batches_tracked pointers, may be null)
+int check_bn(const char* where, const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra, const Modes& md) {
+  for (int st = 0; st < P->num_stage; ++st) {
+    const p2m_posenet_stage_t& S = P->stages[st];
+    const p2m_posenet_train_stage_t* X = extra ? &extra->stages[st] : nullptr;
+    P2M_TRY(check_bn_opts(md.of(st, 0), S.bn1_rm, S.bn1_rv, X ? X->bn1_nbt : nullptr, where));
+    P2M_TRY(check_bn_opts(md.of(st, 1), S.bn2_rm, S.bn2_rv, X ? X->bn2_nbt : nullptr, where));
+  }
+  return P2M_OK;
+}
+
+// forward: the options are checked against the buffers too (the backward reads the saved statistics, not them)
+int check_call(const char* where, const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra, bool forward, int B,
+               const Modes& md, bool pointers_ok, size_t saved_bytes, size_t workspace_bytes) {
+  bool p_ok = true;
+  for (float p : md.p) p_ok = p_ok && p >= 0.f && p <= 1.f;
+  if (!pointers_ok || !params_ok(P) || B <= 0 || !p_ok) {
     set_error(std::string(where) + ": bad argument");
     return P2M_ERR_INVALID;
   }
-  if (B < 2) {
+  if (forward) P2M_TRY(check_bn(where, P, extra, md));
+  if (B < 2 && md.batch_stats) {
     set_error(std::string(where) + ": train-mode BatchNorm needs more than one value per channel (batch of 1)");
     return P2M_ERR_INVALID;
   }
@@ -335,8 +365,19 @@ size_t p2m_posenet_workspace_bytes(int batch, int hidden) {
 
 int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, float* pose3d, float* pose_combine, int B,
                         void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  return p2m_posenet_forward_opts(P, nullptr, pose2d, pose3d, pose_combine, B, workspace, workspace_bytes, stream);
+}
+int p2m_posenet_forward_opts(const p2m_posenet_params_t* P, const p2m_bn_opts_t* bn, const float* pose2d,
+                             float* pose3d, float* pose_combine, int B, void* workspace, size_t workspace_bytes,
+                             p2m_stream_t stream) {
   if (!params_ok(P) || !pose2d || !pose3d || B <= 0 || !workspace) {
     set_error("posenet_forward: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  const Modes md(P->num_stage, bn, P2M_BN_RUNNING, nullptr, 0.f);
+  P2M_TRY(check_bn("posenet_forward", P, nullptr, md));
+  if (md.batch_stats) {
+    set_error("posenet_forward: the eval forward needs running statistics in every BatchNorm (P2M_BN_RUNNING)");
     return P2M_ERR_INVALID;
   }
   if (workspace_bytes < p2m_posenet_workspace_bytes(B, P->hidden)) {
@@ -365,10 +406,11 @@ int p2m_posenet_forward(const p2m_posenet_params_t* P, const float* pose2d, floa
     const p2m_posenet_stage_t& S = P->stages[st];
     // a = relu(bn1(y))
     const long long n = (long long)B * H;
-    k_bn_relu_rows<<<blocks(n), 256, 0, s>>>(w.y, n, H, S.bn1_w, S.bn1_b, S.bn1_rm, S.bn1_rv, w.a);
+    k_bn_relu_rows<<<blocks(n), 256, 0, s>>>(w.y, n, H, S.bn1_w, S.bn1_b, S.bn1_rm, S.bn1_rv, (float)md.of(st, 0).eps,
+                                             w.a);
     P2M_LAUNCH_OK();
     // h = relu(bn2(a Wa^T + ba)): BatchNorm folded into the GEMM epilogue
-    P2M_TRY(launch_bn_fold_eval(S.bn2_w, S.bn2_b, S.bn2_rm, S.bn2_rv, S.w1_b, w.sc, w.sc + H, H, s));
+    P2M_TRY(launch_bn_fold_eval(S.bn2_w, S.bn2_b, S.bn2_rm, S.bn2_rv, S.w1_b, md.of(st, 1).eps, w.sc, w.sc + H, H, s));
     Epilogue ea;
     ea.scale = w.sc;
     ea.shift = w.sc + H;
@@ -394,12 +436,15 @@ size_t p2m_posenet_train_saved_bytes(int batch, int num_joint, int hidden, int n
   return Saved(nullptr, Plan(batch, num_joint, hidden, num_stage)).bytes;
 }
 
-int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra, const float* pose2d, int B,
-                              float p_dropout, const int64_t* seed, float* pose3d, float* pose_combine, void* saved,
-                              size_t saved_bytes, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
-  P2M_TRY(check_call("posenet_train_forward", P, B, p_dropout,
-                     pose2d && seed && pose3d && saved && workspace && (!P || P->num_stage == 0 || (extra && extra->stages)),
-                     saved_bytes, workspace_bytes));
+}  // extern "C"
+
+namespace {
+int train_forward(const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra, const Modes& md, const float* pose2d,
+                  int B, const int64_t* seed, float* pose3d, float* pose_combine, void* saved, size_t saved_bytes,
+                  void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  const bool extra_ok = !P || P->num_stage == 0 || (extra && extra->stages);
+  P2M_TRY(check_call("posenet_train_forward", P, extra_ok ? extra : nullptr, true, B, md,
+                     pose2d && seed && pose3d && saved && workspace && extra_ok, saved_bytes, workspace_bytes));
   int dev;
   P2M_TRY(arrays_device("posenet_train_forward", {pose2d, seed, pose3d, pose_combine, saved, workspace}, &dev));
   DeviceGuard guard(dev);
@@ -421,22 +466,20 @@ int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_t
     const p2m_posenet_train_stage_t& X = extra->stages[st];
     const float* y = sv.y[st];
     // a = drop(relu(bn1(y)))
-    P2M_TRY(launch_col_stats(y, B, H, w.sums, s));
-    P2M_TRY(launch_bn_finalize(w.sums, y, B, H, S.bn1_w, S.bn1_b, const_cast<float*>(S.bn1_rm),
-                               const_cast<float*>(S.bn1_rv), X.bn1_nbt, sv.stat(st, 0, 0), sv.stat(st, 0, 1),
-                               sv.stat(st, 0, 2), sv.stat(st, 0, 3), s));
-    P2M_TRY(bn_relu_drop(y, plan, w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), make_dropout(p_dropout, seed, 2 * st), w.a,
+    P2M_TRY(launch_bn_stats(y, B, H, S.bn1_w, S.bn1_b, const_cast<float*>(S.bn1_rm), const_cast<float*>(S.bn1_rv),
+                            X.bn1_nbt, md.of(st, 0), w.sums, sv.stat(st, 0, 0), sv.stat(st, 0, 1), sv.stat(st, 0, 2),
+                            sv.stat(st, 0, 3), s));
+    P2M_TRY(bn_relu_drop(y, plan, w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), make_dropout(md.p[st], seed, 2 * st), w.a,
                          s));
     // z2 = a Wa^T + ba;  a = drop(relu(bn2(z2)))
     Epilogue ea;
     ea.bias = S.w1_b;
     P2M_TRY(gemm.forward(w.a, S.w1_w, ea, sv.z2[st]));
-    P2M_TRY(launch_col_stats(sv.z2[st], B, H, w.sums, s));
-    P2M_TRY(launch_bn_finalize(w.sums, sv.z2[st], B, H, S.bn2_w, S.bn2_b, const_cast<float*>(S.bn2_rm),
-                               const_cast<float*>(S.bn2_rv), X.bn2_nbt, sv.stat(st, 1, 0), sv.stat(st, 1, 1),
-                               sv.stat(st, 1, 2), sv.stat(st, 1, 3), s));
+    P2M_TRY(launch_bn_stats(sv.z2[st], B, H, S.bn2_w, S.bn2_b, const_cast<float*>(S.bn2_rm),
+                            const_cast<float*>(S.bn2_rv), X.bn2_nbt, md.of(st, 1), w.sums, sv.stat(st, 1, 0),
+                            sv.stat(st, 1, 1), sv.stat(st, 1, 2), sv.stat(st, 1, 3), s));
     P2M_TRY(bn_relu_drop(sv.z2[st], plan, w, sv.stat(st, 1, 2), sv.stat(st, 1, 3),
-                         make_dropout(p_dropout, seed, 2 * st + 1), w.a, s));
+                         make_dropout(md.p[st], seed, 2 * st + 1), w.a, s));
     // y' = y + a Wb^T + bb
     Epilogue eb;
     eb.bias = S.w2_b;
@@ -448,16 +491,16 @@ int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_t
                       pose_combine, s);
 }
 
-int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int B, float p_dropout, const int64_t* seed,
-                         const void* saved, size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
-                         float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+int backward(const p2m_posenet_params_t* P, const Modes& md, const float* pose2d, int B, const int64_t* seed,
+             const void* saved, size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
+             float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
   bool ok = pose2d && seed && saved && d_pose3d && workspace && G && G->w1_w && G->w1_b && G->w2_w && G->w2_b && P &&
             (P->num_stage <= 0 || G->stages);
   for (int st = 0; ok && st < P->num_stage; ++st) {
     const p2m_posenet_stage_grads_t& g = G->stages[st];
     ok = g.w1_w && g.w1_b && g.w2_w && g.w2_b && g.bn1_w && g.bn1_b && g.bn2_w && g.bn2_b;
   }
-  P2M_TRY(check_call("posenet_backward", P, B, p_dropout, ok, saved_bytes, workspace_bytes));
+  P2M_TRY(check_call("posenet_backward", P, nullptr, false, B, md, ok, saved_bytes, workspace_bytes));
   int dev;
   P2M_TRY(arrays_device("posenet_backward", {pose2d, seed, saved, d_pose3d, d_pose2d, workspace}, &dev));
   DeviceGuard guard(dev);
@@ -480,7 +523,8 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
   for (int st = plan.S - 1; st >= 0; --st) {
     const p2m_posenet_stage_t& S = P->stages[st];
     const p2m_posenet_stage_grads_t& D = G->stages[st];
-    const Dropout d1 = make_dropout(p_dropout, seed, 2 * st), d2 = make_dropout(p_dropout, seed, 2 * st + 1);
+    const Dropout d1 = make_dropout(md.p[st], seed, 2 * st), d2 = make_dropout(md.p[st], seed, 2 * st + 1);
+    const int frozen1 = md.of(st, 0).stats == P2M_BN_RUNNING, frozen2 = md.of(st, 1).stats == P2M_BN_RUNNING;
     // second Linear: y' = y + a2 Wb^T + bb with a2 = drop(relu(bn2(z2))) recomputed; g = dL/dy'
     P2M_TRY(launch_col_sum(w.g, B, H, w.sums, D.w2_b, s));
     P2M_TRY(bn_relu_drop(sv.z2[st], plan, w, sv.stat(st, 1, 2), sv.stat(st, 1, 3), d2, w.a, s));
@@ -491,7 +535,8 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
     k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.t, n, d2);
     P2M_LAUNCH_OK();
     P2M_TRY(launch_bn_relu_bwd(sv.z2[st], w.t, B, H, S.bn2_w, sv.stat(st, 1, 2), sv.stat(st, 1, 3), sv.stat(st, 1, 0),
-                               sv.stat(st, 1, 1), 1, w.sums, D.bn2_w, D.bn2_b, w.t, s, plan.tc ? w.g_scale : nullptr));
+                               sv.stat(st, 1, 1), 1, w.sums, D.bn2_w, D.bn2_b, w.t, s, plan.tc ? w.g_scale : nullptr,
+                               frozen2));
     // first Linear: z2 = a1 Wa^T + ba with a1 = drop(relu(bn1(y))) recomputed
     P2M_TRY(launch_col_sum(w.t, B, H, w.sums, D.w1_b, s));
     P2M_TRY(bn_relu_drop(sv.y[st], plan, w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), d1, w.a, s));
@@ -502,7 +547,7 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
     k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.a, n, d1);
     P2M_LAUNCH_OK();
     P2M_TRY(launch_bn_relu_bwd(sv.y[st], w.a, B, H, S.bn1_w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), sv.stat(st, 0, 0),
-                               sv.stat(st, 0, 1), 1, w.sums, D.bn1_w, D.bn1_b, w.a, s));
+                               sv.stat(st, 0, 1), 1, w.sums, D.bn1_w, D.bn1_b, w.a, s, nullptr, frozen1));
     k_pn_add<<<blocks(n), 256, 0, s>>>(w.g, w.a, n);
     P2M_LAUNCH_OK();
   }
@@ -513,6 +558,38 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
   if (d_pose2d != nullptr)
     P2M_TRY(launch_gemm(w.g, H, P->w1_w, 2 * J, 1, d_pose2d, 2 * J, B, 2 * J, H, Epilogue(), s));
   return P2M_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int p2m_posenet_train_forward(const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra, const float* pose2d, int B,
+                              float p_dropout, const int64_t* seed, float* pose3d, float* pose_combine, void* saved,
+                              size_t saved_bytes, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  const Modes md(P ? P->num_stage : 0, nullptr, P2M_BN_BATCH_UPDATE, nullptr, p_dropout);
+  return train_forward(P, extra, md, pose2d, B, seed, pose3d, pose_combine, saved, saved_bytes, workspace,
+                       workspace_bytes, stream);
+}
+int p2m_posenet_train_forward_opts(const p2m_posenet_params_t* P, const p2m_posenet_train_t* extra,
+                                   const p2m_bn_opts_t* bn, const float* p_dropout, const float* pose2d, int B,
+                                   const int64_t* seed, float* pose3d, float* pose_combine, void* saved,
+                                   size_t saved_bytes, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  const Modes md(P ? P->num_stage : 0, bn, P2M_BN_BATCH_UPDATE, p_dropout, 0.f);
+  return train_forward(P, extra, md, pose2d, B, seed, pose3d, pose_combine, saved, saved_bytes, workspace,
+                       workspace_bytes, stream);
+}
+int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int B, float p_dropout, const int64_t* seed,
+                         const void* saved, size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
+                         float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+  const Modes md(P ? P->num_stage : 0, nullptr, P2M_BN_BATCH_UPDATE, nullptr, p_dropout);
+  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream);
+}
+int p2m_posenet_backward_opts(const p2m_posenet_params_t* P, const p2m_bn_opts_t* bn, const float* p_dropout,
+                              const float* pose2d, int B, const int64_t* seed, const void* saved, size_t saved_bytes,
+                              const float* d_pose3d, const p2m_posenet_grads_t* G, float* d_pose2d, void* workspace,
+                              size_t workspace_bytes, p2m_stream_t stream) {
+  const Modes md(P ? P->num_stage : 0, bn, P2M_BN_BATCH_UPDATE, p_dropout, 0.f);
+  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

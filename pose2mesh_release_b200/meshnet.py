@@ -197,7 +197,9 @@ def _param_table(fc_w, fc_b, cl_w, cl_b, bn_w, bn_b, bn_rm=None, bn_rv=None, bn_
 
 
 class _MeshNetFunction(torch.autograd.Function):
-    """Pose2Mesh.forward / backward through p2m_meshnet_forward / p2m_meshnet_backward."""
+    """Pose2Mesh.forward / backward through p2m_meshnet_forward_opts / p2m_meshnet_backward_opts.  ``buffers`` is
+    (running means, running vars, num_batches_tracked[, per-layer _lib.BnOpts array]); without the options array every
+    BatchNorm takes the defaults of ``training`` (batch statistics with update, or running statistics)."""
 
     @staticmethod
     def forward(ctx, x, hier: BakedHierarchy, training: bool, buffers, n_layers, *params):
@@ -210,18 +212,19 @@ class _MeshNetFunction(torch.autograd.Function):
         n_bn = n_layers - 1
         bn_w = list(params[2 + 2 * n_layers:2 + 2 * n_layers + n_bn]) + [None]
         bn_b = list(params[2 + 2 * n_layers + n_bn:2 + 2 * n_layers + 2 * n_bn]) + [None]
-        bn_rm, bn_rv, bn_nbt = buffers
+        bn_rm, bn_rv, bn_nbt, *rest = buffers
+        opts = rest[0] if rest else None
         B = x.shape[0]
         v0 = int(hier.level_size[0])
         cout = int(hier.block_chans[-1])
         y = torch.empty((B, v0, cout), device=dev, dtype=torch.float32)
-        ws_bytes = lib.p2m_meshnet_workspace_bytes(h, B, int(training))
+        ws_bytes = lib.p2m_meshnet_workspace_bytes_opts(h, B, int(training), opts)
         ws = torch.empty(ws_bytes, device=dev, dtype=torch.uint8)
         table = _param_table(fc_w, fc_b, cl_w, cl_b, bn_w, bn_b, bn_rm, bn_rv, bn_nbt)
-        _lib.call("p2m_meshnet_forward", dev, h, C.byref(table), x, y, B, int(training), ws, ws_bytes)
+        _lib.call("p2m_meshnet_forward_opts", dev, h, C.byref(table), opts, x, y, B, int(training), ws, ws_bytes)
         needs_grad = training and any(ctx.needs_input_grad)
-        if needs_grad:
-            ctx.hier, ctx.n_layers, ctx.ws, ctx.ws_bytes = hier, n_layers, ws, ws_bytes
+        if needs_grad:  # the backward takes the options of this forward
+            ctx.hier, ctx.n_layers, ctx.ws, ctx.ws_bytes, ctx.bn_opts = hier, n_layers, ws, ws_bytes, opts
             ctx.save_for_backward(x, *params)
         ctx.differentiable = needs_grad
         ctx.training = training
@@ -266,8 +269,8 @@ class _MeshNetFunction(torch.autograd.Function):
         dx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
         sc_bytes = lib.p2m_meshnet_backward_scratch_bytes(h, B)
         scratch = torch.empty(sc_bytes, device=dev, dtype=torch.uint8)
-        _lib.call("p2m_meshnet_backward", dev, h, C.byref(ptab), C.byref(gtab), x, dy, dx, B, ctx.ws, ctx.ws_bytes,
-                  scratch, sc_bytes)
+        _lib.call("p2m_meshnet_backward_opts", dev, h, C.byref(ptab), C.byref(gtab), ctx.bn_opts, x, dy, dx, B, ctx.ws,
+                  ctx.ws_bytes, scratch, sc_bytes)
         ctx.ws = None
         return (dx, None, None, None, None, *grads)
 
@@ -336,7 +339,30 @@ class Pose2Mesh(nn.Module):
         nbt = [None if m is None else m.num_batches_tracked for m in self.bn]
         return rm, rv, nbt
 
+    def _bn_opts(self):
+        """One p2m_bn_opts_t per layer from each BatchNorm's own state (training flag, track_running_stats, momentum,
+        eps), read on every forward; the last layer's entry (no BatchNorm) is ignored by the library.  ValueError for
+        a BatchNorm the native kernels do not implement."""
+        opts = (_lib.BnOpts * len(self.cl))()
+        for i, m in enumerate(self.bn):
+            if i == len(self.cl) - 1:
+                opts[i].stats = _lib.P2M_BN_RUNNING
+            else:
+                opts[i] = _lib.bn_opts(m)
+        return opts
+
+    def _check_eval_bn(self, what: str, modes: bool):
+        """The inference entry points run the eval schedule with the defaults: running statistics and eps 1e-5 in
+        every BatchNorm (modes: each BatchNorm must also be in eval mode)."""
+        for m in self.bn[:len(self.cl) - 1]:
+            o = _lib.bn_opts(m)
+            if m.running_mean is None or m.running_var is None or o.eps != 1e-5 or (
+                    modes and o.stats != _lib.P2M_BN_RUNNING):
+                raise ValueError(f"{what} needs every BatchNorm in eval mode with running statistics and eps 1e-5; "
+                                 "use forward() for other BatchNorm settings")
+
     def forward(self, x):
+        opts = self._bn_opts()
         n_joint = self.graph_L[-1].shape[0]
         x = x.view(-1, n_joint, self.num_joint_input_chan)
         if not x.is_cuda:
@@ -350,7 +376,7 @@ class Pose2Mesh(nn.Module):
             if p.dtype != torch.float32 or not p.is_contiguous():
                 raise RuntimeError("pose2mesh_release_b200.Pose2Mesh needs contiguous float32 parameters "
                                    f"(got {p.dtype}); the library reads them through raw device pointers")
-        return _MeshNetFunction.apply(x, self._hier, self.training, self._bn_buffers(), n, *params)
+        return _MeshNetFunction.apply(x, self._hier, self.training, (*self._bn_buffers(), opts), n, *params)
 
     @torch.no_grad()
     def forward_vertices(self, x: torch.Tensor, perm_reverse, n_vertex: int) -> torch.Tensor:
@@ -360,6 +386,7 @@ class Pose2Mesh(nn.Module):
         lib = _lib.load()
         if self.training:
             raise RuntimeError("forward_vertices is an inference entry point: call .eval() first")
+        self._check_eval_bn("forward_vertices", True)
         n_joint = self.graph_L[-1].shape[0]
         x = x.view(-1, n_joint, self.num_joint_input_chan)
         if not x.is_cuda:
@@ -398,6 +425,7 @@ class Pose2Mesh(nn.Module):
         ``pred[:, perm_reverse[:n_vertex]]`` (lib/core/base.py:130,201) is fused into the head layer and only the
         ``[B, n_vertex, 3]`` vertices travel back (p2m_meshnet_forward_vertices_host).  bench.py's end-to-end figure."""
         lib = _lib.load()
+        self._check_eval_bn("forward_host", False)
         dev = self.fc.weight.device if device is None else torch.device(device)
         h = self._hier.handle(dev.index)
         n_joint = self.graph_L[-1].shape[0]

@@ -6,8 +6,9 @@
 so PoseNet checkpoints load unchanged.  In eval mode (what FlatPose2Mesh uses for inference, demo/run.py:168) the
 forward runs in libp2m_b200.so (``p2m_posenet_forward``: fp32 GEMMs with the BatchNorm / ReLU / residual fused into
 their epilogues).  In training mode (dropout + batch statistics: lib/core/base.py:116, and the PoseNet pre-training of
-:246-265) forward and backward run there too (``p2m_posenet_train_forward`` / ``p2m_posenet_backward``) for contiguous
-float32 CUDA tensors; the dropout mask follows the rule stated in include/p2m_b200.h, not torch's generator stream.
+:246-265) forward and backward run there too (``p2m_posenet_train_forward_opts`` / ``p2m_posenet_backward_opts``) for
+contiguous float32 CUDA tensors; the dropout mask follows the rule stated in include/p2m_b200.h, not torch's generator
+stream.  Every BatchNorm and each stage's Dropout act by their own state (frozen statistics, momentum, eps, p).
 Anything else (CPU tensors, other dtypes, gradients through an eval-mode forward) runs the reference's torch ops.
 """
 from __future__ import annotations
@@ -50,26 +51,34 @@ class Linear(nn.Module):
         return x + y
 
 
+def _train_forward(module, x, seed, with_combine, modes):
+    """p2m_posenet_train_forward_opts: (pose3d, pose_combine or None, saved).  modes = (BnOpts [2 S], float [S])."""
+    lib = _lib.load()
+    dev, B = x.device, x.shape[0]
+    dims = (B, module.num_joint, module.linear_size, module.num_stage)
+    out = torch.empty((B, module.output_size), device=dev, dtype=torch.float32)
+    comb = torch.empty((B, module.num_joint, 5), device=dev, dtype=torch.float32) if with_combine else None
+    n_saved, n_ws = lib.p2m_posenet_train_saved_bytes(*dims), lib.p2m_posenet_train_workspace_bytes(*dims)
+    saved = torch.empty(n_saved, device=dev, dtype=torch.uint8)
+    ws = torch.empty(n_ws, device=dev, dtype=torch.uint8)
+    native = module._native_params()
+    extra = module._native_train_extra()
+    _lib.call("p2m_posenet_train_forward_opts", dev, C.byref(native), C.byref(extra), modes[0], modes[1], x, B, seed,
+              out, comb, saved, n_saved, ws, n_ws)
+    return out, comb, saved
+
+
 class _PoseNetTrainFunction(torch.autograd.Function):
-    """LinearModel's train-mode forward / backward through p2m_posenet_train_forward / p2m_posenet_backward.
-    params: w1.weight, w1.bias, w2.weight, w2.bias, then per stage w1.weight, w1.bias, w2.weight, w2.bias,
-    batch_norm1.weight, batch_norm1.bias, batch_norm2.weight, batch_norm2.bias."""
+    """LinearModel's train-mode forward / backward through p2m_posenet_train_forward_opts / p2m_posenet_backward_opts.
+    modes: LinearModel._native_modes() of the forward, which the backward takes too.  params: w1.weight, w1.bias,
+    w2.weight, w2.bias, then per stage w1.weight, w1.bias, w2.weight, w2.bias, batch_norm1.weight, batch_norm1.bias,
+    batch_norm2.weight, batch_norm2.bias."""
 
     @staticmethod
-    def forward(ctx, module, x, seed, with_combine, *params):
-        lib = _lib.load()
-        dev, B = x.device, x.shape[0]
-        dims = (B, module.num_joint, module.linear_size, module.num_stage)
-        out = torch.empty((B, module.output_size), device=dev, dtype=torch.float32)
-        comb = torch.empty((B, module.num_joint, 5), device=dev, dtype=torch.float32) if with_combine else None
-        n_saved, n_ws = lib.p2m_posenet_train_saved_bytes(*dims), lib.p2m_posenet_train_workspace_bytes(*dims)
-        saved = torch.empty(n_saved, device=dev, dtype=torch.uint8)
-        ws = torch.empty(n_ws, device=dev, dtype=torch.uint8)
-        native = module._native_params()
-        extra = module._native_train_extra()
-        _lib.call("p2m_posenet_train_forward", dev, C.byref(native), C.byref(extra), x, B, module.p_dropout, seed, out,
-                  comb, saved, n_saved, ws, n_ws)
-        ctx.module, ctx.saved, ctx.dims = module, saved, dims
+    def forward(ctx, module, x, seed, with_combine, modes, *params):
+        dims = (x.shape[0], module.num_joint, module.linear_size, module.num_stage)
+        out, comb, saved = _train_forward(module, x, seed, with_combine, modes)
+        ctx.module, ctx.saved, ctx.dims, ctx.modes = module, saved, dims, modes
         ctx.save_for_backward(x, seed, *params)
         if comb is None:
             return out
@@ -96,10 +105,10 @@ class _PoseNetTrainFunction(torch.autograd.Function):
         n_ws = lib.p2m_posenet_train_workspace_bytes(*ctx.dims)
         ws = torch.empty(n_ws, device=dev, dtype=torch.uint8)
         native = module._native_params()
-        _lib.call("p2m_posenet_backward", dev, C.byref(native), x, ctx.dims[0], module.p_dropout, seed, ctx.saved,
-                  ctx.saved.numel(), d_out.contiguous().float(), C.byref(g), dx, ws, n_ws)
+        _lib.call("p2m_posenet_backward_opts", dev, C.byref(native), ctx.modes[0], ctx.modes[1], x, ctx.dims[0], seed,
+                  ctx.saved, ctx.saved.numel(), d_out.contiguous().float(), C.byref(g), dx, ws, n_ws)
         ctx.saved = None
-        return (None, dx, None, None, *grads)
+        return (None, dx, None, None, None, *grads)
 
 
 class LinearModel(nn.Module):
@@ -127,6 +136,8 @@ class LinearModel(nn.Module):
                     st.batch_norm1.weight, st.batch_norm1.bias, st.batch_norm1.running_mean, st.batch_norm1.running_var,
                     st.batch_norm2.weight, st.batch_norm2.bias, st.batch_norm2.running_mean, st.batch_norm2.running_var]
             for (name, _), t in zip(_lib.PoseNetStage._fields_, vals):
+                if t is None:  # the running statistics of a BatchNorm without them (track_running_stats=False)
+                    continue
                 if t.dtype != torch.float32 or not t.is_contiguous():
                     raise RuntimeError("PoseNet parameters must be contiguous float32")
                 setattr(stages[i], name, t.data_ptr())
@@ -139,10 +150,27 @@ class LinearModel(nn.Module):
         p._keep = (stages, keep)
         return p
 
+    def _native_modes(self):
+        """(BnOpts [2 num_stage], float [num_stage]): each stage's bn1 / bn2 options and its Dropout's p (0 in eval
+        mode) from the submodules' current state.  ValueError for a submodule the native kernels do not implement."""
+        bn = (_lib.BnOpts * (2 * self.num_stage))()
+        p = (C.c_float * self.num_stage)()
+        for i, st in enumerate(self.linear_stages):
+            bn[2 * i], bn[2 * i + 1] = _lib.bn_opts(st.batch_norm1), _lib.bn_opts(st.batch_norm2)
+            p[i] = _lib.dropout_p(st.dropout)
+        return bn, p
+
+    @staticmethod
+    def _batch_stats(modes) -> bool:
+        return any(o.stats != _lib.P2M_BN_RUNNING for o in modes[0])
+
     def forward_native(self, x: torch.Tensor, with_combine: bool = False):
         """Eval forward in libp2m_b200.so.  x [B, 2J] (or [B, J, 2]) on the module's CUDA device -> pose3d [B, 3J];
         with_combine additionally returns pose_combine = cat(pose2d, pose3d / 1000) [B, J, 5]
-        (lib/models/pose2mesh_net.py:18-19)."""
+        (lib/models/pose2mesh_net.py:18-19).  Each BatchNorm and Dropout acts by its own state: when one uses batch
+        statistics or drops (e.g. a BatchNorm without running buffers), the training forward's kernels run instead,
+        without a backward."""
+        modes = self._native_modes()
         lib = _lib.load()
         _lib.cuda_tensor(x, "x")
         x = x.reshape(len(x), -1).contiguous().float()
@@ -151,12 +179,16 @@ class LinearModel(nn.Module):
         dev, B = x.device, x.shape[0]
         if self.w1.weight.device != dev:
             raise RuntimeError("parameters and input live on different devices")
+        if self._batch_stats(modes) or any(p > 0 for p in modes[1]):
+            seed = torch.empty(2, dtype=torch.int64, device=dev).random_()
+            out, comb, _ = _train_forward(self, x, seed, with_combine, modes)
+            return (out, comb) if with_combine else out
         out = torch.empty((B, self.output_size), device=dev, dtype=torch.float32)
         comb = torch.empty((B, self.num_joint, 5), device=dev, dtype=torch.float32) if with_combine else None
         nbytes = lib.p2m_posenet_workspace_bytes(B, self.linear_size)
         ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
         params = self._native_params()
-        _lib.call("p2m_posenet_forward", dev, C.byref(params), x, out, comb, B, ws, nbytes)
+        _lib.call("p2m_posenet_forward_opts", dev, C.byref(params), modes[0], x, out, comb, B, ws, nbytes)
         return (out, comb) if with_combine else out
 
     def _native_train_extra(self):
@@ -181,32 +213,33 @@ class LinearModel(nn.Module):
 
     def native_train_ok(self, x: torch.Tensor) -> bool:
         """Whether the train-mode forward of x runs in libp2m_b200.so: x, the trained tensors and the BatchNorm running
-        statistics are contiguous float32 CUDA tensors on one device."""
+        statistics (where a BatchNorm has them) are contiguous float32 CUDA tensors on one device."""
         if not (x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()):
             return False
         tensors = self._trained_tensors()
         for st in self.linear_stages:
             for bn in (st.batch_norm1, st.batch_norm2):
-                if bn.running_mean is None or bn.running_var is None:
-                    return False
-                tensors += [bn.running_mean, bn.running_var]
+                tensors += [t for t in (bn.running_mean, bn.running_var) if t is not None]
         return all(t.device == x.device and t.dtype == torch.float32 and t.is_contiguous() for t in tensors)
 
     def forward_train_native(self, x: torch.Tensor, seed: torch.Tensor = None, with_combine: bool = False):
         """Train-mode forward in libp2m_b200.so, differentiable (the backward runs there too).  x [B, 2J] (or
         [B, J, 2]) -> pose3d [B, 3J]; with_combine additionally returns the detached pose_combine [B, J, 5].  seed:
         two int64 on x's device that define the dropout masks (include/p2m_b200.h); drawn from torch's generator when
-        not given, so torch.manual_seed reproduces a run.  Updates the BatchNorm running statistics."""
+        not given, so torch.manual_seed reproduces a run.  Each BatchNorm and each stage's Dropout acts by its own state
+        (train / eval, track_running_stats, momentum, eps, p): an eval-mode BatchNorm keeps its running statistics
+        (frozen), a train-mode one with track_running_stats updates them."""
+        modes = self._native_modes()
         x = x.reshape(len(x), -1)
         if not self.native_train_ok(x):
             raise RuntimeError("the native train-mode PoseNet needs contiguous float32 CUDA tensors on one device")
         if x.shape[1] != self.input_size:
             raise ValueError(f"PoseNet expects {self.input_size} inputs per pose, got {x.shape[1]}")
-        if x.shape[0] < 2:
+        if x.shape[0] < 2 and self._batch_stats(modes):
             raise ValueError(f"Expected more than 1 value per channel when training, got input size {tuple(x.shape)}")
         if seed is None:
             seed = torch.empty(2, dtype=torch.int64, device=x.device).random_()
-        return _PoseNetTrainFunction.apply(self, x, seed, with_combine, *self._trained_tensors())
+        return _PoseNetTrainFunction.apply(self, x, seed, with_combine, modes, *self._trained_tensors())
 
     def _forward_torch(self, x):
         """The reference's own op sequence (lib/models/posenet.py:77-87)."""
