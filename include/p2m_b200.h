@@ -377,6 +377,10 @@ int p2m_posenet_backward_opts(const p2m_posenet_params_t* params, const p2m_bn_o
  * p2m_meshnet_forward_vertices.                                                                        */
 int p2m_regress_joints(const float* joint_regressor, const float* vertices, float* joints, int batch, int n_joint,
                        int n_vertex, int chans, p2m_stream_t stream);
+/* Its backward: d_vertices [B, n_vertex, C] = joint_regressor^T @ d_joints [B, n_joint, C] (written, not accumulated;
+ * one thread per (mesh, vertex) walks the joints in order: no atomics, bitwise reproducible). */
+int p2m_regress_joints_backward(const float* joint_regressor, const float* d_joints, float* d_vertices, int batch,
+                                int n_joint, int n_vertex, int chans, p2m_stream_t stream);
 /* The demo's input normalisation (demo/run.py:150-158): joints_px [B, J, 2] in image pixels -> pose2d [B, J, 2],
  * zero mean / unit std per pose and coordinate in the aspect-preserving box of the (input_h, input_w) network input
  * (cfg.MODEL.input_shape = (384, 288)).  truncate_like_int_input = 1 reproduces the reference on INTEGER joint
@@ -395,6 +399,50 @@ int p2m_mesh_losses(const float* coord_out, const float* coord_gt, const int32_t
  * grad_out (optional, n floats) = grad_scale[0] * sign(.) * valid.                                        */
 int p2m_coord_loss(const float* pred, const float* target, const float* valid, int64_t n, const float* grad_scale,
                    double* sum, float* grad_out, p2m_stream_t stream);
+
+/* ---- the Trainer's objective (lib/core/base.py:129-143) ---------------------------------------------------
+ * With x = cam_mesh[:, perm_reverse[:n_vertex]] (the real rows of the padded output) and pred_pose = J (1000 x):
+ *   loss1 = mean |x m - gt_mesh m|                               m = mesh_valid [B, n_vertex] (per vertex)
+ *   loss2 = w_normal NormalVectorLoss(x, gt_mesh)
+ *   loss3 = w_edge EdgeLengthLoss(x, gt_mesh) if *edge != 0, else 0
+ *   loss4 = w_joint mean |pred_pose m - gt_reg3dpose m|         m = reg3dpose_valid [B, n_reg_joint]
+ *   loss5 = w_joint mean |lift_pose m - gt_lift3dpose m|        m = lift3dpose_valid [B, n_lift_joint]
+ *   loss  = loss1 + loss2 + loss3 + loss4 + loss5
+ * Every pointer is device memory of one device.  weights (normal, edge, joint) and the edge flag are read on the
+ * device, so a captured graph picks up a flag written between replays; the backward must see the values of the
+ * forward it differentiates.  scratch holds at least 32 (batch + 1) bytes; its contents on entry do not matter.
+ * Reductions: loss1, loss4 and loss5 are per-mesh partials summed in fixed order (bitwise reproducible); loss2 and
+ * loss3 are p2m_mesh_losses' sums (fp64 atomics across CTAs), and its gradient is accumulated with fp32 atomics.
+ * batch <= 65535, n_reg_joint <= P2M_POSE2MESH_MAX_REG_JOINT, perm_reverse holds distinct rows in [0, n_padded). */
+#define P2M_POSE2MESH_MAX_REG_JOINT 24
+typedef struct {
+  int32_t batch, n_padded, n_vertex, n_face, n_reg_joint, n_lift_joint;
+  const float* cam_mesh;          /* [B, n_padded, 3]      the model's output            */
+  const float* lift_pose;         /* [B, n_lift_joint, 3]  PoseNet's output, mm          */
+  const float* gt_mesh;           /* [B, n_vertex, 3]                                    */
+  const float* gt_reg3dpose;      /* [B, n_reg_joint, 3]                                 */
+  const float* gt_lift3dpose;     /* [B, n_lift_joint, 3]                                */
+  const float* mesh_valid;        /* [B, n_vertex]                                       */
+  const float* reg3dpose_valid;   /* [B, n_reg_joint]                                    */
+  const float* lift3dpose_valid;  /* [B, n_lift_joint]                                   */
+  const int32_t* faces;           /* [n_face, 3] into 0 .. n_vertex - 1                  */
+  const float* joint_regressor;   /* [n_reg_joint, n_vertex]                             */
+  const int32_t* perm_reverse;    /* [n_vertex]: padded row of vertex v                  */
+  const float* weights;           /* [3]: normal, edge, joint weight                     */
+  const float* edge;              /* [1]: nonzero adds the edge term                     */
+  float* pred_pose;               /* [B, n_reg_joint, 3]: written by the forward, read by the backward */
+  void* scratch;
+  float* loss;                    /* [1]  forward output                                 */
+  float* terms;                   /* [5]  forward output: loss1 .. loss5                 */
+  const float* grad_loss;         /* [1]  backward input: d objective / d loss           */
+  float* d_cam_mesh;              /* [B, n_padded, 3] backward output, padding rows 0    */
+  float* d_lift_pose;             /* [B, n_lift_joint, 3] backward output                */
+} p2m_pose2mesh_loss_args_t;
+/* Forward: loss, terms and pred_pose (one vertex / joint launch and the face kernel of p2m_mesh_losses). */
+int p2m_pose2mesh_loss(const p2m_pose2mesh_loss_args_t* a, p2m_stream_t stream);
+/* Backward: d_cam_mesh (zeroed, then the face kernel reading and accumulating through perm_reverse, then one thread per
+ * (mesh, vertex) adding the vertex and joint terms) and d_lift_pose; reads pred_pose of the forward. */
+int p2m_pose2mesh_loss_backward(const p2m_pose2mesh_loss_args_t* a, p2m_stream_t stream);
 
 /* ---- evaluation metrics (SURVEY.md §8 row f5; lib/coord_utils.py:127-149, the datasets' compute_*_err) ----------
  * Both take a batch of point sets pred/A, gt/B [batch, n_point, 3] and an optional subset of point indices (HOST

@@ -104,6 +104,18 @@ class Capture(C.Structure):
     ]
 
 
+class Pose2MeshLossArgs(C.Structure):
+    """p2m_pose2mesh_loss_args_t: the Trainer's objective (sizes, then device pointers)."""
+    _fields_ = [(n, C.c_int32) for n in ("batch", "n_padded", "n_vertex", "n_face", "n_reg_joint", "n_lift_joint")] + [
+        (n, C.c_void_p) for n in ("cam_mesh", "lift_pose", "gt_mesh", "gt_reg3dpose", "gt_lift3dpose", "mesh_valid",
+                                  "reg3dpose_valid", "lift3dpose_valid", "faces", "joint_regressor", "perm_reverse",
+                                  "weights", "edge", "pred_pose", "scratch", "loss", "terms", "grad_loss",
+                                  "d_cam_mesh", "d_lift_pose")]
+
+
+P2M_POSE2MESH_MAX_REG_JOINT = 24
+
+
 class PoseNetStage(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in ("w1_w", "w1_b", "w2_w", "w2_b", "bn1_w", "bn1_b", "bn1_rm", "bn1_rv",
                                           "bn2_w", "bn2_b", "bn2_rm", "bn2_rv")]
@@ -191,7 +203,8 @@ EXPORTS = [
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
     "p2m_posenet_train_workspace_bytes", "p2m_posenet_train_saved_bytes", "p2m_posenet_train_forward", "p2m_posenet_backward",
     "p2m_posenet_forward_opts", "p2m_posenet_train_forward_opts", "p2m_posenet_backward_opts",
-    "p2m_regress_joints", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
+    "p2m_regress_joints", "p2m_regress_joints_backward", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
+    "p2m_pose2mesh_loss", "p2m_pose2mesh_loss_backward",
     "p2m_rigid_align", "p2m_point_errors", "p2m_fit_camera", "p2m_crop_cam_to_orig",
     "p2m_one_euro_smooth", "p2m_accel_error", "p2m_segment_mean",
     "p2m_nearest_distances", "p2m_align_w_scale", "p2m_pck_accumulate",
@@ -309,12 +322,17 @@ def load() -> C.CDLL:
         lib.p2m_posenet_backward_opts.restype = C.c_int
         lib.p2m_regress_joints.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         lib.p2m_regress_joints.restype = C.c_int
+        lib.p2m_regress_joints_backward.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
+        lib.p2m_regress_joints_backward.restype = C.c_int
         lib.p2m_normalize_pose2d.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         lib.p2m_normalize_pose2d.restype = C.c_int
         lib.p2m_mesh_losses.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
         lib.p2m_mesh_losses.restype = C.c_int
         lib.p2m_coord_loss.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp]
         lib.p2m_coord_loss.restype = C.c_int
+        for fn in (lib.p2m_pose2mesh_loss, lib.p2m_pose2mesh_loss_backward):
+            fn.argtypes = [C.POINTER(Pose2MeshLossArgs), vp]
+            fn.restype = C.c_int
         lib.p2m_rigid_align.argtypes = [vp, vp, C.c_int, C.c_int, c_int32_p, C.c_int, vp, vp, vp, vp, vp]
         lib.p2m_rigid_align.restype = C.c_int
         lib.p2m_point_errors.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, c_int32_p, C.c_int, C.c_int, vp, vp, vp]

@@ -7,8 +7,10 @@
 ``install()`` rebinds ``models.meshnet.Pose2Mesh`` / ``get_model``,
 ``models.backbones.cheby_graph_conv.graph_conv_cheby`` and ``models.posenet.LinearModel`` / ``get_model`` (the
 PoseNet in front of MeshNet: the reference's own ``FlatPose2Mesh`` then runs both halves natively in eval mode) and
-swaps ``graph_utils.build_coarse_graphs`` for the native-matching builder; ``uninstall()`` restores the originals.  Nothing in the reference
-tree is modified on disk.
+swaps ``graph_utils.build_coarse_graphs`` for the native-matching builder; ``install(replace_losses=True)`` also rebinds
+``core.loss.CoordLoss`` / ``NormalVectorLoss`` / ``EdgeLengthLoss`` / ``get_loss`` (and ``core.base``'s imported
+``get_loss``) to the native losses, so the Trainer no longer copies the face table from host memory twice per step.
+``uninstall()`` restores the originals.  Nothing in the reference tree is modified on disk.
 """
 from __future__ import annotations
 
@@ -36,7 +38,10 @@ def _rebind_holders(original, replacement):
                 _rebound.append((mod, attr, original))
 
 
-def install(replace_graph_builder: bool = True):
+_LOSS_NAMES = ("CoordLoss", "NormalVectorLoss", "EdgeLengthLoss", "get_loss")
+
+
+def install(replace_graph_builder: bool = True, replace_losses: bool = False):
     from . import cheby_graph_conv as my_conv
     from . import graph as my_graph
     from . import meshnet as my_meshnet
@@ -60,6 +65,13 @@ def install(replace_graph_builder: bool = True):
         _rebind_holders(_saved["graph"], my_graph.build_coarse_graphs)   # includes graph_utils itself
         ref_gu.build_coarse_graphs = my_graph.build_coarse_graphs
     _rebind_holders(_saved["conv"], my_conv.graph_conv_cheby)
+    if replace_losses:
+        from . import loss as my_loss
+
+        ref_loss = importlib.import_module("core.loss")
+        _saved.setdefault("loss", {name: getattr(ref_loss, name) for name in _LOSS_NAMES})
+        for name, original in _saved["loss"].items():
+            _rebind_holders(original, getattr(my_loss, name))               # includes core.loss itself
 
 
 def uninstall():
@@ -76,3 +88,7 @@ def uninstall():
         importlib.import_module("models.backbones.cheby_graph_conv").graph_conv_cheby = _saved.pop("conv")
     if "graph" in _saved:
         importlib.import_module("graph_utils").build_coarse_graphs = _saved.pop("graph")
+    if "loss" in _saved:
+        ref_loss = importlib.import_module("core.loss")
+        for name, original in _saved.pop("loss").items():
+            setattr(ref_loss, name, original)
