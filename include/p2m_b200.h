@@ -371,6 +371,38 @@ int p2m_posenet_backward_opts(const p2m_posenet_params_t* params, const p2m_bn_o
                               size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* grads,
                               float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream);
 
+/* Debug capture of the PoseNet backward's intermediates, which live only in the workspace (the forward's are in
+ * `saved`).  Every pointer is device memory and nullable; the per-stage fields are host arrays [num_stage] of device
+ * pointers (a null array, or a null entry, is not written).  [B, H] row-major unless stated.  For stage s:
+ *   g_y[s]    dL/dy_{s+1}, the gradient entering the stage's backward;
+ *   a2[s]     the recomputed drop(relu(bn2(z2_s)));
+ *   g_a2[s]   g_y[s] Wb, the gradient of a2 (before the dropout backward);
+ *   g_z2[s]   dL/dz2_s after the dropout, ReLU and bn2 backward;
+ *   a1[s], g_a1[s]  the same as a2, g_a2 for drop(relu(bn1(y_s))) and g_z2[s] Wa;
+ *   g_bn1[s]  the gradient of y_s through bn1 alone (g_y[s - 1] = g_y[s] + g_bn1[s]);
+ *   scale[s]  float[4]: the power-of-two range normalisations of the stage's tensor-core GEMM operands a2, g_y[s], a1,
+ *             g_z2[s] (not written on the fp32 path);
+ *   g_y0      dL/dy_0, the gradient entering the input layer's backward.
+ * p2m_debug_posenet_backward_capture is p2m_posenet_backward_opts plus the copies (cudaMemcpyAsync on `stream`); the
+ * results are bitwise those of p2m_posenet_backward_opts.                                                    */
+typedef struct {
+  float* const* g_y;
+  float* const* a2;
+  float* const* g_a2;
+  float* const* g_z2;
+  float* const* a1;
+  float* const* g_a1;
+  float* const* g_bn1;
+  float* const* scale;
+  float* g_y0;
+} p2m_posenet_capture_t;
+int p2m_debug_posenet_backward_capture(const p2m_posenet_params_t* params, const p2m_bn_opts_t* bn,
+                                       const float* p_dropout, const float* pose2d, int batch, const int64_t* seed,
+                                       const void* saved, size_t saved_bytes, const float* d_pose3d,
+                                       const p2m_posenet_grads_t* grads, float* d_pose2d, void* workspace,
+                                       size_t workspace_bytes, const p2m_posenet_capture_t* capture,
+                                       p2m_stream_t stream);
+
 /* ---- the steps either side of the model in the reference's callers (SURVEY.md §8 row f2) ----------
  * Joint regression (lib/core/base.py:131,204; demo/run.py:171): joints [B, n_joint, C] = joint_regressor
  * [n_joint, n_vertex] @ vertices [B, n_vertex, C] (C <= 4), on the gathered vertices of

@@ -144,6 +144,13 @@ class PoseNetGrads(C.Structure):
                 ("stages", C.POINTER(PoseNetStageGrads))]
 
 
+class PoseNetCapture(C.Structure):
+    """p2m_posenet_capture_t: device buffers the PoseNet backward copies its intermediates into
+    (p2m_debug_posenet_backward_capture); the per-stage fields are [num_stage] arrays, scale[s] a float[4]."""
+    _fields_ = [(n, C.POINTER(C.c_void_p)) for n in ("g_y", "a2", "g_a2", "g_z2", "a1", "g_a1", "g_bn1", "scale")] + [
+        ("g_y0", C.c_void_p)]
+
+
 class BodyModelDesc(C.Structure):
     _fields_ = [
         ("n_vertex", C.c_int32), ("n_joint", C.c_int32), ("n_betas", C.c_int32), ("n_out_joints", C.c_int32),
@@ -203,6 +210,7 @@ EXPORTS = [
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
     "p2m_posenet_train_workspace_bytes", "p2m_posenet_train_saved_bytes", "p2m_posenet_train_forward", "p2m_posenet_backward",
     "p2m_posenet_forward_opts", "p2m_posenet_train_forward_opts", "p2m_posenet_backward_opts",
+    "p2m_debug_posenet_backward_capture",
     "p2m_regress_joints", "p2m_regress_joints_backward", "p2m_normalize_pose2d", "p2m_mesh_losses", "p2m_coord_loss",
     "p2m_pose2mesh_loss", "p2m_pose2mesh_loss_backward",
     "p2m_rigid_align", "p2m_point_errors", "p2m_fit_camera", "p2m_crop_cam_to_orig",
@@ -320,6 +328,9 @@ def load() -> C.CDLL:
         lib.p2m_posenet_backward_opts.argtypes = [C.POINTER(PoseNetParams), bn_p, c_float_p, vp, C.c_int, vp, vp, sz,
                                                   vp, C.POINTER(PoseNetGrads), vp, vp, sz, vp]
         lib.p2m_posenet_backward_opts.restype = C.c_int
+        lib.p2m_debug_posenet_backward_capture.argtypes = (lib.p2m_posenet_backward_opts.argtypes[:-1]
+                                                           + [C.POINTER(PoseNetCapture), vp])
+        lib.p2m_debug_posenet_backward_capture.restype = C.c_int
         lib.p2m_regress_joints.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]
         lib.p2m_regress_joints.restype = C.c_int
         lib.p2m_regress_joints_backward.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp]

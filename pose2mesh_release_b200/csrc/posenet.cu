@@ -491,9 +491,19 @@ int train_forward(const p2m_posenet_params_t* P, const p2m_posenet_train_t* extr
                       pose_combine, s);
 }
 
+// p2m_debug_posenet_backward_capture: n floats of src into dst, if the caller asked for that tensor
+int capture_copy(float* dst, const float* src, size_t n, cudaStream_t s) {
+  if (dst == nullptr) return P2M_OK;
+  P2M_CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+  return P2M_OK;
+}
+float* capture_slot(float* const* v, int st) { return v ? v[st] : nullptr; }
+
+// cap (may be null): the debug capture of the backward's intermediates; null issues no copies
 int backward(const p2m_posenet_params_t* P, const Modes& md, const float* pose2d, int B, const int64_t* seed,
              const void* saved, size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
-             float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
+             float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream,
+             const p2m_posenet_capture_t* cap) {
   bool ok = pose2d && seed && saved && d_pose3d && workspace && G && G->w1_w && G->w1_b && G->w2_w && G->w2_b && P &&
             (P->num_stage <= 0 || G->stages);
   for (int st = 0; ok && st < P->num_stage; ++st) {
@@ -525,32 +535,53 @@ int backward(const p2m_posenet_params_t* P, const Modes& md, const float* pose2d
     const p2m_posenet_stage_grads_t& D = G->stages[st];
     const Dropout d1 = make_dropout(md.p[st], seed, 2 * st), d2 = make_dropout(md.p[st], seed, 2 * st + 1);
     const int frozen1 = md.of(st, 0).stats == P2M_BN_RUNNING, frozen2 = md.of(st, 1).stats == P2M_BN_RUNNING;
+    // the four range normalisations of the stage's tensor-core GEMMs: a2, g_y, a1, g_z2
+    float* cap_scale = cap && plan.tc ? capture_slot(cap->scale, st) : nullptr;
+    auto cap_scale_copy = [&](int i, const float* sc) { return capture_copy(cap_scale ? cap_scale + i : nullptr, sc, 1, s); };
+    if (cap) P2M_TRY(capture_copy(capture_slot(cap->g_y, st), w.g, n, s));
     // second Linear: y' = y + a2 Wb^T + bb with a2 = drop(relu(bn2(z2))) recomputed; g = dL/dy'
     P2M_TRY(launch_col_sum(w.g, B, H, w.sums, D.w2_b, s));
     P2M_TRY(bn_relu_drop(sv.z2[st], plan, w, sv.stat(st, 1, 2), sv.stat(st, 1, 3), d2, w.a, s));
+    if (cap) {
+      P2M_TRY(capture_copy(capture_slot(cap->a2, st), w.a, n, s));
+      P2M_TRY(cap_scale_copy(0, w.a_scale));
+    }
     P2M_TRY(gemm.prepare(w.g, false));
+    if (cap) P2M_TRY(cap_scale_copy(1, w.g_scale));
     P2M_TRY(gemm.dw(w.g, w.a, D.w2_w));
     P2M_TRY(gemm.dx(w.g, S.w2_w, w.t));
+    if (cap) P2M_TRY(capture_copy(capture_slot(cap->g_a2, st), w.t, n, s));
     // through drop, ReLU and bn2: t = dL/dz2 (its fp16-range scale found in the same pass on the tensor-core path)
     k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.t, n, d2);
     P2M_LAUNCH_OK();
     P2M_TRY(launch_bn_relu_bwd(sv.z2[st], w.t, B, H, S.bn2_w, sv.stat(st, 1, 2), sv.stat(st, 1, 3), sv.stat(st, 1, 0),
                                sv.stat(st, 1, 1), 1, w.sums, D.bn2_w, D.bn2_b, w.t, s, plan.tc ? w.g_scale : nullptr,
                                frozen2));
+    if (cap) {
+      P2M_TRY(capture_copy(capture_slot(cap->g_z2, st), w.t, n, s));
+      P2M_TRY(cap_scale_copy(3, w.g_scale));
+    }
     // first Linear: z2 = a1 Wa^T + ba with a1 = drop(relu(bn1(y))) recomputed
     P2M_TRY(launch_col_sum(w.t, B, H, w.sums, D.w1_b, s));
     P2M_TRY(bn_relu_drop(sv.y[st], plan, w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), d1, w.a, s));
+    if (cap) {
+      P2M_TRY(capture_copy(capture_slot(cap->a1, st), w.a, n, s));
+      P2M_TRY(cap_scale_copy(2, w.a_scale));
+    }
     P2M_TRY(gemm.prepare(w.t, true));
     P2M_TRY(gemm.dw(w.t, w.a, D.w1_w));
     P2M_TRY(gemm.dx(w.t, S.w1_w, w.a));
+    if (cap) P2M_TRY(capture_copy(capture_slot(cap->g_a1, st), w.a, n, s));
     // through drop, ReLU and bn1, plus the residual branch: g += dL/dy
     k_pn_drop_bwd<<<blocks((n + 3) / 4), 256, 0, s>>>(w.a, n, d1);
     P2M_LAUNCH_OK();
     P2M_TRY(launch_bn_relu_bwd(sv.y[st], w.a, B, H, S.bn1_w, sv.stat(st, 0, 2), sv.stat(st, 0, 3), sv.stat(st, 0, 0),
                                sv.stat(st, 0, 1), 1, w.sums, D.bn1_w, D.bn1_b, w.a, s, nullptr, frozen1));
+    if (cap) P2M_TRY(capture_copy(capture_slot(cap->g_bn1, st), w.a, n, s));
     k_pn_add<<<blocks(n), 256, 0, s>>>(w.g, w.a, n);
     P2M_LAUNCH_OK();
   }
+  if (cap) P2M_TRY(capture_copy(cap->g_y0, w.g, n, s));
   // input layer (thin: fp32): db1, dW1 = g^T pose2d, d_pose2d = g W1
   P2M_TRY(launch_col_sum(w.g, B, H, w.sums, G->w1_b, s));
   P2M_TRY(gemm.transpose(w.g, B, H));
@@ -582,14 +613,26 @@ int p2m_posenet_backward(const p2m_posenet_params_t* P, const float* pose2d, int
                          const void* saved, size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
                          float* d_pose2d, void* workspace, size_t workspace_bytes, p2m_stream_t stream) {
   const Modes md(P ? P->num_stage : 0, nullptr, P2M_BN_BATCH_UPDATE, nullptr, p_dropout);
-  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream);
+  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream,
+                  nullptr);
 }
 int p2m_posenet_backward_opts(const p2m_posenet_params_t* P, const p2m_bn_opts_t* bn, const float* p_dropout,
                               const float* pose2d, int B, const int64_t* seed, const void* saved, size_t saved_bytes,
                               const float* d_pose3d, const p2m_posenet_grads_t* G, float* d_pose2d, void* workspace,
                               size_t workspace_bytes, p2m_stream_t stream) {
   const Modes md(P ? P->num_stage : 0, bn, P2M_BN_BATCH_UPDATE, p_dropout, 0.f);
-  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream);
+  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream,
+                  nullptr);
+}
+
+int p2m_debug_posenet_backward_capture(const p2m_posenet_params_t* P, const p2m_bn_opts_t* bn, const float* p_dropout,
+                                       const float* pose2d, int B, const int64_t* seed, const void* saved,
+                                       size_t saved_bytes, const float* d_pose3d, const p2m_posenet_grads_t* G,
+                                       float* d_pose2d, void* workspace, size_t workspace_bytes,
+                                       const p2m_posenet_capture_t* capture, p2m_stream_t stream) {
+  const Modes md(P ? P->num_stage : 0, bn, P2M_BN_BATCH_UPDATE, p_dropout, 0.f);
+  return backward(P, md, pose2d, B, seed, saved, saved_bytes, d_pose3d, G, d_pose2d, workspace, workspace_bytes, stream,
+                  capture);
 }
 
 }  // extern "C"

@@ -256,6 +256,62 @@ class LinearModel(nn.Module):
         return self._forward_torch(x)
 
 
+CAPTURE_FIELDS = ("g_y", "a2", "g_a2", "g_z2", "a1", "g_a1", "g_bn1", "scale", "g_y0")
+
+
+def debug_train_step_capture(module, x, seed, d_out, capture=CAPTURE_FIELDS):
+    """One native train step of `module` with the backward's intermediates captured
+    (p2m_debug_posenet_backward_capture): p2m_posenet_train_forward_opts, then the capture backward with the same
+    LinearModel._native_modes().  Running statistics are updated as by the module's own forward.  capture: the
+    p2m_posenet_capture_t fields to fill (the others stay null); None runs p2m_posenet_backward_opts instead, without
+    a capture.  Returns a dict with out [B, 3J], combine [B, J, 5], saved (uint8), grads (in the order of
+    LinearModel._trained_tensors()), dx [B, 2J], and per captured field a list of num_stage [B, H] tensors
+    (scale: [S, 4], g_y0: one [B, H] tensor)."""
+    lib = _lib.load()
+    x = x.reshape(len(x), -1).contiguous().float()
+    dev, B, S, H = x.device, x.shape[0], module.num_stage, module.linear_size
+    modes = module._native_modes()
+    out, comb, saved = _train_forward(module, x, seed, True, modes)
+    params = module._trained_tensors()
+    grads = [torch.empty_like(p) for p in params]
+    g = _lib.PoseNetGrads()
+    g.w1_w, g.w1_b, g.w2_w, g.w2_b = (t.data_ptr() for t in grads[:4])
+    stages = (_lib.PoseNetStageGrads * S)()
+    for i in range(S):
+        for (name, _), t in zip(_lib.PoseNetStageGrads._fields_, grads[4 + 8 * i:12 + 8 * i]):
+            setattr(stages[i], name, t.data_ptr())
+    g.stages = stages
+    dx = torch.empty_like(x)
+    res = dict(out=out, combine=comb, saved=saved, grads=grads, dx=dx)
+    n_ws = lib.p2m_posenet_train_workspace_bytes(B, module.num_joint, H, S)
+    ws = torch.empty(n_ws, device=dev, dtype=torch.uint8)
+    native = module._native_params()
+    args = (C.byref(native), modes[0], modes[1], x, B, seed, saved, saved.numel(), d_out.contiguous().float(),
+            C.byref(g), dx, ws, n_ws)
+    if capture is None:
+        _lib.call("p2m_posenet_backward_opts", dev, *args)
+        return res
+    cap = _lib.PoseNetCapture()
+    keep = []
+    for name in CAPTURE_FIELDS[:-1]:
+        if name not in capture:
+            continue
+        shape = (4,) if name == "scale" else (B, H)
+        fill = float("nan") if name == "scale" else 0.0      # an unwritten scale stays NaN
+        ts = [torch.full(shape, fill, device=dev, dtype=torch.float32) for _ in range(S)]
+        arr = (C.c_void_p * max(S, 1))(*[t.data_ptr() for t in ts])
+        keep.append(arr)
+        setattr(cap, name, C.cast(arr, C.POINTER(C.c_void_p)))
+        res[name] = ts
+    if "g_y0" in capture:
+        res["g_y0"] = torch.zeros((B, H), device=dev, dtype=torch.float32)
+        cap.g_y0 = res["g_y0"].data_ptr()
+    _lib.call("p2m_debug_posenet_backward_capture", dev, *args, C.byref(cap))
+    if "scale" in res:
+        res["scale"] = torch.stack(res["scale"]) if S else torch.empty((0, 4), device=dev)
+    return res
+
+
 def get_model(num_joint, hid_dim, num_layer, p_dropout, pretrained=False):
     """lib/models/posenet.py:89-92."""
     return LinearModel(num_joint, hid_dim, num_layer, p_dropout, pretrained)

@@ -371,23 +371,28 @@ def bn_eval_fwd_bound(z, E, gamma, beta, rm, rv, bias, eps=BN_EPS):
     return ey.reshape(np.shape(z))
 
 
-def bn_train_bwd(z, g_a, gamma, beta, relu=False, eps=BN_EPS):
+def bn_train_bwd(z, g_a, gamma, beta, relu=False, eps=BN_EPS, mask=None):
     """Backward of train-mode BatchNorm1d (+ ReLU) over the rows of z [..., F] from the gradient g_a of its output, with
-    the exact batch statistics of z.  Returns (g_z, dgamma, dbeta, mask): g' = g_a [bn(z) > 0],
-    g_z = gamma invstd (g' - mean(g') - zhat mean(g' zhat)), dgamma = sum g' zhat, dbeta = sum g'."""
+    the exact batch statistics of z.  Returns (g_z, dgamma, dbeta, pre): g' = g_a [bn(z) > 0],
+    g_z = gamma invstd (g' - mean(g') - zhat mean(g' zhat)), dgamma = sum g' zhat, dbeta = sum g'.
+    mask (bool, z's shape): the ReLU's open entries as the kernel decided them (relu_mask), in place of the float64
+    pre > 0; given, it implies the ReLU."""
     zr, gr = _rows(z), _rows(g_a)
     mean = zr.mean(axis=0)
     invstd = 1.0 / np.sqrt(((zr - mean) ** 2).mean(axis=0) + eps)
     zh = (zr - mean) * invstd
     pre = zh * np.asarray(gamma, np.float64) + np.asarray(beta, np.float64)
-    mask = pre > 0 if relu else np.ones_like(pre, bool)
+    if mask is not None:
+        mask = _rows(mask)
+    else:
+        mask = pre > 0 if relu else np.ones_like(pre, bool)
     g = np.where(mask, gr, 0.0)
     m1, m2 = g.mean(axis=0), (g * zh).mean(axis=0)
     g_z = np.asarray(gamma, np.float64) * invstd * (g - m1 - zh * m2)
     return g_z.reshape(np.shape(z)), (g * zh).sum(axis=0), g.sum(axis=0), pre.reshape(np.shape(z))
 
 
-def bn_train_bwd_bound(z, g_a, gamma, beta, relu=False, eps=BN_EPS):
+def bn_train_bwd_bound(z, g_a, gamma, beta, relu=False, eps=BN_EPS, mask=None):
     """Element-wise bounds (g_z, dgamma, dbeta) on launch_bn_relu_bwd given the exact z and g_a it read (the captured
     fp32 tensors) and the fp32 mean / invstd the forward saved (bn_train_fwd_bound's bounds with E = 0: the error of
     the statistics sums plus the backward error of z's fp32 storage, u |z|).
@@ -400,17 +405,22 @@ def bn_train_bwd_bound(z, g_a, gamma, beta, relu=False, eps=BN_EPS):
     the affine k_bn_bwd_coef + k_bn_bwd_apply4, g_z = fma(a, g', fma(b, z, c)) with b = -a invstd m2 and
     c = -a m1 + a invstd m2 mean, whose b z + c cancels to a invstd m2 (mean - z): its coefficients' roundings
     (3 u in b, 4 u in c) are relative to |a invstd m2| |z| and |a invstd m2 mean|, i.e. a backward error of ~3 u (|z| +
-    |mean|) in z, which is large next to |zhat| where the channel's mean / sigma is large."""
+    |mean|) in z, which is large next to |zhat| where the channel's mean / sigma is large.
+    mask: as in bn_train_bwd.  With the kernel's own mask the bound needs no ReLU-branch allowance: it holds the kernel
+    to the g' the kernel formed."""
     zr, gr = _rows(z), _rows(g_a)
     n, F = zr.shape
     gam = np.asarray(gamma, np.float64)
-    g_z, dgam, dbet, pre = bn_train_bwd(z, g_a, gamma, beta, relu, eps)
+    g_z, dgam, dbet, pre = bn_train_bwd(z, g_a, gamma, beta, relu, eps, mask)
     pre = _rows(pre)
     st = bn_train_fwd_bound(zr, np.zeros_like(zr), gamma, beta, np.zeros(F), np.zeros(F), eps=eps)
     mean = zr.mean(axis=0)
     invstd = 1.0 / np.sqrt(((zr - mean) ** 2).mean(axis=0) + eps)
     zh = (zr - mean) * invstd
-    g = np.where(pre > 0, gr, 0.0) if relu else gr
+    if mask is not None:
+        g = np.where(_rows(mask), gr, 0.0)
+    else:
+        g = np.where(pre > 0, gr, 0.0) if relu else gr
     ag = np.abs(g)
     a = np.abs(gam) * invstd
     e_a = np.abs(gam) * st["invstd"] + U32 * a
@@ -577,7 +587,7 @@ BN_MUTATIONS = ("one_pass", "unbiased_in_norm", "biased_in_running", "eps_1e-3",
                 "relu_before_affine")
 
 
-def emulate_bn_train(z, gamma, beta, rm, rv, relu=False, mutation: str = ""):
+def emulate_bn_train(z, gamma, beta, rm, rv, relu=False, mutation: str = "", momentum=BN_MOMENTUM, eps=BN_EPS):
     """What k_col_stats + k_bn_finalize + k_affine_act return for an fp32 z [..., F]: per block of STAT_ROWS rows and
     row lane rr (rl = 256 / min(F, 256) lanes), an fp32 running sum of d = z - K and fma(d, d, q) with K = z[0] (the
     shifted accumulation), the lanes added in fp32, the blocks in fp64; then mean = K + S/n, var = Q/n - (S/n)^2 in fp64,
@@ -605,13 +615,13 @@ def emulate_bn_train(z, gamma, beta, rm, rv, relu=False, mutation: str = ""):
     mean = K.astype(np.float64) + d
     var = np.maximum(Q / n - d * d, 0.0)
     unb = var * n / (n - 1) if n > 1 else var
-    eps = 1e-3 if mutation == "eps_1e-3" else BN_EPS
+    eps = 1e-3 if mutation == "eps_1e-3" else eps
     v_norm = unb if mutation == "unbiased_in_norm" else var
     if mutation == "eps_outside_sqrt":
         invstd = (1.0 / (np.sqrt(v_norm) + eps)).astype(f32)
     else:
         invstd = (1.0 / np.sqrt(v_norm + eps)).astype(f32)
-    mom = f32(0.01) if mutation == "momentum_0.01" else f32(0.1)
+    mom = f32(0.01) if mutation == "momentum_0.01" else f32(momentum)
     v_run = var if mutation == "biased_in_running" else unb
     rm_new = (f32(1) - mom) * np.asarray(rm, f32) + mom * mean.astype(f32)
     rv_new = (f32(1) - mom) * np.asarray(rv, f32) + mom * v_run.astype(f32)
@@ -629,13 +639,16 @@ def emulate_bn_train(z, gamma, beta, rm, rv, relu=False, mutation: str = ""):
 BN_BWD_MUTATIONS = ("m2_dropped", "mean_not_subtracted", "rows_minus_one")
 
 
-def emulate_bn_bwd(z, g_a, gamma, beta, mean, invstd, relu=False, mutation: str = ""):
+def emulate_bn_bwd(z, g_a, gamma, beta, mean, invstd, relu=False, mutation: str = "", mask=None, frozen=False):
     """What k_bn_bwd_reduce + k_bn_bwd_coef + k_bn_bwd_apply4 return for fp32 z, g_a [..., F] and the saved fp32
     mean / invstd: per block of STAT_ROWS rows and row lane (as emulate_bn_train) fp32 sums s1 = sum g' and
     s2 = fma(g', zhat, s2) with zhat = fp32((z - mean) invstd), blocks in fp64; then in fp32 m1 = s1 / n, m2 = s2 / n,
     a = gamma invstd, b = -a invstd m2, c = -a m1 + a invstd m2 mean and g_z = fma(a, g', fma(b, z, c)).  The mask
     g' = g_a [fma(z, scale, shift) > 0] uses scale = gamma invstd, shift = beta - mean scale like the forward.
-    `mutation` (one of BN_BWD_MUTATIONS) plants one defect.  Returns (g_z, dgamma, dbeta) as float64."""
+    `mutation` (one of BN_BWD_MUTATIONS) plants one defect.  mask (bool): the ReLU's open entries as given (the device's
+    relu_mask) in place of the emulated test.  frozen: the running-statistics backward, g_z = fp32(a g') (b = c = 0;
+    mean / invstd are then the running mean and the fp32 1 / sqrt(rv + eps)).  Returns (g_z, dgamma, dbeta) as
+    float64."""
     f32 = np.float32
     zr = np.asarray(z, f32).reshape(-1, np.shape(z)[-1])
     gr = np.asarray(g_a, f32).reshape(zr.shape)
@@ -644,7 +657,9 @@ def emulate_bn_bwd(z, g_a, gamma, beta, mean, invstd, relu=False, mutation: str 
     gam = np.asarray(gamma, f32)
     sc = (gam * ist).astype(f32)
     sh = (np.asarray(beta, f32) - (mu * sc).astype(f32)).astype(f32)
-    if relu:
+    if mask is not None:
+        gr = np.where(np.asarray(mask).reshape(zr.shape), gr, f32(0))
+    elif relu:
         gr = np.where((zr.astype(np.float64) * sc + sh).astype(f32) > 0, gr, f32(0))
     zh = (((zr - mu).astype(f32)) * ist).astype(f32)
     rl = 256 // min(F, 256)
@@ -665,6 +680,10 @@ def emulate_bn_bwd(z, g_a, gamma, beta, mean, invstd, relu=False, mutation: str 
     if mutation == "m2_dropped":
         m2 = np.zeros(F, f32)
     a = (gam * ist).astype(f32)
+    if frozen:
+        g_z = (a.astype(np.float64) * gr).astype(f32)
+        return (g_z.astype(np.float64).reshape(np.shape(z)), Q.astype(f32).astype(np.float64),
+                S.astype(f32).astype(np.float64))
     b = (-(a * ist).astype(f32) * m2).astype(f32)
     t = (((a * ist).astype(f32) * m2).astype(f32) * mu).astype(f32)
     c = (-(a * m1).astype(f32) + (f32(0) if mutation == "mean_not_subtracted" else t)).astype(f32)
@@ -679,3 +698,121 @@ def bound_ratio(y, y64, bound) -> float:
     if not np.all(np.isfinite(y)):
         return float("inf")
     return float((np.abs(y - y64) / np.maximum(bound, 1e-300)).max(initial=0.0))
+
+
+# --------------------------------------------------------------------------------------------- PoseNet layer by layer
+def relu_mask(z, scale, shift) -> np.ndarray:
+    """The kernels' activation test fmaf(z, scale, shift) > 0 for fp32 z, scale, shift, reproduced bit for bit: the
+    float64 product of two fp32 values is exact (48 significant bits), and the one rounding of the float64 sum to
+    nearest cannot change the sign of a non-zero exact sum (nor make it zero), so its sign is the exact sum's, which
+    is also the sign of fmaf's single fp32 rounding of it.  Two conditions, both far from any real pre-activation:
+    |z scale| must not underflow float64's normal range (2^-1022), or the product is not exact; and |exact sum| must
+    exceed 2^-150, below which fmaf rounds to zero and the kernel closes the ReLU where relu_mask opens it (the
+    library is built without flushing subnormals to zero)."""
+    z = np.asarray(z, np.float32).astype(np.float64)
+    return z * np.asarray(scale, np.float32).astype(np.float64) + np.asarray(shift, np.float32).astype(np.float64) > 0
+
+
+TC_MMAS_PER_BLOCK = 6      # launch_umma_gemm's k16 MMAs per 32-wide K-block: hi*hi x2, lo*hi x2, hi*lo x2
+
+
+def tc_running_sums(A, B) -> np.ndarray:
+    """sum over the k16 wgmma steps of launch_umma_gemm of |the accumulator after the step|, per element of A @ B, in
+    the kernel's order: per K-block of 32 columns hi*hi over its first and second 16 columns, then lo*hi and hi*lo over
+    both (cheb_umma.cu's main loop), so the accumulator holds the float64 partial sum S after the block's first 16
+    columns once and S after all 32 five times.  The lo products move those sums by <= 2^-10 of their magnitude, a
+    second-order term next to the truncation they bound.  K is padded with zeros to a multiple of 32."""
+    A, B = np.asarray(A, np.float64), np.asarray(B, np.float64)
+    S = np.zeros((A.shape[0], B.shape[1]))
+    acc = np.zeros_like(S)
+    for k0 in range(0, A.shape[1], 32):
+        S = S + A[:, k0:k0 + 16] @ B[k0:k0 + 16]
+        acc += np.abs(S)
+        S = S + A[:, k0 + 16:k0 + 32] @ B[k0 + 16:k0 + 32]
+        acc += (TC_MMAS_PER_BLOCK - 1) * np.abs(S)
+    return acc
+
+
+def dense_gemm_bound(A, B, precision: str, b_side: str = "fixed") -> np.ndarray:
+    """Element-wise bound on C = A @ B (A [m, k], B [k, n]) from one of PoseNet's GEMMs given its exact fp32 operands.
+    fp32 (CUDA cores, FMA): gamma_k |A| |B|.
+    fp16x3 (launch_umma_gemm), worst case per element rather than a probabilistic sum:
+      * the split: SPLIT |A| |B| (two lo roundings and the dropped lo*lo product, as in gamma);
+      * the accumulation: every k16 wgmma adds its products (exact in fp32) to the fp32 accumulator and truncates the
+        result (round toward zero: Fasi et al., PeerJ Comput. Sci. 7:e330, 2021), an error below one ulp, i.e.
+        < 2 u |accumulator after the step|.  Summed over the kernel's steps that is 2 u tc_running_sums(A, B): it
+        grows linearly where the partial sums keep one sign (a dW over a short K = B), and stays small where they
+        cancel (the K = H forward and dX GEMMs);
+      * the floor of the lo parts: A, the activation or gradient operand, is always range-normalised (max|A| scaled
+        into [2^9, 2^10), so a lo part's absolute error, half of fp16's subnormal spacing 2^-24 in the scaled units, is
+        <= 2^-34 max|A|); B enters at the fixed 2^6 when it is a weight matrix (b_side='fixed': 2^-25 / 2^6 per
+        entry), range-normalised like A when it is an activation (b_side='normalised', dW's a: 2^-34 max|B|).  The
+        floor of an entry is its operand's absolute error times the other operand's absolute sums along k."""
+    A, B = np.asarray(A, np.float64), np.asarray(B, np.float64)
+    aA, aB = np.abs(A), np.abs(B)
+    if precision != "fp16x3":
+        return gamma(A.shape[1], precision) * (aA @ aB)
+    e = SPLIT * (aA @ aB) + 2 * U32 * tc_running_sums(A, B)
+    e_a = 2.0 ** -34 * float(aA.max(initial=0.0))
+    e_b = NET_LO / NET_W_SCALE if b_side == "fixed" else 2.0 ** -34 * float(aB.max(initial=0.0))
+    return e + e_a * aB.sum(axis=0, keepdims=True) + e_b * aA.sum(axis=1, keepdims=True)
+
+
+def emulate_dense_gemm(A, B, b_side: str = "fixed", drop_block: int = -1, a_scale: float | None = None,
+                       drop_lo: str = "") -> np.ndarray:
+    """What launch_umma_gemm returns for C = A @ B with fp32 operands: A scaled by a_scale (default: the power of two
+    _pow2_scale(max|A|) the library finds), B by the fixed 2^6 (b_side='fixed') or by its own power of two, each split
+    into fp16 hi + lo, hi*hi + lo*hi + hi*lo summed per K-block of 32 in float64 and accumulated over the blocks in fp32
+    (a slightly better accumulator than the tensor core's), both scales divided out.  drop_block >= 0 leaves out the
+    lo(A) * hi(B) products of K-block `drop_block`; drop_lo='a' leaves out every lo(A) * hi(B) product, 'b' every
+    hi(A) * lo(B) (an fp16x2 split of one operand)."""
+    A = np.asarray(A, np.float32).astype(np.float64)
+    B = np.asarray(B, np.float32).astype(np.float64)
+    sa = _pow2_scale(float(np.abs(A).max(initial=0.0))) if a_scale is None else a_scale
+    sb = NET_W_SCALE if b_side == "fixed" else _pow2_scale(float(np.abs(B).max(initial=0.0)))
+    with np.errstate(over="ignore", invalid="ignore"):
+        ah, al = _f16_split(A * sa)
+        bh, bl = _f16_split(B * sb)
+    if drop_lo == "a":
+        al = 0.0 * al
+    elif drop_lo == "b":
+        bl = 0.0 * bl
+    acc = np.zeros((A.shape[0], B.shape[1]), np.float32)
+    for k0 in range(0, A.shape[1], 32):
+        k = slice(k0, k0 + 32)
+        lo = al[:, k] if k0 // 32 != drop_block else 0.0 * al[:, k]
+        acc = (acc + (ah[:, k] @ bh[k] + lo @ bh[k] + ah[:, k] @ bl[k]).astype(np.float32)).astype(np.float32)
+    return acc.astype(np.float64) / (sa * sb)
+
+
+def bn_frozen_bwd(z, g, gamma, rm, rv, eps=BN_EPS):
+    """Backward of a BatchNorm with running statistics (frozen: mean and variance are constants of the forward) from
+    the masked gradient g' = g [relu open] of its output: g_z = gamma invstd g', dgamma = sum g' zhat, dbeta = sum g',
+    with invstd = 1 / sqrt(rv + eps) and zhat = (z - rm) invstd.  Returns (g_z, dgamma, dbeta)."""
+    zr, gr = _rows(z), _rows(g)
+    invstd = 1.0 / np.sqrt(np.asarray(rv, np.float64) + eps)
+    zh = (zr - np.asarray(rm, np.float64)) * invstd
+    g_z = np.asarray(gamma, np.float64) * invstd * gr
+    return g_z.reshape(np.shape(z)), (gr * zh).sum(axis=0), gr.sum(axis=0)
+
+
+def bn_frozen_bwd_bound(z, g, gamma, rm, rv, eps=BN_EPS):
+    """Bounds (g_z, dgamma, dbeta) on the frozen backward of launch_bn_relu_bwd, given the exact fp32 z and g' it read.
+      invstd = 1.f / sqrtf(rv + (float)eps) (k_bn_fold_eval): eps's cast and the sum 2 u relative, halved by the
+      square root, plus the root's and the division's roundings: 3 u relative;
+      g_z = fp32(fp32(gamma invstd) g'): one rounding in the coefficient, one in the product: 5 u |g_z| in all;
+      zhat = fp32(fp32(z - rm) invstd): the difference, the product and invstd's 3 u: 5 u |zhat|;
+      dgamma, dbeta: the fp32 block sums of k_bn_bwd_reduce (stat_allowance), with dgamma's terms carrying zhat's
+      error, and the final fp32 rounding of the fp64 total.
+    The first-order bound is raised by one u in g_z for the products of the relative errors (O(u^2))."""
+    zr, gr = _rows(z), _rows(g)
+    n, F = zr.shape
+    g_z, dgam, dbet = bn_frozen_bwd(z, g, gamma, rm, rv, eps)
+    invstd = 1.0 / np.sqrt(np.asarray(rv, np.float64) + eps)
+    azh = np.abs(zr - np.asarray(rm, np.float64)) * invstd
+    ag = np.abs(gr)
+    al = stat_allowance(n, F)
+    e_gz = 6 * U32 * np.abs(_rows(g_z))
+    e_dgam = al * (ag * azh).sum(axis=0) + 5 * U32 * (ag * azh).sum(axis=0) + U32 * np.abs(dgam)
+    e_dbet = al * ag.sum(axis=0) + U32 * np.abs(dbet)
+    return e_gz.reshape(np.shape(z)), e_dgam, e_dbet
