@@ -115,6 +115,11 @@ int p2m_debug_set_dedup_padding(p2m_model_t* m, int enable);
  * rows + 1-hop halo) per 128-row tile (0 when the level has no tensor-core metadata), out[8] = isolated rows that
  * padding elision would route to the dense path (0: elision not applicable).                                    */
 int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int32_t out[9]);
+/* Debug: how the tensor-core forward conv of that layer (T1 given, the level's consecutive tiles) is laid out.  out[0] =
+ * output columns per CTA: 64 (128 x 64 tiles), 128 (64 x 128; a 256-wide layer as two column slices) or 256 (64 x 256,
+ * both MMA warpgroups on one tile: Fin = Fout = 256), out[1] = A/B ring slots, out[2] = T1 stages; all 0 off the
+ * tensor cores.                                                                                                    */
+int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, int32_t out[3]);
 /* Debug: the paths the network schedules (p2m_meshnet_forward / _backward) take for layer `layer` at batch `batch`,
  * from the same route decision the schedules make.  need_dx only matters for layer 0 (the network input's gradient).
  * out[0] = forward conv on tensor cores, out[1] = its padding-vertex elision, out[2] = backward by the thin head's

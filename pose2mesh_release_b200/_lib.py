@@ -204,7 +204,7 @@ class H36MError(C.Structure):
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
-    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
+    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_conv_tiling", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_meshnet_workspace_bytes_opts", "p2m_meshnet_forward_opts",
     "p2m_meshnet_backward_opts", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
@@ -268,6 +268,8 @@ def load() -> C.CDLL:
         lib.p2m_debug_set_trace.restype = C.c_int
         lib.p2m_debug_conv_path.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
         lib.p2m_debug_conv_path.restype = C.c_int
+        lib.p2m_debug_conv_tiling.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
+        lib.p2m_debug_conv_tiling.restype = C.c_int
         lib.p2m_debug_layer_route.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
         lib.p2m_debug_layer_route.restype = C.c_int
         lib.p2m_debug_set_capture.argtypes = [vp, C.POINTER(Capture)]

@@ -471,16 +471,18 @@ __host__ __device__ constexpr int tile_rows() { return N == 128 ? 64 : TILE_M; }
 // these byte offsets from its 1024-byte aligned base, the host takes the launch size and every fit test from `bytes`
 // (the conv and dW sizes include 1024 + 32 bytes of slack that the kernels do not use).  Stage sizes are in floats.
 
-// cheb_conv_body<N, NS, XS, MODE> on tiles of at most max_h1 staged rows, metadata blobs meta_stride bytes apart
+// cheb_conv_body<N, NC, NS, XS, MODE> (NC output columns per CTA: 64, 128 or 256) on tiles of at most max_h1 staged
+// rows, metadata blobs meta_stride bytes apart
 struct ConvSmem {
   size_t xs, xs_stage, t1s, t1_stage, meta, bars, flags, ep, stage, own, tail, bytes;
 };
-__host__ __device__ __forceinline__ ConvSmem conv_smem(int N, int NS, int XS, int MODE, int max_h1, int meta_stride) {
+__host__ __device__ __forceinline__ ConvSmem conv_smem(int NC, int NS, int XS, int MODE, int max_h1, int meta_stride) {
+  const int N = NC == 64 ? 64 : 128;  // accumulator columns of an MMA warpgroup
   const int tm = N == 128 ? 64 : TILE_M;
   size_t at = 0, sum = 0;  // next offset; total size of the buffers
   auto take = [&](size_t bytes) { sum += bytes; at += bytes; return at - bytes; };
   ConvSmem L;
-  take((size_t)NS * (tm + N) * 128);  // the ring at offset 0, [NS] slots: A block (tm x 128 B) + B block (N x 128 B)
+  take((size_t)NS * (tm + NC) * 128);  // the ring at offset 0, [NS] slots: A block (tm x 128 B) + B block (NC x 128 B)
   // [XS][tm][32] fp32 own X rows: read in MODE 0 only (MODE 1 reads X from global memory); none at MODE 1, tm = 64
   L.xs_stage = (MODE == 1 && tm == 64) ? 0 : (size_t)tm * FC;
   L.xs = take(XS * L.xs_stage * 4);
@@ -489,7 +491,7 @@ __host__ __device__ __forceinline__ ConvSmem conv_smem(int N, int NS, int XS, in
   L.meta = take(2 * (size_t)meta_stride);    // [2] tile metadata blobs (the dense GEMM: none)
   L.bars = take(8 * (2 * NS + 2 * XS + 6));  // the kernel's barrier map
   L.flags = take(16);                        // word 1: the CTA's abort flag
-  L.ep = take(2 * 4 * N);                    // epilogue vectors ep_mul, ep_add [N]
+  L.ep = take(2 * 4 * NC);                   // epilogue vectors ep_mul, ep_add [NC]
   at = (at + 127) & ~(size_t)127;
   L.stage = take(4 * stg_warp_bytes(N));  // [4 warps] epilogue staging, 128-byte aligned
   L.own = take(4 * 32 * 4);               // [NWG][4 warps][ER] epilogue rows' vertex ids (NWG * ER = 32)
@@ -499,29 +501,34 @@ __host__ __device__ __forceinline__ ConvSmem conv_smem(int N, int NS, int XS, in
 }
 
 // The body of both conv kernels: k_cheb_conv_umma (N = 64) and k_cheb_conv_wide (N = 128) differ in their role map
-// and register targets (ConvRoles<N>) and in their launch size.
-template <int N, int NS, int XS, int MODE>
+// and register targets (ConvRoles<N>) and in their launch size.  NC = output columns per CTA: N, or 2 N (64 x 256,
+// k_cheb_conv_wide only), where both MMA warpgroups work on every tile, warpgroup g on the CTA's columns
+// [g N, g N + N), and read the one A block the producers built for them.
+template <int N, int NC, int NS, int XS, int MODE>
 __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
+  static_assert(NC == N || (N == 128 && NC == 2 * N && MODE == 1),
+                "64 x 256: both MMA warpgroups of the 64 x 128 layout, T1-given convs only (conv_cols)");
   static_assert(NS == 3 || NS == 6, "the producers fill a chunk's three slots back to back");
   using R = ConvRoles<N>;
   constexpr int TM = tile_rows<N>();  // tile rows
   constexpr int NPW = R::prod;        // producer warps
   constexpr int NRG = NPW * 4;        // producer row groups (8 threads each)
   constexpr int RPT = TM / NRG;       // tile rows per producer thread (2: row groups rg and NRG + rg of the row order)
-  constexpr int NWG = N == 128 ? 2 : 1;  // MMA + epilogue warpgroups (they alternate tiles)
+  constexpr int NWG = N == 128 ? 2 : 1;  // MMA + epilogue warpgroups (they alternate tiles, or split NC columns)
+  constexpr bool COLS = NC != N;         // 64 x 256: the warpgroups split the columns of every tile
   static_assert(RPT == 2, "both configurations give a producer thread two tile rows");
   constexpr int H = TM / 64;          // M = 64 halves of the tile (one accumulator each)
   constexpr int ER = 16 * H;          // epilogue rows per warp of the MMA warpgroup
   constexpr bool KT1 = (MODE == 1);
   constexpr bool plain = !KT1;
   constexpr int A_BYTES = TM * 128;  // one K-block of A: TM rows x (32 hi | 32 lo) fp16
-  constexpr int B_BLOCK_BYTES = N * 128;
+  constexpr int B_BLOCK_BYTES = NC * 128;
   constexpr int SLOT_BYTES = A_BYTES + B_BLOCK_BYTES;
-  static_assert(NWG * ER == 32 && SLOT_BYTES == (TM + N) * 128, "conv_smem describes this configuration");
+  static_assert(NWG * ER == 32 && SLOT_BYTES == (TM + NC) * 128, "conv_smem describes this configuration");
 
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  const ConvSmem L = conv_smem(N, NS, XS, MODE, p.max_h1, p.meta_stride);
+  const ConvSmem L = conv_smem(NC, NS, XS, MODE, p.max_h1, p.meta_stride);
   unsigned char* ring = smem_raw;  // 128B-swizzled blocks need 1024-byte alignment (checked below)
   float* Xs = reinterpret_cast<float*>(smem_raw + L.xs);
   float* T1s = reinterpret_cast<float*>(smem_raw + L.t1s);
@@ -534,14 +541,15 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   uint64_t* b_x_empty = b_x_full + XS;       // [XS]
   uint64_t* b_m_full = b_x_empty + XS;       // [2]
   uint64_t* b_m_empty = b_m_full + 2;        // [2]
-  // N = 128: the output stores of the tile before have read the staging buffer, which passes from one MMA warpgroup's
-  // epilogue to the other's (one arrival per warp); the tile before has finished its main loop (one arrival per warp)
+  // N = 128: the output stores of the epilogue before have read the staging buffer, which passes from one MMA
+  // warpgroup's epilogue to the other's (one arrival per warp); the tile before has finished its main loop (one arrival
+  // per warp; not used at NC = 2 N)
   uint64_t* b_stg_free = b_m_empty + 2;      // [1]
   uint64_t* b_turn = b_stg_free + 1;         // [1]
   uint32_t* flags = reinterpret_cast<uint32_t*>(smem_raw + L.flags);
   volatile int* abort_flag = reinterpret_cast<volatile int*>(flags + 1);
-  float* ep_mul = reinterpret_cast<float*>(smem_raw + L.ep);  // [N] acc * mul + add  (weight scale, bias, folded BN)
-  float* ep_add = ep_mul + N;
+  float* ep_mul = reinterpret_cast<float*>(smem_raw + L.ep);  // [NC] acc * mul + add  (weight scale, bias, folded BN)
+  float* ep_add = ep_mul + NC;
   // epilogue staging: N = 64: [4 warps][32 rows][EC floats], 16-byte chunks XOR-swizzled by the row, one 32-column
   // sub-slab at a time; N = 128: [4 warps][16 rows][STG_ROW_BYTES], a warp's whole 16 x 128 block in linear rows
   constexpr int EC = 32;
@@ -563,7 +571,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
     for (int s = 0; s < NS; ++s) {
       // one elected arrive per producer warp + the weight loader (dense GEMM mode: the loader alone)
       mbar_init(smem_u32(b_ab_full + s), p.apack != nullptr ? 1 : NPW + 1);
-      mbar_init(smem_u32(b_ab_empty + s), 4);  // one arrival per warp of the MMA warpgroup
+      mbar_init(smem_u32(b_ab_empty + s), COLS ? 8 : 4);  // one arrival per warp of each MMA warpgroup reading it
     }
     for (int s = 0; s < XS; ++s) {
       mbar_init(smem_u32(b_x_full + s), N_XLOAD * 32 + 1);  // every loader thread (cp.async.mbarrier.arrive.noinc)
@@ -585,13 +593,13 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   }
   const float a_scale = p.a_scale ? *p.a_scale : 1.f;
   const float b_inv = p.b_scale ? 1.f / *p.b_scale : W_INV_SCALE;
-  const int ecol0 = (int)blockIdx.y * N;  // first output column of this CTA's column slice
-  for (int n = threadIdx.x; n < N; n += R::threads) {
-    const float sc = (p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f) / a_scale;
-    const float sh = p.ep.scale ? p.ep.shift[ecol0 + n] : 0.f;
-    const float bi = p.ep.bias ? p.ep.bias[ecol0 + n] : 0.f;
+  const int ccol0 = (int)blockIdx.y * NC;  // first output column of this CTA's column slice
+  for (int n = threadIdx.x; n < NC; n += R::threads) {
+    const float sc = (p.ep.scale ? p.ep.scale[ccol0 + n] : 1.f) / a_scale;
+    const float sh = p.ep.scale ? p.ep.shift[ccol0 + n] : 0.f;
+    const float bi = p.ep.bias ? p.ep.bias[ccol0 + n] : 0.f;
     ep_mul[n] = b_inv * sc;
-    ep_add[n] = fmaf(bi, p.ep.scale ? p.ep.scale[ecol0 + n] : 1.f, sh);
+    ep_add[n] = fmaf(bi, p.ep.scale ? p.ep.scale[ccol0 + n] : 1.f, sh);
   }
   if (N == 64 && p.head_z != nullptr)
     for (int i = threadIdx.x; i < 64 * 12; i += R::threads) head_w_s[i] = p.head_wt[i];
@@ -737,7 +745,13 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
     // uses it * uses ..), so main loops run in tile order: a warpgroup starts one when the other has finished the tile
     // before (b_turn; the ring's parity waits then never run more than one phase ahead), and runs its epilogue while the
     // other issues the next tile's MMAs.  The staging buffer passes from one epilogue to the next (b_stg_free).
+    // NC = 2 N: both warpgroups take every tile, warpgroup g its columns [g N, g N + N) (the B block's rows g N ..),
+    // each slot is freed by the eight warps that read it, and the epilogues take the staging buffer in turn (warpgroup 0,
+    // then 1) while the producers fill the ring for the next tile.
     const int g = mma_g;
+    const int ecol0 = ccol0 + (COLS ? g * N : 0);  // first output column of this warpgroup's accumulator
+    const float* ep_mul_g = ep_mul + (COLS ? g * N : 0);
+    const float* ep_add_g = ep_add + (COLS ? g * N : 0);
     const int wq = warp - (g == 0 ? R::epi0 : R::epi1);
     const int tr = 3 + 2 * g;  // trace role of the warpgroup's warp 0
     constexpr int CPR = EC / 4;             // 16-byte chunks per staged row
@@ -751,7 +765,8 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
     const int trow = (lane >> 4) * 64 + wq * 16 + (lane & 15);  // tile row of local row `lane` (lane < ER)
     const int uses = plain ? n_chunk : n_use;
     int etn = 0;
-    for (int it = g; (int)blockIdx.x + it * (int)gridDim.x < p.n_tiles; it += NWG) {
+    for (int it = COLS ? 0 : g; (int)blockIdx.x + it * (int)gridDim.x < p.n_tiles; it += COLS ? 1 : NWG) {
+      const int e = COLS ? 2 * it + g : it;  // this epilogue's turn at the staging buffer
       const int tile = blockIdx.x + it * gridDim.x;
       const int b = tile / p.P, pat = tile - b * p.P;
       const long long mesh0 = (long long)b * p.V;
@@ -793,7 +808,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
 #pragma unroll
         for (int j = 0; j < 32; ++j) acc[h][j] = 0.f;
       if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 1);
-      if (NWG == 2 && it > 0) {
+      if (NWG == 2 && !COLS && it > 0) {
         mbar_wait(smem_u32(b_turn), (uint32_t)(it - 1) & 1u, abort_flag, p.status, 13);
         if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 3);
       }
@@ -812,7 +827,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           // each A sub-block is read once per K step; every output element sees the same six k16 MMAs in the same
           // order as with two m64n64 column halves
           const uint64_t da = make_desc_sw128(a0);
-          const uint64_t db = make_desc_sw128(a0 + A_BYTES);
+          const uint64_t db = make_desc_sw128(a0 + A_BYTES + (COLS ? (uint32_t)g * (N * 128) : 0u));
           wgmma_m64n128(acc, da + 0, db + 0);  // hi * Whi
           wgmma_m64n128(acc, da + 2, db + 2);
           wgmma_m64n128(acc, da + 4, db + 0);  // lo * Whi
@@ -838,7 +853,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(b_ab_empty + s));  // this warp is done reading the slot
       }
-      if (NWG == 2 && lane == 0) mbar_arrive(smem_u32(b_turn));  // the next tile's main loop may start
+      if (NWG == 2 && !COLS && lane == 0) mbar_arrive(smem_u32(b_turn));  // the next tile's main loop may start
       if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 2);
       // N = 64, phase 1 of sub-slab cb (32 columns): the fragment into the staging rows (16-byte chunks XOR-swizzled by
       // row)
@@ -896,8 +911,8 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
         // stores have read it.  An identity residual then lands in it by bulk copy (one 512-byte row per valid row,
         // straight into the row's slot, from L2: prefetched at tile start).  In the accumulator's own layout, in place:
         // o = act(acc * mul + add), plus that residual, goes to the element's slot of its linear staging row.
-        // (b_res[wq] is armed and waited for by one tile at a time, in tile order: its phase is the tile's parity)
-        if (it > 0) mbar_wait(smem_u32(b_stg_free), (uint32_t)(it - 1) & 1u, abort_flag, p.status, 14);
+        // (b_res[wq] is armed and waited for by one epilogue at a time, in turn order: its phase is the turn's parity)
+        if (e > 0) mbar_wait(smem_u32(b_stg_free), (uint32_t)(e - 1) & 1u, abort_flag, p.status, 14);
         if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 20);
         const bool res_id = p.ep.res != nullptr && p.res_identity;
         if (res_id) {
@@ -910,7 +925,7 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
             bulk_g2s(stg + lane * STG_ROW_BYTES, p.ep.res + (p.ep.res_unpool ? (r >> 1) : r) * p.ep.res_F + ecol0, N * 4,
                      rbar);
           }
-          mbar_wait(rbar, (uint32_t)it & 1u, abort_flag, p.status, 12);
+          mbar_wait(rbar, (uint32_t)e & 1u, abort_flag, p.status, 12);
         }
         if (wq == 0 && lane == 0) trace_ev(p, tr, etn, 21);
 #pragma unroll
@@ -918,8 +933,8 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
 #pragma unroll
           for (int jg = 0; jg < 8; ++jg) {
             const int n = 64 * h + 8 * jg + 2 * (lane & 3);  // column pair of acc[h][4 jg + 2 r + {0, 1}]
-            const float2 mu = *reinterpret_cast<const float2*>(ep_mul + n);
-            const float2 ad = *reinterpret_cast<const float2*>(ep_add + n);
+            const float2 mu = *reinterpret_cast<const float2*>(ep_mul_g + n);
+            const float2 ad = *reinterpret_cast<const float2*>(ep_add_g + n);
 #pragma unroll
             for (int r = 0; r < 2; ++r) {
               const int j = 4 * jg + 2 * r;
@@ -1199,11 +1214,12 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
 template <int N, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
   static_assert(N == 64, "the 64 x 128 configuration is k_cheb_conv_wide");
-  cheb_conv_body<N, NS, XS, MODE>(p);
+  cheb_conv_body<N, N, NS, XS, MODE>(p);
 }
-template <int NS, int XS, int MODE>
+// NC = 128 (64 x 128) or 256 (64 x 256) output columns per CTA
+template <int NC, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS_W, 1) k_cheb_conv_wide(const __grid_constant__ KParams p) {
-  cheb_conv_body<128, NS, XS, MODE>(p);
+  cheb_conv_body<128, NC, NS, XS, MODE>(p);
 }
 
 // =====================================================================================
@@ -1740,6 +1756,7 @@ int launch_pack(const PackSrc& src, long long n_blocks, void* out, cudaStream_t 
 constexpr size_t SMEM_LIMIT = 227 * 1024;
 constexpr int CONV_N = 64;  // output columns per CTA of the 128-row conv configuration (one column slice)
 constexpr int WIDE_N = 128; // ... and of the 64-row configuration (convs with Fout % 128 == 0)
+constexpr int PAIR_N = 256; // ... and of its 64 x 256 mode (both MMA warpgroups on one tile: Fout == 256)
 inline int conv_n(int fout) { return fout % WIDE_N == 0 ? WIDE_N : CONV_N; }
 // the tile metadata a launch with N output columns per CTA runs on: the level's consecutive tiles or the tile family the
 // caller selected, 128-row blobs for N = 64 and 64-row blobs for N = 128
@@ -1747,17 +1764,27 @@ const TileBlobs& conv_tiles(int N, const DevLevel& g, const TileSet* tiles) {
   if (tiles != nullptr) return N == WIDE_N ? tiles->m64 : *tiles;
   return N == WIDE_N ? g.meta64 : g.meta128;
 }
-// A/B ring depth and X staging depth of a conv launch: the deepest that fit, the ring first (N = 128: 6 slots = two
-// chunks, the producers run a chunk ahead of the MMAs, or 3 = one chunk; N = 64: 3), then 2 X stages (prefetch the next
-// chunk's rows during the current chunk) or 1.  {0, 0}: does not fit.
+// A/B ring depth and X staging depth of a conv launch with NC output columns per CTA: the deepest that fit, the ring
+// first (NC = 128: 6 slots = two chunks, the producers run a chunk ahead of the MMAs, or 3 = one chunk; NC = 64 and
+// NC = 256, whose six 40 KB slots never fit: 3), then 2 X stages (prefetch the next chunk's rows during the current
+// chunk) or 1.  {0, 0}: does not fit.
 struct ConvCfg {
   int ns, xs;
 };
-ConvCfg conv_cfg(int N, const TileBlobs& t, bool t1_given) {
-  for (int ns = N == WIDE_N ? 6 : 3; ns >= 3; ns -= 3)
+ConvCfg conv_cfg(int NC, const TileBlobs& t, bool t1_given) {
+  for (int ns = NC == WIDE_N ? 6 : 3; ns >= 3; ns -= 3)
     for (int xs = 2; xs >= 1; --xs)
-      if (conv_smem(N, ns, xs, t1_given, t.max_h1, t.stride).bytes <= SMEM_LIMIT) return {ns, xs};
+      if (conv_smem(NC, ns, xs, t1_given, t.max_h1, t.stride).bytes <= SMEM_LIMIT) return {ns, xs};
   return {0, 0};
+}
+// Output columns per CTA of a conv Fin -> Fout on tiles t.  The 64 x 256 mode builds each A block once for all 256
+// columns, but its two warpgroups finish a tile together, so each tile's epilogue runs behind its main loop instead of
+// under the other warpgroup's: that pays where the main loop is long, the T1-given 256 -> 256 conv (24 K-blocks per
+// tile: 13-21 % faster layers), and not at 12 (128 -> 256: 8 % slower; H100 SXM, README).  It is taken there when its
+// ring of three slots fits; every other conv with Fout % 128 == 0 runs as 128-column slices.
+int conv_cols(int fin, int fout, const TileBlobs& t, bool t1_given) {
+  const bool pair = fout == PAIR_N && fin == PAIR_N && t1_given && conv_cfg(PAIR_N, t, true).ns > 0;
+  return pair ? PAIR_N : conv_n(fout);
 }
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point lookup (no link-time dependency on libcuda)
@@ -1788,21 +1815,22 @@ bool make_row_tmap(CUtensorMap* tm, const float* base, long long rows, int fin, 
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// The conv kernel of configuration N: k_cheb_conv_umma (N = 64) or k_cheb_conv_wide (N = 128)
-template <int N, int NS, int XS, int MODE>
+// The conv kernel with NC output columns per CTA: k_cheb_conv_umma (64) or k_cheb_conv_wide (128, 256)
+template <int NC, int NS, int XS, int MODE>
 constexpr auto conv_kernel() {
-  if constexpr (N == WIDE_N) return k_cheb_conv_wide<NS, XS, MODE>;
-  else return k_cheb_conv_umma<N, NS, XS, MODE>;
+  if constexpr (NC != CONV_N) return k_cheb_conv_wide<NC, NS, XS, MODE>;
+  else return k_cheb_conv_umma<NC, NS, XS, MODE>;
 }
 // A conv kernel's setmaxnreg split is balanced for a launch allocation of ConvRoles<N>::regs_launch registers per
 // thread (80 for k_cheb_conv_umma, 96 for k_cheb_conv_wide): a build that ends up with another count would leave the
 // epilogue's setmaxnreg.inc spinning on an empty pool.
-template <int N, int NS, int XS, int MODE>
+template <int NC, int NS, int XS, int MODE>
 int check_launch_regs() {
+  constexpr int N = NC == CONV_N ? CONV_N : WIDE_N;
   static int state = 0;  // per instantiation; racing first calls all compute the same value
   if (state == 0) {
     cudaFuncAttributes fa;
-    P2M_CUDA_OK(cudaFuncGetAttributes(&fa, conv_kernel<N, NS, XS, MODE>()));
+    P2M_CUDA_OK(cudaFuncGetAttributes(&fa, conv_kernel<NC, NS, XS, MODE>()));
     state = (fa.numRegs == ConvRoles<N>::regs_launch) ? 1 : -1;
   }
   if (state < 0) {
@@ -1814,16 +1842,18 @@ int check_launch_regs() {
   return P2M_OK;
 }
 
-// a.plain selects the instantiation: MODE 0 (plain GEMM) or MODE 1 (T1 given)
-template <int N, int NS, int XS>
+// a.plain selects the instantiation: MODE 0 (plain GEMM) or MODE 1 (T1 given); NC output columns per CTA
+template <int NC, int NS, int XS>
 int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
+  constexpr int N = NC == CONV_N ? CONV_N : WIDE_N;
   constexpr int TM = tile_rows<N>();
   const DevLevel& g = *a.g;
   const TileBlobs& t = conv_tiles(N, g, a.tiles);
-  const size_t smem = conv_smem(N, NS, XS, !a.plain, t.max_h1, t.stride).bytes;
-  auto kern = a.plain ? conv_kernel<N, NS, XS, 0>() : conv_kernel<N, NS, XS, 1>();
+  const size_t smem = conv_smem(NC, NS, XS, !a.plain, t.max_h1, t.stride).bytes;
+  constexpr int M0 = NC == PAIR_N ? 1 : 0;  // MODE of a plain launch (the 64 x 256 mode has none: conv_cols)
+  auto kern = a.plain ? conv_kernel<NC, NS, XS, M0>() : conv_kernel<NC, NS, XS, 1>();
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  P2M_TRY((a.plain ? check_launch_regs<N, NS, XS, 0>() : check_launch_regs<N, NS, XS, 1>()));
+  P2M_TRY((a.plain ? check_launch_regs<NC, NS, XS, M0>() : check_launch_regs<NC, NS, XS, 1>()));
   KParams p;
   p.x = a.x;
   p.in_unpool = a.in_unpool;
@@ -1838,8 +1868,8 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.n_tiles = a.batch * p.P;
   p.wpack = static_cast<const unsigned char*>(a.wpack);
   p.apack = nullptr;
-  // the weight image holds K-blocks of fout rows x 128 bytes; column slice y starts y * N rows into each block
-  p.wslice_bytes = (long long)N * 128;
+  // the weight image holds K-blocks of fout rows x 128 bytes; column slice y starts y * NC rows into each block
+  p.wslice_bytes = (long long)NC * 128;
   p.wblock_stride = (long long)a.fout * 128;
   p.zero_row = zero_row;
   p.ep = to_dev(a.ep);
@@ -1856,7 +1886,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.head_z = a.fout == 64 ? a.head_z : nullptr;
   if (N == WIDE_N) {
     // the epilogue moves whole 512-byte output rows (and identity-residual rows) by cp.async.bulk, which needs 16-byte
-    // aligned addresses (a CTA's first column, 128 blockIdx.y, keeps that)
+    // aligned addresses (a warpgroup's first column, a multiple of 128, keeps that)
     const bool y_ok = (reinterpret_cast<uintptr_t>(p.y) & 15u) == 0 && (p.ldy * 4) % 16 == 0 && (p.y_col0 * 4) % 16 == 0;
     const bool res_ok = !p.res_identity || ((reinterpret_cast<uintptr_t>(p.ep.res) & 15u) == 0 && (p.ep.res_F * 4) % 16 == 0);
     if (!y_ok || !res_ok) {
@@ -1873,7 +1903,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
     if (ok && a.t1 != nullptr) ok = make_row_tmap(&p.tm_t1, a.t1, rows, a.fin, TM);
     p.tma = ok ? 1 : 0;
   }
-  const int n_slices = a.fout / N;
+  const int n_slices = a.fout / NC;
   const dim3 grid(std::min(p.n_tiles, std::max(1, sm_count / n_slices)), n_slices);
   kern<<<grid, ConvRoles<N>::threads, smem, s>>>(p);
   P2M_LAUNCH_OK();
@@ -1882,11 +1912,16 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
 
 int launch_n(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
   const int N = conv_n(a.fout);
-  const ConvCfg c = conv_cfg(N, conv_tiles(N, *a.g, a.tiles), !a.plain);
+  const TileBlobs& t = conv_tiles(N, *a.g, a.tiles);
+  const int NC = conv_cols(a.fin, a.fout, t, !a.plain);
+  const ConvCfg c = conv_cfg(NC, t, !a.plain);
   if (c.ns == 0) {
     set_error("umma_conv: tile family does not fit shared memory");
     return P2M_ERR_INVALID;
   }
+  if (NC == PAIR_N)
+    return c.xs == 2 ? launch_cfg<PAIR_N, 3, 2>(a, status, zero_row, sm_count, s)
+                     : launch_cfg<PAIR_N, 3, 1>(a, status, zero_row, sm_count, s);
   if (N == CONV_N)
     return c.xs == 2 ? launch_cfg<CONV_N, 3, 2>(a, status, zero_row, sm_count, s)
                      : launch_cfg<CONV_N, 3, 1>(a, status, zero_row, sm_count, s);
@@ -2182,10 +2217,17 @@ bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
          conv_smem(N, 3, 1, 0, t.max_h1, t.stride).bytes <= SMEM_LIMIT;
 }
 
-// X staging depth launch_n picks for a conv of Fout columns on the level's consecutive tiles (T1 given, or plain)
-int umma_conv_x_stages(const DevLevel& g, int fout, bool plain) {
+// What launch_n picks for a conv Fin -> Fout on the level's consecutive tiles (T1 given, or plain): its X staging
+// depth, and its output columns per CTA, ring slots and X stages
+int umma_conv_x_stages(const DevLevel& g, int fin, int fout, bool plain) {
+  return umma_conv_tiling(g, fin, fout, plain).xs;
+}
+UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain) {
   const int N = conv_n(fout);
-  return conv_cfg(N, conv_tiles(N, g, nullptr), !plain).xs;
+  const TileBlobs& t = conv_tiles(N, g, nullptr);
+  const int NC = conv_cols(fin, fout, t, !plain);
+  const ConvCfg c = conv_cfg(NC, t, !plain);
+  return {NC, c.ns, c.xs};
 }
 bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && tmap_encoder() != nullptr; }
 

@@ -873,14 +873,28 @@ int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int3
   const DevLevel& g = m->levels[level];
   const ConvRoute r = conv_route(m, level, fin, fout, 1, false);  // what p2m_cheb_conv_fwd / _bwd run
   out[0] = r.tc;
-  out[1] = r.tc ? umma_conv_x_stages(g, fout, false) : 0;
+  out[1] = r.tc ? umma_conv_x_stages(g, fin, fout, false) : 0;
   out[2] = r.tc_dw;
   out[3] = r.tc_dw ? umma_dw_x_stages(g) : 0;
   out[4] = r.tc_dt;
-  out[5] = r.tc_dt ? umma_conv_x_stages(g, fin, true) : 0;
+  out[5] = r.tc_dt ? umma_conv_x_stages(g, fout, fin, true) : 0;
   out[6] = (g.meta128.n_pattern > 0 && umma_tma_rows(g)) ? 1 : 0;
   out[7] = g.meta128.max_h1;
   out[8] = g.n_iso;
+  return P2M_OK;
+}
+
+int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, int32_t out[3]) {
+  if (!m || !out || level < 0 || level >= (int)m->levels.size() || fin <= 0 || fout <= 0) {
+    set_error("debug_conv_tiling: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  const DevLevel& g = m->levels[level];
+  const UmmaConvTiling t = conv_route(m, level, fin, fout, 1, false).tc ? umma_conv_tiling(g, fin, fout, false)
+                                                                        : UmmaConvTiling{0, 0, 0};
+  out[0] = t.cols;
+  out[1] = t.ns;
+  out[2] = t.xs;
   return P2M_OK;
 }
 

@@ -465,7 +465,11 @@ int build_tileset(const std::vector<int>& rows, const int* rowptr, const int* co
                   TileSet* ts, std::vector<void*>* owned);
 bool umma_conv_supported(const DevLevel& g, int fin, int fout);
 // what launch_umma_conv / launch_umma_dw would select on the level's consecutive tiles (p2m_debug_conv_path)
-int umma_conv_x_stages(const DevLevel& g, int fout, bool plain);
+int umma_conv_x_stages(const DevLevel& g, int fin, int fout, bool plain);
+struct UmmaConvTiling {
+  int cols, ns, xs;  // output columns per CTA (64, 128 or 256), A/B ring slots, X / T1 stages (0: does not fit)
+};
+UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain);
 int umma_dw_x_stages(const DevLevel& g);
 bool umma_tma_rows(const DevLevel& g);
 // Weight images of a conv: fp16 [hi | lo] K-blocks of 32 k (x 2^6) from W [fout, fin*3] in the reference layout (column
