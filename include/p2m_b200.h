@@ -38,8 +38,16 @@ enum p2m_status {
 
 enum p2m_precision {
   P2M_PREC_FP32_SIMT = 0, /* fp32 FFMA on CUDA cores (all shapes; the parity baseline)          */
-  P2M_PREC_FP16X3_TC = 1  /* wgmma f16 -> f32, error-compensated 3-term fp16 split (~2^-21) */
+  P2M_PREC_FP16X3_TC = 1, /* wgmma f16 -> f32, error-compensated 3-term fp16 split (~2^-21) */
+  P2M_PREC_FP16_TC = 2    /* inference only: single-pass wgmma, fp16 operands, fp32 accumulate   */
 };
+/* P2M_PREC_FP16_TC: the Chebyshev convs of the eval forward round both operands to the nearest fp16 (activations
+ * unscaled, weights x 2^6) and accumulate in fp32: one MMA per 16 features instead of three, a per-product relative
+ * error of at most 2^-10 + 2^-22 (fp16x3: ~2^-21).  Everything else runs as at fp16x3: the T1 pass, the epilogues, the
+ * fc dense GEMM (fp16x3) and the thin head.  Entry points at this precision: p2m_meshnet_forward(_opts) in the eval
+ * schedule, p2m_meshnet_forward_vertices, p2m_meshnet_forward_host (and _vertices_host) and p2m_cheb_conv_fwd (bn_mode
+ * 0 or 1).  The training schedule (training = 1, or BatchNorm options that select it), p2m_meshnet_backward(_opts),
+ * p2m_cheb_conv_bwd and p2m_cheb_conv_fwd with bn_mode 2 return P2M_ERR_INVALID before any device work.            */
 
 /* ---- the fixed mesh hierarchy + channel plan ---------------------------------------------------
  * Replaces what Pose2Mesh.__init__ derives from graph_L (meshnet.py:17-37,61-62): `n_levels`

@@ -16,7 +16,8 @@ LIB_PATH = os.path.join(_HERE, "libp2m_b200.so")
 
 P2M_PREC_FP32_SIMT = 0
 P2M_PREC_FP16X3_TC = 1
-PRECISIONS = {"fp32": P2M_PREC_FP32_SIMT, "fp16x3": P2M_PREC_FP16X3_TC}
+P2M_PREC_FP16_TC = 2  # inference only: single-pass fp16 operands in the Chebyshev convs (include/p2m_b200.h)
+PRECISIONS = {"fp32": P2M_PREC_FP32_SIMT, "fp16x3": P2M_PREC_FP16X3_TC, "fp16": P2M_PREC_FP16_TC}
 
 
 def default_precision() -> int:

@@ -23,9 +23,10 @@ _default_precision = _lib.default_precision()
 
 
 def set_default_precision(precision: str):
-    """'fp32' (CUDA cores) or 'fp16x3' (wgmma tensor cores) for graph_conv_cheby calls."""
+    """'fp32' (CUDA cores), 'fp16x3' (wgmma tensor cores) or 'fp16' (single-pass wgmma, inference only: a backward or a
+    training-mode BatchNorm raises) for graph_conv_cheby calls."""
     global _default_precision
-    _default_precision = {"fp32": _lib.P2M_PREC_FP32_SIMT, "fp16x3": _lib.P2M_PREC_FP16X3_TC}[precision]
+    _default_precision = _lib.PRECISIONS[precision]
     for _, gh in list(_graph_cache.values()):
         gh.apply_precision()
 
@@ -163,6 +164,9 @@ def graph_conv_cheby(x, cl, bn, L, Fout, K):
     if K != 3:
         raise NotImplementedError("pose2mesh_release_b200 implements the Chebyshev order the reference uses (K=3)")
     B, V, _ = x.shape
+    if bn is not None and bn.training and _default_precision == _lib.P2M_PREC_FP16_TC:
+        raise RuntimeError("graph_conv_cheby: precision 'fp16' is an inference precision; a training-mode BatchNorm "
+                           "needs 'fp16x3' or 'fp32'")
     y = ChebConvLinear.apply(x, cl.weight, cl.bias, graph_handle(L))
     if y.shape[2] != Fout:
         raise ValueError("Fout does not match the Linear layer")

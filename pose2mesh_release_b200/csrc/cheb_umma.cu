@@ -343,9 +343,32 @@ __host__ __device__ __forceinline__ uint32_t sw128_off(int row, int chunk) {
   return (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4);
 }
 
+// K-major, 64B-swizzled operand block of the single-pass fp16 precision (rows of 64 bytes = 32 fp16, 8-row atoms of
+// 512 bytes): the hardware XORs address bits [4,6) with bits [7,9), i.e. the 16-byte chunk with (row >> 1) & 3.
+// Descriptor: as above with SBO = 512 B and layout type SWIZZLE_64B = 2 (blocks are 512-byte aligned).
+__device__ __forceinline__ uint64_t make_desc_sw64(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;           // LBO (unused for swizzled K-major) = 16 B
+  d |= (uint64_t)(512 >> 4) << 32;  // SBO = 512 B between 8-row groups
+  d |= (uint64_t)2 << 62;           // SWIZZLE_64B
+  return d;
+}
+// byte offset of 16-byte chunk `chunk` (0..3) of row `row` inside a 64B-swizzled block
+__host__ __device__ __forceinline__ uint32_t sw64_off(int row, int chunk) {
+  return (uint32_t)row * 64u + (uint32_t)((chunk ^ ((row >> 1) & 3)) << 4);
+}
+// bytes per operand row of a K-block (32 features): fp16 (hi | lo) for fp16x3, hi only for the single pass
+__host__ __device__ constexpr int op_row_bytes(bool f16) { return f16 ? 64 : 128; }
+
 struct Half4 {
   __half2 a, b;
 };
+// fp16 round-to-nearest of four values (the single-pass precision's operand)
+__device__ __forceinline__ uint2 half4(const float4& v) {
+  __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
+  return make_uint2(*reinterpret_cast<uint32_t*>(&h0), *reinterpret_cast<uint32_t*>(&h1));
+}
 __device__ __forceinline__ void split4(const float4& v, uint2& hi, uint2& lo) {
   __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
   float2 f0 = __half22float2(h0), f1 = __half22float2(h1);
@@ -471,18 +494,20 @@ __host__ __device__ constexpr int tile_rows() { return N == 128 ? 64 : TILE_M; }
 // these byte offsets from its 1024-byte aligned base, the host takes the launch size and every fit test from `bytes`
 // (the conv and dW sizes include 1024 + 32 bytes of slack that the kernels do not use).  Stage sizes are in floats.
 
-// cheb_conv_body<N, NC, NS, XS, MODE> (NC output columns per CTA: 64, 128 or 256) on tiles of at most max_h1 staged
-// rows, metadata blobs meta_stride bytes apart
+// cheb_conv_body<N, NC, NS, XS, MODE, F16> (NC output columns per CTA: 64, 128 or 256) on tiles of at most max_h1
+// staged rows, metadata blobs meta_stride bytes apart
 struct ConvSmem {
   size_t xs, xs_stage, t1s, t1_stage, meta, bars, flags, ep, stage, own, tail, bytes;
 };
-__host__ __device__ __forceinline__ ConvSmem conv_smem(int NC, int NS, int XS, int MODE, int max_h1, int meta_stride) {
+__host__ __device__ __forceinline__ ConvSmem conv_smem(int NC, int NS, int XS, int MODE, int max_h1, int meta_stride,
+                                                       bool f16 = false) {
   const int N = NC == 64 ? 64 : 128;  // accumulator columns of an MMA warpgroup
   const int tm = N == 128 ? 64 : TILE_M;
   size_t at = 0, sum = 0;  // next offset; total size of the buffers
   auto take = [&](size_t bytes) { sum += bytes; at += bytes; return at - bytes; };
   ConvSmem L;
-  take((size_t)NS * (tm + NC) * 128);  // the ring at offset 0, [NS] slots: A block (tm x 128 B) + B block (NC x 128 B)
+  // the ring at offset 0, [NS] slots: A block (tm rows) + B block (NC rows) of 128 B (fp16x3) or 64 B (fp16) rows
+  take((size_t)NS * (tm + NC) * op_row_bytes(f16));
   // [XS][tm][32] fp32 own X rows: read in MODE 0 only (MODE 1 reads X from global memory); none at MODE 1, tm = 64
   L.xs_stage = (MODE == 1 && tm == 64) ? 0 : (size_t)tm * FC;
   L.xs = take(XS * L.xs_stage * 4);
@@ -504,7 +529,10 @@ __host__ __device__ __forceinline__ ConvSmem conv_smem(int NC, int NS, int XS, i
 // and register targets (ConvRoles<N>) and in their launch size.  NC = output columns per CTA: N, or 2 N (64 x 256,
 // k_cheb_conv_wide only), where both MMA warpgroups work on every tile, warpgroup g on the CTA's columns
 // [g N, g N + N), and read the one A block the producers built for them.
-template <int N, int NC, int NS, int XS, int MODE>
+// F16: the single-pass fp16 precision (P2M_PREC_FP16_TC, inference): a K-block holds only the fp16 round-to-nearest of
+// each operand (64-byte rows, 64B-swizzled) and every 16 features take one k16 MMA instead of three.  Same chunks, slots
+// and barrier protocol; T1-given and plain convs of the eval forward only (no dense-GEMM mode, no a_scale).
+template <int N, int NC, int NS, int XS, int MODE, bool F16>
 __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
   static_assert(NC == N || (N == 128 && NC == 2 * N && MODE == 1),
@@ -522,13 +550,15 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   constexpr int ER = 16 * H;          // epilogue rows per warp of the MMA warpgroup
   constexpr bool KT1 = (MODE == 1);
   constexpr bool plain = !KT1;
-  constexpr int A_BYTES = TM * 128;  // one K-block of A: TM rows x (32 hi | 32 lo) fp16
-  constexpr int B_BLOCK_BYTES = NC * 128;
+  constexpr int RB = op_row_bytes(F16);  // bytes per operand row of a K-block
+  constexpr int A_BYTES = TM * RB;       // one K-block of A: TM rows x (32 hi | 32 lo) fp16, or 32 fp16 (F16)
+  constexpr int B_BLOCK_BYTES = NC * RB;
   constexpr int SLOT_BYTES = A_BYTES + B_BLOCK_BYTES;
-  static_assert(NWG * ER == 32 && SLOT_BYTES == (TM + NC) * 128, "conv_smem describes this configuration");
+  static_assert(NWG * ER == 32 && SLOT_BYTES == (TM + NC) * RB, "conv_smem describes this configuration");
+  static_assert(SLOT_BYTES % 1024 == 0 && A_BYTES % 1024 == 0, "swizzled blocks stay aligned to their atoms");
 
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  const ConvSmem L = conv_smem(NC, NS, XS, MODE, p.max_h1, p.meta_stride);
+  const ConvSmem L = conv_smem(NC, NS, XS, MODE, p.max_h1, p.meta_stride, F16);
   unsigned char* ring = smem_raw;  // 128B-swizzled blocks need 1024-byte alignment (checked below)
   float* Xs = reinterpret_cast<float*>(smem_raw + L.xs);
   float* T1s = reinterpret_cast<float*>(smem_raw + L.t1s);
@@ -821,8 +851,21 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
         const uint32_t a0 = smem_u32(ring + s * SLOT_BYTES);
         wg_fence();
         // A block columns: [hi 0..31 | lo 32..63], B block columns: [Whi 0..31 | Wlo 32..63] (fp16); a 16-element K
-        // step is 32 bytes = +2 in the descriptor's start-address field
-        if constexpr (N == 128) {
+        // step is 32 bytes = +2 in the descriptor's start-address field.  F16: columns 0..31 only, two k16 steps.
+        if constexpr (F16 && N == 128) {
+          const uint64_t da = make_desc_sw64(a0);
+          const uint64_t db = make_desc_sw64(a0 + A_BYTES + (COLS ? (uint32_t)g * (N * RB) : 0u));
+          wgmma_m64n128(acc, da + 0, db + 0);
+          wgmma_m64n128(acc, da + 2, db + 2);
+        } else if constexpr (F16) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint64_t da = make_desc_sw64(a0 + (uint32_t)h * (64 * RB));
+            const uint64_t db = make_desc_sw64(a0 + A_BYTES);
+            wgmma_m64n64(acc[h], da + 0, db + 0);
+            wgmma_m64n64(acc[h], da + 2, db + 2);
+          }
+        } else if constexpr (N == 128) {
           // the whole 128-row B block is one N = 128 operand (its rows 64..127 are the next eight 1024-byte atoms), so
           // each A sub-block is read once per K step; every output element sees the same six k16 MMAs in the same
           // order as with two m64n64 column halves
@@ -1105,9 +1148,13 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           row[ps] = plain ? (uint32_t)(NRG * ps + rg) : lds_u16(ord2_a + 2 * (NRG * ps + rg));
           re[ps] = plain ? 0u : (lds_u16(rp_a + 2 * row[ps]) | (lds_u16(rp_a + 2 * row[ps] + 2) << 16));
           const uint32_t i = row[ps];
-          const uint32_t a_hi = sw128_off(i, q >> 1) + (q & 1) * 8, a_lo = sw128_off(i, 4 + (q >> 1)) + (q & 1) * 8;
-          so_f[ps] = odd ? a_lo : a_hi;
-          so_s[ps] = odd ? a_hi : a_lo;
+          if (F16) {  // one 8-byte piece per row (a row lies in the 64-byte bank half of its parity)
+            so_f[ps] = so_s[ps] = sw64_off(i, q >> 1) + (q & 1) * 8;
+          } else {
+            const uint32_t a_hi = sw128_off(i, q >> 1) + (q & 1) * 8, a_lo = sw128_off(i, 4 + (q >> 1)) + (q & 1) * 8;
+            so_f[ps] = odd ? a_lo : a_hi;
+            so_s[ps] = odd ? a_hi : a_lo;
+          }
         }
         if (KT1) {
           const int* halo = reinterpret_cast<const int*>(mb + hdr->off_halo);  // slots 0..TM-1 = the tile's own rows
@@ -1134,6 +1181,10 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           const uint32_t i = ps * NRG + rg;
           float4 v = lds_f4(xs_q + (i >> xsh) * 128);
           v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
+          if (F16) {  // rows rg and rg + 1 of a half-warp have opposite parity: different 64-byte bank halves
+            sts_u2(ablk + so_f[ps], half4(v));
+            continue;
+          }
           uint2 hi, lo;
           split4(v, hi, lo);
           // the four consecutive rows of a warp share (row & 4), i.e. the 64-byte half their hi parts go to: odd row
@@ -1164,6 +1215,10 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
           float4 v = vv[ps];
           if (p.a_scale != nullptr) {  // backward-data pass: gradients are scaled into fp16's range (power of two)
             v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
+          }
+          if (F16) {  // (two rows of one parity in a half-warp take two wavefronts: see balance_store_halves)
+            sts_u2(ablk + so_f[ps], half4(v));
+            continue;
           }
           split4(v, hi, lo);
           // 64-bit shared stores are served per HALF-warp (two rows here).  Odd row groups store lo first — by
@@ -1214,12 +1269,22 @@ __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
 template <int N, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_umma(const __grid_constant__ KParams p) {
   static_assert(N == 64, "the 64 x 128 configuration is k_cheb_conv_wide");
-  cheb_conv_body<N, N, NS, XS, MODE>(p);
+  cheb_conv_body<N, N, NS, XS, MODE, false>(p);
 }
 // NC = 128 (64 x 128) or 256 (64 x 256) output columns per CTA
 template <int NC, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS_W, 1) k_cheb_conv_wide(const __grid_constant__ KParams p) {
-  cheb_conv_body<128, NC, NS, XS, MODE>(p);
+  cheb_conv_body<128, NC, NS, XS, MODE, false>(p);
+}
+// The same two configurations at the single-pass fp16 precision (P2M_PREC_FP16_TC): one body, F16 = true
+template <int N, int NS, int XS, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_f16_umma(const __grid_constant__ KParams p) {
+  static_assert(N == 64, "the 64 x 128 configuration is k_cheb_conv_f16_wide");
+  cheb_conv_body<N, N, NS, XS, MODE, true>(p);
+}
+template <int NC, int NS, int XS, int MODE>
+__global__ void __launch_bounds__(NUM_THREADS_W, 1) k_cheb_conv_f16_wide(const __grid_constant__ KParams p) {
+  cheb_conv_body<128, NC, NS, XS, MODE, true>(p);
 }
 
 // =====================================================================================
@@ -1711,7 +1776,8 @@ __global__ void __launch_bounds__(512, 2) k_cheb_t1(const T1Params p) {
 // b = (t * n_chunk + chunk) * orders + order holds rows n = t * rows + [0, rows) and k = 32 chunk + [0, 32):
 // p[n ld_row + k ld_k + order] * scale, zero for n >= n_real or k >= k_real (never read there); `combined`: the isolated
 // rows' combined weights (p[a] + c p[a + 1] + (2c^2 - 1) p[a + 2]) * scale at a = n ld_row + k ld_k.  With dscale the
-// scale is scale * *dscale.
+// scale is scale * *dscale.  hi_only: the single-pass fp16 image, 64-byte rows of the 32 fp16 values (no lo part),
+// 64B-swizzled.
 struct PackSrc {
   const float* p;
   long long ld_row, ld_k;
@@ -1721,13 +1787,15 @@ struct PackSrc {
   float c;
   int k_real = INT_MAX;
   const float* dscale = nullptr;  // device scalar: a power of two found from the operand's largest magnitude
+  int hi_only = 0;
 };
 __global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, unsigned char* __restrict__ out) {
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 16-byte chunk each
   if (idx >= total) return;
-  const int j = (int)(idx & 7);
-  const int row = (int)((idx >> 3) % s.rows);
-  const long long blk = (idx >> 3) / s.rows;
+  const int cl2 = s.hi_only ? 2 : 3;  // log2 of the 16-byte chunks per row
+  const int j = (int)(idx & ((1 << cl2) - 1));
+  const int row = (int)((idx >> cl2) % s.rows);
+  const long long blk = (idx >> cl2) / s.rows;
   const int per_tile = s.n_chunk * s.orders;
   const long long n = blk / per_tile * s.rows + row;
   const int u = (int)(blk % per_tile);
@@ -1744,10 +1812,11 @@ __global__ void __launch_bounds__(256) k_pack(const PackSrc s, long long total, 
     const __half hi = __float2half_rn(w);
     h[e] = (j < 4) ? hi : __float2half_rn(w - __half2float(hi));
   }
-  *reinterpret_cast<uint4*>(out + blk * s.rows * 128 + sw128_off(row, j)) = *reinterpret_cast<const uint4*>(h);
+  const size_t at = s.hi_only ? blk * s.rows * 64 + sw64_off(row, j) : blk * s.rows * 128 + sw128_off(row, j);
+  *reinterpret_cast<uint4*>(out + at) = *reinterpret_cast<const uint4*>(h);
 }
 int launch_pack(const PackSrc& src, long long n_blocks, void* out, cudaStream_t s) {
-  const long long total = n_blocks * src.rows * 8;
+  const long long total = n_blocks * src.rows * (src.hi_only ? 4 : 8);
   k_pack<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(src, total, static_cast<unsigned char*>(out));
   P2M_LAUNCH_OK();
   return P2M_OK;
@@ -1771,10 +1840,10 @@ const TileBlobs& conv_tiles(int N, const DevLevel& g, const TileSet* tiles) {
 struct ConvCfg {
   int ns, xs;
 };
-ConvCfg conv_cfg(int NC, const TileBlobs& t, bool t1_given) {
+ConvCfg conv_cfg(int NC, const TileBlobs& t, bool t1_given, bool f16) {
   for (int ns = NC == WIDE_N ? 6 : 3; ns >= 3; ns -= 3)
     for (int xs = 2; xs >= 1; --xs)
-      if (conv_smem(NC, ns, xs, t1_given, t.max_h1, t.stride).bytes <= SMEM_LIMIT) return {ns, xs};
+      if (conv_smem(NC, ns, xs, t1_given, t.max_h1, t.stride, f16).bytes <= SMEM_LIMIT) return {ns, xs};
   return {0, 0};
 }
 // Output columns per CTA of a conv Fin -> Fout on tiles t.  The 64 x 256 mode builds each A block once for all 256
@@ -1782,8 +1851,8 @@ ConvCfg conv_cfg(int NC, const TileBlobs& t, bool t1_given) {
 // under the other warpgroup's: that pays where the main loop is long, the T1-given 256 -> 256 conv (24 K-blocks per
 // tile: 13-21 % faster layers), and not at 12 (128 -> 256: 8 % slower; H100 SXM, README).  It is taken there when its
 // ring of three slots fits; every other conv with Fout % 128 == 0 runs as 128-column slices.
-int conv_cols(int fin, int fout, const TileBlobs& t, bool t1_given) {
-  const bool pair = fout == PAIR_N && fin == PAIR_N && t1_given && conv_cfg(PAIR_N, t, true).ns > 0;
+int conv_cols(int fin, int fout, const TileBlobs& t, bool t1_given, bool f16) {
+  const bool pair = fout == PAIR_N && fin == PAIR_N && t1_given && conv_cfg(PAIR_N, t, true, f16).ns > 0;
   return pair ? PAIR_N : conv_n(fout);
 }
 
@@ -1815,22 +1884,25 @@ bool make_row_tmap(CUtensorMap* tm, const float* base, long long rows, int fin, 
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// The conv kernel with NC output columns per CTA: k_cheb_conv_umma (64) or k_cheb_conv_wide (128, 256)
-template <int NC, int NS, int XS, int MODE>
+// The conv kernel with NC output columns per CTA: k_cheb_conv_umma (64) or k_cheb_conv_wide (128, 256); F16: their
+// single-pass fp16 instantiations
+template <int NC, int NS, int XS, int MODE, bool F16 = false>
 constexpr auto conv_kernel() {
-  if constexpr (NC != CONV_N) return k_cheb_conv_wide<NC, NS, XS, MODE>;
+  if constexpr (F16 && NC != CONV_N) return k_cheb_conv_f16_wide<NC, NS, XS, MODE>;
+  else if constexpr (F16) return k_cheb_conv_f16_umma<NC, NS, XS, MODE>;
+  else if constexpr (NC != CONV_N) return k_cheb_conv_wide<NC, NS, XS, MODE>;
   else return k_cheb_conv_umma<NC, NS, XS, MODE>;
 }
 // A conv kernel's setmaxnreg split is balanced for a launch allocation of ConvRoles<N>::regs_launch registers per
 // thread (80 for k_cheb_conv_umma, 96 for k_cheb_conv_wide): a build that ends up with another count would leave the
 // epilogue's setmaxnreg.inc spinning on an empty pool.
-template <int NC, int NS, int XS, int MODE>
+template <int NC, int NS, int XS, int MODE, bool F16 = false>
 int check_launch_regs() {
   constexpr int N = NC == CONV_N ? CONV_N : WIDE_N;
   static int state = 0;  // per instantiation; racing first calls all compute the same value
   if (state == 0) {
     cudaFuncAttributes fa;
-    P2M_CUDA_OK(cudaFuncGetAttributes(&fa, conv_kernel<NC, NS, XS, MODE>()));
+    P2M_CUDA_OK(cudaFuncGetAttributes(&fa, conv_kernel<NC, NS, XS, MODE, F16>()));
     state = (fa.numRegs == ConvRoles<N>::regs_launch) ? 1 : -1;
   }
   if (state < 0) {
@@ -1842,18 +1914,19 @@ int check_launch_regs() {
   return P2M_OK;
 }
 
-// a.plain selects the instantiation: MODE 0 (plain GEMM) or MODE 1 (T1 given); NC output columns per CTA
-template <int NC, int NS, int XS>
+// a.plain selects the instantiation: MODE 0 (plain GEMM) or MODE 1 (T1 given); NC output columns per CTA; F16 the
+// single-pass fp16 precision (a.f16)
+template <int NC, int NS, int XS, bool F16>
 int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
   constexpr int N = NC == CONV_N ? CONV_N : WIDE_N;
   constexpr int TM = tile_rows<N>();
   const DevLevel& g = *a.g;
   const TileBlobs& t = conv_tiles(N, g, a.tiles);
-  const size_t smem = conv_smem(NC, NS, XS, !a.plain, t.max_h1, t.stride).bytes;
+  const size_t smem = conv_smem(NC, NS, XS, !a.plain, t.max_h1, t.stride, F16).bytes;
   constexpr int M0 = NC == PAIR_N ? 1 : 0;  // MODE of a plain launch (the 64 x 256 mode has none: conv_cols)
-  auto kern = a.plain ? conv_kernel<NC, NS, XS, M0>() : conv_kernel<NC, NS, XS, 1>();
+  auto kern = a.plain ? conv_kernel<NC, NS, XS, M0, F16>() : conv_kernel<NC, NS, XS, 1, F16>();
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  P2M_TRY((a.plain ? check_launch_regs<NC, NS, XS, M0>() : check_launch_regs<NC, NS, XS, 1>()));
+  P2M_TRY((a.plain ? check_launch_regs<NC, NS, XS, M0, F16>() : check_launch_regs<NC, NS, XS, 1, F16>()));
   KParams p;
   p.x = a.x;
   p.in_unpool = a.in_unpool;
@@ -1868,9 +1941,9 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   p.n_tiles = a.batch * p.P;
   p.wpack = static_cast<const unsigned char*>(a.wpack);
   p.apack = nullptr;
-  // the weight image holds K-blocks of fout rows x 128 bytes; column slice y starts y * NC rows into each block
-  p.wslice_bytes = (long long)NC * 128;
-  p.wblock_stride = (long long)a.fout * 128;
+  // the weight image holds K-blocks of fout rows x 128 (F16: 64) bytes; column slice y starts y * NC rows into each
+  p.wslice_bytes = (long long)NC * op_row_bytes(F16);
+  p.wblock_stride = (long long)a.fout * op_row_bytes(F16);
   p.zero_row = zero_row;
   p.ep = to_dev(a.ep);
   p.res_identity = (a.ep.res != nullptr && a.ep.res_F == a.fout) ? 1 : 0;
@@ -1910,26 +1983,27 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   return P2M_OK;
 }
 
+template <bool F16>
 int launch_n(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
   const int N = conv_n(a.fout);
   const TileBlobs& t = conv_tiles(N, *a.g, a.tiles);
-  const int NC = conv_cols(a.fin, a.fout, t, !a.plain);
-  const ConvCfg c = conv_cfg(NC, t, !a.plain);
+  const int NC = conv_cols(a.fin, a.fout, t, !a.plain, F16);
+  const ConvCfg c = conv_cfg(NC, t, !a.plain, F16);
   if (c.ns == 0) {
     set_error("umma_conv: tile family does not fit shared memory");
     return P2M_ERR_INVALID;
   }
   if (NC == PAIR_N)
-    return c.xs == 2 ? launch_cfg<PAIR_N, 3, 2>(a, status, zero_row, sm_count, s)
-                     : launch_cfg<PAIR_N, 3, 1>(a, status, zero_row, sm_count, s);
+    return c.xs == 2 ? launch_cfg<PAIR_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
+                     : launch_cfg<PAIR_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
   if (N == CONV_N)
-    return c.xs == 2 ? launch_cfg<CONV_N, 3, 2>(a, status, zero_row, sm_count, s)
-                     : launch_cfg<CONV_N, 3, 1>(a, status, zero_row, sm_count, s);
+    return c.xs == 2 ? launch_cfg<CONV_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
+                     : launch_cfg<CONV_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
   if (c.ns == 6)
-    return c.xs == 2 ? launch_cfg<WIDE_N, 6, 2>(a, status, zero_row, sm_count, s)
-                     : launch_cfg<WIDE_N, 6, 1>(a, status, zero_row, sm_count, s);
-  return c.xs == 2 ? launch_cfg<WIDE_N, 3, 2>(a, status, zero_row, sm_count, s)
-                   : launch_cfg<WIDE_N, 3, 1>(a, status, zero_row, sm_count, s);
+    return c.xs == 2 ? launch_cfg<WIDE_N, 6, 2, F16>(a, status, zero_row, sm_count, s)
+                     : launch_cfg<WIDE_N, 6, 1, F16>(a, status, zero_row, sm_count, s);
+  return c.xs == 2 ? launch_cfg<WIDE_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
+                   : launch_cfg<WIDE_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
 }
 
 }  // namespace
@@ -1946,6 +2020,9 @@ namespace {
 // iff both rows of the pair have the SAME half class.  Re-deal a length-sorted order accordingly: [c0 c0 c1 c1] per
 // group, taken in sorted order (a group's rows still have similar lengths).  Pure re-ordering of which thread
 // produces which row: results are unchanged.
+// (The single-pass fp16 precision stores one 64-byte row per tile row, in the bank half of its parity: there a pair
+// of equal parity costs one replay.  Dealing by parity as well cost the fp16x3 schedules about 0.6 % on an H100, so
+// this order, which both precisions share, stays the fp16x3 one.)
 void balance_store_halves(std::vector<unsigned short>* ord) {
   std::vector<unsigned short> q0, q1;
   for (unsigned short r : *ord) ((r & 4) ? q1 : q0).push_back(r);
@@ -2222,11 +2299,11 @@ bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
 int umma_conv_x_stages(const DevLevel& g, int fin, int fout, bool plain) {
   return umma_conv_tiling(g, fin, fout, plain).xs;
 }
-UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain) {
+UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain, bool f16) {
   const int N = conv_n(fout);
   const TileBlobs& t = conv_tiles(N, g, nullptr);
-  const int NC = conv_cols(fin, fout, t, !plain);
-  const ConvCfg c = conv_cfg(NC, t, !plain);
+  const int NC = conv_cols(fin, fout, t, !plain, f16);
+  const ConvCfg c = conv_cfg(NC, t, !plain, f16);
   return {NC, c.ns, c.xs};
 }
 bool umma_tma_rows(const DevLevel& g) { return g.V % TILE_M == 0 && tmap_encoder() != nullptr; }
@@ -2311,9 +2388,10 @@ int launch_umma_gemm(GemmOperand X, GemmOperand W, int M, int N, int K, const Ep
 size_t umma_wpack_bytes(int fin, int fout) { return (size_t)(fin / FC) * 3 * fout * 128; }
 
 int launch_umma_pack_weights(const float* W, int fin, int fout, bool transposed, int order, float c, void* wpack,
-                             cudaStream_t s) {
+                             cudaStream_t s, bool f16) {
   const int rows = transposed ? fin : fout, K = transposed ? fout : fin;
   PackSrc src{W, transposed ? 3 : 3LL * fin, transposed ? 3LL * fin : 3, rows, K / FC, 1, rows, W_SCALE, 0, c};
+  src.hi_only = f16 ? 1 : 0;
   if (order == WPACK_ALL) src.orders = 3;
   else if (order == WPACK_COMBINED) src.combined = 1;
   else src.p = W + order;
@@ -2338,7 +2416,11 @@ int launch_umma_conv(const UmmaConvArgs& a, int* status, const float* zero_row, 
     set_error("umma_conv: index-list tiles need at most 256 staged rows");
     return P2M_ERR_INVALID;
   }
-  return launch_n(a, status, zero_row, sm_count, s);
+  if (a.f16 && a.plain && a.a_scale != nullptr) {
+    set_error("umma_conv: the single-pass fp16 plain GEMM has no operand scale (inference only)");
+    return P2M_ERR_INVALID;
+  }
+  return a.f16 ? launch_n<true>(a, status, zero_row, sm_count, s) : launch_n<false>(a, status, zero_row, sm_count, s);
 }
 
 }  // namespace p2m

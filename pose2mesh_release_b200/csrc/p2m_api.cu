@@ -298,6 +298,17 @@ BwdMap map_scratch(const p2m_model* m, int B, void* base) {
 }
 
 // ---- which kernels run a Chebyshev conv
+// The precisions whose convs run on the tensor cores: fp16x3, and the single-pass fp16 (eval forward only)
+inline bool tc_precision(int precision) { return precision == P2M_PREC_FP16X3_TC || precision == P2M_PREC_FP16_TC; }
+// P2M_PREC_FP16_TC is an inference precision: the entry points that train or differentiate refuse it before any device
+// work (so a refused training forward leaves the running statistics as they were)
+int refuse_fp16(const p2m_model* m, const char* where) {
+  if (m->precision != P2M_PREC_FP16_TC) return P2M_OK;
+  set_error(std::string(where) + ": precision fp16 (P2M_PREC_FP16_TC) is an inference precision; the training schedule "
+            "and the backward need fp16x3 or fp32");
+  return P2M_ERR_INVALID;
+}
+
 // Padding-vertex elision of a conv with `width` output columns over `rows` rows under p2m_debug_set_elide_padding's
 // `mode`: connected rows through the conv on index-list tiles, isolated rows (DevLevel::n_iso) through a plain GEMM with
 // the combined weights.  Mode 1 (default) takes the levels where they are >= 40 % of the rows (measured break-even),
@@ -325,7 +336,7 @@ ConvRoute conv_route(const p2m_model* m, int level, int fin, int fout, int batch
                      bool need_dx = true) {
   const DevLevel& g = m->levels[level];
   const long long rows = (long long)batch * g.V;
-  const bool tc = m->precision == P2M_PREC_FP16X3_TC;
+  const bool tc = tc_precision(m->precision);
   const size_t cap = wpack_capacity(network, fin, fout);
   ConvRoute r;
   r.tc = tc && umma_conv_supported(g, fin, fout);
@@ -377,14 +388,16 @@ int run_tc_conv(p2m_model* m, UmmaConvArgs a, const float* W, bool transposed, b
     const char* tn = getenv("P2M_TRACE_NTH");
     if (a.trace != nullptr && tn && m->trace_seen++ != atoi(tn)) a.trace = nullptr;
   }
-  P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_ALL, 0.f, wpack, s));
+  // single-pass fp16: forward convs only (refuse_fp16 keeps the backward-data conv away from it)
+  a.f16 = (m->precision == P2M_PREC_FP16_TC && !transposed) ? 1 : 0;
+  P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_ALL, 0.f, wpack, s, a.f16 != 0));
   if (!t1_given) P2M_TRY(launch_cheb_t1(g, a.x, a.in_unpool, a.batch, a.fin, T, s, elide ? &g.real_tiles : nullptr));
   a.t1 = T;
   a.wpack = wpack;
   if (elide) a.tiles = &g.real_tiles;
   P2M_TRY(launch_umma_conv(a, m->kernel_status, m->zero_row, m->sm_count, s));
   if (!elide || iso_mode == 2) return P2M_OK;
-  P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_COMBINED, g.iso_diag, w_iso, s));
+  P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_COMBINED, g.iso_diag, w_iso, s, a.f16 != 0));
   a.t1 = nullptr;
   a.plain = 1;
   a.trace = nullptr;  // the trace buffer holds the connected rows' launch; the isolated rows' GEMM would overwrite it
@@ -471,11 +484,12 @@ int tc_dw(p2m_model* m, const DevLevel& g, int batch, const float* x, int in_unp
                                       m->sm_count, s);
 }
 
-// fc: joints -> coarsest mesh level (meshnet.py:104-106), as a dense GEMM on the tensor cores (wgmma, fp16x3) or SIMT
+// fc: joints -> coarsest mesh level (meshnet.py:104-106), as a dense GEMM on the tensor cores (wgmma, fp16x3: also at
+// the single-pass fp16 precision, which only changes the Chebyshev convs) or SIMT
 int run_fc(const p2m_model* m, const p2m_params_t* P, const WsCommon& w, int B, const float* x, float* out, cudaStream_t s) {
   Epilogue ep;
   ep.bias = P->fc_b;
-  if (m->precision == P2M_PREC_FP16X3_TC && w.fc_apack != nullptr)
+  if (tc_precision(m->precision) && w.fc_apack != nullptr)
     return launch_umma_gemm({x, m->fc_in, 1}, {P->fc_w, m->fc_in, 1}, B, m->fc_out, m->fc_in, ep, out, w.fc_apack,
                             w.fc_wpack, m->kernel_status, m->sm_count, s);
   return launch_gemm(x, m->fc_in, P->fc_w, m->fc_in, 0, out, m->fc_out, B, m->fc_out, m->fc_in, ep, s);
@@ -890,8 +904,9 @@ int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, in
     return P2M_ERR_INVALID;
   }
   const DevLevel& g = m->levels[level];
-  const UmmaConvTiling t = conv_route(m, level, fin, fout, 1, false).tc ? umma_conv_tiling(g, fin, fout, false)
-                                                                        : UmmaConvTiling{0, 0, 0};
+  const UmmaConvTiling t = conv_route(m, level, fin, fout, 1, false).tc
+                               ? umma_conv_tiling(g, fin, fout, false, m->precision == P2M_PREC_FP16_TC)
+                               : UmmaConvTiling{0, 0, 0};
   out[0] = t.cols;
   out[1] = t.ns;
   out[2] = t.xs;
@@ -982,7 +997,7 @@ int p2m_model_layer_times_ms(p2m_model_t* m, float* out, int n) {
 }
 
 int p2m_model_set_precision(p2m_model_t* m, int precision) {
-  if (!m || (precision != P2M_PREC_FP32_SIMT && precision != P2M_PREC_FP16X3_TC)) {
+  if (!m || (precision != P2M_PREC_FP32_SIMT && precision != P2M_PREC_FP16X3_TC && precision != P2M_PREC_FP16_TC)) {
     set_error("set_precision: bad argument");
     return P2M_ERR_INVALID;
   }
@@ -1168,6 +1183,7 @@ static int meshnet_forward(p2m_model_t* m, const p2m_params_t* P, const p2m_bn_o
     set_error("meshnet_forward_vertices: every BatchNorm must use running statistics");
     return P2M_ERR_INVALID;
   }
+  if (!eval) P2M_TRY(refuse_fp16(m, "meshnet_forward (training schedule)"));
   P2M_TRY(check_params(m, P, &bn));
   P2M_TRY(check_kernel_status(m, "meshnet_forward"));
   DeviceGuard guard(m->device);
@@ -1274,6 +1290,7 @@ int p2m_meshnet_backward_opts(p2m_model_t* m, const p2m_params_t* P, const p2m_p
     set_error("meshnet_backward: bad argument");
     return P2M_ERR_INVALID;
   }
+  P2M_TRY(refuse_fp16(m, "meshnet_backward"));
   P2M_TRY(check_params(m, P, nullptr));
   P2M_TRY(check_params(m, G, nullptr));
   const std::vector<p2m_bn_opts_t> bn = resolve_bn_opts(m, 1, bn_opts);
@@ -1494,6 +1511,7 @@ int p2m_cheb_conv_fwd(p2m_model_t* m, const p2m_conv_fwd_args_t* a, void* worksp
     set_error("cheb_conv_fwd: bad argument");
     return P2M_ERR_INVALID;
   }
+  if (a->bn_mode == 2) P2M_TRY(refuse_fp16(m, "cheb_conv_fwd (batch-statistics BatchNorm)"));
   if (workspace_bytes < p2m_cheb_conv_workspace_bytes(m, a->level, a->batch, a->fin, a->fout)) {
     set_error("cheb_conv_fwd: workspace too small");
     return P2M_ERR_WORKSPACE;
@@ -1560,6 +1578,7 @@ int p2m_cheb_conv_bwd(p2m_model_t* m, const p2m_conv_bwd_args_t* a, void* worksp
     set_error("cheb_conv_bwd: bad argument");
     return P2M_ERR_INVALID;
   }
+  P2M_TRY(refuse_fp16(m, "cheb_conv_bwd"));
   if (workspace_bytes < p2m_cheb_conv_workspace_bytes(m, a->level, a->batch, a->fin, a->fout)) {
     set_error("cheb_conv_bwd: workspace too small");
     return P2M_ERR_WORKSPACE;

@@ -455,6 +455,9 @@ struct UmmaConvArgs {
   // optional: run on this tile family instead of the level's consecutive tiles
   const TileSet* tiles = nullptr;
   long long* trace = nullptr;       // debug (P2M_UMMA_TRACE builds only): [8][512] event log of CTA 0
+  // single-pass fp16 (P2M_PREC_FP16_TC): wpack is a hi-only image (launch_umma_pack_weights with f16), one k16 MMA per
+  // 16 features; T1-given convs and plain GEMMs without a_scale only (the eval forward)
+  int f16 = 0;
 };
 // Host: build the per-tile halo metadata of one level (uploads; device pointers appended to `owned`).  A level whose
 // tiles stage more than 512 rows or more than 65535 local-CSR entries gets none (meta128 stays empty: it runs on SIMT).
@@ -469,7 +472,7 @@ int umma_conv_x_stages(const DevLevel& g, int fin, int fout, bool plain);
 struct UmmaConvTiling {
   int cols, ns, xs;  // output columns per CTA (64, 128 or 256), A/B ring slots, X / T1 stages (0: does not fit)
 };
-UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain);
+UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain, bool f16 = false);
 int umma_dw_x_stages(const DevLevel& g);
 bool umma_tma_rows(const DevLevel& g);
 // Weight images of a conv: fp16 [hi | lo] K-blocks of 32 k (x 2^6) from W [fout, fin*3] in the reference layout (column
@@ -478,11 +481,13 @@ bool umma_tma_rows(const DevLevel& g);
 //   WPACK_ALL       blocks u = chunk*3 + k of all three orders, umma_wpack_bytes(K, rows) bytes (the conv);
 //   WPACK_COMBINED  the isolated rows' combined weights W0 + c W1 + (2c^2 - 1) W2 (padding-vertex elision), and
 //   0, 1, 2         W_k alone (the backward's dT = dz W_k): plain images of umma_plain_pack_bytes(rows, K) bytes.
+// f16: the single-pass fp16 image (P2M_PREC_FP16_TC) of the same blocks, the round-to-nearest fp16 of W x 2^6 only (half
+// the bytes; the sizes below are those of the fp16x3 image and bound both).
 constexpr int WPACK_ALL = -1, WPACK_COMBINED = -2;
 size_t umma_wpack_bytes(int fin, int fout);
 size_t umma_plain_pack_bytes(int N, int K);
 int launch_umma_pack_weights(const float* W, int fin, int fout, bool transposed, int order, float c, void* wpack,
-                             cudaStream_t s);
+                             cudaStream_t s, bool f16 = false);
 // scale_out[0] = 2^e with max|x| * 2^e in [2^(9-h), 2^(10-h)), h = headroom_log2  (1 if x is all zero or not
 // finite); scratch-free, two tiny launches
 int launch_absmax_scale(const float* x, long long n, float* scale_out, cudaStream_t s, int headroom_log2 = 0);

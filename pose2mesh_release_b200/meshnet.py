@@ -316,9 +316,9 @@ class Pose2Mesh(nn.Module):
 
     # -- knobs ---------------------------------------------------------------------------------
     def set_precision(self, precision: str):
-        """'fp32' (CUDA-core FFMA) or 'fp16x3' (wgmma tensor cores, error-compensated split)."""
-        table = {"fp32": _lib.P2M_PREC_FP32_SIMT, "fp16x3": _lib.P2M_PREC_FP16X3_TC}
-        self._hier.set_precision(table[precision])
+        """'fp32' (CUDA-core FFMA), 'fp16x3' (wgmma tensor cores, error-compensated split) or 'fp16' (single-pass
+        wgmma with fp16 operands, inference only: a train-mode forward or a backward raises RuntimeError)."""
+        self._hier.set_precision(_lib.PRECISIONS[precision])
         return self
 
     @property

@@ -1,0 +1,58 @@
+"""CPU-only checks of the build of the single-pass fp16 conv kernels (csrc/cheb_umma.cu: k_cheb_conv_f16_umma and
+k_cheb_conv_f16_wide, cheb_conv_body with F16 = true): each launches with the register count its setmaxnreg split
+assumes, and its main loop issues two k16 wgmma per K-block (per 64-row half in the 128 x 64 configuration) where the
+fp16x3 instantiations issue six."""
+import re
+import shutil
+import subprocess
+import os
+
+import pytest
+
+
+def _cuobjdump():
+    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(tool):
+        pytest.skip("cuobjdump not available")
+    return tool
+
+
+def _kernels(tool, lib, name):
+    """{mangled name: launch registers} of every instantiation of kernel `name` in the library."""
+    out = subprocess.run([tool, "-res-usage", lib], capture_output=True, text=True).stdout
+    found = re.findall(r"Function (\S*" + name + r"I\S*?):?\n[^\n]*REG:(\d+)", out)
+    return {n: int(regs) for n, regs in found}
+
+
+def _hgmma(tool, lib, fn):
+    sass = subprocess.run([tool, "-sass", "-fun", fn, lib], capture_output=True, text=True).stdout
+    return re.findall(r"HGMMA\.(\d+x\d+x\d+)", sass)
+
+
+def test_f16_wide_conv_launches_with_96_registers_and_issues_two_m64n128():
+    """64 x 128 and 64 x 256: the instantiations the eval forward launches (ring of 6 or 3 slots x 1 or 2 T1 stages,
+    T1 given or plain; the 64 x 256 mode T1 given only), at the 96 registers of the 640-thread split."""
+    from pose2mesh_release_b200 import build
+
+    tool = _cuobjdump()
+    lib = build.build()
+    kernels = _kernels(tool, lib, "k_cheb_conv_f16_wide")
+    assert len([k for k in kernels if "ILi128E" in k]) == 8, sorted(kernels)
+    assert len([k for k in kernels if "ILi256E" in k]) == 2, sorted(kernels)
+    assert set(kernels.values()) == {96}, kernels
+    for name in kernels:
+        hgmma = _hgmma(tool, lib, name)
+        assert hgmma.count("64x128x16") == 2 and set(hgmma) == {"64x128x16"}, (name, hgmma)
+
+
+def test_f16_conv_umma_launches_with_80_registers_and_issues_two_k16_per_half():
+    from pose2mesh_release_b200 import build
+
+    tool = _cuobjdump()
+    lib = build.build()
+    kernels = _kernels(tool, lib, "k_cheb_conv_f16_umma")
+    assert len(kernels) == 4, sorted(kernels)
+    assert set(kernels.values()) == {80}, kernels
+    for name in kernels:
+        hgmma = _hgmma(tool, lib, name)
+        assert hgmma.count("64x64x16") == 4 and set(hgmma) == {"64x64x16"}, (name, hgmma)

@@ -1,0 +1,361 @@
+"""The single-pass fp16 precision (P2M_PREC_FP16_TC, inference only) on the device.
+
+1. Single layer (p2m_cheb_conv_fwd) against float64: every width of the three kernel configurations (128 x 64,
+   64 x 128, 64 x 256), the graph families of tests/graphs.py, the persistent CTA loop.  Every element lies within
+   fp16_ref's bound (SPLIT16 = 2^-10 + 2^-22), and at least one element of each case lies beyond
+   the fp16x3 bound: the single pass is what ran.
+2. The eval network layer by layer (p2m_debug_set_capture), each layer from its own captured input: elision 0 / 1 / 2
+   (index-list tiles and the isolated rows' combined-weight GEMM), the virtual unpool, residuals, the fused head.
+3. Full size (SMPL hierarchy, B = 256): finite, two runs, forward_vertices and CUDA-graph replay equal to the plain
+   forward bit for bit, batch split and elision / dedup within a tolerance derived from SPLIT16, the per-mesh deviation
+   from the float64 oracle on test_gpu_parity's 32-mesh sample (written to P2M_FP16_REPORT if set).
+4. Refusal: training forwards and backwards raise and leave the BatchNorm running statistics untouched; back at fp16x3
+   the results are bitwise those of a model that never left it.
+Every test ends with kernel_status == 0."""
+import ctypes as C
+import json
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import fp16_ref as R16
+import fp64_ref as R
+import graphs as G
+from helpers import CASES, graph_from_fixture
+
+pytestmark = pytest.mark.gpu
+
+
+def dev():
+    return torch.device("cuda:0")
+
+
+def level(name):
+    fx, i = {"tma": ("smpl_small", 1), "ragged": ("mano_like", 0)}[name]
+    return graph_from_fixture(fx)[0][i]
+
+
+def make_layer(V, B, fin, fout, seed):
+    rng = np.random.default_rng(seed)
+    x = rng.standard_normal((B, V, fin)).astype(np.float32)
+    W = ((rng.random((fout, 3 * fin)) * 2 - 1) * np.sqrt(2.0 / (3 * fin + fout))).astype(np.float32)
+    b = (rng.standard_normal(fout) * 0.1).astype(np.float32)
+    return x, W, b
+
+
+def conv_info(gh, fin, fout):
+    from pose2mesh_release_b200 import _lib
+
+    lib = _lib.load()
+    path, til = (C.c_int32 * 9)(), (C.c_int32 * 3)()
+    _lib.check(lib.p2m_debug_conv_path(gh.handle(0), 0, fin, fout, path), "conv_path")
+    _lib.check(lib.p2m_debug_conv_tiling(gh.handle(0), 0, fin, fout, til), "conv_tiling")
+    return int(path[0]), tuple(til)
+
+
+def run_layer(L, x, W, b):
+    """p2m_cheb_conv_fwd at fp16: (y as float64, on tensor cores, (cols, ns, xs))."""
+    from pose2mesh_release_b200 import cheby_graph_conv as cgc
+
+    cgc.set_default_precision("fp16")
+    try:
+        gh = cgc.graph_handle(L)
+        with torch.no_grad():
+            y = cgc.ChebConvLinear.apply(torch.as_tensor(x).to(dev()), torch.as_tensor(W).to(dev()),
+                                         torch.as_tensor(b).to(dev()), gh)
+        torch.cuda.synchronize()
+        assert gh.kernel_status(0) == 0, "a tensor-core kernel timed out on an mbarrier"
+        tc, til = conv_info(gh, x.shape[2], W.shape[0])
+    finally:
+        cgc.set_default_precision("fp16x3")
+    return y.double().cpu().numpy(), tc, til
+
+
+def check_single_pass(tag, L, x, W, b, y, on_tc=True):
+    L = L.tocsr().astype(np.float32).astype(np.float64)
+    ref = R.cheb_conv_fwd(x, L, W, b)
+    err = np.abs(y - ref)
+    r16 = float((err / R16.cheb_conv_fwd_bound16(x, L, W, b)).max())
+    assert r16 <= 1.0, f"{tag}: max |err| / fp16 bound = {r16:.3g}"
+    if on_tc:
+        r3 = float((err / R.cheb_conv_fwd_bound(x, L, W, b, "fp16x3")).max())
+        assert r3 > 1.0, f"{tag}: within the fp16x3 bound ({r3:.3g}): the single pass did not run"
+
+
+# ------------------------------------------------------------------------------------------------------ 1. one layer
+WIDTHS = [(fin, fout) for fin in (32, 64, 96, 128, 160, 192, 224, 256) for fout in (64, 128, 256)]
+
+
+@pytest.mark.parametrize("lvl", ["tma", "ragged"])
+@pytest.mark.parametrize("fin,fout", WIDTHS, ids=lambda v: str(v))
+def test_single_layer_width_grid(fin, fout, lvl):
+    L = level(lvl)
+    x, W, b = make_layer(L.shape[0], 1, fin, fout, seed=fin * 1000 + fout)
+    y, tc, til = run_layer(L, x, W, b)
+    assert tc == 1
+    assert til[0] == (256 if fin == fout == 256 else (64 if fout == 64 else 128)), til
+    check_single_pass(f"width {fin}->{fout} {lvl}", L, x, W, b, y)
+
+
+SYMMETRIC_FAMILIES = ["V1", "V64", "V127", "V128", "V129", "V1088", "V2048", "band8", "band12", "band14", "band16",
+                      "band20", "h1_256", "h1_257", "far", "hub", "empty_rows", "iso_uniform", "iso_two_diag", "dense"]
+
+
+@pytest.mark.parametrize("fin,fout", [(64, 64), (128, 128), (256, 256)], ids=lambda v: str(v))
+@pytest.mark.parametrize("name", SYMMETRIC_FAMILIES)
+def test_single_layer_graph_family(name, fin, fout):
+    L = G.get(name)
+    x, W, b = make_layer(L.shape[0], 2, fin, fout, seed=L.shape[0] + fin)
+    y, tc, _ = run_layer(L, x, W, b)
+    check_single_pass(f"{name} {fin}->{fout}", L, x, W, b, y, on_tc=bool(tc))
+
+
+@pytest.mark.parametrize("fin,fout", [(64, 64), (128, 128), (256, 256)], ids=lambda v: str(v))
+def test_single_layer_persistent_cta_loop(fin, fout):
+    """V = 128: n_tiles = B (128 x 64) or 2 B (64-row tiles); B around the grid makes CTAs run 0, 1, 2 or more tiles."""
+    L = G.get("V128")
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    grid = sms // max(1, fout // (64 if fout == 64 else 128))
+    for B in (1, grid - 1, grid + 1, 3 * grid + 5):
+        x, W, b = make_layer(128, B, fin, fout, seed=B)
+        y, tc, _ = run_layer(L, x, W, b)
+        assert tc == 1
+        check_single_pass(f"persistent B={B} {fin}->{fout}", L, x, W, b, y)
+
+
+# ------------------------------------------------------------------------------------------- 2. network, layer by layer
+def fp16_net(name, seed):
+    import test_gpu_network_fp64 as N
+    from pose2mesh_release_b200 import _lib
+
+    net = N.Net(name, "fp16x3", seed=seed, open_relus=False)
+    net.precision = "fp16"
+    net.hier.set_precision(_lib.P2M_PREC_FP16_TC)
+    return net
+
+
+def eval_layer16(net, li, inp, block_in, on_tc):
+    """test_gpu_network_fp64.eval_layer with the conv bound at fp16 (network split) on the tensor cores."""
+    import test_gpu_network_fp64 as N
+
+    L = net.layers[li]
+    W, b = net.p[f"cl.{li}.weight"], net.p[f"cl.{li}.bias"]
+    Lm = net.L32[L["level"]]
+    z64 = R.cheb_conv_fwd(inp, Lm, W, b)
+    E = R16.cheb_conv_fwd_bound16(inp, Lm, W, b, "network") if on_tc else \
+        R.cheb_conv_fwd_bound(inp, Lm, W, b, "fp32", split="network")
+    if not L["bn"]:
+        return z64, E
+    g, be = net.p[f"bn.{li}.weight"], net.p[f"bn.{li}.bias"]
+    rm, rv = net.p[f"bn.{li}.running_mean"], net.p[f"bn.{li}.running_var"]
+    y64 = R.bn_eval_fwd(z64, g, be, rm, rv, relu=True)
+    bound = R.bn_eval_fwd_bound(z64, E, g, be, rm, rv, b)
+    res, eres = N.residual(net, li, block_in)
+    return y64 + res, bound + eres + R.U32 * np.abs(y64 + res)
+
+
+EVAL_CASES = [(name, elide, B) for name in ("smpl_small", "mano_like", "custom") for elide, B in ((0, 3), (1, 1), (2, 3))]
+
+
+@pytest.mark.parametrize("name,elide,B", EVAL_CASES, ids=lambda v: str(v))
+def test_eval_network_layer_by_layer(name, elide, B):
+    import test_gpu_network_fp64 as N
+
+    net = fp16_net(name, seed=31 + B + elide)
+    x, _ = N.train_inputs(net, B, seed=5 + elide)
+    y, cap = N.forward_eval(net, x, elide, dedup=False, fuse=False)
+    n = net.n_layers
+    act = {li: cap["y"][li].reshape(B, net.V(li), -1) for li in range(n)}
+    fc_out = cap["fc_out"]
+    tag = f"{name} fp16 eval elide={elide} B={B}"
+    assert np.array_equal(act[n - 1], y.reshape(act[n - 1].shape)), tag
+    beyond = 0
+    for li in range(n):
+        inp, block_in = N.layer_input(net, li, x, fc_out, act)
+        on_tc = net.route(li, B)["tc"]
+        ref, bound = eval_layer16(net, li, inp, block_in, on_tc)
+        err = np.abs(act[li] - ref)
+        r = float((err / bound).max())
+        assert r <= 1.0, f"{tag} layer {li}: max |err| / bound = {r:.3g}"
+        if on_tc:
+            net.precision = "fp16x3"   # (eval_layer's bound at fp16x3)
+            _, b3 = N.eval_layer(net, li, inp, block_in, True)
+            net.precision = "fp16"
+            beyond += int((err > b3).any())
+        if li == net.blocks[0]["first"] + net.blocks[0]["n"] - 1:   # the fc stays an fp16x3 dense GEMM
+            ref_fc, b_fc = N.fc_ref(act[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], "fp16x3")
+            assert float((np.abs(fc_out - ref_fc) / b_fc).max()) <= 1.0, f"{tag} fc_out"
+    assert beyond >= 1, f"{tag}: no tensor-core layer beyond the fp16x3 bound"
+    # the fused head from the fused layer's captured input
+    yf, capf = N.forward_eval(net, x, elide, dedup=False, fuse=True)
+    fused = [li for li in range(n) if net.route(li, B)["fuse_head"]]
+    if B * net.V(n - 2) >= 64:
+        assert fused == [n - 2], (tag, fused)
+    if fused:
+        li = fused[0]
+        act_f = {k: capf["y"][k].reshape(B, net.V(k), -1) for k in range(n) if k != li}
+        inp, block_in = N.layer_input(net, li, x, capf["fc_out"], act_f)
+        y1, e1 = eval_layer16(net, li, inp, block_in, True)
+        Lh = net.L32[net.layers[n - 1]["level"]]
+        Wh, bh = net.p[f"cl.{n - 1}.weight"], net.p[f"cl.{n - 1}.bias"]
+        ref = R.cheb_conv_fwd(y1, Lh, Wh, bh)
+        bound = R.cheb_conv_fwd_bound(y1, Lh, Wh, bh, "fp32") + R.thin_head_fused_bound(y1, e1, Lh, Wh)
+        r = float((np.abs(yf.reshape(ref.shape) - ref) / bound).max())
+        assert r <= 1.0, f"{tag} fused head: max |err| / bound = {r:.3g}"
+    # dedup on against off: the representative rows are computed by the same GEMM, bit for bit
+    for fuse in (False, True):
+        yd, _ = N.forward_eval(net, x, elide, dedup=True, fuse=fuse, capture=False)
+        assert np.array_equal(yd, y if not fuse else yf), (tag, "dedup", fuse)
+    assert net.hier.kernel_status(0) == 0
+
+
+# ------------------------------------------------------------------------------------------------- 3. full size
+def smpl_model(precision):
+    from oracle import meshnet_oracle as mo
+    from pose2mesh_release_b200 import graph as pg
+    from pose2mesh_release_b200.meshnet import Pose2Mesh
+
+    n, seed, levels, _ = CASES["smpl_like"]
+    face = pg.synthetic_sphere_faces(n, seed)
+    _, graph_L, _, perm_rev = pg.build_coarse_graphs(face, 17, pg.H36M_SKELETON, pg.H36M_FLIP_PAIRS, levels=levels)
+    torch.manual_seed(123)
+    model = Pose2Mesh(5, 3, graph_L, joint_set="human36")
+    sd = mo.randomize_bn_({k: v.detach().clone() for k, v in model.state_dict().items()}, seed=7)
+    model.load_state_dict(sd)
+    return model.to(dev()).set_precision(precision).eval(), sd, graph_L, perm_rev, n
+
+
+def per_mesh(y, ref):
+    y, ref = y.detach().double().cpu(), ref.detach().double().cpu()
+    d = (y - ref).abs().flatten(1).max(dim=1).values
+    s = ref.abs().flatten(1).max(dim=1).values.clamp_min(1e-30)
+    return d / s
+
+
+# Two fp16 forwards of one mesh that round differently: elision and dedup change how the isolated rows' weights are
+# rounded (the combined W0 + c W1 + (2c^2 - 1) W2 once, not each order), and a batch split changes the fc's operand
+# scale (found over the whole batch: its outputs may differ in the last bits, which the next conv's fp16 rounding can
+# turn into one fp16 step).  Per layer the two differ by at most the two forwards' rounding, 2 SPLIT16 relative,
+# compounded through the 21 layers of the SMPL plan at O(1) gain per layer: 21 * 2 * SPLIT16 = 4.1e-2 per mesh of
+# max|y| is the ceiling.  (fp16x3 holds a batch split to 1e-6: its split keeps those last bits.)
+ROUNDING_TOL = 21 * 2 * R16.SPLIT16
+PARITY_CEILING = 5e-2   # a chosen limit against layout or indexing bugs, not a derived bound
+PICK = sorted({0, 1, 2, 3, 36, 37, 73, 74, 110, 111, 127, 128, 131, 147, 148, 149, 184, 185, 221, 222, 254, 255}
+              | set(range(9, 256, 25)) | {200})
+
+
+def test_full_size_smpl_b256():
+    from oracle import meshnet_oracle as mo
+
+    model, sd, graph_L, perm_rev, n = smpl_model("fp16")
+    hier, d = model._hier, torch.cuda.current_device()
+    B = 256
+    x = torch.randn(B, 17, 5, generator=torch.Generator().manual_seed(0)).to(dev())
+    with torch.no_grad():
+        y = model(x)
+        y2 = model(x)
+        y_split = torch.cat([model(x[:100]), model(x[100:])])
+        verts = model.forward_vertices(x, perm_rev, n)
+    assert y.shape == (B, 12288, 3) and torch.isfinite(y).all()
+    assert torch.equal(y, y2), "two runs differ"
+    assert float(per_mesh(y_split, y).max()) < ROUNDING_TOL
+    real = torch.as_tensor(np.asarray(perm_rev[:n])).to(dev())
+    assert torch.equal(verts, y[:, real])
+    # CUDA-graph replay equals eager
+    xs = x.clone()
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        model(xs)
+    torch.cuda.current_stream().wait_stream(s)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g), torch.no_grad():
+        yg = model(xs)
+    g.replay()
+    torch.cuda.synchronize()
+    assert torch.equal(yg, y), "CUDA-graph replay differs from the eager forward"
+    # elision 0 / 2 and dedup off against the default
+    try:
+        for mode, dedup in ((0, True), (2, True), (1, False)):
+            hier.set_debug(d, elide_padding=mode, dedup_padding=dedup)
+            with torch.no_grad():
+                ym = model(x)
+            assert float(per_mesh(ym, y).max()) < ROUNDING_TOL, (mode, dedup)
+    finally:
+        hier.set_debug(d, elide_padding=1, dedup_padding=True)
+    # per-mesh deviation from the float64 oracle on test_gpu_parity's sample
+    laps = [t.to(torch.float64) for t in mo.laplacians_to_torch(graph_L)]
+    sd64 = {k: (v.double() if v.is_floating_point() else v) for k, v in sd.items()}
+    with torch.no_grad():
+        yo = mo.forward(sd64, laps, x[PICK].cpu().double(), training=False)
+    dev_mesh = per_mesh(y[PICK], yo)
+    with torch.no_grad():
+        y3 = smpl_model("fp16x3")[0](x)
+    dev_x3 = per_mesh(y, y3)
+    out = os.environ.get("P2M_FP16_REPORT")
+    if out:
+        with open(out, "w") as f:
+            json.dump({"per_mesh_vs_fp64_oracle": {"max": float(dev_mesh.max()), "median": float(dev_mesh.median()),
+                                                   "all": [float(v) for v in dev_mesh]},
+                       "per_mesh_vs_fp16x3": {"max": float(dev_x3.max()), "median": float(dev_x3.median())},
+                       "meshes": PICK}, f, indent=1)
+    assert float(dev_mesh.max()) < PARITY_CEILING, float(dev_mesh.max())
+    assert float(dev_x3.max()) > 1e-5, "fp16 and fp16x3 agree to fp16x3 accuracy: the single pass did not run"
+    assert hier.kernel_status(d) == 0
+
+
+# --------------------------------------------------------------------------------------------------- 4. refusal
+def test_training_and_backward_refused():
+    from pose2mesh_release_b200 import cheby_graph_conv as cgc
+    from pose2mesh_release_b200.meshnet import Pose2Mesh
+
+    mats, _ = graph_from_fixture("smpl_small")
+    torch.manual_seed(5)
+    ref = Pose2Mesh(5, 3, mats, joint_set="human36").to(dev()).set_precision("fp16x3")
+    torch.manual_seed(5)
+    model = Pose2Mesh(5, 3, mats, joint_set="human36").to(dev()).set_precision("fp16")
+    x = torch.randn(4, 17, 5, generator=torch.Generator().manual_seed(1)).to(dev())
+    before = {k: v.clone() for k, v in model.state_dict().items()}
+    buffers = dict(model.named_buffers())
+    # module: a train-mode forward
+    model.train()
+    with pytest.raises(RuntimeError, match="fp16"):
+        model(x)
+    # module: a backward (of a train-mode forward taken at fp16x3, called after switching to fp16)
+    model.set_precision("fp16x3")
+    y = model(x)
+    with torch.no_grad():                       # that forward did update the running statistics: restore them
+        for k, v in buffers.items():
+            v.copy_(before[k])
+    model.set_precision("fp16")
+    with pytest.raises(RuntimeError, match="fp16"):
+        y.sum().backward()
+    for k, v in model.state_dict().items():
+        assert torch.equal(v, before[k]), k
+    # single-layer functional: a training-mode BatchNorm, and a backward
+    L = mats[1]
+    V = L.shape[0]
+    cl = torch.nn.Linear(3 * 64, 64).to(dev())
+    bn = torch.nn.BatchNorm1d(64).to(dev()).train()
+    bn_before = {k: v.clone() for k, v in bn.state_dict().items()}
+    xi = torch.randn(2, V, 64, device=dev(), requires_grad=True)
+    cgc.set_default_precision("fp16")
+    try:
+        with pytest.raises(RuntimeError, match="fp16"):
+            cgc.graph_conv_cheby(xi, cl, bn, L, 64, 3)
+        yi = cgc.graph_conv_cheby(xi, cl, None, L, 64, 3)
+        with pytest.raises(RuntimeError, match="fp16"):
+            yi.sum().backward()
+        assert cgc.graph_handle(L).kernel_status(0) == 0
+    finally:
+        cgc.set_default_precision("fp16x3")
+    for k, v in bn.state_dict().items():
+        assert torch.equal(v, bn_before[k]), k
+    # back at fp16x3: bitwise the model that never left it
+    model.set_precision("fp16x3").eval()
+    ref.eval()
+    with torch.no_grad():
+        assert torch.equal(model(x), ref(x))
+    assert model._hier.kernel_status(0) == 0
