@@ -128,6 +128,11 @@ int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int3
  * both MMA warpgroups on one tile: Fin = Fout = 256), out[1] = A/B ring slots, out[2] = T1 stages; all 0 off the
  * tensor cores.                                                                                                    */
 int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, int32_t out[3]);
+/* Debug: size this handle's persistent tensor-core grids (conv, dW, the fc's dense GEMM) for n SMs instead of the
+ * device's count, as on a part with fewer SMs: a CTA walks ceil(n_tiles / grid.x) tiles.  No route reads the count, so
+ * the same kernels run; only which CTA (and warpgroup) takes each tile changes.  0 <= n <= the device's count;
+ * 0 restores it.                                                                                                    */
+int p2m_debug_set_sm_count(p2m_model_t* m, int n);
 /* Debug: the paths the network schedules (p2m_meshnet_forward / _backward) take for layer `layer` at batch `batch`,
  * from the same route decision the schedules make.  need_dx only matters for layer 0 (the network input's gradient).
  * out[0] = forward conv on tensor cores, out[1] = its padding-vertex elision, out[2] = backward by the thin head's
@@ -883,6 +888,12 @@ const char* p2m_version(void);
 /* Number of kernels this library launched on behalf of the calling thread since the last reset.    */
 int64_t p2m_launch_count(void);
 void p2m_launch_count_reset(void);
+/* Debug: the process-wide log of tensor-core launches since the last reset, one entry of 9 int32 per launch:
+ * kind (0 = Chebyshev conv, 1 = dW, 2 = dense GEMM), output columns per CTA, ring slots, X / T1 stages, MODE (1 = T1
+ * given, 0 = plain GEMM), single-pass fp16 (0 / 1), grid.x, grid.y, tiles.  Copies the first min(count, 32768,
+ * max_entries) entries into out (NULL: none) and returns the count, which keeps counting past the 32768 it stores. */
+int64_t p2m_debug_conv_log(int32_t* out, int max_entries);
+void p2m_debug_conv_log_reset(void);
 
 #ifdef __cplusplus
 }

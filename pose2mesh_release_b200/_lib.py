@@ -205,7 +205,7 @@ class H36MError(C.Structure):
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
-    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_conv_tiling", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
+    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_conv_tiling", "p2m_debug_set_sm_count", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_meshnet_workspace_bytes_opts", "p2m_meshnet_forward_opts",
     "p2m_meshnet_backward_opts", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
@@ -225,6 +225,7 @@ EXPORTS = [
     "p2m_training_pose2d", "p2m_augm_params", "p2m_training_pose2d_augmented", "p2m_sample_targets",
     "p2m_layer_joint_targets",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
+    "p2m_debug_conv_log", "p2m_debug_conv_log_reset",
 ]
 
 _lib = None
@@ -271,6 +272,8 @@ def load() -> C.CDLL:
         lib.p2m_debug_conv_path.restype = C.c_int
         lib.p2m_debug_conv_tiling.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
         lib.p2m_debug_conv_tiling.restype = C.c_int
+        lib.p2m_debug_set_sm_count.argtypes = [vp, C.c_int]
+        lib.p2m_debug_set_sm_count.restype = C.c_int
         lib.p2m_debug_layer_route.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
         lib.p2m_debug_layer_route.restype = C.c_int
         lib.p2m_debug_set_capture.argtypes = [vp, C.POINTER(Capture)]
@@ -432,8 +435,38 @@ def load() -> C.CDLL:
         lib.p2m_launch_count.restype = i64
         lib.p2m_launch_count_reset.argtypes = []
         lib.p2m_launch_count_reset.restype = None
+        lib.p2m_debug_conv_log.argtypes = [c_int32_p, C.c_int]
+        lib.p2m_debug_conv_log.restype = i64
+        lib.p2m_debug_conv_log_reset.argtypes = []
+        lib.p2m_debug_conv_log_reset.restype = None
         _lib = lib
     return _lib
+
+
+CONV_LOG_FIELDS = ("kind", "nc", "ns", "xs", "mode", "f16", "grid_x", "grid_y", "n_tiles")
+TC_KINDS = ("conv", "dw", "gemm")
+
+
+def conv_log(reset: bool = False) -> list:
+    """Debug: the tensor-core launches logged since the last reset (p2m_debug_conv_log), one dict per launch with
+    the fields of CONV_LOG_FIELDS (kind as a TC_KINDS name) and tiles_per_cta = ceil(n_tiles / grid_x).  Raises if the
+    log overflowed.  reset: clear the log after reading it."""
+    lib = load()
+    n = lib.p2m_debug_conv_log(None, 0)
+    buf = (C.c_int32 * (9 * max(n, 1)))()
+    if lib.p2m_debug_conv_log(buf, n) != n:
+        raise RuntimeError("conv log: launches were logged while it was read")
+    if n > 32768:
+        raise RuntimeError(f"conv log overflowed: {n} launches, 32768 stored")
+    if reset:
+        lib.p2m_debug_conv_log_reset()
+    out = []
+    for i in range(n):
+        e = dict(zip(CONV_LOG_FIELDS, buf[9 * i:9 * i + 9]))
+        e["kind"] = TC_KINDS[e["kind"]]
+        e["tiles_per_cta"] = -(-e["n_tiles"] // e["grid_x"])
+        out.append(e)
+    return out
 
 
 def check(status: int, what: str = "p2m call"):

@@ -1979,6 +1979,7 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   const int n_slices = a.fout / NC;
   const dim3 grid(std::min(p.n_tiles, std::max(1, sm_count / n_slices)), n_slices);
   kern<<<grid, ConvRoles<N>::threads, smem, s>>>(p);
+  log_tc_launch(TC_CONV, NC, NS, XS, a.plain ? M0 : 1, F16, grid, p.n_tiles);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }
@@ -2242,6 +2243,7 @@ int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_u
     for (int c0 = 0; c0 < gathered_width / FC; ++c0) {  // one feature chunk per launch (the kernel's n_chunk)
       p.chunk0 = c0;
       kern<<<grid, NUM_THREADS2, smem, s>>>(p);
+      log_tc_launch(TC_DW, p.m_cols, DW_NS, xs, 1, 0, dim3(grid), p.n_tiles);
       P2M_LAUNCH_OK();
     }
   }
@@ -2329,6 +2331,7 @@ int launch_gemm_cfg(KParams p, int n_slices, int sm_count, cudaStream_t s) {
   p.wblock_stride = (long long)N * 128;
   const dim3 grid(std::min(p.n_tiles, sm_count), n_slices);
   kern<<<grid, ConvRoles<N>::threads, smem, s>>>(p);
+  log_tc_launch(TC_GEMM, N, NS, 1, 0, 0, grid, p.n_tiles);
   P2M_LAUNCH_OK();
   return P2M_OK;
 }

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstring>
 #include <memory>
@@ -19,6 +20,19 @@ static thread_local std::string g_error;
 static thread_local int64_t g_launches = 0;
 void set_error(const std::string& msg) { g_error = msg; }
 void count_launch(int n) { g_launches += n; }
+
+// p2m_debug_conv_log: process-wide (the autograd engine runs backwards on its own thread), bounded; a slot is claimed
+// by one atomic increment, so logging costs the launch paths no lock
+constexpr int CONV_LOG_CAP = 1 << 15;
+constexpr int CONV_LOG_FIELDS = 9;
+static int32_t g_conv_log[CONV_LOG_CAP][CONV_LOG_FIELDS];
+static std::atomic<int64_t> g_conv_log_n{0};
+void log_tc_launch(int kind, int nc, int ns, int xs, int mode, int f16, dim3 grid, int n_tiles) {
+  const int64_t i = g_conv_log_n.fetch_add(1, std::memory_order_relaxed);
+  if (i >= CONV_LOG_CAP) return;  // counted, not stored
+  const int32_t e[CONV_LOG_FIELDS] = {kind, nc, ns, xs, mode, f16, (int32_t)grid.x, (int32_t)grid.y, n_tiles};
+  std::memcpy(g_conv_log[i], e, sizeof(e));
+}
 
 int arrays_device(const char* where, std::initializer_list<const void*> arrays, int* dev) {
   int found = -1;
@@ -74,7 +88,8 @@ using namespace p2m;
 
 struct p2m_model {
   int device = 0;
-  int sm_count = 132;
+  int sm_count = 132;            // SMs the persistent tensor-core grids are sized for (p2m_debug_set_sm_count)
+  int sm_count_device = 132;     // ... the device's own count
   int precision = P2M_PREC_FP32_SIMT;
   std::vector<DevLevel> levels;
   std::vector<Layer> layers;
@@ -652,6 +667,16 @@ const char* p2m_version(void) { return "pose2mesh_release_b200 0.1 (sm_90a)"; }
 int64_t p2m_launch_count(void) { return g_launches; }
 void p2m_launch_count_reset(void) { g_launches = 0; }
 
+int64_t p2m_debug_conv_log(int32_t* out, int max_entries) {
+  const int64_t n = g_conv_log_n.load(std::memory_order_relaxed);
+  if (out != nullptr && max_entries > 0) {
+    const int64_t k = std::min<int64_t>(std::min<int64_t>(n, CONV_LOG_CAP), max_entries);
+    std::memcpy(out, g_conv_log, (size_t)k * sizeof(g_conv_log[0]));
+  }
+  return n;
+}
+void p2m_debug_conv_log_reset(void) { g_conv_log_n.store(0, std::memory_order_relaxed); }
+
 int p2m_model_create(const p2m_model_desc_t* d, p2m_model_t** out) {
   if (!d || !out || d->n_levels < 1 || (d->n_blocks != 0 && (d->n_blocks < 3 || d->n_levels < 2))) {
     set_error("model_create: bad descriptor");
@@ -678,7 +703,7 @@ int p2m_model_create(const p2m_model_desc_t* d, p2m_model_t** out) {
   DeviceGuard guard(d->device);
   p2m_model* m = new p2m_model();
   m->device = d->device;
-  m->sm_count = prop.multiProcessorCount;
+  m->sm_count = m->sm_count_device = prop.multiProcessorCount;
   // ---- levels: CSR with relative offsets
   for (int l = 0; l < d->n_levels; ++l) {
     DevLevel g;
@@ -867,6 +892,15 @@ int p2m_debug_set_trace(p2m_model_t* m, void* dev_buf) {
   set_error("debug_set_trace: this library was built without P2M_UMMA_TRACE");
   return P2M_ERR_INVALID;
 #endif
+}
+
+int p2m_debug_set_sm_count(p2m_model_t* m, int n) {
+  if (!m || n < 0 || n > m->sm_count_device) {
+    set_error("debug_set_sm_count: need 0 <= n <= the device's SM count");
+    return P2M_ERR_INVALID;
+  }
+  m->sm_count = n == 0 ? m->sm_count_device : n;
+  return P2M_OK;
 }
 
 int p2m_debug_set_elide_padding(p2m_model_t* m, int enable) {

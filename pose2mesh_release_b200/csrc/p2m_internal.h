@@ -14,6 +14,9 @@ namespace p2m {
 // ---------------------------------------------------------------- error plumbing (thread-local)
 void set_error(const std::string& msg);
 void count_launch(int n = 1);
+// p2m_debug_conv_log: one entry per launch of the tensor-core conv, dW or dense-GEMM kernel (process-wide)
+enum TcKind { TC_CONV = 0, TC_DW = 1, TC_GEMM = 2 };
+void log_tc_launch(int kind, int nc, int ns, int xs, int mode, int f16, dim3 grid, int n_tiles);
 
 #define P2M_CUDA_OK(expr)                                                                     \
   do {                                                                                        \

@@ -100,11 +100,14 @@ class BakedHierarchy:
         _lib.check(_lib.load().p2m_model_set_profiling(self.handle(device_index), int(enable)), "set_profiling")
 
     def set_debug(self, device_index: int, fuse_head: Optional[bool] = None, elide_padding: Optional[int] = None,
-                  dedup_padding: Optional[bool] = None):
+                  dedup_padding: Optional[bool] = None, sm_count: Optional[int] = None):
         """Ablation switches of the tensor-core path: fused 64->3 head in eval (default on), isolated padding vertices
         through a plain GEMM with combined weights (0 off, 1 = default: levels with >= 40 % isolated rows, 2 = every
-        level that has the tile families)."""
+        level that has the tile families), the SM count the persistent tensor-core grids are sized for (0 = the
+        device's own; a smaller count gives each CTA more tiles, as on a part with fewer SMs)."""
         lib, h = _lib.load(), self.handle(device_index)
+        if sm_count is not None:
+            _lib.check(lib.p2m_debug_set_sm_count(h, int(sm_count)), "set_sm_count")
         if fuse_head is not None:
             _lib.check(lib.p2m_debug_set_fuse_head(h, int(fuse_head)), "set_fuse_head")
         if elide_padding is not None:

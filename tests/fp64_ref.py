@@ -152,11 +152,13 @@ def cheb_conv_bwd(x, L, W, dz):
     return dx, dW, db
 
 
-def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised"):
+def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised", dw_chain=0):
     """Bounds (dx, dW, db) of cheb_conv_bwd.  split: see cheb_conv_fwd_bound; in the network backward dz is scaled into
     fp16's range by a power of two (floor 2^-34 max|dz| per entry), the weights are at the fixed 2^6 and the x side of
     dW is unscaled.  dX there is either the dT GEMMs + the basis backward or a conv on dz ([dz | L dz | T2 dz] against
-    the transposed weights), dW either on the basis of x or on the basis of dz: the floor is the larger of the two."""
+    the transposed weights), dW either on the basis of x or on the basis of dz: the floor is the larger of the two.
+    dw_chain > 0: hold dW to n u of a sequential chain of that many fp32 adds at least (a grid capped to a few CTAs
+    accumulates the rows of many tiles in one CTA, where dW's one-signed partial sums grow linearly, not as sqrt(n))."""
     Labs = abs(sp.csr_matrix(L, dtype=np.float64))
     W = np.abs(np.asarray(W, dtype=np.float64))
     adz = np.abs(np.asarray(dz, dtype=np.float64))
@@ -194,6 +196,8 @@ def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised"):
     Tf = Tabs.reshape(B * V, 3, F)
     R = B * V
     g_dw = gamma(R, precision, deg) + (R.bit_length() * U32)   # + the cross-CTA fp32 atomic adds (log-depth tree)
+    if dw_chain:   # the fp32 accumulation as a sequential chain of dw_chain adds: the deterministic worst case
+        g_dw = max(g_dw, dw_chain * U32 + (SPLIT if precision == "fp16x3" else 0.0))
     b_dw = g_dw * _contract_rows(dzf, Tf)
     if split == "network":
         Tdz = basis(adz, Labs)

@@ -96,6 +96,35 @@ def isolated(V=1024, n_real=512, two_diagonals=False):
     return out
 
 
+def band_far(V, bw, n_far):
+    """band(V, bw) plus rows 0..n_far-1 joined to rows V-1, V-2, ...: tile 0 stages its band halo and n_far far rows
+    on top of a band's CSR, so a large staged-row count and a large metadata blob come together."""
+    e = [(a, a + d) for d in range(1, bw + 1) for a in range(V - d)] + [(i, V - 1 - i) for i in range(n_far)]
+    return rescaled_laplacian(_edges_to_adj(V, e))
+
+
+def block_clique(V, e, blk=64):
+    """Cliques of blk consecutive vertices (one per 64-row tile), each vertex also joined to the first e vertices of
+    the next block: a 64-row tile stages few rows (its block, the next e, the previous block) but holds a CSR entry for
+    nearly every (own row, staged row) pair, so its metadata blob is large for its halo."""
+    edges = []
+    for b0 in range(0, V, blk):
+        own = np.arange(b0, min(V, b0 + blk))
+        nxt = np.arange(b0 + blk, min(V, b0 + blk + e))
+        for other in (own, nxt):
+            a, b = np.meshgrid(own, other)
+            edges.append(np.stack([a.ravel(), b.ravel()], axis=1))
+    return rescaled_laplacian(_edges_to_adj(V, np.concatenate(edges)))
+
+
+def two_cliques(a):
+    """Two 64-vertex cliques (one per 64-row tile), the last a vertices of the first joined to the first a of the
+    second: each tile stages 64 + a rows and holds 64 * 64 + a * a CSR entries."""
+    edges = [(i, j) for b0 in (0, 64) for i in range(b0, b0 + 64) for j in range(i + 1, b0 + 64)]
+    edges += [(i, j) for i in range(64 - a, 64) for j in range(64, 64 + a)]
+    return rescaled_laplacian(_edges_to_adj(128, edges))
+
+
 def dense(V=2048, degree=64, seed=0):
     """Random graph of degree ~64: every 128-row tile stages far more than 512 rows (own rows + 1-hop halo), beyond
     what the tile-metadata builder accepts."""
@@ -125,6 +154,15 @@ FAMILIES = {
     # 20: the conv still fits with one, the weight-gradient kernel no longer fits (SIMT dW)
     **{f"band{bw}": ((lambda bw=bw: band(1024, bw)), "X stages 2 -> 1 and the shared-memory cut-off to SIMT")
        for bw in (8, 12, 14, 16, 20)},
+    # bands sized for the 64-row tiles of the 128- and 256-wide convs: 18, a ring of 3 slots in the 64 x 128
+    # configuration; 21, the 64 x 256 mode with one T1 stage (tests/test_gpu_persistent_tiles_fp64.py)
+    **{f"band{bw}": ((lambda bw=bw: band(1024, bw)), "64-row tiles: ring of 3 / one T1 stage") for bw in (18, 21)},
+    "farband20": ((lambda: band_far(512, 20, 80)), "single-pass fp16, 128 x 64: one X stage"),
+    **{f"clique{e}": ((lambda e=e: block_clique(512, e)), "64-row tiles with large blobs for their halo")
+       for e in (12, 14)},
+    # a = 49: the largest blobs for 113 staged rows that still fit a ring of 3 with one T1 stage; the 128-column plain
+    # GEMM (the backward's dT GEMMs) then needs one X stage too
+    "twoclique49": ((lambda: two_cliques(49)), "64-row tiles: the plain GEMM's ring of 3 with one X stage"),
     "h1_256": (lambda: far_edges(1024, 126), "max_h1 = 256: still tensor cores"),
     "h1_257": (lambda: far_edges(1024, 127), "max_h1 = 257: the 256-staged-row cut-off to SIMT"),
     "far": (lambda: far_edges(1088, 64), "halos that cross the whole graph (tile 0 <-> last, ragged) tile"),

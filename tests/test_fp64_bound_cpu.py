@@ -278,6 +278,17 @@ def test_graph_family_structure(name):
         c = sp.csr_matrix(L)
         staged = set(range(128)) | set(c[:128].indices.tolist())
         assert len(staged) == (256 if name == "h1_256" else 257)
+    if name == "farband20":
+        c = sp.csr_matrix(L)
+        staged = set(range(128)) | set(c[:128].indices.tolist())
+        assert V == 512 and deg.max() == 2 * 20 + 2 and len(staged) == 128 + 20 + 80
+    if name.startswith("clique"):
+        e = int(name[6:])
+        assert V == 512 and deg.max() == 128 + e and np.all(L[:64, :64].toarray() != 0)
+    if name == "twoclique49":
+        c = sp.csr_matrix(L)
+        staged = set(range(64)) | set(c[:64].indices.tolist())
+        assert V == 128 and len(staged) == 64 + 49 and c[:64].nnz == 64 * 64 + 49 * 49
     if name == "far":
         assert V == 1088 and L[0, V - 1] != 0 and L[63, V - 64] != 0
     if name == "hub":

@@ -55,13 +55,16 @@ def conv_info(gh, fin, fout):
     return int(path[0]), tuple(til)
 
 
-def run_layer(L, x, W, b):
-    """p2m_cheb_conv_fwd at fp16: (y as float64, on tensor cores, (cols, ns, xs))."""
+def run_layer(L, x, W, b, sm_cap=0):
+    """p2m_cheb_conv_fwd at fp16: (y as float64, on tensor cores, (cols, ns, xs)).  sm_cap > 0: the persistent
+    tensor-core grids are sized for that many SMs (p2m_debug_set_sm_count)."""
+    from pose2mesh_release_b200 import _lib
     from pose2mesh_release_b200 import cheby_graph_conv as cgc
 
     cgc.set_default_precision("fp16")
+    gh = cgc.graph_handle(L)
     try:
-        gh = cgc.graph_handle(L)
+        _lib.check(_lib.load().p2m_debug_set_sm_count(gh.handle(0), sm_cap), "set_sm_count")
         with torch.no_grad():
             y = cgc.ChebConvLinear.apply(torch.as_tensor(x).to(dev()), torch.as_tensor(W).to(dev()),
                                          torch.as_tensor(b).to(dev()), gh)
@@ -69,6 +72,7 @@ def run_layer(L, x, W, b):
         assert gh.kernel_status(0) == 0, "a tensor-core kernel timed out on an mbarrier"
         tc, til = conv_info(gh, x.shape[2], W.shape[0])
     finally:
+        _lib.check(_lib.load().p2m_debug_set_sm_count(gh.handle(0), 0), "set_sm_count")
         cgc.set_default_precision("fp16x3")
     return y.double().cpu().numpy(), tc, til
 
@@ -114,15 +118,25 @@ def test_single_layer_graph_family(name, fin, fout):
 
 @pytest.mark.parametrize("fin,fout", [(64, 64), (128, 128), (256, 256)], ids=lambda v: str(v))
 def test_single_layer_persistent_cta_loop(fin, fout):
-    """V = 128: n_tiles = B (128 x 64) or 2 B (64-row tiles); B around the grid makes CTAs run 0, 1, 2 or more tiles."""
+    """V = 128: n_tiles = B (128 x 64) or 2 B (64-row tiles; 256 -> 256 in the 64 x 256 mode, one column slice), on a
+    grid capped at 8 SMs (grid.x = min(n_tiles, 8), read back from the launch log): B = 1, 7, 9 and 29 make each CTA
+    run from 1 to 8 tiles.
+    tests/test_gpu_persistent_tiles_fp64.py covers every configuration."""
+    from pose2mesh_release_b200 import _lib
+
     L = G.get("V128")
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    grid = sms // max(1, fout // (64 if fout == 64 else 128))
-    for B in (1, grid - 1, grid + 1, 3 * grid + 5):
+    grid = 8
+    most = 0
+    for B in (1, 7, 9, 29):
         x, W, b = make_layer(128, B, fin, fout, seed=B)
-        y, tc, _ = run_layer(L, x, W, b)
+        _lib.conv_log(reset=True)
+        y, tc, _ = run_layer(L, x, W, b, sm_cap=grid)
+        conv = next(e for e in _lib.conv_log(reset=True) if e["kind"] == "conv")
+        assert conv["grid_x"] == min(conv["n_tiles"], max(1, grid // conv["grid_y"])) and conv["f16"] == 1, conv
+        most = max(most, conv["tiles_per_cta"])
         assert tc == 1
         check_single_pass(f"persistent B={B} {fin}->{fout}", L, x, W, b, y)
+    assert most >= 4, most
 
 
 # ------------------------------------------------------------------------------------------- 2. network, layer by layer

@@ -52,13 +52,16 @@ def conv_path(gh, fin, fout):
     return dict(zip(("conv", "conv_xs", "dw", "dw_xs", "dt", "dt_xs", "tma", "max_h1", "n_iso"), list(out)))
 
 
-def run(L, x, W, b, precision, dz=None):
-    """graph_conv_cheby's linear part on the GPU: returns (y, dx, dW, db, path) as float64 numpy (grads None without dz)."""
+def run(L, x, W, b, precision, dz=None, sm_cap=0):
+    """graph_conv_cheby's linear part on the GPU: returns (y, dx, dW, db, path) as float64 numpy (grads None without dz).
+    sm_cap > 0: the persistent tensor-core grids are sized for that many SMs (p2m_debug_set_sm_count)."""
+    from pose2mesh_release_b200 import _lib
     from pose2mesh_release_b200 import cheby_graph_conv as cgc
 
     cgc.set_default_precision(precision)
+    gh = cgc.graph_handle(L)
     try:
-        gh = cgc.graph_handle(L)
+        _lib.check(_lib.load().p2m_debug_set_sm_count(gh.handle(0), sm_cap), "set_sm_count")
         xg = torch.as_tensor(np.asarray(x, np.float32)).to(dev()).requires_grad_(dz is not None)
         Wg = torch.as_tensor(np.asarray(W, np.float32)).to(dev()).requires_grad_(dz is not None)
         bg = torch.as_tensor(np.asarray(b, np.float32)).to(dev()).requires_grad_(dz is not None)
@@ -70,6 +73,7 @@ def run(L, x, W, b, precision, dz=None):
         assert gh.kernel_status(0) == 0, "a tensor-core kernel timed out on an mbarrier"
         p = conv_path(gh, x.shape[2], W.shape[0])
     finally:
+        _lib.check(_lib.load().p2m_debug_set_sm_count(gh.handle(0), 0), "set_sm_count")
         cgc.set_default_precision("fp32")
     return (y.detach().double().cpu().numpy(),) + grads + (p,)
 
@@ -130,21 +134,33 @@ def test_width_grid_forward_and_backward(fin, fout, precision, lvl):
 
 
 # ------------------------------------------------------------------------------------------------- persistent loop
-@pytest.mark.parametrize("fin,fout", [(64, 64), (128, 128), (32, 256)], ids=lambda v: str(v))
+PERSISTENT_CAP = 8   # SMs the grids are sized for: independent of the part's own count
+
+
+@pytest.mark.parametrize("fin,fout", [(64, 64), (128, 128), (32, 256), (256, 256)], ids=lambda v: str(v))
 def test_persistent_cta_loop(fin, fout):
-    """V = 128: one tile per mesh, so n_tiles = B and the conv grid is min(B, SMs / column slices): B = 1, grid - 1,
-    grid, grid + 1 and 3 grid + 5 make every CTA run 0, 1, 2 or 4 tiles (ring slots and mbarrier phases reused)."""
+    """V = 128 is one 128-row tile per mesh (Fout = 64) or two 64-row tiles (Fout % 128 == 0; 32 -> 256 as two
+    128-column slices, 256 -> 256 in the 64 x 256 mode), so n_tiles = B or 2 B, on a grid capped at 8 SMs: grid.x =
+    min(n_tiles, 8 / column slices), read back from the launch log.  B = 1, 7, 8, 9 and 29 make each CTA run from 1 to
+    15 tiles (ring slots and mbarrier phases reused).  tests/test_gpu_persistent_tiles_fp64.py covers every
+    configuration."""
+    from pose2mesh_release_b200 import _lib
+
     L = G.get("V128")
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    grid = sms // (fout // 64)
-    for B in (1, grid - 1, grid, grid + 1, 3 * grid + 5):
+    most = 0
+    for B in (1, 7, 8, 9, 29):
         x, W, b = make_layer(128, B, fin, fout, seed=B)
         dz = np.random.default_rng(B).standard_normal((B, 128, fout)).astype(np.float32)
-        y, dx, dW, db, p = run(L, x, W, b, "fp16x3", dz if B in (grid + 1, 3 * grid + 5) else None)
+        _lib.conv_log(reset=True)
+        y, dx, dW, db, p = run(L, x, W, b, "fp16x3", dz if B in (9, 29) else None, sm_cap=PERSISTENT_CAP)
+        conv = next(e for e in _lib.conv_log(reset=True) if e["kind"] == "conv")
+        assert conv["grid_x"] == min(conv["n_tiles"], max(1, PERSISTENT_CAP // conv["grid_y"])), conv
+        most = max(most, conv["tiles_per_cta"])
         expect_tc(p, "fp16x3", fin, fout, 128)
         check_fwd(f"persistent B={B} {fin}->{fout}", L, x, W, b, "fp16x3", y)
         if dx is not None:
             check_bwd(f"persistent B={B} {fin}->{fout}", L, x, W, dz, "fp16x3", dx, dW, db)
+    assert most >= 4, most
 
 
 # ------------------------------------------------------------------------------------------------- graph families

@@ -266,7 +266,8 @@ def check_train(net, tag, x, y, cap, grads, bufs, need_dx):
         on_dw = r["tc_dw"] or r["dw_dz_basis"]
         on_dx = r["tc_dx"] or r["tc_dt"]
         bdx, _, bdb = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, prec_of(net, on_dx), split="network")
-        _, bdw, _ = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, prec_of(net, on_dw), split="network")
+        _, bdw, _ = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, prec_of(net, on_dw), split="network",
+                                          dw_chain=dw_chain(net, li, B))
         check(t + " dW", prec, grads[f"cl.{li}.weight"], dW64, bdw)
         if not L["bn"]:
             check(t + " db", prec, grads[f"cl.{li}.bias"], db64, R.col_sum_bound(g_z))
@@ -293,6 +294,18 @@ def check_train(net, tag, x, y, cap, grads, bufs, need_dx):
             check(f"{tag} fc dx", prec, cap["fc_dx"], ref_fx,
                   R.gamma(Wf.shape[0], "fp32") * (np.abs(gf) @ np.abs(Wf)))
             assert np.array_equal(cap["fc_dx"].reshape(B, -1), cap["g_a"][blk["first"] - 1].reshape(B, -1)), tag
+
+
+def dw_chain(net, li, B):
+    """With the persistent grids capped at net.sm_cap SMs (tests/test_gpu_persistent_tiles_fp64.py): the fp32 adds a dW
+    element of layer li goes through, the rows of one CTA's 128-row tiles and then one atomic add per CTA; 0 (the
+    default bound) without a cap."""
+    cap = getattr(net, "sm_cap", 0)
+    if not cap:
+        return 0
+    n_tiles = B * -(-net.V(li) // 128)
+    grid = min(n_tiles, cap)
+    return -(-n_tiles // grid) * 128 + grid
 
 
 def train_inputs(net, B, seed):
@@ -388,11 +401,24 @@ def test_eval_forward_layer_by_layer(name, elide, B, precision):
     combined-weight GEMM as with every isolated row computed, and no connected row reads an isolated one."""
     net = Net(name, precision, seed=31 + B + elide, open_relus=False)
     x, _ = train_inputs(net, B, seed=5 + elide)
+    tag = f"{name} eval elide={elide} B={B}"
+    y, yf = check_eval(net, tag, x, elide)
+    # dedup: bit for bit against dedup off, with the fused head on and off
+    for fuse in (False, True):
+        yd, _ = forward_eval(net, x, elide, dedup=True, fuse=fuse, capture=False)
+        yo = y if not fuse else yf
+        assert np.array_equal(yd, yo), (tag, "dedup", fuse, float(np.abs(yd - yo).max()))
+
+
+def check_eval(net, tag, x, elide):
+    """The eval forward with dedup off, fused head off and then on: every layer's output (and the fc's) from its
+    captured input, then the fused head from the fused layer's captured input.  Returns (y, y with the fused head)."""
+    precision = net.precision
+    B = x.shape[0]
     y, cap = forward_eval(net, x, elide, dedup=False, fuse=False)
     n = net.n_layers
     act = {li: cap["y"][li].reshape(B, net.V(li), -1) for li in range(n)}
     fc_out = cap["fc_out"]
-    tag = f"{name} eval elide={elide} B={B}"
     assert np.array_equal(act[n - 1], y.reshape(act[n - 1].shape)), tag
     for li in range(n):
         inp, block_in = layer_input(net, li, x, fc_out, act)
@@ -416,11 +442,7 @@ def test_eval_forward_layer_by_layer(name, elide, B, precision):
         ref = R.cheb_conv_fwd(y1, Lh, Wh, bh)
         bound = R.cheb_conv_fwd_bound(y1, Lh, Wh, bh, "fp32") + R.thin_head_fused_bound(y1, e1, Lh, Wh)
         check(f"{tag} fused head", precision, yf.reshape(ref.shape), ref, bound)
-    # dedup: bit for bit against dedup off, with the fused head on and off
-    for fuse in (False, True):
-        yd, _ = forward_eval(net, x, elide, dedup=True, fuse=fuse, capture=False)
-        yo = y if not fuse else yf
-        assert np.array_equal(yd, yo), (tag, "dedup", fuse, float(np.abs(yd - yo).max()))
+    return y, yf
 
 
 # ------------------------------------------------------------------------------------------- launches and coverage
