@@ -18,7 +18,7 @@ import pytest
 import torch
 
 import fp64_ref as R
-from helpers import graph_from_fixture
+from helpers import CASES, graph_from_fixture
 
 pytestmark = pytest.mark.gpu
 
@@ -67,7 +67,14 @@ def net_levels(name):
         return [next(m for m in mats if m.shape[0] == V) for V in (128, 64, 17)], CUSTOM_PLAN
     from pose2mesh_release_b200.meshnet import channel_plan
 
-    mats = list(graph_from_fixture(name)[0])
+    if name == "smpl_like":   # its fixture stores digests only: rebuild the hierarchy (test_gpu_at_size._hierarchy)
+        from pose2mesh_release_b200 import graph as pg
+
+        n, seed, levels, _ = CASES[name]
+        face = pg.synthetic_sphere_faces(n, seed)
+        mats = list(pg.build_coarse_graphs(face, 17, pg.H36M_SKELETON, pg.H36M_FLIP_PAIRS, levels=levels)[1])
+    else:
+        mats = list(graph_from_fixture(name)[0])
     del mats[-2]   # meshnet.py:35
     return mats, channel_plan(5, 3, name == "mano_like")
 
@@ -124,9 +131,11 @@ class Net:
         return L["j"] == 0 and self.blocks[L["block"]]["in_unpool"]
 
 
-def layer_input(net, li, x, fc_out, act):
+def layer_input(net, li, x, fc_out, act, ref=R):
     """The conv input of layer li (unpooled where the block reads its input through the virtual x2 unpool) and the
-    block input (for the residual), from the captured activations act[l]."""
+    block input (for the residual), from the captured activations act[l].  ref: the reference module (fp64_ref, or
+    fp64_ref_torch for device tensors)."""
+    R = ref
     L = net.layers[li]
     blk = net.blocks[L["block"]]
     b = L["block"]
@@ -163,12 +172,12 @@ def fc_ref(a0, W, b, precision):
     return ref, bound
 
 
-def residual(net, li, block_in):
+def residual(net, li, block_in, ref=R):
     """The residual added at the end of layer li's block (resampled or identity) and its fp32 evaluation bound."""
     L, blk = net.layers[li], net.blocks[net.layers[li]["block"]]
     if not (L["end"] and blk["res"]):
         return 0.0, 0.0
-    return R.channel_resample(block_in, blk["cout"]), R.channel_resample_bound(block_in, blk["cout"])
+    return ref.channel_resample(block_in, blk["cout"]), ref.channel_resample_bound(block_in, blk["cout"])
 
 
 # ----------------------------------------------------------------------------------------------------------- running
