@@ -128,6 +128,15 @@ int p2m_debug_conv_path(const p2m_model_t* m, int level, int fin, int fout, int3
  * both MMA warpgroups on one tile: Fin = Fout = 256), out[1] = A/B ring slots, out[2] = T1 stages; all 0 off the
  * tensor cores.                                                                                                    */
 int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, int32_t out[3]);
+/* Debug: the level's tile families and what a tensor-core conv fin -> fout would launch on each (host only, no device
+ * work).  out[f][k][15] for family f = consecutive tiles, padding elision's connected-row tiles (real_tiles), its
+ * isolated-row tiles (iso_tiles), its eval-mode class representatives (rep_tiles), and tile size k = 128 rows, 64
+ * rows: [0] tiles (0: the family does not exist), [1] largest staged-row count (own rows + 1-hop halo), [2] metadata
+ * blob stride in bytes; then (output columns per CTA, A/B ring slots, X / T1 stages) for the T1-given conv at fp16x3
+ * [3..5], the plain GEMM at fp16x3 [6..8], the T1-given conv at fp16 [9..11], the plain GEMM at fp16 [12..14], all 0
+ * where it does not fit shared memory or on the tile size a conv to fout does not run on (fout 64: 128-row tiles,
+ * 128 and 256: 64-row tiles).  fin a multiple of 32 in [32, 256], fout 64, 128 or 256.                            */
+int p2m_debug_tile_families(const p2m_model_t* m, int level, int fin, int fout, int32_t out[120]);
 /* Debug: size this handle's persistent tensor-core grids (conv, dW, the fc's dense GEMM) for n SMs instead of the
  * device's count, as on a part with fewer SMs: a CTA walks ceil(n_tiles / grid.x) tiles.  No route reads the count, so
  * the same kernels run; only which CTA (and warpgroup) takes each tile changes.  0 <= n <= the device's count;

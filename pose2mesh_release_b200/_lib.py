@@ -205,7 +205,7 @@ class H36MError(C.Structure):
 
 EXPORTS = [
     "p2m_model_create", "p2m_model_destroy", "p2m_model_num_layers", "p2m_model_layer_info",
-    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_conv_tiling", "p2m_debug_set_sm_count", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
+    "p2m_model_set_precision", "p2m_debug_kernel_status", "p2m_debug_set_trace", "p2m_debug_set_fuse_head", "p2m_debug_set_elide_padding", "p2m_debug_set_dedup_padding", "p2m_debug_conv_path", "p2m_debug_conv_tiling", "p2m_debug_tile_families", "p2m_debug_set_sm_count", "p2m_debug_layer_route", "p2m_debug_set_capture", "p2m_model_set_profiling", "p2m_model_layer_times_ms", "p2m_meshnet_workspace_bytes", "p2m_meshnet_backward_scratch_bytes",
     "p2m_meshnet_forward", "p2m_meshnet_backward", "p2m_meshnet_workspace_bytes_opts", "p2m_meshnet_forward_opts",
     "p2m_meshnet_backward_opts", "p2m_model_set_output_gather", "p2m_meshnet_forward_vertices", "p2m_meshnet_host_io_bytes", "p2m_meshnet_forward_host", "p2m_meshnet_forward_vertices_host",
     "p2m_cheb_conv_workspace_bytes", "p2m_cheb_conv_fwd", "p2m_cheb_conv_bwd", "p2m_graph_match_level", "p2m_posenet_workspace_bytes", "p2m_posenet_forward",
@@ -272,6 +272,8 @@ def load() -> C.CDLL:
         lib.p2m_debug_conv_path.restype = C.c_int
         lib.p2m_debug_conv_tiling.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
         lib.p2m_debug_conv_tiling.restype = C.c_int
+        lib.p2m_debug_tile_families.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
+        lib.p2m_debug_tile_families.restype = C.c_int
         lib.p2m_debug_set_sm_count.argtypes = [vp, C.c_int]
         lib.p2m_debug_set_sm_count.restype = C.c_int
         lib.p2m_debug_layer_route.argtypes = [vp, C.c_int, C.c_int, C.c_int, c_int32_p]
@@ -467,6 +469,28 @@ def conv_log(reset: bool = False) -> list:
         e["tiles_per_cta"] = -(-e["n_tiles"] // e["grid_x"])
         out.append(e)
     return out
+
+
+TILE_FAMILIES = ("consecutive", "real", "iso", "rep")
+TILE_CONFIGS = ("t1_fp16x3", "plain_fp16x3", "t1_fp16", "plain_fp16")
+
+
+def tile_families(handle, level: int, fin: int, fout: int) -> dict:
+    """Debug: a model handle's tile families on `level` (p2m_debug_tile_families, host only).  Returns
+    {family: {128: d, 64: d}} for the TILE_FAMILIES, d = {"n_pattern", "max_h1", "stride"} plus, per TILE_CONFIGS
+    name, the (output columns per CTA, ring slots, X stages) a conv fin -> fout would launch with on those tiles
+    ((0, 0, 0): does not fit, or not the tile size the conv runs on)."""
+    out = (C.c_int32 * 120)()
+    check(load().p2m_debug_tile_families(handle, level, fin, fout, out), "tile_families")
+    res = {}
+    for f, fam in enumerate(TILE_FAMILIES):
+        res[fam] = {}
+        for k, tm in enumerate((128, 64)):
+            o = out[(2 * f + k) * 15:(2 * f + k + 1) * 15]
+            d = dict(n_pattern=o[0], max_h1=o[1], stride=o[2])
+            d.update({name: tuple(o[3 + 3 * c:6 + 3 * c]) for c, name in enumerate(TILE_CONFIGS)})
+            res[fam][tm] = d
+    return res
 
 
 def check(status: int, what: str = "p2m call"):

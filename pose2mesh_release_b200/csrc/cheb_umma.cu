@@ -1846,6 +1846,13 @@ ConvCfg conv_cfg(int NC, const TileBlobs& t, bool t1_given, bool f16) {
       if (conv_smem(NC, ns, xs, t1_given, t.max_h1, t.stride, f16).bytes <= SMEM_LIMIT) return {ns, xs};
   return {0, 0};
 }
+// A tile family the conv can run on with N accumulator columns per MMA warpgroup (64: its 128-row tiles, 128: its
+// 64-row tiles): the T1-given conv and the plain GEMM both fit one ring of 3 and one X stage at fp16x3, whose slots
+// are twice the single-pass fp16 ones, and k_cheb_t1 stages its rows (at most 256)
+bool conv_family_fits(const TileBlobs& t, int N) {
+  return t.n_pattern > 0 && t.max_h1 <= 256 && conv_smem(N, 3, 1, 1, t.max_h1, t.stride).bytes <= SMEM_LIMIT &&
+         conv_smem(N, 3, 1, 0, t.max_h1, t.stride).bytes <= SMEM_LIMIT;
+}
 // Output columns per CTA of a conv Fin -> Fout on tiles t.  The 64 x 256 mode builds each A block once for all 256
 // columns, but its two warpgroups finish a tile together, so each tile's epilogue runs behind its main loop instead of
 // under the other warpgroup's: that pays where the main loop is long, the T1-given 256 -> 256 conv (24 K-blocks per
@@ -1914,19 +1921,18 @@ int check_launch_regs() {
   return P2M_OK;
 }
 
-// a.plain selects the instantiation: MODE 0 (plain GEMM) or MODE 1 (T1 given); NC output columns per CTA; F16 the
-// single-pass fp16 precision (a.f16)
-template <int NC, int NS, int XS, bool F16>
+// MODE 0 (plain GEMM, a.plain) or MODE 1 (T1 given); NC output columns per CTA; F16 the single-pass fp16 precision
+// (a.f16)
+template <int NC, int NS, int XS, int MODE, bool F16>
 int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
   constexpr int N = NC == CONV_N ? CONV_N : WIDE_N;
   constexpr int TM = tile_rows<N>();
   const DevLevel& g = *a.g;
   const TileBlobs& t = conv_tiles(N, g, a.tiles);
-  const size_t smem = conv_smem(NC, NS, XS, !a.plain, t.max_h1, t.stride, F16).bytes;
-  constexpr int M0 = NC == PAIR_N ? 1 : 0;  // MODE of a plain launch (the 64 x 256 mode has none: conv_cols)
-  auto kern = a.plain ? conv_kernel<NC, NS, XS, M0, F16>() : conv_kernel<NC, NS, XS, 1, F16>();
+  const size_t smem = conv_smem(NC, NS, XS, MODE, t.max_h1, t.stride, F16).bytes;
+  auto kern = conv_kernel<NC, NS, XS, MODE, F16>();
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  P2M_TRY((a.plain ? check_launch_regs<NC, NS, XS, M0, F16>() : check_launch_regs<NC, NS, XS, 1, F16>()));
+  P2M_TRY((check_launch_regs<NC, NS, XS, MODE, F16>()));
   KParams p;
   p.x = a.x;
   p.in_unpool = a.in_unpool;
@@ -1979,9 +1985,31 @@ int launch_cfg(const UmmaConvArgs& a, int* status, const float* zero_row, int sm
   const int n_slices = a.fout / NC;
   const dim3 grid(std::min(p.n_tiles, std::max(1, sm_count / n_slices)), n_slices);
   kern<<<grid, ConvRoles<N>::threads, smem, s>>>(p);
-  log_tc_launch(TC_CONV, NC, NS, XS, a.plain ? M0 : 1, F16, grid, p.n_tiles);
+  log_tc_launch(TC_CONV, NC, NS, XS, MODE, F16, grid, p.n_tiles);
   P2M_LAUNCH_OK();
   return P2M_OK;
+}
+
+// The instantiations launch_n can select.  Every family a conv runs on fits one ring of 3 fp16x3 slots with one stage
+// (umma_conv_supported, build_umma_level_meta), and six fp16 slots take no more (6 (64 + 128) 64 B = 3 (64 + 128) 128 B;
+// the barrier map's 48 B more fit the 64 B that conv_smem's fixed terms leave below any multiple of 128): at fp16 the
+// 64 x 128 ring is always 6.  The single-pass fp16 plain GEMM runs only on the isolated rows' tiles (their own rows,
+// one CSR entry each: blobs of at most 2176 B), where the deepest ring and both X stages fit.  The 64 x 256 mode is
+// T1-given only (conv_cols).
+template <int NC, int NS, int XS, int MODE, bool F16>
+constexpr bool launchable() {
+  if (MODE == 0 && (NC == PAIR_N || (F16 && (XS != 2 || NS != (NC == WIDE_N ? 6 : 3))))) return false;
+  return !(F16 && NC == WIDE_N && NS != 6);
+}
+template <int NC, int NS, int XS, bool F16>
+int launch_mode(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_count, cudaStream_t s) {
+  if (a.plain) {
+    if constexpr (launchable<NC, NS, XS, 0, F16>()) return launch_cfg<NC, NS, XS, 0, F16>(a, status, zero_row, sm_count, s);
+  } else {
+    if constexpr (launchable<NC, NS, XS, 1, F16>()) return launch_cfg<NC, NS, XS, 1, F16>(a, status, zero_row, sm_count, s);
+  }
+  set_error("umma_conv: no kernel instantiation for this tile family's shared-memory configuration");
+  return P2M_ERR_INVALID;
 }
 
 template <bool F16>
@@ -1995,16 +2023,16 @@ int launch_n(const UmmaConvArgs& a, int* status, const float* zero_row, int sm_c
     return P2M_ERR_INVALID;
   }
   if (NC == PAIR_N)
-    return c.xs == 2 ? launch_cfg<PAIR_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
-                     : launch_cfg<PAIR_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
+    return c.xs == 2 ? launch_mode<PAIR_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
+                     : launch_mode<PAIR_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
   if (N == CONV_N)
-    return c.xs == 2 ? launch_cfg<CONV_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
-                     : launch_cfg<CONV_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
+    return c.xs == 2 ? launch_mode<CONV_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
+                     : launch_mode<CONV_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
   if (c.ns == 6)
-    return c.xs == 2 ? launch_cfg<WIDE_N, 6, 2, F16>(a, status, zero_row, sm_count, s)
-                     : launch_cfg<WIDE_N, 6, 1, F16>(a, status, zero_row, sm_count, s);
-  return c.xs == 2 ? launch_cfg<WIDE_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
-                   : launch_cfg<WIDE_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
+    return c.xs == 2 ? launch_mode<WIDE_N, 6, 2, F16>(a, status, zero_row, sm_count, s)
+                     : launch_mode<WIDE_N, 6, 1, F16>(a, status, zero_row, sm_count, s);
+  return c.xs == 2 ? launch_mode<WIDE_N, 3, 2, F16>(a, status, zero_row, sm_count, s)
+                   : launch_mode<WIDE_N, 3, 1, F16>(a, status, zero_row, sm_count, s);
 }
 
 }  // namespace
@@ -2174,10 +2202,14 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
       }
     }
     out->n_iso = 0;
+    // the families are kept only where every conv a layer of any width can launch on them fits, as on the consecutive
+    // tiles (umma_conv_supported): connected rows packed 128 to a tile have larger halos and blobs than the
+    // consecutive tiles, which hold the isolated rows too.  Otherwise the level runs on the consecutive tiles.
+    auto fits = [](const TileSet& t) { return conv_family_fits(t, CONV_N) && conv_family_fits(t.m64, WIDE_N); };
     if (uniform && (int)iso_rows.size() >= TILE_M && (int)real_rows.size() >= TILE_M) {
       TileSet rt, it;
       if (build_tileset(real_rows, rowptr, colidx, val, V, &rt, owned) == P2M_OK &&
-          build_tileset(iso_rows, rowptr, colidx, val, V, &it, owned) == P2M_OK && rt.max_h1 <= 256) {
+          build_tileset(iso_rows, rowptr, colidx, val, V, &it, owned) == P2M_OK && fits(rt) && fits(it)) {
         out->real_tiles = rt;
         out->iso_tiles = it;
         out->n_iso = (int)iso_rows.size();
@@ -2291,9 +2323,35 @@ bool umma_conv_supported(const DevLevel& g, int fin, int fout) {
   if (g.meta128.max_h1 > 256) return false;  // k_cheb_t1 keeps <= 4 staged rows per row group
   if (fout != 64 && fout != 128 && fout != 256) return false;
   const int N = conv_n(fout);
-  const TileBlobs& t = conv_tiles(N, g, nullptr);
-  return t.n_pattern > 0 && conv_smem(N, 3, 1, 1, t.max_h1, t.stride).bytes <= SMEM_LIMIT &&
-         conv_smem(N, 3, 1, 0, t.max_h1, t.stride).bytes <= SMEM_LIMIT;
+  return conv_family_fits(conv_tiles(N, g, nullptr), N);
+}
+
+int umma_tile_families(const DevLevel& g, int fin, int fout, int32_t out[4][2][15]) {
+  if (fin % FC != 0 || fin < FC || fin > 256 || (fout != 64 && fout != 128 && fout != 256)) return P2M_ERR_INVALID;
+  const TileBlobs* fams[4][2] = {{&g.meta128, &g.meta64},
+                                 {&g.real_tiles, &g.real_tiles.m64},
+                                 {&g.iso_tiles, &g.iso_tiles.m64},
+                                 {&g.rep_tiles, &g.rep_tiles.m64}};
+  const int N = conv_n(fout);
+  for (int f = 0; f < 4; ++f)
+    for (int k = 0; k < 2; ++k) {
+      const TileBlobs& t = *fams[f][k];
+      int32_t* o = out[f][k];
+      std::fill(o, o + 15, 0);
+      o[0] = t.n_pattern;
+      o[1] = t.max_h1;
+      o[2] = t.stride;
+      if (t.n_pattern <= 0 || (k == 0) != (N == CONV_N)) continue;  // only the tile size a conv to fout runs on
+      for (int c = 0; c < 4; ++c) {  // T1-given fp16x3, plain fp16x3, T1-given fp16, plain fp16
+        const bool t1_given = (c & 1) == 0, f16 = c >= 2;
+        const int NC = conv_cols(fin, fout, t, t1_given, f16);
+        const ConvCfg cfg = conv_cfg(NC, t, t1_given, f16);
+        o[3 + 3 * c] = cfg.ns > 0 ? NC : 0;
+        o[4 + 3 * c] = cfg.ns;
+        o[5 + 3 * c] = cfg.xs;
+      }
+    }
+  return P2M_OK;
 }
 
 // What launch_n picks for a conv Fin -> Fout on the level's consecutive tiles (T1 given, or plain): its X staging

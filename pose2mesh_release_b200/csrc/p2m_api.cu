@@ -947,6 +947,15 @@ int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, in
   return P2M_OK;
 }
 
+int p2m_debug_tile_families(const p2m_model_t* m, int level, int fin, int fout, int32_t out[120]) {
+  if (!m || !out || level < 0 || level >= (int)m->levels.size() ||
+      umma_tile_families(m->levels[level], fin, fout, reinterpret_cast<int32_t(*)[2][15]>(out)) != P2M_OK) {
+    set_error("debug_tile_families: bad argument");
+    return P2M_ERR_INVALID;
+  }
+  return P2M_OK;
+}
+
 int p2m_debug_layer_route(const p2m_model_t* m, int layer, int batch, int need_dx, int32_t out[9]) {
   if (!m || !out || layer < 0 || layer >= (int)m->layers.size() || batch <= 0) {
     set_error("debug_layer_route: bad argument");

@@ -476,6 +476,11 @@ struct UmmaConvTiling {
   int cols, ns, xs;  // output columns per CTA (64, 128 or 256), A/B ring slots, X / T1 stages (0: does not fit)
 };
 UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain, bool f16 = false);
+// p2m_debug_tile_families: per family (consecutive, real_tiles, iso_tiles, rep_tiles) and tile size (128, 64 rows)
+// n_pattern, max_h1, blob stride, then (columns per CTA, ring slots, X stages) of what launch_n picks for a conv
+// fin -> fout on it: T1-given and plain at fp16x3, T1-given and plain at fp16 ({0, 0, 0}: does not fit, or not the
+// tile size fout runs on)
+int umma_tile_families(const DevLevel& g, int fin, int fout, int32_t out[4][2][15]);
 int umma_dw_x_stages(const DevLevel& g);
 bool umma_tma_rows(const DevLevel& g);
 // Weight images of a conv: fp16 [hi | lo] K-blocks of 32 k (x 2^6) from W [fout, fin*3] in the reference layout (column

@@ -146,6 +146,95 @@ def nonsymmetric(V=256, seed=0):
     return out
 
 
+def padded(V, real, edges):
+    """V rows whose connected rows are `real` (ascending) joined by `edges` (pairs of positions in `real`), every other
+    row isolated: one uniform diagonal, so padding elision builds its index-list tile families (DevLevel::real_tiles
+    packs the connected rows 128 and 64 to a tile, iso_tiles the isolated ones)."""
+    real = np.asarray(real)
+    e = np.asarray(edges, dtype=np.int64).reshape(-1, 2)
+    L = rescaled_laplacian(_edges_to_adj(V, real[e]))
+    # isolated rows at 0.25, not 2 / lmax - 1: that is 0 (no entry at all) where the connected rows are bipartite
+    iso = np.ones(V, dtype=bool)
+    iso[real] = False
+    L = sp.csr_matrix(L + sp.diags(np.where(iso, 0.25 - L.diagonal(), 0.0)))
+    L.eliminate_zeros()
+    L.sort_indices()
+    return L
+
+
+def pair_rows(V, n_real):
+    """n_real connected rows of a padded level of V rows, the isolated ones in sibling pairs (2p, 2p + 1) spread evenly
+    (an odd count: the last connected row isolated too): every 128-row tile of consecutive rows holds about the level's
+    share of isolated rows, so the consecutive tiles stay small where the connected rows packed 128 to a tile do not."""
+    n_iso = V - n_real
+    iso = np.zeros(V // 2, dtype=bool)
+    iso[(np.arange(n_iso // 2) * (V // 2)) // max(n_iso // 2, 1)] = True
+    real = np.flatnonzero(~np.repeat(iso, 2))
+    return real[:-1] if n_iso % 2 else real
+
+
+def real_path_far(V, n_far):
+    """Half the rows isolated (pair_rows); the connected ones a path in row order, the first n_far joined to the last
+    n_far: the first connected-row tile stages 128 own rows, the next one and n_far far ones (max_h1 = 129 + n_far)."""
+    real = pair_rows(V, V // 2)
+    n = len(real)
+    e = [(i, i + 1) for i in range(n - 1)] + [(i, n - 1 - i) for i in range(n_far)]
+    return padded(V, real, e)
+
+
+def real_cliques(V, c):
+    """Half the rows isolated (pair_rows); the connected ones in cliques of c consecutive ones and a path through all: a
+    connected-row tile holds ~128 c CSR entries, a consecutive tile only its share of connected rows' (half as many)."""
+    real = pair_rows(V, V // 2)
+    n = len(real)
+    e = [(i, i + 1) for i in range(n - 1)]
+    for b0 in range(0, n, c):
+        blk = np.arange(b0, min(n, b0 + c))
+        a, b = np.meshgrid(blk, blk)
+        e += list(zip(a.ravel(), b.ravel()))
+    return padded(V, real, e)
+
+
+def real_count(V, n_real):
+    """n_real connected rows (pair_rows; a path with chords of 7), the others isolated: the last connected-row tile is
+    ragged unless n_real is a multiple of its tile size."""
+    real = pair_rows(V, n_real)
+    return padded(V, real, path_chords(len(real)))
+
+
+def elision_hierarchy(level0, joints=17):
+    """A MeshNet Laplacian list around one padded level: level0 (V rows), a level of V / 2 rows whose row p is
+    connected iff row 2p or 2p + 1 of level0 is (so both children of an isolated row are isolated: the eval forward's
+    dedup classes exist), its connected rows a path with chords of 7, and a joint graph of `joints` rows (a path)."""
+    V = level0.shape[0]
+    L0 = sp.csr_matrix(level0)
+    iso0 = (np.diff(L0.indptr) == 1) & (L0.indices[L0.indptr[:-1]] == np.arange(V))
+    real1 = np.flatnonzero(~(iso0[0::2] & iso0[1::2]))
+    level1 = padded(V // 2, real1, path_chords(len(real1)))
+    return [level0, level1, sized(joints)]
+
+
+# MeshNet channels around an elision hierarchy (levels V, V / 2, joint): the padded level runs 128 -> 256 (two
+# 128-column slices), 256 -> 256 (the 64 x 256 mode), 256 -> 64 (128 x 64), 64 -> 128 and the 128 -> 64 -> 3 head
+ELISION_PLAN = [(5, 32, 64), (64, 128), (128, 256, 256, 64, 128), (128, 64, 3)]
+
+# name -> (builder, what the padded level's index-list tiles target): every level has >= 128 isolated rows with one
+# diagonal (tests/test_gpu_elision_tiles_fp64.py builds a MeshNet around it with elision_hierarchy)
+ELISION = {
+    "el_h1_256": (lambda: real_path_far(1024, 127), "connected-row tiles stage 256 rows: the max_h1 limit"),
+    "el_h1_257": (lambda: real_path_far(1024, 128), "257 staged rows: no families, the level runs on consecutive tiles"),
+    "el_clique24": (lambda: real_cliques(1024, 24), "64-row connected-row blobs: the 64 x 128 ring of 6, one T1 stage"),
+    "el_clique40": (lambda: real_cliques(1024, 40), "the 64 x 128 ring of 3, 64 x 256 and 128 x 64 with one T1 stage"),
+    "el_clique48": (lambda: real_cliques(1024, 48), "128-row connected-row blobs that fit no ring: no families"),
+    "el_ragged": (lambda: real_count(1024, 600), "600 connected rows: the last tile ragged at 128 and at 64 rows"),
+    "el_real128": (lambda: real_count(512, 128), "exactly one 128-row connected-row tile"),
+    "el_real129": (lambda: real_count(512, 129), "129 connected rows: a second tile of one row"),
+    **{f"el_iso{n}": ((lambda n=n: real_count(640, 640 - n)), f"{n} isolated rows of 640: 5 n_iso vs 2 V")
+       for n in (255, 256, 257)},
+    "el_rows2w": (lambda: real_count(256, 128), "V = 256: B V vs 2 width for the 256-wide convs"),
+}
+
+
 # name -> (builder, branch)
 FAMILIES = {
     **{f"V{V}": ((lambda V=V: sized(V)), "ragged last tile / V < 128 / TMA (V % 128 == 0) vs cp.async rows")
@@ -180,6 +269,12 @@ _cache = {}
 def get(name: str) -> sp.csr_matrix:
     if name not in _cache:
         _cache[name] = FAMILIES[name][0]()
+    return _cache[name]
+
+
+def elision(name: str) -> sp.csr_matrix:
+    if name not in _cache:
+        _cache[name] = ELISION[name][0]()
     return _cache[name]
 
 

@@ -18,6 +18,7 @@ import pytest
 import torch
 
 import fp64_ref as R
+import graphs as G
 from helpers import CASES, graph_from_fixture
 
 pytestmark = pytest.mark.gpu
@@ -62,6 +63,8 @@ def npy(t):
 
 # ------------------------------------------------------------------------------------------------------------- nets
 def net_levels(name):
+    if name in G.ELISION:   # a padded level and its hierarchy (tests/test_gpu_elision_tiles_fp64.py)
+        return G.elision_hierarchy(G.elision(name)), G.ELISION_PLAN
     if name == "custom":
         mats = graph_from_fixture("smpl_small")[0]
         return [next(m for m in mats if m.shape[0] == V) for V in (128, 64, 17)], CUSTOM_PLAN
@@ -181,8 +184,9 @@ def residual(net, li, block_in, ref=R):
 
 
 # ----------------------------------------------------------------------------------------------------------- running
-def forward_train_backward(net, x, tgt, need_dx=True):
-    """One train-mode forward + L1 loss + backward with every tensor captured.  Returns (cap, grads, buffers, y)."""
+def forward_train_backward(net, x, tgt, need_dx=True, loss_fn=None):
+    """One train-mode forward + L1 loss (or loss_fn(y, tgt)) + backward with every tensor captured.  Returns (cap,
+    grads, buffers, y)."""
     from pose2mesh_release_b200.meshnet import _MeshNetFunction
 
     B = x.shape[0]
@@ -206,7 +210,7 @@ def forward_train_backward(net, x, tgt, need_dx=True):
     try:
         xg = cuda(x).requires_grad_(need_dx)
         y = _MeshNetFunction.apply(xg, net.hier, True, buffers, n, *[p[k] for k in names])
-        loss = (y - cuda(tgt)).abs().mean()
+        loss = (y - cuda(tgt)).abs().mean() if loss_fn is None else loss_fn(y, cuda(tgt))
         loss.backward()
         torch.cuda.synchronize()
     finally:

@@ -341,8 +341,8 @@ def test_train_network_capped(name, need_dx):
 #   Every other term is a multiple of 128 B, and the fixed small ones (barriers at NS = 3, XS = 1: 112; flags 16;
 #   residual mbarriers 32; slack 1184) sum to 1344 = 64 mod 128, so conv_smem(128, 3, 1, MODE) <= 227 KB, which
 #   umma_conv_supported requires at fp16x3, means <= 227 KB - 64, and six fp16 slots with one stage fit with 16 B to
-#   spare: conv_cfg never goes below six.  Only the padding elision's index-list tiles (DevLevel::real_tiles) escape
-#   this argument: conv_route does not hold them to umma_conv_supported's limit.
+#   spare: conv_cfg never goes below six.  build_umma_level_meta holds the padding elision's index-list tiles to the
+#   same limit, so those instantiations are not built (cheb_umma.cu: launchable).
 REACHABLE = {
     ("conv", 64, 3, 2, 1, 0), ("conv", 64, 3, 1, 1, 0), ("conv", 128, 6, 2, 1, 0), ("conv", 128, 6, 1, 1, 0),
     ("conv", 128, 3, 2, 1, 0), ("conv", 128, 3, 1, 1, 0), ("conv", 256, 3, 2, 1, 0), ("conv", 256, 3, 1, 1, 0),
