@@ -39,7 +39,8 @@ enum p2m_status {
 enum p2m_precision {
   P2M_PREC_FP32_SIMT = 0, /* fp32 FFMA on CUDA cores (all shapes; the parity baseline)          */
   P2M_PREC_FP16X3_TC = 1, /* wgmma f16 -> f32, error-compensated 3-term fp16 split (~2^-21) */
-  P2M_PREC_FP16_TC = 2    /* inference only: single-pass wgmma, fp16 operands, fp32 accumulate   */
+  P2M_PREC_FP16_TC = 2,   /* inference only: single-pass wgmma, fp16 operands, fp32 accumulate   */
+  P2M_PREC_FP16_MIXED_TC = 3 /* mixed-precision training: single-pass wgmma in forward and backward */
 };
 /* P2M_PREC_FP16_TC: the Chebyshev convs of the eval forward round both operands to the nearest fp16 (activations
  * unscaled, weights x 2^6) and accumulate in fp32: one MMA per 16 features instead of three, a per-product relative
@@ -48,6 +49,13 @@ enum p2m_precision {
  * schedule, p2m_meshnet_forward_vertices, p2m_meshnet_forward_host (and _vertices_host) and p2m_cheb_conv_fwd (bn_mode
  * 0 or 1).  The training schedule (training = 1, or BatchNorm options that select it), p2m_meshnet_backward(_opts),
  * p2m_cheb_conv_bwd and p2m_cheb_conv_fwd with bn_mode 2 return P2M_ERR_INVALID before any device work.            */
+/* P2M_PREC_FP16_MIXED_TC: fp16 operands, fp32 accumulation, fp32 master weights and fp32 BatchNorm, for training.  The
+ * eval forward runs exactly the kernels of P2M_PREC_FP16_TC (bitwise equal outputs).  In the training forward and the
+ * backward every Chebyshev-conv pass that runs on the tensor cores at fp16x3 runs single-pass instead: the forward
+ * convs (with the padding elision's index-list tiles and isolated-row GEMM), backward-data (the conv on dz, its
+ * isolated-row GEMM, or the three dT GEMMs; dz scaled into fp16's range by a power of two found on the device) and the
+ * weight gradient (k_cheb_dw_f16_umma).  Each pass runs where it runs at fp16x3 (the same routes).  The fc keeps its
+ * fp16x3 dense GEMM, the thin layers their CUDA-core kernels and PoseNet its fp16x3 GEMMs.  Every entry point accepts it. */
 
 /* ---- the fixed mesh hierarchy + channel plan ---------------------------------------------------
  * Replaces what Pose2Mesh.__init__ derives from graph_L (meshnet.py:17-37,61-62): `n_levels`
@@ -89,6 +97,7 @@ void p2m_model_destroy(p2m_model_t* m);
 int p2m_model_num_layers(const p2m_model_t* m);
 /* layer geometry: out[0]=level index, [1]=V, [2]=Fin, [3]=Fout, [4]=has_bn, [5]=relu */
 int p2m_model_layer_info(const p2m_model_t* m, int layer, int32_t out[6]);
+/* precision: a P2M_PREC_* value: fp32, fp16x3 (the default), fp16 (inference only) or fp16_mixed (training too) */
 int p2m_model_set_precision(p2m_model_t* m, int precision);
 /* Profiling: when enabled, the eval forward records a CUDA event pair (on the caller's stream) around
  * every conv layer; p2m_model_layer_times_ms returns the last forward's per-layer device times.      */

@@ -17,14 +17,19 @@ LIB_PATH = os.path.join(_HERE, "libp2m_b200.so")
 P2M_PREC_FP32_SIMT = 0
 P2M_PREC_FP16X3_TC = 1
 P2M_PREC_FP16_TC = 2  # inference only: single-pass fp16 operands in the Chebyshev convs (include/p2m_b200.h)
-PRECISIONS = {"fp32": P2M_PREC_FP32_SIMT, "fp16x3": P2M_PREC_FP16X3_TC, "fp16": P2M_PREC_FP16_TC}
+P2M_PREC_FP16_MIXED_TC = 3  # training too: single-pass fp16 in the forward, backward-data and weight-gradient convs
+PRECISIONS = {"fp32": P2M_PREC_FP32_SIMT, "fp16x3": P2M_PREC_FP16X3_TC, "fp16": P2M_PREC_FP16_TC,
+              "fp16_mixed": P2M_PREC_FP16_MIXED_TC}
 
 
 def default_precision() -> int:
     """Precision of new modules / graph handles: the tensor-core path (fp16x3: error-compensated split, fp32
     accumulate, 1e-4 parity like the fp32 path) unless the environment says ``P2M_PRECISION=fp32`` (the CUDA-core
-    escape hatch for activations beyond fp16's range).  A drop-in user (install.py) therefore gets the fast path
-    without touching the module; ``Pose2Mesh.set_precision`` / ``set_default_precision`` still override it."""
+    escape hatch for activations beyond fp16's range), ``P2M_PRECISION=fp16`` (single-pass fp16 Chebyshev convs,
+    inference only) or ``P2M_PRECISION=fp16_mixed`` (single-pass fp16 in the training forward and backward as well:
+    fp16 operands, fp32 accumulation, fp32 weights and BatchNorm).  A drop-in user (install.py) therefore gets the
+    fast path without touching the module; ``Pose2Mesh.set_precision`` / ``set_default_precision`` still override
+    it."""
     name = os.environ.get("P2M_PRECISION", "fp16x3").strip().lower()
     if name not in PRECISIONS:
         raise RuntimeError(f"P2M_PRECISION={name!r}: expected one of {sorted(PRECISIONS)}")

@@ -23,8 +23,9 @@ _default_precision = _lib.default_precision()
 
 
 def set_default_precision(precision: str):
-    """'fp32' (CUDA cores), 'fp16x3' (wgmma tensor cores) or 'fp16' (single-pass wgmma, inference only: a backward or a
-    training-mode BatchNorm raises) for graph_conv_cheby calls."""
+    """'fp32' (CUDA cores), 'fp16x3' (wgmma tensor cores), 'fp16' (single-pass wgmma, inference only: a backward or a
+    training-mode BatchNorm raises) or 'fp16_mixed' (single-pass wgmma in the forward and the backward, for mixed-
+    precision training) for graph_conv_cheby calls."""
     global _default_precision
     _default_precision = _lib.PRECISIONS[precision]
     for _, gh in list(_graph_cache.values()):

@@ -529,9 +529,10 @@ __host__ __device__ __forceinline__ ConvSmem conv_smem(int NC, int NS, int XS, i
 // and register targets (ConvRoles<N>) and in their launch size.  NC = output columns per CTA: N, or 2 N (64 x 256,
 // k_cheb_conv_wide only), where both MMA warpgroups work on every tile, warpgroup g on the CTA's columns
 // [g N, g N + N), and read the one A block the producers built for them.
-// F16: the single-pass fp16 precision (P2M_PREC_FP16_TC, inference): a K-block holds only the fp16 round-to-nearest of
-// each operand (64-byte rows, 64B-swizzled) and every 16 features take one k16 MMA instead of three.  Same chunks, slots
-// and barrier protocol; T1-given and plain convs of the eval forward only (no dense-GEMM mode, no a_scale).
+// F16: the single-pass fp16 precisions (P2M_PREC_FP16_TC, P2M_PREC_FP16_MIXED_TC): a K-block holds only the fp16
+// round-to-nearest of each operand (64-byte rows, 64B-swizzled) and every 16 features take one k16 MMA instead of three.
+// Same chunks, slots and barrier protocol; T1-given and plain convs (a_scale applied before the rounding), no dense-GEMM
+// mode.
 template <int N, int NC, int NS, int XS, int MODE, bool F16>
 __device__ __forceinline__ void cheb_conv_body(const KParams& p) {
   static_assert(N == 64 || N == 128, "one warpgroup holds the CTA's 128 x 64 or 64 x 128 accumulator in registers");
@@ -1276,7 +1277,7 @@ template <int NC, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS_W, 1) k_cheb_conv_wide(const __grid_constant__ KParams p) {
   cheb_conv_body<128, NC, NS, XS, MODE, false>(p);
 }
-// The same two configurations at the single-pass fp16 precision (P2M_PREC_FP16_TC): one body, F16 = true
+// The same two configurations at the single-pass fp16 precisions (fp16, fp16_mixed): one body, F16 = true
 template <int N, int NS, int XS, int MODE>
 __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_conv_f16_umma(const __grid_constant__ KParams p) {
   static_assert(N == 64, "the 64 x 128 configuration is k_cheb_conv_f16_wide");
@@ -1340,19 +1341,37 @@ __device__ __forceinline__ uint64_t make_desc_sw128_mn(uint32_t saddr, uint32_t 
   return d;
 }
 
+// The single-pass fp16 weight gradient (k_cheb_dw_f16_umma, P2M_PREC_FP16_MIXED_TC) keeps the chunks, ring, barriers
+// and producers, and stores only the fp16 round-to-nearest of each operand: a T block is 128 rows x 32 fp16 = 64-byte
+// rows, the canonical MN-major SWIZZLE_64B tile (8-row K groups of 512 bytes, N = 32 = one swizzle atom), and the
+// plain-side tile is the hi block of its 64 channels alone (128-byte rows, MN-major SWIZZLE_128B as above).  Each
+// 16-row K step issues one wgmma.m64n32k16 (g T) where fp16x3 issues three.
+__device__ __forceinline__ uint64_t make_desc_sw64_mn(uint32_t saddr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
+  d |= (uint64_t)(8192 >> 4) << 16;  // LBO: distance between 32-element MN groups (N = 32: only one is read)
+  d |= (uint64_t)(512 >> 4) << 32;   // SBO: distance between 8-row K groups
+  d |= (uint64_t)2 << 62;            // SWIZZLE_64B
+  return d;
+}
+
 constexpr int DW_NS = 3;
 constexpr int DW_G_BYTES = 4 * A_BLOCK_BYTES;  // dz tile: (hi, lo) x two 64-channel groups
+// bytes of one ring slot (a T block) and of the plain-side tile; f16: the single-pass layout
+__host__ __device__ constexpr int dw_t_bytes(bool f16) { return f16 ? TILE_M * 64 : A_BLOCK_BYTES; }
+__host__ __device__ constexpr int dw_g_bytes(bool f16) { return f16 ? A_BLOCK_BYTES : DW_G_BYTES; }
 
-// k_cheb_dw_umma<XS> on the level's 128-row tiles (at most max_h1 staged rows, blobs meta_stride bytes apart)
+// k_cheb_dw_umma<XS> (k_cheb_dw_f16_umma<XS>: f16) on the level's 128-row tiles (at most max_h1 staged rows, blobs
+// meta_stride bytes apart)
 struct DwSmem {
   size_t gblk, xs, t1s, t1_stage, meta, bars, flags, bytes;
 };
-__host__ __device__ __forceinline__ DwSmem dw_smem(int XS, int max_h1, int meta_stride) {
+__host__ __device__ __forceinline__ DwSmem dw_smem(int XS, int max_h1, int meta_stride, bool f16 = false) {
   size_t at = 0;
   auto take = [&](size_t bytes) { at += bytes; return at - bytes; };
   DwSmem L;
-  take(DW_NS * A_BLOCK_BYTES);                // the ring at offset 0: [DW_NS] T blocks
-  L.gblk = take(DW_G_BYTES);                  // dz tile blocks: hi g0, hi g1, lo g0, lo g1
+  take(DW_NS * (size_t)dw_t_bytes(f16));      // the ring at offset 0: [DW_NS] T blocks
+  L.gblk = take(dw_g_bytes(f16));             // dz tile blocks: hi g0, hi g1, lo g0, lo g1 (f16: hi g0)
   L.xs = take(XS * (size_t)TILE_M * FC * 4);  // [XS][128][32] fp32: the tile's own rows of x
   L.t1_stage = (size_t)max_h1 * FC;           // [XS][max_h1][32] fp32: T1 rows of the tile and its 1-hop halo
   L.t1s = take(XS * L.t1_stage * 4);
@@ -1363,10 +1382,12 @@ __host__ __device__ __forceinline__ DwSmem dw_smem(int XS, int max_h1, int meta_
   return L;
 }
 
-template <int XS>
-__global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_constant__ DwParams p) {
+// The body of both dW kernels: k_cheb_dw_umma (fp16x3) and k_cheb_dw_f16_umma (F16: the single-pass layout above)
+template <int XS, bool F16>
+__device__ __forceinline__ void cheb_dw_body(const DwParams& p) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  const DwSmem L = dw_smem(XS, p.max_h1, p.meta_stride);
+  const DwSmem L = dw_smem(XS, p.max_h1, p.meta_stride, F16);
+  constexpr int T_BYTES = dw_t_bytes(F16);
   unsigned char* ring = smem_raw;                      // [DW_NS] T blocks
   unsigned char* gblk = smem_raw + L.gblk;
   float* Xs = reinterpret_cast<float*>(smem_raw + L.xs);
@@ -1511,13 +1532,21 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
       for (int k = 0; k < 3; ++k, ++ucnt) {
         const int s = ucnt % DW_NS;
         mbar_wait(smem_u32(b_t_full + s), (ucnt / DW_NS) & 1, abort_flag, p.status, 25);
-        const uint64_t dt = make_desc_sw128_mn(smem_u32(ring + s * A_BLOCK_BYTES), A_BLOCK_BYTES);
-        wg_fence();
+        if constexpr (F16) {
+          const uint64_t dt = make_desc_sw64_mn(smem_u32(ring + s * T_BYTES));
+          wg_fence();
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks) {  // 16 mesh rows per K step = 2048 bytes = +128 in the address field
-          wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 128);      // g_hi T_hi
-          wgmma_m64n32(acc[k], dl + ks * 128, dt + ks * 128);      // g_lo T_hi
-          wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 128 + 4);  // g_hi T_lo (+64 B)
+          for (int ks = 0; ks < 8; ++ks)  // 16 mesh rows: 2048 bytes of g (+128), 1024 bytes of T (+64)
+            wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 64);
+        } else {
+          const uint64_t dt = make_desc_sw128_mn(smem_u32(ring + s * A_BLOCK_BYTES), A_BLOCK_BYTES);
+          wg_fence();
+#pragma unroll
+          for (int ks = 0; ks < 8; ++ks) {  // 16 mesh rows per K step = 2048 bytes = +128 in the address field
+            wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 128);      // g_hi T_hi
+            wgmma_m64n32(acc[k], dl + ks * 128, dt + ks * 128);      // g_lo T_hi
+            wgmma_m64n32(acc[k], dh + ks * 128, dt + ks * 128 + 4);  // g_hi T_lo (+64 B)
+          }
         }
         wg_commit();
         wg_wait0();
@@ -1555,7 +1584,8 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
       // The plain-side tile goes global -> registers -> fp16 blocks.  Its loads are issued FIRST, so that their
       // latency overlaps the waits below (metadata, and above all g_empty: the previous tile's MMAs still read the
       // single-buffered plain blocks) instead of following them.
-      float4 pv[2][4];
+      constexpr int NJ = F16 ? 2 : 4;  // 32-channel pieces per row (F16: the 64 channels of the launch's slice only)
+      float4 pv[2][NJ];
       {
         const int n_rows = min(TILE_M, p.V - pat * TILE_M);
         const long long r_base = (long long)b * p.V + (long long)pat * TILE_M;
@@ -1563,7 +1593,7 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
         for (int ps = 0; ps < 2; ++ps) {
           const int i = ps * 64 + rg;
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
+          for (int jj = 0; jj < NJ; ++jj) {
             const int col = q * 4 + 32 * (jj ^ (rg & 1));
             pv[ps][jj] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (i < n_rows && col < p.m_cols) {
@@ -1592,13 +1622,17 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
         for (int ps = 0; ps < 2; ++ps) {
           const int i = ps * 64 + rg;
 #pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
+          for (int jj = 0; jj < NJ; ++jj) {
             // odd row groups take the 32-channel pieces in the order 1,0,3,2: the two rows of a half-warp then store
             // into different 64-byte bank halves (their swizzle bits agree: consecutive rows)
             const int col = q * 4 + 32 * (jj ^ (rg & 1));  // channel inside this launch's slice (< m_cols <= 64)
             float4 v = pv[ps][jj];
             if (!p.swap) {  // input role: this side is the gradient
               v.x *= a_scale; v.y *= a_scale; v.z *= a_scale; v.w *= a_scale;
+            }
+            if constexpr (F16) {  // the hi block alone
+              sts_u2(g_a + sw128_off(i, col >> 3) + ((col >> 2) & 1) * 8, half4(v));
+              continue;
             }
             uint2 hi, lo;
             split4(v, hi, lo);
@@ -1641,10 +1675,14 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
         for (int k = 0; k < 3; ++k, ++ucnt) {
           const int s = ucnt % DW_NS;
           mbar_wait(smem_u32(b_t_empty + s), ((ucnt / DW_NS) & 1) ^ 1, abort_flag, p.status, 30);
-          const uint32_t blk = ring_a + s * A_BLOCK_BYTES + (q & 1) * 8;
+          const uint32_t blk = ring_a + s * T_BYTES + (q & 1) * 8;
 #pragma unroll
           for (int ps = 0; ps < 2; ++ps) {
             const uint32_t i = ps ? row1 : row0;
+            if constexpr (F16) {  // one 8-byte piece per row, as in the conv's F16 producers
+              sts_u2(blk + sw64_off(i, q >> 1), half4(tv[k][ps]));
+              continue;
+            }
             uint2 hi, lo;
             split4(tv[k][ps], hi, lo);
             const uint32_t a_hi = blk + sw128_off(i, q >> 1), a_lo = blk + sw128_off(i, 4 + (q >> 1));
@@ -1667,6 +1705,16 @@ __global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_c
       }
     }
   }
+}
+
+template <int XS>
+__global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_umma(const __grid_constant__ DwParams p) {
+  cheb_dw_body<XS, false>(p);
+}
+// the single-pass fp16 weight gradient (P2M_PREC_FP16_MIXED_TC): one wgmma per K step
+template <int XS>
+__global__ void __launch_bounds__(NUM_THREADS2, 1) k_cheb_dw_f16_umma(const __grid_constant__ DwParams p) {
+  cheb_dw_body<XS, true>(p);
 }
 
 // =====================================================================================
@@ -2221,18 +2269,20 @@ int build_umma_level_meta(const int* rowptr, const int* colidx, const float* val
 }
 
 
-bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width) {
+bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width, bool f16) {
   if (g.meta128.n_pattern <= 0 || g.meta128.max_h1 > 256) return false;
   if (gathered_width % FC != 0 || gathered_width < FC || gathered_width > 256) return false;
   if (plain_width != 64 && plain_width != 128 && plain_width != 256) return false;
-  return dw_smem(1, g.meta128.max_h1, g.meta128.stride).bytes <= SMEM_LIMIT;
+  return dw_smem(1, g.meta128.max_h1, g.meta128.stride, f16).bytes <= SMEM_LIMIT;
 }
-int umma_dw_x_stages(const DevLevel& g) { return dw_smem(2, g.meta128.max_h1, g.meta128.stride).bytes <= SMEM_LIMIT ? 2 : 1; }
+int umma_dw_x_stages(const DevLevel& g, bool f16) {
+  return dw_smem(2, g.meta128.max_h1, g.meta128.stride, f16).bytes <= SMEM_LIMIT ? 2 : 1;
+}
 
 int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_unpool, int gathered_width,
                    const float* t1, const float* plain, int g_unpool, int plain_width, int swap, const float* a_scale,
-                   float* dw_ref, int* status, int sm_count, cudaStream_t s) {
-  if (!umma_dw_supported(g, gathered_width, plain_width) || t1 == nullptr) {
+                   float* dw_ref, int* status, int sm_count, cudaStream_t s, bool f16) {
+  if (!umma_dw_supported(g, gathered_width, plain_width, f16) || t1 == nullptr) {
     set_error("umma_dw: unsupported shape");
     return P2M_ERR_INVALID;
   }
@@ -2264,9 +2314,10 @@ int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_u
     p.tma = (make_row_tmap(&p.tm_x, gathered, rows, gathered_width, TILE_M) &&
              make_row_tmap(&p.tm_t1, t1, rows, gathered_width, TILE_M)) ? 1 : 0;
   }
-  const int xs = umma_dw_x_stages(g);
-  const size_t smem = dw_smem(xs, t.max_h1, t.stride).bytes;
-  auto kern = (xs == 2) ? k_cheb_dw_umma<2> : k_cheb_dw_umma<1>;
+  const int xs = umma_dw_x_stages(g, f16);
+  const size_t smem = dw_smem(xs, t.max_h1, t.stride, f16).bytes;
+  auto kern = f16 ? (xs == 2 ? k_cheb_dw_f16_umma<2> : k_cheb_dw_f16_umma<1>)
+                  : (xs == 2 ? k_cheb_dw_umma<2> : k_cheb_dw_umma<1>);
   P2M_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = std::min(p.n_tiles, sm_count);
   for (int m_off = 0; m_off < plain_width; m_off += 64) {
@@ -2275,7 +2326,7 @@ int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_u
     for (int c0 = 0; c0 < gathered_width / FC; ++c0) {  // one feature chunk per launch (the kernel's n_chunk)
       p.chunk0 = c0;
       kern<<<grid, NUM_THREADS2, smem, s>>>(p);
-      log_tc_launch(TC_DW, p.m_cols, DW_NS, xs, 1, 0, dim3(grid), p.n_tiles);
+      log_tc_launch(TC_DW, p.m_cols, DW_NS, xs, 1, f16 ? 1 : 0, dim3(grid), p.n_tiles);
       P2M_LAUNCH_OK();
     }
   }
@@ -2475,10 +2526,6 @@ int launch_umma_conv(const UmmaConvArgs& a, int* status, const float* zero_row, 
   if (a.tiles != nullptr && (a.tiles->max_h1 > 256 || a.tiles->n_pattern <= 0 ||
                              (a.fout % WIDE_N == 0 && a.tiles->m64.n_pattern <= 0))) {
     set_error("umma_conv: index-list tiles need at most 256 staged rows");
-    return P2M_ERR_INVALID;
-  }
-  if (a.f16 && a.plain && a.a_scale != nullptr) {
-    set_error("umma_conv: the single-pass fp16 plain GEMM has no operand scale (inference only)");
     return P2M_ERR_INVALID;
   }
   return a.f16 ? launch_n<true>(a, status, zero_row, sm_count, s) : launch_n<false>(a, status, zero_row, sm_count, s);

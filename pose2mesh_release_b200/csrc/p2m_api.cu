@@ -313,8 +313,13 @@ BwdMap map_scratch(const p2m_model* m, int B, void* base) {
 }
 
 // ---- which kernels run a Chebyshev conv
-// The precisions whose convs run on the tensor cores: fp16x3, and the single-pass fp16 (eval forward only)
-inline bool tc_precision(int precision) { return precision == P2M_PREC_FP16X3_TC || precision == P2M_PREC_FP16_TC; }
+// The precisions whose convs run on the tensor cores: fp16x3, the single-pass fp16 (eval forward only) and the
+// single-pass mixed precision (training as well)
+inline bool tc_precision(int precision) {
+  return precision == P2M_PREC_FP16X3_TC || precision == P2M_PREC_FP16_TC || precision == P2M_PREC_FP16_MIXED_TC;
+}
+// The precisions whose tensor-core Chebyshev passes issue one MMA per 16 features (fp16 operands rounded once)
+inline bool single_pass(int precision) { return precision == P2M_PREC_FP16_TC || precision == P2M_PREC_FP16_MIXED_TC; }
 // P2M_PREC_FP16_TC is an inference precision: the entry points that train or differentiate refuse it before any device
 // work (so a refused training forward leaves the running statistics as they were)
 int refuse_fp16(const p2m_model* m, const char* where) {
@@ -403,8 +408,8 @@ int run_tc_conv(p2m_model* m, UmmaConvArgs a, const float* W, bool transposed, b
     const char* tn = getenv("P2M_TRACE_NTH");
     if (a.trace != nullptr && tn && m->trace_seen++ != atoi(tn)) a.trace = nullptr;
   }
-  // single-pass fp16: forward convs only (refuse_fp16 keeps the backward-data conv away from it)
-  a.f16 = (m->precision == P2M_PREC_FP16_TC && !transposed) ? 1 : 0;
+  // single-pass fp16: every conv at fp16_mixed; at fp16 the forward convs only (refuse_fp16 keeps the backward away)
+  a.f16 = single_pass(m->precision) ? 1 : 0;
   P2M_TRY(launch_umma_pack_weights(W, fin, fout, transposed, WPACK_ALL, 0.f, wpack, s, a.f16 != 0));
   if (!t1_given) P2M_TRY(launch_cheb_t1(g, a.x, a.in_unpool, a.batch, a.fin, T, s, elide ? &g.real_tiles : nullptr));
   a.t1 = T;
@@ -422,13 +427,16 @@ int run_tc_conv(p2m_model* m, UmmaConvArgs a, const float* W, bool transposed, b
 }
 
 // dT = dz * Wp  ([rows, Fout] x [Fout, 3 Fin]) into T on the tensor cores: three plain GEMMs (one per Chebyshev order,
-// N = Fin, K = Fout, B_k[f][o] = W[o][f*3 + k]) with dz scaled into fp16's range by a_scale
+// N = Fin, K = Fout, B_k[f][o] = W[o][f*3 + k]) with dz scaled into fp16's range by a_scale; single pass (hi-only
+// images) at the single-pass precisions
 int run_tc_dt(p2m_model* m, const DevLevel& g, int batch, const float* dz, int fin, int fout, const float* W,
               const Epilogue& ep, const float* a_scale, unsigned char* wpack, float* T, cudaStream_t s) {
+  const bool f16 = single_pass(m->precision);
   for (int k = 0; k < 3; ++k) {
-    P2M_TRY(launch_umma_pack_weights(W, fin, fout, true, k, 0.f, wpack, s));
+    P2M_TRY(launch_umma_pack_weights(W, fin, fout, true, k, 0.f, wpack, s, f16));
     UmmaConvArgs a = umma_args(g, batch, dz, 0, fout, fin, ep, T, a_scale);
     a.wpack = wpack;
+    a.f16 = f16 ? 1 : 0;
     a.plain = 1;
     a.ldy = 3LL * fin;
     a.y_col0 = k * fin;
@@ -488,15 +496,17 @@ int simt_dw(const DevLevel& g, const float* x, int in_unpool, int rows, int fin,
 
 // dW [fout, 3 fin] of a conv on the tensor cores: T1 of one side into T, then launch_umma_dw on that basis and plain
 // tiles of the other side; basis_of_dz: T1 = L~dz (swap = 1), else T1 = L~x.  a_scale scales dz into fp16's range.
+// At the single-pass precisions the kernel is k_cheb_dw_f16_umma.
 int tc_dw(p2m_model* m, const DevLevel& g, int batch, const float* x, int in_unpool, int fin, const float* dz, int fout,
           bool basis_of_dz, const float* a_scale, float* T, float* dw, cudaStream_t s) {
   P2M_TRY(basis_of_dz ? launch_cheb_t1(g, dz, 0, batch, fout, T, s, nullptr)
                       : launch_cheb_t1(g, x, in_unpool, batch, fin, T, s, nullptr));
   P2M_TRY(launch_fill_zero(dw, sizeof(float) * fout * 3 * fin, s));
+  const bool f16 = single_pass(m->precision);
   return basis_of_dz ? launch_umma_dw(g, batch, dz, 0, fout, T, x, in_unpool, fin, 1, a_scale, dw, m->kernel_status,
-                                      m->sm_count, s)
+                                      m->sm_count, s, f16)
                      : launch_umma_dw(g, batch, x, in_unpool, fin, T, dz, 0, fout, 0, a_scale, dw, m->kernel_status,
-                                      m->sm_count, s);
+                                      m->sm_count, s, f16);
 }
 
 // fc: joints -> coarsest mesh level (meshnet.py:104-106), as a dense GEMM on the tensor cores (wgmma, fp16x3: also at
@@ -939,7 +949,7 @@ int p2m_debug_conv_tiling(const p2m_model_t* m, int level, int fin, int fout, in
   }
   const DevLevel& g = m->levels[level];
   const UmmaConvTiling t = conv_route(m, level, fin, fout, 1, false).tc
-                               ? umma_conv_tiling(g, fin, fout, false, m->precision == P2M_PREC_FP16_TC)
+                               ? umma_conv_tiling(g, fin, fout, false, single_pass(m->precision))
                                : UmmaConvTiling{0, 0, 0};
   out[0] = t.cols;
   out[1] = t.ns;
@@ -1040,7 +1050,8 @@ int p2m_model_layer_times_ms(p2m_model_t* m, float* out, int n) {
 }
 
 int p2m_model_set_precision(p2m_model_t* m, int precision) {
-  if (!m || (precision != P2M_PREC_FP32_SIMT && precision != P2M_PREC_FP16X3_TC && precision != P2M_PREC_FP16_TC)) {
+  if (!m || (precision != P2M_PREC_FP32_SIMT && precision != P2M_PREC_FP16X3_TC && precision != P2M_PREC_FP16_TC &&
+             precision != P2M_PREC_FP16_MIXED_TC)) {
     set_error("set_precision: bad argument");
     return P2M_ERR_INVALID;
   }

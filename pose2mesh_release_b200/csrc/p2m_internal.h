@@ -458,8 +458,8 @@ struct UmmaConvArgs {
   // optional: run on this tile family instead of the level's consecutive tiles
   const TileSet* tiles = nullptr;
   long long* trace = nullptr;       // debug (P2M_UMMA_TRACE builds only): [8][512] event log of CTA 0
-  // single-pass fp16 (P2M_PREC_FP16_TC): wpack is a hi-only image (launch_umma_pack_weights with f16), one k16 MMA per
-  // 16 features; T1-given convs and plain GEMMs without a_scale only (the eval forward)
+  // single-pass fp16 (P2M_PREC_FP16_TC, P2M_PREC_FP16_MIXED_TC): wpack is a hi-only image (launch_umma_pack_weights
+  // with f16), one k16 MMA per 16 features; T1-given convs and plain GEMMs, a_scale applied before the rounding
   int f16 = 0;
 };
 // Host: build the per-tile halo metadata of one level (uploads; device pointers appended to `owned`).  A level whose
@@ -481,7 +481,7 @@ UmmaConvTiling umma_conv_tiling(const DevLevel& g, int fin, int fout, bool plain
 // fin -> fout on it: T1-given and plain at fp16x3, T1-given and plain at fp16 ({0, 0, 0}: does not fit, or not the
 // tile size fout runs on)
 int umma_tile_families(const DevLevel& g, int fin, int fout, int32_t out[4][2][15]);
-int umma_dw_x_stages(const DevLevel& g);
+int umma_dw_x_stages(const DevLevel& g, bool f16 = false);
 bool umma_tma_rows(const DevLevel& g);
 // Weight images of a conv: fp16 [hi | lo] K-blocks of 32 k (x 2^6) from W [fout, fin*3] in the reference layout (column
 // f*3 + k), rows = output channels o and K = input features f; `transposed`: rows f and K = o, the backward-data conv's
@@ -489,7 +489,7 @@ bool umma_tma_rows(const DevLevel& g);
 //   WPACK_ALL       blocks u = chunk*3 + k of all three orders, umma_wpack_bytes(K, rows) bytes (the conv);
 //   WPACK_COMBINED  the isolated rows' combined weights W0 + c W1 + (2c^2 - 1) W2 (padding-vertex elision), and
 //   0, 1, 2         W_k alone (the backward's dT = dz W_k): plain images of umma_plain_pack_bytes(rows, K) bytes.
-// f16: the single-pass fp16 image (P2M_PREC_FP16_TC) of the same blocks, the round-to-nearest fp16 of W x 2^6 only (half
+// f16: the single-pass fp16 image (P2M_PREC_FP16_TC, P2M_PREC_FP16_MIXED_TC) of the same blocks, transposed or not, the round-to-nearest fp16 of W x 2^6 only (half
 // the bytes; the sizes below are those of the fp16x3 image and bound both).
 constexpr int WPACK_ALL = -1, WPACK_COMBINED = -2;
 size_t umma_wpack_bytes(int fin, int fout);
@@ -514,11 +514,12 @@ int launch_rescaled_epilogue(const Epilogue& ep, const float* w_scale, float w_p
 // the Chebyshev basis of one side (`gathered` [rows(/2), gathered_width], t1 = L~ gathered for EVERY row, from
 // launch_cheb_t1) and plain tiles of the other (`plain` [rows(/2), plain_width]).  swap = 0: gathered = x, plain = dz;
 // swap = 1 (L~ symmetric: sum_rows dz (x) T_k(x) = sum_rows T_k(dz) (x) x): gathered = dz, plain = x.  a_scale (device
-// scalar) scales dz into fp16's range and is divided out.
-bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width);
+// scalar) scales dz into fp16's range and is divided out.  f16: the single-pass kernel (k_cheb_dw_f16_umma,
+// P2M_PREC_FP16_MIXED_TC), both operands rounded once to fp16, one MMA per 16 rows; it fits wherever the fp16x3 one does.
+bool umma_dw_supported(const DevLevel& g, int gathered_width, int plain_width, bool f16 = false);
 int launch_umma_dw(const DevLevel& g, int batch, const float* gathered, int in_unpool, int gathered_width,
                    const float* t1, const float* plain, int g_unpool, int plain_width, int swap, const float* a_scale,
-                   float* dw_ref, int* status, int sm_count, cudaStream_t s);
+                   float* dw_ref, int* status, int sm_count, cudaStream_t s, bool f16 = false);
 // T1 = L~ x for all rows of a level (tile-staged gather), t1 [batch*V, fin] fp32
 int launch_cheb_t1(const DevLevel& g, const float* x, int in_unpool, int batch, int fin, float* t1, cudaStream_t s,
                    const TileSet* tiles = nullptr);

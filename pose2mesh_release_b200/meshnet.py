@@ -319,8 +319,10 @@ class Pose2Mesh(nn.Module):
 
     # -- knobs ---------------------------------------------------------------------------------
     def set_precision(self, precision: str):
-        """'fp32' (CUDA-core FFMA), 'fp16x3' (wgmma tensor cores, error-compensated split) or 'fp16' (single-pass
-        wgmma with fp16 operands, inference only: a train-mode forward or a backward raises RuntimeError)."""
+        """'fp32' (CUDA-core FFMA), 'fp16x3' (wgmma tensor cores, error-compensated split), 'fp16' (single-pass
+        wgmma with fp16 operands, inference only: a train-mode forward or a backward raises RuntimeError) or
+        'fp16_mixed' (the same single-pass convs in the training forward, backward-data and weight gradient: fp16
+        operands, fp32 accumulation, fp32 weights and BatchNorm; its eval forward is bitwise that of 'fp16')."""
         self._hier.set_precision(_lib.PRECISIONS[precision])
         return self
 
