@@ -15,20 +15,25 @@ gamma_K, fp16x3 (wgmma, each operand split as hi = fp16(v), lo = fp16(v - hi), p
   * fp32 accumulation of 3K products and the fp32 sparse products of the basis (row length deg): rounding errors of
     unit roundoff u = 2^-24 that are independent with mean zero grow like sqrt(n) u (the probabilistic bound of
     Higham & Mary, SIAM J. Sci. Comput. 41(5), 2019, with lambda = LAMBDA)          -> LAMBDA (sqrt(3K) + sqrt(2 deg + 3)) u
-gamma_K, fp32 (CUDA cores, FMA): only the last line.
+gamma_K, fp16 and fp16_mixed (single pass: each operand rounded to the nearest fp16 once, one product per pair):
+  * |fl(a) fl(b) - ab| <= (2u + u^2) |ab| with fp16's unit roundoff u = 2^-11                  -> 2^-10 + 2^-22
+  * the same fp32 accumulation term as fp16x3.
+gamma_K, fp32 (CUDA cores, FMA): only the accumulation term.
+SPLIT_TERM holds each precision's product-split term (SPLIT16 for the single pass).
 
 floor (only matters where |A||B| is tiny, i.e. a row of zeros or an entry of exact cancellation): fp16's subnormal
-spacing 2^-24 bounds the absolute error of a lo part.  The operands enter the split scaled into [2^(9-h), 2^(10-h))
-by a power of two (h = 0 for the weights, h = ceil(log2(2 r^2 + 1)) for the basis, r = max absolute row sum of L~),
-so the absolute error per operand entry is <= 2^(h-34) max|operand| and the floor is that times the other operand's
-absolute row sum.  It scales with the inputs: it is never an absolute constant.
+spacing 2^-24 bounds the absolute error of a lo part, or of a single-pass operand rounded to fp16.  The operands enter
+the split scaled into [2^(9-h), 2^(10-h)) by a power of two (h = 0 for the weights, h = ceil(log2(2 r^2 + 1)) for the
+basis, r = max absolute row sum of L~), so the absolute error per operand entry is <= 2^(h-34) max|operand| and the
+floor is that times the other operand's absolute row sum.  It scales with the inputs: it is never an absolute
+constant.
 
 The network schedules (p2m_meshnet_forward / _backward) do not range-normalise every operand: the forward conv's
 activations and the x side of dW enter the split as they are, the weights at the fixed scale 2^6.  There a lo part's
 absolute error is <= 2^-25 (half of fp16's subnormal spacing) divided by that fixed scale (split="network" of the conv
-bounds).  Next to the normalised floor 2^-34 max|x| this dominates once max|x| < 2^9, but next to the relative term
-SPLIT |x| = 3 2^-22 |x| only where |x| falls below 2^-25 / SPLIT = 1/24 (about 2^-4.6): activations after a
-BatchNorm are O(1).
+bounds).  Next to the normalised floor 2^-34 max|x| this dominates once max|x| < 2^9, but next to fp16x3's relative
+term 3 2^-22 |x| only where |x| falls below 2^-25 / (3 2^-22) = 1/24 (about 2^-4.6): activations after a BatchNorm
+are O(1).
 """
 from __future__ import annotations
 
@@ -38,13 +43,15 @@ import numpy as np
 import scipy.sparse as sp
 
 U32 = 2.0 ** -24          # fp32 unit roundoff
-SPLIT = 3 * 2.0 ** -22    # fp16x3: two lo roundings + the dropped lo*lo term
+SPLIT16 = 2.0 ** -10 + 2.0 ** -22    # single-pass fp16: one rounding of each operand
+# the product-split term of each precision (see the module docstring); fp16x3: two lo roundings + the dropped lo*lo term
+SPLIT_TERM = {"fp32": 0.0, "fp16x3": 3 * 2.0 ** -22, "fp16": SPLIT16, "fp16_mixed": SPLIT16}
 LAMBDA = 1.0              # probabilistic accumulation constant (see the module docstring)
 
 
 def gamma(k: int, precision: str, deg: int = 0) -> float:
     acc = LAMBDA * (math.sqrt(3 * k) + math.sqrt(2 * deg + 3)) * U32
-    return acc + (SPLIT if precision == "fp16x3" else 0.0)
+    return acc + SPLIT_TERM[precision]
 
 
 def headroom_log2(L: sp.spmatrix) -> int:
@@ -157,6 +164,9 @@ def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised", 
     fp16's range by a power of two (floor 2^-34 max|dz| per entry), the weights are at the fixed 2^6 and the x side of
     dW is unscaled.  dX there is either the dT GEMMs + the basis backward or a conv on dz ([dz | L dz | T2 dz] against
     the transposed weights), dW either on the basis of x or on the basis of dz: the floor is the larger of the two.
+    For the symmetric L~ the two dX paths have one absolute contraction, |dT0| + |dT2| + |L|^T (|dT1| + 2 |L|^T |dT2|)
+    = |T(dz)| |W'|, and so have the two dW paths, sum_rows |dz| (x) |T_k(x)| = sum_rows |T_k(dz)| (x) |x|: gamma's
+    split term covers either (at fp16_mixed every pass rounds its two operands to fp16 once).
     dw_chain > 0: hold dW to n u of a sequential chain of that many fp32 adds at least (a grid capped to a few CTAs
     accumulates the rows of many tiles in one CTA, where dW's one-signed partial sums grow linearly, not as sqrt(n))."""
     Labs = abs(sp.csr_matrix(L, dtype=np.float64))
@@ -197,7 +207,7 @@ def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised", 
     R = B * V
     g_dw = gamma(R, precision, deg) + (R.bit_length() * U32)   # + the cross-CTA fp32 atomic adds (log-depth tree)
     if dw_chain:   # the fp32 accumulation as a sequential chain of dw_chain adds: the deterministic worst case
-        g_dw = max(g_dw, dw_chain * U32 + (SPLIT if precision == "fp16x3" else 0.0))
+        g_dw = max(g_dw, dw_chain * U32 + SPLIT_TERM[precision])
     b_dw = g_dw * _contract_rows(dzf, Tf)
     if split == "network":
         Tdz = basis(adz, Labs)
@@ -741,7 +751,7 @@ def dense_gemm_bound(A, B, precision: str, b_side: str = "fixed") -> np.ndarray:
     """Element-wise bound on C = A @ B (A [m, k], B [k, n]) from one of PoseNet's GEMMs given its exact fp32 operands.
     fp32 (CUDA cores, FMA): gamma_k |A| |B|.
     fp16x3 (launch_umma_gemm), worst case per element rather than a probabilistic sum:
-      * the split: SPLIT |A| |B| (two lo roundings and the dropped lo*lo product, as in gamma);
+      * the split: SPLIT_TERM["fp16x3"] |A| |B| (two lo roundings and the dropped lo*lo product, as in gamma);
       * the accumulation: every k16 wgmma adds its products (exact in fp32) to the fp32 accumulator and truncates the
         result (round toward zero: Fasi et al., PeerJ Comput. Sci. 7:e330, 2021), an error below one ulp, i.e.
         < 2 u |accumulator after the step|.  Summed over the kernel's steps that is 2 u tc_running_sums(A, B): it
@@ -756,7 +766,7 @@ def dense_gemm_bound(A, B, precision: str, b_side: str = "fixed") -> np.ndarray:
     aA, aB = np.abs(A), np.abs(B)
     if precision != "fp16x3":
         return gamma(A.shape[1], precision) * (aA @ aB)
-    e = SPLIT * (aA @ aB) + 2 * U32 * tc_running_sums(A, B)
+    e = SPLIT_TERM["fp16x3"] * (aA @ aB) + 2 * U32 * tc_running_sums(A, B)
     e_a = 2.0 ** -34 * float(aA.max(initial=0.0))
     e_b = NET_LO / NET_W_SCALE if b_side == "fixed" else 2.0 ** -34 * float(aB.max(initial=0.0))
     return e + e_a * aB.sum(axis=0, keepdims=True) + e_b * aA.sum(axis=1, keepdims=True)

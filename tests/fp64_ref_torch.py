@@ -1,4 +1,4 @@
-"""tests/fp64_ref.py and tests/fp16_ref.py in torch float64, on any device, for the sizes the network runs at.
+"""tests/fp64_ref.py in torch float64, on any device, for the sizes the network runs at.
 
 fp64_ref.py stays the specification: every function here computes the same quantity by the same formula (its CPU
 cross-check is tests/test_fp64_torch_ref_cpu.py), only laid out for a batch of a few million rows:
@@ -19,7 +19,6 @@ import numpy as np
 import scipy.sparse as sp
 import torch
 
-import fp16_ref as R16
 import fp64_ref as R
 
 F64 = torch.float64
@@ -122,14 +121,12 @@ def _abs_contraction(ax, lp, aW) -> torch.Tensor:
     return Ta, Ta @ aW.T
 
 
-def cheb_conv_fwd_bound(x, L, W, b, precision: str, split: str = "normalised", chunk=None,
-                        extra: float = 0.0) -> torch.Tensor:
-    """extra: added to gamma_K (fp16_ref's SPLIT16 of the single-pass fp16 bound)."""
+def cheb_conv_fwd_bound(x, L, W, b, precision: str, split: str = "normalised", chunk=None) -> torch.Tensor:
     x = t64(x)
     dv = x.device
     lp, aW = lap(L, dv), t64(W, dv).abs()
     B, V, F = x.shape
-    g = R.gamma(3 * F, precision, lp.deg) + extra
+    g = R.gamma(3 * F, precision, lp.deg)
     mx = float(x.abs().max()) if x.numel() else 0.0
     mw = float(aW.max()) if aW.numel() else 0.0
     wsum = aW.sum(dim=1)[None, :]
@@ -145,11 +142,6 @@ def cheb_conv_fwd_bound(x, L, W, b, precision: str, split: str = "normalised", c
             fl = 2.0 ** (lp.h - 34) * mx * wsum + 2.0 ** -34 * mw * Ta.sum(dim=1, keepdim=True)
         out[c] = (bound + fl).reshape(-1, V, aW.shape[0])
     return out
-
-
-def cheb_conv_fwd_bound16(x, L, W, b, split: str = "normalised", chunk=None) -> torch.Tensor:
-    """fp16_ref.cheb_conv_fwd_bound16: the fp32 bound plus SPLIT16 |T| |W|."""
-    return cheb_conv_fwd_bound(x, L, W, b, "fp32", split, chunk, extra=R16.SPLIT16)
 
 
 def cheb_conv_bwd(x, L, W, dz, chunk=None):
@@ -225,7 +217,7 @@ def cheb_conv_bwd_bound(x, L, W, dz, precision: str, split: str = "normalised", 
     g_dw0 = dw_gamma_default(Rn, precision_dw, lp.deg)
     g_dw = g_dw0
     if dw_chain:
-        g_dw = max(g_dw, dw_chain * R.U32 + (R.SPLIT if precision_dw == "fp16x3" else 0.0))
+        g_dw = max(g_dw, dw_chain * R.U32 + R.SPLIT_TERM[precision_dw])
     if split == "network":
         on_x = e_dz * t_sum.reshape(1, 3 * F) + R.NET_LO * dz_sum[:, None]
         on_dz = (e_dz * torch.repeat_interleave(x_sum, 3)[None, :]

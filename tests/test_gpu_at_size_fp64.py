@@ -19,8 +19,8 @@ dW is held to the larger of the default bound and n u of the chain of the launch
 the ratio against the default bound alone is reported.
 
 Every run also asserts the path it took: each layer's route (p2m_debug_layer_route), and from the conv log each
-layer's forward launches (columns per CTA, slices, ring slots, stages, single-pass fp16 exactly in the fp16 case, the
-persistent grid, many tiles per CTA on the two finest levels), its dW launches and the fc's GEMM.
+layer's forward launches (columns per CTA, slices, ring slots, stages, single-pass fp16 exactly at fp16 and
+fp16_mixed, the persistent grid, many tiles per CTA on the two finest levels), its dW launches and the fc's GEMM.
 P2M_AT_SIZE_FP64_REPORT names a JSON report."""
 import json
 import os
@@ -262,10 +262,10 @@ def forward_launches(net, case, B, log, train):
     """The tensor-core launches of the forward, per layer in schedule order (a conv of the layer's tiles, then on an
     elided level the isolated rows' plain GEMM; the fc's GEMM after block 0), each asserted to be the instantiation
     the layer is named after: columns per CTA and slices by conv_cfg_named, ring slots and stages by
-    p2m_debug_conv_tiling (ELIDED_CFG on elided levels), single-pass fp16 exactly at the fp16 precision, the persistent
-    grid min(tiles, SMs / slices) and, on the two finest levels, many tiles per CTA.  Returns the launches after the
-    forward's (the backward's)."""
-    f16 = int(net.precision == "fp16")
+    p2m_debug_conv_tiling (ELIDED_CFG on elided levels), single-pass fp16 exactly at the single-pass precisions, the
+    persistent grid min(tiles, SMs / slices) and, on the two finest levels, many tiles per CTA.  Returns the launches
+    after the forward's (the backward's), whose convs and dWs carry the same single-pass bit."""
+    f16 = int(net.precision in ("fp16", "fp16_mixed"))
     tc_prec = net.precision != "fp32"
     rep = _REPORT["tiles_per_cta"].setdefault(case + (" forward" if train else " eval"), {})
     i = 0
@@ -306,6 +306,7 @@ def forward_launches(net, case, B, log, train):
             rep["fc"] = dict(cfg=(e["nc"], e["grid_y"], e["ns"], e["xs"]), grid_x=e["grid_x"], n_tiles=e["n_tiles"])
     if not train:
         assert i == len(log), (case, "launches the eval schedule does not account for", log[i:])
+    assert all(e["f16"] == f16 for e in log[i:] if e["kind"] in ("conv", "dw")), (case, log[i:])
     return log[i:]
 
 
@@ -363,7 +364,7 @@ def relu_mask(net, li, z, a, g_a, g_z, pre, E_y, case, blk):
 
 def check_train_layer(net, case, li, x, y, cap, grads, bufs, chain, need_dx):
     """test_gpu_network_fp64.check_train for layer li, in torch on the device, from the tensors of its own run."""
-    prec, B = net.precision, x.shape[0]
+    B = x.shape[0]
     L, blk = net.layers[li], block_of(net, li)
     r = net.route(li, B, need_dx)
     ch = chunk_of(net, li)
@@ -374,9 +375,8 @@ def check_train_layer(net, case, li, x, y, cap, grads, bufs, chain, need_dx):
     Lm = net.lap[L["level"]]
     W, bias = net.p[f"cl.{li}.weight"], net.p[f"cl.{li}.bias"]
     t = f"layer {li} ({L['fin']}->{L['fout']} V={net.V(li)})"
-    p_fwd = N.prec_of(net, r["tc"])
     z64 = T.cheb_conv_fwd(inp, Lm, W, bias, ch)
-    E = T.cheb_conv_fwd_bound(inp, Lm, W, bias, p_fwd, "network", ch)
+    E = T.cheb_conv_fwd_bound(inp, Lm, W, bias, net.conv_precision(r["tc"]), "network", ch)
     g_a = cap["g_a"][li].reshape(B, net.V(li), -1)
     g_z = cap["g_z"][li].reshape(g_a.shape)
     mirrored(case, t + " g_z", g_z, B)
@@ -403,7 +403,8 @@ def check_train_layer(net, case, li, x, y, cap, grads, bufs, chain, need_dx):
         check(case, t + " running_mean", bufs[f"bn.{li}.running_mean"], rm64, bd["rm"])
         check(case, t + " running_var", bufs[f"bn.{li}.running_var"], rv64, bd["rv"])
         if li == last_of(net.blocks[0]):
-            check(case, "fc_out", fc_out, *T.fc(a[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], prec))
+            check(case, "fc_out", fc_out,
+                  *T.fc(a[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], net.fc_precision()))
         # backward of the BatchNorm: the ReLU's branches as the device took them
         gz64, dg64, db64, pre = T.bn_train_bwd(z, g_a, g, be, relu=True, chunk=ch)
         del gz64
@@ -421,8 +422,8 @@ def check_train_layer(net, case, li, x, y, cap, grads, bufs, chain, need_dx):
     on_dx = r["tc_dx"] or r["tc_dt"]
     want_dx = not (li == 0 and not need_dx)
     dx64, dW64, db64 = T.cheb_conv_bwd(inp, Lm, W, g_z, ch)
-    bdx, bdw, _, bdw0 = T.cheb_conv_bwd_bound(inp, Lm, W, g_z, N.prec_of(net, on_dx), "network", chain, ch,
-                                              precision_dw=N.prec_of(net, on_dw), with_default=True)
+    bdx, bdw, _, bdw0 = T.cheb_conv_bwd_bound(inp, Lm, W, g_z, net.conv_precision(on_dx), "network", chain, ch,
+                                              precision_dw=net.conv_precision(on_dw), with_default=True)
     del inp
     dW = grads[f"cl.{li}.weight"]
     _REPORT["dw_vs_default"].setdefault(case, {})[str(li)] = T.bound_ratio(dW, dW64, bdw0)
@@ -547,10 +548,7 @@ def eval_layer(net, li, inp, block_in, on_tc, ch):
     W, bias = net.p[f"cl.{li}.weight"], net.p[f"cl.{li}.bias"]
     Lm = net.lap[L["level"]]
     z64 = T.cheb_conv_fwd(inp, Lm, W, bias, ch)
-    if net.precision == "fp16" and on_tc:
-        E = T.cheb_conv_fwd_bound16(inp, Lm, W, bias, "network", ch)
-    else:
-        E = T.cheb_conv_fwd_bound(inp, Lm, W, bias, N.prec_of(net, on_tc), "network", ch)
+    E = T.cheb_conv_fwd_bound(inp, Lm, W, bias, net.conv_precision(on_tc), "network", ch)
     if not L["bn"]:
         return z64, E
     g, be = net.p[f"bn.{li}.weight"], net.p[f"bn.{li}.bias"]
@@ -571,7 +569,7 @@ def run_eval_case(net, name, case, B, fused_check):
     n = net.n_layers
     for li in range(n):
         got = {k for k in FWD_KEYS if net.route(li, B)[k]}
-        assert got == {k for k in expected_route(net, name, "fp16x3", li) if k in FWD_KEYS}, (case, li, got)
+        assert got == {k for k in expected_route(net, name, net.precision, li) if k in FWD_KEYS}, (case, li, got)
     y_off, _ = eval_run(net, x, dedup=False, fuse=False, want=None, check_log=case)
     for li in range(n):
         y, cap = eval_run(net, x, dedup=False, fuse=False, want=eval_window(net, li), check_log=case)
@@ -585,8 +583,8 @@ def run_eval_case(net, name, case, B, fused_check):
         check(case, f"layer {li} y", act[li], ref, bound)
         del ref, bound
         if li == last_of(net.blocks[0]):
-            check(case, "fc_out", cap["fc_out"], *T.fc(act[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"],
-                                                       "fp16x3" if net.precision != "fp32" else "fp32"))
+            check(case, "fc_out", cap["fc_out"],
+                  *T.fc(act[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], net.fc_precision()))
         del cap, act
         torch.cuda.empty_cache()
     y_on, _ = eval_run(net, x, dedup=False, fuse=True, want=None, check_log=case + " fused")
@@ -621,9 +619,5 @@ def test_smpl_b256_eval_fp16x3():
 
 
 def test_smpl_b256_eval_fp16():
-    from pose2mesh_release_b200 import _lib
-
-    net = at_size_net("smpl_like", "fp16x3", seed=4, open_relus=False)
-    net.precision = "fp16"
-    net.hier.set_precision(_lib.P2M_PREC_FP16_TC)
+    net = at_size_net("smpl_like", "fp16", seed=4, open_relus=False)
     run_eval_case(net, "smpl_like", "smpl_like B=256 fp16 eval", 256, False)

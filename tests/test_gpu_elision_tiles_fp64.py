@@ -10,7 +10,7 @@ level runs on its consecutive tiles.
 Each hierarchy of graphs.ELISION (a padded level, a level of half its size, the joint graph) runs the network schedules
 of test_gpu_network_fp64 (eval with the fused head off and on and dedup off and on, the training forward and backward
 with dX) at elision 0, 1 and 2, with the persistent grids at the device's SM count and capped, so that CTAs run several
-index-list tiles.  Every captured layer is held to fp64_ref's (fp16_ref's) bounds from its own captured inputs.  Each
+index-list tiles.  Every captured layer is held to fp64_ref's bounds from its own captured inputs.  Each
 case asserts its routes (p2m_debug_layer_route) against the elision rule, and the conv log against the configurations
 p2m_debug_tile_families reports for the family each elided conv runs on."""
 import numpy as np
@@ -100,14 +100,6 @@ def read_log(tag, want, capped):
     return log
 
 
-def make_net(name, precision, seed, open_relus):
-    if precision == "fp16":
-        import test_gpu_fp16_inference as F
-
-        return F.fp16_net(name, seed)
-    return N.Net(name, precision, seed=seed, open_relus=open_relus)
-
-
 # ------------------------------------------------------------------------------------------------- the families
 # family -> the padded level's (real_tiles at 128 rows: n_pattern, max_h1), and per conv (fin, fout) the T1-given
 # fp16x3 configuration on its connected-row tiles; None: build_umma_level_meta keeps no families
@@ -171,11 +163,8 @@ MODES = {"fp16x3": (0, 1, 2), "fp16": (0, 1, 2), "fp32": (2,)}
 def test_eval_layer_by_layer(name, precision):
     """Eval forward at elision 0 / 1 / 2 (capped at 2): every layer (fused head off, then the fused head) from
     its captured input; dedup on (the isolated rows' GEMM on rep_tiles) bitwise equal to dedup off (on iso_tiles)."""
-    from test_gpu_persistent_tiles_fp64 import check_eval16
-
     B = EVAL_B.get(name, 1)
-    net = make_net(name, precision, seed=17, open_relus=False)
-    n = net.n_layers
+    net = N.Net(name, precision, seed=17, open_relus=False)
     try:
         for mode in MODES[precision]:
             x, _ = N.train_inputs(net, B, seed=3 + mode)
@@ -184,19 +173,11 @@ def test_eval_layer_by_layer(name, precision):
             tag = f"{name} {precision} eval elide={mode} cap={cap}"
             lib().conv_log(reset=True)
             want = check_routes(net, tag, B, mode) if precision != "fp32" else set()
-            if precision == "fp16":
-                y, c = N.forward_eval(net, x, mode, dedup=False, fuse=False)
-                act = {li: c["y"][li].reshape(B, net.V(li), -1) for li in range(n)}
-                check_eval16(net, tag, x, act, c["fc_out"])
-                yf = None
-            else:
-                y, yf = N.check_eval(net, tag, x, mode)
+            y, yf, _, _ = N.check_eval(net, tag, x, mode)
             read_log(tag, want, cap > 0)
             for fuse in (False, True):
                 yd, _ = N.forward_eval(net, x, mode, dedup=True, fuse=fuse, capture=False)
-                yo = y if not fuse else yf
-                if yo is not None:
-                    assert np.array_equal(yd, yo), (tag, "dedup", fuse)
+                assert np.array_equal(yd, y if not fuse else yf), (tag, "dedup", fuse)
             read_log(tag, set(), cap > 0)
             assert net.hier.kernel_status(0) == 0, tag
     finally:
@@ -219,7 +200,7 @@ def test_train_layer_by_layer(name, precision):
     """Training forward and backward with dX at elision 0 / 1 / 2 (capped at elision 2): every layer from its captured
     inputs, the backward-data convs on the connected-row tiles where dx_elide."""
     B = EVAL_B.get(name, 1)
-    net = make_net(name, precision, seed=29, open_relus=True)
+    net = N.Net(name, precision, seed=29, open_relus=True)
     try:
         for mode in MODES[precision]:
             cap = CAP if mode == 2 else 0

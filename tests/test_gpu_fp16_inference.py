@@ -2,10 +2,11 @@
 
 1. Single layer (p2m_cheb_conv_fwd) against float64: every width of the three kernel configurations (128 x 64,
    64 x 128, 64 x 256), the graph families of tests/graphs.py, the persistent CTA loop.  Every element lies within
-   fp16_ref's bound (SPLIT16 = 2^-10 + 2^-22), and at least one element of each case lies beyond
+   fp64_ref's bound at "fp16" (SPLIT16 = 2^-10 + 2^-22), and at least one element of each case lies beyond
    the fp16x3 bound: the single pass is what ran.
-2. The eval network layer by layer (p2m_debug_set_capture), each layer from its own captured input: elision 0 / 1 / 2
-   (index-list tiles and the isolated rows' combined-weight GEMM), the virtual unpool, residuals, the fused head.
+2. The eval network layer by layer (test_gpu_network_fp64.check_eval on an fp16 net), each layer from its own captured
+   input: elision 0 / 1 / 2 (index-list tiles and the isolated rows' combined-weight GEMM), the virtual unpool,
+   residuals, the fused head, dedup.
 3. Full size (SMPL hierarchy, B = 256): finite, two runs, forward_vertices and CUDA-graph replay equal to the plain
    forward bit for bit, batch split and elision / dedup within a tolerance derived from SPLIT16, the per-mesh deviation
    from the float64 oracle on test_gpu_parity's 32-mesh sample (written to P2M_FP16_REPORT if set).
@@ -20,7 +21,6 @@ import numpy as np
 import pytest
 import torch
 
-import fp16_ref as R16
 import fp64_ref as R
 import graphs as G
 from helpers import CASES, graph_from_fixture
@@ -81,7 +81,7 @@ def check_single_pass(tag, L, x, W, b, y, on_tc=True):
     L = L.tocsr().astype(np.float32).astype(np.float64)
     ref = R.cheb_conv_fwd(x, L, W, b)
     err = np.abs(y - ref)
-    r16 = float((err / R16.cheb_conv_fwd_bound16(x, L, W, b)).max())
+    r16 = float((err / R.cheb_conv_fwd_bound(x, L, W, b, "fp16")).max())
     assert r16 <= 1.0, f"{tag}: max |err| / fp16 bound = {r16:.3g}"
     if on_tc:
         r3 = float((err / R.cheb_conv_fwd_bound(x, L, W, b, "fp16x3")).max())
@@ -140,36 +140,6 @@ def test_single_layer_persistent_cta_loop(fin, fout):
 
 
 # ------------------------------------------------------------------------------------------- 2. network, layer by layer
-def fp16_net(name, seed):
-    import test_gpu_network_fp64 as N
-    from pose2mesh_release_b200 import _lib
-
-    net = N.Net(name, "fp16x3", seed=seed, open_relus=False)
-    net.precision = "fp16"
-    net.hier.set_precision(_lib.P2M_PREC_FP16_TC)
-    return net
-
-
-def eval_layer16(net, li, inp, block_in, on_tc):
-    """test_gpu_network_fp64.eval_layer with the conv bound at fp16 (network split) on the tensor cores."""
-    import test_gpu_network_fp64 as N
-
-    L = net.layers[li]
-    W, b = net.p[f"cl.{li}.weight"], net.p[f"cl.{li}.bias"]
-    Lm = net.L32[L["level"]]
-    z64 = R.cheb_conv_fwd(inp, Lm, W, b)
-    E = R16.cheb_conv_fwd_bound16(inp, Lm, W, b, "network") if on_tc else \
-        R.cheb_conv_fwd_bound(inp, Lm, W, b, "fp32", split="network")
-    if not L["bn"]:
-        return z64, E
-    g, be = net.p[f"bn.{li}.weight"], net.p[f"bn.{li}.bias"]
-    rm, rv = net.p[f"bn.{li}.running_mean"], net.p[f"bn.{li}.running_var"]
-    y64 = R.bn_eval_fwd(z64, g, be, rm, rv, relu=True)
-    bound = R.bn_eval_fwd_bound(z64, E, g, be, rm, rv, b)
-    res, eres = N.residual(net, li, block_in)
-    return y64 + res, bound + eres + R.U32 * np.abs(y64 + res)
-
-
 EVAL_CASES = [(name, elide, B) for name in ("smpl_small", "mano_like", "custom") for elide, B in ((0, 3), (1, 1), (2, 3))]
 
 
@@ -177,47 +147,18 @@ EVAL_CASES = [(name, elide, B) for name in ("smpl_small", "mano_like", "custom")
 def test_eval_network_layer_by_layer(name, elide, B):
     import test_gpu_network_fp64 as N
 
-    net = fp16_net(name, seed=31 + B + elide)
+    net = N.Net(name, "fp16", seed=31 + B + elide, open_relus=False)
     x, _ = N.train_inputs(net, B, seed=5 + elide)
-    y, cap = N.forward_eval(net, x, elide, dedup=False, fuse=False)
-    n = net.n_layers
-    act = {li: cap["y"][li].reshape(B, net.V(li), -1) for li in range(n)}
-    fc_out = cap["fc_out"]
     tag = f"{name} fp16 eval elide={elide} B={B}"
-    assert np.array_equal(act[n - 1], y.reshape(act[n - 1].shape)), tag
+    y, yf, act, fc_out = N.check_eval(net, tag, x, elide)
+    # at least one tensor-core layer beyond the fp16x3 bound: the single pass is what ran
     beyond = 0
-    for li in range(n):
-        inp, block_in = N.layer_input(net, li, x, fc_out, act)
-        on_tc = net.route(li, B)["tc"]
-        ref, bound = eval_layer16(net, li, inp, block_in, on_tc)
-        err = np.abs(act[li] - ref)
-        r = float((err / bound).max())
-        assert r <= 1.0, f"{tag} layer {li}: max |err| / bound = {r:.3g}"
-        if on_tc:
-            net.precision = "fp16x3"   # (eval_layer's bound at fp16x3)
-            _, b3 = N.eval_layer(net, li, inp, block_in, True)
-            net.precision = "fp16"
-            beyond += int((err > b3).any())
-        if li == net.blocks[0]["first"] + net.blocks[0]["n"] - 1:   # the fc stays an fp16x3 dense GEMM
-            ref_fc, b_fc = N.fc_ref(act[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], "fp16x3")
-            assert float((np.abs(fc_out - ref_fc) / b_fc).max()) <= 1.0, f"{tag} fc_out"
+    for li in range(net.n_layers):
+        if net.route(li, B)["tc"]:
+            inp, block_in = N.layer_input(net, li, x, fc_out, act)
+            ref, b3 = N.eval_layer(net, li, inp, block_in, "fp16x3")
+            beyond += int((np.abs(act[li] - ref) > b3).any())
     assert beyond >= 1, f"{tag}: no tensor-core layer beyond the fp16x3 bound"
-    # the fused head from the fused layer's captured input
-    yf, capf = N.forward_eval(net, x, elide, dedup=False, fuse=True)
-    fused = [li for li in range(n) if net.route(li, B)["fuse_head"]]
-    if B * net.V(n - 2) >= 64:
-        assert fused == [n - 2], (tag, fused)
-    if fused:
-        li = fused[0]
-        act_f = {k: capf["y"][k].reshape(B, net.V(k), -1) for k in range(n) if k != li}
-        inp, block_in = N.layer_input(net, li, x, capf["fc_out"], act_f)
-        y1, e1 = eval_layer16(net, li, inp, block_in, True)
-        Lh = net.L32[net.layers[n - 1]["level"]]
-        Wh, bh = net.p[f"cl.{n - 1}.weight"], net.p[f"cl.{n - 1}.bias"]
-        ref = R.cheb_conv_fwd(y1, Lh, Wh, bh)
-        bound = R.cheb_conv_fwd_bound(y1, Lh, Wh, bh, "fp32") + R.thin_head_fused_bound(y1, e1, Lh, Wh)
-        r = float((np.abs(yf.reshape(ref.shape) - ref) / bound).max())
-        assert r <= 1.0, f"{tag} fused head: max |err| / bound = {r:.3g}"
     # dedup on against off: the representative rows are computed by the same GEMM, bit for bit
     for fuse in (False, True):
         yd, _ = N.forward_eval(net, x, elide, dedup=True, fuse=fuse, capture=False)
@@ -254,7 +195,7 @@ def per_mesh(y, ref):
 # turn into one fp16 step).  Per layer the two differ by at most the two forwards' rounding, 2 SPLIT16 relative,
 # compounded through the 21 layers of the SMPL plan at O(1) gain per layer: 21 * 2 * SPLIT16 = 4.1e-2 per mesh of
 # max|y| is the ceiling.  (fp16x3 holds a batch split to 1e-6: its split keeps those last bits.)
-ROUNDING_TOL = 21 * 2 * R16.SPLIT16
+ROUNDING_TOL = 21 * 2 * R.SPLIT16
 PARITY_CEILING = 5e-2   # a chosen limit against layout or indexing bugs, not a derived bound
 PICK = sorted({0, 1, 2, 3, 36, 37, 73, 74, 110, 111, 127, 128, 131, 147, 148, 149, 184, 185, 221, 222, 254, 255}
               | set(range(9, 256, 25)) | {200})

@@ -2,31 +2,22 @@
 
 1. One layer against float64: p2m_cheb_conv_fwd with batch-statistics BatchNorm, and p2m_cheb_conv_fwd / _bwd over
    every width of the three conv configurations, the graph families of tests/graphs.py and the persistent CTA loop.
-   y, dX, dW and db lie within the single-pass bounds (fp16_ref, fp16_train_ref), and at least one element of y, dX
-   and dW of each tensor-core case lies beyond the fp16x3 bound: the single pass is what ran.
+   y, dX, dW and db lie within fp64_ref's bounds at "fp16_mixed", and at least one element of y, dX and dW of each
+   tensor-core case lies beyond the fp16x3 bound: the single pass is what ran.
 2. The training step layer by layer on test_gpu_network_fp64's TRAIN_CASES and its shifted-channel case: every layer
-   from its own captured inputs, with the conv bounds swapped for the single-pass ones (below).  Every conv and dW
-   launch of the step is single-pass, the fc's dense GEMM is not, and every layer's route equals fp16x3's.
+   from its own captured inputs, the convs held to their single-pass bounds and the fc (an fp16x3 dense GEMM at every
+   tensor-core precision) to its fp16x3 bound.  Every conv and dW launch of the step is single-pass, the fc's dense
+   GEMM is not, and every layer's route equals fp16x3's.
 3. At size: the SMPL B = 256 and MANO B = 1024 training steps layer by layer (test_gpu_at_size_fp64.run_train_case).
 4. Eval: bitwise fp16's outputs at full SMPL size, also from a CUDA-graph replay; a model switched back to fp16x3 gives
    bitwise the results of one that never left it.
 5. A short seeded Adam fit converges as at fp16x3.
-Every test ends with kernel_status == 0.
-
-The bound swap: fp64_ref's (and fp64_ref_torch's) Chebyshev-conv bounds at precision "fp16x3" are gamma_K |A| |B| +
-floors with gamma_K = accumulation + SPLIT.  With SPLIT read as SPLIT16 = 2^-10 + 2^-22 they are exactly fp16_ref's and
-fp16_train_ref's single-pass bounds: the fp32 bound plus SPLIT16 times the same contraction (also under dw_chain, whose
-fp16x3 term is max(gamma, chain u + SPLIT)).  The fixture `single_pass_conv_bounds` does that for the conv bound
-functions only, so the fc (still an fp16x3 dense GEMM) keeps its fp16x3 bound; the nets keep the label "fp16x3", which
-the shared checks read as "on the tensor cores"."""
+Every test ends with kernel_status == 0."""
 import numpy as np
 import pytest
 import torch
 
-import fp16_ref as R16
-import fp16_train_ref as RT
 import fp64_ref as R
-import fp64_ref_torch as T
 import graphs as G
 from helpers import CASES, graph_from_fixture
 
@@ -52,44 +43,6 @@ def clear_conv_log():
     lib.p2m_debug_conv_log_reset()
 
 
-@pytest.fixture
-def single_pass_conv_bounds(monkeypatch):
-    def swap(mod, name):
-        orig = getattr(mod, name)
-
-        def wrapped(*a, **k):
-            saved = R.SPLIT
-            R.SPLIT = R16.SPLIT16
-            try:
-                return orig(*a, **k)
-            finally:
-                R.SPLIT = saved
-
-        monkeypatch.setattr(mod, name, wrapped)
-
-    for mod in (R, T):
-        swap(mod, "cheb_conv_fwd_bound")
-        swap(mod, "cheb_conv_bwd_bound")
-
-
-def test_bound_swap_is_the_single_pass_bound(single_pass_conv_bounds):
-    """The swapped fp16x3 bounds equal fp16_ref's and fp16_train_ref's (to rounding), with and without dw_chain."""
-    L = graph_from_fixture("smpl_small")[0][2].tocsr().astype(np.float32).astype(np.float64)
-    rng = np.random.default_rng(0)
-    x = rng.standard_normal((2, L.shape[0], 64))
-    W = rng.standard_normal((128, 192)) * 0.1
-    b = rng.standard_normal(128) * 0.1
-    dz = rng.standard_normal((2, L.shape[0], 128)) * 1e-3
-    for split in ("network", "normalised"):
-        np.testing.assert_allclose(R.cheb_conv_fwd_bound(x, L, W, b, "fp16x3", split=split),
-                                   R16.cheb_conv_fwd_bound16(x, L, W, b, split), rtol=1e-12)
-        for chain in (0, 5000):
-            got = R.cheb_conv_bwd_bound(x, L, W, dz, "fp16x3", split=split, dw_chain=chain)
-            want = RT.cheb_conv_bwd_bound16(x, L, W, dz, split, dw_chain=chain)
-            for g, w in zip(got, want):
-                np.testing.assert_allclose(g, w, rtol=1e-12)
-
-
 # ------------------------------------------------------------------------------------------------------ 1. one layer
 def run_layer(L, x, W, b, dz, sm_cap=0):
     import test_gpu_kernels_fp64 as K
@@ -104,7 +57,7 @@ def check_layer(tag, L, x, W, b, dz, y, dx, dW, db, p):
     L = L.tocsr().astype(np.float32).astype(np.float64)
     y64 = R.cheb_conv_fwd(x, L, W, b)
     dx64, dW64, db64 = R.cheb_conv_bwd(x, L, W, dz)
-    b16 = (R16.cheb_conv_fwd_bound16(x, L, W, b),) + RT.cheb_conv_bwd_bound16(x, L, W, dz)
+    b16 = (R.cheb_conv_fwd_bound(x, L, W, b, MIXED),) + R.cheb_conv_bwd_bound(x, L, W, dz, MIXED)
     b3 = (R.cheb_conv_fwd_bound(x, L, W, b, "fp16x3"),) + R.cheb_conv_bwd_bound(x, L, W, dz, "fp16x3")
     for i, (what, got, ref) in enumerate((("y", y, y64), ("dx", dx, dx64), ("dW", dW, dW64), ("db", db, db64))):
         err = np.abs(got - ref)
@@ -185,7 +138,7 @@ def test_single_layer_persistent_cta_loop(fin, fout):
 
 @pytest.mark.parametrize("fin,fout", [(64, 64), (128, 256), (256, 256)], ids=lambda v: str(v))
 @pytest.mark.parametrize("lvl", ["tma", "ragged"])
-def test_single_layer_batch_statistics_batchnorm(fin, fout, lvl, single_pass_conv_bounds):
+def test_single_layer_batch_statistics_batchnorm(fin, fout, lvl):
     """p2m_cheb_conv_fwd with bn_mode 2 (refused at fp16) runs at fp16_mixed: y, save_mean / save_invstd and the
     running statistics against float64 with the conv error held to the single-pass bound."""
     import test_gpu_batchnorm_fp64 as BN
@@ -195,27 +148,19 @@ def test_single_layer_batch_statistics_batchnorm(fin, fout, lvl, single_pass_con
     for relu in (False, True):
         got, p = BN.run_bn_layer(L, x, W, b, bn, 2, relu, MIXED)
         assert p["conv"] == 1 and got["nbt"] == 8, (p, got["nbt"])
-        BN.check_train(f"bn2 {fin}->{fout} {lvl} relu={relu}", "fp16x3", L.tocsr(), x, W, b, bn, got, relu)
+        BN.check_train(f"bn2 {fin}->{fout} {lvl} relu={relu}", MIXED, L.tocsr(), x, W, b, bn, got, relu)
 
 
 # ------------------------------------------------------------------------------------------- 2. network, layer by layer
-def mixed_net(name, seed, **kw):
-    import test_gpu_network_fp64 as N
-    from pose2mesh_release_b200 import _lib
-
-    net = N.Net(name, "fp16x3", seed=seed, open_relus=True, **kw)
-    net.hier.set_precision(_lib.P2M_PREC_FP16_MIXED_TC)
-    return net
-
-
 def routes_at(net, B, need_dx, precision):
     from pose2mesh_release_b200 import _lib
 
+    own = net.hier.precision
     net.hier.set_precision(_lib.PRECISIONS[precision])
     try:
         return [net.route(li, B, need_dx) for li in range(net.n_layers)]
     finally:
-        net.hier.set_precision(_lib.P2M_PREC_FP16_MIXED_TC)
+        net.hier.set_precision(own)
 
 
 def train_and_check(net, tag, x, tgt, need_dx):
@@ -242,51 +187,32 @@ def _train_cases():
 
 
 @pytest.mark.parametrize("name,elide,B,need_dx", _train_cases(), ids=lambda v: str(v))
-def test_train_step_layer_by_layer(name, elide, B, need_dx, single_pass_conv_bounds):
+def test_train_step_layer_by_layer(name, elide, B, need_dx):
     import test_gpu_network_fp64 as N
 
-    net = mixed_net(name, seed=100 * elide + B)
+    net = N.Net(name, MIXED, seed=100 * elide + B, open_relus=True)
     net.hier.set_debug(0, elide_padding=elide)
     x, tgt = N.train_inputs(net, B, seed=B + elide)
     train_and_check(net, f"{name} fp16_mixed elide={elide} B={B} dx={need_dx}", x, tgt, need_dx)
 
 
-def test_train_step_with_shifted_channels(single_pass_conv_bounds):
+def test_train_step_with_shifted_channels():
     import test_gpu_network_fp64 as N
 
-    net = mixed_net("custom", seed=7, bias_shift=1000.0)
+    net = N.Net("custom", MIXED, seed=7, open_relus=True, bias_shift=1000.0)
     x, tgt = N.train_inputs(net, 3, seed=9)
     train_and_check(net, "custom shifted fp16_mixed", x, tgt, True)
 
 
 # ------------------------------------------------------------------------------------------------------ 3. at size
 @pytest.mark.parametrize("name,B", [("smpl_like", 256), ("mano_like", 1024)])
-def test_train_at_size(name, B, single_pass_conv_bounds, monkeypatch):
-    """test_gpu_at_size_fp64.run_train_case on a net switched to fp16_mixed: its launch check then expects the
-    single-pass bit on every forward conv (its fp16 case), its bounds are the single-pass ones and its routes fp16x3's."""
+def test_train_at_size(name, B):
+    """test_gpu_at_size_fp64.run_train_case at fp16_mixed: its launch check expects the single-pass bit on every conv
+    and dW launch, its bounds are the single-pass ones and its routes fp16x3's."""
     import test_gpu_at_size_fp64 as A
-    from pose2mesh_release_b200 import _lib
 
-    make, launches = A.at_size_net, A.forward_launches
-
-    def at_size_net(*a, **k):
-        net = make(*a, **k)
-        net.hier.set_precision(_lib.P2M_PREC_FP16_MIXED_TC)
-        return net
-
-    def forward_launches(net, case, B_, log, train):
-        net.precision = "fp16"          # the single-pass bit on every conv of the forward
-        try:
-            rest = launches(net, case, B_, log, train)
-        finally:
-            net.precision = "fp16x3"
-        assert all(e["f16"] == 1 for e in rest if e["kind"] in ("conv", "dw")), (case, rest)
-        return rest
-
-    monkeypatch.setattr(A, "at_size_net", at_size_net)
-    monkeypatch.setattr(A, "forward_launches", forward_launches)
     torch.cuda.reset_peak_memory_stats()
-    net = A.run_train_case(name, B, "fp16x3")
+    net = A.run_train_case(name, B, MIXED)
     assert net.hier.kernel_status(0) == 0
 
 

@@ -24,7 +24,7 @@ from helpers import CASES, graph_from_fixture
 pytestmark = pytest.mark.gpu
 
 PRECISIONS = ["fp32", "fp16x3"]
-_WORST = {"fp32": [0.0, ""], "fp16x3": [0.0, ""]}
+_WORST = {}
 
 # levels {128, 64, joint 17}: block 0 on the joint level, block 1's 64 -> 256 has Fout > 3 Fin (dX by the dT GEMMs:
 # the conv on dz needs Fout <= 3 Fin, and a 64-wide output) and ends in a resampled residual + unpool, block 2 in an
@@ -48,7 +48,7 @@ def dev():
 
 def check(what, precision, got, ref, bound):
     r = R.bound_ratio(got, ref, bound)
-    if r > _WORST[precision][0]:
+    if r > _WORST.setdefault(precision, [0.0, ""])[0]:
         _WORST[precision] = [r, what]
     assert r <= 1.0, f"{what}: max |err| / bound = {r:.3g}"
 
@@ -90,7 +90,6 @@ class Net:
         import test_gpu_batchnorm_fp64 as T
 
         self.levels, self.plan = net_levels(name)
-        self.precision = precision
         self.hier, self.sd, self.n_layers, _ = T.small_net(self.levels, self.plan, precision, seed, open_relus,
                                                            bias_shift)
         # the Laplacians as the device holds them (fp32 values)
@@ -115,6 +114,21 @@ class Net:
 
     def route(self, li, B, need_dx=True):
         return self.hier.layer_route(0, li, B, need_dx)
+
+    @property
+    def precision(self):
+        """The precision the net's hierarchy runs at, by its name in _lib.PRECISIONS."""
+        from pose2mesh_release_b200 import _lib
+
+        return next(k for k, v in _lib.PRECISIONS.items() if v == self.hier.precision)
+
+    def conv_precision(self, on_tc):
+        """The precision a conv pass runs at: the net's on the tensor cores, fp32 on the CUDA cores."""
+        return self.precision if on_tc else "fp32"
+
+    def fc_precision(self):
+        """The precision the fc runs at: an fp16x3 dense GEMM at every tensor-core precision."""
+        return "fp32" if self.precision == "fp32" else "fp16x3"
 
     def capture_buffers(self, B, names):
         cap = {}
@@ -155,14 +169,10 @@ def layer_input(net, li, x, fc_out, act, ref=R):
     return inp, block_in
 
 
-def prec_of(net, on_tc):
-    return "fp16x3" if (net.precision == "fp16x3" and on_tc) else "fp32"
-
-
-def conv_ref(net, li, inp, on_tc):
+def conv_ref(net, li, inp, precision):
     W, b = net.p[f"cl.{li}.weight"], net.p[f"cl.{li}.bias"]
     L = net.L32[net.layers[li]["level"]]
-    return R.cheb_conv_fwd(inp, L, W, b), R.cheb_conv_fwd_bound(inp, L, W, b, prec_of(net, on_tc), split="network")
+    return R.cheb_conv_fwd(inp, L, W, b), R.cheb_conv_fwd_bound(inp, L, W, b, precision, split="network")
 
 
 def fc_ref(a0, W, b, precision):
@@ -234,7 +244,7 @@ def check_train(net, tag, x, y, cap, grads, bufs, need_dx):
     for li, L in enumerate(net.layers):
         r = net.route(li, B, need_dx)
         inp, block_in = layer_input(net, li, x, fc_out, a)
-        z64, E = conv_ref(net, li, inp, r["tc"])
+        z64, E = conv_ref(net, li, inp, net.conv_precision(r["tc"]))
         t = f"{tag} layer {li} ({L['fin']}->{L['fout']} V={net.V(li)})"
         if not L["bn"]:
             check(t + " y", prec, y.reshape(z64.shape), z64, E)
@@ -251,7 +261,8 @@ def check_train(net, tag, x, y, cap, grads, bufs, need_dx):
         check(t + " running_mean", prec, bufs[f"bn.{li}.running_mean"], rm64, bd["rm"])
         check(t + " running_var", prec, bufs[f"bn.{li}.running_var"], rv64, bd["rv"])
         if li == net.blocks[0]["first"] + net.blocks[0]["n"] - 1:   # the fc
-            check(f"{tag} fc_out", prec, fc_out, *fc_ref(a[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], prec))
+            check(f"{tag} fc_out", prec, fc_out,
+                  *fc_ref(a[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], net.fc_precision()))
     # ---- backward
     for li in range(n - 1, -1, -1):
         L = net.layers[li]
@@ -278,8 +289,8 @@ def check_train(net, tag, x, y, cap, grads, bufs, need_dx):
         dx64, dW64, db64 = R.cheb_conv_bwd(inp, Lm, W, g_z)
         on_dw = r["tc_dw"] or r["dw_dz_basis"]
         on_dx = r["tc_dx"] or r["tc_dt"]
-        bdx, _, bdb = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, prec_of(net, on_dx), split="network")
-        _, bdw, _ = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, prec_of(net, on_dw), split="network",
+        bdx, _, bdb = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, net.conv_precision(on_dx), split="network")
+        _, bdw, _ = R.cheb_conv_bwd_bound(inp, Lm, W, g_z, net.conv_precision(on_dw), split="network",
                                           dw_chain=dw_chain(net, li, B))
         check(t + " dW", prec, grads[f"cl.{li}.weight"], dW64, bdw)
         if not L["bn"]:
@@ -387,10 +398,11 @@ def forward_eval(net, x, elide, dedup, fuse, capture=True):
     return npy(y), {k: ([npy(t) for t in v] if isinstance(v, list) else npy(v)) for k, v in cap.items()}
 
 
-def eval_layer(net, li, inp, block_in, on_tc):
-    """Float64 eval output of layer li (folded BatchNorm + ReLU + residual, or the head's conv) and its bound."""
+def eval_layer(net, li, inp, block_in, precision):
+    """Float64 eval output of layer li (folded BatchNorm + ReLU + residual, or the head's conv) and its bound with the
+    conv at `precision`."""
     L = net.layers[li]
-    z64, E = conv_ref(net, li, inp, on_tc)
+    z64, E = conv_ref(net, li, inp, precision)
     if not L["bn"]:
         return z64, E
     g, be = net.p[f"bn.{li}.weight"], net.p[f"bn.{li}.bias"]
@@ -415,7 +427,7 @@ def test_eval_forward_layer_by_layer(name, elide, B, precision):
     net = Net(name, precision, seed=31 + B + elide, open_relus=False)
     x, _ = train_inputs(net, B, seed=5 + elide)
     tag = f"{name} eval elide={elide} B={B}"
-    y, yf = check_eval(net, tag, x, elide)
+    y, yf, _, _ = check_eval(net, tag, x, elide)
     # dedup: bit for bit against dedup off, with the fused head on and off
     for fuse in (False, True):
         yd, _ = forward_eval(net, x, elide, dedup=True, fuse=fuse, capture=False)
@@ -425,7 +437,8 @@ def test_eval_forward_layer_by_layer(name, elide, B, precision):
 
 def check_eval(net, tag, x, elide):
     """The eval forward with dedup off, fused head off and then on: every layer's output (and the fc's) from its
-    captured input, then the fused head from the fused layer's captured input.  Returns (y, y with the fused head)."""
+    captured input, then the fused head from the fused layer's captured input.  Returns (y, y with the fused head,
+    the layers' captured outputs, the fc's), the captures of the run with the fused head off."""
     precision = net.precision
     B = x.shape[0]
     y, cap = forward_eval(net, x, elide, dedup=False, fuse=False)
@@ -435,27 +448,27 @@ def check_eval(net, tag, x, elide):
     assert np.array_equal(act[n - 1], y.reshape(act[n - 1].shape)), tag
     for li in range(n):
         inp, block_in = layer_input(net, li, x, fc_out, act)
-        ref, bound = eval_layer(net, li, inp, block_in, net.route(li, B)["tc"])
+        ref, bound = eval_layer(net, li, inp, block_in, net.conv_precision(net.route(li, B)["tc"]))
         check(f"{tag} layer {li}", precision, act[li], ref, bound)
         if li == net.blocks[0]["first"] + net.blocks[0]["n"] - 1:
             check(f"{tag} fc_out", precision, fc_out,
-                  *fc_ref(act[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], precision))
+                  *fc_ref(act[li].reshape(B, -1), net.p["fc.weight"], net.p["fc.bias"], net.fc_precision()))
     # fused head
     yf, capf = forward_eval(net, x, elide, dedup=False, fuse=True)
     fused = [li for li in range(n) if net.route(li, B)["fuse_head"]]
-    if precision == "fp16x3" and B * net.V(n - 2) >= 64:
+    if precision != "fp32" and B * net.V(n - 2) >= 64:
         assert fused == [n - 2], (tag, fused)
     if fused:
         li = fused[0]
         act_f = {k: capf["y"][k].reshape(B, net.V(k), -1) for k in range(n) if k != li}
         inp, block_in = layer_input(net, li, x, capf["fc_out"], act_f)
-        y1, e1 = eval_layer(net, li, inp, block_in, True)
+        y1, e1 = eval_layer(net, li, inp, block_in, precision)
         Lh = net.L32[net.layers[n - 1]["level"]]
         Wh, bh = net.p[f"cl.{n - 1}.weight"], net.p[f"cl.{n - 1}.bias"]
         ref = R.cheb_conv_fwd(y1, Lh, Wh, bh)
         bound = R.cheb_conv_fwd_bound(y1, Lh, Wh, bh, "fp32") + R.thin_head_fused_bound(y1, e1, Lh, Wh)
         check(f"{tag} fused head", precision, yf.reshape(ref.shape), ref, bound)
-    return y, yf
+    return y, yf, act, fc_out
 
 
 # ------------------------------------------------------------------------------------------- launches and coverage

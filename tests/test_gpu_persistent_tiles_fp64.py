@@ -10,7 +10,7 @@ p2m_debug_conv_log reports which instantiation ran and with how many tiles per C
 
 1. Single layer (p2m_cheb_conv_fwd / _bwd): every kernel configuration at caps that give each CTA 1, 2, 3 and all
    (>= 8) of its launch's tiles, with grids that are multiples of and coprime to the level's tile-pattern count.
-   y, dx, dW and db against fp64_ref's bounds (fp16x3), y against fp16_ref's (single-pass fp16).
+   y, dx, dW and db against fp64_ref's bounds at fp16x3, y at single-pass fp16.
 2. The network schedules (eval at elision 0 / 1 / 2 with the fused head off and on, training forward and backward
    with and without dx) at caps 1 and 3, every layer from its captured inputs.
 3. Coverage: every instantiation launch_n can select ran with >= 4 tiles on some CTA (see REACHABLE).
@@ -24,7 +24,6 @@ import numpy as np
 import pytest
 import torch
 
-import fp16_ref as R16
 import fp64_ref as R
 import graphs as G
 from helpers import graph_from_fixture
@@ -159,10 +158,9 @@ LAYERS = [
 
 
 def layer_refs(L, x, W, b, dz, precision):
-    """name -> (float64 reference, bound) of y and, with dz, of dx, dW and db."""
-    if precision == "fp16":
-        L32 = L.tocsr().astype(np.float32).astype(np.float64)
-        return {"y": (R.cheb_conv_fwd(x, L32, W, b), R16.cheb_conv_fwd_bound16(x, L32, W, b))}
+    """name -> (float64 reference, bound) of y and, with dz, of dx, dW and db, on the Laplacian's fp32 values as the
+    device holds them."""
+    L = L.tocsr().astype(np.float32).astype(np.float64)
     out = {"y": (R.cheb_conv_fwd(x, L, W, b), R.cheb_conv_fwd_bound(x, L, W, b, precision))}
     if dz is not None:
         refs = R.cheb_conv_bwd(x, L, W, dz)
@@ -234,30 +232,15 @@ def captured_equal(tag, a, b):
             assert np.array_equal(va, vb, equal_nan=True), (tag, k)
 
 
-def check_eval16(net, tag, x, act, fc_out):
-    """Every layer of an fp16 eval forward from its captured input (test_gpu_fp16_inference.eval_layer16's bound)."""
-    import test_gpu_fp16_inference as F
-    import test_gpu_network_fp64 as N
-
-    B = x.shape[0]
-    for li in range(net.n_layers):
-        inp, block_in = N.layer_input(net, li, x, fc_out, act)
-        ref, bound = F.eval_layer16(net, li, inp, block_in, net.route(li, B)["tc"])
-        r = R.bound_ratio(act[li], ref, bound)
-        assert r <= 1.0, f"{tag} layer {li}: max |err| / bound = {r:.3g}"
-
-
 @pytest.mark.parametrize("precision", ["fp16x3", "fp16"])
 @pytest.mark.parametrize("name", NETS)
 def test_eval_network_capped(name, precision):
     """Eval forward at elision 0 / 1 / 2, fused head off and on, dedup off: at caps 1 and 3 every captured layer output
     and the result are bitwise those of the uncapped run; at cap 1 every layer is checked against float64."""
-    import test_gpu_fp16_inference as F
     import test_gpu_network_fp64 as N
 
     B = 3
-    net = F.fp16_net(name, seed=41) if precision == "fp16" else N.Net(name, "fp16x3", seed=41, open_relus=False)
-    n = net.n_layers
+    net = N.Net(name, precision, seed=41, open_relus=False)
     try:
         for elide in (0, 1, 2):
             x, _ = N.train_inputs(net, B, seed=7 + elide)
@@ -278,12 +261,7 @@ def test_eval_network_capped(name, precision):
                     assert np.array_equal(y, base[fuse][0]), t + ": y differs from the uncapped run"
                     captured_equal(t, c, base[fuse][1])
                 if cap == 1:
-                    if precision == "fp16x3":
-                        N.check_eval(net, f"{tag} cap=1", x, elide)
-                    else:
-                        c = base[False][1]
-                        act = {li: c["y"][li].reshape(B, net.V(li), -1) for li in range(n)}
-                        check_eval16(net, f"{tag} cap=1", x, act, c["fc_out"])
+                    N.check_eval(net, f"{tag} cap=1", x, elide)
     finally:
         set_cap(net, 0)
     assert net.hier.kernel_status(0) == 0
