@@ -893,6 +893,39 @@ int p2m_training_pose2d_augmented(const float* joints_px, int batch, int n_joint
                                   const int32_t* flip, int flip_joint_set, int flip_before_noise, float* pose2d,
                                   p2m_stream_t stream);
 
+/* ---- optimizer: the RMSprop step (torch.optim.RMSprop, lib/funcs_utils.py:87-91) ---------------------------------
+ * One step of every segment, a segment being one parameter tensor of numel float32 elements: param, grad and
+ * square_avg, momentum_buffer when its group has momentum > 0, grad_avg when it is centred (the others may be NULL),
+ * and step (a float32 scalar, nullable) incremented by 1.  Per element, in fp32 and in torch's _multi_tensor_rmsprop
+ * operation order (each foreach op rounded once, a + alpha * op(b, c) as one fma):
+ *   g = g + wd p (wd != 0);  s = s alpha;  s = s + (1 - alpha) g^2;
+ *   centred: ga = lerp(ga, g, 1 - alpha), avg = sqrt(s - ga^2) + eps;  else avg = sqrt(s) + eps;
+ *   momentum: buf = buf mu + g / avg, p = p - lr buf;  else p = p - lr (g / avg).
+ * A group's lr is read from lr_device (a device float32 scalar, read when the kernel runs: a captured step follows a
+ * schedule that writes it) or, when that is NULL, is the host lr.  Each element is read and written once: 16-byte
+ * accesses where every array of a segment has the same address modulo 16, 4-byte ones for the rest.  Up to 448
+ * segments of up to 16 groups per launch, more take more launches.  The segment table is passed as a kernel parameter
+ * (capture-safe), no host synchronisation, no atomics: bitwise deterministic.  Every data array is checked to be
+ * device memory of one device.                                                                                    */
+typedef struct {
+  float* param;
+  const float* grad;
+  float* square_avg;
+  float* momentum_buffer;
+  float* grad_avg;
+  float* step;
+  int64_t numel;
+  int32_t group; /* index into the groups array */
+} p2m_rmsprop_segment_t;
+typedef struct {
+  double lr;              /* used when lr_device is NULL; finite */
+  const void* lr_device;  /* device float32 scalar, or NULL */
+  double alpha, eps, weight_decay, momentum; /* finite, >= 0 */
+  int32_t centered;       /* 0 or 1 */
+} p2m_rmsprop_group_t;
+int p2m_rmsprop_step(const p2m_rmsprop_segment_t* segments, int n_segments, const p2m_rmsprop_group_t* groups,
+                     int n_groups, p2m_stream_t stream);
+
 /* ---- host-side graph baking helper (CPU; no device work) -------------------------------------------
  * One level of the reference's greedy heavy-edge matching (lib/coarsening.py:153-211, HEM_one_level),
  * entries sorted by (row, col); returns the number of clusters (or -1).  Driven by

@@ -204,6 +204,18 @@ P2M_AREA_TIGHT = 0
 P2M_AREA_CROP = 1
 
 
+class RmspropSegment(C.Structure):
+    """p2m_rmsprop_segment_t: one parameter tensor of an RMSprop step (device pointers, element count, group)."""
+    _fields_ = [(n, C.c_void_p) for n in ("param", "grad", "square_avg", "momentum_buffer", "grad_avg", "step")] + [
+        ("numel", C.c_int64), ("group", C.c_int32)]
+
+
+class RmspropGroup(C.Structure):
+    """p2m_rmsprop_group_t: one param group's hyperparameters (lr_device: a device float32 lr, or None for lr)."""
+    _fields_ = [("lr", C.c_double), ("lr_device", C.c_void_p), ("alpha", C.c_double), ("eps", C.c_double),
+                ("weight_decay", C.c_double), ("momentum", C.c_double), ("centered", C.c_int32)]
+
+
 class H36MError(C.Structure):
     _fields_ = [("mean", C.c_double * 2), ("std", C.c_double * 2), ("weight", C.c_double)]
 
@@ -228,7 +240,7 @@ EXPORTS = [
     "p2m_camera_frame_workspace_bytes", "p2m_camera_frame_coords", "p2m_h36m_regressors_create",
     "p2m_h36m_regressors_destroy", "p2m_h36m_targets", "p2m_synthesize_pose", "p2m_h36m_syn_error",
     "p2m_training_pose2d", "p2m_augm_params", "p2m_training_pose2d_augmented", "p2m_sample_targets",
-    "p2m_layer_joint_targets",
+    "p2m_layer_joint_targets", "p2m_rmsprop_step",
     "p2m_last_error", "p2m_version", "p2m_launch_count", "p2m_launch_count_reset",
     "p2m_debug_conv_log", "p2m_debug_conv_log_reset",
 ]
@@ -431,6 +443,8 @@ def load() -> C.CDLL:
         lib.p2m_layer_joint_targets.argtypes = [C.c_int, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp,
                                                 vp, vp, vp, vp, vp, vp, vp, vp]
         lib.p2m_layer_joint_targets.restype = C.c_int
+        lib.p2m_rmsprop_step.argtypes = [C.POINTER(RmspropSegment), C.c_int, C.POINTER(RmspropGroup), C.c_int, vp]
+        lib.p2m_rmsprop_step.restype = C.c_int
         lib.p2m_graph_match_level.argtypes = [i64, c_int32_p, c_int32_p, C.POINTER(C.c_double), c_int64_p,
                                               C.POINTER(C.c_double), c_int32_p]
         lib.p2m_graph_match_level.restype = i32

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libp2m_b200.so")
 SOURCES = ["p2m_api.cu", "kernels_simt.cu", "cheb_umma.cu", "metrics.cu", "body_model.cu", "camera.cu", "temporal.cu",
-           "fscore.cu", "render.cu", "posenet.cu", "front_back.cu", "targets.cu", "inputs.cu", "graph_host.cpp"]
+           "fscore.cu", "render.cu", "posenet.cu", "front_back.cu", "targets.cu", "inputs.cu", "optim.cu", "graph_host.cpp"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 if os.environ.get("P2M_TRACE") == "1":  # debug build: per-role event timeline of the tensor-core conv kernel (tools/umma_trace.py)

@@ -35,8 +35,13 @@ void log_tc_launch(int kind, int nc, int ns, int xs, int mode, int f16, dim3 gri
 }
 
 int arrays_device(const char* where, std::initializer_list<const void*> arrays, int* dev) {
+  return arrays_device(where, arrays.begin(), arrays.size(), dev);
+}
+
+int arrays_device(const char* where, const void* const* arrays, size_t n, int* dev) {
   int found = -1;
-  for (const void* p : arrays) {
+  for (size_t i = 0; i < n; ++i) {
+    const void* p = arrays[i];
     if (!p) continue;
     cudaPointerAttributes attr;
     if (cudaPointerGetAttributes(&attr, p) != cudaSuccess ||

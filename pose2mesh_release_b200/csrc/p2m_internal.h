@@ -67,6 +67,7 @@ struct DeviceGuard {
 // outputs, optional arrays and workspace, not host-side tables.  Null entries are skipped; every other entry must be
 // device or managed memory, all of one device, which is stored to *dev.  Otherwise P2M_ERR_INVALID, naming `where`.
 int arrays_device(const char* where, std::initializer_list<const void*> arrays, int* dev);
+int arrays_device(const char* where, const void* const* arrays, size_t n, int* dev);  // a run-time count of arrays
 
 // n elements of T allocated on stream s (cudaMallocAsync), optionally filled from host memory, and freed on the same
 // stream at scope exit, i.e. after the kernels enqueued in between.  n == 0 allocates nothing and leaves ptr null.

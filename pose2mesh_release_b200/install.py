@@ -9,8 +9,10 @@
 PoseNet in front of MeshNet: the reference's own ``FlatPose2Mesh`` then runs both halves natively in eval mode) and
 swaps ``graph_utils.build_coarse_graphs`` for the native-matching builder; ``install(replace_losses=True)`` also rebinds
 ``core.loss.CoordLoss`` / ``NormalVectorLoss`` / ``EdgeLengthLoss`` / ``get_loss`` (and ``core.base``'s imported
-``get_loss``) to the native losses, so the Trainer no longer copies the face table from host memory twice per step.
-``uninstall()`` restores the originals.  Nothing in the reference tree is modified on disk.
+``get_loss``) to the native losses, so the Trainer no longer copies the face table from host memory twice per step;
+``install(replace_optimizer=True)`` rebinds ``funcs_utils.get_optimizer`` (and ``core.base``'s imported one) to one
+that builds the native ``optim.RMSprop`` for ``cfg.TRAIN.optimizer == 'rmsprop'``.  ``uninstall()`` restores the
+originals.  Nothing in the reference tree is modified on disk.
 """
 from __future__ import annotations
 
@@ -41,7 +43,22 @@ def _rebind_holders(original, replacement):
 _LOSS_NAMES = ("CoordLoss", "NormalVectorLoss", "EdgeLengthLoss", "get_loss")
 
 
-def install(replace_graph_builder: bool = True, replace_losses: bool = False):
+def _native_get_optimizer(original):
+    """funcs_utils.get_optimizer (lib/funcs_utils.py:78-99) with the native RMSprop, built with the same arguments,
+    for cfg.TRAIN.optimizer == 'rmsprop'; for every other optimizer, what `original` returns.  cfg is the one
+    `original` reads (funcs_utils' ``from core.config import cfg``)."""
+    def get_optimizer(model):
+        cfg = original.__globals__["cfg"]
+        if cfg.TRAIN.optimizer == "rmsprop":
+            from .optim import RMSprop
+
+            return RMSprop(model.parameters(), lr=cfg.TRAIN.lr)
+        return original(model=model)
+
+    return get_optimizer
+
+
+def install(replace_graph_builder: bool = True, replace_losses: bool = False, replace_optimizer: bool = False):
     from . import cheby_graph_conv as my_conv
     from . import graph as my_graph
     from . import meshnet as my_meshnet
@@ -72,6 +89,10 @@ def install(replace_graph_builder: bool = True, replace_losses: bool = False):
         _saved.setdefault("loss", {name: getattr(ref_loss, name) for name in _LOSS_NAMES})
         for name, original in _saved["loss"].items():
             _rebind_holders(original, getattr(my_loss, name))               # includes core.loss itself
+    if replace_optimizer and "optimizer" not in _saved:
+        ref_fu = importlib.import_module("funcs_utils")
+        _saved["optimizer"] = ref_fu.get_optimizer
+        _rebind_holders(_saved["optimizer"], _native_get_optimizer(_saved["optimizer"]))  # funcs_utils, core.base
 
 
 def uninstall():
@@ -88,6 +109,8 @@ def uninstall():
         importlib.import_module("models.backbones.cheby_graph_conv").graph_conv_cheby = _saved.pop("conv")
     if "graph" in _saved:
         importlib.import_module("graph_utils").build_coarse_graphs = _saved.pop("graph")
+    if "optimizer" in _saved:
+        importlib.import_module("funcs_utils").get_optimizer = _saved.pop("optimizer")
     if "loss" in _saved:
         ref_loss = importlib.import_module("core.loss")
         for name, original in _saved.pop("loss").items():
